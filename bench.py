@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — explanations/sec of the transformer-attribution hot path on B200 (BASELINE.json metric).
+"""bench.py — explanations/sec of the transformer-attribution hot path on H100 (BASELINE.json metric).
 
     python bench.py --gpus N --steps K --warmup W            # this engine
     python bench.py --impl reference --gpus N --steps K ...  # the reference's CPU implementation, same metric
@@ -35,9 +35,9 @@ WORKLOADS = {
     "vit_base": dict(kind="vit", factory="vit_base_patch16_224", oracle="vit_base_patch16_224", batch=256, tokens=197,
                      dim=768, depth=12, heads=12, mlp=3072,
                      label="ViT-B/16 transformer_attribution, batch 256, 224x224, start_layer 0"),
-    "vit_large": dict(kind="vit", factory="vit_large_patch16_224", oracle="vit_large_patch16_224", batch=128, tokens=197,
+    "vit_large": dict(kind="vit", factory="vit_large_patch16_224", oracle="vit_large_patch16_224", batch=64, tokens=197,
                       dim=1024, depth=24, heads=16, mlp=4096,
-                      label="ViT-L/16 transformer_attribution, batch 128, 224x224, start_layer 0"),
+                      label="ViT-L/16 transformer_attribution, batch 64, 224x224, start_layer 0"),
     "deit_base": dict(kind="vit", factory="deit_base_patch16_224", oracle="deit_base_patch16_224", batch=256, tokens=197,
                       dim=768, depth=12, heads=12, mlp=3072,
                       label="DeiT-B/16 (reference 197-token model) transformer_attribution, batch 256, start_layer 0"),
@@ -66,8 +66,13 @@ def parse():
                     help="weak: the BASELINE batch PER GPU (default, what the driver's scaling run uses); strong: the "
                          "BASELINE batch as the GLOBAL batch, sharded over the GPUs (SURVEY 8e: 256 -> 32 per GPU at 8). "
                          "With N > 1 the weak run also reports the strong-scaling numbers under the key 'strong'.")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="after the timed steps, write what the last timed step returned (maps, class index) as DIR/<name>.npy")
     ap.add_argument("--no-graph", action="store_true", help="strong-scaling line without CUDA-graph replay")
-    return ap.parse_args()
+    args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1: the result and --dump-outputs come from the timed steps")
+    return args
 
 
 def peaks():
@@ -77,25 +82,11 @@ def peaks():
             d = json.load(f)
         return dict(hbm_gbs=d["hbm_gbs"], bf16_tflops=d["bf16_tflops"], bf16_sustained=d.get("bf16_tflops_sustained"),
                     source="measured (MEASURED_PEAKS.json)")
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_sustained=1400.0, source="fallback (B200_PROFILING.md)")
-
-
-def measured_traffic(key, units=None):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch (group) from the committed ncu --set full capture of the
-    same kernel at the same shape (profiles/ncu_traffic.json), or None.  Entries captured at another batch carry
-    `bytes_per_unit` (bytes per explanation) and are scaled by `units`."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "ncu_traffic.json")) as f:
-            e = json.load(f).get(key, {})
-        if units is not None and e.get("bytes_per_unit") is not None:
-            return int(e["bytes_per_unit"] * units)
-        return e.get("bytes")
-    except (OSError, ValueError):
-        return None
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, bf16_sustained=989.0, source="fallback (NVIDIA H100 SXM data sheet, dense, 700 W)")
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -230,15 +221,14 @@ def roofline_zplus(w, batch, flags, pk):
     flops = 8.0 * rows * inf * outf
     achieved = flops / (ms * 1e-3) / 1e12
     # TF32 dense peak = half the measured bf16 peak (nominal 1.1 vs 2.25 PF); the fp32 SIMT path is judged
-    # against the same tensor roof: it is the baseline the tcgen05 path replaces.
+    # against the same tensor roof: it is the baseline the wgmma path replaces.
     peak = pk["bf16_tflops"] / 2.0
-    traffic = measured_traffic("zplus_tc" if tc else "zplus_simt")
-    return {"kernel": "zplus_linear_relprop[%s] rows=%d in=%d out=%d" % ("tcgen05-tf32" if tc else "simt-fp32", rows, inf, outf),
+    return {"kernel": "zplus_linear_relprop[%s] rows=%d in=%d out=%d" % ("wgmma-tf32" if tc else "simt-fp32", rows, inf, outf),
             "bound": "tensor", "achieved": round(achieved, 2), "peak": round(peak, 1), "unit": "TFLOP/s",
-            "frac": round(achieved / peak, 4), "traffic": traffic, "ms_per_launch_group": round(ms, 3),
+            "frac": round(achieved / peak, 4), "ms_per_launch_group": round(ms, 3),
             "algorithmic_flops": flops,
             "executed_flops": (6.0 if tc else 8.0) * rows * inf * outf,
-            "note": ("algorithmic = 8*rows*in*out (SURVEY 8a); the tcgen05 path executes 6*rows*in*out: the denominator is "
+            "note": ("algorithmic = 8*rows*in*out (SURVEY 8a); the wgmma path executes 6*rows*in*out: the denominator is "
                      "formed in one pass from the saved forward output, ((y-b) + |x||W|^T)/2; each launch also derives "
                      "the TF32 weight copies (prepare kernel, <1% of the time)") if tc else "fp32 SIMT reference path",
             "peak_source": pk["source"] + "; TF32 dense taken as bf16/2 (tf32_matmul_measured_tflops: cuBLAS TF32 8192^3 on this box)"}
@@ -291,21 +281,21 @@ def roofline_linear(w, batch, flags, pk):
         # fp16 (hi, lo) split: 3 fp16 MMAs per product against the measured bf16/fp16 MMA peak; the timed call includes the
         # weight split (once per model in the engine) and the activation pre-pass (fused into LayerNorm in the engine)
         fpeak = pk["bf16_tflops"]
-        out["forward"] = {"kernel": "linear_forward[tcgen05-fp16 split, weight split + block-split pre-pass + GEMM] rows=%d in=%d out=%d" % (rows, inf, outf),
+        out["forward"] = {"kernel": "linear_forward[wgmma-fp16 split, weight split + block-split pre-pass + GEMM] rows=%d in=%d out=%d" % (rows, inf, outf),
                           "bound": "tensor", "achieved": round(flops / ms / 1e9, 2), "peak": round(fpeak, 1), "unit": "TFLOP/s",
                           "frac": round(flops / ms / 1e9 / fpeak, 4), "ms": round(ms, 3),
                           "note": "fp32-grade: 3 fp16 MMAs per product (issue rate = 3x achieved); peak = measured bf16"}
     else:
-        out["forward"] = {"kernel": "linear_forward[%s] rows=%d in=%d out=%d" % ("tcgen05-3xTF32" if tc else "simt-fp32", rows, inf, outf),
+        out["forward"] = {"kernel": "linear_forward[%s] rows=%d in=%d out=%d" % ("wgmma-3xTF32" if tc else "simt-fp32", rows, inf, outf),
                           "bound": "tensor", "achieved": round(flops / ms / 1e9, 2), "peak": round(peak, 1), "unit": "TFLOP/s",
                           "frac": round(flops / ms / 1e9 / peak, 4), "ms": round(ms, 3),
                           "note": "fp32-grade: 3 TF32 MMAs per product (issue rate = 3x achieved)"}
     if tc and (flags & _lib.FLAG_BACKWARD_TF32):
         ms = _time_ms(lambda: ops.linear_backward_tf32(dy, wt))
-        what = "tcgen05-TF32 persistent pair"
+        what = "wgmma-TF32"
     else:
         ms = _time_ms(lambda: ops.linear_backward(dy, wt, tensor_cores=tc))
-        what = "tcgen05-3xTF32" if tc else "simt-fp32"
+        what = "wgmma-3xTF32" if tc else "simt-fp32"
     out["backward"] = {"kernel": "linear_backward[%s] rows=%d in=%d out=%d" % (what, rows, inf, outf), "bound": "tensor",
                        "achieved": round(flops / ms / 1e9, 2), "peak": round(peak, 1), "unit": "TFLOP/s",
                        "frac": round(flops / ms / 1e9 / peak, 4), "ms": round(ms, 3)}
@@ -315,7 +305,7 @@ def roofline_linear(w, batch, flags, pk):
 def roofline_rollout(w, flags, pk, B=32, dense=False):
     """The fused-rollout target of the north star: aggregation + rollout over resident G/cam, HBM-bound.
     Algorithmic bytes per explanation = 2*L*H*N^2*4 (+ 4N out; + 4N^2 when the dense joint is returned)  (SURVEY.md §8d).
-    dense: the [B,N,N] joint through the aggregation kernel + the N x N x N chain on tcgen05 (compute_rollout_attention's
+    dense: the [B,N,N] joint through the aggregation kernel + the N x N x N chain on wgmma (compute_rollout_attention's
     consumers); otherwise row 0 only (all generate_LRP reads) through the single fused kernel."""
     from transformer_explainability_b200 import ops, _lib
     L, H, N = w["depth"], w["heads"], w["tokens"]
@@ -329,10 +319,9 @@ def roofline_rollout(w, flags, pk, B=32, dense=False):
     nbytes = B * (2.0 * L * H * N * N * 4 + 4 * N + (4.0 * N * N if dense else 0.0))
     achieved = nbytes / (ms * 1e-3) / 1e9
     return {"kernel": "attribution_rollout[%s] L=%d B=%d H=%d N=%d" % (
-                ("aggregate + tcgen05 N^3 chain, dense joint" if dense else "fused row-only") if fused else "aggregate+bmm", L, B, H, N),
+                ("aggregate + wgmma N^3 chain, dense joint" if dense else "fused row-only") if fused else "aggregate+bmm", L, B, H, N),
             "bound": "hbm", "achieved": round(achieved, 1), "peak": pk["hbm_gbs"], "unit": "GB/s",
             "frac": round(achieved / pk["hbm_gbs"], 4),
-            "traffic": None if dense else measured_traffic("rollout_fused" if fused else "rollout", units=B),
             "algorithmic_bytes": nbytes, "ms": round(ms, 3), "peak_source": pk["source"]}
 
 
@@ -469,8 +458,15 @@ def main():
     sampler = ClockSampler(local)
     l0 = lib.te_kernel_launch_count()
     sampler.start()
-    ms = timed_steps(lambda: explain_call(w, eng, x_dev, batch), args.steps, args.warmup, world)
+    last = {}
+
+    def timed_step():
+        last["out"] = explain_call(w, eng, x_dev, batch)
+
+    ms = timed_steps(timed_step, args.steps, args.warmup, world)
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last["out"])
     launches = (lib.te_kernel_launch_count() - l0) // max(1, (args.steps + args.warmup)) * args.steps
     value = world * batch * args.steps / (ms * 1e-3)
 
@@ -517,7 +513,7 @@ def main():
                        "global_batch": batch * world if args.scaling == "weak" else strong["global_batch"],
                        "weights": "random-init (reference constructor distributions)", "engine_flags": flags,
                        "l2": "working set exceeds L2 by orders of magnitude: >50 GB of saved activations are written and "
-                             "re-read every step (126 MB L2)",
+                             "re-read every step (50 MB L2)",
                        "outputs_finite": finite},
             "clocks": clocks,
             "e2e": {"value": round(e2e, 2), "unit": "expl/s", "h2d_bytes_per_step": host.numel() * host.element_size(),
@@ -548,10 +544,28 @@ def main():
         dist.destroy_process_group()
 
 
+def dump_outputs(out_dir, result, cap_bytes=64 << 20):
+    """The arrays the timed path returned in its last step: relevance maps (float32) and class indices (float64).  Inputs and
+    weights are seeded, so two builds run with the same arguments can be compared output for output.  Maps larger than
+    cap_bytes are reduced to a fixed, seeded sample of rows."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    maps, idx = result
+    maps = maps.detach().float().cpu()
+    idx = idx.detach().cpu().double()
+    if maps.numel() * 4 > cap_bytes:
+        keep = max(1, cap_bytes // (4 * max(1, maps[0].numel())))
+        rows = torch.randperm(maps.shape[0], generator=torch.Generator().manual_seed(0))[:keep].sort().values
+        maps, idx = maps[rows], idx[rows]
+        np.save(os.path.join(out_dir, "sample_rows.npy"), rows.double().numpy())
+    np.save(os.path.join(out_dir, "maps.npy"), maps.numpy())
+    np.save(os.path.join(out_dir, "class_index.npy"), idx.numpy())
+
+
 def default_flags():
     """Best validated kernel selection (see DESIGN.md): updated as faster paths pass parity."""
     from transformer_explainability_b200 import _lib
-    # 51 = tcgen05 z+ rule (1) + fused row-only rollout (2) + tcgen05 Linears (16) + attention contractions (32);
+    # 51 = wgmma z+ rule (1) + fused row-only rollout (2) + wgmma Linears (16) + attention contractions (32);
     # + 256 single-pass TF32 backward + 1024 single-pass TF32 relevance-side attention products + 2048 bf16 z+ denominator term
     # + 4096 forward Linears as the block-scaled fp16 split  = 7475
     return _lib.FLAG_BENCH_DEFAULT

@@ -1,4 +1,4 @@
-/* te_b200 — C ABI of the B200-native transformer-attribution engine.
+/* te_b200 — C ABI of the transformer-attribution engine (CUDA, sm_90a / H100).
  *
  * Drop-in boundary for the `transformer_attribution` path of hila-chefer/Transformer-Explainability.
  * The reference has no FFI: its interface for this path is a Python "relprop protocol"
@@ -35,31 +35,31 @@ extern "C" {
 #define TE_ERR_UNSUPPORTED (-4)
 
 /* te_vit_attribute / te_vit_explain flags */
-#define TE_FLAG_ZPLUS_TENSOR_CORES 1u /* z+ Linear-rule GEMMs on tcgen05 (TF32 in, fp32 acc) instead of fp32 SIMT */
+#define TE_FLAG_ZPLUS_TENSOR_CORES 1u /* z+ Linear-rule GEMMs on wgmma tensor cores (TF32 in, fp32 acc) instead of fp32 SIMT */
 #define TE_FLAG_ROLLOUT_FUSED 2u      /* single fused aggregation+rollout kernel instead of aggregate + bmm chain */
 #define TE_FLAG_KEEP_ALL_CAMS 4u      /* run the relprop below start_layer too (accessor parity with the reference) */
-#define TE_FLAG_LINEAR_TENSOR_CORES 16u /* forward / backward Linear GEMMs on tcgen05 with the fp32-grade 3xTF32 split */
-#define TE_FLAG_ATTN_TENSOR_CORES 32u  /* the N x N attention contractions (QK^T, dctx V^T, S2 V^T) on tcgen05, 3xTF32 */
+#define TE_FLAG_LINEAR_TENSOR_CORES 16u /* forward / backward Linear GEMMs on wgmma with the fp32-grade 3xTF32 split */
+#define TE_FLAG_ATTN_TENSOR_CORES 32u  /* the N x N attention contractions (QK^T, dctx V^T, S2 V^T) on wgmma, 3xTF32 */
 #define TE_FLAG_ZPLUS_BF16 64u          /* with TE_FLAG_ZPLUS_TENSOR_CORES: S = R/Z stored as bf16 and the second z+ contraction
-                                         (R_in = x+ (S W+) + x- (S W-)) on tcgen05 kind::f16 with bf16 operands */
+                                         (R_in = x+ (S W+) + x- (S W-)) on bf16 wgmma */
 #define TE_FLAG_GRADIENTS_ONLY 128u    /* te_*_attribute stops after the class-gradient backward: only "attn_grad" of the layers
                                          >= start_layer is produced (maps may be NULL) — the attention-GradCAM baselines */
 #define TE_FLAG_BACKWARD_TF32 256u     /* with TE_FLAG_LINEAR_TENSOR_CORES: the activation-gradient backward Linears run as
-                                         single-pass TF32 GEMMs (persistent CTA-pair kernel) instead of the 3xTF32 split.
-                                         The gradients only enter the result linearly (relu(G * cam)), never a
-                                         safe_divide denominator: measured effect in profiles/ (r02 parity table) */
+                                         single-pass TF32 GEMMs instead of the 3xTF32 split.  The gradients only enter the
+                                         result linearly (relu(G * cam)), never a safe_divide denominator
+                                         (tests/test_gpu_parity_full.py bounds the effect) */
 #define TE_FLAG_RELPROP_TF32 1024u     /* with TE_FLAG_ATTN_TENSOR_CORES: the attention-shaped contractions of the relprop whose
                                          result is relevance (attn_cam = P * (S V^T) / 2, P^T S, S1 K, S1^T Q) run single-pass
                                          TF32 like the z+ rule does; the denominator Q K^T keeps the 3xTF32 split */
 #define TE_FLAG_ZPLUS_S1_BF16 2048u    /* with TE_FLAG_ZPLUS_TENSOR_CORES: the |x| |W|^T term of the single-pass z+ denominator with bf16
                                          operands (a sum of K non-negative products: rounding errors average to ~2^-9 / sqrt(K)) */
-#define TE_FLAG_LINEAR_F16_SPLIT 4096u  /* with TE_FLAG_LINEAR_TENSOR_CORES: the forward Linears on tcgen05 kind::f16 with a row-scaled
+#define TE_FLAG_LINEAR_F16_SPLIT 4096u  /* with TE_FLAG_LINEAR_TENSOR_CORES: the forward Linears on fp16 wgmma with a block-scaled
                                          * fp16 (hi, lo) split of both operands (3 MMAs per k-step, same 22-bit operand precision
-                                         * as the 3xTF32 split at half the tensor cycles and a third of the staged bytes) */
+                                         * as the 3xTF32 split, fp16 MMAs run at twice the TF32 rate) */
 #define TE_FLAG_ZPLUS_R_F16 8192u        /* with TE_FLAG_ZPLUS_TENSOR_CORES: the second contraction of the z+ rule, x+ (S W+) + x- (S W-), on
-                                         * tcgen05 kind::f16: S as block-scaled fp16 (one power of two per row and 128 columns),
-                                         * W+^T / W-^T as row-scaled fp16 — the 11 significant bits of the TF32 form, rounded to
-                                         * nearest instead of truncated, at twice the tensor rate */
+                                         * fp16 wgmma: S as block-scaled fp16 (one power of two per row and 128 columns),
+                                         * W+^T / W-^T as row-scaled fp16 — the 11 significant bits of the TF32 form, at twice
+                                         * the tensor rate */
 #define TE_FLAG_BACKWARD_F16 16384u      /* with TE_FLAG_LINEAR_TENSOR_CORES: the activation-gradient backward Linears as ONE fp16 MMA per
                                          * k-step (block-scaled fp16 gradients, row-scaled fp16 weights) instead of one TF32 MMA
                                          * (TE_FLAG_BACKWARD_TF32): same 11 significant bits, twice the tensor rate */
@@ -70,18 +70,11 @@ extern "C" {
                                          model.relprop() returns in the reference) is left in tensor "relevance_in" */
 
 TE_API const char* te_last_error(void);
-/* Process-wide tuning switches (not part of the reference surface).  name = "zplus_pair_kernels": run the z+ Linear rule
- * with the CTA-pair (tcgen05 cta_group::2, 256 x 256 MMA) kernels instead of the single-CTA ones (2: R kernel only);
- * name = "linear_pair_kernels": the same for the 3xTF32 forward / backward Linear GEMMs.  Both default to 0.
- * name = "zplus_persistent": 1 (default) runs the z+ rule with the persistent CTA-pair kernels (te_tc_pair.cu), 0 with
- * the round-1 kernels selected by "zplus_pair_kernels".
- * name = "attn_persistent": 1 runs the fp32-grade N x N attention kernel in its persistent, TMEM-double-buffered form (N <= 224),
- * 0 (default) one tile per CTA, two CTAs per SM.
- * name = "linear_mixed": 1 runs the forward Linears with the mixed-kind split (main term TF32, the two correction terms as bf16
- * MMAs: two thirds of the tensor cycles of the 3xTF32 kernel at the same fp32-grade accuracy), 2 its persistent CTA-pair form
- * (48 KiB staged per k-block instead of 80), 0 with 3xTF32.
+/* Process-wide tuning switches (not part of the reference surface).
  * name = "cls_row_top_block": 1 (default) runs the three z+ rules of the top block on the pooled-token rows only (exact:
  * the relevance entering the top block is zero in every other row), 0 on all rows.
+ * name = "gelu_split_fused": 1 (default) lets the fp16-split forward Linears reuse the fp16 split of the LayerNorm / GELU
+ * outputs written next to them, 0 splits every Linear input in a stand-alone pre-pass.
  * Returns TE_OK, or a negative status for an unknown name. */
 TE_API int te_set_option(const char* name, int value);
 TE_API int te_version(void);
@@ -282,7 +275,7 @@ TE_API int te_compute_rollout_attention(const float* mats, int layers, int batch
                                  float* joint, void* workspace, long long workspace_bytes, void* stream);
 
 /* Plain Linear GEMMs — exported for kernel unit tests only.  flags & TE_FLAG_LINEAR_TENSOR_CORES selects the
- * tcgen05 3xTF32 path (scratch: 16*in*out floats for the derived weight copies; may be NULL otherwise); with
+ * wgmma 3xTF32 path (scratch: 16*in*out floats for the derived weight copies; may be NULL otherwise); with
  * TE_FLAG_LINEAR_F16_SPLIT as well, te_linear_forward_ex runs the fp16-split kernel (scratch: 16*in*out +
  * round_up(rows*in,64) + rows*ceil(in/128) floats). */
 TE_API int te_linear_forward(const float* x, const float* w, const float* bias, float* y, int rows, int in_features,

@@ -1,5 +1,5 @@
 """CPU restatement (numpy) of the block-scaled fp16 (hi, lo) operand format of the fp16-split forward Linear
-(transformer_explainability_b200/csrc/te_common.cuh: te_f16_block_scale / te_f16_split4; te_tc_fwd16.cu).
+(transformer_explainability_b200/csrc/te_common.cuh: te_f16_block_scale / te_f16_split4; te_tc_wgmma.cu).
 
 Test infrastructure only (tests/test_f16_split_format.py): it pins the NUMBER FORMAT the kernels use — exact power-of-two
 scaling, 22 significant bits down to 2^-17 of the block maximum, no overflow for any finite input — independently of a GPU.

@@ -123,8 +123,7 @@ def test_host_only_queries_and_option_errors():
     assert lib.te_patch_embed_relprop_workspace_bytes(1, 3, 225, 16, 768) < 0          # patch does not divide the image
     assert lib.te_set_option(b"no_such_option", 1) < 0
     assert b"unknown option" in lib.te_last_error()
-    assert lib.te_set_option(b"zplus_pair_kernels", 0) == 0 and lib.te_set_option(b"linear_pair_kernels", 0) == 0
-    assert lib.te_set_option(b"zplus_persistent", 1) == 0
+    assert lib.te_set_option(b"cls_row_top_block", 1) == 0 and lib.te_set_option(b"gelu_split_fused", 1) == 0
 
 
 def test_baseline_and_generator_surfaces_resolve():
@@ -160,4 +159,4 @@ def test_flag_constants_match_the_header():
     for v in flags.values():
         known |= v
     assert _lib.FLAG_BENCH_DEFAULT & ~known == 0
-    assert _lib.FLAG_BENCH_DEFAULT == 7475           # what DESIGN.md / profiles/ document as the benched selection
+    assert _lib.FLAG_BENCH_DEFAULT == 7475           # what DESIGN.md documents as the benched selection

@@ -1,5 +1,5 @@
 """The block-scaled fp16 (hi, lo) operand format of the fp16-split forward Linear, pinned on CPU (oracle/f16_split.py restates
-te_f16_block_scale / te_f16_split4 of csrc/te_common.cuh and the three-term product of te_tc_fwd16.cu)."""
+te_f16_block_scale / te_f16_split4 of csrc/te_common.cuh and the three-term product of te_tc_wgmma.cu)."""
 import numpy as np
 
 from oracle import f16_split as F

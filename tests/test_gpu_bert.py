@@ -98,7 +98,7 @@ def test_bert_tiny_batched_and_relprop_api(golden_dir):
 @pytest.mark.parametrize("seq,start", [(128, 0), (512, 11)])
 def test_bert_base_vs_oracle(seq, start):
     """BERT-base (BASELINE configs[4] shape; S=512 with the pipeline default start_layer=11, S=128 with the notebook's
-    start_layer=0), fp32 SIMT and tcgen05 z+ paths.
+    start_layer=0), fp32 SIMT and tensor-core z+ paths.
 
     At random init the reference itself is badly conditioned on this model: its fp32 result (== oracle fp32, bit-equal)
     deviates from its fp64 result by 2e-2 ... 7e-1 of the map maximum depending on the thread count (measured,

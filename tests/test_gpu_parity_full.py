@@ -204,7 +204,7 @@ def _g(t):
 def test_rules_teacher_forced_at_vit_base_size(tc):
     """Every relprop rule of blocks 11, 10, 9 of a random-init ViT-B/16 (the ill-conditioned data the bench runs on), each
     kernel fed with the ORACLE's inputs for that step (batch 2).  Bounds: Add / Clone 1e-6; z+ Linear 1e-5 (fp32 SIMT) /
-    3e-3 (tcgen05 TF32, with the saved forward output: the single-pass kernel the engines run); matmul2 rule 5e-4; the
+    3e-3 (tensor-core TF32, with the saved forward output: the single-pass kernel the engines run); matmul2 rule 5e-4; the
     matmul1 rule divides by signed near-zero Q K^T — its fp32 evaluation is itself ill-conditioned, so it is judged
     against the fp32 CPU oracle evaluated on the same inputs (error <= 10x that, or 1e-5)."""
     from transformer_explainability_b200 import ops

@@ -148,7 +148,7 @@ def test_aggregation_rollout(ops, L, B, H, N, normalize):
         _, row_f = ops.attribution_rollout(dev(grad), dev(cam), start_layer=start, normalize=normalize, fused=True,
                                            want_joint=False)
         assert rel_err(row_f, ref[:, 0]) < 1e-5
-        # dense joint with the fast flag: N x N x N chain on tcgen05 (3xTF32) when N <= 224, SIMT otherwise
+        # dense joint with the fast flag: N x N x N chain on the tensor cores (3xTF32)
         joint_tc, row_tc = ops.attribution_rollout(dev(grad), dev(cam), start_layer=start, normalize=normalize,
                                                    fused=True, want_joint=True)
         assert rel_err(joint_tc, ref) < 1e-5 and rel_err(row_tc, ref[:, 0]) < 1e-5

@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 (TF32 tensor-core) z+ Linear rule against the fp32 SIMT path and the fp64 oracle.
+"""GPU: the tensor-core (TF32 tensor-core) z+ Linear rule against the fp32 SIMT path and the fp64 oracle.
 
 Tolerance: TF32 operands carry a 10-bit mantissa (rna), accumulation is fp32, Z is a sum of non-negative
 products -> relative error of a few 1e-4 on Z/S and on the output (stated: 2e-3 of the tensor maximum)."""
@@ -29,40 +29,14 @@ def test_tc_linear_relprop_matches_simt_and_oracle(rows, inf, outf):
     torch.cuda.synchronize()
     ref = rules.linear_relprop(x.double(), w.double(), r.double())
     assert rel(simt, ref) < 2e-5
-    assert rel(tc, ref) < 2e-3, "tcgen05 path: rel err %g" % rel(tc, ref)
+    assert rel(tc, ref) < 2e-3, "tensor-core path: rel err %g" % rel(tc, ref)
     # conservation of relevance survives the reduced-precision operands
     assert abs(tc.double().sum().item() - r.double().sum().item()) < 2e-3 * r.sum().item()
     # single-pass variant fed with the saved forward output: Z = ((y - b) + |x||W|^T)/2 (what the engines run)
     b = torch.randn(outf, generator=g)
     y = ops.linear_forward(xd, wd, b.cuda())
     tc1 = ops.linear_relprop(xd, wd, rd, tensor_cores=True, y=y, bias=b.cuda())
-    assert rel(tc1, ref) < 3e-3, "single-pass tcgen05 path: rel err %g" % rel(tc1, ref)
-
-
-@pytest.mark.parametrize("rows,inf,outf", [(128, 256, 256), (394, 768, 3072), (1000, 3072, 768), (77, 768, 2304)])
-def test_tc_pair_kernels_cta_group2(rows, inf, outf):
-    """The opt-in CTA-pair (tcgen05 cta_group::2) z+ kernels against the fp64 oracle and the single-CTA kernels
-    (odd tile counts get an all-padding partner CTA)."""
-    from transformer_explainability_b200 import _lib, ops
-    g = torch.Generator().manual_seed(rows + 1)
-    x = torch.randn(rows, inf, generator=g)
-    w = torch.randn(outf, inf, generator=g) * 0.05
-    r = torch.rand(rows, outf, generator=g)
-    b = torch.randn(outf, generator=g)
-    xd, wd, rd, bd = x.cuda(), w.cuda(), r.cuda(), b.cuda()
-    y = ops.linear_forward(xd, wd, bd)
-    one = ops.linear_relprop(xd, wd, rd, tensor_cores=True, y=y, bias=bd)
-    lib = _lib.load()
-    _lib.check(lib.te_set_option(b"zplus_pair_kernels", 1), "te_set_option")
-    try:
-        pair = ops.linear_relprop(xd, wd, rd, tensor_cores=True, y=y, bias=bd)
-        pair_two_pass = ops.linear_relprop(xd, wd, rd, tensor_cores=True)          # two-pass S kernel + pair R kernel
-        torch.cuda.synchronize()
-    finally:
-        _lib.check(lib.te_set_option(b"zplus_pair_kernels", 0), "te_set_option")
-    ref = rules.linear_relprop(x.double(), w.double(), r.double())
-    assert rel(pair, ref) < 3e-3 and rel(pair_two_pass, ref) < 3e-3
-    assert rel(pair, one.double()) < 1e-5          # same operands, same accumulation order per output tile
+    assert rel(tc1, ref) < 3e-3, "single-pass tensor-core path: rel err %g" % rel(tc1, ref)
 
 
 def test_tc_engine_vit_base_vs_simt_and_oracle():
@@ -89,12 +63,12 @@ def test_tc_engine_vit_base_vs_simt_and_oracle():
     for s in range(2):
         ref, ridx = ovit.explain({k: v.double() for k, v in params.items()}, xs[s:s + 1].double(), heads)
         check_parity(simt[s * trials:(s + 1) * trials], ref[0], "sample %d fp32 SIMT" % s)
-        check_parity(tc[s * trials:(s + 1) * trials], ref[0], "sample %d tcgen05 z+" % s)
+        check_parity(tc[s * trials:(s + 1) * trials], ref[0], "sample %d tensor-core z+" % s)
 
 
 @pytest.mark.parametrize("rows,inf,outf", [(128, 256, 256), (394, 768, 3072), (1000, 3072, 768), (77, 768, 2304)])
 def test_tc_3xtf32_linear_is_fp32_grade(rows, inf, outf):
-    """Forward / backward Linear GEMMs on tcgen05 with the error-compensated 3xTF32 split.  The split removes the
+    """Forward / backward Linear GEMMs on tensor-core with the error-compensated 3xTF32 split.  The split removes the
     TF32 operand rounding (1e-3 -> 1e-6); what remains is the tensor core's own fp32 accumulation, which truncates
     (round-toward-zero) at every MMA, so the error grows linearly with the reduction length: measured 7e-9 * K
     (K = 3072: 2e-5) against 5e-7 for the fp32 SIMT kernel.  Stated bound: 1.5e-8 * K + 2e-6."""
@@ -116,17 +90,6 @@ def test_tc_3xtf32_linear_is_fp32_grade(rows, inf, outf):
             assert ey < 1.5e-8 * inf + 2e-6 and edx < 1.5e-8 * outf + 2e-6
         else:
             assert ey < 3e-6 and edx < 3e-6
-    # the opt-in CTA-pair (tcgen05 cta_group::2) form of the same kernel: same operands, same chunked accumulation
-    from transformer_explainability_b200 import _lib
-    lib = _lib.load()
-    _lib.check(lib.te_set_option(b"linear_pair_kernels", 1), "te_set_option")
-    try:
-        y2 = ops.linear_forward(x.cuda(), w.cuda(), b.cuda(), tensor_cores=True)
-        dx2 = ops.linear_backward(dy.cuda(), w.cuda(), tensor_cores=True)
-        torch.cuda.synchronize()
-    finally:
-        _lib.check(lib.te_set_option(b"linear_pair_kernels", 0), "te_set_option")
-    assert rel(y2, y.double()) < 1e-6 and rel(dx2, dx.double()) < 1e-6
 
 
 def test_tc_linear_engine_vit_base():
@@ -160,7 +123,7 @@ def test_tc_linear_engine_vit_base():
 
 
 def test_tc_attention_contractions_engine():
-    """Every attention-shaped contraction on tcgen05 (3xTF32): the N x N ones (QK^T, dctx V^T, attn_cam, S1; K-major
+    """Every attention-shaped contraction on tensor-core (3xTF32): the N x N ones (QK^T, dctx V^T, attn_cam, S1; K-major
     operands) and the N x d ones reduced over tokens (attn v, attn^T dctx, dS k, dS^T q, S1 k, S1^T q, attn^T S2; MN-major
     tf32 operands in the SWIZZLE_128B_BASE32B layout).  Attention probabilities and attention gradients of every layer
     stay at fp32 accuracy (they chain through all of these kernels); maps in the same noise class."""
@@ -194,7 +157,7 @@ def test_tc_attention_contractions_engine():
 
 @pytest.mark.parametrize("rows,inf,outf", [(394, 768, 3072), (1000, 3072, 768), (128, 256, 256)])
 def test_tc_bf16_second_contraction(rows, inf, outf):
-    """TE_FLAG_ZPLUS_BF16: S stored as bf16 and R_in = x+ (S W+) + x- (S W-) on tcgen05 kind::f16 with bf16 operands
+    """TE_FLAG_ZPLUS_BF16: S stored as bf16 and R_in = x+ (S W+) + x- (S W-) on fp16 / bf16 tensor-core MMAs with bf16 operands
     (8-bit mantissa, fp32 accumulate).  Stated tolerance 1.5e-2 of the tensor maximum; relevance is conserved to 1e-2."""
     from transformer_explainability_b200 import ops
     g = torch.Generator().manual_seed(rows + 7)
@@ -216,12 +179,11 @@ def test_tc_bf16_second_contraction(rows, inf, outf):
 @pytest.mark.parametrize("rows,inf,outf", [(128, 256, 256), (394, 768, 3072), (1000, 3072, 768), (77, 768, 2304),
                                            (50432, 768, 768)])
 def test_tc_persistent_pair_kernels(rows, inf, outf):
-    """The persistent CTA-pair (cta_group::2) kernels of te_tc_pair.cu — what the engines run by default: single-pass S
-    kernel with the |x| transform + R kernel whose two products share one A tile, against the round-1 single-CTA kernels
-    (same TF32 operands) and the fp64 oracle; the single-pass TF32 backward Linear against fp64 (TF32 operand error,
-    stated 2e-3 of the tensor maximum).  Shapes include odd tile counts (all-padding partner CTA) and more tiles than
-    clusters (several tiles per persistent cluster, both TMEM accumulator buffers reused)."""
-    from transformer_explainability_b200 import _lib, ops
+    """The z+ kernels the engines run by default — single-pass S kernel with the |x| transform + R kernel whose two products
+    share one A tile — against the fp64 oracle; the single-pass TF32 backward Linear against fp64 (TF32 operand error,
+    stated 2e-3 of the tensor maximum).  Every shape is also compared element by element with the fp32 SIMT path.  Shapes include
+    partial row tiles and many more tiles than SMs."""
+    from transformer_explainability_b200 import ops
     g = torch.Generator().manual_seed(rows + 3)
     x = torch.randn(rows, inf, generator=g)
     w = torch.randn(outf, inf, generator=g) * 0.05
@@ -231,50 +193,19 @@ def test_tc_persistent_pair_kernels(rows, inf, outf):
     xd, wd, rd, bd = x.cuda(), w.cuda(), r.cuda(), b.cuda()
     y = ops.linear_forward(xd, wd, bd)
     new = ops.linear_relprop(xd, wd, rd, tensor_cores=True, y=y, bias=bd)
-    lib = _lib.load()
-    _lib.check(lib.te_set_option(b"zplus_persistent", 0), "te_set_option")
-    try:
-        old = ops.linear_relprop(xd, wd, rd, tensor_cores=True, y=y, bias=bd)
-        torch.cuda.synchronize()
-    finally:
-        _lib.check(lib.te_set_option(b"zplus_persistent", 1), "te_set_option")
+    simt = ops.linear_relprop(xd, wd, rd, tensor_cores=False)        # fp32 SIMT path: every element, every tile, all shapes
+    torch.cuda.synchronize()
+    assert rel(new, simt) < 3e-3, "z+ kernels vs fp32 SIMT: rel err %g" % rel(new, simt)
     if rows <= 4096:
         ref = rules.linear_relprop(x.double(), w.double(), r.double())
-        assert rel(new, ref) < 3e-3, "persistent pair z+ kernels: rel err %g" % rel(new, ref)
-    assert rel(new, old.double()) < 2e-5          # same TF32 operands; only the accumulation order inside a tile differs
+        assert rel(new, ref) < 3e-3, "z+ kernels: rel err %g" % rel(new, ref)
     assert abs(new.double().sum().item() - r.double().sum().item()) < 2e-3 * r.sum().item()
     dx = ops.linear_backward_tf32(dy.cuda(), wd)
     torch.cuda.synchronize()
     ref_dx = (dy.double().cuda() @ w.double().cuda()).cpu()
     e = rel(dx, ref_dx)
-    print("tf32 pair backward rows %d in %d out %d: rel %.2e" % (rows, inf, outf, e))
+    print("tf32 backward rows %d in %d out %d: rel %.2e" % (rows, inf, outf, e))
     assert e < 2e-3
-
-
-@pytest.mark.parametrize("rows,inf,outf", [(128, 256, 256), (394, 768, 3072), (1000, 3072, 768), (77, 768, 2304),
-                                           (20000, 768, 768)])
-def test_tc_mixed_kind_linear_is_fp32_grade(rows, inf, outf):
-    """Forward Linear with the mixed-kind split (te_set_option("linear_mixed", 1)): main term TF32, the two correction terms
-    as bf16 MMAs (SWIZZLE_64B operand tiles).  Same fp32-grade bound as the 3xTF32 kernel, every epilogue."""
-    from transformer_explainability_b200 import _lib, ops
-    g = torch.Generator().manual_seed(rows + 11)
-    x = torch.randn(rows, inf, generator=g) * torch.logspace(-3, 1, inf)          # activations spanning four decades
-    w = torch.randn(outf, inf, generator=g) * 0.05
-    b = torch.randn(outf, generator=g)
-    ref_y = torch.nn.functional.linear(x.double(), w.double(), b.double())
-    lib = _lib.load()
-    y3 = ops.linear_forward(x.cuda(), w.cuda(), b.cuda(), tensor_cores=True)
-    try:
-        _lib.check(lib.te_set_option(b"linear_mixed", 1), "te_set_option")
-        ym = ops.linear_forward(x.cuda(), w.cuda(), b.cuda(), tensor_cores=True)
-        _lib.check(lib.te_set_option(b"linear_mixed", 2), "te_set_option")         # persistent CTA-pair form
-        yp = ops.linear_forward(x.cuda(), w.cuda(), b.cuda(), tensor_cores=True)
-        torch.cuda.synchronize()
-    finally:
-        _lib.check(lib.te_set_option(b"linear_mixed", 0), "te_set_option")
-    e3, em, ep = rel(y3, ref_y), rel(ym, ref_y), rel(yp, ref_y)
-    print("rows %d in %d out %d: 3xTF32 %.2e  mixed %.2e  mixed persistent pair %.2e" % (rows, inf, outf, e3, em, ep))
-    assert em < 1.5e-8 * inf + 2e-6 and ep < 1.5e-8 * inf + 2e-6
 
 
 @pytest.mark.parametrize("rows,inf,outf", [(128, 256, 256), (394, 768, 3072), (1000, 3072, 768), (77, 768, 2304)])
@@ -302,8 +233,8 @@ def test_tc_bf16_single_pass_denominator(rows, inf, outf):
 @pytest.mark.parametrize("rows,inf,outf", [(128, 256, 256), (394, 768, 3072), (1000, 3072, 768), (77, 768, 2304),
                                            (20000, 768, 768), (300, 64, 256)])
 def test_tc_f16_split_linear_is_fp32_grade(rows, inf, outf):
-    """TE_FLAG_LINEAR_F16_SPLIT: forward Linear on tcgen05 kind::f16 with the row-scaled fp16 (hi, lo) split of both operands
-    (te_tc_fwd16.cu).  fp16 carries the same 11-bit significand as TF32, so the bound is the 3xTF32 one; the per-row power-of-two
+    """TE_FLAG_LINEAR_F16_SPLIT: forward Linear on fp16 / bf16 tensor-core MMAs with the row-scaled fp16 (hi, lo) split of both operands
+    (te_tc_wgmma.cu).  fp16 carries the same 11-bit significand as TF32, so the bound is the 3xTF32 one; the per-row power-of-two
     scaling has to cope with rows and weight rows whose magnitudes span 12 decades, zero rows, and activations spanning four
     decades inside a row."""
     from transformer_explainability_b200 import ops
@@ -333,8 +264,8 @@ def test_tc_f16_split_linear_is_fp32_grade(rows, inf, outf):
 
 @pytest.mark.parametrize("rows,inf,outf", [(128, 256, 256), (394, 768, 3072), (1000, 3072, 768), (77, 768, 2304), (20000, 768, 768)])
 def test_tc_fp16_second_contraction(rows, inf, outf):
-    """TE_FLAG_ZPLUS_R_F16: R_in = x+ (S W+) + x- (S W-) on tcgen05 kind::f16 — S as hi-only block-scaled fp16 (one power of two
-    per row and 128 columns), W+^T / W-^T as row-scaled fp16 (te_tc_fwd16.cu, FM_R).  Same 11 significant bits as the TF32 form
+    """TE_FLAG_ZPLUS_R_F16: R_in = x+ (S W+) + x- (S W-) on fp16 / bf16 tensor-core MMAs — S as hi-only block-scaled fp16 (one power of two
+    per row and 128 columns), W+^T / W-^T as row-scaled fp16 (te_tc_wgmma.cu).  Same 11 significant bits as the TF32 form
     (rounded to nearest): the rule error must not exceed the TF32 path's bound.  The relevance rows span 12 decades (S = R / Z
     inherits them): fp16 without the block scaling would over- / underflow."""
     from transformer_explainability_b200 import ops
@@ -362,7 +293,7 @@ def test_tc_fp16_second_contraction(rows, inf, outf):
 
 @pytest.mark.parametrize("rows,inf,outf", [(128, 256, 256), (394, 768, 3072), (1000, 3072, 768), (77, 768, 2304), (20000, 768, 768)])
 def test_tc_fp16_single_pass_backward(rows, inf, outf):
-    """TE_FLAG_BACKWARD_F16: dx = dy W as ONE fp16 MMA per k-step (te_tc_fwd16.cu, FM_LIN1): block-scaled fp16 gradient rows that
+    """TE_FLAG_BACKWARD_F16: dx = dy W as ONE fp16 MMA per k-step (te_tc_wgmma.cu): block-scaled fp16 gradient rows that
     span 12 decades, row-scaled fp16 weights.  The operands keep TF32's 11 significant bits, rounded to nearest: the error
     stays below the single-pass TF32 kernel's bound, per row."""
     from transformer_explainability_b200 import ops

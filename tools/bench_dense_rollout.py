@@ -1,4 +1,4 @@
-"""Time the dense-joint rollout (aggregation + N x N x N chain): SIMT fp32 chain vs tcgen05 3xTF32 chain.
+"""Time the dense-joint rollout (aggregation + N x N x N chain): SIMT fp32 chain vs tensor-core 3xTF32 chain.
 
     python tools/bench_dense_rollout.py [L B H N]
 """
@@ -21,7 +21,7 @@ def main():
         grad, cam = grad.contiguous(), cam.contiguous()
     res = {"L": L, "B": B, "H": H, "N": N}
     outs = {}
-    for name, fused in (("simt", False), ("tcgen05", True)):
+    for name, fused in (("simt", False), ("tensor_cores", True)):
         for _ in range(2):
             j, r = ops.attribution_rollout(grad, cam, fused=fused, want_joint=True)
         torch.cuda.synchronize()
@@ -33,7 +33,7 @@ def main():
         torch.cuda.synchronize()
         res[name + "_ms"] = e0.elapsed_time(e1) / 5
         outs[name] = j
-    res["max_abs_diff"] = (outs["simt"] - outs["tcgen05"]).abs().max().item()
+    res["max_abs_diff"] = (outs["simt"] - outs["tensor_cores"]).abs().max().item()
     res["chain_flops"] = 2.0 * (L - 1) * B * N ** 3
     print(json.dumps(res))
 

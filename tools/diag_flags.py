@@ -3,7 +3,7 @@ ViT-B?  For samples 0..3, 32 copies of the input perturbed by 1e-7 relative nois
 error vs the fp64 oracle, beside the fp32 CPU oracle (== the reference, bit-equal) evaluated on the SAME perturbed
 inputs.  A selection is "in the reference's noise class" when its quartiles match the CPU fp32 column.
 
-    python tools/diag_flags.py [trials] > profiles/r02_flag_bisect.log
+    python tools/diag_flags.py [trials] > flag_bisect.log
 """
 import os
 import sys

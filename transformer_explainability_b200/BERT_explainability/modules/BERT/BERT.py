@@ -32,7 +32,7 @@ class BertModel(_BertModel):
         self.config = config
 
     def forward(self, *args, **kwargs):
-        raise NotImplementedError("the B200 engine runs encoder + pooler + classifier as one call: wrap the weights in "
+        raise NotImplementedError("the CUDA engine runs encoder + pooler + classifier as one call: wrap the weights in "
                                   "BertForSequenceClassification (BERT_explainability.modules.BERT."
                                   "BertForSequenceClassification) and call that")
 

@@ -117,7 +117,7 @@ class BertForSequenceClassification(nn.Module):
     def engine(self):
         dev = self.classifier.weight.device
         if dev.type != "cuda":
-            raise RuntimeError("the B200 engine has no CPU path: move the model to a CUDA device (model.cuda())")
+            raise RuntimeError("the CUDA engine has no CPU path: move the model to a CUDA device (model.cuda())")
         v = self._version()
         if self._engine is None or self._engine.device != dev:
             self._engine = BertEngine(self._cfg, device=dev, flags=self.engine_flags)

@@ -1,8 +1,8 @@
-"""transformer_explainability_b200 — B200-native transformer-attribution engine.
+"""transformer_explainability_b200 — transformer-attribution engine for the H100.
 
 Drop-in for the ``transformer_attribution`` hot path of hila-chefer/Transformer-Explainability:
 ``LRP(model).generate_LRP`` / ``model.relprop`` / ``compute_rollout_attention`` /
-``generate_visualization`` keep the reference API; the work is done by hand-written sm_100a CUDA
+``generate_visualization`` keep the reference API; the work is done by hand-written sm_90a CUDA
 kernels behind the C ABI of ``include/te_b200.h``.  There is no CPU fallback.
 
 ``install_aliases()`` registers the reference's top-level module names (``modules.layers_ours``,

@@ -150,7 +150,7 @@ class VisionTransformer(nn.Module):
         """The CUDA engine holding a packed copy of the (frozen) parameters; re-packed when they change."""
         dev = self.pos_embed.device
         if dev.type != "cuda":
-            raise RuntimeError("the B200 engine has no CPU path: move the model to a CUDA device (model.cuda())")
+            raise RuntimeError("the CUDA engine has no CPU path: move the model to a CUDA device (model.cuda())")
         v = self._version()
         if self._engine is None or self._engine.device != dev:
             self._engine = ViTEngine(self._cfg, device=dev, flags=self.engine_flags | self._rule_flags)

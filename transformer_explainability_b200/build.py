@@ -1,4 +1,4 @@
-"""Build the C-ABI CUDA library (sm_100a) in-tree: ``lib/libte_b200.so``.
+"""Build the C-ABI CUDA library (sm_90a) in-tree: ``lib/libte_b200.so``.
 
     python -m transformer_explainability_b200.build [--force] [--verbose]
 
@@ -17,7 +17,7 @@ OBJDIR = os.path.join(HERE, "build")
 LIB = os.path.join(LIBDIR, "libte_b200.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "--compiler-options", "-fPIC", "-Xcompiler", "-fvisibility=hidden",
 ]
 
@@ -78,7 +78,7 @@ def build(force=False, verbose=False):
 
     with concurrent.futures.ThreadPoolExecutor(max_workers=min(8, os.cpu_count() or 2)) as ex:
         objs = list(ex.map(compile_one, sources()))
-    cmd = [nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-lcudart"]
+    cmd = [nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-lcudart"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError("link failed:\n%s\n%s" % (r.stdout, r.stderr))

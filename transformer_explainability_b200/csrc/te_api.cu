@@ -207,11 +207,6 @@ void te_engine_set_gelu_split(int on) { g_gelu_split = on ? 1 : 0; }
 
 extern "C" int te_set_option(const char* name, int value) {
     REQ(name != nullptr, "te_set_option: null name");
-    if (strcmp(name, "zplus_pair_kernels") == 0) { te_tc_set_pair_kernels(value); return TE_OK; }
-    if (strcmp(name, "linear_pair_kernels") == 0) { te_tc_set_pair_linear(value); return TE_OK; }
-    if (strcmp(name, "attn_persistent") == 0) { te_tc_set_attn_persistent(value); return TE_OK; }
-    if (strcmp(name, "linear_mixed") == 0) { te_tc_set_mixed_linear(value); return TE_OK; }
-    if (strcmp(name, "zplus_persistent") == 0) { te_tc_set_zplus_persistent(value); return TE_OK; }
     if (strcmp(name, "cls_row_top_block") == 0) { te_engine_set_cls_rows(value); return TE_OK; }
     if (strcmp(name, "gelu_split_fused") == 0) { te_engine_set_gelu_split(value); return TE_OK; }
     te_set_last_error("te_set_option: unknown option");

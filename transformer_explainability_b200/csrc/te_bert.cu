@@ -265,7 +265,7 @@ extern "C" int te_bert_forward(const te_bert_config* cfg, const float* weights, 
     }
     const float* lbase = (flags & TE_FLAG_LINEAR_TENSOR_CORES) ? derived : nullptr;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    // fp16-split forward Linears (te_tc_fwd16.cu): split of the D-wide inputs in A = tD[1] (+ scales tD[2]), of the GELU output in
+    // fp16-split forward Linears (te_tc_wgmma.cu): split of the D-wide inputs in A = tD[1] (+ scales tD[2]), of the GELU output in
     // B = tF[1] (+ scales tD[3]); all idle until the backward pass.  Every LayerNorm emits the split of its output (the hidden
     // state feeds the next layer's qkv); the attention context and the GELU output go through the pre-pass.
     const bool f16 = lbase && (flags & TE_FLAG_LINEAR_F16_SPLIT) && d.F >= d.D && te_tc_fwd16_supported(d.M, d.D, 3 * d.D, d.D) &&

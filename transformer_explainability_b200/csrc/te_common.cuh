@@ -1,4 +1,4 @@
-// Shared device helpers for the sm_100a transformer-attribution kernels.
+// Shared device helpers for the sm_90a transformer-attribution kernels.
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -91,7 +91,7 @@ __device__ __forceinline__ float te_warp_max(float v) {
     return v;
 }
 
-// ---- block-scaled fp16 (hi, lo) split: the operand format of the fp16-split Linear GEMM (te_tc_fwd16.cu) -------------------
+// ---- block-scaled fp16 (hi, lo) split: the operand format of the fp16-split Linear GEMM (te_tc_wgmma.cu) -------------------
 // A block of values with largest magnitude m is stored as 2^-e (hi + lo) with 2^e m in [2^14, 2^15): hi = fp16(2^e x),
 // lo = fp16(2^e x - hi).  s = 2^e, si = 2^-e (exact powers of two).  Zero / non-finite blocks keep e = 0.
 __device__ __forceinline__ void te_f16_block_scale(float m, float& s, float& si) {

@@ -79,7 +79,7 @@ __device__ __forceinline__ void row_stats(const float* __restrict__ xr, int D, i
 }
 
 // SPLIT: also emit the block-scaled fp16 (hi, lo) split of y (one scale per 128 columns: exactly one warp iteration), the A
-// operand of the fp16-split Linear that consumes y (te_tc_fwd16.cu) — saves that GEMM's pre-pass over y.
+// operand of the fp16-split Linear that consumes y (te_tc_wgmma.cu) — saves that GEMM's pre-pass over y.
 template <bool SPLIT>
 __global__ void layernorm_kernel(const float* __restrict__ x, const float* __restrict__ w,
                                  const float* __restrict__ b, float* __restrict__ y, float* __restrict__ mean_o,
@@ -736,7 +736,7 @@ __global__ void fill_kernel(float* __restrict__ p, float v, long long n) {
 
 inline int flat_grid(long long work) {
     long long g = (work + kThreads - 1) / kThreads;
-    const long long cap = 148LL * 16;
+    const long long cap = 132LL * 16;
     return (int)(g < 1 ? 1 : (g > cap ? cap : g));
 }
 inline int warp_rows_grid(long long rows) { return (int)((rows + (kThreads / 32) - 1) / (kThreads / 32)); }

@@ -42,7 +42,7 @@ static inline int linear_bwd(const float* dy, const float* w, float* dx, const f
 }
 
 // tensor-core (3xTF32) variants when the derived weight copies are supplied and the shape qualifies
-// fp16-split forward Linear (TE_FLAG_LINEAR_F16_SPLIT, te_tc_fwd16.cu): where the block-scaled split of the input lives
+// fp16-split forward Linear (TE_FLAG_LINEAR_F16_SPLIT, te_tc_wgmma.cu): where the block-scaled split of the input lives
 // (M*in floats + M*ceil(in/128) floats), whether its producer already filled it (ready: te_launch_layernorm_split or the previous
 // GEMM's GELU epilogue), and where the GELU epilogue puts the split of y2 for the next Linear (may be NULL)
 struct F16Split { float* split; float* scale; bool ready; float* split_out; float* scale_out; };

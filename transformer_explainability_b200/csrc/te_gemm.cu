@@ -232,7 +232,7 @@ template <int ALAY, int BLAY, int XF, int EPI>
 int launch_tm(const TeGemm& p, cudaStream_t st) {
     // small tiles when the problem would leave most of a 128x128 tile empty or the grid tiny
     const long long ctas128 = (long long)te_cdiv(p.M, 128) * te_cdiv(p.N, 128) * p.nb1 * p.nb2;
-    const bool small = (p.M <= 64 || p.N <= 64 || ctas128 < 148 ||
+    const bool small = (p.M <= 64 || p.N <= 64 || ctas128 < 132 ||
                         (p.M < 256 && (p.M % 128) != 0 && (p.M % 128) <= 80) );
     if (small) return launch_one<4, ALAY, BLAY, XF, EPI>(p, st);
     return launch_one<8, ALAY, BLAY, XF, EPI>(p, st);

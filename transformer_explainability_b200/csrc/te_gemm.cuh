@@ -3,8 +3,8 @@
 // This is the fp32-exact workhorse of the engine: every contraction whose result feeds a
 // safe_divide denominator or the arg-max (forward, activation-gradient backward, both attention
 // matmul rules) runs here, because SURVEY.md §7b shows those paths do not tolerate TF32 inputs.
-// The z+ Linear rule (97 % of the relprop flops, well conditioned) has a tcgen05 path in
-// te_tc_zplus.cu / te_tc_gemm3x.cu / te_tc_attn.cu; this kernel is its fp32 fallback and its checker.
+// The z+ Linear rule (97 % of the relprop flops, well conditioned) has a tensor-core (wgmma) path in
+// te_tc_wgmma.cu; this kernel is its fp32 fallback and its checker.
 //
 //   C[m,n] = epi( alpha * sum_k xfA(A[m,k]) * xfB(B[k,n]) )
 //

@@ -1,18 +1,18 @@
-// tcgen05 (5th-gen tensor core) path of the z+ Linear rule — TF32 operands, fp32 accumulation in TMEM.
+// Tensor-core (Hopper wgmma) GEMMs of the engines (te_tc_wgmma.cu): TF32 / bf16 / fp16 operands, fp32 accumulation.
 #pragma once
 #include "te_common.cuh"
 
-// shapes the tensor-core path accepts (in/out multiples of 256, 16-byte aligned rows)
+// shapes the tensor-core z+ path accepts (in/out multiples of 128, 16-byte aligned rows)
 bool te_tc_zplus_supported(long long rows, int in_features, int out_features, long long ldx);
 // derived copies of one frozen weight W [out,in], all K-major and rounded to TF32:
 //   [ W+ | W- | W+^T | W-^T ]        operands of the z+ rule kernels
 //   [ W_hi | W_lo | W^T_hi | W^T_lo ] error-compensated split (x_hi = tf32(x), x_lo = tf32(x - x_hi)) for the
 //                                     fp32-grade 3xTF32 forward / backward Linear GEMMs
 //   [ |W| ]                          operand of the single-pass S kernel
-//   [ bf16(W+^T) | bf16(W-^T) ]      2-byte operands of the bf16 R kernel (kind::f16)
-//   [ bf16(W_hi) | bf16(W_lo) ]      2-byte operands of the correction terms of the mixed-kind forward GEMM
+//   [ bf16(W+^T) | bf16(W-^T) ]      2-byte operands of the bf16 R kernel
+//   (10 n .. 11 n unused)
 //   [ bf16(|W|) ]                    2-byte operand of the bf16 S1 kernel (TE_FLAG_ZPLUS_S1_BF16), in*out/2 floats
-//   [ fp16 hi | fp16 lo | 2^-f ]     row-scaled fp16 split of W [out,in] for the fp16-split forward GEMM (te_tc_fwd16.cu):
+//   [ fp16 hi | fp16 lo | 2^-f ]     row-scaled fp16 split of W [out,in] for the fp16-split forward GEMM:
 //                                     in*out/2 + in*out/2 + out floats, starting at 11.5*in*out
 //   [ fp16(W^T) | 2^-f ]             row-scaled fp16 of tf32(W)^T [in,out] (single-pass backward Linear): in*out/2 + in floats at 13*in*out
 //   [ fp16(W+^T) | fp16(W-^T) | 2^-f+ | 2^-f- ]   row-scaled fp16 operands of the fp16 R kernel: at 14*in*out, scales at 15*in*out
@@ -25,12 +25,12 @@ int te_tc_zplus_linear_relprop(const float* x, long long ldx, const float* deriv
                                float* out,
                                float* s_scratch, long long rows, int in_features, int out_features, cudaStream_t st,
                                const float* y = nullptr, long long ldy = 0, const float* bias = nullptr,
-                               int bf16 = 0 /* bit 0: round-1 bf16 R kernel (flag 64); bit 1: bf16 single-pass S kernel (flag 2048);
+                               int bf16 = 0 /* bit 0: bf16 S and R kernel (flag 64); bit 1: bf16 single-pass S kernel (flag 2048);
                                                bit 2: fp16 R kernel fed by the S kernel's fp16 epilogue (flag 8192) */,
                                long long ld_out = 0 /* row stride of out; 0 = in_features */,
-                               float* xabs = nullptr /* scratch [rows, in]: enables the persistent pair kernels */);
+                               float* xabs = nullptr /* scratch [rows, in]: operand of the bf16 single-pass S kernel */);
 
-// fp32-grade (3xTF32 split) Linear GEMMs on tcgen05; epilogues mirror the SIMT ones
+// fp32-grade (3xTF32 split) Linear GEMMs; epilogues mirror the SIMT ones
 enum { TE_TC_EPI_STORE = 0, TE_TC_EPI_BIAS = 1, TE_TC_EPI_BIAS_GELU = 2, TE_TC_EPI_BIAS_ADD = 3, TE_TC_EPI_GELU_BWD = 4 };
 bool te_tc_gemm3x_supported(long long rows, int K, int N, long long lda);
 int te_tc_linear_fwd(const float* x, long long ldx, const float* derived, int in_features, int out_features,
@@ -38,9 +38,9 @@ int te_tc_linear_fwd(const float* x, long long ldx, const float* derived, int in
 int te_tc_linear_bwd(const float* dy, const float* derived, int in_features, int out_features, float* dx, const float* e0,
                      long long rows, int epi, cudaStream_t st);
 
-// fp32-grade forward Linear on tcgen05 kind::f16 (te_tc_fwd16.cu): block-scaled fp16 (hi, lo) split of both operands, three MMAs
-// per k-step, persistent CTA pairs.  Activations: one scale per (row, 128 k) — split = [hi | lo] fp16 [rows, in] (rows*in floats),
-// scale [rows, ceil(in/128)]; weights: one scale per row of W (derived buffer).
+// fp32-grade forward Linear on fp16 MMAs: block-scaled fp16 (hi, lo) split of both operands, three MMAs per k-step.
+// Activations: one scale per (row, 128 k) — split = [hi | lo] fp16 [rows, in] (rows*in floats), scale [rows, ceil(in/128)];
+// weights: one scale per row of W (derived buffer).
 bool te_tc_fwd16_supported(long long rows, int K, int N, long long lda);
 int te_tc_rowsplit_f16(const float* x, long long ldx, long long rows, int cols, void* hi, void* lo, float* scale_inv,
                        cudaStream_t st);
@@ -60,38 +60,28 @@ int te_tc_linear_bwd16(const float* dy, long long lddy, float* split, float* sca
 int te_tc_zplus_r16(const float* s, float* split, float* scale, const float* derived, const float* x, long long ldx, float* out,
                     long long ld_out, long long rows, int in_features, int out_features, cudaStream_t st);
 
-// attention-shaped N x N contractions (Q K^T, dctx V^T, S2 V^T) on tcgen05, fp32-grade 3xTF32, head slices in place
+// attention-shaped N x N contractions (Q K^T, dctx V^T, S2 V^T), fp32-grade 3xTF32, head slices in place
 enum { TE_TC_ATTN_STORE = 0, TE_TC_ATTN_MUL = 1, TE_TC_ATTN_SD = 2, TE_TC_ATTN_SOFTMAX = 3 };   // SOFTMAX: N <= 256
 bool te_tc_attn_supported(int N, int dh, long long lda, long long ldb, int ld_out);
-// single_pass (STORE / MUL epilogues): one TF32 MMA per k-step on the raw operands (gradient / relevance products only)
+// single_pass (STORE / MUL epilogues): one TF32 MMA per k-step on TF32-rounded operands (gradient / relevance products only)
 int te_tc_attn_nn(const float* A, long long lda, const float* B, long long ldb, int batch, int H, int N, int dh,
                   float* out, int ld_out, const float* E, float alpha, int epi, cudaStream_t st, bool single_pass = false);
 
 // attention-shaped N x d contractions with the reduction over tokens (attn v, attn^T dctx, dS k, dS^T q, S1 k, S1^T q ...)
 bool te_tc_attn_nk_supported(int N, int dh, int NP, long long ldx, long long ld_out);
-// single_pass (STORE / MUL epilogues): one TF32 MMA per k-step on the raw operands instead of the 3xTF32 split — the
-// activation-gradient contractions under TE_FLAG_BACKWARD_TF32, the relevance contractions under TE_FLAG_RELPROP_TF32
+// single_pass (STORE / MUL epilogues): one TF32 MMA per k-step instead of the 3xTF32 split — the activation-gradient
+// contractions under TE_FLAG_BACKWARD_TF32, the relevance contractions under TE_FLAG_RELPROP_TF32
 int te_tc_attn_nk(const float* map, int NP, int amn, const float* X, long long ldx, int batch, int H, int N, float* out,
                   int ld_out, const float* E, float alpha, int epi, cudaStream_t st, bool single_pass = false);
 
-// 1: run the z+ rule with the CTA-pair (tcgen05 cta_group::2) kernels instead of the single-CTA ones (default 0,
-// or the environment variable TE_B200_ZPLUS_2CTA=1)
-void te_tc_set_pair_kernels(int on);
-// 1: run the 3xTF32 Linear GEMMs with the CTA-pair kernel (default 0, or TE_B200_LINEAR_2CTA=1)
-void te_tc_set_pair_linear(int on);
-// 1: forward Linears with the mixed-kind split (main term TF32, correction terms bf16), single CTA; 2: its persistent CTA-pair form
-// (default 0, or TE_B200_LINEAR_MIXED=1|2)
-void te_tc_set_mixed_linear(int on);
-
-// dense rollout product out[b] = A[b] * Bm[b] ([batch, N, ld], N <= 224) on tcgen05, fp32-grade 3xTF32
+// dense rollout product out[b] = A[b] * J[b] + diag(rowscale[b]) J[b] ([batch, N, ld]), fp32-grade 3xTF32
 bool te_tc_bmm_nk_supported(int N, int ld);
 int te_tc_bmm_nk_resid(const float* A, const float* J, const float* rowscale, float* out, int batch, int N, int ld,
                        cudaStream_t st);
 
-// persistent CTA-pair (cta_group::2) kernels (te_tc_pair.cu): z+ rule contractions and the single-pass TF32 backward Linear
+// z+ rule contractions and the single-pass TF32 backward Linear
 bool te_tc_pair_supported(long long rows, int K, int N, long long lda);
-int te_tc_abs_tf32(const float* x, long long ldx, float* out, long long rows, int cols, cudaStream_t st);
-// xabs: scratch [rows, in] for tf32(|x|), the A operand of the single-pass S kernel
+// xabs: scratch [rows, in] for bf16(|x|), the A operand of the bf16 single-pass S kernel
 int te_tc_pair_zplus_s1(const float* x, long long ldx, float* xabs, const float* derived, const float* r, long long ldr,
                         const float* y, long long ldy, const float* bias, float* s_out, long long rows, int in_features,
                         int out_features, cudaStream_t st, bool bf16 = false, float* s16 = nullptr, float* s16_scale = nullptr);
@@ -101,7 +91,3 @@ int te_tc_pair_zplus_r(const float* s, const float* derived, const float* x, lon
                        long long rows, int in_features, int out_features, cudaStream_t st);
 int te_tc_pair_linear_bwd(const float* dy, long long lddy, const float* derived, int in_features, int out_features, float* dx,
                           const float* e0, long long rows, int epi, cudaStream_t st);
-// 1 (default): z+ rule on the persistent pair kernels
-void te_tc_set_zplus_persistent(int on);
-// 1: the 3xTF32 N x N attention kernel runs in its persistent, TMEM-double-buffered form when N <= 224 (default 0: measured slower)
-void te_tc_set_attn_persistent(int on);

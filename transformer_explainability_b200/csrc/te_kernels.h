@@ -10,7 +10,7 @@ int te_launch_assemble_tokens(const float* patch_out, const float* cls, const fl
 // ---- normalisation ---------------------------------------------------------------------------
 int te_launch_layernorm(const float* x, const float* w, const float* b, float* y, float* mean, float* rstd,
                         long long rows, int D, float eps, cudaStream_t st);
-// same, also emitting the block-scaled fp16 (hi, lo) split of y for the fp16-split Linear that consumes it (te_tc_fwd16.cu):
+// same, also emitting the block-scaled fp16 (hi, lo) split of y for the fp16-split Linear that consumes it (te_tc_wgmma.cu):
 // split = [hi | lo] fp16 [rows, D] (rows*D floats), scale [rows, ceil(D/128)]
 int te_launch_layernorm_split(const float* x, const float* w, const float* b, float* y, float* mean, float* rstd,
                               long long rows, int D, float eps, float* split, float* scale, cudaStream_t st);

@@ -109,7 +109,7 @@ __global__ void zb_combine_kernel(const float* __restrict__ img, const float* __
 
 inline int flat_grid(long long n) {
     long long g = (n + kThreads - 1) / kThreads;
-    return (int)(g < 1 ? 1 : (g > 148LL * 16 ? 148LL * 16 : g));
+    return (int)(g < 1 ? 1 : (g > 132LL * 16 ? 132LL * 16 : g));
 }
 }  // namespace
 

@@ -40,7 +40,7 @@ int te_rollout_layers(const float* G0, const float* cam0, long long layer_stride
                                     bert_fix, st);
     } else if ((flags & 2u) && te_tc_bmm_nk_supported(N, ld) && (!normalize || diag)) {
         // dense joint on the tensor cores, residual form: J <- A_l J + d_l J with A_l = M_l without its identity part
-        // (tcgen05, 3xTF32) and the identity's share d_l (1, or 1/rowsum for BERT) applied in fp32 in the epilogue
+        // (tensor cores, 3xTF32) and the identity's share d_l (1, or 1/rowsum for BERT) applied in fp32 in the epilogue
         const long long ms = (long long)B * N * ld;
         const bool one_launch = ld_in % 4 == 0 && ld % 4 == 0 && ld_in >= ((N + 3) & ~3) && layer_stride % 4 == 0 &&
                                 ((reinterpret_cast<uintptr_t>(G0) | reinterpret_cast<uintptr_t>(cam0) |

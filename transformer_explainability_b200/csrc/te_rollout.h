@@ -5,7 +5,7 @@
 
 // G0 / cam0: layer-0 tensors [B,H,N,ld_in]; layer l lives at +l*layer_stride floats.
 // mats [L,B,N,ld], joint_a / joint_b [B,N,ld] scratch.  joint_out [B,N,N] and row_out [B,N-first] optional.
-// flags & 2: row-only consumers get the fused streaming kernel; a dense joint is chained on tcgen05 (diag [L,B,N] scratch
+// flags & 2: row-only consumers get the fused streaming kernel; a dense joint is chained on the tensor cores (diag [L,B,N] scratch
 // is needed for that when normalize != 0).
 int te_rollout_layers(const float* G0, const float* cam0, long long layer_stride, int L, int B, int H, int N,
                       int ld_in, int ld, int start_layer, int normalize, unsigned flags, float* mats, float* joint_a, float* joint_b,

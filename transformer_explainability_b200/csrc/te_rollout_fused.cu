@@ -1,7 +1,7 @@
 // Fused aggregation + rollout (row-only).  HBM-bound by construction: per explanation it reads
 // 2*(L-start)*H*N*ld*4 bytes (G and cam, once) and writes N floats.
 //
-// Mapping: a cluster of K CTAs (K in {1,2,4,8}, chosen so that B*K covers the 148 SMs about twice) owns one
+// Mapping: a cluster of K CTAs (K in {1,2,4,8}, chosen so that B*K covers the 132 SMs about twice) owns one
 // sample; warp w of CTA c owns rows i = c + K*w, + K*nwarps, ...  For its row a warp issues 2*6 independent
 // 128-bit loads per lane (6 heads of G and cam) before consuming them, keeps the head-mean of the row in
 // registers, and accumulates r[i] * (m_i + e_i) into a per-warp register accumulator.  Per layer: one
@@ -166,7 +166,7 @@ int te_rollout_fused_row(const float* G0, const float* cam0, long long layer_str
         return TE_ERR_UNSUPPORTED;
     }
     int K = 1;
-    while (K < 8 && B * K < 296) K *= 2;                            // ~2 CTAs per SM over 148 SMs
+    while (K < 8 && B * K < 264) K *= 2;                            // ~2 CTAs per SM over 132 SMs
     if (ld_in <= 128) return launch<1>(G0, cam0, layer_stride, L, B, H, N, ld_in, start_layer, normalize, row_out, first, bert_fix, K, st);
     if (ld_in <= 256) return launch<2>(G0, cam0, layer_stride, L, B, H, N, ld_in, start_layer, normalize, row_out, first, bert_fix, K, st);
     return launch<4>(G0, cam0, layer_stride, L, B, H, N, ld_in, start_layer, normalize, row_out, first, bert_fix, K, st);

@@ -1,0 +1,1157 @@
+// Tensor-core GEMMs of the engines on Hopper (sm_90a): every contraction of te_gemm_tc.h runs on ONE kernel template,
+// wg_kernel<P>, built on wgmma.mma_async with fp32 accumulators in registers.
+//
+//   CTA = 2 warpgroups (256 threads), tile BM = 128 rows (64 per warpgroup) x P::BN columns.
+//   Operand tiles are K-major, one 128-byte row per tile row (32 tf32 / 64 fp16 / bf16 elements), in the 128-byte
+//   swizzled layout wgmma reads (16-byte chunk c of row r at r * 128 + ((c ^ (r % 8)) << 4)).  Every thread of the CTA
+//   loads its share of the next k-block from global memory into registers, applies the problem's element transform
+//   (TF32 rounding, |x|, x+ / x-, hi / lo split, transposition of MN-major sources) and stores it into the other of two
+//   shared-memory stages while the wgmmas of the current k-block run.
+//   P::CHUNK > 0: the reduction is cut into chunks of CHUNK k-blocks; each chunk accumulates in its own registers and is
+//   added into fp32 sums with round-to-nearest adds (optionally times a per-row power-of-two block scale), so a long
+//   reduction does not ride on the tensor core's accumulator rounding and block-scaled fp16 operands get their scale.
+//
+// Problems (structs below): the z+ rule's two contractions (two-pass S, single-pass S1, R; TF32, bf16 and block-scaled fp16
+// operand forms), the fp32-grade 3xTF32 and fp16-split Linear GEMMs, the single-pass TF32 / fp16 backward Linear, the
+// attention-shaped N x N and token-reduced N x d contractions and the dense rollout product.
+#include <cuda.h>
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
+#include <cuda_runtime.h>
+#include <string.h>
+
+#include "te_gemm_tc.h"
+#include "te_wgmma.cuh"
+
+namespace {
+
+constexpr int BM = 128, NTHREADS = 256;
+
+// ---- PTX helpers --------------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+
+__device__ __forceinline__ float to_tf32(float x) {
+    uint32_t u;
+    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x));
+    return __uint_as_float(u);
+}
+__device__ __forceinline__ float4 tf32x4(float4 v) { return make_float4(to_tf32(v.x), to_tf32(v.y), to_tf32(v.z), to_tf32(v.w)); }
+__device__ __forceinline__ float4 absx4(float4 v) { return make_float4(fabsf(v.x), fabsf(v.y), fabsf(v.z), fabsf(v.w)); }
+__device__ __forceinline__ float4 posx4(float4 v) { return make_float4(fmaxf(v.x, 0.f), fmaxf(v.y, 0.f), fmaxf(v.z, 0.f), fmaxf(v.w, 0.f)); }
+__device__ __forceinline__ float4 negx4(float4 v) { return make_float4(fminf(v.x, 0.f), fminf(v.y, 0.f), fminf(v.z, 0.f), fminf(v.w, 0.f)); }
+__device__ __forceinline__ float4 subx4(float4 a, float4 b) { return make_float4(a.x - b.x, a.y - b.y, a.z - b.z, a.w - b.w); }
+
+// 2^x for x <= 0 in one MUFU instruction (ex2.approx.ftz: 2^-22 relative)
+__device__ __forceinline__ float ex2_approx(float x) {
+    float y;
+    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+    return y;
+}
+
+// byte offset of 16-byte chunk c of row r in a swizzled K-major tile
+__device__ __forceinline__ uint32_t swz(int r, int c) { return (uint32_t)r * 128u + ((uint32_t)(c ^ (r & 7)) << 4); }
+
+// wgmma shared-memory descriptor of a K-major, 128-byte-swizzled tile (1024-byte aligned): start >> 4, LBO = 1 (unused for
+// swizzled K-major), SBO = 1024 B (8 rows x 128 B), layout type 1 = SWIZZLE_128B.  Advancing K by 32 bytes inside the
+// 128-byte row adds 2 to the start field.
+__device__ __forceinline__ uint64_t sdesc(uint32_t saddr) {
+    uint64_t d = (uint64_t)((saddr & 0x3FFFFu) >> 4);
+    d |= (uint64_t)1 << 16;
+    d |= (uint64_t)(1024 >> 4) << 32;
+    d |= (uint64_t)1 << 62;
+    return d;
+}
+
+constexpr int TILE128 = 128 * 128;                         // bytes of a 128-row operand tile
+
+// ---- operand loaders: each thread handles 16-byte chunks idx = tid, tid + 256, ... of a rows x 128-byte tile ----------
+// fp32 source, K-major: tile row r = source row row0 + r (valid below nrows), chunk c = elements k0 + 4c .. +3 (valid below K).
+// f(r, c, v) stores the (transformed) chunk.
+template <class F>
+__device__ __forceinline__ void for_k32(int rows, const float* __restrict__ base, long long ld, long long row0, long long nrows,
+                                        int k0, int K, int tid, F f) {
+    for (int idx = tid; idx < rows * 8; idx += NTHREADS) {
+        const int r = idx >> 3, c = idx & 7;
+        const long long gr = row0 + r;
+        const int k = k0 + 4 * c;
+        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (gr < nrows) {
+            const float* src = base + gr * ld + k;
+            if (k + 3 < K) v = *reinterpret_cast<const float4*>(src);
+            else {
+                if (k < K) v.x = src[0];
+                if (k + 1 < K) v.y = src[1];
+                if (k + 2 < K) v.z = src[2];
+            }
+        }
+        f(r, c, v);
+    }
+}
+// fp32 source, MN-major: tile row r = source column col0 + r (valid below ncols), chunk c = source rows k0 + 4c .. +3 (valid
+// below K).  Consecutive threads take consecutive columns (coalesced).
+template <class F>
+__device__ __forceinline__ void for_mn32(int rows, const float* __restrict__ base, long long ld, int col0, int ncols, int k0,
+                                         int K, int tid, F f) {
+    for (int idx = tid; idx < rows * 8; idx += NTHREADS) {
+        const int r = idx % rows, c = idx / rows;
+        const int col = col0 + r;
+        const int k = k0 + 4 * c;
+        float e[4] = {0.f, 0.f, 0.f, 0.f};
+        if (col < ncols) {
+#pragma unroll
+            for (int u = 0; u < 4; ++u)
+                if (k + u < K) e[u] = base[(long long)(k + u) * ld + col];
+        }
+        f(r, c, make_float4(e[0], e[1], e[2], e[3]));
+    }
+}
+// 16-bit source, K-major, row stride ld elements, K % 8 == 0: straight copy
+__device__ __forceinline__ void copy_k16(uint8_t* tile, int rows, const uint16_t* __restrict__ base, long long ld, long long row0,
+                                         long long nrows, int k0, int tid) {
+    for (int idx = tid; idx < rows * 8; idx += NTHREADS) {
+        const int r = idx >> 3, c = idx & 7;
+        const long long gr = row0 + r;
+        uint4 v = make_uint4(0u, 0u, 0u, 0u);
+        if (gr < nrows) v = *reinterpret_cast<const uint4*>(base + gr * ld + k0 + 8 * c);
+        *reinterpret_cast<uint4*>(tile + swz(r, c)) = v;
+    }
+}
+__device__ __forceinline__ void st4(uint8_t* tile, int r, int c, float4 v) { *reinterpret_cast<float4*>(tile + swz(r, c)) = v; }
+// hi / lo split of a chunk into two tiles: hi = tf32(v), lo = tf32(v - hi)
+__device__ __forceinline__ void st_split(uint8_t* hi, uint8_t* lo, int r, int c, float4 v) {
+    const float4 h = tf32x4(v);
+    st4(hi, r, c, h);
+    st4(lo, r, c, tf32x4(subx4(v, h)));
+}
+
+// ---- accumulator fragments: element j of a warpgroup's m64nN accumulator sits at
+//      row = 16 * warp + lane / 4 + 8 * ((j / 2) % 2), column = 8 * (j / 4) + 2 * (lane % 4) + j % 2 --------------------
+__device__ __forceinline__ int frag_row(int tid, int j) { return 64 * (tid >> 7) + 16 * ((tid >> 5) & 3) + ((tid & 31) >> 2) + 8 * ((j >> 1) & 1); }
+__device__ __forceinline__ int frag_col(int tid, int j) { return 8 * (j >> 2) + 2 * (tid & 3) + (j & 1); }
+
+// ---- the kernel -----------------------------------------------------------------------------------------------------
+template <class P>
+__global__ void __launch_bounds__(NTHREADS, 1) wg_kernel(const P p) {
+    constexpr int NR = P::BN / 2;
+    constexpr int NA = P::NACC;
+    constexpr int NT = P::CHUNK ? NA : 1, NTR = P::CHUNK ? NR : 1;
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+    const int tid = threadIdx.x, wg = tid >> 7;
+    const int m0 = blockIdx.x * BM, n0 = blockIdx.y * P::BN, z = blockIdx.z;
+    float acc[NA][NR];
+    float tot[NT][NTR];
+#pragma unroll
+    for (int a = 0; a < NA; ++a)
+#pragma unroll
+        for (int j = 0; j < NR; ++j) acc[a][j] = 0.f;
+#pragma unroll
+    for (int a = 0; a < NT; ++a)
+#pragma unroll
+        for (int j = 0; j < NTR; ++j) tot[a][j] = 0.f;
+
+    const int kb = p.kblocks();
+    p.load(smem, 0, m0, n0, z, tid);
+    fence_proxy_async();
+    __syncthreads();
+    for (int it = 0; it < kb; ++it) {
+        const bool fresh = P::CHUNK ? (it % P::CHUNK == 0) : (it == 0);
+        wg_fence();
+        p.mma(smem_u32(smem + (it & 1) * P::STAGE), wg, acc, fresh ? 0u : 1u);
+        wg_commit();
+        if (it + 1 < kb) p.load(smem + ((it + 1) & 1) * P::STAGE, it + 1, m0, n0, z, tid);
+        wg_wait0();
+        if constexpr (P::CHUNK > 0) {
+            if ((it + 1) % P::CHUNK == 0 || it + 1 == kb) {
+                const int ch = it / P::CHUNK;
+                const float s0 = p.chunk_scale(m0 + frag_row(tid, 0), ch, z), s1 = p.chunk_scale(m0 + frag_row(tid, 2), ch, z);
+#pragma unroll
+                for (int a = 0; a < NA; ++a)
+#pragma unroll
+                    for (int j = 0; j < NR; ++j) tot[a][j] = fmaf(acc[a][j], ((j >> 1) & 1) ? s1 : s0, tot[a][j]);
+            }
+        }
+        fence_proxy_async();
+        __syncthreads();
+    }
+    if constexpr (P::CHUNK > 0) p.epilogue(tot, m0, n0, z, tid);
+    else p.epilogue(acc, m0, n0, z, tid);
+}
+
+// unit block scale for the plain chunked problems
+struct NoScale {
+    __device__ __forceinline__ float chunk_scale(int, int, int) const { return 1.f; }
+};
+
+// ---- z+ rule, first contraction: S = sd(R, Z) ---------------------------------------------------------------------
+// Z two-pass:    x+ W+^T + x- W-^T                        (A tiles x+ / x- transformed on load, B = W+ / W-)
+// Z single-pass: ((y - bias) + |x| |W|^T) / 2             (the saved forward output y = x W^T + bias)
+// OUT: 0 = S as TF32-rounded fp32, 1 = bf16, 2 = hi-only block-scaled fp16 (one 2^-e per row and 128 columns)
+enum { ZO_F32 = 0, ZO_BF16 = 1, ZO_F16S = 2 };
+template <bool SINGLE, bool BF, int OUT>
+struct ZsProb : NoScale {
+    static constexpr int BN = 128, NACC = 1, CHUNK = 0;
+    static constexpr int STAGE = SINGLE ? 2 * TILE128 : 4 * TILE128;
+    int M, N, K;
+    const float* x; long long ldx;
+    const void* xabs;                       // BF: bf16(|x|) [M, K]
+    const void* wa; const void* wb;         // SINGLE: |W| (tf32 or bf16) ; else W+ / W- (tf32) [N, K]
+    const float* r; long long ldr; const float* y; long long ldy; const float* bias;
+    void* out; long long ldo; float* hs;    // hs: ZO_F16S block scales [M, N / 128]
+
+    __device__ int kblocks() const { return K / (BF ? 64 : 32); }
+    __device__ void load(uint8_t* st, int kb, int m0, int n0, int, int tid) const {
+        if (BF) {
+            copy_k16(st, BM, (const uint16_t*)xabs, K, m0, M, kb * 64, tid);
+            copy_k16(st + TILE128, BN, (const uint16_t*)wa, K, n0, N, kb * 64, tid);
+            return;
+        }
+        if (SINGLE) {
+            for_k32(BM, x, ldx, m0, M, kb * 32, K, tid, [&](int rr, int c, float4 v) { st4(st, rr, c, tf32x4(absx4(v))); });
+            for_k32(BN, (const float*)wa, K, n0, N, kb * 32, K, tid, [&](int rr, int c, float4 v) { st4(st + TILE128, rr, c, v); });
+        } else {
+            for_k32(BM, x, ldx, m0, M, kb * 32, K, tid, [&](int rr, int c, float4 v) {
+                st4(st, rr, c, tf32x4(posx4(v)));
+                st4(st + TILE128, rr, c, tf32x4(negx4(v)));
+            });
+            for_k32(BN, (const float*)wa, K, n0, N, kb * 32, K, tid, [&](int rr, int c, float4 v) { st4(st + 2 * TILE128, rr, c, v); });
+            for_k32(BN, (const float*)wb, K, n0, N, kb * 32, K, tid, [&](int rr, int c, float4 v) { st4(st + 3 * TILE128, rr, c, v); });
+        }
+    }
+    __device__ void mma(uint32_t st, int wg, float (&acc)[1][BN / 2], uint32_t sd) const {
+        const uint32_t aoff = (uint32_t)wg * 64u * 128u;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const uint64_t o = (uint64_t)(2 * k);
+            if (BF) wgmma_bf16(acc[0], sdesc(st + aoff) + o, sdesc(st + TILE128) + o, (k == 0) ? sd : 1u);
+            else if (SINGLE) wgmma_tf32(acc[0], sdesc(st + aoff) + o, sdesc(st + TILE128) + o, (k == 0) ? sd : 1u);
+            else {
+                wgmma_tf32(acc[0], sdesc(st + aoff) + o, sdesc(st + 2 * TILE128) + o, (k == 0) ? sd : 1u);
+                wgmma_tf32(acc[0], sdesc(st + TILE128 + aoff) + o, sdesc(st + 3 * TILE128) + o, 1u);
+            }
+        }
+    }
+    __device__ void epilogue(float (&acc)[1][BN / 2], int m0, int n0, int, int tid) const {
+        float sv[BN / 2];
+        float rmax[2] = {0.f, 0.f};
+#pragma unroll
+        for (int j = 0; j < BN / 2; j += 2) {
+            const int row = m0 + frag_row(tid, j), col = n0 + frag_col(tid, j);
+            float2 rr = make_float2(0.f, 0.f), z = make_float2(acc[0][j], acc[0][j + 1]);
+            if (row < M) {
+                rr = *reinterpret_cast<const float2*>(r + (long long)row * ldr + col);
+                if (SINGLE) {
+                    const float2 yy = *reinterpret_cast<const float2*>(y + (long long)row * ldy + col);
+                    const float2 bb = bias ? *reinterpret_cast<const float2*>(bias + col) : make_float2(0.f, 0.f);
+                    // x+ W+^T + x- W-^T == (x W^T + |x| |W|^T) / 2 ; a negative result is cancellation noise of a sum of
+                    // non-negative terms
+                    z.x = fmaxf(0.5f * ((yy.x - bb.x) + z.x), 0.f);
+                    z.y = fmaxf(0.5f * ((yy.y - bb.y) + z.y), 0.f);
+                }
+            }
+            sv[j] = te_sd(rr.x, z.x);
+            sv[j + 1] = te_sd(rr.y, z.y);
+            if (OUT == ZO_F16S) rmax[(j >> 1) & 1] = fmaxf(rmax[(j >> 1) & 1], fmaxf(fabsf(sv[j]), fabsf(sv[j + 1])));
+            if (row >= M) continue;
+            if (OUT == ZO_F32) {
+                *reinterpret_cast<float2*>((float*)out + (long long)row * ldo + col) = make_float2(to_tf32(sv[j]), to_tf32(sv[j + 1]));
+            } else if (OUT == ZO_BF16) {
+                *reinterpret_cast<__nv_bfloat162*>((__nv_bfloat16*)out + (long long)row * ldo + col) = __floats2bfloat162_rn(sv[j], sv[j + 1]);
+            }
+        }
+        if (OUT == ZO_F16S) {
+            // the tile's 128 columns of a row are one scale block, held by the 4 lanes of a quad
+            float sc[2];
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                float m = rmax[h];
+                m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
+                m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+                float si;
+                te_f16_block_scale(m, sc[h], si);
+                const int row = m0 + frag_row(tid, 2 * h);
+                if ((tid & 3) == 0 && row < M) hs[(long long)row * (N / 128) + n0 / 128] = si;
+            }
+#pragma unroll
+            for (int j = 0; j < BN / 2; j += 2) {
+                const int row = m0 + frag_row(tid, j), col = n0 + frag_col(tid, j);
+                const float s = sc[(j >> 1) & 1];
+                if (row < M) *reinterpret_cast<__half2*>((__half*)out + (long long)row * N + col) = __floats2half2_rn(sv[j] * s, sv[j + 1] * s);
+            }
+        }
+    }
+};
+
+// ---- z+ rule, second contraction: R_in = x+ (S W+) + x- (S W-) --------------------------------------------------------
+// KIND 0: S and W+-^T TF32 fp32 ; 1: bf16 ; 2: block-scaled fp16 S (scale per row and 128 k) with row-scaled fp16 W+-^T
+template <int KIND>
+struct ZrProb {
+    static constexpr int BN = (KIND == 2) ? 64 : 128, NACC = 2, CHUNK = (KIND == 2) ? 2 : 0;
+    static constexpr int BT = BN * 128;
+    static constexpr int STAGE = TILE128 + 2 * BT;
+    int M, N, K;
+    const void* s; const void* wp; const void* wn;     // S [M, K] (row stride K), W+^T / W-^T [N, K]
+    const float* rs; int rs_ld; const float* cp; const float* cn;   // KIND 2: scales of S, of the rows of W+^T / W-^T
+    const float* x; long long ldx; float* out; long long ldo;
+
+    __device__ int kblocks() const { return K / (KIND ? 64 : 32); }
+    __device__ float chunk_scale(int row, int ch, int) const { return (KIND == 2 && row < M) ? rs[(long long)row * rs_ld + ch] : 1.f; }
+    __device__ void load(uint8_t* st, int kb, int m0, int n0, int, int tid) const {
+        if (KIND) {
+            copy_k16(st, BM, (const uint16_t*)s, K, m0, M, kb * 64, tid);
+            copy_k16(st + TILE128, BN, (const uint16_t*)wp, K, n0, N, kb * 64, tid);
+            copy_k16(st + TILE128 + BT, BN, (const uint16_t*)wn, K, n0, N, kb * 64, tid);
+        } else {
+            for_k32(BM, (const float*)s, K, m0, M, kb * 32, K, tid, [&](int r, int c, float4 v) { st4(st, r, c, v); });
+            for_k32(BN, (const float*)wp, K, n0, N, kb * 32, K, tid, [&](int r, int c, float4 v) { st4(st + TILE128, r, c, v); });
+            for_k32(BN, (const float*)wn, K, n0, N, kb * 32, K, tid, [&](int r, int c, float4 v) { st4(st + TILE128 + BT, r, c, v); });
+        }
+    }
+    __device__ void mma(uint32_t st, int wg, float (&acc)[2][BN / 2], uint32_t sd) const {
+        const uint64_t a = sdesc(st + (uint32_t)wg * 64u * 128u), b0 = sdesc(st + TILE128), b1 = sdesc(st + TILE128 + BT);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const uint64_t o = (uint64_t)(2 * k);
+            const uint32_t d = (k == 0) ? sd : 1u;
+            if (KIND == 0) { wgmma_tf32(acc[0], a + o, b0 + o, d); wgmma_tf32(acc[1], a + o, b1 + o, d); }
+            else if (KIND == 1) { wgmma_bf16(acc[0], a + o, b0 + o, d); wgmma_bf16(acc[1], a + o, b1 + o, d); }
+            else { wgmma_f16(acc[0], a + o, b0 + o, d); wgmma_f16(acc[1], a + o, b1 + o, d); }
+        }
+    }
+    __device__ void epilogue(float (&acc)[2][BN / 2], int m0, int n0, int, int tid) const {
+#pragma unroll
+        for (int j = 0; j < BN / 2; j += 2) {
+            const int row = m0 + frag_row(tid, j), col = n0 + frag_col(tid, j);
+            if (row >= M) continue;
+            const float2 xv = *reinterpret_cast<const float2*>(x + (long long)row * ldx + col);
+            float2 ap = make_float2(acc[0][j], acc[0][j + 1]), an = make_float2(acc[1][j], acc[1][j + 1]);
+            if (KIND == 2) {
+                ap.x *= cp[col]; ap.y *= cp[col + 1];
+                an.x *= cn[col]; an.y *= cn[col + 1];
+            }
+            *reinterpret_cast<float2*>(out + (long long)row * ldo + col) =
+                make_float2(fmaxf(xv.x, 0.f) * ap.x + fminf(xv.x, 0.f) * an.x, fmaxf(xv.y, 0.f) * ap.y + fminf(xv.y, 0.f) * an.y);
+        }
+    }
+};
+
+// ---- Linear epilogues (ids of te_gemm_tc.h) -----------------------------------------------------------------------
+struct LinOut {
+    int M, N;
+    const float* bias; const float* E; long long lde;
+    float* C; long long ldc; float* C2; long long ldc2;
+};
+// v: the product for columns col, col + 1 (already scaled)
+template <int EPI, bool FAST_GRAD = false>
+__device__ __forceinline__ void lin_store(const LinOut& o, int row, int col, float v0, float v1) {
+    if (row >= o.M) return;
+    float2 b = make_float2(0.f, 0.f);
+    if ((EPI == TE_TC_EPI_BIAS || EPI == TE_TC_EPI_BIAS_GELU || EPI == TE_TC_EPI_BIAS_ADD) && o.bias)
+        b = *reinterpret_cast<const float2*>(o.bias + col);
+    float2 y = make_float2(v0 + b.x, v1 + b.y), y2 = make_float2(0.f, 0.f);
+    if (EPI == TE_TC_EPI_BIAS_GELU) y2 = make_float2(te_gelu(y.x), te_gelu(y.y));
+    if (EPI == TE_TC_EPI_BIAS_ADD || EPI == TE_TC_EPI_GELU_BWD) {
+        const float2 e = *reinterpret_cast<const float2*>(o.E + (long long)row * o.lde + col);
+        if (EPI == TE_TC_EPI_BIAS_ADD) y2 = make_float2(e.x + y.x, e.y + y.y);
+        else if (FAST_GRAD) y = make_float2(v0 * te_gelu_grad_fast(e.x), v1 * te_gelu_grad_fast(e.y));
+        else y = make_float2(v0 * te_gelu_grad(e.x), v1 * te_gelu_grad(e.y));
+    }
+    *reinterpret_cast<float2*>(o.C + (long long)row * o.ldc + col) = y;
+    if (EPI == TE_TC_EPI_BIAS_GELU || EPI == TE_TC_EPI_BIAS_ADD) *reinterpret_cast<float2*>(o.C2 + (long long)row * o.ldc2 + col) = y2;
+}
+
+// ---- fp32-grade Linear, 3xTF32: C = A B^T ~ A_hi B_hi^T + A_lo B_hi^T + A_hi B_lo^T (A split on load, B pre-split) -------
+template <int EPI>
+struct Lin3Prob : NoScale {
+    static constexpr int BN = 128, NACC = 1, CHUNK = 4;
+    static constexpr int STAGE = 4 * TILE128;
+    int K;
+    const float* a; long long lda; const float* bh; const float* bl;
+    LinOut o;
+    __device__ int kblocks() const { return K / 32; }
+    __device__ void load(uint8_t* st, int kb, int m0, int n0, int, int tid) const {
+        for_k32(BM, a, lda, m0, o.M, kb * 32, K, tid, [&](int r, int c, float4 v) { st_split(st, st + TILE128, r, c, v); });
+        for_k32(BN, bh, K, n0, o.N, kb * 32, K, tid, [&](int r, int c, float4 v) { st4(st + 2 * TILE128, r, c, v); });
+        for_k32(BN, bl, K, n0, o.N, kb * 32, K, tid, [&](int r, int c, float4 v) { st4(st + 3 * TILE128, r, c, v); });
+    }
+    __device__ void mma(uint32_t st, int wg, float (&acc)[1][BN / 2], uint32_t sd) const {
+        const uint32_t aoff = (uint32_t)wg * 64u * 128u;
+        const uint64_t ah = sdesc(st + aoff), al = sdesc(st + TILE128 + aoff), bhd = sdesc(st + 2 * TILE128), bld = sdesc(st + 3 * TILE128);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const uint64_t q = (uint64_t)(2 * k);
+            wgmma_tf32(acc[0], al + q, bhd + q, (k == 0) ? sd : 1u);          // small terms first
+            wgmma_tf32(acc[0], ah + q, bld + q, 1u);
+            wgmma_tf32(acc[0], ah + q, bhd + q, 1u);
+        }
+    }
+    __device__ void epilogue(float (&acc)[1][BN / 2], int m0, int n0, int, int tid) const {
+#pragma unroll
+        for (int j = 0; j < BN / 2; j += 2) lin_store<EPI>(o, m0 + frag_row(tid, j), n0 + frag_col(tid, j), acc[0][j], acc[0][j + 1]);
+    }
+};
+
+// ---- single-pass TF32 Linear (activation-gradient backward): C = tf32(A) B^T, B rounded once ---------------------------
+template <int EPI>
+struct Lin1Prob : NoScale {
+    static constexpr int BN = 128, NACC = 1, CHUNK = 0;
+    static constexpr int STAGE = 2 * TILE128;
+    int K;
+    const float* a; long long lda; const float* b;
+    LinOut o;
+    __device__ int kblocks() const { return K / 32; }
+    __device__ void load(uint8_t* st, int kb, int m0, int n0, int, int tid) const {
+        for_k32(BM, a, lda, m0, o.M, kb * 32, K, tid, [&](int r, int c, float4 v) { st4(st, r, c, tf32x4(v)); });
+        for_k32(BN, b, K, n0, o.N, kb * 32, K, tid, [&](int r, int c, float4 v) { st4(st + TILE128, r, c, v); });
+    }
+    __device__ void mma(uint32_t st, int wg, float (&acc)[1][BN / 2], uint32_t sd) const {
+        const uint64_t a0 = sdesc(st + (uint32_t)wg * 64u * 128u), b0 = sdesc(st + TILE128);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) wgmma_tf32(acc[0], a0 + (uint64_t)(2 * k), b0 + (uint64_t)(2 * k), (k == 0) ? sd : 1u);
+    }
+    __device__ void epilogue(float (&acc)[1][BN / 2], int m0, int n0, int, int tid) const {
+#pragma unroll
+        for (int j = 0; j < BN / 2; j += 2)
+            lin_store<EPI, true>(o, m0 + frag_row(tid, j), n0 + frag_col(tid, j), acc[0][j], acc[0][j + 1]);
+    }
+};
+
+// ---- fp16-split Linear: block-scaled fp16 operands (te_common.cuh).  TERMS 3: hi*hi + lo*hi + hi*lo (fp32 grade);
+//      TERMS 1: hi*hi (single pass).  One chunk = 128 k = one activation scale block; the columns carry the weight row scale.
+template <int EPI, int TERMS>
+struct F16Prob {
+    static constexpr int BN = 128, NACC = 1, CHUNK = 2;
+    static constexpr int STAGE = (TERMS == 3 ? 4 : 2) * TILE128;
+    int K;
+    const __half* ah; const __half* al; const __half* bh; const __half* bl;
+    const float* rs; int rs_ld; const float* cs;
+    LinOut o;
+    __device__ int kblocks() const { return K / 64; }
+    __device__ float chunk_scale(int row, int ch, int) const { return row < o.M ? rs[(long long)row * rs_ld + ch] : 1.f; }
+    __device__ void load(uint8_t* st, int kb, int m0, int n0, int, int tid) const {
+        copy_k16(st, BM, (const uint16_t*)ah, K, m0, o.M, kb * 64, tid);
+        copy_k16(st + TILE128, BN, (const uint16_t*)bh, K, n0, o.N, kb * 64, tid);
+        if (TERMS == 3) {
+            copy_k16(st + 2 * TILE128, BM, (const uint16_t*)al, K, m0, o.M, kb * 64, tid);
+            copy_k16(st + 3 * TILE128, BN, (const uint16_t*)bl, K, n0, o.N, kb * 64, tid);
+        }
+    }
+    __device__ void mma(uint32_t st, int wg, float (&acc)[1][BN / 2], uint32_t sd) const {
+        const uint32_t aoff = (uint32_t)wg * 64u * 128u;
+        const uint64_t a0 = sdesc(st + aoff), b0 = sdesc(st + TILE128), a1 = sdesc(st + 2 * TILE128 + aoff), b1 = sdesc(st + 3 * TILE128);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const uint64_t q = (uint64_t)(2 * k);
+            if (TERMS == 3) {
+                wgmma_f16(acc[0], a1 + q, b0 + q, (k == 0) ? sd : 1u);
+                wgmma_f16(acc[0], a0 + q, b1 + q, 1u);
+                wgmma_f16(acc[0], a0 + q, b0 + q, 1u);
+            } else {
+                wgmma_f16(acc[0], a0 + q, b0 + q, (k == 0) ? sd : 1u);
+            }
+        }
+    }
+    __device__ void epilogue(float (&acc)[1][BN / 2], int m0, int n0, int, int tid) const {
+#pragma unroll
+        for (int j = 0; j < BN / 2; j += 2) {
+            const int col = n0 + frag_col(tid, j);
+            lin_store<EPI>(o, m0 + frag_row(tid, j), col, acc[0][j] * cs[col], acc[0][j + 1] * cs[col + 1]);   // exact scaling
+        }
+    }
+};
+
+// ---- attention-shaped N x N contraction: out[b,h,i,j] = epi(alpha * sum_d A[b*N+i, h*dh+d] B[b*N+j, h*dh+d]) ------------
+enum { AT_STORE = 0, AT_MUL = 1, AT_SD = 2, AT_SOFTMAX = 3, AT_RESID = 4 };
+template <int EPI, bool SP, int BN_>
+struct NnProb : NoScale {
+    static constexpr int BN = BN_, NACC = 1, CHUNK = 0;
+    static constexpr int BT = BN * 128;
+    static constexpr int STAGE = SP ? TILE128 + BT : 2 * (TILE128 + BT);
+    int N, H, dh, ld_out, batch;
+    const float* a; long long lda; const float* b; long long ldb;
+    const float* E; float* out; float alpha;
+    __device__ int kblocks() const { return dh / 32; }
+    __device__ void load(uint8_t* st, int kb, int m0, int n0, int bh, int tid) const {
+        const int s = bh / H, h = bh % H;
+        const long long rows = (long long)batch * N;
+        const int k0 = h * dh + kb * 32, kend = h * dh + dh;
+        if (SP) {
+            for_k32(BM, a, lda, (long long)s * N + m0, rows, k0, kend, tid, [&](int r, int c, float4 v) { st4(st, r, c, tf32x4(v)); });
+            for_k32(BN, b, ldb, (long long)s * N + n0, rows, k0, kend, tid, [&](int r, int c, float4 v) { st4(st + TILE128, r, c, tf32x4(v)); });
+        } else {
+            for_k32(BM, a, lda, (long long)s * N + m0, rows, k0, kend, tid, [&](int r, int c, float4 v) { st_split(st, st + TILE128, r, c, v); });
+            for_k32(BN, b, ldb, (long long)s * N + n0, rows, k0, kend, tid,
+                    [&](int r, int c, float4 v) { st_split(st + 2 * TILE128, st + 2 * TILE128 + BT, r, c, v); });
+        }
+    }
+    __device__ void mma(uint32_t st, int wg, float (&acc)[1][BN / 2], uint32_t sd) const {
+        const uint32_t aoff = (uint32_t)wg * 64u * 128u;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const uint64_t q = (uint64_t)(2 * k);
+            if (SP) {
+                wgmma_tf32(acc[0], sdesc(st + aoff) + q, sdesc(st + TILE128) + q, (k == 0) ? sd : 1u);
+            } else {
+                const uint64_t ah = sdesc(st + aoff), al = sdesc(st + TILE128 + aoff), bhd = sdesc(st + 2 * TILE128),
+                               bld = sdesc(st + 2 * TILE128 + BT);
+                wgmma_tf32(acc[0], al + q, bhd + q, (k == 0) ? sd : 1u);
+                wgmma_tf32(acc[0], ah + q, bld + q, 1u);
+                wgmma_tf32(acc[0], ah + q, bhd + q, 1u);
+            }
+        }
+    }
+    __device__ void epilogue(float (&acc)[1][BN / 2], int m0, int n0, int bh, int tid) const {
+        const int ncols = (N + 3) & ~3;                  // the row padding up to a multiple of 4 is written as zeros
+        if constexpr (EPI == AT_SOFTMAX) {
+            // softmax(alpha * A B^T) over the key axis: the tile holds every key (N <= BN); a row's values sit in one quad
+            float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+            for (int j = 0; j < BN / 2; ++j)
+                if (n0 + frag_col(tid, j) < N) mx[(j >> 1) & 1] = fmaxf(mx[(j >> 1) & 1], alpha * acc[0][j]);
+            float sum[2] = {0.f, 0.f}, m2[2];
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+                mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
+                m2[h] = -mx[h] * 1.4426950408889634f;
+            }
+            const float a2 = alpha * 1.4426950408889634f;
+#pragma unroll
+            for (int j = 0; j < BN / 2; ++j) {
+                const float e = (n0 + frag_col(tid, j) < N) ? ex2_approx(fmaf(a2, acc[0][j], m2[(j >> 1) & 1])) : 0.f;
+                acc[0][j] = e;
+                sum[(j >> 1) & 1] += e;
+            }
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                sum[h] += __shfl_xor_sync(0xffffffffu, sum[h], 1);
+                sum[h] += __shfl_xor_sync(0xffffffffu, sum[h], 2);
+                sum[h] = 1.0f / sum[h];
+            }
+#pragma unroll
+            for (int j = 0; j < BN / 2; j += 2) {
+                const int r = m0 + frag_row(tid, j), col = n0 + frag_col(tid, j);
+                if (r >= N || col >= ncols) continue;
+                const float inv = sum[(j >> 1) & 1];
+                *reinterpret_cast<float2*>(out + ((long long)bh * N + r) * ld_out + col) = make_float2(acc[0][j] * inv, acc[0][j + 1] * inv);
+            }
+        } else {
+#pragma unroll
+        for (int j = 0; j < BN / 2; j += 2) {
+            const int r = m0 + frag_row(tid, j), col = n0 + frag_col(tid, j);
+            if (r >= N || col >= ncols) continue;
+            const long long off = ((long long)bh * N + r) * ld_out + col;
+            float2 e = make_float2(0.f, 0.f);
+            if (EPI != AT_STORE) e = *reinterpret_cast<const float2*>(E + off);
+            float v[2] = {alpha * acc[0][j], alpha * acc[0][j + 1]};
+            const float ee[2] = {e.x, e.y};
+#pragma unroll
+            for (int u = 0; u < 2; ++u) {
+                if (EPI == AT_MUL) v[u] *= ee[u];
+                else if (EPI == AT_SD) v[u] = te_sd_fast(ee[u], v[u]);
+                if (col + u >= N) v[u] = 0.f;
+            }
+            *reinterpret_cast<float2*>(out + off) = make_float2(v[0], v[1]);
+        }
+        }
+    }
+};
+
+// ---- token-reduced N x d contraction: out[b, m, h*BN + d] = epi(alpha * sum_k A_h[m,k] X[b, k, h*BN + d]) ----------------
+//   AMN 0: A_h[m,k] = map[bh][m][k] (K-major) ; AMN 1: A_h[m,k] = map[bh][k][m] (MN-major, transposed on load)
+//   X is MN-major (transposed on load).  a_shared: A indexed by the batch only (dense rollout product, "heads" = column tiles).
+template <int AMN, int EPI, bool SP, int BN_>
+struct NkProb : NoScale {
+    static constexpr int BN = BN_, NACC = 1, CHUNK = SP ? 0 : 4;
+    static constexpr int BT = BN * 128;
+    static constexpr int STAGE = SP ? TILE128 + BT : 2 * (TILE128 + BT);
+    int N, H, NP, ld_out, n_out, n_pad, a_shared;
+    const float* map; const float* X; long long ldx;
+    const float* rowscale; const float* E; float* out; float alpha;
+    __device__ int kblocks() const { return (N + 31) / 32; }
+    template <class F>
+    __device__ __forceinline__ void load_a(int kb, int m0, int bh, int tid, F f) const {
+        const int s = bh / H;
+        const float* base = map + (long long)(a_shared ? s : bh) * N * NP;
+        if (AMN == 0) for_k32(BM, base, NP, m0, N, kb * 32, N, tid, f);
+        else for_mn32(BM, base, NP, m0, N, kb * 32, N, tid, f);
+    }
+    __device__ void load(uint8_t* st, int kb, int m0, int, int bh, int tid) const {
+        const int s = bh / H, h = bh % H;
+        const float* xb = X + (long long)s * N * ldx;
+        if (SP) {
+            load_a(kb, m0, bh, tid, [&](int r, int c, float4 v) { st4(st, r, c, tf32x4(v)); });
+            for_mn32(BN, xb, ldx, h * BN, n_pad, kb * 32, N, tid, [&](int r, int c, float4 v) { st4(st + TILE128, r, c, tf32x4(v)); });
+        } else {
+            load_a(kb, m0, bh, tid, [&](int r, int c, float4 v) { st_split(st, st + TILE128, r, c, v); });
+            for_mn32(BN, xb, ldx, h * BN, n_pad, kb * 32, N, tid,
+                     [&](int r, int c, float4 v) { st_split(st + 2 * TILE128, st + 2 * TILE128 + BT, r, c, v); });
+        }
+    }
+    __device__ void mma(uint32_t st, int wg, float (&acc)[1][BN / 2], uint32_t sd) const {
+        const uint32_t aoff = (uint32_t)wg * 64u * 128u;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const uint64_t q = (uint64_t)(2 * k);
+            if (SP) {
+                wgmma_tf32(acc[0], sdesc(st + aoff) + q, sdesc(st + TILE128) + q, (k == 0) ? sd : 1u);
+            } else {
+                const uint64_t ah = sdesc(st + aoff), al = sdesc(st + TILE128 + aoff), bhd = sdesc(st + 2 * TILE128),
+                               bld = sdesc(st + 2 * TILE128 + BT);
+                wgmma_tf32(acc[0], al + q, bhd + q, (k == 0) ? sd : 1u);
+                wgmma_tf32(acc[0], ah + q, bld + q, 1u);
+                wgmma_tf32(acc[0], ah + q, bhd + q, 1u);
+            }
+        }
+    }
+    __device__ void epilogue(float (&acc)[1][BN / 2], int m0, int, int bh, int tid) const {
+        const int s = bh / H, h = bh % H;
+#pragma unroll
+        for (int j = 0; j < BN / 2; j += 2) {
+            const int m = m0 + frag_row(tid, j), gcol = h * BN + frag_col(tid, j);
+            if (m >= N || gcol >= n_pad) continue;
+            const long long off = ((long long)s * N + m) * ld_out + gcol;
+            float v[2] = {alpha * acc[0][j], alpha * acc[0][j + 1]};
+            if (EPI == AT_MUL) {
+                const float2 e = *reinterpret_cast<const float2*>(E + off);
+                v[0] *= e.x; v[1] *= e.y;
+            } else if (EPI == AT_RESID) {
+                // the identity's share of the rollout step, added in fp32: out = A J + diag(rowscale) J
+                const float rsc = rowscale ? rowscale[(long long)s * N + m] : 1.f;
+                const float2 e = *reinterpret_cast<const float2*>(E + off);
+                v[0] += rsc * e.x; v[1] += rsc * e.y;
+            }
+            if (gcol >= n_out) v[0] = 0.f;
+            if (gcol + 1 >= n_out) v[1] = 0.f;
+            *reinterpret_cast<float2*>(out + off) = make_float2(v[0], v[1]);
+        }
+    }
+};
+
+// ---- launch ---------------------------------------------------------------------------------------------------------
+inline bool a16(const void* p) { return ((uintptr_t)p & 15u) == 0; }
+
+template <class P>
+int launch(const P& p, dim3 grid, cudaStream_t st) {
+    constexpr int SMEM = 2 * P::STAGE + 1024;
+    // cudaFuncAttributeMaxDynamicSharedMemorySize is per device: one bit per device ordinal
+    static unsigned long long done = 0;
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess) { te_set_last_error("te_tc: cudaGetDevice failed"); return TE_ERR_CUDA; }
+    if (!(done & (1ull << (dev & 63)))) {
+        if (cudaFuncSetAttribute(wg_kernel<P>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM) != cudaSuccess) {
+            te_set_last_error("te_tc: cannot raise dynamic shared memory");
+            return TE_ERR_CUDA;
+        }
+        done |= 1ull << (dev & 63);
+    }
+    if (grid.y > 65535 || grid.z > 65535) { te_set_last_error("te_tc: grid too large for one launch"); return TE_ERR_ARG; }
+    wg_kernel<P><<<grid, NTHREADS, SMEM, st>>>(p);
+    TE_CUDA_CHECK_LAUNCH();
+    return TE_OK;
+}
+inline unsigned mtiles(long long M) { return (unsigned)((M + BM - 1) / BM); }
+
+// ---- weight preparation: W [out,in] -> the derived operand copies of te_gemm_tc.h ------------------------------------
+__global__ void prepare_weights_kernel(const float* __restrict__ w, float* __restrict__ d, int out_f, int in_f) {
+    const long long n = (long long)out_f * in_f;
+    float *wp = d, *wn = d + n, *wpt = d + 2 * n, *wnt = d + 3 * n, *wh = d + 4 * n, *wl = d + 5 * n, *wth = d + 6 * n,
+          *wtl = d + 7 * n, *wa = d + 8 * n;
+    __shared__ float tile[32][33];
+    const int bx = blockIdx.x * 32, by = blockIdx.y * 32;      // bx: in index, by: out index
+    for (int i = threadIdx.y; i < 32; i += blockDim.y) {
+        const int o = by + i, c = bx + threadIdx.x;
+        float v = 0.f;
+        if (o < out_f && c < in_f) {
+            const long long idx = (long long)o * in_f + c;
+            v = w[idx];
+            wp[idx] = to_tf32(fmaxf(v, 0.f));
+            wn[idx] = to_tf32(fminf(v, 0.f));
+            const float hi = to_tf32(v);
+            wh[idx] = hi;
+            wl[idx] = to_tf32(v - hi);
+            wa[idx] = to_tf32(fabsf(v));
+            reinterpret_cast<__nv_bfloat16*>(d + 11 * n)[idx] = __float2bfloat16_rn(fabsf(v));      // bf16(|W|): bf16 S1 kernel
+        }
+        tile[i][threadIdx.x] = v;
+    }
+    __syncthreads();
+    for (int i = threadIdx.y; i < 32; i += blockDim.y) {
+        const int c = bx + i, o = by + threadIdx.x;
+        if (o < out_f && c < in_f) {
+            const float v = tile[threadIdx.x][i];
+            const long long idx = (long long)c * out_f + o;
+            wpt[idx] = to_tf32(fmaxf(v, 0.f));
+            wnt[idx] = to_tf32(fminf(v, 0.f));
+            __nv_bfloat16* bp = reinterpret_cast<__nv_bfloat16*>(d + 9 * n);
+            bp[idx] = __float2bfloat16_rn(fmaxf(v, 0.f));
+            bp[n + idx] = __float2bfloat16_rn(fminf(v, 0.f));
+            const float hi = to_tf32(v);
+            wth[idx] = hi;
+            wtl[idx] = to_tf32(v - hi);
+        }
+    }
+}
+
+// ---- fp16 split pre-passes ------------------------------------------------------------------------------------------
+// Activations: one warp per row, one scale block per warp iteration (128 columns): single pass, one read of x.
+__global__ void __launch_bounds__(256) blocksplit_f16_kernel(const float* __restrict__ x, long long ldx, long long rows, int cols,
+                                                             __half* __restrict__ hi, __half* __restrict__ lo,
+                                                             float* __restrict__ inv) {
+    const int lane = threadIdx.x & 31;
+    const long long wpb = blockDim.x >> 5;
+    const int nblk = (cols + 127) / 128;
+    for (long long row = blockIdx.x * wpb + (threadIdx.x >> 5); row < rows; row += (long long)gridDim.x * wpb) {
+        const float* xr = x + row * ldx;
+#pragma unroll 2
+        for (int base = 0; base < cols; base += 128) {
+            const int i = base + lane * 4;
+            float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (i < cols) v = *reinterpret_cast<const float4*>(xr + i);
+            float s, si;
+            te_f16_block_scale(te_warp_max(te_absmax4(v)), s, si);
+            if (i < cols) {
+                uint2 h, l;
+                te_f16_split4(v, s, h, l);
+                *reinterpret_cast<uint2*>(hi + row * cols + i) = h;
+                if (lo) *reinterpret_cast<uint2*>(lo + row * cols + i) = l;
+            }
+            if (lane == 0) inv[row * nblk + base / 128] = si;
+        }
+    }
+}
+// Weights: one scale per row of W (two passes over the row; the second hits L1 / L2).
+__global__ void __launch_bounds__(256) rowsplit_f16_kernel(const float* __restrict__ x, long long ldx, long long rows, int cols4,
+                                                           __half* __restrict__ hi, __half* __restrict__ lo,
+                                                           float* __restrict__ inv) {
+    const int lane = threadIdx.x & 31;
+    const long long wpb = blockDim.x >> 5;
+    for (long long row = blockIdx.x * wpb + (threadIdx.x >> 5); row < rows; row += (long long)gridDim.x * wpb) {
+        const float4* xr = reinterpret_cast<const float4*>(x + row * ldx);
+        float m = 0.f;
+#pragma unroll 4
+        for (int c = lane; c < cols4; c += 32) m = fmaxf(m, te_absmax4(xr[c]));
+        float s, si;
+        te_f16_block_scale(te_warp_max(m), s, si);
+        uint2* hr = reinterpret_cast<uint2*>(hi + row * (long long)cols4 * 4);
+        uint2* lr = reinterpret_cast<uint2*>(lo + row * (long long)cols4 * 4);
+#pragma unroll 4
+        for (int c = lane; c < cols4; c += 32) {
+            uint2 h, l;
+            te_f16_split4(xr[c], s, h, l);
+            hr[c] = h;
+            if (lo) lr[c] = l;
+        }
+        if (lane == 0) inv[row] = si;
+    }
+}
+// |x| as bf16: the A operand of the bf16 single-pass S kernel.  x rows at stride ldx -> compact [rows, cols].
+__global__ void abs_bf16_kernel(const float* __restrict__ x, long long ldx, __nv_bfloat16* __restrict__ out, long long rows, int cols4) {
+    const long long total = rows * cols4;
+    for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < total; t += (long long)gridDim.x * blockDim.x) {
+        const long long r = t / cols4;
+        const int c = (int)(t - r * cols4);
+        const float4 v = *reinterpret_cast<const float4*>(x + r * ldx + 4 * c);
+        const __nv_bfloat162 a = __floats2bfloat162_rn(fabsf(v.x), fabsf(v.y)), b = __floats2bfloat162_rn(fabsf(v.z), fabsf(v.w));
+        uint2 pk;
+        pk.x = *reinterpret_cast<const uint32_t*>(&a);
+        pk.y = *reinterpret_cast<const uint32_t*>(&b);
+        *reinterpret_cast<uint2*>(out + t * 4) = pk;
+    }
+}
+// grid of a grid-stride elementwise pass: at most 16 blocks per SM
+unsigned stride_blocks(long long work, int per_block) {
+    static int sms[64];
+    int dev = 0;
+    cudaGetDevice(&dev);
+    int& n = sms[dev & 63];
+    if (n == 0 && cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) n = 1;
+    long long b = (work + per_block - 1) / per_block;
+    const long long cap = (long long)n * 16;
+    if (b > cap) b = cap;
+    return (unsigned)(b < 1 ? 1 : b);
+}
+
+template <int EPI>
+int lin3(const float* a, long long lda, const float* bh, const float* bl, int K, const LinOut& o, cudaStream_t st) {
+    Lin3Prob<EPI> p;
+    p.K = K; p.a = a; p.lda = lda; p.bh = bh; p.bl = bl; p.o = o;
+    return launch(p, dim3(mtiles(o.M), o.N / 128), st);
+}
+template <int EPI, int TERMS>
+int f16(const __half* ah, const __half* al, const __half* bh, const __half* bl, const float* rs, const float* cs, int K,
+        const LinOut& o, cudaStream_t st) {
+    F16Prob<EPI, TERMS> p;
+    p.K = K; p.ah = ah; p.al = al; p.bh = bh; p.bl = bl; p.rs = rs; p.rs_ld = (K + 127) / 128; p.cs = cs; p.o = o;
+    return launch(p, dim3(mtiles(o.M), o.N / 128), st);
+}
+LinOut lin_out(long long rows, int N, const float* bias, const float* e0, float* y, float* y2) {
+    LinOut o;
+    o.M = (int)rows; o.N = N; o.bias = bias; o.E = e0; o.lde = N; o.C = y; o.ldc = N; o.C2 = y2; o.ldc2 = N;
+    return o;
+}
+
+template <bool SINGLE, bool BF, int OUT>
+int zs(const ZsProb<SINGLE, BF, OUT>& p, cudaStream_t st) { return launch(p, dim3(mtiles(p.M), p.N / 128), st); }
+
+}  // namespace
+
+// =====================================================================================================================
+// public entry points (te_gemm_tc.h)
+// =====================================================================================================================
+long long te_tc_derived_floats(int in_features, int out_features) { return 16LL * in_features * out_features; }
+
+int te_tc_prepare_weights(const float* w, float* derived, int in_features, int out_features, cudaStream_t st) {
+    dim3 grid((in_features + 31) / 32, (out_features + 31) / 32), block(32, 8);
+    prepare_weights_kernel<<<grid, block, 0, st>>>(w, derived, out_features, in_features);
+    TE_CUDA_CHECK_LAUNCH();
+    const long long n = (long long)in_features * out_features;
+    if (in_features % 8 == 0 && in_features >= 8 && a16(w))        // row-scaled fp16 split: [hi | lo | 2^-f] from 11.5 n
+        TE_TRY(te_tc_rowsplit_f16(w, in_features, out_features, in_features, derived + 11 * n + n / 2, derived + 12 * n,
+                                  derived + 12 * n + n / 2, st));
+    if (out_features % 8 == 0 && in_features >= 2) {               // single-pass fp16 operands from the TF32-rounded transposes [in, out]
+        TE_TRY(te_tc_rowsplit_f16(derived + 6 * n, out_features, in_features, out_features, derived + 13 * n, nullptr,
+                                  derived + 13 * n + n / 2, st));
+        TE_TRY(te_tc_rowsplit_f16(derived + 2 * n, out_features, in_features, out_features, derived + 14 * n, nullptr,
+                                  derived + 15 * n, st));
+        TE_TRY(te_tc_rowsplit_f16(derived + 3 * n, out_features, in_features, out_features, derived + 14 * n + n / 2, nullptr,
+                                  derived + 15 * n + in_features, st));
+    }
+    return TE_OK;
+}
+
+int te_tc_rowsplit_f16(const float* x, long long ldx, long long rows, int cols, void* hi, void* lo, float* scale_inv,
+                       cudaStream_t st) {
+    if (cols % 4 != 0 || ldx % 4 != 0 || !a16(x) || ((uintptr_t)hi & 7u) || (lo && ((uintptr_t)lo & 7u))) {
+        te_set_last_error("te_tc_rowsplit_f16: alignment");
+        return TE_ERR_ARG;
+    }
+    rowsplit_f16_kernel<<<stride_blocks(rows, 8), 256, 0, st>>>(x, ldx, rows, cols / 4, reinterpret_cast<__half*>(hi),
+                                                                reinterpret_cast<__half*>(lo), scale_inv);
+    TE_CUDA_CHECK_LAUNCH();
+    return TE_OK;
+}
+
+int te_tc_blocksplit_f16(const float* x, long long ldx, long long rows, int cols, float* split, float* scale_inv, cudaStream_t st,
+                         bool hi_only) {
+    if (cols % 4 != 0 || ldx % 4 != 0 || !a16(x) || !a16(split) || !scale_inv) {
+        te_set_last_error("te_tc_blocksplit_f16: alignment");
+        return TE_ERR_ARG;
+    }
+    __half* hi = reinterpret_cast<__half*>(split);
+    blocksplit_f16_kernel<<<stride_blocks(rows, 8), 256, 0, st>>>(x, ldx, rows, cols, hi, hi_only ? nullptr : hi + rows * cols,
+                                                                  scale_inv);
+    TE_CUDA_CHECK_LAUNCH();
+    return TE_OK;
+}
+
+// ---- z+ rule --------------------------------------------------------------------------------------------------------
+bool te_tc_zplus_supported(long long rows, int in_features, int out_features, long long ldx) {
+    return rows > 0 && rows < (1LL << 31) && in_features % 128 == 0 && out_features % 128 == 0 && ldx % 4 == 0;
+}
+bool te_tc_pair_supported(long long rows, int K, int N, long long lda) {
+    return rows > 0 && rows < (1LL << 31) && K % 32 == 0 && N % 128 == 0 && lda % 4 == 0;
+}
+
+int te_tc_pair_zplus_s1(const float* x, long long ldx, float* xabs, const float* derived, const float* r, long long ldr,
+                        const float* y, long long ldy, const float* bias, float* s_out, long long rows, int in_features,
+                        int out_features, cudaStream_t st, bool bf16, float* s16, float* s16_scale) {
+    const long long n = (long long)in_features * out_features;
+    if (ldx % 4 != 0 || !a16(x) || !a16(r) || !a16(y) || ldr % 2 != 0 || ldy % 2 != 0) {
+        te_set_last_error("te_tc_pair_zplus_s1: alignment");
+        return TE_ERR_ARG;
+    }
+    auto fill = [&](auto& p) {
+        p.M = (int)rows; p.N = out_features; p.K = in_features;
+        p.x = x; p.ldx = ldx; p.xabs = xabs; p.wb = nullptr;
+        p.r = r; p.ldr = ldr; p.y = y; p.ldy = ldy; p.bias = bias;
+        p.out = s16 ? (void*)s16 : (void*)s_out; p.ldo = out_features; p.hs = s16_scale;
+    };
+    if (bf16 && in_features % 64 == 0) {
+        if (!a16(xabs)) { te_set_last_error("te_tc_pair_zplus_s1: alignment"); return TE_ERR_ARG; }
+        abs_bf16_kernel<<<stride_blocks(rows * (in_features / 4), 256), 256, 0, st>>>(
+            x, ldx, reinterpret_cast<__nv_bfloat16*>(xabs), rows, in_features / 4);
+        TE_CUDA_CHECK_LAUNCH();
+        if (s16) { ZsProb<true, true, ZO_F16S> p; fill(p); p.wa = derived + 11 * n; return zs(p, st); }
+        ZsProb<true, true, ZO_F32> p; fill(p); p.wa = derived + 11 * n; return zs(p, st);
+    }
+    if (s16) { ZsProb<true, false, ZO_F16S> p; fill(p); p.wa = derived + 8 * n; return zs(p, st); }
+    ZsProb<true, false, ZO_F32> p; fill(p); p.wa = derived + 8 * n; return zs(p, st);
+}
+
+int te_tc_pair_zplus_r(const float* s, const float* derived, const float* x, long long ldx, float* out, long long ld_out,
+                       long long rows, int in_features, int out_features, cudaStream_t st) {
+    const long long n = (long long)in_features * out_features;
+    ZrProb<0> p;
+    memset(&p, 0, sizeof(p));
+    p.M = (int)rows; p.N = in_features; p.K = out_features;
+    p.s = s; p.wp = derived + 2 * n; p.wn = derived + 3 * n; p.x = x; p.ldx = ldx; p.out = out; p.ldo = ld_out;
+    return launch(p, dim3(mtiles(rows), in_features / 128), st);
+}
+
+int te_tc_zplus_r16(const float* s, float* split, float* scale, const float* derived, const float* x, long long ldx, float* out,
+                    long long ld_out, long long rows, int in_features, int out_features, cudaStream_t st) {
+    const long long n = (long long)in_features * out_features;
+    if (!a16(split) || !scale || !a16(derived) || !a16(x) || !a16(out) || ldx % 4 != 0 || ld_out % 4 != 0) {
+        te_set_last_error("te_tc_zplus_r16: bad operands");
+        return TE_ERR_ARG;
+    }
+    if (s) TE_TRY(te_tc_blocksplit_f16(s, out_features, rows, out_features, split, scale, st, true));
+    ZrProb<2> p;
+    p.M = (int)rows; p.N = in_features; p.K = out_features;
+    p.s = split; p.wp = derived + 14 * n; p.wn = derived + 14 * n + n / 2;
+    p.rs = scale; p.rs_ld = (out_features + 127) / 128; p.cp = derived + 15 * n; p.cn = derived + 15 * n + in_features;
+    p.x = x; p.ldx = ldx; p.out = out; p.ldo = ld_out;
+    return launch(p, dim3(mtiles(rows), in_features / 64), st);
+}
+
+int te_tc_zplus_linear_relprop(const float* x, long long ldx, const float* derived, const float* r, long long ldr,
+                               float* out, float* s_scratch, long long rows, int in_features, int out_features, cudaStream_t st,
+                               const float* y, long long ldy, const float* bias, int bf16, long long ld_out, float* xabs) {
+    if (ld_out == 0) ld_out = in_features;
+    if (!a16(x) || !a16(derived) || !a16(r) || !a16(out) || !a16(s_scratch)) {
+        te_set_last_error("te_gemm_tc: operands must be 16-byte aligned");
+        return TE_ERR_ARG;
+    }
+    const long long n = (long long)in_features * out_features;
+    const bool single = y && a16(y) && ldy % 4 == 0 && (!bias || a16(bias));
+    const bool rb = (bf16 & 1) && (out_features % 64 == 0);          // S as bf16, R kernel with bf16 operands
+    if (!rb && single && xabs && a16(xabs)) {
+        if ((bf16 & 4) && te_tc_f16_single_supported(rows, out_features, in_features, out_features)) {
+            // second contraction on block-scaled fp16: S leaves the S kernel in that format, straight into s_scratch
+            // ([rows, out] fp16, then the [rows, out/128] scales: rows*out floats hold both)
+            float* s16_scale = s_scratch + ((rows * out_features / 2 + 63) & ~63LL);
+            TE_TRY(te_tc_pair_zplus_s1(x, ldx, xabs, derived, r, ldr, y, ldy, bias, nullptr, rows, in_features, out_features, st,
+                                       (bf16 & 2) != 0, s_scratch, s16_scale));
+            return te_tc_zplus_r16(nullptr, s_scratch, s16_scale, derived, x, ldx, out, ld_out, rows, in_features, out_features, st);
+        }
+        TE_TRY(te_tc_pair_zplus_s1(x, ldx, xabs, derived, r, ldr, y, ldy, bias, s_scratch, rows, in_features, out_features, st,
+                                   (bf16 & 2) != 0));
+        return te_tc_pair_zplus_r(s_scratch, derived, x, ldx, out, ld_out, rows, in_features, out_features, st);
+    }
+    // S = sd(R, Z) [rows, out]
+    if (single) {
+        if (rb) {
+            ZsProb<true, false, ZO_BF16> p;
+            p.M = (int)rows; p.N = out_features; p.K = in_features; p.x = x; p.ldx = ldx; p.xabs = nullptr;
+            p.wa = derived + 8 * n; p.wb = nullptr; p.r = r; p.ldr = ldr; p.y = y; p.ldy = ldy; p.bias = bias;
+            p.out = s_scratch; p.ldo = out_features; p.hs = nullptr;
+            TE_TRY(zs(p, st));
+        } else {
+            ZsProb<true, false, ZO_F32> p;
+            p.M = (int)rows; p.N = out_features; p.K = in_features; p.x = x; p.ldx = ldx; p.xabs = nullptr;
+            p.wa = derived + 8 * n; p.wb = nullptr; p.r = r; p.ldr = ldr; p.y = y; p.ldy = ldy; p.bias = bias;
+            p.out = s_scratch; p.ldo = out_features; p.hs = nullptr;
+            TE_TRY(zs(p, st));
+        }
+    } else if (rb) {
+        ZsProb<false, false, ZO_BF16> p;
+        p.M = (int)rows; p.N = out_features; p.K = in_features; p.x = x; p.ldx = ldx; p.xabs = nullptr;
+        p.wa = derived; p.wb = derived + n; p.r = r; p.ldr = ldr; p.y = nullptr; p.ldy = 0; p.bias = nullptr;
+        p.out = s_scratch; p.ldo = out_features; p.hs = nullptr;
+        TE_TRY(zs(p, st));
+    } else {
+        ZsProb<false, false, ZO_F32> p;
+        p.M = (int)rows; p.N = out_features; p.K = in_features; p.x = x; p.ldx = ldx; p.xabs = nullptr;
+        p.wa = derived; p.wb = derived + n; p.r = r; p.ldr = ldr; p.y = nullptr; p.ldy = 0; p.bias = nullptr;
+        p.out = s_scratch; p.ldo = out_features; p.hs = nullptr;
+        TE_TRY(zs(p, st));
+    }
+    if (rb) {
+        ZrProb<1> p;
+        memset(&p, 0, sizeof(p));
+        p.M = (int)rows; p.N = in_features; p.K = out_features;
+        p.s = s_scratch; p.wp = derived + 9 * n; p.wn = (const __nv_bfloat16*)(derived + 9 * n) + n;
+        p.x = x; p.ldx = ldx; p.out = out; p.ldo = ld_out;
+        return launch(p, dim3(mtiles(rows), in_features / 128), st);
+    }
+    return te_tc_pair_zplus_r(s_scratch, derived, x, ldx, out, ld_out, rows, in_features, out_features, st);
+}
+
+// ---- Linear GEMMs ---------------------------------------------------------------------------------------------------
+bool te_tc_gemm3x_supported(long long rows, int K, int N, long long lda) {
+    return rows > 0 && rows < (1LL << 31) && K % 32 == 0 && N % 128 == 0 && lda % 4 == 0;
+}
+
+int te_tc_linear_fwd(const float* x, long long ldx, const float* derived, int in_features, int out_features, const float* bias,
+                     float* y, float* y2, const float* e0, long long rows, int epi, cudaStream_t st) {
+    const long long n = (long long)in_features * out_features;
+    if (!a16(x) || !a16(derived) || !a16(y) || (y2 && !a16(y2)) || (e0 && !a16(e0)) || (bias && !a16(bias))) {
+        te_set_last_error("te_tc_linear_fwd: operands must be 16-byte aligned");
+        return TE_ERR_ARG;
+    }
+    const LinOut o = lin_out(rows, out_features, bias, e0, y, y2);
+    const float *bh = derived + 4 * n, *bl = derived + 5 * n;
+    switch (epi) {
+        case TE_TC_EPI_STORE: return lin3<TE_TC_EPI_STORE>(x, ldx, bh, bl, in_features, o, st);
+        case TE_TC_EPI_BIAS: return lin3<TE_TC_EPI_BIAS>(x, ldx, bh, bl, in_features, o, st);
+        case TE_TC_EPI_BIAS_GELU: return lin3<TE_TC_EPI_BIAS_GELU>(x, ldx, bh, bl, in_features, o, st);
+        case TE_TC_EPI_BIAS_ADD: return lin3<TE_TC_EPI_BIAS_ADD>(x, ldx, bh, bl, in_features, o, st);
+    }
+    te_set_last_error("te_tc_linear_fwd: unsupported epilogue");
+    return TE_ERR_UNSUPPORTED;
+}
+
+int te_tc_linear_bwd(const float* dy, const float* derived, int in_features, int out_features, float* dx, const float* e0,
+                     long long rows, int epi, cudaStream_t st) {
+    const long long n = (long long)in_features * out_features;
+    if (!a16(dy) || !a16(derived) || !a16(dx) || (e0 && !a16(e0))) {
+        te_set_last_error("te_tc_linear_bwd: operands must be 16-byte aligned");
+        return TE_ERR_ARG;
+    }
+    const LinOut o = lin_out(rows, in_features, nullptr, e0, dx, nullptr);
+    if (epi == TE_TC_EPI_STORE) return lin3<TE_TC_EPI_STORE>(dy, out_features, derived + 6 * n, derived + 7 * n, out_features, o, st);
+    if (epi == TE_TC_EPI_GELU_BWD) return lin3<TE_TC_EPI_GELU_BWD>(dy, out_features, derived + 6 * n, derived + 7 * n, out_features, o, st);
+    te_set_last_error("te_tc_linear_bwd: unsupported epilogue");
+    return TE_ERR_UNSUPPORTED;
+}
+
+int te_tc_pair_linear_bwd(const float* dy, long long lddy, const float* derived, int in_features, int out_features, float* dx,
+                          const float* e0, long long rows, int epi, cudaStream_t st) {
+    const long long n = (long long)in_features * out_features;
+    if (!a16(dy) || lddy % 4 != 0 || !a16(derived) || !a16(dx) || (e0 && !a16(e0))) {
+        te_set_last_error("te_tc_pair_linear_bwd: operands must be 16-byte aligned");
+        return TE_ERR_ARG;
+    }
+    const LinOut o = lin_out(rows, in_features, nullptr, e0, dx, nullptr);
+    const dim3 grid(mtiles(rows), in_features / 128);
+    if (epi == TE_TC_EPI_STORE) {
+        Lin1Prob<TE_TC_EPI_STORE> p; p.K = out_features; p.a = dy; p.lda = lddy; p.b = derived + 6 * n; p.o = o;
+        return launch(p, grid, st);
+    }
+    if (epi == TE_TC_EPI_GELU_BWD) {
+        Lin1Prob<TE_TC_EPI_GELU_BWD> p; p.K = out_features; p.a = dy; p.lda = lddy; p.b = derived + 6 * n; p.o = o;
+        return launch(p, grid, st);
+    }
+    te_set_last_error("te_tc_pair_linear_bwd: unsupported epilogue");
+    return TE_ERR_UNSUPPORTED;
+}
+
+bool te_tc_fwd16_supported(long long rows, int K, int N, long long lda) {
+    return rows > 0 && rows < (1LL << 31) && K % 64 == 0 && N % 128 == 0 && lda % 4 == 0;
+}
+bool te_tc_f16_single_supported(long long rows, int K, int N, long long lda) { return te_tc_fwd16_supported(rows, K, N, lda); }
+
+int te_tc_linear_fwd16(const float* x, long long ldx, float* split, float* scale, const float* derived, int in_features,
+                       int out_features, const float* bias, float* y, float* y2, const float* e0, long long rows, int epi,
+                       cudaStream_t st, float* split_out, float* scale_out) {
+    const long long n = (long long)in_features * out_features;
+    if (!a16(split) || !scale || !a16(derived) || !a16(y) || (y2 && !a16(y2)) || (e0 && !a16(e0)) || (bias && !a16(bias)) ||
+        (split_out && (!a16(split_out) || !scale_out || !y2 || epi != TE_TC_EPI_BIAS_GELU))) {
+        te_set_last_error("te_tc_linear_fwd16: bad operands");
+        return TE_ERR_ARG;
+    }
+    const __half* ah = reinterpret_cast<const __half*>(split);
+    const __half* al = ah + rows * in_features;
+    if (x) TE_TRY(te_tc_blocksplit_f16(x, ldx, rows, in_features, split, scale, st));
+    const __half* bh = reinterpret_cast<const __half*>(derived + 11 * n + n / 2);
+    const __half* bl = reinterpret_cast<const __half*>(derived + 12 * n);
+    const float* cs = derived + 12 * n + n / 2;
+    const LinOut o = lin_out(rows, out_features, bias, e0, y, y2);
+    switch (epi) {
+        case TE_TC_EPI_STORE: return f16<TE_TC_EPI_STORE, 3>(ah, al, bh, bl, scale, cs, in_features, o, st);
+        case TE_TC_EPI_BIAS: return f16<TE_TC_EPI_BIAS, 3>(ah, al, bh, bl, scale, cs, in_features, o, st);
+        case TE_TC_EPI_BIAS_GELU:
+            TE_TRY((f16<TE_TC_EPI_BIAS_GELU, 3>(ah, al, bh, bl, scale, cs, in_features, o, st)));
+            // the next Linear's A operand: the block-scaled split of y2 = gelu(y)
+            if (split_out) return te_tc_blocksplit_f16(y2, out_features, rows, out_features, split_out, scale_out, st);
+            return TE_OK;
+        case TE_TC_EPI_BIAS_ADD: return f16<TE_TC_EPI_BIAS_ADD, 3>(ah, al, bh, bl, scale, cs, in_features, o, st);
+    }
+    te_set_last_error("te_tc_linear_fwd16: unsupported epilogue");
+    return TE_ERR_UNSUPPORTED;
+}
+
+int te_tc_linear_bwd16(const float* dy, long long lddy, float* split, float* scale, const float* derived, int in_features,
+                       int out_features, float* dx, const float* e0, long long rows, int epi, cudaStream_t st) {
+    const long long n = (long long)in_features * out_features;
+    if (!a16(split) || !scale || !a16(derived) || !a16(dx) || (e0 && !a16(e0))) {
+        te_set_last_error("te_tc_linear_bwd16: bad operands");
+        return TE_ERR_ARG;
+    }
+    if (dy) TE_TRY(te_tc_blocksplit_f16(dy, lddy, rows, out_features, split, scale, st, true));
+    const __half* ah = reinterpret_cast<const __half*>(split);
+    const __half* bt = reinterpret_cast<const __half*>(derived + 13 * n);
+    const float* cs = derived + 13 * n + n / 2;
+    const LinOut o = lin_out(rows, in_features, nullptr, e0, dx, nullptr);
+    if (epi == TE_TC_EPI_GELU_BWD) return f16<TE_TC_EPI_GELU_BWD, 1>(ah, nullptr, bt, nullptr, scale, cs, out_features, o, st);
+    if (epi == TE_TC_EPI_STORE) return f16<TE_TC_EPI_STORE, 1>(ah, nullptr, bt, nullptr, scale, cs, out_features, o, st);
+    te_set_last_error("te_tc_linear_bwd16: unsupported epilogue");
+    return TE_ERR_UNSUPPORTED;
+}
+
+// ---- attention-shaped contractions -------------------------------------------------------------------------------------
+bool te_tc_attn_supported(int N, int dh, long long lda, long long ldb, int ld_out) {
+    return N >= 1 && (dh == 32 || dh == 64) && lda % 4 == 0 && ldb % 4 == 0 && ld_out % 4 == 0;
+}
+bool te_tc_attn_nk_supported(int N, int dh, int NP, long long ldx, long long ld_out) {
+    return N >= 1 && dh == 64 && NP % 4 == 0 && ldx % 4 == 0 && ld_out % 4 == 0;
+}
+bool te_tc_bmm_nk_supported(int N, int ld) { return N >= 1 && ld % 4 == 0 && ld >= N; }
+
+namespace {
+template <int EPI, bool SP, int BN>
+int nn(const float* A, long long lda, const float* B, long long ldb, int batch, int H, int N, int dh, float* out, int ld_out,
+       const float* E, float alpha, cudaStream_t st) {
+    NnProb<EPI, SP, BN> p;
+    p.N = N; p.H = H; p.dh = dh; p.ld_out = ld_out; p.batch = batch;
+    p.a = A; p.lda = lda; p.b = B; p.ldb = ldb; p.E = E; p.out = out; p.alpha = alpha;
+    return launch(p, dim3(mtiles(N), (unsigned)((N + BN - 1) / BN), (unsigned)(batch * H)), st);
+}
+template <int AMN, int EPI, bool SP, int BN>
+int nk(const float* map, int NP, const float* X, long long ldx, int batch, int H, int N, float* out, int ld_out, int n_out,
+       int n_pad, int a_shared, const float* rowscale, const float* E, float alpha, cudaStream_t st) {
+    NkProb<AMN, EPI, SP, BN> p;
+    p.N = N; p.H = H; p.NP = NP; p.ld_out = ld_out; p.n_out = n_out; p.n_pad = n_pad; p.a_shared = a_shared;
+    p.map = map; p.X = X; p.ldx = ldx; p.rowscale = rowscale; p.E = E; p.out = out; p.alpha = alpha;
+    return launch(p, dim3(mtiles(N), 1, (unsigned)(batch * H)), st);
+}
+}  // namespace
+
+// out[b,h,i,j] = epi(alpha * sum_d A[b*N+i, h*dh+d] * B[b*N+j, h*dh+d]);  out / E are [batch,H,N,ld_out]
+int te_tc_attn_nn(const float* A, long long lda, const float* B, long long ldb, int batch, int H, int N, int dh,
+                  float* out, int ld_out, const float* E, float alpha, int epi, cudaStream_t st, bool single_pass) {
+#define TE_NN(EPI, SP, BN) nn<EPI, SP, BN>(A, lda, B, ldb, batch, H, N, dh, out, ld_out, E, alpha, st)
+    if (single_pass && epi == TE_TC_ATTN_STORE) return TE_NN(AT_STORE, true, 128);
+    if (single_pass && epi == TE_TC_ATTN_MUL) return TE_NN(AT_MUL, true, 128);
+    switch (epi) {
+        case TE_TC_ATTN_STORE: return TE_NN(AT_STORE, false, 128);
+        case TE_TC_ATTN_MUL: return TE_NN(AT_MUL, false, 128);
+        case TE_TC_ATTN_SD: return TE_NN(AT_SD, false, 128);
+        case TE_TC_ATTN_SOFTMAX:
+            if (N > 256) break;                       // the whole key axis must sit in one tile
+            return TE_NN(AT_SOFTMAX, false, 256);
+    }
+#undef TE_NN
+    te_set_last_error("te_gemm_tc: unsupported attention epilogue");
+    return TE_ERR_UNSUPPORTED;
+}
+
+// out[b, m, h, :] = epi(alpha * sum_k A_h[m,k] X[b,k,h,:]) ; A_h = map[b,h] (amn = 0) or its transpose (amn = 1);
+// X, out, E: packed activations [batch, N, ld] (head h at columns h*64..); epi: TE_TC_ATTN_STORE / TE_TC_ATTN_MUL
+int te_tc_attn_nk(const float* map, int NP, int amn, const float* X, long long ldx, int batch, int H, int N, float* out,
+                  int ld_out, const float* E, float alpha, int epi, cudaStream_t st, bool single_pass) {
+#define TE_NK(AMN, EPI, SP) nk<AMN, EPI, SP, 64>(map, NP, X, ldx, batch, H, N, out, ld_out, H * 64, H * 64, 0, nullptr, E, alpha, st)
+    if (epi == TE_TC_ATTN_STORE) {
+        if (single_pass) return amn ? TE_NK(1, AT_STORE, true) : TE_NK(0, AT_STORE, true);
+        return amn ? TE_NK(1, AT_STORE, false) : TE_NK(0, AT_STORE, false);
+    }
+    if (epi == TE_TC_ATTN_MUL) {
+        if (single_pass) return amn ? TE_NK(1, AT_MUL, true) : TE_NK(0, AT_MUL, true);
+        return amn ? TE_NK(1, AT_MUL, false) : TE_NK(0, AT_MUL, false);
+    }
+#undef TE_NK
+    te_set_last_error("te_gemm_tc: unsupported attention nk epilogue");
+    return TE_ERR_UNSUPPORTED;
+}
+
+// One step of the rollout chain in residual form: out[b] = A[b] * J[b] + diag(rowscale[b]) * J[b], all [batch, N, ld]
+// (fp32-grade 3xTF32).  The padding columns of out are zeroed so that it can be the next J.
+int te_tc_bmm_nk_resid(const float* A, const float* J, const float* rowscale, float* out, int batch, int N, int ld,
+                       cudaStream_t st) {
+    return nk<0, AT_RESID, false, 128>(A, ld, J, ld, batch, (ld + 127) / 128, N, out, ld, N, ld, 1, rowscale, J, 1.f, st);
+}

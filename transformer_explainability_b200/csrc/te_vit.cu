@@ -248,7 +248,7 @@ extern "C" int te_vit_forward(const te_vit_config* cfg, const float* weights, co
         return TE_ERR_ARG;
     }
     const float* lbase = (flags & TE_FLAG_LINEAR_TENSOR_CORES) ? derived : nullptr;
-    // fp16-split forward Linears (te_tc_fwd16.cu).  The block-scaled split of every Linear input lives in buffers that are idle
+    // fp16-split forward Linears (te_tc_wgmma.cu).  The block-scaled split of every Linear input lives in buffers that are idle
     // until the backward pass: A = tD[1] (+ scales tD[0]) for the D-wide inputs, B = tF[1] (+ scales tD[2]) for the GELU output.
     // LayerNorm emits the split of what it produces; the attention output and the GELU output go through the pre-pass (emitting
     // the split from the fc1 GELU epilogue was measured: 1.01 ms against 0.56 + 0.2 ms, profiles/r02_results.md).

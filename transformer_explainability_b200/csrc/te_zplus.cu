@@ -1,4 +1,4 @@
-// z+ Linear rule driver: fp32 SIMT path (te_gemm.cu) or tcgen05 tensor-core path (te_tc_zplus.cu).
+// z+ Linear rule driver: fp32 SIMT path (te_gemm.cu) or wgmma tensor-core path (te_tc_wgmma.cu).
 #include "te_zplus.h"
 #include "te_gemm.cuh"
 #include "te_gemm_tc.h"

@@ -5,7 +5,7 @@
 
 // x [rows, in] with row stride ldx ; w [out, in] ; r [rows, out] ; out [rows, in] ; s_scratch [rows, out].
 // w_derived: the te_tc_prepare_weights() copies of w, or NULL.  When given (and the shape qualifies) both
-// contractions run on tcgen05 tensor cores (TF32 inputs, fp32 accumulate); otherwise — and as the checker —
+// contractions run on wgmma tensor cores (TF32 inputs, fp32 accumulate); otherwise — and as the checker —
 // the fp32 SIMT path.
 int te_zplus_linear_relprop(const float* x, long long ldx, const float* w, const float* w_derived, const float* r,
                             float* out, float* s_scratch, long long rows, int in_features, int out_features,
@@ -18,7 +18,7 @@ int te_zplus_linear_relprop_ldr(const float* x, long long ldx, const float* w, c
                                 const float* bias = nullptr, int bf16 = 0, long long ld_out = 0,
                                 float* xabs = nullptr);
 // bf16: bit 0 round-1 bf16 R kernel (TE_FLAG_ZPLUS_BF16), bit 1 bf16 |x||W|^T term (TE_FLAG_ZPLUS_S1_BF16), bit 2 second
-// contraction on tcgen05 kind::f16 with a block-scaled fp16 S written by the S kernel's epilogue (TE_FLAG_ZPLUS_R_F16)
+// contraction on fp16 MMAs with a block-scaled fp16 S written by the S kernel's epilogue (TE_FLAG_ZPLUS_R_F16)
 // xabs: scratch [rows, in] (the tf32(|x|) operand of the persistent single-pass S kernel); without it the tensor-core path
 // uses the round-1 kernels.
 // ld_out: row stride of out (0 = in_features).  With row strides on x, r, y and out the rule runs on a strided subset of

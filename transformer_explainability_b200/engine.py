@@ -1,6 +1,6 @@
 """Host-side engine objects: flat frozen-weight buffer, workspace, and the explain call.
 
-The engine is the B200 replacement for the stateful hook machinery of the reference
+The engine is the CUDA replacement for the stateful hook machinery of the reference
 (``modules/layers_ours.py:16-27`` forward hooks, ``retain_graph=True`` autograd graph): it owns one
 flat fp32 weight buffer (the unit of the single NCCL broadcast) and one activation workspace per
 stream, and issues O(1) launches per block per BATCH through the C ABI.
@@ -36,7 +36,7 @@ class ViTEngine:
 
     def __init__(self, cfg, state_dict=None, device=None, flags=0):
         if not torch.cuda.is_available():
-            raise RuntimeError("transformer_explainability_b200 needs a CUDA device (B200, sm_100a); "
+            raise RuntimeError("transformer_explainability_b200 needs a CUDA device (H100, sm_90a); "
                                "there is no CPU fallback")
         self.lib = _lib.load()
         self.cfg = cfg
@@ -78,7 +78,7 @@ class ViTEngine:
 
     @_on_engine_device
     def _derived(self, flags):
-        """W+/W-/W+^T/W-^T TF32 copies for the tcgen05 z+ path (built once per weight load)."""
+        """W+/W-/W+^T/W-^T TF32 copies for the tensor-core z+ path (built once per weight load)."""
         if not (flags & _lib.FLAG_TENSOR_CORES):
             return None
         if self.derived is None:
@@ -288,7 +288,7 @@ class BertEngine:
 
     def __init__(self, cfg, state_dict=None, device=None, flags=0):
         if not torch.cuda.is_available():
-            raise RuntimeError("transformer_explainability_b200 needs a CUDA device (B200, sm_100a); "
+            raise RuntimeError("transformer_explainability_b200 needs a CUDA device (H100, sm_90a); "
                                "there is no CPU fallback")
         self.lib = _lib.load()
         self.cfg = cfg

@@ -1,5 +1,5 @@
 """Drop-in for the reference's ``modules/layers_ours.py``: same names, same ``relprop(R, alpha)``
-protocol, but every rule runs as a sm_100a CUDA kernel through the C ABI (``ops``) instead of a
+protocol, but every rule runs as an sm_90a CUDA kernel through the C ABI (``ops``) instead of a
 re-forward + ``torch.autograd.grad``.
 
 Only alpha=1 is supported (the only value any caller of the reference passes).  Layers whose

@@ -62,8 +62,8 @@ def _workspace(nbytes, device):
 
 @_on_device
 def linear_forward(x, w, bias=None, tensor_cores=False, f16_split=False):
-    """y = x W^T + b.  tensor_cores: fp32-grade 3xTF32 split on tcgen05 (shapes that do not qualify fall back);
-    f16_split (with tensor_cores): the row-scaled fp16 (hi, lo) split on tcgen05 kind::f16 (TE_FLAG_LINEAR_F16_SPLIT)."""
+    """y = x W^T + b.  tensor_cores: fp32-grade 3xTF32 split on the tensor cores (shapes that do not qualify fall back);
+    f16_split (with tensor_cores): the row-scaled fp16 (hi, lo) split on fp16 tensor-core MMAs (TE_FLAG_LINEAR_F16_SPLIT)."""
     _req(x, w, bias)
     if w.dim() != 2 or x.shape[-1] != w.shape[1] or (bias is not None and bias.numel() != w.shape[0]):
         raise ValueError("linear_forward: x [...,in], w [out,in], bias [out] expected")

@@ -2,7 +2,7 @@
 
 Every explanation is independent (and must be computed independently, SURVEY.md §0-6), so the only
 exchange on the path is the start-up broadcast of the flat frozen-weight buffer from rank 0 (NCCL over
-NVLink 5 / NVSwitch on a B200 box; gloo in the CPU tests).  No collective runs on the per-sample path;
+NVLink / NVSwitch on a multi-GPU H100 node; gloo in the CPU tests).  No collective runs on the per-sample path;
 results are gathered with one small all_gather of [B/G, N] maps when the caller asks for it.
 """
 import os
