@@ -210,8 +210,8 @@ def test_tc_persistent_pair_kernels(rows, inf, outf):
 
 @pytest.mark.parametrize("rows,inf,outf", [(128, 256, 256), (394, 768, 3072), (1000, 3072, 768), (77, 768, 2304)])
 def test_tc_bf16_single_pass_denominator(rows, inf, outf):
-    """TE_FLAG_ZPLUS_S1_BF16: the |x||W|^T term of the single-pass z+ denominator with bf16 operands (persistent pair kernel,
-    kind::f16).  A sum of K non-negative products: the 2^-9 operand roundings average out; stated tolerance = the TF32 path's."""
+    """TE_FLAG_ZPLUS_S1_BF16: the |x||W|^T term of the single-pass z+ denominator with bf16 operands (bf16 wgmma
+    S kernel).  A sum of K non-negative products: the 2^-9 operand roundings average out; stated tolerance = the TF32 path's."""
     from transformer_explainability_b200 import ops
     g = torch.Generator().manual_seed(rows + 5)
     x = torch.randn(rows, inf, generator=g)

@@ -5,6 +5,7 @@
 #include <string>
 
 #include "../../include/te_b200.h"
+#include "te_engine_util.h"
 #include "te_kernels.h"
 #include "te_rollout.h"
 #include "te_zplus.h"
@@ -42,21 +43,17 @@ extern "C" int te_linear_forward(const float* x, const float* w, const float* bi
 extern "C" int te_linear_forward_ex(const float* x, const float* w, const float* bias, float* y, float* scratch, int rows,
                                     int in_features, int out_features, unsigned flags, void* stream) {
     REQ(x && w && y && rows > 0 && in_features > 0 && out_features > 0, "te_linear_forward_ex: bad argument");
-    if ((flags & TE_FLAG_LINEAR_TENSOR_CORES) && (flags & TE_FLAG_LINEAR_F16_SPLIT) && scratch &&
-        te_tc_fwd16_supported(rows, in_features, out_features, in_features)) {
-        // scratch layout with both flags: [16*in*out derived | round_up(rows*in,64) fp16 hi,lo split of x | rows*ceil(in/128) block scales]
-        TE_TRY(te_tc_prepare_weights(w, scratch, in_features, out_features, ST(stream)));
-        float* split = scratch + te_tc_derived_floats(in_features, out_features);
-        float* scale = split + (((long long)rows * in_features + 63) & ~63LL);
-        return te_tc_linear_fwd16(x, in_features, split, scale, scratch, in_features, out_features, bias, y, nullptr, nullptr,
-                                  rows, TE_TC_EPI_BIAS, ST(stream));
-    }
-    if ((flags & TE_FLAG_LINEAR_TENSOR_CORES) && scratch && te_tc_gemm3x_supported(rows, in_features, out_features, in_features)) {
-        TE_TRY(te_tc_prepare_weights(w, scratch, in_features, out_features, ST(stream)));
-        return te_tc_linear_fwd(x, in_features, scratch, in_features, out_features, bias, y, nullptr, nullptr, rows,
-                                TE_TC_EPI_BIAS, ST(stream));
-    }
-    return te_linear_forward(x, w, bias, y, rows, in_features, out_features, stream);
+    // every tensor-core path takes the shapes of the 3xTF32 kernel; the derived copies are made only when one is taken
+    const bool tc = (flags & TE_FLAG_LINEAR_TENSOR_CORES) && scratch &&
+                    te_tc_gemm3x_supported(rows, in_features, out_features, in_features);
+    if (tc) TE_TRY(te_tc_prepare_weights(w, scratch, in_features, out_features, ST(stream)));
+    // scratch layout with TE_FLAG_LINEAR_F16_SPLIT as well:
+    // [16*in*out derived | round_up(rows*in,64) fp16 hi,lo split of x | rows*ceil(in/128) block scales]
+    float* split = (tc && (flags & TE_FLAG_LINEAR_F16_SPLIT)) ? scratch + te_tc_derived_floats(in_features, out_features) : nullptr;
+    const te_util::F16Split fs = {split, split ? split + (((long long)rows * in_features + 63) & ~63LL) : nullptr, false, nullptr,
+                                  nullptr};
+    return te_util::linear_fwd_tc(tc ? scratch : nullptr, x, in_features, w, bias, y, nullptr, nullptr, rows, in_features,
+                                  out_features, TE_EPI_BIAS, ST(stream), &fs);
 }
 
 extern "C" int te_f16_block_split(const float* x, int rows, int cols, void* hi, void* lo, float* scale_inv, void* stream) {
@@ -69,24 +66,15 @@ extern "C" int te_f16_block_split(const float* x, int rows, int cols, void* hi, 
 extern "C" int te_linear_backward_ex(const float* dy, const float* w, float* dx, float* scratch, int rows, int in_features,
                                      int out_features, unsigned flags, void* stream) {
     REQ(dy && w && dx && rows > 0 && in_features > 0 && out_features > 0, "te_linear_backward_ex: bad argument");
-    if ((flags & TE_FLAG_LINEAR_TENSOR_CORES) && scratch && te_tc_gemm3x_supported(rows, out_features, in_features, out_features)) {
-        TE_TRY(te_tc_prepare_weights(w, scratch, in_features, out_features, ST(stream)));
-        if ((flags & TE_FLAG_BACKWARD_F16) && te_tc_f16_single_supported(rows, out_features, in_features, out_features)) {
-            // scratch layout with the flag: [16*in*out derived | round_up(rows*out/2,64) fp16 dy | rows*ceil(out/128) block scales]
-            float* split = scratch + te_tc_derived_floats(in_features, out_features);
-            float* scale = split + (((long long)rows * out_features / 2 + 63) & ~63LL);
-            return te_tc_linear_bwd16(dy, out_features, split, scale, scratch, in_features, out_features, dx, nullptr, rows,
-                                      TE_TC_EPI_STORE, ST(stream));
-        }
-        if ((flags & TE_FLAG_BACKWARD_TF32) && te_tc_pair_supported(rows, out_features, in_features, out_features))
-            return te_tc_pair_linear_bwd(dy, out_features, scratch, in_features, out_features, dx, nullptr, rows, TE_TC_EPI_STORE,
-                                         ST(stream));
-        return te_tc_linear_bwd(dy, scratch, in_features, out_features, dx, nullptr, rows, TE_TC_EPI_STORE, ST(stream));
-    }
-    TeGemm p = g0(1);
-    p.A = dy; p.lda = out_features; p.B = w; p.ldb = in_features; p.C = dx; p.ldc = in_features;
-    p.M = rows; p.N = in_features; p.K = out_features;
-    return te_gemm_launch(p, TE_L_K, TE_L_MN, TE_XF_NONE, TE_EPI_STORE, ST(stream));
+    const bool tc = (flags & TE_FLAG_LINEAR_TENSOR_CORES) && scratch &&
+                    te_tc_gemm3x_supported(rows, out_features, in_features, out_features);
+    if (tc) TE_TRY(te_tc_prepare_weights(w, scratch, in_features, out_features, ST(stream)));
+    // scratch layout with TE_FLAG_BACKWARD_F16: [16*in*out derived | round_up(rows*out/2,64) fp16 dy | rows*ceil(out/128) block scales]
+    float* split = (tc && (flags & TE_FLAG_BACKWARD_F16)) ? scratch + te_tc_derived_floats(in_features, out_features) : nullptr;
+    const te_util::F16Split fs = {split, split ? split + (((long long)rows * out_features / 2 + 63) & ~63LL) : nullptr, false,
+                                  nullptr, nullptr};
+    return te_util::linear_bwd_tc(tc ? scratch : nullptr, dy, w, dx, nullptr, rows, in_features, out_features, TE_EPI_STORE,
+                                  ST(stream), (flags & TE_FLAG_BACKWARD_TF32) != 0, &fs);
 }
 
 extern "C" int te_linear_relprop(const float* x, const float* w, const float* r, float* out, float* scratch, int rows,
@@ -120,10 +108,7 @@ extern "C" int te_linear_relprop_ex(const float* x, const float* w, const float*
         xabs = d + te_tc_derived_floats(in_features, out_features);
     }
     return te_zplus_linear_relprop_ldr(x, in_features, w, derived, r, out_features, out, scratch, rows, in_features,
-                                       out_features, ST(stream), y, out_features, bias,
-                                       ((flags & TE_FLAG_ZPLUS_BF16) ? 1 : 0) | ((flags & TE_FLAG_ZPLUS_S1_BF16) ? 2 : 0) |
-                                           ((flags & TE_FLAG_ZPLUS_R_F16) ? 4 : 0),
-                                       0, xabs);
+                                       out_features, ST(stream), y, out_features, bias, te_zplus_from_flags(flags), 0, xabs);
 }
 
 extern "C" int te_add_relprop(const float* x1, const float* x2, const float* r, float* r1, float* r2, void* scratch,

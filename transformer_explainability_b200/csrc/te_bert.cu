@@ -9,8 +9,6 @@
 // q/k/v Linears are packed into one [3D, D] weight so that the forward is one GEMM and the per-head slices are
 // addressed in place exactly like the ViT engine; their three z+ rules stay separate (Clone(3) needs them apart).
 #include <string.h>
-#include <string>
-#include <vector>
 
 #include "../../include/te_b200.h"
 #include "te_engine_util.h"
@@ -47,10 +45,8 @@ static bool make_dims(const te_bert_config* c, int B, int S, Dims& d) {
 }
 
 // ---- flat weight buffer (HF state_dict keys) -------------------------------------------------------
-struct WEntry { std::string name; long long numel; long long offset; };
-
-static std::vector<WEntry> weight_table(const te_bert_config* c) {
-    std::vector<WEntry> t;
+static WTable weight_table(const te_bert_config* c) {
+    WTable t;
     Dims d;
     if (!make_dims(c, 1, 1, d)) return t;
     long long off = 0;
@@ -101,7 +97,7 @@ struct Weights {
 };
 
 static void bind_weights(const te_bert_config* c, const float* base, Weights& w) {
-    const std::vector<WEntry> t = weight_table(c);
+    const WTable t = weight_table(c);
     size_t i = 0;
     auto next = [&]() { return base + t[i++].offset; };
     w.word = next(); w.pos = next(); w.type = next(); w.elnw = next(); w.elnb = next();
@@ -148,12 +144,7 @@ struct Workspace {
 };
 
 static void carve(const Dims& d, char* base, Workspace& ws) {
-    long long off = 0;
-    auto take = [&](long long nfloat) -> float* {
-        float* p = base ? reinterpret_cast<float*>(base + off) : nullptr;
-        off += ((nfloat * 4 + 255) / 256) * 256;
-        return p;
-    };
+    Bump take{base};
     const long long MD = d.M * d.D, MF = d.M * d.F, M3D = d.M * 3LL * d.D;
     const long long AT = (long long)d.B * d.H * d.N * d.NP;
     for (int l = 0; l < d.L; ++l) {
@@ -176,47 +167,23 @@ static void carve(const Dims& d, char* base, Workspace& ws) {
     ws.joint[0] = take((long long)d.B * d.N * d.NP);
     ws.joint[1] = take((long long)d.B * d.N * d.NP);
     ws.addpart = reinterpret_cast<double*>(take((long long)d.B * TE_ADD_SPLIT * 3 * 2));
-    ws.bytes = off;
+    ws.bytes = take.off;
 }
 
 static int check_ws(const te_bert_config* cfg, int batch, int seq, void* workspace, long long bytes, Dims& d,
                     Workspace& ws) {
-    if (batch <= 0 || !workspace) { te_set_last_error("te_bert: batch <= 0 or null workspace"); return TE_ERR_ARG; }
-    if (!make_dims(cfg, batch, seq, d)) return TE_ERR_ARG;
-    if (((uintptr_t)workspace & 255u) != 0) { te_set_last_error("te_bert: workspace must be 256-byte aligned"); return TE_ERR_ARG; }
-    carve(d, reinterpret_cast<char*>(workspace), ws);
-    if (ws.bytes > bytes) { te_set_last_error("te_bert: workspace too small"); return TE_ERR_WORKSPACE; }
-    return TE_OK;
+    return te_util::check_ws("te_bert", batch, workspace, bytes, [&] { return make_dims(cfg, batch, seq, d); },
+                             [&] { carve(d, reinterpret_cast<char*>(workspace), ws); return ws.bytes; });
 }
 
 }  // namespace
 
 // =====================================================================================================
-extern "C" int te_bert_num_weights(const te_bert_config* cfg) {
-    const auto t = weight_table(cfg);
-    return t.empty() ? TE_ERR_ARG : (int)t.size() - 1;
-}
-extern "C" const char* te_bert_weight_name(const te_bert_config* cfg, int i) {
-    static thread_local std::string s;
-    const auto t = weight_table(cfg);
-    if (i < 0 || i + 1 >= (int)t.size()) return nullptr;
-    s = t[i].name;
-    return s.c_str();
-}
-extern "C" long long te_bert_weight_numel(const te_bert_config* cfg, int i) {
-    const auto t = weight_table(cfg);
-    if (i < 0 || i + 1 >= (int)t.size()) return TE_ERR_ARG;
-    return t[i].numel;
-}
-extern "C" long long te_bert_weight_offset(const te_bert_config* cfg, int i) {
-    const auto t = weight_table(cfg);
-    if (i < 0 || i + 1 >= (int)t.size()) return TE_ERR_ARG;
-    return t[i].offset;
-}
-extern "C" long long te_bert_weight_total(const te_bert_config* cfg) {
-    const auto t = weight_table(cfg);
-    return t.empty() ? TE_ERR_ARG : t.back().offset;
-}
+extern "C" int te_bert_num_weights(const te_bert_config* cfg) { return wt_count(weight_table(cfg)); }
+extern "C" const char* te_bert_weight_name(const te_bert_config* cfg, int i) { return wt_name(weight_table(cfg), i); }
+extern "C" long long te_bert_weight_numel(const te_bert_config* cfg, int i) { return wt_numel(weight_table(cfg), i); }
+extern "C" long long te_bert_weight_offset(const te_bert_config* cfg, int i) { return wt_offset(weight_table(cfg), i); }
+extern "C" long long te_bert_weight_total(const te_bert_config* cfg) { return wt_total(weight_table(cfg)); }
 extern "C" long long te_bert_workspace_bytes(const te_bert_config* cfg, int batch, int seq) {
     Dims d;
     if (batch <= 0 || !make_dims(cfg, batch, seq, d)) return TE_ERR_ARG;
@@ -259,26 +226,16 @@ extern "C" int te_bert_forward(const te_bert_config* cfg, const float* weights, 
     Dims d; Workspace ws;
     TE_TRY(check_ws(cfg, batch, seq, workspace, workspace_bytes, d, ws));
     if (!weights || !input_ids || !attention_mask) { te_set_last_error("te_bert_forward: null pointer"); return TE_ERR_ARG; }
-    if ((flags & TE_FLAG_LINEAR_TENSOR_CORES) && !derived) {
-        te_set_last_error("te_bert_forward: TE_FLAG_LINEAR_TENSOR_CORES needs the derived weight buffer");
-        return TE_ERR_ARG;
-    }
-    const float* lbase = (flags & TE_FLAG_LINEAR_TENSOR_CORES) ? derived : nullptr;
+    Select sel;
+    TE_TRY(decode_flags(sel, "te_bert_forward", flags, derived, 0, false));
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    // fp16-split forward Linears (te_tc_wgmma.cu): split of the D-wide inputs in A = tD[1] (+ scales tD[2]), of the GELU output in
-    // B = tF[1] (+ scales tD[3]); all idle until the backward pass.  Every LayerNorm emits the split of its output (the hidden
-    // state feeds the next layer's qkv); the attention context and the GELU output go through the pre-pass.
-    const bool f16 = lbase && (flags & TE_FLAG_LINEAR_F16_SPLIT) && d.F >= d.D && te_tc_fwd16_supported(d.M, d.D, 3 * d.D, d.D) &&
-                     te_tc_fwd16_supported(d.M, d.D, d.D, d.D) && te_tc_fwd16_supported(d.M, d.D, d.F, d.D) &&
-                     te_tc_fwd16_supported(d.M, d.F, d.D, d.F);
-    const te_util::F16Split fsA_ready = {ws.tD[1], ws.tD[2], true};
-    const te_util::F16Split fsA_pre = {ws.tD[1], ws.tD[2], false};
-    const bool gsf = te_engine_gelu_split();
-    const te_util::F16Split fsA_w1 = {ws.tD[1], ws.tD[2], true, gsf ? ws.tF[1] : nullptr, gsf ? ws.tD[3] : nullptr};
-    const te_util::F16Split fsB = {ws.tF[1], ws.tD[3], gsf};
+    // fp16-split forward Linears: split of the D-wide inputs in tD[1] (+ scales tD[2]), of the GELU output in tF[1] (+ scales
+    // tD[3]); all idle until the backward pass.  Every LayerNorm emits the split of its output (the hidden state feeds the next
+    // layer's qkv).
+    const F16Forward f16 = f16_forward(sel, d.M, d.D, d.F, ws.tD[1], ws.tD[2], ws.tF[1], ws.tD[3]);
     auto layernorm = [&](const float* x, const float* g, const float* b, float* y, float* mean, float* rstd) {
-        return f16 ? te_launch_layernorm_split(x, g, b, y, mean, rstd, d.M, d.D, d.eps, ws.tD[1], ws.tD[2], st)
-                   : te_launch_layernorm(x, g, b, y, mean, rstd, d.M, d.D, d.eps, st);
+        return f16.on ? te_launch_layernorm_split(x, g, b, y, mean, rstd, d.M, d.D, d.eps, f16.qkv.split, f16.qkv.scale, st)
+                      : te_launch_layernorm(x, g, b, y, mean, rstd, d.M, d.D, d.eps, st);
     };
     Weights w;
     bind_weights(cfg, weights, w);
@@ -292,27 +249,22 @@ extern "C" int te_bert_forward(const te_bert_config* cfg, const float* weights, 
         LayerAct& a = ws.layer[l];
         const LayerW& lw = w.layer[l];
         float* h_next = (l + 1 < d.L) ? ws.layer[l + 1].h : ws.h_last;
-        const DerivedW tw = bind_derived(d, lbase, l);
+        const DerivedW tw = bind_derived(d, sel.lbase, l);
         TE_TRY(linear_fwd_tc(tw.qkv, a.h, d.D, lw.qkvw, lw.qkvb, a.qkv, nullptr, nullptr, d.M, d.D, 3 * d.D, TE_EPI_BIAS, st,
-                             f16 ? &fsA_ready : nullptr));
-        const HeadOp q = head_rows(a.qkv, 3 * d.D, d.N, d.dh);
-        const HeadOp k = head_rows(a.qkv + d.D, 3 * d.D, d.N, d.dh);
-        const HeadOp v = head_rows(a.qkv + 2 * d.D, 3 * d.D, d.N, d.dh);
+                             &f16.qkv));
         // scores = q k^T / sqrt(d) ; + extended mask ; softmax      (:338-345)
-        TE_TRY(attn_nn((flags & TE_FLAG_ATTN_TENSOR_CORES) != 0, d.B, d.H, d.N, d.NP, d.dh, a.qkv, 3 * d.D, a.qkv + d.D,
-                       3 * d.D, a.P, nullptr, scale, TE_EPI_STORE, st));
+        TE_TRY(attn_nn(sel.atc, d.B, d.H, d.N, d.NP, d.dh, a.qkv, 3 * d.D, a.qkv + d.D, 3 * d.D, a.P, nullptr, scale,
+                       TE_EPI_STORE, st));
         TE_TRY(te_launch_softmax_masked(a.P, (long long)d.B * d.H * d.N, d.N, d.NP, ws.maskadd, (long long)d.H * d.N, st));
-        TE_TRY(attn_nk((flags & TE_FLAG_ATTN_TENSOR_CORES) != 0, d.B, d.H, d.N, d.NP, d.dh, a.P, 0, a.qkv + 2 * d.D, 3 * d.D,
-                       a.ctx, d.D, nullptr, 1.f, TE_EPI_STORE, st));
+        TE_TRY(attn_nk(sel.atc, d.B, d.H, d.N, d.NP, d.dh, a.P, 0, a.qkv + 2 * d.D, 3 * d.D, a.ctx, d.D, nullptr, 1.f,
+                       TE_EPI_STORE, st));
         // BertSelfOutput: dense -> add([dense, input]) -> LayerNorm
-        TE_TRY(linear_fwd_tc(tw.o, a.ctx, d.D, lw.ow, lw.ob, a.d1, a.s1, a.h, d.M, d.D, d.D, TE_EPI_BIAS_ADD, st,
-                             f16 ? &fsA_pre : nullptr));
+        TE_TRY(linear_fwd_tc(tw.o, a.ctx, d.D, lw.ow, lw.ob, a.d1, a.s1, a.h, d.M, d.D, d.D, TE_EPI_BIAS_ADD, st, &f16.proj));
         TE_TRY(layernorm(a.s1, lw.ln1w, lw.ln1b, a.ao, a.mean1, a.rstd1));
         // BertIntermediate (dense + GELU), BertOutput (dense -> add -> LayerNorm)
         TE_TRY(linear_fwd_tc(tw.w1, a.ao, d.D, lw.w1, lw.b1, a.hpre, a.g, nullptr, d.M, d.D, d.F, TE_EPI_BIAS_GELU, st,
-                             f16 ? &fsA_w1 : nullptr));
-        TE_TRY(linear_fwd_tc(tw.w2, a.g, d.F, lw.w2, lw.b2, a.d2, a.s2, a.ao, d.M, d.F, d.D, TE_EPI_BIAS_ADD, st,
-                             f16 ? &fsB : nullptr));
+                             &f16.fc1));
+        TE_TRY(linear_fwd_tc(tw.w2, a.g, d.F, lw.w2, lw.b2, a.d2, a.s2, a.ao, d.M, d.F, d.D, TE_EPI_BIAS_ADD, st, &f16.fc2));
         TE_TRY(layernorm(a.s2, lw.ln2w, lw.ln2b, h_next, a.mean2, a.rstd2));
     }
     // pooler (first token -> dense -> tanh), classifier
@@ -336,26 +288,14 @@ extern "C" int te_bert_attribute(const te_bert_config* cfg, const float* weights
     TE_TRY(check_ws(cfg, batch, seq, workspace, workspace_bytes, d, ws));
     if (!weights || !index || (!maps && !(flags & TE_FLAG_GRADIENTS_ONLY))) { te_set_last_error("te_bert_attribute: null pointer"); return TE_ERR_ARG; }
     if (start_layer < 0 || start_layer >= d.L) { te_set_last_error("te_bert_attribute: start_layer out of range"); return TE_ERR_ARG; }
-    if ((flags & (TE_FLAG_ZPLUS_TENSOR_CORES | TE_FLAG_LINEAR_TENSOR_CORES)) && !derived) {
-        te_set_last_error("te_bert_attribute: tensor-core flags need the derived weight buffer");
-        return TE_ERR_ARG;
-    }
-    const float* lbase = (flags & TE_FLAG_LINEAR_TENSOR_CORES) ? derived : nullptr;
-    const bool atc = (flags & TE_FLAG_ATTN_TENSOR_CORES) != 0;
-    const bool btf = (flags & TE_FLAG_BACKWARD_TF32) != 0;       // single-pass TF32 backward Linears
-    // single-pass fp16 backward Linears: hi-only split of the incoming gradient in tF[1], block scales in t3D[1] (idle until the relprop)
-    const te_util::F16Split bfs_v = {ws.tF[1], ws.t3D[1], false};
-    const te_util::F16Split* bfs = (lbase && (flags & TE_FLAG_BACKWARD_F16)) ? &bfs_v : nullptr;
-    const bool rtf = (flags & TE_FLAG_RELPROP_TF32) != 0;        // single-pass TF32 relevance-side attention contractions
-    const int zb = ((flags & TE_FLAG_ZPLUS_BF16) ? 1 : 0) | ((flags & TE_FLAG_ZPLUS_S1_BF16) ? 2 : 0) |
-                   ((flags & TE_FLAG_ZPLUS_R_F16) ? 4 : 0);                                               // bf16 / fp16 variants of the z+ rule
+    // fp16 backward split of dy in tF[1], block scales in t3D[1] (idle until the relprop)
+    Select sel;
+    TE_TRY(decode_flags(sel, "te_bert_attribute", flags, derived, start_layer, true, ws.tF[1], ws.t3D[1]));
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     Weights w;
     bind_weights(cfg, weights, w);
-    const float* dbase = (flags & TE_FLAG_ZPLUS_TENSOR_CORES) ? derived : nullptr;
     const float scale = 1.0f / sqrtf((float)d.dh);
     const long long MD = d.M * d.D, DD = (long long)d.D * d.D;
-    const int low = (flags & (TE_FLAG_KEEP_ALL_CAMS | TE_FLAG_RELPROP_TO_INPUT)) ? 0 : start_layer;
 
     TE_TRY(te_launch_argmax(ws.logits, index, d.B, d.C, 1, st));
     TE_TRY(te_launch_onehot(index, ws.seed, d.B, d.C, 1.0f, st));
@@ -375,25 +315,17 @@ extern "C" int te_bert_attribute(const te_bert_config* cfg, const float* weights
     for (int l = d.L - 1; l >= start_layer; --l) {
         LayerAct& a = ws.layer[l];
         const LayerW& lw = w.layer[l];
-        const HeadOp q = head_rows(a.qkv, 3 * d.D, d.N, d.dh);
-        const HeadOp k = head_rows(a.qkv + d.D, 3 * d.D, d.N, d.dh);
-        const HeadOp v = head_rows(a.qkv + 2 * d.D, 3 * d.D, d.N, d.dh);
         TE_TRY(te_launch_layernorm_bwd(dxa, a.s2, lw.ln2w, a.mean2, a.rstd2, nullptr, dsx, d.M, d.D, st));    // d s2
-        const DerivedW tw = bind_derived(d, lbase, l);
-        TE_TRY(linear_bwd_tc(tw.w2, dsx, lw.w2, dF, a.hpre, d.M, d.F, d.D, TE_EPI_GELU_BWD, st, btf, bfs));
-        TE_TRY(linear_bwd_tc(tw.w1, dF, lw.w1, dxn, nullptr, d.M, d.D, d.F, TE_EPI_STORE, st, btf, bfs));
+        const DerivedW tw = bind_derived(d, sel.lbase, l);
+        TE_TRY(linear_bwd_tc(tw.w2, dsx, lw.w2, dF, a.hpre, d.M, d.F, d.D, TE_EPI_GELU_BWD, st, sel.btf, &sel.bfs));
+        TE_TRY(linear_bwd_tc(tw.w1, dF, lw.w1, dxn, nullptr, d.M, d.D, d.F, TE_EPI_STORE, st, sel.btf, &sel.bfs));
         TE_TRY(te_launch_add2(dxn, dsx, dxn, MD, st));                                                          // d ao
         TE_TRY(te_launch_layernorm_bwd(dxn, a.s1, lw.ln1w, a.mean1, a.rstd1, nullptr, dsx, d.M, d.D, st));    // d s1
-        TE_TRY(linear_bwd_tc(tw.o, dsx, lw.ow, dctx, nullptr, d.M, d.D, d.D, TE_EPI_STORE, st, btf, bfs));
-        TE_TRY(attn_nn(atc, d.B, d.H, d.N, d.NP, d.dh, dctx, d.D, a.qkv + 2 * d.D, 3 * d.D, a.G, nullptr, 1.f,
-                       TE_EPI_STORE, st, btf));                                                                      // G = dctx v^T
-        if (l == start_layer) break;
-        TE_TRY(attn_nk(atc, d.B, d.H, d.N, d.NP, d.dh, a.P, 1, dctx, d.D, dqkv + 2 * d.D, 3 * d.D, nullptr, 1.f,
-                       TE_EPI_STORE, st, btf));                                                                 // dV = P^T dctx
-        TE_TRY(te_launch_softmax_bwd(a.P, a.G, dS, (long long)d.B * d.H * d.N, d.N, d.NP, scale, st));
-        TE_TRY(attn_nk(atc, d.B, d.H, d.N, d.NP, d.dh, dS, 0, a.qkv + d.D, 3 * d.D, dqkv, 3 * d.D, nullptr, 1.f, TE_EPI_STORE, st, btf));   // dQ
-        TE_TRY(attn_nk(atc, d.B, d.H, d.N, d.NP, d.dh, dS, 1, a.qkv, 3 * d.D, dqkv + d.D, 3 * d.D, nullptr, 1.f, TE_EPI_STORE, st, btf));   // dK
-        TE_TRY(linear_bwd_tc(tw.qkv, dqkv, lw.qkvw, dxn, nullptr, d.M, d.D, 3 * d.D, TE_EPI_STORE, st, btf, bfs));
+        TE_TRY(linear_bwd_tc(tw.o, dsx, lw.ow, dctx, nullptr, d.M, d.D, d.D, TE_EPI_STORE, st, sel.btf, &sel.bfs));
+        const bool last = (l == start_layer);
+        TE_TRY(attn_block_bwd(sel, d.B, d.H, d.N, d.NP, d.dh, a.qkv, a.P, dctx, a.G, dS, dqkv, scale, last, st));
+        if (last) break;
+        TE_TRY(linear_bwd_tc(tw.qkv, dqkv, lw.qkvw, dxn, nullptr, d.M, d.D, 3 * d.D, TE_EPI_STORE, st, sel.btf, &sel.bfs));
         TE_TRY(te_launch_add2(dxn, dsx, dxa, MD, st));                                                          // d h
     }
 
@@ -408,13 +340,10 @@ extern "C" int te_bert_attribute(const te_bert_config* cfg, const float* weights
                                    d.D, d.D, st));
     TE_TRY(te_launch_index_select_relprop(ws.h_last, ws.rfirst, nullptr, R, d.B, d.N, d.D, st));
 
-    for (int l = d.L - 1; l >= low; --l) {
+    for (int l = d.L - 1; l >= sel.low; --l) {
         LayerAct& a = ws.layer[l];
         const LayerW& lw = w.layer[l];
-        const DerivedW dw = bind_derived(d, dbase, l);
-        const HeadOp q = head_rows(a.qkv, 3 * d.D, d.N, d.dh);
-        const HeadOp k = head_rows(a.qkv + d.D, 3 * d.D, d.N, d.dh);
-        const HeadOp v = head_rows(a.qkv + 2 * d.D, 3 * d.D, d.N, d.dh);
+        const DerivedW dw = bind_derived(d, sel.dbase, l);
         // BertOutput.relprop :474-487 ; BertIntermediate.relprop :451-456 ; BertLayer.clone
         // top layer: relevance is non-zero only in the first token's row (pooler, BERT.py:181-190) and every rule down
         // to the attention-output dense rule is row-wise -> its three z+ rules run on the B first-token rows only (exact)
@@ -422,36 +351,29 @@ extern "C" int te_bert_attribute(const te_bert_config* cfg, const float* weights
         const long long zr = top ? d.B : d.M;
         const long long sD = top ? (long long)d.N * d.D : d.D, sF = top ? (long long)d.N * d.F : d.F;
         TE_TRY(te_launch_add_relprop(a.d2, a.ao, R, R1, R2, ws.addpart, d.B, (long long)d.N * d.D, st));
-        TE_TRY(te_zplus_linear_relprop_ldr(a.g, sF, lw.w2, dw.w2, R1, sD, RF, S, zr, d.F, d.D, st, a.d2, sD, lw.b2, zb, sF, SF));
-        TE_TRY(te_zplus_linear_relprop_ldr(a.ao, sD, lw.w1, dw.w1, RF, sF, R1, SF, zr, d.D, d.F, st, a.hpre, sF, lw.b1, zb, sD, S));
+        TE_TRY(te_zplus_linear_relprop_ldr(a.g, sF, lw.w2, dw.w2, R1, sD, RF, S, zr, d.F, d.D, st, a.d2, sD, lw.b2, sel.zv, sF, SF));
+        TE_TRY(te_zplus_linear_relprop_ldr(a.ao, sD, lw.w1, dw.w1, RF, sF, R1, SF, zr, d.D, d.F, st, a.hpre, sF, lw.b1, sel.zv, sD, S));
         TE_TRY(te_launch_clone_relprop(a.ao, R1, R2, nullptr, R, MD, st));
         // BertSelfOutput.relprop :427-434
         TE_TRY(te_launch_add_relprop(a.d1, a.h, R, R1, R2, ws.addpart, d.B, (long long)d.N * d.D, st));
         if (top) TE_TRY(te_launch_fill(R3, 0.f, MD, st));
-        TE_TRY(te_zplus_linear_relprop_ldr(a.ctx, sD, lw.ow, dw.o, R1, sD, R3, S, zr, d.D, d.D, st, a.d1, sD, lw.ob, zb, sD, S + MD));
-        // BertSelfAttention.relprop :367-409
-        TE_TRY(te_launch_sd(R3, a.ctx, S, MD, st));                                       // matmul2: Z == saved ctx
-        TE_TRY(attn_nn(atc, d.B, d.H, d.N, d.NP, d.dh, S, d.D, a.qkv + 2 * d.D, 3 * d.D, a.cam, a.P, 0.5f, TE_EPI_MUL,
-                       st, rtf));                                                              // attn_cam   :380
-        if (l == low && !(flags & TE_FLAG_RELPROP_TO_INPUT)) break;
-        TE_TRY(attn_nk(atc, d.B, d.H, d.N, d.NP, d.dh, a.P, 1, S, d.D, Rqkv + 2 * d.D, 3 * d.D, a.qkv + 2 * d.D, 0.5f, TE_EPI_MUL,
-                       st, rtf));
+        TE_TRY(te_zplus_linear_relprop_ldr(a.ctx, sD, lw.ow, dw.o, R1, sD, R3, S, zr, d.D, d.D, st, a.d1, sD, lw.ob, sel.zv, sD, S + MD));
+        // BertSelfAttention.relprop :367-409: matmul2 rule -> attn_cam (:380), cam_v
+        const bool last = (l == sel.low && !(flags & TE_FLAG_RELPROP_TO_INPUT));
+        TE_TRY(attn_relprop_pv(sel, d.B, d.H, d.N, d.NP, d.dh, a.qkv, a.P, R3, a.ctx, S, a.cam, Rqkv, last, st));
+        if (last) break;
         // add([scores, mask]).relprop : scores = q k^T / sqrt(d) recomputed ; relevance renormalised  :386-388
-        TE_TRY(attn_nn(atc, d.B, d.H, d.N, d.NP, d.dh, a.qkv, 3 * d.D, a.qkv + d.D, 3 * d.D, ws.tA[0], nullptr, scale,
+        TE_TRY(attn_nn(sel.atc, d.B, d.H, d.N, d.NP, d.dh, a.qkv, 3 * d.D, a.qkv + d.D, 3 * d.D, ws.tA[0], nullptr, scale,
                        TE_EPI_STORE, st));
         TE_TRY(te_launch_add_relprop_keymask(ws.tA[0], ws.maskadd, a.cam, ws.tA[1], ws.addpart, d.B, d.H, d.N, d.NP, st));
-        // matmul1 rule on the unscaled product
-        TE_TRY(attn_nn(atc, d.B, d.H, d.N, d.NP, d.dh, a.qkv, 3 * d.D, a.qkv + d.D, 3 * d.D, ws.tA[0], ws.tA[1], 1.f,
-                       TE_EPI_SD, st));
-        TE_TRY(attn_nk(atc, d.B, d.H, d.N, d.NP, d.dh, ws.tA[0], 0, a.qkv + d.D, 3 * d.D, Rqkv, 3 * d.D, a.qkv, 0.5f, TE_EPI_MUL, st, rtf));
-        TE_TRY(attn_nk(atc, d.B, d.H, d.N, d.NP, d.dh, ws.tA[0], 1, a.qkv, 3 * d.D, Rqkv + d.D, 3 * d.D, a.qkv + d.D, 0.5f,
-                       TE_EPI_MUL, st, rtf));
+        // matmul1 rule on the unscaled product -> cam_q, cam_k
+        TE_TRY(attn_relprop_qk(sel, d.B, d.H, d.N, d.NP, d.dh, a.qkv, ws.tA[1], ws.tA[0], Rqkv, st));
         // query / key / value z+ rules (separate Linears), Clone(3), Clone(2)
-        TE_TRY(te_zplus_linear_relprop_ldr(a.h, d.D, lw.qkvw, dw.q, Rqkv, 3 * d.D, R, S, d.M, d.D, d.D, st, a.qkv, 3 * d.D, lw.qkvb, zb, 0, S + MD));
+        TE_TRY(te_zplus_linear_relprop_ldr(a.h, d.D, lw.qkvw, dw.q, Rqkv, 3 * d.D, R, S, d.M, d.D, d.D, st, a.qkv, 3 * d.D, lw.qkvb, sel.zv, 0, S + MD));
         TE_TRY(te_zplus_linear_relprop_ldr(a.h, d.D, lw.qkvw + DD, dw.k, Rqkv + d.D, 3 * d.D, R1, S, d.M, d.D, d.D, st, a.qkv + d.D, 3 * d.D,
-                                           lw.qkvb + d.D, zb, 0, S + MD));
+                                           lw.qkvb + d.D, sel.zv, 0, S + MD));
         TE_TRY(te_zplus_linear_relprop_ldr(a.h, d.D, lw.qkvw + 2 * DD, dw.v, Rqkv + 2 * d.D, 3 * d.D, R3, S, d.M, d.D, d.D, st,
-                                           a.qkv + 2 * d.D, 3 * d.D, lw.qkvb + 2 * d.D, zb, 0, S + MD));
+                                           a.qkv + 2 * d.D, 3 * d.D, lw.qkvb + 2 * d.D, sel.zv, 0, S + MD));
         TE_TRY(te_launch_clone_relprop(a.h, R, R1, R3, SF, MD, st));                      // self.clone (3-way)
         TE_TRY(te_launch_clone_relprop(a.h, SF, R2, nullptr, R, MD, st));                 // attention.clone
     }
@@ -480,12 +402,7 @@ extern "C" int te_bert_tensor(const te_bert_config* cfg, int batch, int seq, voi
     if (batch <= 0 || !make_dims(cfg, batch, seq, d)) return TE_ERR_ARG;
     carve(d, reinterpret_cast<char*>(workspace), ws);
     const std::string n(name);
-    auto set = [&](float* p, long long d0, long long d1, long long d2, long long d3, long long s0, long long s1,
-                   long long s2, long long s3) {
-        *ptr = p; dims[0] = d0; dims[1] = d1; dims[2] = d2; dims[3] = d3;
-        strides[0] = s0; strides[1] = s1; strides[2] = s2; strides[3] = s3;
-        return TE_OK;
-    };
+    const View set{ptr, dims, strides};
     if (n == "logits") return set(ws.logits, d.B, d.C, 1, 1, d.C, 1, 1, 1);
     if (n == "relevance_in") return set(ws.tD[0], d.B, d.N, d.D, 1, (long long)d.N * d.D, d.D, 1, 1);
     if (layer < 0 || layer >= d.L) { te_set_last_error("te_bert_tensor: layer out of range"); return TE_ERR_ARG; }

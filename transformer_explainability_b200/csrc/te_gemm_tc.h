@@ -1,6 +1,7 @@
 // Tensor-core (Hopper wgmma) GEMMs of the engines (te_tc_wgmma.cu): TF32 / bf16 / fp16 operands, fp32 accumulation.
 #pragma once
 #include "te_common.cuh"
+#include "te_zplus.h"
 
 // shapes the tensor-core z+ path accepts (in/out multiples of 128, 16-byte aligned rows)
 bool te_tc_zplus_supported(long long rows, int in_features, int out_features, long long ldx);
@@ -21,14 +22,11 @@ long long te_tc_derived_floats(int in_features, int out_features);
 int te_tc_prepare_weights(const float* w, float* derived, int in_features, int out_features, cudaStream_t st);
 // y / bias (optional): the Linear's saved forward output y = x W^T + bias [rows, out] (row stride ldy).  When given,
 // Z is formed in ONE pass as ((y - bias) + |x| |W|^T) / 2  ==  x+ W+^T + x- W-^T  (exact identity), halving the S kernel.
+// zv, ld_out, xabs: as in te_zplus_linear_relprop_ldr (te_zplus.h).
 int te_tc_zplus_linear_relprop(const float* x, long long ldx, const float* derived, const float* r, long long ldr,
-                               float* out,
-                               float* s_scratch, long long rows, int in_features, int out_features, cudaStream_t st,
-                               const float* y = nullptr, long long ldy = 0, const float* bias = nullptr,
-                               int bf16 = 0 /* bit 0: bf16 S and R kernel (flag 64); bit 1: bf16 single-pass S kernel (flag 2048);
-                                               bit 2: fp16 R kernel fed by the S kernel's fp16 epilogue (flag 8192) */,
-                               long long ld_out = 0 /* row stride of out; 0 = in_features */,
-                               float* xabs = nullptr /* scratch [rows, in]: operand of the bf16 single-pass S kernel */);
+                               float* out, float* s_scratch, long long rows, int in_features, int out_features, cudaStream_t st,
+                               const float* y, long long ldy, const float* bias, ZplusVariant zv, long long ld_out,
+                               float* xabs);
 
 // fp32-grade (3xTF32 split) Linear GEMMs; epilogues mirror the SIMT ones
 enum { TE_TC_EPI_STORE = 0, TE_TC_EPI_BIAS = 1, TE_TC_EPI_BIAS_GELU = 2, TE_TC_EPI_BIAS_ADD = 3, TE_TC_EPI_GELU_BWD = 4 };
@@ -51,8 +49,8 @@ int te_tc_blocksplit_f16(const float* x, long long ldx, long long rows, int cols
 int te_tc_linear_fwd16(const float* x, long long ldx, float* split, float* scale, const float* derived, int in_features,
                        int out_features, const float* bias, float* y, float* y2, const float* e0, long long rows, int epi,
                        cudaStream_t st, float* split_out = nullptr, float* scale_out = nullptr);
-// single-pass fp16 products on the same kernel (A = hi only: fp16 keeps TF32's 11 significant bits, rounded to nearest)
-bool te_tc_f16_single_supported(long long rows, int K, int N, long long lda);
+// single-pass fp16 products on the same kernel (A = hi only: fp16 keeps TF32's 11 significant bits, rounded to nearest);
+// shapes: te_tc_fwd16_supported
 // dx = epi(dy W): split (rows*out/2 floats) / scale ([rows, ceil(out/128)]) hold the hi-only split of dy (dy != NULL: pre-pass here)
 int te_tc_linear_bwd16(const float* dy, long long lddy, float* split, float* scale, const float* derived, int in_features,
                        int out_features, float* dx, const float* e0, long long rows, int epi, cudaStream_t st);
@@ -79,15 +77,14 @@ bool te_tc_bmm_nk_supported(int N, int ld);
 int te_tc_bmm_nk_resid(const float* A, const float* J, const float* rowscale, float* out, int batch, int N, int ld,
                        cudaStream_t st);
 
-// z+ rule contractions and the single-pass TF32 backward Linear
-bool te_tc_pair_supported(long long rows, int K, int N, long long lda);
+// z+ rule contractions and the single-pass TF32 backward Linear (shapes: te_tc_gemm3x_supported)
 // xabs: scratch [rows, in] for bf16(|x|), the A operand of the bf16 single-pass S kernel
-int te_tc_pair_zplus_s1(const float* x, long long ldx, float* xabs, const float* derived, const float* r, long long ldr,
-                        const float* y, long long ldy, const float* bias, float* s_out, long long rows, int in_features,
-                        int out_features, cudaStream_t st, bool bf16 = false, float* s16 = nullptr, float* s16_scale = nullptr);
+int te_tc_zplus_s1(const float* x, long long ldx, float* xabs, const float* derived, const float* r, long long ldr,
+                   const float* y, long long ldy, const float* bias, float* s_out, long long rows, int in_features,
+                   int out_features, cudaStream_t st, bool bf16 = false, float* s16 = nullptr, float* s16_scale = nullptr);
 // s16 / s16_scale: when given, S leaves as hi-only block-scaled fp16 [rows, out] (+ [rows, out/128] scales) — the A operand of
 // te_tc_zplus_r16 — instead of fp32 in s_out
-int te_tc_pair_zplus_r(const float* s, const float* derived, const float* x, long long ldx, float* out, long long ld_out,
-                       long long rows, int in_features, int out_features, cudaStream_t st);
-int te_tc_pair_linear_bwd(const float* dy, long long lddy, const float* derived, int in_features, int out_features, float* dx,
+int te_tc_zplus_r(const float* s, const float* derived, const float* x, long long ldx, float* out, long long ld_out,
+                  long long rows, int in_features, int out_features, cudaStream_t st);
+int te_tc_linear_bwd_tf32(const float* dy, long long lddy, const float* derived, int in_features, int out_features, float* dx,
                           const float* e0, long long rows, int epi, cudaStream_t st);

@@ -795,8 +795,19 @@ LinOut lin_out(long long rows, int N, const float* bias, const float* e0, float*
     return o;
 }
 
+// S = sd(R, Z) [rows, out] on the z+ S kernel.  Single-pass: wa = |W| (xabs = bf16(|x|) with BF); two-pass: wa / wb = W+ / W-.
+// hs: block scales of the ZO_F16S output.
 template <bool SINGLE, bool BF, int OUT>
-int zs(const ZsProb<SINGLE, BF, OUT>& p, cudaStream_t st) { return launch(p, dim3(mtiles(p.M), p.N / 128), st); }
+int zs(const float* x, long long ldx, const void* xabs, const void* wa, const void* wb, const float* r, long long ldr,
+       const float* y, long long ldy, const float* bias, void* out, float* hs, long long rows, int in_features, int out_features,
+       cudaStream_t st) {
+    ZsProb<SINGLE, BF, OUT> p;
+    p.M = (int)rows; p.N = out_features; p.K = in_features;
+    p.x = x; p.ldx = ldx; p.xabs = xabs; p.wa = wa; p.wb = wb;
+    p.r = r; p.ldr = ldr; p.y = y; p.ldy = ldy; p.bias = bias;
+    p.out = out; p.ldo = out_features; p.hs = hs;
+    return launch(p, dim3(mtiles(p.M), p.N / 128), st);
+}
 
 }  // namespace
 
@@ -853,38 +864,30 @@ int te_tc_blocksplit_f16(const float* x, long long ldx, long long rows, int cols
 bool te_tc_zplus_supported(long long rows, int in_features, int out_features, long long ldx) {
     return rows > 0 && rows < (1LL << 31) && in_features % 128 == 0 && out_features % 128 == 0 && ldx % 4 == 0;
 }
-bool te_tc_pair_supported(long long rows, int K, int N, long long lda) {
-    return rows > 0 && rows < (1LL << 31) && K % 32 == 0 && N % 128 == 0 && lda % 4 == 0;
-}
-
-int te_tc_pair_zplus_s1(const float* x, long long ldx, float* xabs, const float* derived, const float* r, long long ldr,
-                        const float* y, long long ldy, const float* bias, float* s_out, long long rows, int in_features,
-                        int out_features, cudaStream_t st, bool bf16, float* s16, float* s16_scale) {
+int te_tc_zplus_s1(const float* x, long long ldx, float* xabs, const float* derived, const float* r, long long ldr,
+                   const float* y, long long ldy, const float* bias, float* s_out, long long rows, int in_features,
+                   int out_features, cudaStream_t st, bool bf16, float* s16, float* s16_scale) {
     const long long n = (long long)in_features * out_features;
     if (ldx % 4 != 0 || !a16(x) || !a16(r) || !a16(y) || ldr % 2 != 0 || ldy % 2 != 0) {
-        te_set_last_error("te_tc_pair_zplus_s1: alignment");
+        te_set_last_error("te_tc_zplus_s1: alignment");
         return TE_ERR_ARG;
     }
-    auto fill = [&](auto& p) {
-        p.M = (int)rows; p.N = out_features; p.K = in_features;
-        p.x = x; p.ldx = ldx; p.xabs = xabs; p.wb = nullptr;
-        p.r = r; p.ldr = ldr; p.y = y; p.ldy = ldy; p.bias = bias;
-        p.out = s16 ? (void*)s16 : (void*)s_out; p.ldo = out_features; p.hs = s16_scale;
+    void* o = s16 ? (void*)s16 : (void*)s_out;
+    auto run = [&](auto zs_fn, const float* wa) {
+        return zs_fn(x, ldx, xabs, wa, nullptr, r, ldr, y, ldy, bias, o, s16_scale, rows, in_features, out_features, st);
     };
     if (bf16 && in_features % 64 == 0) {
-        if (!a16(xabs)) { te_set_last_error("te_tc_pair_zplus_s1: alignment"); return TE_ERR_ARG; }
+        if (!a16(xabs)) { te_set_last_error("te_tc_zplus_s1: alignment"); return TE_ERR_ARG; }
         abs_bf16_kernel<<<stride_blocks(rows * (in_features / 4), 256), 256, 0, st>>>(
             x, ldx, reinterpret_cast<__nv_bfloat16*>(xabs), rows, in_features / 4);
         TE_CUDA_CHECK_LAUNCH();
-        if (s16) { ZsProb<true, true, ZO_F16S> p; fill(p); p.wa = derived + 11 * n; return zs(p, st); }
-        ZsProb<true, true, ZO_F32> p; fill(p); p.wa = derived + 11 * n; return zs(p, st);
+        return s16 ? run(zs<true, true, ZO_F16S>, derived + 11 * n) : run(zs<true, true, ZO_F32>, derived + 11 * n);
     }
-    if (s16) { ZsProb<true, false, ZO_F16S> p; fill(p); p.wa = derived + 8 * n; return zs(p, st); }
-    ZsProb<true, false, ZO_F32> p; fill(p); p.wa = derived + 8 * n; return zs(p, st);
+    return s16 ? run(zs<true, false, ZO_F16S>, derived + 8 * n) : run(zs<true, false, ZO_F32>, derived + 8 * n);
 }
 
-int te_tc_pair_zplus_r(const float* s, const float* derived, const float* x, long long ldx, float* out, long long ld_out,
-                       long long rows, int in_features, int out_features, cudaStream_t st) {
+int te_tc_zplus_r(const float* s, const float* derived, const float* x, long long ldx, float* out, long long ld_out,
+                  long long rows, int in_features, int out_features, cudaStream_t st) {
     const long long n = (long long)in_features * out_features;
     ZrProb<0> p;
     memset(&p, 0, sizeof(p));
@@ -911,7 +914,7 @@ int te_tc_zplus_r16(const float* s, float* split, float* scale, const float* der
 
 int te_tc_zplus_linear_relprop(const float* x, long long ldx, const float* derived, const float* r, long long ldr,
                                float* out, float* s_scratch, long long rows, int in_features, int out_features, cudaStream_t st,
-                               const float* y, long long ldy, const float* bias, int bf16, long long ld_out, float* xabs) {
+                               const float* y, long long ldy, const float* bias, ZplusVariant zv, long long ld_out, float* xabs) {
     if (ld_out == 0) ld_out = in_features;
     if (!a16(x) || !a16(derived) || !a16(r) || !a16(out) || !a16(s_scratch)) {
         te_set_last_error("te_gemm_tc: operands must be 16-byte aligned");
@@ -919,48 +922,29 @@ int te_tc_zplus_linear_relprop(const float* x, long long ldx, const float* deriv
     }
     const long long n = (long long)in_features * out_features;
     const bool single = y && a16(y) && ldy % 4 == 0 && (!bias || a16(bias));
-    const bool rb = (bf16 & 1) && (out_features % 64 == 0);          // S as bf16, R kernel with bf16 operands
+    const bool rb = zv.r_bf16 && (out_features % 64 == 0);          // S as bf16, R kernel with bf16 operands
     if (!rb && single && xabs && a16(xabs)) {
-        if ((bf16 & 4) && te_tc_f16_single_supported(rows, out_features, in_features, out_features)) {
+        if (zv.r_f16 && te_tc_fwd16_supported(rows, out_features, in_features, out_features)) {
             // second contraction on block-scaled fp16: S leaves the S kernel in that format, straight into s_scratch
             // ([rows, out] fp16, then the [rows, out/128] scales: rows*out floats hold both)
             float* s16_scale = s_scratch + ((rows * out_features / 2 + 63) & ~63LL);
-            TE_TRY(te_tc_pair_zplus_s1(x, ldx, xabs, derived, r, ldr, y, ldy, bias, nullptr, rows, in_features, out_features, st,
-                                       (bf16 & 2) != 0, s_scratch, s16_scale));
+            TE_TRY(te_tc_zplus_s1(x, ldx, xabs, derived, r, ldr, y, ldy, bias, nullptr, rows, in_features, out_features, st,
+                                  zv.s1_bf16, s_scratch, s16_scale));
             return te_tc_zplus_r16(nullptr, s_scratch, s16_scale, derived, x, ldx, out, ld_out, rows, in_features, out_features, st);
         }
-        TE_TRY(te_tc_pair_zplus_s1(x, ldx, xabs, derived, r, ldr, y, ldy, bias, s_scratch, rows, in_features, out_features, st,
-                                   (bf16 & 2) != 0));
-        return te_tc_pair_zplus_r(s_scratch, derived, x, ldx, out, ld_out, rows, in_features, out_features, st);
+        TE_TRY(te_tc_zplus_s1(x, ldx, xabs, derived, r, ldr, y, ldy, bias, s_scratch, rows, in_features, out_features, st,
+                              zv.s1_bf16));
+        return te_tc_zplus_r(s_scratch, derived, x, ldx, out, ld_out, rows, in_features, out_features, st);
     }
-    // S = sd(R, Z) [rows, out]
-    if (single) {
-        if (rb) {
-            ZsProb<true, false, ZO_BF16> p;
-            p.M = (int)rows; p.N = out_features; p.K = in_features; p.x = x; p.ldx = ldx; p.xabs = nullptr;
-            p.wa = derived + 8 * n; p.wb = nullptr; p.r = r; p.ldr = ldr; p.y = y; p.ldy = ldy; p.bias = bias;
-            p.out = s_scratch; p.ldo = out_features; p.hs = nullptr;
-            TE_TRY(zs(p, st));
-        } else {
-            ZsProb<true, false, ZO_F32> p;
-            p.M = (int)rows; p.N = out_features; p.K = in_features; p.x = x; p.ldx = ldx; p.xabs = nullptr;
-            p.wa = derived + 8 * n; p.wb = nullptr; p.r = r; p.ldr = ldr; p.y = y; p.ldy = ldy; p.bias = bias;
-            p.out = s_scratch; p.ldo = out_features; p.hs = nullptr;
-            TE_TRY(zs(p, st));
-        }
-    } else if (rb) {
-        ZsProb<false, false, ZO_BF16> p;
-        p.M = (int)rows; p.N = out_features; p.K = in_features; p.x = x; p.ldx = ldx; p.xabs = nullptr;
-        p.wa = derived; p.wb = derived + n; p.r = r; p.ldr = ldr; p.y = nullptr; p.ldy = 0; p.bias = nullptr;
-        p.out = s_scratch; p.ldo = out_features; p.hs = nullptr;
-        TE_TRY(zs(p, st));
-    } else {
-        ZsProb<false, false, ZO_F32> p;
-        p.M = (int)rows; p.N = out_features; p.K = in_features; p.x = x; p.ldx = ldx; p.xabs = nullptr;
-        p.wa = derived; p.wb = derived + n; p.r = r; p.ldr = ldr; p.y = nullptr; p.ldy = 0; p.bias = nullptr;
-        p.out = s_scratch; p.ldo = out_features; p.hs = nullptr;
-        TE_TRY(zs(p, st));
-    }
+    // S = sd(R, Z) [rows, out]: single-pass from y, or two-pass
+    auto run = [&](auto zs_fn) {
+        return single ? zs_fn(x, ldx, nullptr, derived + 8 * n, nullptr, r, ldr, y, ldy, bias, s_scratch, nullptr, rows,
+                              in_features, out_features, st)
+                      : zs_fn(x, ldx, nullptr, derived, derived + n, r, ldr, nullptr, 0, nullptr, s_scratch, nullptr, rows,
+                              in_features, out_features, st);
+    };
+    if (single) TE_TRY(rb ? run(zs<true, false, ZO_BF16>) : run(zs<true, false, ZO_F32>));
+    else TE_TRY(rb ? run(zs<false, false, ZO_BF16>) : run(zs<false, false, ZO_F32>));
     if (rb) {
         ZrProb<1> p;
         memset(&p, 0, sizeof(p));
@@ -969,7 +953,7 @@ int te_tc_zplus_linear_relprop(const float* x, long long ldx, const float* deriv
         p.x = x; p.ldx = ldx; p.out = out; p.ldo = ld_out;
         return launch(p, dim3(mtiles(rows), in_features / 128), st);
     }
-    return te_tc_pair_zplus_r(s_scratch, derived, x, ldx, out, ld_out, rows, in_features, out_features, st);
+    return te_tc_zplus_r(s_scratch, derived, x, ldx, out, ld_out, rows, in_features, out_features, st);
 }
 
 // ---- Linear GEMMs ---------------------------------------------------------------------------------------------------
@@ -1010,11 +994,11 @@ int te_tc_linear_bwd(const float* dy, const float* derived, int in_features, int
     return TE_ERR_UNSUPPORTED;
 }
 
-int te_tc_pair_linear_bwd(const float* dy, long long lddy, const float* derived, int in_features, int out_features, float* dx,
+int te_tc_linear_bwd_tf32(const float* dy, long long lddy, const float* derived, int in_features, int out_features, float* dx,
                           const float* e0, long long rows, int epi, cudaStream_t st) {
     const long long n = (long long)in_features * out_features;
     if (!a16(dy) || lddy % 4 != 0 || !a16(derived) || !a16(dx) || (e0 && !a16(e0))) {
-        te_set_last_error("te_tc_pair_linear_bwd: operands must be 16-byte aligned");
+        te_set_last_error("te_tc_linear_bwd_tf32: operands must be 16-byte aligned");
         return TE_ERR_ARG;
     }
     const LinOut o = lin_out(rows, in_features, nullptr, e0, dx, nullptr);
@@ -1027,14 +1011,13 @@ int te_tc_pair_linear_bwd(const float* dy, long long lddy, const float* derived,
         Lin1Prob<TE_TC_EPI_GELU_BWD> p; p.K = out_features; p.a = dy; p.lda = lddy; p.b = derived + 6 * n; p.o = o;
         return launch(p, grid, st);
     }
-    te_set_last_error("te_tc_pair_linear_bwd: unsupported epilogue");
+    te_set_last_error("te_tc_linear_bwd_tf32: unsupported epilogue");
     return TE_ERR_UNSUPPORTED;
 }
 
 bool te_tc_fwd16_supported(long long rows, int K, int N, long long lda) {
     return rows > 0 && rows < (1LL << 31) && K % 64 == 0 && N % 128 == 0 && lda % 4 == 0;
 }
-bool te_tc_f16_single_supported(long long rows, int K, int N, long long lda) { return te_tc_fwd16_supported(rows, K, N, lda); }
 
 int te_tc_linear_fwd16(const float* x, long long ldx, float* split, float* scale, const float* derived, int in_features,
                        int out_features, const float* bias, float* y, float* y2, const float* e0, long long rows, int epi,

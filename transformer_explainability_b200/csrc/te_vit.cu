@@ -6,8 +6,6 @@
 // Reference wiring: baselines/ViT/ViT_LRP.py (forward :305-322, relprop :324-369, Block :196-213,
 // Attention :132-177, Mlp :61-74), baselines/ViT/ViT_explanation_generator.py:25-41.
 #include <string.h>
-#include <string>
-#include <vector>
 
 #include "../../include/te_b200.h"
 #include "te_engine_util.h"
@@ -44,11 +42,11 @@ static bool make_dims(const te_vit_config* c, int B, Dims& d) {
 }
 
 // ---- flat weight buffer ------------------------------------------------------------------------
-struct WEntry { std::string name; long long numel; long long offset; };
+using te_util::WTable;
 
-static std::vector<WEntry> weight_table(const te_vit_config* c) {
+static WTable weight_table(const te_vit_config* c) {
     Dims d;
-    std::vector<WEntry> t;
+    WTable t;
     if (!make_dims(c, 1, d)) return t;
     long long off = 0;
     auto add = [&](const std::string& n, long long numel) {
@@ -96,7 +94,7 @@ struct Weights {
 };
 
 static void bind_weights(const te_vit_config* c, const float* base, Weights& w) {
-    const std::vector<WEntry> t = weight_table(c);
+    const WTable t = weight_table(c);
     size_t i = 0;
     auto next = [&]() { return base + t[i++].offset; };
     w.patchw = next(); w.patchb = next(); w.cls = next();
@@ -146,12 +144,7 @@ struct Workspace {
 };
 
 static void carve(const Dims& d, char* base, Workspace& ws) {
-    long long off = 0;
-    auto take = [&](long long nfloat) -> float* {
-        float* p = base ? reinterpret_cast<float*>(base + off) : nullptr;
-        off += ((nfloat * 4 + 255) / 256) * 256;
-        return p;
-    };
+    te_util::Bump take{base};
     const long long MD = d.M * d.D, MF = d.M * d.F, M3D = d.M * 3LL * d.D;
     const long long AT = (long long)d.B * d.H * d.N * d.NP;
     for (int l = 0; l < d.L; ++l) {
@@ -178,22 +171,16 @@ static void carve(const Dims& d, char* base, Workspace& ws) {
     ws.pix = take(te_patch_relprop_scratch_floats(d.B, d.Cin, d.img, d.P, d.D));
     ws.addpart = reinterpret_cast<double*>(take((long long)d.B * TE_ADD_SPLIT * 3 * 2));
     ws.index_tmp = reinterpret_cast<int*>(take(d.B));
-    ws.bytes = off;
+    ws.bytes = take.off;
 }
 
 // ---- GEMM parameter helpers (shared builders live in te_engine_util.h) ----------------------------
-using te_util::HeadOp;
-using te_util::head_rows;
 using te_util::linear_bwd;
 using te_util::linear_fwd;
 
 static int check_ws(const te_vit_config* cfg, int batch, void* workspace, long long bytes, Dims& d, Workspace& ws) {
-    if (batch <= 0 || !workspace) { te_set_last_error("te_vit: batch <= 0 or null workspace"); return TE_ERR_ARG; }
-    if (!make_dims(cfg, batch, d)) return TE_ERR_ARG;
-    if (((uintptr_t)workspace & 255u) != 0) { te_set_last_error("te_vit: workspace must be 256-byte aligned"); return TE_ERR_ARG; }
-    carve(d, reinterpret_cast<char*>(workspace), ws);
-    if (ws.bytes > bytes) { te_set_last_error("te_vit: workspace too small"); return TE_ERR_WORKSPACE; }
-    return TE_OK;
+    return te_util::check_ws("te_vit", batch, workspace, bytes, [&] { return make_dims(cfg, batch, d); },
+                             [&] { carve(d, reinterpret_cast<char*>(workspace), ws); return ws.bytes; });
 }
 
 }  // namespace
@@ -201,31 +188,11 @@ static int check_ws(const te_vit_config* cfg, int batch, void* workspace, long l
 // ================================================================================================
 // public: weights / workspace description
 // ================================================================================================
-extern "C" int te_vit_num_weights(const te_vit_config* cfg) {
-    const auto t = weight_table(cfg);
-    return t.empty() ? TE_ERR_ARG : (int)t.size() - 1;
-}
-extern "C" const char* te_vit_weight_name(const te_vit_config* cfg, int i) {
-    static thread_local std::string s;
-    const auto t = weight_table(cfg);
-    if (i < 0 || i + 1 >= (int)t.size()) return nullptr;
-    s = t[i].name;
-    return s.c_str();
-}
-extern "C" long long te_vit_weight_numel(const te_vit_config* cfg, int i) {
-    const auto t = weight_table(cfg);
-    if (i < 0 || i + 1 >= (int)t.size()) return TE_ERR_ARG;
-    return t[i].numel;
-}
-extern "C" long long te_vit_weight_offset(const te_vit_config* cfg, int i) {
-    const auto t = weight_table(cfg);
-    if (i < 0 || i + 1 >= (int)t.size()) return TE_ERR_ARG;
-    return t[i].offset;
-}
-extern "C" long long te_vit_weight_total(const te_vit_config* cfg) {
-    const auto t = weight_table(cfg);
-    return t.empty() ? TE_ERR_ARG : t.back().offset;
-}
+extern "C" int te_vit_num_weights(const te_vit_config* cfg) { return te_util::wt_count(weight_table(cfg)); }
+extern "C" const char* te_vit_weight_name(const te_vit_config* cfg, int i) { return te_util::wt_name(weight_table(cfg), i); }
+extern "C" long long te_vit_weight_numel(const te_vit_config* cfg, int i) { return te_util::wt_numel(weight_table(cfg), i); }
+extern "C" long long te_vit_weight_offset(const te_vit_config* cfg, int i) { return te_util::wt_offset(weight_table(cfg), i); }
+extern "C" long long te_vit_weight_total(const te_vit_config* cfg) { return te_util::wt_total(weight_table(cfg)); }
 extern "C" long long te_vit_workspace_bytes(const te_vit_config* cfg, int batch) {
     Dims d;
     if (batch <= 0 || !make_dims(cfg, batch, d)) return TE_ERR_ARG;
@@ -243,24 +210,16 @@ extern "C" int te_vit_forward(const te_vit_config* cfg, const float* weights, co
     Dims d; Workspace ws;
     TE_TRY(check_ws(cfg, batch, workspace, workspace_bytes, d, ws));
     if (!weights || !images) { te_set_last_error("te_vit_forward: null pointer"); return TE_ERR_ARG; }
-    if ((flags & TE_FLAG_LINEAR_TENSOR_CORES) && !derived) {
-        te_set_last_error("te_vit_forward: TE_FLAG_LINEAR_TENSOR_CORES needs the derived weight buffer");
-        return TE_ERR_ARG;
-    }
-    const float* lbase = (flags & TE_FLAG_LINEAR_TENSOR_CORES) ? derived : nullptr;
-    // fp16-split forward Linears (te_tc_wgmma.cu).  The block-scaled split of every Linear input lives in buffers that are idle
-    // until the backward pass: A = tD[1] (+ scales tD[0]) for the D-wide inputs, B = tF[1] (+ scales tD[2]) for the GELU output.
-    // LayerNorm emits the split of what it produces; the attention output and the GELU output go through the pre-pass (emitting
-    // the split from the fc1 GELU epilogue was measured: 1.01 ms against 0.56 + 0.2 ms, profiles/r02_results.md).
-    const bool f16 = lbase && (flags & TE_FLAG_LINEAR_F16_SPLIT) && d.F >= d.D && te_tc_fwd16_supported(d.M, d.D, 3 * d.D, d.D) &&
-                     te_tc_fwd16_supported(d.M, d.D, d.D, d.D) && te_tc_fwd16_supported(d.M, d.D, d.F, d.D) &&
-                     te_tc_fwd16_supported(d.M, d.F, d.D, d.F);
-    const te_util::F16Split fsA_ready = {ws.tD[1], ws.tD[0], true};
-    const te_util::F16Split fsA_pre = {ws.tD[1], ws.tD[0], false};
-    const bool gsf = te_engine_gelu_split();
-    const te_util::F16Split fsA_fc1 = {ws.tD[1], ws.tD[0], true, gsf ? ws.tF[1] : nullptr, gsf ? ws.tD[2] : nullptr};
-    const te_util::F16Split fsB = {ws.tF[1], ws.tD[2], gsf};
+    te_util::Select sel;
+    TE_TRY(te_util::decode_flags(sel, "te_vit_forward", flags, derived, 0, false));
+    // fp16-split forward Linears: split of the D-wide inputs in tD[1] (+ scales tD[0]), of the GELU output in tF[1] (+ scales
+    // tD[2]); all idle until the backward pass
+    const te_util::F16Forward f16 = te_util::f16_forward(sel, d.M, d.D, d.F, ws.tD[1], ws.tD[0], ws.tF[1], ws.tD[2]);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    auto layernorm = [&](const float* x, const float* g, const float* b, float* y, float* mean, float* rstd) {
+        return f16.on ? te_launch_layernorm_split(x, g, b, y, mean, rstd, d.M, d.D, cfg->eps_block, f16.qkv.split, f16.qkv.scale, st)
+                      : te_launch_layernorm(x, g, b, y, mean, rstd, d.M, d.D, cfg->eps_block, st);
+    };
     Weights w;
     bind_weights(cfg, weights, w);
     const float scale = 1.0f / sqrtf((float)d.dh);
@@ -277,35 +236,23 @@ extern "C" int te_vit_forward(const te_vit_config* cfg, const float* weights, co
         LayerAct& a = ws.layer[l];
         const BlockW& bw = w.blk[l];
         float* x_next = (l + 1 < d.L) ? ws.layer[l + 1].x_in : ws.x_last;
-        const DerivedW lw = bind_derived(d, lbase, l);
-        if (f16)
-            TE_TRY(te_launch_layernorm_split(a.x_in, bw.n1w, bw.n1b, a.xn1, a.mean1, a.rstd1, d.M, d.D, cfg->eps_block, ws.tD[1],
-                                             ws.tD[0], st));
-        else
-            TE_TRY(te_launch_layernorm(a.x_in, bw.n1w, bw.n1b, a.xn1, a.mean1, a.rstd1, d.M, d.D, cfg->eps_block, st));
+        const DerivedW lw = bind_derived(d, sel.lbase, l);
+        TE_TRY(layernorm(a.x_in, bw.n1w, bw.n1b, a.xn1, a.mean1, a.rstd1));
         TE_TRY(te_util::linear_fwd_tc(lw.qkv, a.xn1, d.D, bw.qkvw, bw.qkvb, a.qkv, nullptr, nullptr, d.M, d.D, 3 * d.D,
-                                      TE_EPI_BIAS, st, f16 ? &fsA_ready : nullptr));
-        const HeadOp q = head_rows(a.qkv, 3 * d.D, d.N, d.dh);
-        const HeadOp k = head_rows(a.qkv + d.D, 3 * d.D, d.N, d.dh);
-        const HeadOp v = head_rows(a.qkv + 2 * d.D, 3 * d.D, d.N, d.dh);
+                                      TE_EPI_BIAS, st, &f16.qkv));
         // dots = q k^T * scale ; attn = softmax(dots)        (:139-141)
-        TE_TRY(te_util::attn_probs((flags & TE_FLAG_ATTN_TENSOR_CORES) != 0, d.B, d.H, d.N, d.NP, d.dh, a.qkv, 3 * d.D,
-                                   a.qkv + d.D, 3 * d.D, a.P, scale, st));
+        TE_TRY(te_util::attn_probs(sel.atc, d.B, d.H, d.N, d.NP, d.dh, a.qkv, 3 * d.D, a.qkv + d.D, 3 * d.D, a.P, scale, st));
         // out = attn v -> 'b h n d -> b n (h d)'              (:147-148)
-        TE_TRY(te_util::attn_nk((flags & TE_FLAG_ATTN_TENSOR_CORES) != 0, d.B, d.H, d.N, d.NP, d.dh, a.P, 0, a.qkv + 2 * d.D,
-                                3 * d.D, a.ctx, d.D, nullptr, 1.f, TE_EPI_STORE, st));
+        TE_TRY(te_util::attn_nk(sel.atc, d.B, d.H, d.N, d.NP, d.dh, a.P, 0, a.qkv + 2 * d.D, 3 * d.D, a.ctx, d.D, nullptr, 1.f,
+                                TE_EPI_STORE, st));
         // proj + residual add1                                  (:150, :198)
         TE_TRY(te_util::linear_fwd_tc(lw.proj, a.ctx, d.D, bw.projw, bw.projb, a.attn_out, a.x_mid, a.x_in, d.M, d.D, d.D,
-                                      TE_EPI_BIAS_ADD, st, f16 ? &fsA_pre : nullptr));
-        if (f16)
-            TE_TRY(te_launch_layernorm_split(a.x_mid, bw.n2w, bw.n2b, a.xn2, a.mean2, a.rstd2, d.M, d.D, cfg->eps_block, ws.tD[1],
-                                             ws.tD[0], st));
-        else
-            TE_TRY(te_launch_layernorm(a.x_mid, bw.n2w, bw.n2b, a.xn2, a.mean2, a.rstd2, d.M, d.D, cfg->eps_block, st));
+                                      TE_EPI_BIAS_ADD, st, &f16.proj));
+        TE_TRY(layernorm(a.x_mid, bw.n2w, bw.n2b, a.xn2, a.mean2, a.rstd2));
         TE_TRY(te_util::linear_fwd_tc(lw.fc1, a.xn2, d.D, bw.fc1w, bw.fc1b, a.h, a.g, nullptr, d.M, d.D, d.F,
-                                      TE_EPI_BIAS_GELU, st, f16 ? &fsA_fc1 : nullptr));
+                                      TE_EPI_BIAS_GELU, st, &f16.fc1));
         TE_TRY(te_util::linear_fwd_tc(lw.fc2, a.g, d.F, bw.fc2w, bw.fc2b, a.mlp_out, x_next, a.x_mid, d.M, d.F, d.D,
-                                      TE_EPI_BIAS_ADD, st, f16 ? &fsB : nullptr));
+                                      TE_EPI_BIAS_ADD, st, &f16.fc2));
     }
     // final norm, pool token 0 (and 1), head(s)                (:318-321)
     TE_TRY(te_launch_layernorm(ws.x_last, w.normw, w.normb, ws.xf, nullptr, nullptr, d.M, d.D, cfg->eps_final, st));
@@ -362,22 +309,10 @@ extern "C" int te_vit_attribute(const te_vit_config* cfg, const float* weights, 
     bind_weights(cfg, weights, w);
     const float scale = 1.0f / sqrtf((float)d.dh);
     const long long MD = d.M * d.D;
-    const int low = (flags & (TE_FLAG_KEEP_ALL_CAMS | TE_FLAG_RELPROP_TO_INPUT)) ? 0 : start_layer;   // lowest block the relprop must reach
-    const float* dbase = (flags & TE_FLAG_ZPLUS_TENSOR_CORES) ? derived : nullptr;
-    if ((flags & (TE_FLAG_ZPLUS_TENSOR_CORES | TE_FLAG_LINEAR_TENSOR_CORES)) && !derived) {
-        te_set_last_error("te_vit_attribute: tensor-core flags need the derived weight buffer");
-        return TE_ERR_ARG;
-    }
-    const float* lbase = (flags & TE_FLAG_LINEAR_TENSOR_CORES) ? derived : nullptr;
-    const bool atc = (flags & TE_FLAG_ATTN_TENSOR_CORES) != 0;
-    const bool btf = (flags & TE_FLAG_BACKWARD_TF32) != 0;       // single-pass TF32 backward Linears
-    // single-pass fp16 backward Linears: hi-only split of the incoming gradient in tF[1], block scales in t3D[1] (idle until the relprop)
-    const te_util::F16Split bfs_v = {ws.tF[1], ws.t3D[1], false};
-    const te_util::F16Split* bfs = (lbase && (flags & TE_FLAG_BACKWARD_F16)) ? &bfs_v : nullptr;
-    const bool rtf = (flags & TE_FLAG_RELPROP_TF32) != 0;        // single-pass TF32 relevance-side attention contractions
+    // fp16 backward split of dy in tF[1], block scales in t3D[1] (idle until the relprop)
+    te_util::Select sel;
+    TE_TRY(te_util::decode_flags(sel, "te_vit_attribute", flags, derived, start_layer, true, ws.tF[1], ws.t3D[1]));
     const bool lrpv = (flags & TE_FLAG_RULES_LRP) != 0;         // rule library of modules/layers_lrp.py (ViT_orig_LRP.py)
-    const int zb = ((flags & TE_FLAG_ZPLUS_BF16) ? 1 : 0) | ((flags & TE_FLAG_ZPLUS_S1_BF16) ? 2 : 0) |
-                   ((flags & TE_FLAG_ZPLUS_R_F16) ? 4 : 0);                                               // bf16 / fp16 variants of the z+ rule
 
     // ---- class index and seeds  (ViT_explanation_generator.py:28-35) ---------------------------
     TE_TRY(te_launch_argmax(ws.logits, index, d.B, d.C, /*only_negative=*/1, st));
@@ -402,27 +337,17 @@ extern "C" int te_vit_attribute(const te_vit_config* cfg, const float* weights, 
     for (int l = d.L - 1; l >= start_layer; --l) {
         LayerAct& a = ws.layer[l];
         const BlockW& bw = w.blk[l];
-        const HeadOp q = head_rows(a.qkv, 3 * d.D, d.N, d.dh);
-        const HeadOp k = head_rows(a.qkv + d.D, 3 * d.D, d.N, d.dh);
-        const HeadOp v = head_rows(a.qkv + 2 * d.D, 3 * d.D, d.N, d.dh);
-        const DerivedW lw = bind_derived(d, lbase, l);
+        const DerivedW lw = bind_derived(d, sel.lbase, l);
         // mlp branch
-        TE_TRY(te_util::linear_bwd_tc(lw.fc2, dxa, bw.fc2w, dF, a.h, d.M, d.F, d.D, TE_EPI_GELU_BWD, st, btf, bfs));
-        TE_TRY(te_util::linear_bwd_tc(lw.fc1, dF, bw.fc1w, dxn, nullptr, d.M, d.D, d.F, TE_EPI_STORE, st, btf, bfs));
+        TE_TRY(te_util::linear_bwd_tc(lw.fc2, dxa, bw.fc2w, dF, a.h, d.M, d.F, d.D, TE_EPI_GELU_BWD, st, sel.btf, &sel.bfs));
+        TE_TRY(te_util::linear_bwd_tc(lw.fc1, dF, bw.fc1w, dxn, nullptr, d.M, d.D, d.F, TE_EPI_STORE, st, sel.btf, &sel.bfs));
         TE_TRY(te_launch_layernorm_bwd(dxn, a.x_mid, bw.n2w, a.mean2, a.rstd2, dxa, dxb, d.M, d.D, st));
         // attention branch
-        TE_TRY(te_util::linear_bwd_tc(lw.proj, dxb, bw.projw, dctx, nullptr, d.M, d.D, d.D, TE_EPI_STORE, st, btf, bfs));
-        TE_TRY(te_util::attn_nn(atc, d.B, d.H, d.N, d.NP, d.dh, dctx, d.D, a.qkv + 2 * d.D, 3 * d.D, a.G, nullptr, 1.f,
-                                TE_EPI_STORE, st, btf));                                 // G = dctx v^T
-        if (l == start_layer) break;                                                // lower gradients are never read
-        TE_TRY(te_util::attn_nk(atc, d.B, d.H, d.N, d.NP, d.dh, a.P, 1, dctx, d.D, dqkv + 2 * d.D, 3 * d.D, nullptr, 1.f,
-                                TE_EPI_STORE, st, btf));                                 // dV = P^T dctx
-        TE_TRY(te_launch_softmax_bwd(a.P, a.G, dS, (long long)d.B * d.H * d.N, d.N, d.NP, scale, st));
-        TE_TRY(te_util::attn_nk(atc, d.B, d.H, d.N, d.NP, d.dh, dS, 0, a.qkv + d.D, 3 * d.D, dqkv, 3 * d.D, nullptr, 1.f,
-                                TE_EPI_STORE, st, btf));                                 // dQ = dS k
-        TE_TRY(te_util::attn_nk(atc, d.B, d.H, d.N, d.NP, d.dh, dS, 1, a.qkv, 3 * d.D, dqkv + d.D, 3 * d.D, nullptr, 1.f,
-                                TE_EPI_STORE, st, btf));                                 // dK = dS^T q
-        TE_TRY(te_util::linear_bwd_tc(lw.qkv, dqkv, bw.qkvw, dxn, nullptr, d.M, d.D, 3 * d.D, TE_EPI_STORE, st, btf, bfs));
+        TE_TRY(te_util::linear_bwd_tc(lw.proj, dxb, bw.projw, dctx, nullptr, d.M, d.D, d.D, TE_EPI_STORE, st, sel.btf, &sel.bfs));
+        const bool last = (l == start_layer);                                       // lower gradients are never read
+        TE_TRY(te_util::attn_block_bwd(sel, d.B, d.H, d.N, d.NP, d.dh, a.qkv, a.P, dctx, a.G, dS, dqkv, scale, last, st));
+        if (last) break;
+        TE_TRY(te_util::linear_bwd_tc(lw.qkv, dqkv, bw.qkvw, dxn, nullptr, d.M, d.D, 3 * d.D, TE_EPI_STORE, st, sel.btf, &sel.bfs));
         TE_TRY(te_launch_layernorm_bwd(dxn, a.x_in, bw.n1w, a.mean1, a.rstd1, dxb, dxa, d.M, d.D, st));
     }
 
@@ -437,7 +362,7 @@ extern "C" int te_vit_attribute(const te_vit_config* cfg, const float* weights, 
                      float* sbuf, long long rows, int in, int outf, const float* y, long long ldy, const float* bias,
                      long long ld_out, float* xabs) -> int {
         if (lrpv) return te_zplus_linear_relprop_lrp(x, ldx, wt, r, ldr, out, sbuf, rows, in, outf, st);
-        return te_zplus_linear_relprop_ldr(x, ldx, wt, dwt, r, ldr, out, sbuf, rows, in, outf, st, y, ldy, bias, zb, ld_out, xabs);
+        return te_zplus_linear_relprop_ldr(x, ldx, wt, dwt, r, ldr, out, sbuf, rows, in, outf, st, y, ldy, bias, sel.zv, ld_out, xabs);
     };
     auto addrule = [&](const float* x1, const float* x2, const float* r, float* r1, float* r2) -> int {
         return te_launch_add_relprop(x1, x2, r, r1, r2, lrpv ? nullptr : ws.addpart, d.B, (long long)d.N * d.D, st);
@@ -449,13 +374,10 @@ extern "C" int te_vit_attribute(const te_vit_config* cfg, const float* weights, 
                      nullptr, 0, nullptr, 0, nullptr));
     TE_TRY(te_launch_index_select_relprop(ws.xf, ws.rhead0, cfg->distilled ? ws.rhead1 : nullptr, R, d.B, d.N, d.D, st));
 
-    for (int l = d.L - 1; l >= low; --l) {
+    for (int l = d.L - 1; l >= sel.low; --l) {
         LayerAct& a = ws.layer[l];
         const BlockW& bw = w.blk[l];
-        const DerivedW dw = bind_derived(d, dbase, l);
-        const HeadOp q = head_rows(a.qkv, 3 * d.D, d.N, d.dh);
-        const HeadOp k = head_rows(a.qkv + d.D, 3 * d.D, d.N, d.dh);
-        const HeadOp v = head_rows(a.qkv + 2 * d.D, 3 * d.D, d.N, d.dh);
+        const DerivedW dw = bind_derived(d, sel.dbase, l);
         // Block.relprop :203-213
         // In the TOP block the relevance that enters is non-zero only in the pooled token's row (IndexSelect.relprop, a7),
         // and every rule down to the proj rule is row-wise: Add / Clone map a zero row to a zero row, the z+ rule computes
@@ -472,20 +394,11 @@ extern "C" int te_vit_attribute(const te_vit_config* cfg, const float* weights, 
         // Attention.relprop :154-177
         if (top) TE_TRY(te_launch_fill(R3, 0.f, MD, st));                                   // rows the strided rule does not write
         TE_TRY(zrule(a.ctx, sD, bw.projw, dw.proj, R2, sD, R3, S, zr, d.D, d.D, a.attn_out, sD, bw.projb, sD, S + MD));   // proj
-        // matmul2 rule: Z = attn v is the saved ctx itself (bit-identical recomputation in the reference)
-        TE_TRY(te_launch_sd(R3, a.ctx, S, MD, st));
-        TE_TRY(te_util::attn_nn(atc, d.B, d.H, d.N, d.NP, d.dh, S, d.D, a.qkv + 2 * d.D, 3 * d.D, a.cam, a.P, 0.5f,
-                                TE_EPI_MUL, st, rtf));                                   // attn_cam = (P * (S v^T)) / 2   :160-165
-        if (l == low && !(flags & TE_FLAG_RELPROP_TO_INPUT)) break;                                                        // nothing below is consumed
-        TE_TRY(te_util::attn_nk(atc, d.B, d.H, d.N, d.NP, d.dh, a.P, 1, S, d.D, Rqkv + 2 * d.D, 3 * d.D, a.qkv + 2 * d.D, 0.5f,
-                                TE_EPI_MUL, st, rtf));                                   // cam_v
-        // matmul1 rule (unscaled Z = q k^T)  :170-173
-        TE_TRY(te_util::attn_nn(atc, d.B, d.H, d.N, d.NP, d.dh, a.qkv, 3 * d.D, a.qkv + d.D, 3 * d.D, S1, a.cam, 1.f,
-                                TE_EPI_SD, st));
-        TE_TRY(te_util::attn_nk(atc, d.B, d.H, d.N, d.NP, d.dh, S1, 0, a.qkv + d.D, 3 * d.D, Rqkv, 3 * d.D, a.qkv, 0.5f,
-                                TE_EPI_MUL, st, rtf));                                   // cam_q
-        TE_TRY(te_util::attn_nk(atc, d.B, d.H, d.N, d.NP, d.dh, S1, 1, a.qkv, 3 * d.D, Rqkv + d.D, 3 * d.D, a.qkv + d.D, 0.5f,
-                                TE_EPI_MUL, st, rtf));                                   // cam_k
+        // matmul2 rule -> attn_cam (:160-165), cam_v ; matmul1 rule -> cam_q, cam_k (:170-173)
+        const bool last = (l == sel.low && !(flags & TE_FLAG_RELPROP_TO_INPUT));      // nothing below attn_cam is consumed
+        TE_TRY(te_util::attn_relprop_pv(sel, d.B, d.H, d.N, d.NP, d.dh, a.qkv, a.P, R3, a.ctx, S, a.cam, Rqkv, last, st));
+        if (last) break;
+        TE_TRY(te_util::attn_relprop_qk(sel, d.B, d.H, d.N, d.NP, d.dh, a.qkv, a.cam, S1, Rqkv, st));
         TE_TRY(zrule(a.xn1, d.D, bw.qkvw, dw.qkv, Rqkv, 3 * d.D, R2, S, d.M, d.D, 3 * d.D, a.qkv, 3 * d.D, bw.qkvb, 0, RF));   // qkv ; norm1 id
         TE_TRY(te_launch_clone_relprop(a.x_in, R1, R2, nullptr, R, MD, st));                                       // clone1
     }
@@ -551,12 +464,7 @@ extern "C" int te_vit_tensor(const te_vit_config* cfg, int batch, void* workspac
     if (batch <= 0 || !make_dims(cfg, batch, d)) return TE_ERR_ARG;
     carve(d, reinterpret_cast<char*>(workspace), ws);
     const std::string n(name);
-    auto set = [&](float* p, long long d0, long long d1, long long d2, long long d3, long long s0, long long s1,
-                   long long s2, long long s3) {
-        *ptr = p; dims[0] = d0; dims[1] = d1; dims[2] = d2; dims[3] = d3;
-        strides[0] = s0; strides[1] = s1; strides[2] = s2; strides[3] = s3;
-        return TE_OK;
-    };
+    const te_util::View set{ptr, dims, strides};
     if (n == "logits") return set(ws.logits, d.B, d.C, 1, 1, d.C, 1, 1, 1);
     if (n == "relevance_in") return set(ws.tD[0], d.B, d.N, d.D, 1, (long long)d.N * d.D, d.D, 1, 1);
     if (n == "rollout_mats") return set(ws.mats, d.L, d.B, d.N, d.N, (long long)d.B * d.N * d.NP, (long long)d.N * d.NP, d.NP, 1);

@@ -1,8 +1,13 @@
 // z+ Linear rule driver: fp32 SIMT path (te_gemm.cu) or wgmma tensor-core path (te_tc_wgmma.cu).
 #include "te_zplus.h"
+#include "../../include/te_b200.h"
 #include "te_gemm.cuh"
 #include "te_gemm_tc.h"
 #include <string.h>
+
+ZplusVariant te_zplus_from_flags(unsigned flags) {
+    return {(flags & TE_FLAG_ZPLUS_BF16) != 0, (flags & TE_FLAG_ZPLUS_S1_BF16) != 0, (flags & TE_FLAG_ZPLUS_R_F16) != 0};
+}
 
 int te_zplus_linear_relprop(const float* x, long long ldx, const float* w, const float* w_derived, const float* r,
                             float* out, float* s_scratch, long long rows, int in_features, int out_features,
@@ -13,14 +18,14 @@ int te_zplus_linear_relprop(const float* x, long long ldx, const float* w, const
 
 int te_zplus_linear_relprop_ldr(const float* x, long long ldx, const float* w, const float* w_derived, const float* r,
                                 long long ldr, float* out, float* s_scratch, long long rows, int in_features,
-                                int out_features, cudaStream_t st, const float* y, long long ldy, const float* bias, int bf16,
+                                int out_features, cudaStream_t st, const float* y, long long ldy, const float* bias, ZplusVariant zv,
                                 long long ld_out, float* xabs) {
     if (rows <= 0) return TE_OK;
     if (ld_out == 0) ld_out = in_features;
     if (rows > 0x7fffffffLL || ldx > 0x7fffffffLL) { te_set_last_error("zplus: rows/ldx overflow int"); return TE_ERR_ARG; }
     if (w_derived && ldr % 4 == 0 && ld_out % 4 == 0 && te_tc_zplus_supported(rows, in_features, out_features, ldx)) {
         const int rc = te_tc_zplus_linear_relprop(x, ldx, w_derived, r, ldr, out, s_scratch, rows, in_features, out_features, st, y,
-                                                  ldy, bias, bf16, ld_out, xabs);
+                                                  ldy, bias, zv, ld_out, xabs);
         if (rc != TE_ERR_UNSUPPORTED) return rc;
     }
     if (ld_out > 0x7fffffffLL) { te_set_last_error("zplus: ld_out overflow int"); return TE_ERR_ARG; }

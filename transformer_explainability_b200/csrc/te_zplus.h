@@ -3,6 +3,13 @@
 #pragma once
 #include "te_common.cuh"
 
+// Reduced-precision variants of the tensor-core z+ rule, decoded from the engine flags by te_zplus_from_flags:
+//   r_bf16  (TE_FLAG_ZPLUS_BF16)     S is stored as bf16 and the second contraction runs on bf16 operands
+//   s1_bf16 (TE_FLAG_ZPLUS_S1_BF16)  the |x| |W|^T term of the single-pass S kernel on bf16 operands
+//   r_f16   (TE_FLAG_ZPLUS_R_F16)    the second contraction on fp16 MMAs, fed a block-scaled fp16 S by the S kernel's epilogue
+struct ZplusVariant { bool r_bf16, s1_bf16, r_f16; };
+ZplusVariant te_zplus_from_flags(unsigned flags);
+
 // x [rows, in] with row stride ldx ; w [out, in] ; r [rows, out] ; out [rows, in] ; s_scratch [rows, out].
 // w_derived: the te_tc_prepare_weights() copies of w, or NULL.  When given (and the shape qualifies) both
 // contractions run on wgmma tensor cores (TF32 inputs, fp32 accumulate); otherwise — and as the checker —
@@ -15,12 +22,10 @@ int te_zplus_linear_relprop(const float* x, long long ldx, const float* w, const
 int te_zplus_linear_relprop_ldr(const float* x, long long ldx, const float* w, const float* w_derived, const float* r,
                                 long long ldr, float* out, float* s_scratch, long long rows, int in_features,
                                 int out_features, cudaStream_t st, const float* y = nullptr, long long ldy = 0,
-                                const float* bias = nullptr, int bf16 = 0, long long ld_out = 0,
+                                const float* bias = nullptr, ZplusVariant zv = {}, long long ld_out = 0,
                                 float* xabs = nullptr);
-// bf16: bit 0 round-1 bf16 R kernel (TE_FLAG_ZPLUS_BF16), bit 1 bf16 |x||W|^T term (TE_FLAG_ZPLUS_S1_BF16), bit 2 second
-// contraction on fp16 MMAs with a block-scaled fp16 S written by the S kernel's epilogue (TE_FLAG_ZPLUS_R_F16)
-// xabs: scratch [rows, in] (the tf32(|x|) operand of the persistent single-pass S kernel); without it the tensor-core path
-// uses the round-1 kernels.
+// xabs: scratch [rows, in] (the |x| operand of the single-pass S kernel); without it the tensor-core path uses the two-pass
+// S kernel.
 // ld_out: row stride of out (0 = in_features).  With row strides on x, r, y and out the rule runs on a strided subset of
 // token rows — the CLS rows of the top block, the only rows whose relevance is non-zero there (SURVEY.md 8a).
 

@@ -125,7 +125,7 @@ def linear_backward_f16(dy, w):
 
 @_on_device
 def linear_backward_tf32(dy, w):
-    """dx = dy W as a single-pass TF32 GEMM on the persistent CTA-pair kernel (what TE_FLAG_BACKWARD_TF32 selects)."""
+    """dx = dy W as a single-pass TF32 wgmma GEMM (what TE_FLAG_BACKWARD_TF32 selects)."""
     _req(dy, w)
     if w.dim() != 2 or dy.shape[-1] != w.shape[0]:
         raise ValueError("linear_backward_tf32: dy [...,out], w [out,in] expected")
