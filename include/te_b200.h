@@ -289,6 +289,47 @@ TE_API int te_f16_block_split(const float* x, int rows, int cols, void* hi, void
 TE_API int te_linear_backward_ex(const float* dy, const float* w, float* dx, float* scratch, int rows, int in_features,
                           int out_features, unsigned flags, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Diagnostic entry points — exported for kernel unit tests only.  Each runs the named tensor-core kernel (or kernel family)
+ * directly: a shape or epilogue that kernel does not take returns TE_ERR_UNSUPPORTED with a te_last_error() message, never a
+ * fall-back to another kernel, so a call that succeeds has run the kernel it asked for.
+ * ---------------------------------------------------------------------------------------------- */
+/* Linear GEMMs with their fused epilogues, through the engines' own kernel selection.  epi: 0 STORE (y = x W^T), 1 BIAS (+ bias),
+ * 2 BIAS_GELU (y2 = erf-GELU(y) as well), 3 BIAS_ADD (y2 = e0 + y as well); backward 0 STORE (dx = dy W), 4 GELU_BWD
+ * (dx = (dy W) * GELU'(e0)).  e0 / y2 share the row stride of y (dx).  flags select the family: 0 fp32 SIMT;
+ * TE_FLAG_LINEAR_TENSOR_CORES 3xTF32; + TE_FLAG_LINEAR_F16_SPLIT (forward) fp16 split; + TE_FLAG_BACKWARD_TF32 / TE_FLAG_BACKWARD_F16
+ * (backward) single-pass TF32 / fp16.  scratch as for te_linear_forward_ex / te_linear_backward_ex. */
+TE_API int te_linear_forward_epi(const float* x, const float* w, const float* bias, const float* e0, float* y, float* y2,
+                                 float* scratch, int rows, int in_features, int out_features, int epi, unsigned flags,
+                                 void* stream);
+TE_API int te_linear_backward_epi(const float* dy, const float* w, const float* e0, float* dx, float* scratch, int rows,
+                                  int in_features, int out_features, int epi, unsigned flags, void* stream);
+/* LayerNorm over the last dimension of x [rows, D] (D % 4 == 0) that also emits the fp16-split operand of y in the format of
+ * te_f16_block_split: y [rows, D], mean / rstd [rows] (each may be NULL), hi, lo fp16 [rows, D] with lo == hi + rows*D,
+ * scale_inv [rows, ceil(D / 128)]. */
+TE_API int te_layernorm_split(const float* x, const float* w, const float* b, float* y, float* mean, float* rstd, void* hi,
+                              void* lo, float* scale_inv, int rows, int D, float eps, void* stream);
+/* S = safe_divide(r, Z) of the z+ Linear rule on the single-pass tensor-core S kernel, Z formed from the saved forward output
+ * y = x W^T + bias [rows, out] (bias may be NULL).  Either s (S TF32-rounded, fp32 [rows, out]) or s16 + s16_scale (S as
+ * hi-only block-scaled fp16 [rows, out], scale_inv [rows, out / 128] chosen as in te_f16_block_split: the operand of the fp16
+ * second contraction, TE_FLAG_ZPLUS_R_F16).  flags: 0 or TE_FLAG_ZPLUS_S1_BF16.  in, out multiples of 128.
+ * scratch: 16*in*out + rows*in floats. */
+TE_API int te_tc_zplus_s(const float* x, const float* w, const float* bias, const float* y, const float* r, float* s, void* s16,
+                         float* s16_scale, float* scratch, int rows, int in_features, int out_features, unsigned flags,
+                         void* stream);
+/* Attention-shaped N x N contraction on head slices of packed activations:
+ * out[b,h,i,j] = epi(alpha * sum_d A[b*n+i, h*dh+d] B[b*n+j, h*dh+d]), out / E [batch, heads, n, ld_out].
+ * epi: 0 STORE, 1 MUL (* E), 2 SD (safe_divide(E, .)), 3 SOFTMAX (over j; n <= 256).  Columns n .. round_up(n,4)-1 are written as
+ * zeros; the columns from round_up(n,4) to ld_out are not touched.  dh in {32, 64}; single_pass (STORE / MUL): one TF32 MMA per
+ * k-step instead of the 3xTF32 split. */
+TE_API int te_tc_attention_nn(const float* A, long long lda, const float* B, long long ldb, int batch, int heads, int n, int dh,
+                              float* out, int ld_out, const float* E, float alpha, int epi, int single_pass, void* stream);
+/* Attention-shaped N x 64 contraction reduced over tokens: out[b*n+m, h*64+d] = epi(alpha * sum_k M_h[m,k] X[b*n+k, h*64+d]) with
+ * M_h = map[b,h] (amn 0) or its transpose (amn 1); map [batch, heads, n, np] (np % 4 == 0, np >= n; its padding columns are
+ * never read), X / out / E packed rows of stride ldx / ld_out.  epi: 0 STORE, 1 MUL (* E). */
+TE_API int te_tc_attention_nk(const float* map, int np, int amn, const float* X, long long ldx, int batch, int heads, int n,
+                              float* out, int ld_out, const float* E, float alpha, int epi, int single_pass, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -333,3 +333,204 @@ def test_f16_block_split_format_bit_exact():
     ok = np.ones_like(rh, dtype=bool)
     ok[9, :128] = False                                          # lo of the non-finite block is inf - inf = NaN (payload unspecified)
     assert np.array_equal(lo.cpu().numpy().view(np.uint16)[ok], rl.view(np.uint16)[ok])
+
+
+# ---- fused Linear epilogues of every kernel family (te_linear_forward_epi / te_linear_backward_epi: no fall-back) -----------
+# Bounds per element, relative to the element's own scale |x||W|^T (+ |bias|): fp32 SIMT 3e-6 (test_tc_3xtf32_linear_is_fp32_grade),
+# 3xTF32 and the fp16 split 1.5e-8 * K + 2e-6 (same test; the fp16 split keeps the 3xTF32 operand precision), single-pass
+# TF32 / fp16 2e-3 (test_tc_persistent_pair_kernels).
+LIN_BOUND = {"simt": lambda K: 3e-6, "3xtf32": lambda K: 1.5e-8 * K + 2e-6, "f16_split": lambda K: 1.5e-8 * K + 2e-6,
+             "tf32": lambda K: 2e-3, "f16": lambda K: 2e-3}
+# GELU'(x) = Phi(x) + x phi(x) in the epilogue, absolute error: the erff / expf form (every family but single-pass TF32) to a
+# few fp32 ulp of values <= 1.13; te_gelu_grad_fast (single-pass TF32 backward) has erf by Abramowitz-Stegun 7.1.26 (1.5e-7
+# absolute, so 7.5e-8 on Phi) with ex2.approx / rcp.approx operands.  Measured maxima over e0 in [-12, 12] on one H100 80GB HBM3
+# at a 400 W power limit: 1.9e-7 (SIMT, 3xTF32, single-pass fp16), 3.2e-7 (te_gelu_grad_fast).  Measured per-element GEMM errors:
+# forward y 4.3e-7 (SIMT), 6.1e-7 (3xTF32), 4.7e-7 (fp16 split); GELU_BWD at most 0.19 of its bound in every family.
+GELU_GRAD_EXACT = 3e-7
+GELU_GRAD_FAST = 6e-7
+
+
+def _gelu64(y):
+    return 0.5 * y * (1 + torch.erf(y / 2 ** 0.5))
+
+
+def _gelu_grad64(x):
+    return 0.5 * (1 + torch.erf(x / 2 ** 0.5)) + x * torch.exp(-0.5 * x * x) / (2 * torch.pi) ** 0.5
+
+
+def _e0_grid(rows, cols, g):
+    """GELU inputs over [-12, 12]: uniform, plus 0, +-1e-6, +-1 and the tails, where the erf approximation is weakest"""
+    e0 = torch.rand(rows, cols, generator=g, device="cuda") * 24 - 12
+    special = torch.tensor([0.0, 1e-6, -1e-6, 1.0, -1.0, 0.5, -0.5, 3.0, -3.0, 6.0, -6.0, 12.0, -12.0], device="cuda")
+    flat = e0.view(-1)
+    flat[:special.numel() * (flat.numel() // (4 * special.numel()))] = special.repeat(flat.numel() // (4 * special.numel()))
+    return e0
+
+
+@pytest.mark.parametrize("K", [64, 768, 3072])
+@pytest.mark.parametrize("rows", [1, 77, 591, 20000])
+def test_linear_forward_epilogues(rows, K):
+    """BIAS_GELU (y, y2 = erf-GELU(y)) and BIAS_ADD (y, y2 = e0 + y) on fp32 SIMT, 3xTF32 and the fp16 split against fp64.
+    Rows span six decades of magnitude (the fp16 split scales every 128-column block on its own)."""
+    from transformer_explainability_b200 import ops
+    N = 256
+    g = torch.Generator(device="cuda").manual_seed(rows * 3 + K)
+    x = torch.randn(rows, K, generator=g, device="cuda") * torch.logspace(-3, 3, rows, device="cuda")[:, None]
+    w = torch.randn(N, K, generator=g, device="cuda") * 0.05
+    b = torch.randn(N, generator=g, device="cuda") * 0.1
+    e0 = torch.randn(rows, N, generator=g, device="cuda")
+    y64 = x.double() @ w.double().T + b.double()
+    scale = x.double().abs() @ w.double().abs().T + b.double().abs()
+    for family in ("simt", "3xtf32", "f16_split"):
+        bound = LIN_BOUND[family](K)
+        for epi in ("bias_gelu", "bias_add"):
+            y, y2 = ops.linear_forward_epi(x, w, b, e0 if epi == "bias_add" else None, epi=epi, family=family)
+            torch.cuda.synchronize()
+            ey = ((y.double() - y64).abs() / scale).max().item()
+            if epi == "bias_gelu":      # |GELU'| <= 1.13, plus the fp32 GELU itself
+                e2 = ((y2.double() - _gelu64(y64)).abs() / (1.13 * scale)).max().item()
+                b2 = bound + 5e-7
+            else:                       # e0 + y in fp32: one rounding of |e0| + |y|
+                e2 = ((y2.double() - (e0.double() + y64)).abs() / (scale + e0.double().abs())).max().item()
+                b2 = bound + 1.2e-7
+            print("linear fwd %s %s rows %d K %d: y %.2e y2 %.2e (per element; bound %.1e)" % (family, epi, rows, K, ey, e2, bound))
+            assert ey < bound and e2 < b2, (family, epi)
+
+
+@pytest.mark.parametrize("K", [64, 768, 3072])
+@pytest.mark.parametrize("rows", [1, 77, 591, 20000])
+def test_linear_backward_gelu_epilogue(rows, K):
+    """GELU_BWD, dx = (dy W) * GELU'(e0), on fp32 SIMT, 3xTF32, single-pass TF32 (te_gelu_grad_fast) and single-pass fp16
+    against fp64, e0 over [-12, 12] with 0, +-1e-6 and the tails.  The GEMM part keeps the family's bound per element; the
+    gradient itself is isolated by dividing by the same family's STORE result (the same accumulation, so the quotient is
+    GELU'(e0) up to one fp32 rounding) and held to GELU_GRAD_FAST / GELU_GRAD_EXACT absolute — the exact families no worse
+    than SIMT."""
+    from transformer_explainability_b200 import ops
+    N = 256
+    g = torch.Generator(device="cuda").manual_seed(rows * 5 + K)
+    dy = torch.randn(rows, K, generator=g, device="cuda")
+    w = torch.randn(K, N, generator=g, device="cuda") * 0.05
+    e0 = _e0_grid(rows, N, g)
+    gp = _gelu_grad64(e0.double())
+    v64 = dy.double() @ w.double()
+    scale = dy.double().abs() @ w.double().abs()
+    grad_err = {}
+    for family in ("simt", "3xtf32", "tf32", "f16"):
+        bound = LIN_BOUND[family](K)
+        gb = GELU_GRAD_FAST if family == "tf32" else GELU_GRAD_EXACT
+        dx = ops.linear_backward_epi(dy, w, e0, epi="gelu_bwd", family=family)
+        v = ops.linear_backward_epi(dy, w, None, epi="store", family=family)
+        torch.cuda.synchronize()
+        e_full = ((dx.double() - v64 * gp).abs() / (scale * ((bound + 1.2e-7) * gp.abs() + gb))).max().item()
+        live = v != 0
+        ratio = dx.double()[live] / v.double()[live]
+        grad_err[family] = (ratio - gp[live]).abs().max().item()
+        print("linear bwd GELU_BWD %s rows %d K %d: %.2f of the bound (per element), GELU' abs err %.2e" % (
+            family, rows, K, e_full, grad_err[family]))
+        assert e_full < 1, family
+        assert grad_err[family] < gb + 6e-8 * 1.13, family
+    for family in ("3xtf32", "f16"):
+        assert grad_err[family] <= grad_err["simt"] + 1.2e-7, "%s: GELU' worse than the SIMT epilogue" % family
+
+
+def test_linear_epilogue_entry_points_do_not_fall_back():
+    """A family that does not take the shape / epilogue is TE_ERR_UNSUPPORTED, never a silent fall-back: width 64 (BERT-tiny)
+    for every tensor-core family, K % 64 != 0 for the fp16 ones."""
+    from transformer_explainability_b200 import _lib, ops
+    x = torch.randn(10, 96, device="cuda")
+    for fam in ("3xtf32", "f16_split"):
+        with pytest.raises(_lib.TeError) as ex:
+            ops.linear_forward_epi(x, torch.randn(64, 96, device="cuda"), None, epi="store", family=fam)
+        assert ex.value.status == _lib.TE_ERR_UNSUPPORTED
+    with pytest.raises(_lib.TeError) as ex:
+        ops.linear_forward_epi(x, torch.randn(128, 96, device="cuda"), None, epi="store", family="f16_split")   # K = 96
+    assert ex.value.status == _lib.TE_ERR_UNSUPPORTED
+    dy = torch.randn(10, 96, device="cuda")
+    for fam in ("3xtf32", "tf32", "f16"):
+        with pytest.raises(_lib.TeError) as ex:
+            ops.linear_backward_epi(dy, torch.randn(96, 64, device="cuda"), None, epi="store", family=fam)
+        assert ex.value.status == _lib.TE_ERR_UNSUPPORTED
+    with pytest.raises(_lib.TeError) as ex:
+        ops.linear_backward_epi(dy, torch.randn(96, 128, device="cuda"), None, epi="store", family="f16")      # K = 96
+    assert ex.value.status == _lib.TE_ERR_UNSUPPORTED
+    y, _ = ops.linear_forward_epi(x, torch.randn(64, 96, device="cuda"), None, epi="store", family="simt")
+    assert torch.isfinite(y).all()
+
+
+# ---- the other producers of the fp16-split operand format ----------------------------------------------------------------
+@pytest.mark.parametrize("D", [768, 1024, 64])
+def test_layernorm_split_format_bit_exact(D):
+    """te_launch_layernorm_split (feeds every qkv / fc1 GEMM under TE_FLAG_LINEAR_F16_SPLIT): y against fp64 LayerNorm,
+    mean / rstd against fp64, and hi, lo and the block scales BIT-identical to oracle/f16_split.split_rows applied to the
+    kernel's own y.  Stress data as in test_f16_block_split_format_bit_exact: y spans 60 decades (through the LayerNorm
+    weight), one row of x is constant (y = bias = 0: a zero row).  The y error is measured against (|x| + |mean|) rstd |w|,
+    the scale the fp32 subtraction x - mean works at."""
+    import numpy as np
+    from oracle import f16_split as F
+    from transformer_explainability_b200 import ops
+    g = torch.Generator().manual_seed(D)
+    rows, eps = 300, 1e-6
+    x = torch.randn(rows, D, generator=g) * torch.logspace(-3, 1, D) + torch.randn(rows, 1, generator=g)
+    x[7] = 0.0                                                              # constant row: y == bias
+    w = (torch.randn(D, generator=g) * torch.logspace(-30, 30, D)).float()  # y spans 60 decades inside every row
+    b = torch.zeros(D)
+    y, mean, rstd, hi, lo, si = ops.layernorm_split(x.cuda(), w.cuda(), b.cuda(), eps)
+    torch.cuda.synchronize()
+    xd = x.double()
+    m64 = xd.mean(1, keepdim=True)
+    r64 = 1 / torch.sqrt(((xd - m64) ** 2).mean(1, keepdim=True) + eps)
+    y64 = (xd - m64) * r64 * w.double() + b.double()
+    ey = ((y.double().cpu() - y64).abs() / ((xd.abs() + m64.abs()) * r64 * w.double().abs() + 1e-300)).max().item()
+    print("layernorm split D %d: y per element %.2e" % (D, ey))
+    assert ey < 1e-5
+    assert (y[7] == 0).all()
+    rh, rl, rs = F.split_rows(y.cpu().numpy())
+    assert np.array_equal(si.cpu().numpy(), rs)
+    assert np.array_equal(hi.cpu().numpy().view(np.uint16), rh.view(np.uint16))
+    assert np.array_equal(lo.cpu().numpy().view(np.uint16), rl.view(np.uint16))
+    assert (si.cpu()[7] == 1).all() and (hi.cpu()[7] == 0).all()
+
+
+@pytest.mark.parametrize("rows,inf,outf", [(77, 768, 2304), (591, 768, 768), (300, 3072, 768)])
+def test_zplus_s1_f16_output(rows, inf, outf):
+    """te_tc_zplus_s1 with S leaving as hi-only block-scaled fp16 (ZO_F16S, the A operand of te_tc_zplus_r16), against the fp32
+    form of the same kernel on the same inputs.  The fp32 form is tf32(S) while the fp16 form scales the unrounded S, so they
+    are not compared bit for bit.  Instead: every block scale equals the one oracle/f16_split picks from the fp32 form's block
+    maximum, except where tf32 rounding lifted that maximum onto a power of two (counted: rare); hi decodes, per element, to the
+    fp32 form within half an fp16 ulp plus the 2^-11 of its tf32 rounding; the fp32 form is the z+ rule's S to the TF32 bound
+    (3e-3) against fp64; a zero row of R gives zero hi and the neutral scale; the scale array holds N / 128 columns per row,
+    the row stride te_tc_zplus_r16 reads it with."""
+    import numpy as np
+    from oracle import f16_split as F
+    from transformer_explainability_b200 import ops
+    g = torch.Generator(device="cuda").manual_seed(rows + inf)
+    x = torch.randn(rows, inf, generator=g, device="cuda")
+    w = torch.randn(outf, inf, generator=g, device="cuda") * 0.05
+    b = torch.randn(outf, generator=g, device="cuda") * 0.1
+    r = torch.rand(rows, outf, generator=g, device="cuda") * torch.logspace(-6, 6, rows, device="cuda")[:, None]
+    r[rows // 3] = 0.0
+    y = ops.linear_forward(x, w, b)
+    s32 = ops.tc_zplus_s(x, w, r, y, bias=b)
+    s16, sc = ops.tc_zplus_s(x, w, r, y, bias=b, f16=True)
+    torch.cuda.synchronize()
+    assert sc.shape == (rows, outf // 128) and torch.isfinite(sc).all(), "a block scale was not written"
+    z64 = x.double().clamp(min=0) @ w.double().clamp(min=0).T + x.double().clamp(max=0) @ w.double().clamp(max=0).T
+    s64 = rules.safe_divide(r.double(), z64)
+    es = ((s32.double() - s64).abs() / s64.abs().clamp_min(1e-300)).max().item()
+    m = s32.abs().view(rows, outf // 128, 128).amax(-1).cpu().numpy()
+    _, want = F.block_scale(m)
+    got = sc.cpu().numpy()
+    on_pow2 = (m > 0) & (np.frexp(m)[0] == 0.5)
+    mismatch = got != want
+    print("zplus S fp16 rows %d in %d out %d: fp32 S vs fp64 %.1e, %d of %d block maxima on a power of two, %d scale mismatches" % (
+        rows, inf, outf, es, on_pow2.sum(), m.size, mismatch.sum()))
+    assert es < 3e-3
+    assert not (mismatch & ~on_pow2).any(), "a block scale differs from the one the format prescribes"
+    assert (got[mismatch] == 0.5 * want[mismatch]).all()                # the unrounded maximum sat just below 2^k
+    assert on_pow2.sum() <= max(2, m.size // 100), "the exemption must stay rare"
+    sc64 = sc.double()[..., None]
+    hi = s16.double().view(rows, outf // 128, 128) * sc64
+    s32b = s32.double().view(rows, outf // 128, 128)
+    # fp16 spacing in [2^14, 2^15) is 16: half an ulp of the block maximum is 8 * 2^-e
+    assert ((hi - s32b).abs() <= 8 * sc64 + 2.0 ** -11 * s32b.abs()).all(), "decoded hi off by more than half an fp16 ulp"
+    assert (s16[rows // 3] == 0).all() and (sc[rows // 3] == 1).all()

@@ -6,6 +6,8 @@
 (``engine.BertEngine``) for a batch of independent sequences.  ``config`` is a ``transformers.BertConfig`` or any
 object with the same attribute names.  No ``param.grad`` side effect, no autograd graph.
 """
+import weakref
+
 import torch
 import torch.nn as nn
 
@@ -23,14 +25,25 @@ class _SelfAttention(nn.Module):
         self._layer = -1
 
     # accessors of BERT.py:281-297, served from the engine workspace
+    def _t(self, name):
+        owner = self._owner() if self._owner is not None else None
+        if owner is None:
+            raise RuntimeError("this attention view's model no longer exists")
+        return owner._engine_tensor(name, self._layer)
+
     def get_attn(self):
-        return self._owner[0]._engine_tensor("attn", self._layer)
+        return self._t("attn")
 
     def get_attn_cam(self):
-        return self._owner[0]._engine_tensor("attn_cam", self._layer)
+        return self._t("attn_cam")
 
     def get_attn_gradients(self):
-        return self._owner[0]._engine_tensor("attn_grad", self._layer)
+        return self._t("attn_grad")
+
+    def __getstate__(self):                    # the back-reference is re-made by the owning model's __setstate__
+        state = self.__dict__.copy()
+        state["_owner"] = None
+        return state
 
 
 class _DenseLN(nn.Module):
@@ -95,9 +108,7 @@ class BertForSequenceClassification(nn.Module):
         self.num_labels = config.num_labels
         self.bert = _BertModel(config)
         self.classifier = nn.Linear(config.hidden_size, config.num_labels)
-        for i, l in enumerate(self.bert.encoder.layer):
-            l.attention.self._owner = (self,)
-            l.attention.self._layer = i
+        self._link_views()
         self._cfg = bert_config(config.vocab_size, config.max_position_embeddings, config.type_vocab_size,
                                 config.hidden_size, config.num_hidden_layers, config.num_attention_heads,
                                 config.intermediate_size, config.num_labels, config.layer_norm_eps)
@@ -110,6 +121,17 @@ class BertForSequenceClassification(nn.Module):
                 nn.init.normal_(m.weight, mean=0.0, std=std)
             if isinstance(m, nn.Linear) and m.bias is not None:
                 nn.init.zeros_(m.bias)
+
+    def _link_views(self):
+        # a weak back-reference: a strong one would make model <-> view a reference cycle, so a dropped model and its
+        # engine's device memory would live on until Python's cyclic garbage collector happened to run
+        for i, l in enumerate(self.bert.encoder.layer):
+            l.attention.self._owner = weakref.ref(self)
+            l.attention.self._layer = i
+
+    def __setstate__(self, state):             # pickle / copy.deepcopy: the views answer for the new model
+        super().__setstate__(state)
+        self._link_views()
 
     def _version(self):
         return tuple(p._version for p in self.parameters()) + (str(self.classifier.weight.device),)

@@ -105,6 +105,12 @@ PROTOTYPES = {
     "te_linear_forward_ex": (c_int, [_P, _P, _P, _P, _P, c_int, c_int, c_int, c_uint, _P]),
     "te_linear_backward_ex": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_uint, _P]),
     "te_f16_block_split": (c_int, [_P, c_int, c_int, _P, _P, _P, _P]),
+    "te_linear_forward_epi": (c_int, [_P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_uint, _P]),
+    "te_linear_backward_epi": (c_int, [_P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_uint, _P]),
+    "te_layernorm_split": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_float, _P]),
+    "te_tc_zplus_s": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_uint, _P]),
+    "te_tc_attention_nn": (c_int, [_P, c_ll, _P, c_ll, c_int, c_int, c_int, c_int, _P, c_int, _P, c_float, c_int, c_int, _P]),
+    "te_tc_attention_nk": (c_int, [_P, c_int, c_int, _P, c_ll, c_int, c_int, c_int, _P, c_int, _P, c_float, c_int, c_int, _P]),
 }
 
 _lib = None
@@ -133,14 +139,20 @@ def load():
     return lib
 
 
+TE_ERR_UNSUPPORTED = -4
+
+
 class TeError(RuntimeError):
-    pass
+    """A negative status of the C library; ``status`` holds it (TE_ERR_*)."""
+    def __init__(self, msg, status=None):
+        super().__init__(msg)
+        self.status = status
 
 
 def check(status, what=""):
     if status < 0:
         msg = load().te_last_error()
-        raise TeError("%s failed (%d): %s" % (what or "te_b200 call", status, msg.decode() if msg else ""))
+        raise TeError("%s failed (%d): %s" % (what or "te_b200 call", status, msg.decode() if msg else ""), status)
     return status
 
 

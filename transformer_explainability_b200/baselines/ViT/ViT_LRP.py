@@ -11,6 +11,8 @@ side effect (documented deviation, SURVEY.md §8b).
 ``deit_base_distilled_patch16_224`` (198 tokens, dist token + second head) is an extension that the
 reference does not contain (SURVEY.md §7f).
 """
+import weakref
+
 import torch
 import torch.nn as nn
 
@@ -41,9 +43,20 @@ class _AttentionView(nn.Module):
         self._layer = -1
 
     def _t(self, name):
-        return self._owner[0]._engine_tensor(name, self._layer)
+        owner = self._owner() if self._owner is not None else None
+        if owner is None:
+            raise RuntimeError("this attention view's model no longer exists")
+        return owner._engine_tensor(name, self._layer)
+
+    def __getstate__(self):                    # the back-reference is re-made by the owning model's __setstate__
+        state = self.__dict__.copy()
+        state["_owner"] = None
+        return state
 
     def get_attn(self):
+        return self._t("attn")
+
+    def get_attention_map(self):               # ViT_new.py's name for the same probabilities
         return self._t("attn")
 
     def get_attn_cam(self):
@@ -112,9 +125,7 @@ class VisionTransformer(nn.Module):
         self.head = nn.Linear(embed_dim, num_classes)
         if distilled:
             self.head_dist = nn.Linear(embed_dim, num_classes)
-        for i, blk in enumerate(self.blocks):
-            blk.attn._owner = (self,)          # tuple: keep the back-reference out of the module tree
-            blk.attn._layer = i
+        self._link_views()
         self._cfg = vit_config(img_size, patch_size, in_chans, num_classes, embed_dim, depth, num_heads, mlp_ratio,
                                distilled, self.blocks[0].norm1.eps, self.norm.eps)
         self._engine = None
@@ -122,6 +133,18 @@ class VisionTransformer(nn.Module):
         self.engine_flags = 0
         self._rule_flags = 0                   # ViT_orig_LRP sets TE_FLAG_RULES_LRP (the modules/layers_lrp.py rule library)
         self._init_weights()
+
+    def _link_views(self):
+        # a weak back-reference, kept out of the module tree: a strong one would make model <-> view a reference cycle,
+        # so a dropped model and its engine's device memory (weights, derived copies, workspace) would live on until
+        # Python's cyclic garbage collector happened to run
+        for i, blk in enumerate(self.blocks):
+            blk.attn._owner = weakref.ref(self)
+            blk.attn._layer = i
+
+    def __setstate__(self, state):             # pickle / copy.deepcopy: the views answer for the new model
+        super().__setstate__(state)
+        self._link_views()
 
     def _init_weights(self):
         # reference init (ViT_LRP.py:276-299): trunc_normal(.02) for Linear / pos / cls, LayerNorm 1/0

@@ -21,8 +21,6 @@ class VisionTransformer(_lrp.VisionTransformer):
         super().__init__(img_size=img_size, patch_size=patch_size, in_chans=in_chans, num_classes=num_classes,
                          embed_dim=embed_dim, depth=depth, num_heads=num_heads, mlp_ratio=mlp_ratio, qkv_bias=qkv_bias,
                          norm_eps=eps)
-        for blk in self.blocks:
-            blk.attn.get_attention_map = blk.attn.get_attn
 
     def forward(self, x, register_hook=False):
         return super().forward(x)

@@ -40,20 +40,127 @@ extern "C" int te_linear_forward(const float* x, const float* w, const float* bi
     return te_gemm_launch(p, TE_L_K, TE_L_K, TE_XF_NONE, TE_EPI_BIAS, ST(stream));
 }
 
-extern "C" int te_linear_forward_ex(const float* x, const float* w, const float* bias, float* y, float* scratch, int rows,
-                                    int in_features, int out_features, unsigned flags, void* stream) {
-    REQ(x && w && y && rows > 0 && in_features > 0 && out_features > 0, "te_linear_forward_ex: bad argument");
-    // every tensor-core path takes the shapes of the 3xTF32 kernel; the derived copies are made only when one is taken
+// forward Linear with the kernel family the flags select.  strict: a tensor-core family that does not take the shape is an
+// error; otherwise every tensor-core path takes the shapes of the 3xTF32 kernel and the derived copies are made only when one is
+// taken.  Scratch layout with TE_FLAG_LINEAR_F16_SPLIT as well:
+// [16*in*out derived | round_up(rows*in,64) fp16 hi,lo split of x | rows*ceil(in/128) block scales]
+static int linear_forward_flags(const float* x, const float* w, const float* bias, const float* e0, float* y, float* y2,
+                                float* scratch, int rows, int in_features, int out_features, int epi, unsigned flags,
+                                bool strict, cudaStream_t st) {
     const bool tc = (flags & TE_FLAG_LINEAR_TENSOR_CORES) && scratch &&
-                    te_tc_gemm3x_supported(rows, in_features, out_features, in_features);
-    if (tc) TE_TRY(te_tc_prepare_weights(w, scratch, in_features, out_features, ST(stream)));
-    // scratch layout with TE_FLAG_LINEAR_F16_SPLIT as well:
-    // [16*in*out derived | round_up(rows*in,64) fp16 hi,lo split of x | rows*ceil(in/128) block scales]
+                    (strict || te_tc_gemm3x_supported(rows, in_features, out_features, in_features));
+    if (tc) TE_TRY(te_tc_prepare_weights(w, scratch, in_features, out_features, st));
     float* split = (tc && (flags & TE_FLAG_LINEAR_F16_SPLIT)) ? scratch + te_tc_derived_floats(in_features, out_features) : nullptr;
     const te_util::F16Split fs = {split, split ? split + (((long long)rows * in_features + 63) & ~63LL) : nullptr, false, nullptr,
                                   nullptr};
-    return te_util::linear_fwd_tc(tc ? scratch : nullptr, x, in_features, w, bias, y, nullptr, nullptr, rows, in_features,
-                                  out_features, TE_EPI_BIAS, ST(stream), &fs);
+    return te_util::linear_fwd_tc(tc ? scratch : nullptr, x, in_features, w, bias, y, y2, e0, rows, in_features, out_features,
+                                  epi, st, &fs, strict);
+}
+
+// activation-gradient backward Linear, same selection.  Scratch layout with TE_FLAG_BACKWARD_F16:
+// [16*in*out derived | round_up(rows*out/2,64) fp16 dy | rows*ceil(out/128) block scales]
+static int linear_backward_flags(const float* dy, const float* w, const float* e0, float* dx, float* scratch, int rows,
+                                 int in_features, int out_features, int epi, unsigned flags, bool strict, cudaStream_t st) {
+    const bool tc = (flags & TE_FLAG_LINEAR_TENSOR_CORES) && scratch &&
+                    (strict || te_tc_gemm3x_supported(rows, out_features, in_features, out_features));
+    if (tc) TE_TRY(te_tc_prepare_weights(w, scratch, in_features, out_features, st));
+    float* split = (tc && (flags & TE_FLAG_BACKWARD_F16)) ? scratch + te_tc_derived_floats(in_features, out_features) : nullptr;
+    const te_util::F16Split fs = {split, split ? split + (((long long)rows * out_features / 2 + 63) & ~63LL) : nullptr, false,
+                                  nullptr, nullptr};
+    return te_util::linear_bwd_tc(tc ? scratch : nullptr, dy, w, dx, e0, rows, in_features, out_features, epi, st,
+                                  (flags & TE_FLAG_BACKWARD_TF32) != 0, &fs, strict);
+}
+
+extern "C" int te_linear_forward_ex(const float* x, const float* w, const float* bias, float* y, float* scratch, int rows,
+                                    int in_features, int out_features, unsigned flags, void* stream) {
+    REQ(x && w && y && rows > 0 && in_features > 0 && out_features > 0, "te_linear_forward_ex: bad argument");
+    return linear_forward_flags(x, w, bias, nullptr, y, nullptr, scratch, rows, in_features, out_features, TE_EPI_BIAS, flags,
+                                false, ST(stream));
+}
+
+extern "C" int te_linear_forward_epi(const float* x, const float* w, const float* bias, const float* e0, float* y, float* y2,
+                                     float* scratch, int rows, int in_features, int out_features, int epi, unsigned flags,
+                                     void* stream) {
+    REQ(x && w && y && rows > 0 && in_features > 0 && out_features > 0, "te_linear_forward_epi: bad argument");
+    REQ(epi >= TE_EPI_STORE && epi <= TE_EPI_BIAS_ADD, "te_linear_forward_epi: epilogue must be STORE, BIAS, BIAS_GELU or BIAS_ADD");
+    REQ(y2 || (epi != TE_EPI_BIAS_GELU && epi != TE_EPI_BIAS_ADD), "te_linear_forward_epi: BIAS_GELU / BIAS_ADD need y2");
+    REQ(e0 || epi != TE_EPI_BIAS_ADD, "te_linear_forward_epi: BIAS_ADD needs e0");
+    REQ(!(flags & ~(TE_FLAG_LINEAR_TENSOR_CORES | TE_FLAG_LINEAR_F16_SPLIT)), "te_linear_forward_epi: unknown family flags");
+    REQ(!(flags & TE_FLAG_LINEAR_F16_SPLIT) || (flags & TE_FLAG_LINEAR_TENSOR_CORES),
+        "te_linear_forward_epi: TE_FLAG_LINEAR_F16_SPLIT needs TE_FLAG_LINEAR_TENSOR_CORES");
+    REQ(scratch || !(flags & TE_FLAG_LINEAR_TENSOR_CORES), "te_linear_forward_epi: the tensor-core families need scratch");
+    return linear_forward_flags(x, w, bias, e0, y, y2, scratch, rows, in_features, out_features, epi, flags, true, ST(stream));
+}
+
+extern "C" int te_linear_backward_epi(const float* dy, const float* w, const float* e0, float* dx, float* scratch, int rows,
+                                      int in_features, int out_features, int epi, unsigned flags, void* stream) {
+    REQ(dy && w && dx && rows > 0 && in_features > 0 && out_features > 0, "te_linear_backward_epi: bad argument");
+    REQ(epi == TE_EPI_STORE || epi == TE_EPI_GELU_BWD, "te_linear_backward_epi: epilogue must be STORE or GELU_BWD");
+    REQ(e0 || epi != TE_EPI_GELU_BWD, "te_linear_backward_epi: GELU_BWD needs e0");
+    REQ(!(flags & ~(TE_FLAG_LINEAR_TENSOR_CORES | TE_FLAG_BACKWARD_TF32 | TE_FLAG_BACKWARD_F16)),
+        "te_linear_backward_epi: unknown family flags");
+    REQ(!(flags & (TE_FLAG_BACKWARD_TF32 | TE_FLAG_BACKWARD_F16)) || (flags & TE_FLAG_LINEAR_TENSOR_CORES),
+        "te_linear_backward_epi: the single-pass families need TE_FLAG_LINEAR_TENSOR_CORES");
+    REQ(scratch || !(flags & TE_FLAG_LINEAR_TENSOR_CORES), "te_linear_backward_epi: the tensor-core families need scratch");
+    return linear_backward_flags(dy, w, e0, dx, scratch, rows, in_features, out_features, epi, flags, true, ST(stream));
+}
+
+extern "C" int te_layernorm_split(const float* x, const float* w, const float* b, float* y, float* mean, float* rstd, void* hi,
+                                  void* lo, float* scale_inv, int rows, int D, float eps, void* stream) {
+    REQ(x && w && b && y && hi && lo && scale_inv && rows > 0 && D > 0 && D % 4 == 0, "te_layernorm_split: bad argument");
+    REQ(reinterpret_cast<char*>(lo) == reinterpret_cast<char*>(hi) + (long long)rows * D * 2,
+        "te_layernorm_split: lo must follow hi ([hi | lo] in one buffer, as the kernels lay the split out)");
+    return te_launch_layernorm_split(x, w, b, y, mean, rstd, rows, D, eps, reinterpret_cast<float*>(hi), scale_inv, ST(stream));
+}
+
+static bool al16(const void* p) { return ((uintptr_t)p & 15u) == 0; }
+
+extern "C" int te_tc_zplus_s(const float* x, const float* w, const float* bias, const float* y, const float* r, float* s,
+                             void* s16, float* s16_scale, float* scratch, int rows, int in_features, int out_features,
+                             unsigned flags, void* stream) {
+    REQ(x && w && y && r && scratch && rows > 0 && in_features > 0 && out_features > 0, "te_tc_zplus_s: bad argument");
+    REQ((s != nullptr) != (s16 != nullptr) && (!s16 || s16_scale), "te_tc_zplus_s: give either s or s16 + s16_scale");
+    REQ(!(flags & ~TE_FLAG_ZPLUS_S1_BF16), "te_tc_zplus_s: only TE_FLAG_ZPLUS_S1_BF16 selects a variant");
+    if (!te_tc_zplus_supported(rows, in_features, out_features, in_features))
+        return te_util::no_fallback("te_tc_zplus_s: the tensor-core S kernel needs in / out multiples of 128");
+    REQ(al16(x) && al16(y) && al16(r) && al16(scratch) && (!bias || al16(bias)) && (!s || al16(s)) && (!s16 || al16(s16)),
+        "te_tc_zplus_s: operands must be 16-byte aligned");
+    cudaStream_t st = ST(stream);
+    // scratch: [16*in*out derived weight copies | rows*in for bf16(|x|)]
+    TE_TRY(te_tc_prepare_weights(w, scratch, in_features, out_features, st));
+    float* xabs = scratch + te_tc_derived_floats(in_features, out_features);
+    return te_tc_zplus_s1(x, in_features, xabs, scratch, r, out_features, y, out_features, bias, s, rows, in_features,
+                          out_features, st, (flags & TE_FLAG_ZPLUS_S1_BF16) != 0, reinterpret_cast<float*>(s16), s16_scale);
+}
+
+extern "C" int te_tc_attention_nn(const float* A, long long lda, const float* B, long long ldb, int batch, int heads, int n,
+                                  int dh, float* out, int ld_out, const float* E, float alpha, int epi, int single_pass,
+                                  void* stream) {
+    REQ(A && B && out && batch > 0 && heads > 0 && n > 0 && dh > 0, "te_tc_attention_nn: bad argument");
+    REQ(epi >= TE_TC_ATTN_STORE && epi <= TE_TC_ATTN_SOFTMAX, "te_tc_attention_nn: unknown epilogue");
+    REQ(E || epi == TE_TC_ATTN_STORE || epi == TE_TC_ATTN_SOFTMAX, "te_tc_attention_nn: MUL / SD need E");
+    if (!te_tc_attn_supported(n, dh, lda, ldb, ld_out))
+        return te_util::no_fallback("te_tc_attention_nn: the tensor-core kernel needs dh in {32, 64} and lda, ldb, ld_out multiples of 4");
+    if (epi == TE_TC_ATTN_SOFTMAX && n > 256)
+        return te_util::no_fallback("te_tc_attention_nn: the fused softmax needs every key in one tile (n <= 256)");
+    if (single_pass && (epi == TE_TC_ATTN_SD || epi == TE_TC_ATTN_SOFTMAX))
+        return te_util::no_fallback("te_tc_attention_nn: the single-pass kernel has the STORE / MUL epilogues only");
+    REQ(ld_out >= ((n + 3) & ~3) && lda >= (long long)heads * dh && ldb >= (long long)heads * dh,
+        "te_tc_attention_nn: ld_out < round_up(n, 4) or a row stride below heads * dh");
+    REQ(al16(A) && al16(B) && al16(out) && (!E || al16(E)), "te_tc_attention_nn: operands must be 16-byte aligned");
+    return te_tc_attn_nn(A, lda, B, ldb, batch, heads, n, dh, out, ld_out, E, alpha, epi, ST(stream), single_pass != 0);
+}
+
+extern "C" int te_tc_attention_nk(const float* map, int np, int amn, const float* X, long long ldx, int batch, int heads, int n,
+                                  float* out, int ld_out, const float* E, float alpha, int epi, int single_pass, void* stream) {
+    REQ(map && X && out && batch > 0 && heads > 0 && n > 0 && (amn == 0 || amn == 1), "te_tc_attention_nk: bad argument");
+    REQ(epi == TE_TC_ATTN_STORE || epi == TE_TC_ATTN_MUL, "te_tc_attention_nk: epilogue must be STORE or MUL");
+    REQ(E || epi == TE_TC_ATTN_STORE, "te_tc_attention_nk: MUL needs E");
+    if (!te_tc_attn_nk_supported(n, 64, np, ldx, ld_out))
+        return te_util::no_fallback("te_tc_attention_nk: the tensor-core kernel needs np, ldx, ld_out multiples of 4");
+    REQ(np >= n && ldx >= 64LL * heads && ld_out >= 64 * heads, "te_tc_attention_nk: np < n or a row stride below heads * 64");
+    REQ(al16(map) && al16(X) && al16(out) && (!E || al16(E)), "te_tc_attention_nk: operands must be 16-byte aligned");
+    return te_tc_attn_nk(map, np, amn, X, ldx, batch, heads, n, out, ld_out, E, alpha, epi, ST(stream), single_pass != 0);
 }
 
 extern "C" int te_f16_block_split(const float* x, int rows, int cols, void* hi, void* lo, float* scale_inv, void* stream) {
@@ -66,15 +173,8 @@ extern "C" int te_f16_block_split(const float* x, int rows, int cols, void* hi, 
 extern "C" int te_linear_backward_ex(const float* dy, const float* w, float* dx, float* scratch, int rows, int in_features,
                                      int out_features, unsigned flags, void* stream) {
     REQ(dy && w && dx && rows > 0 && in_features > 0 && out_features > 0, "te_linear_backward_ex: bad argument");
-    const bool tc = (flags & TE_FLAG_LINEAR_TENSOR_CORES) && scratch &&
-                    te_tc_gemm3x_supported(rows, out_features, in_features, out_features);
-    if (tc) TE_TRY(te_tc_prepare_weights(w, scratch, in_features, out_features, ST(stream)));
-    // scratch layout with TE_FLAG_BACKWARD_F16: [16*in*out derived | round_up(rows*out/2,64) fp16 dy | rows*ceil(out/128) block scales]
-    float* split = (tc && (flags & TE_FLAG_BACKWARD_F16)) ? scratch + te_tc_derived_floats(in_features, out_features) : nullptr;
-    const te_util::F16Split fs = {split, split ? split + (((long long)rows * out_features / 2 + 63) & ~63LL) : nullptr, false,
-                                  nullptr, nullptr};
-    return te_util::linear_bwd_tc(tc ? scratch : nullptr, dy, w, dx, nullptr, rows, in_features, out_features, TE_EPI_STORE,
-                                  ST(stream), (flags & TE_FLAG_BACKWARD_TF32) != 0, &fs);
+    return linear_backward_flags(dy, w, nullptr, dx, scratch, rows, in_features, out_features, TE_EPI_STORE, flags, false,
+                                 ST(stream));
 }
 
 extern "C" int te_linear_relprop(const float* x, const float* w, const float* r, float* out, float* scratch, int rows,

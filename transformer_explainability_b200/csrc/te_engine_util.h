@@ -46,6 +46,13 @@ static inline int linear_bwd(const float* dy, const float* w, float* dx, const f
     return te_gemm_launch(p, TE_L_K, TE_L_MN, TE_XF_NONE, epi, st);
 }
 
+// strict: a requested kernel family that does not take the shape / epilogue is an error (TE_ERR_UNSUPPORTED), not a fall-back to
+// the next family — what the diagnostic entry points te_linear_forward_epi / te_linear_backward_epi need
+static inline int no_fallback(const char* msg) {
+    te_set_last_error(msg);
+    return TE_ERR_UNSUPPORTED;
+}
+
 // tensor-core (3xTF32) variants when the derived weight copies are supplied and the shape qualifies
 // fp16-split forward Linear (TE_FLAG_LINEAR_F16_SPLIT, te_tc_wgmma.cu): where the block-scaled split of the input lives
 // (M*in floats + M*ceil(in/128) floats), whether its producer already filled it (ready: te_launch_layernorm_split or the previous
@@ -53,24 +60,32 @@ static inline int linear_bwd(const float* dy, const float* w, float* dx, const f
 struct F16Split { float* split; float* scale; bool ready; float* split_out; float* scale_out; };
 static inline int linear_fwd_tc(const float* dw, const float* x, int lda, const float* w, const float* bias, float* y,
                                 float* y2, const float* e0, long long M, int in, int out, int epi, cudaStream_t st,
-                                const F16Split* fs = nullptr) {
-    if (dw && fs && fs->split && epi != TE_EPI_GELU_BWD && te_tc_fwd16_supported(M, in, out, lda))
+                                const F16Split* fs = nullptr, bool strict = false) {
+    const bool f16 = dw && fs && fs->split;
+    if (f16 && epi != TE_EPI_GELU_BWD && te_tc_fwd16_supported(M, in, out, lda))
         return te_tc_linear_fwd16(fs->ready ? nullptr : x, lda, fs->split, fs->scale, dw, in, out, bias, y, y2, e0, M, epi, st,
                                   epi == TE_EPI_BIAS_GELU ? fs->split_out : nullptr, epi == TE_EPI_BIAS_GELU ? fs->scale_out : nullptr);
+    if (strict && f16) return no_fallback("linear forward: the fp16-split kernel does not take this shape / epilogue");
     if (dw && te_tc_gemm3x_supported(M, in, out, lda))
         return te_tc_linear_fwd(x, lda, dw, in, out, bias, y, y2, e0, M, epi, st);      // epilogue ids coincide
+    if (strict && dw) return no_fallback("linear forward: the 3xTF32 kernel does not take this shape");
     return linear_fwd(x, lda, w, bias, y, y2, e0, M, in, out, epi, st);
 }
 // tf32: single-pass TF32 wgmma kernel (TE_FLAG_BACKWARD_TF32) instead of the 3xTF32 split
 // fs: hi-only split scratch of dy (M*out/2 floats + M*ceil(out/128)) -> single-pass fp16 kernel (TE_FLAG_BACKWARD_F16)
 static inline int linear_bwd_tc(const float* dw, const float* dy, const float* w, float* dx, const float* e0, long long M,
-                                int in, int out, int epi, cudaStream_t st, bool tf32 = false, const F16Split* fs = nullptr) {
-    if (dw && fs && fs->split && (epi == TE_EPI_STORE || epi == TE_EPI_GELU_BWD) && te_tc_fwd16_supported(M, out, in, out))
+                                int in, int out, int epi, cudaStream_t st, bool tf32 = false, const F16Split* fs = nullptr,
+                                bool strict = false) {
+    const bool f16 = dw && fs && fs->split, single_epi = epi == TE_EPI_STORE || epi == TE_EPI_GELU_BWD;
+    if (f16 && single_epi && te_tc_fwd16_supported(M, out, in, out))
         return te_tc_linear_bwd16(fs->ready ? nullptr : dy, out, fs->split, fs->scale, dw, in, out, dx, e0, M, epi, st);
-    if (dw && tf32 && (epi == TE_EPI_STORE || epi == TE_EPI_GELU_BWD) && te_tc_gemm3x_supported(M, out, in, out))
+    if (strict && f16) return no_fallback("linear backward: the single-pass fp16 kernel does not take this shape / epilogue");
+    if (dw && tf32 && single_epi && te_tc_gemm3x_supported(M, out, in, out))
         return te_tc_linear_bwd_tf32(dy, out, dw, in, out, dx, e0, M, epi, st);
+    if (strict && dw && tf32) return no_fallback("linear backward: the single-pass TF32 kernel does not take this shape / epilogue");
     if (dw && te_tc_gemm3x_supported(M, out, in, out))
         return te_tc_linear_bwd(dy, dw, in, out, dx, e0, M, epi, st);
+    if (strict && dw) return no_fallback("linear backward: the 3xTF32 kernel does not take this shape");
     return linear_bwd(dy, w, dx, e0, M, in, out, epi, st);
 }
 

@@ -138,6 +138,122 @@ def linear_backward_tf32(dy, w):
     return dx
 
 
+# ---- diagnostic wrappers of the kernels (include/te_b200.h: "Diagnostic entry points"): no fall-back, a shape the requested
+# kernel does not take raises TeError with status TE_ERR_UNSUPPORTED -------------------------------------------------------
+LINEAR_FAMILIES = {
+    "simt": 0,
+    "3xtf32": _lib.FLAG_LINEAR_TENSOR_CORES,
+    "f16_split": _lib.FLAG_LINEAR_TENSOR_CORES | _lib.FLAG_LINEAR_F16_SPLIT,          # forward only
+    "tf32": _lib.FLAG_LINEAR_TENSOR_CORES | _lib.FLAG_BACKWARD_TF32,                  # backward only
+    "f16": _lib.FLAG_LINEAR_TENSOR_CORES | _lib.FLAG_BACKWARD_F16,                    # backward only
+}
+LINEAR_EPI = {"store": 0, "bias": 1, "bias_gelu": 2, "bias_add": 3, "gelu_bwd": 4}
+ATTN_EPI = {"store": 0, "mul": 1, "sd": 2, "softmax": 3}
+
+
+@_on_device
+def linear_forward_epi(x, w, bias=None, e0=None, epi="bias", family="simt"):
+    """y = x W^T (+ bias) with a fused epilogue on the kernel family named (LINEAR_FAMILIES) -> (y, y2); y2 is None unless
+    epi is "bias_gelu" (erf GELU of y) or "bias_add" (e0 + y)."""
+    _req(x, w, bias, e0)
+    if x.dim() != 2 or w.dim() != 2 or w.shape[1] != x.shape[1] or (e0 is not None and e0.shape != (x.shape[0], w.shape[0])):
+        raise ValueError("linear_forward_epi: x [rows,in], w [out,in], e0 [rows,out] expected")
+    rows, K, N = x.shape[0], x.shape[1], w.shape[0]
+    flags = LINEAR_FAMILIES[family]
+    y = torch.empty(rows, N, device=x.device, dtype=torch.float32)
+    y2 = torch.empty_like(y) if epi in ("bias_gelu", "bias_add") else None
+    nscratch = 16 * w.numel() + ((rows * K + 63) // 64 * 64 + rows * ((K + 127) // 128) if family == "f16_split" else 0)
+    scratch = torch.empty(nscratch, device=x.device, dtype=torch.float32) if flags else None
+    check(_lib.load().te_linear_forward_epi(ptr(x), ptr(w), ptr(bias), ptr(e0), ptr(y), ptr(y2), ptr(scratch), rows, K, N,
+                                            LINEAR_EPI[epi], flags, _stream()), "te_linear_forward_epi")
+    return y, y2
+
+
+@_on_device
+def linear_backward_epi(dy, w, e0=None, epi="store", family="simt"):
+    """dx = dy W, times GELU'(e0) with epi="gelu_bwd", on the kernel family named (LINEAR_FAMILIES)."""
+    _req(dy, w, e0)
+    if dy.dim() != 2 or w.dim() != 2 or dy.shape[1] != w.shape[0] or (e0 is not None and e0.shape != (dy.shape[0], w.shape[1])):
+        raise ValueError("linear_backward_epi: dy [rows,out], w [out,in], e0 [rows,in] expected")
+    rows, K, N = dy.shape[0], w.shape[0], w.shape[1]
+    flags = LINEAR_FAMILIES[family]
+    dx = torch.empty(rows, N, device=dy.device, dtype=torch.float32)
+    nscratch = 16 * w.numel() + ((rows * K // 2 + 63) // 64 * 64 + rows * ((K + 127) // 128) if family == "f16" else 0)
+    scratch = torch.empty(nscratch, device=dy.device, dtype=torch.float32) if flags else None
+    check(_lib.load().te_linear_backward_epi(ptr(dy), ptr(w), ptr(e0), ptr(dx), ptr(scratch), rows, N, K, LINEAR_EPI[epi],
+                                             flags, _stream()), "te_linear_backward_epi")
+    return dx
+
+
+@_on_device
+def layernorm_split(x, w, b, eps):
+    """LayerNorm of x [rows, D] that also emits the fp16-split operand of y -> (y, mean, rstd, hi, lo, scale_inv)
+    (see include/te_b200.h: te_layernorm_split)."""
+    _req(x, w, b)
+    rows, D = x.shape
+    y = torch.empty_like(x)
+    mean = torch.empty(rows, device=x.device, dtype=torch.float32)
+    rstd = torch.empty_like(mean)
+    buf = torch.empty(2, rows, D, device=x.device, dtype=torch.float16)
+    scale = torch.empty(rows, (D + 127) // 128, device=x.device, dtype=torch.float32)
+    check(_lib.load().te_layernorm_split(ptr(x), ptr(w), ptr(b), ptr(y), ptr(mean), ptr(rstd), ptr(buf[0]), ptr(buf[1]),
+                                         ptr(scale), rows, D, eps, _stream()), "te_layernorm_split")
+    return y, mean, rstd, buf[0], buf[1], scale
+
+
+@_on_device
+def tc_zplus_s(x, w, r, y, bias=None, f16=False, bf16=False):
+    """S = safe_divide(r, Z) of the z+ rule on the single-pass tensor-core S kernel (Z from the saved forward output y).
+    f16=False: S fp32 (TF32-rounded) [rows, out]; f16=True: (s16 fp16 [rows, out], scale_inv [rows, out / 128])."""
+    _req(x, w, r, y, bias)
+    if x.dim() != 2 or w.dim() != 2 or w.shape[1] != x.shape[1] or r.shape != y.shape or r.shape != (x.shape[0], w.shape[0]):
+        raise ValueError("tc_zplus_s: x [rows,in], w [out,in], r / y [rows,out] expected")
+    rows, K, N = x.shape[0], x.shape[1], w.shape[0]
+    scratch = torch.empty(16 * w.numel() + rows * K, device=x.device, dtype=torch.float32)
+    s = None if f16 else torch.empty(rows, N, device=x.device, dtype=torch.float32)
+    s16 = torch.empty(rows, N, device=x.device, dtype=torch.float16) if f16 else None
+    sc = torch.full((rows, N // 128), float("nan"), device=x.device, dtype=torch.float32) if f16 else None
+    check(_lib.load().te_tc_zplus_s(ptr(x), ptr(w), ptr(bias), ptr(y), ptr(r), ptr(s), ptr(s16), ptr(sc), ptr(scratch), rows,
+                                    K, N, _lib.FLAG_ZPLUS_S1_BF16 if bf16 else 0, _stream()), "te_tc_zplus_s")
+    return (s16, sc) if f16 else s
+
+
+def _span(t, n, what):
+    """t must be an fp32 CUDA tensor (a view is fine) whose storage holds n floats from its first element."""
+    if not (t.is_cuda and t.dtype == torch.float32):
+        raise ValueError("%s: fp32 CUDA tensor expected" % what)
+    if t.untyped_storage().nbytes() // 4 - t.storage_offset() < n:
+        raise ValueError("%s: the kernel would address %d floats, the tensor's storage holds fewer" % (what, n))
+
+
+@_on_device
+def tc_attention_nn(a, lda, b, ldb, batch, heads, n, dh, out, ld_out, e=None, alpha=1.0, epi="store", single_pass=False):
+    """out[b,h,i,j] = epi(alpha * sum_d a[b*n+i, h*dh+d] b[b*n+j, h*dh+d]) on the tensor-core N x N kernel, in place into out
+    ([batch, heads, n, ld_out] storage).  a / b: the first element of head 0 of packed rows (views into [rows, 3D] allowed)."""
+    _span(a, (batch * n - 1) * lda + heads * dh, "a")
+    _span(b, (batch * n - 1) * ldb + heads * dh, "b")
+    for t, nm in ((out, "out"), (e, "e")):
+        if t is not None:
+            _span(t, (batch * heads * n - 1) * ld_out + ((n + 3) & ~3), nm)
+    check(_lib.load().te_tc_attention_nn(ptr(a), lda, ptr(b), ldb, batch, heads, n, dh, ptr(out), ld_out, ptr(e), alpha,
+                                         ATTN_EPI[epi], int(single_pass), _stream()), "te_tc_attention_nn")
+    return out
+
+
+@_on_device
+def tc_attention_nk(amap, np_, amn, x, ldx, batch, heads, n, out, ld_out, e=None, alpha=1.0, epi="store", single_pass=False):
+    """out[b*n+m, h*64+d] = epi(alpha * sum_k M_h[m,k] x[b*n+k, h*64+d]), M_h = amap[b,h] ([n, np]) or its transpose (amn=1), on
+    the tensor-core token-reduction kernel, in place into out (packed rows of stride ld_out)."""
+    _span(amap, batch * heads * n * np_, "map")
+    _span(x, (batch * n - 1) * ldx + heads * 64, "x")
+    for t, nm in ((out, "out"), (e, "e")):
+        if t is not None:
+            _span(t, (batch * n - 1) * ld_out + heads * 64, nm)
+    check(_lib.load().te_tc_attention_nk(ptr(amap), np_, amn, ptr(x), ldx, batch, heads, n, ptr(out), ld_out, ptr(e), alpha,
+                                         ATTN_EPI[epi], int(single_pass), _stream()), "te_tc_attention_nk")
+    return out
+
+
 @_on_device
 def linear_relprop(x, w, r, tensor_cores=False, y=None, bias=None, bf16=False, variant="ours", r_f16=False):
     """``Linear.relprop`` (layers_ours.py:207-230): x [...,in], w [out,in], r [...,out] -> [...,in].
