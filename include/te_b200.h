@@ -330,6 +330,31 @@ TE_API int te_tc_attention_nn(const float* A, long long lda, const float* B, lon
 TE_API int te_tc_attention_nk(const float* map, int np, int amn, const float* X, long long ldx, int batch, int heads, int n,
                               float* out, int ld_out, const float* E, float alpha, int epi, int single_pass, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Perturbation evaluation  (baselines/ViT/pertubation_eval_from_hdf5.py:17-23,57-68,88-118)
+ * ---------------------------------------------------------------------------------------------- */
+#define TE_PERTURB_MAX_STEPS 64
+#define TE_PERTURB_MAX_CHANNELS 16
+/* Workspace of te_perturb_images for `batch` samples of `pixels` pixels (one threshold pair per sample and step). */
+TE_API long long te_perturb_workspace_bytes(int batch, long long pixels);
+/* Every perturbed, normalised input of a batch in one call: images [batch, channels, pixels] (raw, in [0, 1]), saliency
+ * [batch, pixels], host ks[steps] non-decreasing pixel counts in [0, pixels], host mean / std [channels] ->
+ * out [steps, batch, channels, pixels] (step-major: step i is one contiguous forward batch).
+ * Order key v = negate ? -s : s; pixels are ordered NaN first, then by descending v, then by ascending pixel index (-0 == +0).
+ * Pixel p is removed at step i iff its position in that order is < ks[i], and
+ *   out[i,b,c,p] = ((removed ? 0 : images[b,c,p]) - mean[c]) / std[c]    (fp32 subtract, then IEEE division)
+ * = normalize(data.clone().scatter_(-1, topk(v, ks[i]).indices, 0)) of the reference with its choice among tied values fixed.
+ * steps <= TE_PERTURB_MAX_STEPS, channels <= TE_PERTURB_MAX_CHANNELS. */
+TE_API int te_perturb_images(const float* images, const float* saliency, int batch, int channels, long long pixels,
+                             const int* ks, int steps, int negate, const float* mean, const float* std, float* out,
+                             void* workspace, long long workspace_bytes, void* stream);
+/* Per row of logits [rows, classes] (classes >= 2) with target [rows] (int32, device): pred = first index of the maximum,
+ * max_logit, max_prob = the largest fp32 softmax probability, dissim = log(p_target / p_second) with p_second the
+ * second-largest probability counting duplicates (topk(2)[0][:, 1]), in fp32 as the reference writes it (an underflowed
+ * p_target gives -inf, an underflowed p_second +inf; a target outside [0, classes) gives NaN). */
+TE_API int te_logit_stats(const float* logits, const int* target, int rows, int classes, int* pred, float* max_logit,
+                          float* max_prob, float* dissim, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -6,7 +6,7 @@ Drop-in for the ``transformer_attribution`` hot path of hila-chefer/Transformer-
 kernels behind the C ABI of ``include/te_b200.h``.  There is no CPU fallback.
 
 ``install_aliases()`` registers the reference's top-level module names (``modules.layers_ours``,
-``baselines.ViT.ViT_LRP``, ``baselines.ViT.ViT_explanation_generator``,
+``baselines.ViT.ViT_LRP``, ``baselines.ViT.ViT_explanation_generator``, ``dataset.expl_hdf5``,
 ``BERT_explainability.modules.BERT.ExplanationGenerator`` ...) so that the reference's notebooks and
 eval scripts import this engine unchanged.
 """
@@ -25,6 +25,8 @@ _ALIASES = {
     "baselines.ViT.ViT_new": "transformer_explainability_b200.baselines.ViT.ViT_new",
     "baselines.ViT.ViT_orig_LRP": "transformer_explainability_b200.baselines.ViT.ViT_orig_LRP",
     "baselines.ViT.ViT_explanation_generator": "transformer_explainability_b200.baselines.ViT.ViT_explanation_generator",
+    "dataset": "transformer_explainability_b200.dataset",
+    "dataset.expl_hdf5": "transformer_explainability_b200.dataset.expl_hdf5",
 }
 
 

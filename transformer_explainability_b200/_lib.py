@@ -111,7 +111,14 @@ PROTOTYPES = {
     "te_tc_zplus_s": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_uint, _P]),
     "te_tc_attention_nn": (c_int, [_P, c_ll, _P, c_ll, c_int, c_int, c_int, c_int, _P, c_int, _P, c_float, c_int, c_int, _P]),
     "te_tc_attention_nk": (c_int, [_P, c_int, c_int, _P, c_ll, c_int, c_int, c_int, _P, c_int, _P, c_float, c_int, c_int, _P]),
+    "te_perturb_workspace_bytes": (c_ll, [c_int, c_ll]),
+    "te_perturb_images": (c_int, [_P, _P, c_int, c_int, c_ll, ctypes.POINTER(c_int), c_int, c_int, ctypes.POINTER(c_float),
+                                  ctypes.POINTER(c_float), _P, _P, c_ll, _P]),
+    "te_logit_stats": (c_int, [_P, _P, c_int, c_int, _P, _P, _P, _P, _P]),
 }
+
+PERTURB_MAX_STEPS = 64          # TE_PERTURB_MAX_STEPS
+PERTURB_MAX_CHANNELS = 16       # TE_PERTURB_MAX_CHANNELS
 
 _lib = None
 

@@ -458,3 +458,51 @@ def compute_rollout_attention(all_layer_matrices, start_layer=0, normalize=False
     check(lib.te_compute_rollout_attention(ptr(mats), L, B, N, start_layer, int(normalize), ptr(joint), ptr(ws),
                                            ws.numel() * 4, _stream()), "te_compute_rollout_attention")
     return joint
+
+
+# ---- perturbation evaluation (baselines/ViT/pertubation_eval_from_hdf5.py) ------------------------------------------------
+@_on_device
+def perturb_images(images, saliency, ks, negate=False, mean=(0.5, 0.5, 0.5), std=(0.5, 0.5, 0.5)):
+    """Every perturbed, normalised input of a batch: images [B,C,H,W] (or [B,C,P]) in [0, 1], saliency [B,H,W] / [B,1,H,W] /
+    [B,P], ks non-decreasing pixel counts -> out [S,B,C,H,W] (or [S,B,C,P]).  Step i removes the ks[i] pixels that come first
+    in the order NaN, descending (negate ? -s : s), ascending pixel index, and normalises ((x - mean) / std, fp32)
+    (see include/te_b200.h: te_perturb_images)."""
+    _req(images, saliency)
+    if images.dim() < 3:
+        raise ValueError("perturb_images: images [B,C,H,W] or [B,C,P] expected")
+    B, C = images.shape[0], images.shape[1]
+    P = images[0, 0].numel()
+    if saliency.shape[0] != B or saliency.numel() != B * P:
+        raise ValueError("perturb_images: saliency must hold one value per pixel of each sample, got %s for images %s"
+                         % (tuple(saliency.shape), tuple(images.shape)))
+    ks = [int(k) for k in ks]
+    if len(mean) != C or len(std) != C:
+        raise ValueError("perturb_images: mean / std need one value per channel")
+    lib = _lib.load()
+    nbytes = check(lib.te_perturb_workspace_bytes(B, P), "te_perturb_workspace_bytes")
+    ws = _workspace(nbytes, images.device)
+    out = torch.empty((len(ks),) + tuple(images.shape), device=images.device, dtype=torch.float32)
+    ks_c = (_lib.c_int * max(len(ks), 1))(*ks)
+    mean_c = (_lib.c_float * C)(*[float(m) for m in mean])
+    std_c = (_lib.c_float * C)(*[float(s) for s in std])
+    check(lib.te_perturb_images(ptr(images), ptr(saliency), B, C, P, ks_c, len(ks), int(bool(negate)), mean_c, std_c, ptr(out),
+                                ptr(ws), ws.numel() * 4, _stream()), "te_perturb_images")
+    return out
+
+
+@_on_device
+def logit_stats(logits, target):
+    """Per row of logits [R,K] and target [R]: (pred int32, max_logit, max_prob, dissim) with dissim =
+    log(p_target / p_second) in fp32 (see include/te_b200.h: te_logit_stats)."""
+    _req(logits)
+    if logits.dim() != 2 or target.dim() != 1 or target.shape[0] != logits.shape[0] or not target.is_cuda:
+        raise ValueError("logit_stats: logits [R,K] and a CUDA target [R] expected")
+    if target.device != logits.device:
+        raise ValueError("te_b200 ops: all tensors of one call must live on the same device")
+    R, K = logits.shape
+    t = target.to(torch.int32).contiguous()
+    pred = torch.empty(R, device=logits.device, dtype=torch.int32)
+    max_logit, max_prob, dissim = (torch.empty(R, device=logits.device, dtype=torch.float32) for _ in range(3))
+    check(_lib.load().te_logit_stats(ptr(logits), ptr(t), R, K, ptr(pred), ptr(max_logit), ptr(max_prob), ptr(dissim),
+                                     _stream()), "te_logit_stats")
+    return pred, max_logit, max_prob, dissim
