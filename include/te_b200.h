@@ -355,6 +355,40 @@ TE_API int te_perturb_images(const float* images, const float* saliency, int bat
 TE_API int te_logit_stats(const float* logits, const int* target, int rows, int classes, int* pred, float* max_logit,
                           float* max_prob, float* dissim, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Segmentation evaluation  (baselines/ViT/imagenet_seg_eval.py:212-277,312-314; utils/metrices.py)
+ * A sort key is bits(score) << 1 | is_positive for a score >= 0 (-0 is mapped to +0): ascending keys are ascending scores,
+ * and bit-equal scores form one contiguous run.
+ * ---------------------------------------------------------------------------------------------- */
+/* Workspace of te_sort_keys_u32 for n keys in `segments` equal segments (n % segments == 0, n / segments < 2^31). */
+TE_API long long te_sort_workspace_bytes(long long n, int segments);
+/* Stable LSD radix sort of uint32 keys, ascending, each of the `segments` equal segments of keys_in [n] on its own ->
+ * keys_out [n] (keys_out == keys_in is allowed).  Bit-exact: the output is numpy's stable sort of each segment. */
+TE_API int te_sort_keys_u32(const unsigned* keys_in, unsigned* keys_out, long long n, int segments, void* workspace,
+                            long long workspace_bytes, void* stream);
+/* Workspace of te_seg_metrics. */
+TE_API long long te_seg_workspace_bytes(int batch, int grid, int scale);
+/* Per sample of maps [batch, grid*grid] and labels [batch, P] (int32, 0 / 1), P = (grid*scale)^2:
+ *   Res = bilinear x scale of the map (the arithmetic of te_relevance_heatmap; scale 1: the map as given), min-max
+ *   normalised in fp32; mean[b] = the mean of Res (fp64 accumulation, one rounding to fp32); a pixel is foreground iff
+ *   Res > mean.  counts[b] = (TP, FP, FN, TN) of that mask against label 1, row_counts [batch, grid*scale, 3] = (TP, FP, FN)
+ *   of each image row (the reference's F1 is taken per row, utils/metrices.py:26-38); ap[b] = sklearn's average_precision_score of the
+ *   2P scores (1 - Res, Res) against the one-hot label, in fp64; pr_keys [batch, P] (may be NULL) = the keys of
+ *   clamp(Res, min=thr) / max(Res), positive on label 1.
+ *   A degenerate map (max == min, or NaN in it) sets degenerate[b] = 1: every pixel is background, every AP and PR score 0.
+ *   invalid[b] = the number of labels other than 0 / 1 (the results of such a sample are meaningless).
+ * Needs 4 * grid^2 (scale > 1 only) + 12 * grid * scale <= 45056 (shared memory). */
+TE_API int te_seg_metrics(const float* maps, const int* labels, int batch, int grid, int scale, float thr, float* mean,
+                          long long* counts, int* row_counts, double* ap, int* degenerate, long long* invalid, unsigned* pr_keys,
+                          void* workspace, long long workspace_bytes, void* stream);
+/* Workspace of te_pr_curve for n keys. */
+TE_API long long te_pr_curve_workspace_bytes(long long n);
+/* sklearn's _binary_clf_curve over n keys sorted ascending (te_sort_keys_u32): one entry per distinct score, in descending
+ * score order: thresholds (fp32), tps = positives with score >= threshold, fps = negatives with score >= threshold (int64).
+ * The outputs need room for n entries; *count (device) receives the number written. */
+TE_API int te_pr_curve(const unsigned* keys, long long n, float* thresholds, long long* tps, long long* fps, long long* count,
+                       void* workspace, long long workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -115,6 +115,12 @@ PROTOTYPES = {
     "te_perturb_images": (c_int, [_P, _P, c_int, c_int, c_ll, ctypes.POINTER(c_int), c_int, c_int, ctypes.POINTER(c_float),
                                   ctypes.POINTER(c_float), _P, _P, c_ll, _P]),
     "te_logit_stats": (c_int, [_P, _P, c_int, c_int, _P, _P, _P, _P, _P]),
+    "te_sort_workspace_bytes": (c_ll, [c_ll, c_int]),
+    "te_sort_keys_u32": (c_int, [_P, _P, c_ll, c_int, _P, c_ll, _P]),
+    "te_seg_workspace_bytes": (c_ll, [c_int, c_int, c_int]),
+    "te_seg_metrics": (c_int, [_P, _P, c_int, c_int, c_int, c_float, _P, _P, _P, _P, _P, _P, _P, _P, c_ll, _P]),
+    "te_pr_curve_workspace_bytes": (c_ll, [c_ll]),
+    "te_pr_curve": (c_int, [_P, c_ll, _P, _P, _P, _P, _P, c_ll, _P]),
 }
 
 PERTURB_MAX_STEPS = 64          # TE_PERTURB_MAX_STEPS

@@ -506,3 +506,81 @@ def logit_stats(logits, target):
     check(_lib.load().te_logit_stats(ptr(logits), ptr(t), R, K, ptr(pred), ptr(max_logit), ptr(max_prob), ptr(dissim),
                                      _stream()), "te_logit_stats")
     return pred, max_logit, max_prob, dissim
+
+
+# ---- segmentation evaluation (baselines/ViT/imagenet_seg_eval.py) ----------------------------------------------------------
+def _req_u32(t, what):
+    if not (t.is_cuda and t.dtype in (torch.int32, torch.uint32) and t.is_contiguous()):
+        raise ValueError("%s: a contiguous int32 / uint32 CUDA tensor expected" % what)
+
+
+@_on_device
+def seg_metrics(maps, labels, grid=14, scale=16, thr=0.0, pr_keys=False):
+    """Per sample of maps [B, grid*grid] (any shape with B leading) and labels [B, P] (0 / 1, any integer dtype),
+    P = (grid*scale)^2: the mean threshold of the min-max normalised, up-sampled map, the confusion counts of Res > mean,
+    the average precision of the two score channels and, with ``pr_keys``, the PR-curve keys of the sample
+    (see include/te_b200.h: te_seg_metrics).  Returns a dict of CUDA tensors: ``mean`` fp32 [B], ``counts`` int64 [B,4]
+    (TP, FP, FN, TN), ``row_counts`` int32 [B, grid*scale, 3] (TP, FP, FN per image row), ``ap`` fp64 [B], ``degenerate`` int32 [B], ``invalid`` int64 [B], ``pr_keys`` int32 [B,P] (bit
+    patterns of uint32 keys) or None."""
+    B = maps.shape[0]
+    m = maps.reshape(B, -1)
+    _req(m)
+    if m.shape[1] != grid * grid:
+        raise ValueError("seg_metrics: maps must hold grid*grid = %d values per sample, got %d" % (grid * grid, m.shape[1]))
+    P = (grid * scale) ** 2
+    if not labels.is_cuda or labels.device != m.device or labels.shape[0] != B or labels.numel() != B * P:
+        raise ValueError("seg_metrics: labels [B, %d] on the maps' device expected" % P)
+    lab = labels.reshape(B, P).to(torch.int32).contiguous()
+    lib = _lib.load()
+    ws = _workspace(check(lib.te_seg_workspace_bytes(B, grid, scale), "te_seg_workspace_bytes"), m.device)
+    dev = m.device
+    out = {"mean": torch.empty(B, device=dev, dtype=torch.float32),
+           "counts": torch.empty(B, 4, device=dev, dtype=torch.int64),
+           "row_counts": torch.empty(B, grid * scale, 3, device=dev, dtype=torch.int32),
+           "ap": torch.empty(B, device=dev, dtype=torch.float64),
+           "degenerate": torch.empty(B, device=dev, dtype=torch.int32),
+           "invalid": torch.empty(B, device=dev, dtype=torch.int64),
+           "pr_keys": torch.empty(B, P, device=dev, dtype=torch.int32) if pr_keys else None}
+    check(lib.te_seg_metrics(ptr(m), ptr(lab), B, grid, scale, float(thr), ptr(out["mean"]), ptr(out["counts"]), ptr(out["row_counts"]),
+                             ptr(out["ap"]),
+                             ptr(out["degenerate"]), ptr(out["invalid"]), ptr(out["pr_keys"]), ptr(ws), ws.numel() * 4,
+                             _stream()), "te_seg_metrics")
+    return out
+
+
+@_on_device
+def sort_keys(keys, segments=1, out=None):
+    """Stable ascending sort of uint32 keys (int32 / uint32 tensor holding the bit patterns), each of ``segments`` equal
+    segments on its own (see include/te_b200.h: te_sort_keys_u32).  ``out`` may be ``keys`` (in place)."""
+    _req_u32(keys, "sort_keys")
+    n = keys.numel()
+    out = torch.empty_like(keys) if out is None else out
+    _req_u32(out, "sort_keys")
+    if out.numel() != n:
+        raise ValueError("sort_keys: out must hold as many keys as the input")
+    lib = _lib.load()
+    ws = _workspace(check(lib.te_sort_workspace_bytes(n, segments), "te_sort_workspace_bytes"), keys.device)
+    check(lib.te_sort_keys_u32(ptr(keys), ptr(out), n, segments, ptr(ws), ws.numel() * 4, _stream()), "te_sort_keys_u32")
+    return out
+
+
+@_on_device
+def pr_curve(sorted_keys):
+    """sklearn's ``_binary_clf_curve`` over ascending-sorted keys (``sort_keys``): (thresholds fp32, tps int64, fps int64),
+    one entry per distinct score in descending score order (see include/te_b200.h: te_pr_curve)."""
+    _req_u32(sorted_keys, "pr_curve")
+    n = sorted_keys.numel()
+    dev = sorted_keys.device
+    if n == 0:
+        return (torch.empty(0, device=dev), torch.empty(0, device=dev, dtype=torch.int64),
+                torch.empty(0, device=dev, dtype=torch.int64))
+    lib = _lib.load()
+    ws = _workspace(check(lib.te_pr_curve_workspace_bytes(n), "te_pr_curve_workspace_bytes"), dev)
+    thr = torch.empty(n, device=dev, dtype=torch.float32)
+    tps = torch.empty(n, device=dev, dtype=torch.int64)
+    fps = torch.empty(n, device=dev, dtype=torch.int64)
+    count = torch.empty(1, device=dev, dtype=torch.int64)
+    check(lib.te_pr_curve(ptr(sorted_keys), n, ptr(thr), ptr(tps), ptr(fps), ptr(count), ptr(ws), ws.numel() * 4, _stream()),
+          "te_pr_curve")
+    k = int(count.item())
+    return thr[:k], tps[:k], fps[:k]
