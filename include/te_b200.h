@@ -137,8 +137,11 @@ TE_API int te_vit_explain(const te_vit_config* cfg, const float* weights, const 
                    long long workspace_bytes, void* stream);
 
 /* Accessors into the workspace — get_attn / get_attn_gradients / get_attn_cam / get_v ...
- * (ViT_LRP.py:102-130).  name in {"attn","attn_grad","attn_cam","qkv","x_in","ctx","logits","rollout_mats"}.
- * Returns a device pointer, 4 dims and 4 element strides (unused dims are 1). */
+ * (ViT_LRP.py:102-130).  name in {"attn","attn_grad","attn_cam","qkv","x_in","ctx","logits","rollout_mats"}, and the
+ * scratch regions of the last attribute call, "tmp_d0".."tmp_d3" [B,N,D], "tmp_f0","tmp_f1" [B,N,F], "tmp_3d0","tmp_3d1"
+ * [B,N,3D] (diagnostics; a region may be larger than its view).
+ * Returns a device pointer, 4 dims and 4 element strides (unused dims are 1).  Host-only address arithmetic: nothing on
+ * the device is read. */
 TE_API int te_vit_tensor(const te_vit_config* cfg, int batch, void* workspace, const char* name, int layer,
                   float** ptr, long long dims[4], long long strides[4]);
 /* method="full" (ViT_LRP.py:337-343): relevance carried through ``self.add`` (tokens + pos_embed), ``[:, 1:]``,
@@ -199,7 +202,8 @@ TE_API int te_bert_explain(const te_bert_config* cfg, const float* weights, cons
                     int start_layer, unsigned flags, float* maps, float* logits, void* workspace,
                     long long workspace_bytes, void* stream);
 /* get_attn / get_attn_gradients / get_attn_cam of BertSelfAttention (BERT.py:281-297):
- * name in {"attn","attn_grad","attn_cam","hidden","logits"}. */
+ * name in {"attn","attn_grad","attn_cam","hidden","logits","relevance_in"} and the scratch regions "tmp_d0".."tmp_d3",
+ * "tmp_f0","tmp_f1", "tmp_3d0","tmp_3d1" as for te_vit_tensor. */
 TE_API int te_bert_tensor(const te_bert_config* cfg, int batch, int seq, void* workspace, const char* name, int layer,
                    float** ptr, long long dims[4], long long strides[4]);
 

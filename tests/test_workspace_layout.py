@@ -1,0 +1,121 @@
+"""CPU: every workspace region an engine lends to a kernel is at least as large as that kernel's use of it.
+
+The ViT and BERT engines keep a few scratch regions (``tmp_f0/1`` [M, F], ``tmp_3d0/1`` [M, 3D], M = batch * tokens) and
+lend them to kernels that run while they are idle: the hi-only fp16 split of the output gradient of every backward Linear
+(``TE_FLAG_BACKWARD_F16``, rows * out / 2 floats, scales rows * ceil(out / 128) floats), the ``|x|`` scratch of the
+single-pass z+ rules ([rows, in]), the 3-way clone's sum.  Those uses are not all F wide: the qkv backward splits a 3D-wide
+gradient, the qkv z+ rule a D-wide input.  So with mlp_ratio < 1.5 a region sized M * F would be overrun, and the kernel
+would write into the next region, which may be the very tensor it is reading.  The regions are laid out back to back,
+so the extent of one is the distance to the next; ``te_*_tensor`` computes the views on the host without touching a
+device, with any 256-byte-aligned address as the workspace.
+"""
+import ctypes
+
+import pytest
+
+from transformer_explainability_b200 import _lib
+from transformer_explainability_b200.engine import bert_config, vit_config
+
+FAKE_WS = 1 << 40                                    # 256-byte aligned; never dereferenced
+
+
+def _views(lib, fn, cfg, *shape):
+    out = {}
+    for name in ("tmp_f0", "tmp_f1", "tmp_3d0", "tmp_3d1"):
+        p, dims, strides = ctypes.c_void_p(), (ctypes.c_longlong * 4)(), (ctypes.c_longlong * 4)()
+        assert fn(ctypes.byref(cfg), *shape, ctypes.c_void_p(FAKE_WS), name.encode(), 0, ctypes.byref(p), dims,
+                  strides) == 0, lib.te_last_error()
+        numel = 1
+        for d in dims:
+            numel *= d
+        out[name] = (p.value, numel)
+    return out
+
+
+def _extents(views):
+    """floats from each region to the next one in the carve order; the last is known only by its view"""
+    order = ["tmp_f0", "tmp_f1", "tmp_3d0", "tmp_3d1"]
+    ext = {}
+    for a, b in zip(order, order[1:]):
+        assert views[b][0] > views[a][0]
+        ext[a] = (views[b][0] - views[a][0]) // 4
+    ext["tmp_3d1"] = views["tmp_3d1"][1]
+    return ext
+
+
+def _bwd_split_uses(M, D, F):
+    """(split floats, scale floats) of the hi-only fp16 split of dy of each backward Linear: fc2, fc1, proj, qkv"""
+    return [(M * out // 2, M * -(-out // 128)) for out in (D, F, D, 3 * D)]
+
+
+def _check(ext, uses):
+    for region, need, what in uses:
+        assert ext[region] >= need, "%s: %d floats, %s needs %d" % (region, ext[region], what, need)
+
+
+VIT = [dict(embed_dim=256, num_heads=4, mlp_ratio=r) for r in (0.5, 1.0, 1.5, 2.0, 4.0)] + \
+      [dict(embed_dim=256, num_heads=4, mlp_ratio=1.0, distilled=True), dict(), dict(embed_dim=768, mlp_ratio=1.0)]
+
+
+@pytest.mark.parametrize("kw", VIT, ids=lambda kw: "-".join("%s%s" % (k, v) for k, v in kw.items()) or "vit_b16")
+@pytest.mark.parametrize("batch", [1, 3])
+def test_vit_lent_regions_cover_their_uses(kw, batch):
+    lib = _lib.load()
+    cfg = vit_config(**kw)
+    D, F = cfg.dim, cfg.mlp_dim
+    npatch = (cfg.img_size // cfg.patch_size) ** 2
+    M = batch * (npatch + (2 if cfg.distilled else 1))
+    ext = _extents(_views(lib, lib.te_vit_tensor, cfg, batch))
+    uses = [("tmp_f0", M * F, "dF / RF"),
+            ("tmp_f0", batch * npatch * cfg.in_chans * cfg.patch_size ** 2, "the im2col patches"),
+            ("tmp_f0", M * D, "the |x| scratch of the qkv z+ rule"),
+            ("tmp_f1", M * F, "SF, the |x| scratch of the fc2 z+ rule, the GELU-output fp16 split"),
+            ("tmp_3d0", M * 3 * D, "dqkv / S of the qkv z+ rule"),
+            ("tmp_3d0", 2 * M * D, "the |x| scratch of the proj z+ rule at S + M*D")]
+    for split, scale in _bwd_split_uses(M, D, F):
+        uses += [("tmp_f1", split, "the fp16 split of dy"), ("tmp_3d1", scale, "the block scales of dy")]
+    _check(ext, uses)
+
+
+BERT = [dict(hidden_size=256, num_attention_heads=4, intermediate_size=f) for f in (128, 256, 384, 512, 1024)] + \
+       [dict(), dict(intermediate_size=768)]
+
+
+@pytest.mark.parametrize("kw", BERT, ids=lambda kw: "-".join("%s%s" % (k, v) for k, v in kw.items()) or "bert_base")
+@pytest.mark.parametrize("batch,seq", [(1, 130), (3, 512)])
+def test_bert_lent_regions_cover_their_uses(kw, batch, seq):
+    lib = _lib.load()
+    cfg = bert_config(**kw)
+    D, F, M = cfg.hidden, cfg.intermediate, batch * seq
+    ext = _extents(_views(lib, lib.te_bert_tensor, cfg, batch, seq))
+    uses = [("tmp_f0", M * F, "dF / RF"),
+            ("tmp_f1", M * F, "SF, the |x| scratch of the output-dense z+ rule, the GELU-output fp16 split"),
+            ("tmp_f1", M * D, "the 3-way clone's sum"),
+            ("tmp_3d0", M * 3 * D, "dqkv / S"),
+            ("tmp_3d0", 2 * M * D, "the |x| scratch of the attention z+ rules at S + M*D")]
+    for split, scale in _bwd_split_uses(M, D, F):
+        uses += [("tmp_f1", split, "the fp16 split of dy"), ("tmp_3d1", scale, "the block scales of dy")]
+    _check(ext, uses)
+
+
+# te_*_workspace_bytes of the benchmarked configurations (batch 1 and the benchmarked batch), as laid out before the
+# lent regions were sized by their uses: with F = 4D every use fits in M*F, so the size must not move
+BASELINE_BYTES = [
+    ("vit", dict(), 1, 218101760),
+    ("vit", dict(), 256, 55828030464),
+    ("vit", dict(embed_dim=1024, depth=24, num_heads=16), 1, 556246272),
+    ("vit", dict(embed_dim=1024, depth=24, num_heads=16), 64, 35597718272),
+    ("vit", dict(distilled=True), 1, 219188224),
+    ("vit", dict(distilled=True), 256, 56107475968),
+    ("bert", dict(), (1, 512), 862579712),
+    ("bert", dict(), (64, 512), 55205061632),
+]
+
+
+@pytest.mark.parametrize("model,kw,shape,nbytes", BASELINE_BYTES)
+def test_baseline_workspace_bytes_unchanged(model, kw, shape, nbytes):
+    lib = _lib.load()
+    if model == "vit":
+        assert lib.te_vit_workspace_bytes(ctypes.byref(vit_config(**kw)), shape) == nbytes
+    else:
+        assert lib.te_bert_workspace_bytes(ctypes.byref(bert_config(**kw)), *shape) == nbytes

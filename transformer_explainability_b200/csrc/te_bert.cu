@@ -10,6 +10,8 @@
 // addressed in place exactly like the ViT engine; their three z+ rules stay separate (Clone(3) needs them apart).
 #include <string.h>
 
+#include <algorithm>
+
 #include "../../include/te_b200.h"
 #include "te_engine_util.h"
 #include "te_gemm_tc.h"
@@ -138,6 +140,7 @@ struct Workspace {
     LayerAct layer[kMaxDepth];
     float *h_last, *maskadd, *pd, *pooled, *logits, *seed, *dpool, *dpd, *dfirst, *rpool, *rfirst, *shead;
     float *tD[4], *tF[2], *t3D[2], *tA[2];
+    long long nF[2];                  // floats of tF[0], tF[1]
     float *mats, *joint[2];
     double* addpart;
     long long bytes;
@@ -160,7 +163,12 @@ static void carve(const Dims& d, char* base, Workspace& ws) {
     ws.rpool = take(BD); ws.rfirst = take(BD);
     ws.logits = take(BC); ws.seed = take(BC); ws.shead = take(BC > BD ? BC : BD);
     for (int i = 0; i < 4; ++i) ws.tD[i] = take(MD);
-    ws.tF[0] = take(MF); ws.tF[1] = take(MF);
+    // tF[1] is sized by its largest use, not by F alone (with intermediate < 1.5 hidden a use is wider than M*F):
+    //   SF [M, F] (and the |x| scratch of the output-dense z+ rule); the GELU-output fp16 split [M, F] of the forward; the
+    //   3-way clone's sum [M, D]; the hi-only fp16 split of dy of every backward Linear, widest for qkv [M, 3D / 2]
+    ws.nF[0] = MF;
+    ws.nF[1] = std::max({MF, MD, bwd_split_floats(d.M, 3 * d.D)});
+    ws.tF[0] = take(ws.nF[0]); ws.tF[1] = take(ws.nF[1]);
     ws.t3D[0] = take(M3D); ws.t3D[1] = take(M3D);
     ws.tA[0] = take(AT); ws.tA[1] = take(AT);
     ws.mats = take((long long)d.L * d.B * d.N * d.NP);
@@ -290,7 +298,8 @@ extern "C" int te_bert_attribute(const te_bert_config* cfg, const float* weights
     if (start_layer < 0 || start_layer >= d.L) { te_set_last_error("te_bert_attribute: start_layer out of range"); return TE_ERR_ARG; }
     // fp16 backward split of dy in tF[1], block scales in t3D[1] (idle until the relprop)
     Select sel;
-    TE_TRY(decode_flags(sel, "te_bert_attribute", flags, derived, start_layer, true, ws.tF[1], ws.t3D[1]));
+    TE_TRY(decode_flags(sel, "te_bert_attribute", flags, derived, start_layer, true, {ws.tF[1], ws.nF[1]},
+                        {ws.t3D[1], d.M * 3LL * d.D}, d.M, std::max(3 * d.D, d.F)));
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     Weights w;
     bind_weights(cfg, weights, w);
@@ -405,6 +414,13 @@ extern "C" int te_bert_tensor(const te_bert_config* cfg, int batch, int seq, voi
     const View set{ptr, dims, strides};
     if (n == "logits") return set(ws.logits, d.B, d.C, 1, 1, d.C, 1, 1, 1);
     if (n == "relevance_in") return set(ws.tD[0], d.B, d.N, d.D, 1, (long long)d.N * d.D, d.D, 1, 1);
+    // scratch of the last attribute() call (debug / diagnostics): tmp_d0..3 [B,N,D], tmp_f0..1 [B,N,F], tmp_3d0..1 [B,N,3D]
+    if (n.rfind("tmp_d", 0) == 0 && n.size() == 6 && n[5] >= '0' && n[5] <= '3')
+        return set(ws.tD[n[5] - '0'], d.B, d.N, d.D, 1, (long long)d.N * d.D, d.D, 1, 1);
+    if (n.rfind("tmp_f", 0) == 0 && n.size() == 6 && n[5] >= '0' && n[5] <= '1')
+        return set(ws.tF[n[5] - '0'], d.B, d.N, d.F, 1, (long long)d.N * d.F, d.F, 1, 1);
+    if (n.rfind("tmp_3d", 0) == 0 && n.size() == 7 && n[6] >= '0' && n[6] <= '1')
+        return set(ws.t3D[n[6] - '0'], d.B, d.N, 3LL * d.D, 1, (long long)d.N * 3 * d.D, 3LL * d.D, 1, 1);
     if (layer < 0 || layer >= d.L) { te_set_last_error("te_bert_tensor: layer out of range"); return TE_ERR_ARG; }
     LayerAct& a = ws.layer[layer];
     const long long hs = (long long)d.N * d.NP, bs = hs * d.H;

@@ -160,10 +160,20 @@ struct Select {
     ZplusVariant zv;      // bf16 / fp16 variants of the tensor-core z+ rule
     int low;              // lowest block the relprop must reach
 };
+// A workspace region an engine lends to a kernel while the region is idle, with the floats it holds.
+struct Lent { float* ptr; long long floats; };
+// The hi-only fp16 split of dy [rows, out] (TE_FLAG_BACKWARD_F16): rows*out/2 floats of fp16 values, rows*ceil(out/128)
+// floats of block scales.
+static inline long long bwd_split_floats(long long rows, int out) { return rows * out / 2; }
+static inline long long bwd_scale_floats(long long rows, int out) { return rows * ((out + 127) / 128); }
+
 // fn: prefix of the error message.  zplus: the call runs the z+ rules, so TE_FLAG_ZPLUS_TENSOR_CORES needs `derived` as well.
-// bwd_split / bwd_scale: buffers idle during the class-gradient backward, lent for the fp16 split of dy.
+// bwd_split / bwd_scale: regions idle during the class-gradient backward, lent for the fp16 split of dy; rows / widest_out:
+// the rows and the widest output of the backward Linears.  A lent region smaller than that use is an error
+// (TE_ERR_WORKSPACE), never a write past its end into the next region.
 static inline int decode_flags(Select& s, const char* fn, unsigned flags, const float* derived, int start_layer, bool zplus,
-                               float* bwd_split = nullptr, float* bwd_scale = nullptr) {
+                               Lent bwd_split = {nullptr, 0}, Lent bwd_scale = {nullptr, 0}, long long rows = 0,
+                               int widest_out = 0) {
     if ((flags & (TE_FLAG_LINEAR_TENSOR_CORES | (zplus ? TE_FLAG_ZPLUS_TENSOR_CORES : 0u))) && !derived) {
         te_set_last_error((std::string(fn) + ": tensor-core flags need the derived weight buffer").c_str());
         return TE_ERR_ARG;
@@ -174,7 +184,12 @@ static inline int decode_flags(Select& s, const char* fn, unsigned flags, const 
     s.btf = (flags & TE_FLAG_BACKWARD_TF32) != 0;
     s.rtf = (flags & TE_FLAG_RELPROP_TF32) != 0;
     s.f16 = s.lbase && (flags & TE_FLAG_LINEAR_F16_SPLIT);
-    s.bfs = {(s.lbase && (flags & TE_FLAG_BACKWARD_F16)) ? bwd_split : nullptr, bwd_scale, false, nullptr, nullptr};
+    const bool bf16 = s.lbase && (flags & TE_FLAG_BACKWARD_F16) && bwd_split.ptr;
+    if (bf16 && (bwd_split.floats < bwd_split_floats(rows, widest_out) || bwd_scale.floats < bwd_scale_floats(rows, widest_out))) {
+        te_set_last_error((std::string(fn) + ": the region lent for the fp16 split of the backward gradients is too small").c_str());
+        return TE_ERR_WORKSPACE;
+    }
+    s.bfs = {bf16 ? bwd_split.ptr : nullptr, bwd_scale.ptr, false, nullptr, nullptr};
     s.zv = te_zplus_from_flags(flags);
     s.low = (flags & (TE_FLAG_KEEP_ALL_CAMS | TE_FLAG_RELPROP_TO_INPUT)) ? 0 : start_layer;
     return TE_OK;

@@ -7,6 +7,8 @@
 // Attention :132-177, Mlp :61-74), baselines/ViT/ViT_explanation_generator.py:25-41.
 #include <string.h>
 
+#include <algorithm>
+
 #include "../../include/te_b200.h"
 #include "te_engine_util.h"
 #include "te_kernels.h"
@@ -136,6 +138,7 @@ struct Workspace {
     LayerAct layer[kMaxDepth];
     float *x_last, *xf, *logits, *logits2, *seed, *dpool, *rhead0, *rhead1, *shead;
     float *tD[4], *tF[2], *t3D[2], *tA;
+    long long nF[2];                  // floats of tF[0], tF[1]
     float *mats, *joint[2];
     float* pix;                       // scratch of the first-layer (pixel) relprop, method="full"
     double* addpart;
@@ -160,9 +163,15 @@ static void carve(const Dims& d, char* base, Workspace& ws) {
     ws.dpool = take((long long)d.B * d.D); ws.rhead0 = take((long long)d.B * d.D);
     ws.rhead1 = take((long long)d.B * d.D);
     for (int i = 0; i < 4; ++i) ws.tD[i] = take(MD);
+    // tF[0], tF[1] are sized by their largest use, not by F alone (with mlp_ratio < 1.5 a use is wider than M*F):
+    //   tF[0]: dF / RF [M, F]; the im2col patches; the |x| scratch [M, D] of the qkv z+ rule
+    //   tF[1]: SF [M, F] (and the |x| scratch of the fc2 z+ rule); the GELU-output fp16 split [M, F] of the forward; the
+    //          hi-only fp16 split of dy of every backward Linear, widest for qkv [M, 3D / 2]
     const long long patches = (long long)d.B * d.npatch * d.KP;
-    ws.tF[0] = take(MF > patches ? MF : patches);
-    ws.tF[1] = take(MF);
+    ws.nF[0] = std::max({MF, patches, MD});
+    ws.nF[1] = std::max(MF, te_util::bwd_split_floats(d.M, 3 * d.D));
+    ws.tF[0] = take(ws.nF[0]);
+    ws.tF[1] = take(ws.nF[1]);
     ws.t3D[0] = take(M3D); ws.t3D[1] = take(M3D);
     ws.tA = take(AT);
     ws.mats = take((long long)d.L * d.B * d.N * d.NP);
@@ -308,10 +317,11 @@ extern "C" int te_vit_attribute(const te_vit_config* cfg, const float* weights, 
     Weights w;
     bind_weights(cfg, weights, w);
     const float scale = 1.0f / sqrtf((float)d.dh);
-    const long long MD = d.M * d.D;
+    const long long MD = d.M * d.D, M3D = d.M * 3LL * d.D;
     // fp16 backward split of dy in tF[1], block scales in t3D[1] (idle until the relprop)
     te_util::Select sel;
-    TE_TRY(te_util::decode_flags(sel, "te_vit_attribute", flags, derived, start_layer, true, ws.tF[1], ws.t3D[1]));
+    TE_TRY(te_util::decode_flags(sel, "te_vit_attribute", flags, derived, start_layer, true, {ws.tF[1], ws.nF[1]},
+                                 {ws.t3D[1], M3D}, d.M, std::max(3 * d.D, d.F)));
     const bool lrpv = (flags & TE_FLAG_RULES_LRP) != 0;         // rule library of modules/layers_lrp.py (ViT_orig_LRP.py)
 
     // ---- class index and seeds  (ViT_explanation_generator.py:28-35) ---------------------------
