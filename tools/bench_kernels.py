@@ -1,7 +1,6 @@
 """Time the tensor-core GEMM families alone at the bench shapes (CUDA events, 5 reps after 2 warm-ups):
 
     python tools/bench_kernels.py            # every family, the default kernel selection
-    TE_B200_ZPLUS_PERSISTENT=0 python tools/bench_kernels.py        # round-1 single-CTA z+ kernels
 
 Prints one line per (family, shape): ms, algorithmic TFLOP/s and the fraction of the TF32 roof (measured bf16 / 2).
 """

@@ -135,14 +135,15 @@ __device__ __forceinline__ int frag_col(int tid, int j) { return 8 * (j >> 2) + 
 
 // ---- the kernel -----------------------------------------------------------------------------------------------------
 template <class P>
-__global__ void __launch_bounds__(NTHREADS, 1) wg_kernel(const P p) {
+__global__ void __launch_bounds__(NTHREADS, 1) wg_kernel(const P p, int col_fast) {
     constexpr int NR = P::BN / 2;
     constexpr int NA = P::NACC;
     constexpr int NT = P::CHUNK ? NA : 1, NTR = P::CHUNK ? NR : 1;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     const int tid = threadIdx.x, wg = tid >> 7;
-    const int m0 = blockIdx.x * BM, n0 = blockIdx.y * P::BN, z = blockIdx.z;
+    const int m0 = (col_fast ? blockIdx.y : blockIdx.x) * BM, n0 = (col_fast ? blockIdx.x : blockIdx.y) * P::BN;
+    const int z = blockIdx.z;
     float acc[NA][NR];
     float tot[NT][NTR];
 #pragma unroll
@@ -196,6 +197,7 @@ template <bool SINGLE, bool BF, int OUT>
 struct ZsProb : NoScale {
     static constexpr int BN = 128, NACC = 1, CHUNK = 0;
     static constexpr int STAGE = SINGLE ? 2 * TILE128 : 4 * TILE128;
+    static constexpr bool COL_FAST = true;
     int M, N, K;
     const float* x; long long ldx;
     const void* xabs;                       // BF: bf16(|x|) [M, K]
@@ -293,6 +295,7 @@ struct ZrProb {
     static constexpr int BN = (KIND == 2) ? 64 : 128, NACC = 2, CHUNK = (KIND == 2) ? 2 : 0;
     static constexpr int BT = BN * 128;
     static constexpr int STAGE = TILE128 + 2 * BT;
+    static constexpr bool COL_FAST = true;
     int M, N, K;
     const void* s; const void* wp; const void* wn;     // S [M, K] (row stride K), W+^T / W-^T [N, K]
     const float* rs; int rs_ld; const float* cp; const float* cn;   // KIND 2: scales of S, of the rows of W+^T / W-^T
@@ -369,6 +372,7 @@ template <int EPI>
 struct Lin3Prob : NoScale {
     static constexpr int BN = 128, NACC = 1, CHUNK = 4;
     static constexpr int STAGE = 4 * TILE128;
+    static constexpr bool COL_FAST = true;
     int K;
     const float* a; long long lda; const float* bh; const float* bl;
     LinOut o;
@@ -400,6 +404,7 @@ template <int EPI>
 struct Lin1Prob : NoScale {
     static constexpr int BN = 128, NACC = 1, CHUNK = 0;
     static constexpr int STAGE = 2 * TILE128;
+    static constexpr bool COL_FAST = true;
     int K;
     const float* a; long long lda; const float* b;
     LinOut o;
@@ -426,6 +431,7 @@ template <int EPI, int TERMS>
 struct F16Prob {
     static constexpr int BN = 128, NACC = 1, CHUNK = 2;
     static constexpr int STAGE = (TERMS == 3 ? 4 : 2) * TILE128;
+    static constexpr bool COL_FAST = true;
     int K;
     const __half* ah; const __half* al; const __half* bh; const __half* bl;
     const float* rs; int rs_ld; const float* cs;
@@ -471,6 +477,7 @@ struct NnProb : NoScale {
     static constexpr int BN = BN_, NACC = 1, CHUNK = 0;
     static constexpr int BT = BN * 128;
     static constexpr int STAGE = SP ? TILE128 + BT : 2 * (TILE128 + BT);
+    static constexpr bool COL_FAST = false;
     int N, H, dh, ld_out, batch;
     const float* a; long long lda; const float* b; long long ldb;
     const float* E; float* out; float alpha;
@@ -569,6 +576,7 @@ struct NkProb : NoScale {
     static constexpr int BN = BN_, NACC = 1, CHUNK = SP ? 0 : 4;
     static constexpr int BT = BN * 128;
     static constexpr int STAGE = SP ? TILE128 + BT : 2 * (TILE128 + BT);
+    static constexpr bool COL_FAST = false;
     int N, H, NP, ld_out, n_out, n_pad, a_shared;
     const float* map; const float* X; long long ldx;
     const float* rowscale; const float* E; float* out; float alpha;
@@ -635,8 +643,15 @@ struct NkProb : NoScale {
 // ---- launch ---------------------------------------------------------------------------------------------------------
 inline bool a16(const void* p) { return ((uintptr_t)p & 15u) == 0; }
 
+// grid: (m-tiles, column tiles, z).  P::COL_FAST problems (the Linear-rule GEMMs) are launched with the column tile in
+// blockIdx.x, so that consecutively scheduled CTAs share an A panel and the panel is read from HBM about once instead of
+// once per column tile; the weights, at most a few tens of MB, stay in L2.  More than 65535 m-tiles do not fit in grid.y:
+// those launches keep the m-tile in blockIdx.x, which is why the order is a kernel argument.  The tiles and their
+// arithmetic do not change.
 template <class P>
 int launch(const P& p, dim3 grid, cudaStream_t st) {
+    const int col_fast = P::COL_FAST && grid.x <= 65535;
+    if (col_fast) grid = dim3(grid.y, grid.x, grid.z);
     constexpr int SMEM = 2 * P::STAGE + 1024;
     // cudaFuncAttributeMaxDynamicSharedMemorySize is per device: one bit per device ordinal
     static unsigned long long done = 0;
@@ -650,7 +665,7 @@ int launch(const P& p, dim3 grid, cudaStream_t st) {
         done |= 1ull << (dev & 63);
     }
     if (grid.y > 65535 || grid.z > 65535) { te_set_last_error("te_tc: grid too large for one launch"); return TE_ERR_ARG; }
-    wg_kernel<P><<<grid, NTHREADS, SMEM, st>>>(p);
+    wg_kernel<P><<<grid, NTHREADS, SMEM, st>>>(p, col_fast);
     TE_CUDA_CHECK_LAUNCH();
     return TE_OK;
 }
