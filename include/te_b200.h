@@ -107,9 +107,10 @@ TE_API long long te_vit_weight_numel(const te_vit_config* cfg, int i);
 TE_API long long te_vit_weight_offset(const te_vit_config* cfg, int i);
 TE_API long long te_vit_weight_total(const te_vit_config* cfg); /* floats */
 
-/* Tensor-core copies of the frozen Linear weights (W+, W-, W+^T, W-^T rounded to TF32, all K-major) used by
- * the z+ rule when TE_FLAG_ZPLUS_TENSOR_CORES is set: te_vit_derived_total() floats, filled once per weight
- * load by te_vit_prepare_derived().  `derived` may be NULL when the flag is not used. */
+/* Tensor-core operand copies of the frozen Linear weights (TF32, bf16 and row-scaled fp16 forms of W, W^T, their positive /
+ * negative parts and |W|), read by the tensor-core Linear GEMMs and z+ rule kernels that TE_FLAG_LINEAR_TENSOR_CORES,
+ * TE_FLAG_ZPLUS_TENSOR_CORES and the precision flags select: te_vit_derived_total() floats, filled once per weight load by
+ * te_vit_prepare_derived().  `derived` may be NULL when no such flag is used. */
 TE_API long long te_vit_derived_total(const te_vit_config* cfg);
 TE_API int te_vit_prepare_derived(const te_vit_config* cfg, const float* weights, float* derived, void* stream);
 
@@ -281,7 +282,8 @@ TE_API int te_compute_rollout_attention(const float* mats, int layers, int batch
 /* Plain Linear GEMMs — exported for kernel unit tests only.  flags & TE_FLAG_LINEAR_TENSOR_CORES selects the
  * wgmma 3xTF32 path (scratch: 16*in*out floats for the derived weight copies; may be NULL otherwise); with
  * TE_FLAG_LINEAR_F16_SPLIT as well, te_linear_forward_ex runs the fp16-split kernel (scratch: 16*in*out +
- * round_up(rows*in,64) + rows*ceil(in/128) floats). */
+ * round_up(rows*in,64) + rows*ceil(in/128) floats).  te_linear_backward_ex with TE_FLAG_BACKWARD_F16 as well: scratch
+ * 16*in*out + round_up(rows*out/2,64) + rows*ceil(out/128) floats. */
 TE_API int te_linear_forward(const float* x, const float* w, const float* bias, float* y, int rows, int in_features,
                       int out_features, void* stream);
 TE_API int te_linear_forward_ex(const float* x, const float* w, const float* bias, float* y, float* scratch, int rows,

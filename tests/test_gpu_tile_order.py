@@ -32,15 +32,15 @@ def rand(*shape, seed=0, scale=1.0):
 def test_forward_families():
     x = rand(TALL, 64, seed=1)
     w, b = rand(128, 64, seed=2, scale=0.125), rand(128, seed=3, scale=0.1)
-    check_rows(lambda xx: ops.linear_forward_epi(xx, w, b, epi="bias", family="f16_split")[0], x)      # F16Prob<BIAS, 3>
-    check_rows(lambda xx: ops.linear_forward_epi(xx, w, b, epi="bias", family="3xtf32")[0], x)         # Lin3Prob<BIAS>
+    check_rows(lambda xx: ops.linear_forward_epi(xx, w, b, epi="bias", family="f16_split")[0], x)      # LinProb<BIAS, LIN_F16X3>
+    check_rows(lambda xx: ops.linear_forward_epi(xx, w, b, epi="bias", family="3xtf32")[0], x)         # LinProb<BIAS, LIN_3XTF32>
 
 
 def test_backward_families():
     w = rand(64, 128, seed=4, scale=0.125)
     dy = rand(TALL, 64, seed=5)
-    check_rows(lambda d: ops.linear_backward_tf32(d, w), dy)                                            # Lin1Prob
-    check_rows(lambda d: ops.linear_backward_epi(d, w, epi="store", family="f16"), dy)                 # F16Prob<STORE, 1>
+    check_rows(lambda d: ops.linear_backward_tf32(d, w), dy)                                            # LinProb<STORE, LIN_TF32>
+    check_rows(lambda d: ops.linear_backward_epi(d, w, epi="store", family="f16"), dy)                 # LinProb<STORE, LIN_F16>
 
 
 def test_zplus_rule():

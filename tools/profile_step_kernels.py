@@ -21,7 +21,7 @@ from transformer_explainability_b200.baselines.ViT.ViT_LRP import vit_base_patch
 
 
 def family(name):
-    """'wg_kernel<F16Prob<2, 3> >' -> 'F16Prob<2, 3>' ; other kernels keep their base name."""
+    """'wg_kernel<LinProb<2, 2> >' -> 'LinProb<2, 2>' ; other kernels keep their base name."""
     n = name.replace("(anonymous namespace)::", "")
     m = re.search(r"wg_kernel<(\w+<[^>]*>)", n)
     if m:
@@ -76,7 +76,7 @@ def main():
     print("\nper kernel name (kernel ms, share of the step, launches):")
     for name, us in per_name.most_common(args.top):
         print("  %9.2f ms  %5.1f %%  %4d  %s" % (us / 1e3, 100.0 * us / 1e3 / step_ms, calls[name], name[:160]))
-    linear = ("F16Prob", "Lin1Prob", "Lin3Prob", "ZsProb", "ZrProb")
+    linear = ("LinProb", "ZsProb", "ZrProb")
     share = sum(us for n, us in per_family.items() if n.startswith(linear)) / 1e3
     print("\nLinear-rule GEMMs (%s): %.1f ms = %.1f %% of the step" % (" + ".join(linear), share, 100.0 * share / step_ms))
 

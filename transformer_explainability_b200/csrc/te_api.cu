@@ -40,33 +40,49 @@ extern "C" int te_linear_forward(const float* x, const float* w, const float* bi
     return te_gemm_launch(p, TE_L_K, TE_L_K, TE_XF_NONE, TE_EPI_BIAS, ST(stream));
 }
 
+// The scratch of the stand-alone tensor-core entry points, in the layouts include/te_b200.h documents:
+// [S: s_floats, rounded up to 64 | the derived copies of W [out,in] | an operand: op_floats, rounded up to 64 | block scales]
+// (each entry point uses the regions it needs; an empty region takes no room).
+struct TcScratch { float* s; float* derived; float* op; float* scale; };
+static TcScratch tc_scratch(float* scratch, long long s_floats, int in_features, int out_features, long long op_floats) {
+    TcScratch c;
+    c.s = scratch;
+    c.derived = scratch + ((s_floats + 63) & ~63LL);
+    c.op = c.derived + te_tc_derived_floats(in_features, out_features);
+    c.scale = c.op + ((op_floats + 63) & ~63LL);
+    return c;
+}
+
 // forward Linear with the kernel family the flags select.  strict: a tensor-core family that does not take the shape is an
 // error; otherwise every tensor-core path takes the shapes of the 3xTF32 kernel and the derived copies are made only when one is
-// taken.  Scratch layout with TE_FLAG_LINEAR_F16_SPLIT as well:
-// [16*in*out derived | round_up(rows*in,64) fp16 hi,lo split of x | rows*ceil(in/128) block scales]
+// taken.  With TE_FLAG_LINEAR_F16_SPLIT the operand is the fp16 hi, lo split of x (rows*in floats).
 static int linear_forward_flags(const float* x, const float* w, const float* bias, const float* e0, float* y, float* y2,
                                 float* scratch, int rows, int in_features, int out_features, int epi, unsigned flags,
                                 bool strict, cudaStream_t st) {
     const bool tc = (flags & TE_FLAG_LINEAR_TENSOR_CORES) && scratch &&
                     (strict || te_tc_gemm3x_supported(rows, in_features, out_features, in_features));
     if (tc) TE_TRY(te_tc_prepare_weights(w, scratch, in_features, out_features, st));
-    float* split = (tc && (flags & TE_FLAG_LINEAR_F16_SPLIT)) ? scratch + te_tc_derived_floats(in_features, out_features) : nullptr;
-    const te_util::F16Split fs = {split, split ? split + (((long long)rows * in_features + 63) & ~63LL) : nullptr, false, nullptr,
-                                  nullptr};
+    te_util::F16Split fs = {nullptr, nullptr, false, nullptr, nullptr};
+    if (tc && (flags & TE_FLAG_LINEAR_F16_SPLIT)) {
+        const TcScratch c = tc_scratch(scratch, 0, in_features, out_features, (long long)rows * in_features);
+        fs.split = c.op; fs.scale = c.scale;
+    }
     return te_util::linear_fwd_tc(tc ? scratch : nullptr, x, in_features, w, bias, y, y2, e0, rows, in_features, out_features,
                                   epi, st, &fs, strict);
 }
 
-// activation-gradient backward Linear, same selection.  Scratch layout with TE_FLAG_BACKWARD_F16:
-// [16*in*out derived | round_up(rows*out/2,64) fp16 dy | rows*ceil(out/128) block scales]
+// activation-gradient backward Linear, same selection.  With TE_FLAG_BACKWARD_F16 the operand is the fp16 hi part of dy
+// (rows*out/2 floats).
 static int linear_backward_flags(const float* dy, const float* w, const float* e0, float* dx, float* scratch, int rows,
                                  int in_features, int out_features, int epi, unsigned flags, bool strict, cudaStream_t st) {
     const bool tc = (flags & TE_FLAG_LINEAR_TENSOR_CORES) && scratch &&
                     (strict || te_tc_gemm3x_supported(rows, out_features, in_features, out_features));
     if (tc) TE_TRY(te_tc_prepare_weights(w, scratch, in_features, out_features, st));
-    float* split = (tc && (flags & TE_FLAG_BACKWARD_F16)) ? scratch + te_tc_derived_floats(in_features, out_features) : nullptr;
-    const te_util::F16Split fs = {split, split ? split + (((long long)rows * out_features / 2 + 63) & ~63LL) : nullptr, false,
-                                  nullptr, nullptr};
+    te_util::F16Split fs = {nullptr, nullptr, false, nullptr, nullptr};
+    if (tc && (flags & TE_FLAG_BACKWARD_F16)) {
+        const TcScratch c = tc_scratch(scratch, 0, in_features, out_features, (long long)rows * out_features / 2);
+        fs.split = c.op; fs.scale = c.scale;
+    }
     return te_util::linear_bwd_tc(tc ? scratch : nullptr, dy, w, dx, e0, rows, in_features, out_features, epi, st,
                                   (flags & TE_FLAG_BACKWARD_TF32) != 0, &fs, strict);
 }
@@ -126,10 +142,9 @@ extern "C" int te_tc_zplus_s(const float* x, const float* w, const float* bias, 
     REQ(al16(x) && al16(y) && al16(r) && al16(scratch) && (!bias || al16(bias)) && (!s || al16(s)) && (!s16 || al16(s16)),
         "te_tc_zplus_s: operands must be 16-byte aligned");
     cudaStream_t st = ST(stream);
-    // scratch: [16*in*out derived weight copies | rows*in for bf16(|x|)]
-    TE_TRY(te_tc_prepare_weights(w, scratch, in_features, out_features, st));
-    float* xabs = scratch + te_tc_derived_floats(in_features, out_features);
-    return te_tc_zplus_s1(x, in_features, xabs, scratch, r, out_features, y, out_features, bias, s, rows, in_features,
+    const TcScratch c = tc_scratch(scratch, 0, in_features, out_features, 0);    // operand: bf16(|x|)
+    TE_TRY(te_tc_prepare_weights(w, c.derived, in_features, out_features, st));
+    return te_tc_zplus_s1(x, in_features, c.op, c.derived, r, out_features, y, out_features, bias, s, rows, in_features,
                           out_features, st, (flags & TE_FLAG_ZPLUS_S1_BF16) != 0, reinterpret_cast<float*>(s16), s16_scale);
 }
 
@@ -185,10 +200,9 @@ extern "C" int te_linear_relprop(const float* x, const float* w, const float* r,
                                            ST(stream));
     const float* derived = nullptr;
     if ((flags & TE_FLAG_ZPLUS_TENSOR_CORES) && te_tc_zplus_supported(rows, in_features, out_features, in_features)) {
-        // scratch layout with the flag: [rows*out S | 16*in*out derived weight copies]
-        float* d = scratch + (((long long)rows * out_features + 63) & ~63LL);
-        TE_TRY(te_tc_prepare_weights(w, d, in_features, out_features, ST(stream)));
-        derived = d;
+        const TcScratch c = tc_scratch(scratch, (long long)rows * out_features, in_features, out_features, 0);
+        TE_TRY(te_tc_prepare_weights(w, c.derived, in_features, out_features, ST(stream)));
+        derived = c.derived;
     }
     return te_zplus_linear_relprop(x, in_features, w, derived, r, out, scratch, rows, in_features, out_features,
                                    ST(stream));
@@ -201,11 +215,10 @@ extern "C" int te_linear_relprop_ex(const float* x, const float* w, const float*
     const float* derived = nullptr;
     float* xabs = nullptr;
     if ((flags & TE_FLAG_ZPLUS_TENSOR_CORES) && te_tc_zplus_supported(rows, in_features, out_features, in_features)) {
-        // scratch layout with the flag: [rows*out S (64-float aligned) | 16*in*out derived weight copies | rows*in tf32(|x|)]
-        float* d = scratch + (((long long)rows * out_features + 63) & ~63LL);
-        TE_TRY(te_tc_prepare_weights(w, d, in_features, out_features, ST(stream)));
-        derived = d;
-        xabs = d + te_tc_derived_floats(in_features, out_features);
+        const TcScratch c = tc_scratch(scratch, (long long)rows * out_features, in_features, out_features, 0);   // operand: |x|
+        TE_TRY(te_tc_prepare_weights(w, c.derived, in_features, out_features, ST(stream)));
+        derived = c.derived;
+        xabs = c.op;
     }
     return te_zplus_linear_relprop_ldr(x, in_features, w, derived, r, out_features, out, scratch, rows, in_features,
                                        out_features, ST(stream), y, out_features, bias, te_zplus_from_flags(flags), 0, xabs);

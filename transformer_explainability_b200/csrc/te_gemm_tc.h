@@ -1,23 +1,57 @@
 // Tensor-core (Hopper wgmma) GEMMs of the engines (te_tc_wgmma.cu): TF32 / bf16 / fp16 operands, fp32 accumulation.
 #pragma once
+#include <cuda_bf16.h>
+#include <type_traits>
+
 #include "te_common.cuh"
 #include "te_zplus.h"
 
 // shapes the tensor-core z+ path accepts (in/out multiples of 128, 16-byte aligned rows)
 bool te_tc_zplus_supported(long long rows, int in_features, int out_features, long long ldx);
-// derived copies of one frozen weight W [out,in], all K-major and rounded to TF32:
-//   [ W+ | W- | W+^T | W-^T ]        operands of the z+ rule kernels
-//   [ W_hi | W_lo | W^T_hi | W^T_lo ] error-compensated split (x_hi = tf32(x), x_lo = tf32(x - x_hi)) for the
-//                                     fp32-grade 3xTF32 forward / backward Linear GEMMs
-//   [ |W| ]                          operand of the single-pass S kernel
-//   [ bf16(W+^T) | bf16(W-^T) ]      2-byte operands of the bf16 R kernel
-//   (10 n .. 11 n unused)
-//   [ bf16(|W|) ]                    2-byte operand of the bf16 S1 kernel (TE_FLAG_ZPLUS_S1_BF16), in*out/2 floats
-//   [ fp16 hi | fp16 lo | 2^-f ]     row-scaled fp16 split of W [out,in] for the fp16-split forward GEMM:
-//                                     in*out/2 + in*out/2 + out floats, starting at 11.5*in*out
-//   [ fp16(W^T) | 2^-f ]             row-scaled fp16 of tf32(W)^T [in,out] (single-pass backward Linear): in*out/2 + in floats at 13*in*out
-//   [ fp16(W+^T) | fp16(W-^T) | 2^-f+ | 2^-f- ]   row-scaled fp16 operands of the fp16 R kernel: at 14*in*out, scales at 15*in*out
-// = 16*in*out floats (the tails are padding)
+
+// The derived copies of one frozen weight W [out,in] in its buffer of floats(in, out) = 16 n floats (n = in*out), all K-major.
+// F = float where the copies are made, const float where the kernels read them.  Offsets in floats:
+//   0 .. 4n     W+, W-, W+^T, W-^T rounded to TF32: operands of the two-pass z+ S and the TF32 R kernels
+//   4n .. 8n    W_hi, W_lo, W^T_hi, W^T_lo: error-compensated split (x_hi = tf32(x), x_lo = tf32(x - x_hi)) of the fp32-grade
+//               3xTF32 forward / backward Linear; W^T_hi is also the operand of the single-pass TF32 backward
+//   8n          tf32(|W|): operand of the single-pass S kernel
+//   9n          bf16(W+^T), bf16(W-^T) [in,out]: operands of the bf16 R kernel
+//   10n .. 11n  gap (unused)
+//   11n         bf16(|W|): operand of the bf16 S1 kernel (TE_FLAG_ZPLUS_S1_BF16), n/2 floats
+//   11n + n/2   fp16 hi, fp16 lo of W and the 2^-f of each of its out rows: the fp16-split forward Linear
+//   13n         fp16(tf32(W)^T) and the 2^-f of each of its in rows: the single-pass fp16 backward Linear
+//   14n         fp16(W+^T), fp16(W-^T), then their 2^-f per row (in each, from 15n): the fp16 R kernel
+// What follows each fp16 group up to the next whole multiple of n is tail padding.
+template <class F>
+struct TeDerived {
+    template <class T> using P = std::conditional_t<std::is_const<F>::value, const T*, T*>;
+    F *wp, *wn, *wpt, *wnt;
+    F *wh, *wl, *wth, *wtl;
+    F* wabs;
+    P<__nv_bfloat16> bf_wpt, bf_wnt;
+    F* gap;
+    P<__nv_bfloat16> bf_wabs;
+    P<__half> h_w, l_w;
+    F* s_w;
+    P<__half> h_wt;
+    F* s_wt;
+    P<__half> h_wpt, h_wnt;
+    F *s_wpt, *s_wnt;
+    static constexpr long long floats(int in_features, int out_features) { return 16LL * in_features * out_features; }
+    __host__ __device__ TeDerived(F* d, int in_features, int out_features) {
+        const long long n = (long long)in_features * out_features;
+        wp = d; wn = d + n; wpt = d + 2 * n; wnt = d + 3 * n;
+        wh = d + 4 * n; wl = d + 5 * n; wth = d + 6 * n; wtl = d + 7 * n;
+        wabs = d + 8 * n;
+        bf_wpt = reinterpret_cast<P<__nv_bfloat16>>(d + 9 * n); bf_wnt = bf_wpt + n;
+        gap = d + 10 * n;
+        bf_wabs = reinterpret_cast<P<__nv_bfloat16>>(d + 11 * n);
+        h_w = reinterpret_cast<P<__half>>(d + 11 * n + n / 2); l_w = reinterpret_cast<P<__half>>(d + 12 * n); s_w = d + 12 * n + n / 2;
+        h_wt = reinterpret_cast<P<__half>>(d + 13 * n); s_wt = d + 13 * n + n / 2;
+        h_wpt = reinterpret_cast<P<__half>>(d + 14 * n); h_wnt = reinterpret_cast<P<__half>>(d + 14 * n + n / 2);
+        s_wpt = d + 15 * n; s_wnt = d + 15 * n + in_features;
+    }
+};
 long long te_tc_derived_floats(int in_features, int out_features);
 int te_tc_prepare_weights(const float* w, float* derived, int in_features, int out_features, cudaStream_t st);
 // y / bias (optional): the Linear's saved forward output y = x W^T + bias [rows, out] (row stride ldy).  When given,

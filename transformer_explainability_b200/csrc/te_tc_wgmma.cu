@@ -10,15 +10,21 @@
 //   P::CHUNK > 0: the reduction is cut into chunks of CHUNK k-blocks; each chunk accumulates in its own registers and is
 //   added into fp32 sums with round-to-nearest adds (optionally times a per-row power-of-two block scale), so a long
 //   reduction does not ride on the tensor core's accumulator rounding and block-scaled fp16 operands get their scale.
+//   A problem declares its operand format (P::FMT), its tile width (P::BN) and its products in issue order (P::PRODS);
+//   the stage layout and the wgmma sequence of every k-block follow from those (Stage, issue below).
 //
 // Problems (structs below): the z+ rule's two contractions (two-pass S, single-pass S1, R; TF32, bf16 and block-scaled fp16
-// operand forms), the fp32-grade 3xTF32 and fp16-split Linear GEMMs, the single-pass TF32 / fp16 backward Linear, the
-// attention-shaped N x N and token-reduced N x d contractions and the dense rollout product.
+// operand forms), the Linear GEMMs (3xTF32, single-pass TF32, fp16 split, single-pass fp16), the attention-shaped N x N and
+// token-reduced N x d contractions and the dense rollout product.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <string.h>
+#include <algorithm>
+#include <string>
+#include <type_traits>
+#include <utility>
 
 #include "te_gemm_tc.h"
 #include "te_wgmma.cuh"
@@ -67,6 +73,66 @@ __device__ __forceinline__ uint64_t sdesc(uint32_t saddr) {
 }
 
 constexpr int TILE128 = 128 * 128;                         // bytes of a 128-row operand tile
+
+// ---- products and stage layout ----------------------------------------------------------------------------------------
+// One product of a k-step: accumulator ACC += A tile A times B tile B.  Prods lists a problem's products in issue order; the
+// order of products into one accumulator fixes its rounding, so it is part of the problem's arithmetic.
+template <int ACC, int A, int B>
+struct Pr {
+    static constexpr int acc = ACC, a = A, b = B;
+};
+template <class... T>
+struct Prods {
+    static constexpr int N = sizeof...(T), NACC = 1 + std::max({T::acc...});
+    static constexpr int NTA = 1 + std::max({T::a...}), NTB = 1 + std::max({T::b...});
+    // the first product into its accumulator: the one that takes scale_d (0 starts a sum) on k-step 0
+    __host__ __device__ static constexpr bool first(int i) {
+        constexpr int acc[] = {T::acc...};
+        for (int j = 0; j < i; ++j)
+            if (acc[j] == acc[i]) return false;
+        return true;
+    }
+};
+using One = Prods<Pr<0, 0, 0>>;
+// A = [hi | lo], B = [hi | lo]: hi*hi + lo*hi + hi*lo, the small terms first (3xTF32 and the three-term fp16 split)
+using Split3 = Prods<Pr<0, 1, 0>, Pr<0, 0, 1>, Pr<0, 0, 0>>;
+
+// A stage: the problem's A tiles (BM rows each), then its B tiles (BN rows each); a(i) / b(j) are byte offsets in it.
+template <class PRODS, int BN>
+struct Stage {
+    static constexpr int NTA = PRODS::NTA, NTB = PRODS::NTB;
+    static constexpr int BYTES = NTA * TILE128 + NTB * BN * 128;
+    __host__ __device__ static constexpr uint32_t a(int i) { return (uint32_t)i * TILE128; }
+    __host__ __device__ static constexpr uint32_t b(int j) { return (uint32_t)(NTA * TILE128 + j * BN * 128); }
+};
+
+enum { OP_TF32 = 0, OP_BF16 = 1, OP_F16 = 2 };
+template <int FMT, int NR>
+__device__ __forceinline__ void wgmma_fmt(float (&d)[NR], uint64_t a, uint64_t b, uint32_t scale_d) {
+    if constexpr (FMT == OP_TF32) wgmma_tf32(d, a, b, scale_d);
+    else if constexpr (FMT == OP_BF16) wgmma_bf16(d, a, b, scale_d);
+    else wgmma_f16(d, a, b, scale_d);
+}
+template <int FMT, class... T, size_t... I, int NA, int NR, int TA, int TB>
+__device__ __forceinline__ void issue_kstep(Prods<T...>, std::index_sequence<I...>, float (&acc)[NA][NR], const uint64_t (&a)[TA],
+                                            const uint64_t (&b)[TB], uint64_t q, uint32_t sd) {
+    (wgmma_fmt<FMT>(acc[T::acc], a[T::a] + q, b[T::b] + q, Prods<T...>::first(I) ? sd : 1u), ...);
+}
+// The wgmmas of one k-block (the four 32-byte k-steps of a 128-byte row) on stage st; sd = 0 starts the sums.
+// Warpgroup wg takes rows 64 wg .. 64 wg + 63 of every A tile.
+template <class P, int NA, int NR>
+__device__ __forceinline__ void issue(uint32_t st, int wg, float (&acc)[NA][NR], uint32_t sd) {
+    using L = typename P::L;
+    uint64_t a[L::NTA], b[L::NTB];
+#pragma unroll
+    for (int i = 0; i < L::NTA; ++i) a[i] = sdesc(st + L::a(i) + (uint32_t)wg * 64u * 128u);
+#pragma unroll
+    for (int j = 0; j < L::NTB; ++j) b[j] = sdesc(st + L::b(j));
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+        issue_kstep<P::FMT>(typename P::PRODS{}, std::make_index_sequence<P::PRODS::N>{}, acc, a, b, (uint64_t)(2 * k),
+                            (k == 0) ? sd : 1u);
+}
 
 // ---- operand loaders: each thread handles 16-byte chunks idx = tid, tid + 256, ... of a rows x 128-byte tile ----------
 // fp32 source, K-major: tile row r = source row row0 + r (valid below nrows), chunk c = elements k0 + 4c .. +3 (valid below K).
@@ -137,7 +203,8 @@ __device__ __forceinline__ int frag_col(int tid, int j) { return 8 * (j >> 2) + 
 template <class P>
 __global__ void __launch_bounds__(NTHREADS, 1) wg_kernel(const P p, int col_fast) {
     constexpr int NR = P::BN / 2;
-    constexpr int NA = P::NACC;
+    constexpr int NA = P::PRODS::NACC;
+    constexpr int STAGE = P::L::BYTES;
     constexpr int NT = P::CHUNK ? NA : 1, NTR = P::CHUNK ? NR : 1;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -162,9 +229,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) wg_kernel(const P p, int col_fast
     for (int it = 0; it < kb; ++it) {
         const bool fresh = P::CHUNK ? (it % P::CHUNK == 0) : (it == 0);
         wg_fence();
-        p.mma(smem_u32(smem + (it & 1) * P::STAGE), wg, acc, fresh ? 0u : 1u);
+        issue<P>(smem_u32(smem + (it & 1) * STAGE), wg, acc, fresh ? 0u : 1u);
         wg_commit();
-        if (it + 1 < kb) p.load(smem + ((it + 1) & 1) * P::STAGE, it + 1, m0, n0, z, tid);
+        if (it + 1 < kb) p.load(smem + ((it + 1) & 1) * STAGE, it + 1, m0, n0, z, tid);
         wg_wait0();
         if constexpr (P::CHUNK > 0) {
             if ((it + 1) % P::CHUNK == 0 || it + 1 == kb) {
@@ -195,8 +262,9 @@ struct NoScale {
 enum { ZO_F32 = 0, ZO_BF16 = 1, ZO_F16S = 2 };
 template <bool SINGLE, bool BF, int OUT>
 struct ZsProb : NoScale {
-    static constexpr int BN = 128, NACC = 1, CHUNK = 0;
-    static constexpr int STAGE = SINGLE ? 2 * TILE128 : 4 * TILE128;
+    static constexpr int BN = 128, CHUNK = 0, FMT = BF ? OP_BF16 : OP_TF32;
+    using PRODS = std::conditional_t<SINGLE, One, Prods<Pr<0, 0, 0>, Pr<0, 1, 1>>>;    // two-pass: x+ W+^T, then x- W-^T
+    using L = Stage<PRODS, BN>;
     static constexpr bool COL_FAST = true;
     int M, N, K;
     const float* x; long long ldx;
@@ -208,33 +276,20 @@ struct ZsProb : NoScale {
     __device__ int kblocks() const { return K / (BF ? 64 : 32); }
     __device__ void load(uint8_t* st, int kb, int m0, int n0, int, int tid) const {
         if (BF) {
-            copy_k16(st, BM, (const uint16_t*)xabs, K, m0, M, kb * 64, tid);
-            copy_k16(st + TILE128, BN, (const uint16_t*)wa, K, n0, N, kb * 64, tid);
+            copy_k16(st + L::a(0), BM, (const uint16_t*)xabs, K, m0, M, kb * 64, tid);
+            copy_k16(st + L::b(0), BN, (const uint16_t*)wa, K, n0, N, kb * 64, tid);
             return;
         }
         if (SINGLE) {
-            for_k32(BM, x, ldx, m0, M, kb * 32, K, tid, [&](int rr, int c, float4 v) { st4(st, rr, c, tf32x4(absx4(v))); });
-            for_k32(BN, (const float*)wa, K, n0, N, kb * 32, K, tid, [&](int rr, int c, float4 v) { st4(st + TILE128, rr, c, v); });
+            for_k32(BM, x, ldx, m0, M, kb * 32, K, tid, [&](int rr, int c, float4 v) { st4(st + L::a(0), rr, c, tf32x4(absx4(v))); });
+            for_k32(BN, (const float*)wa, K, n0, N, kb * 32, K, tid, [&](int rr, int c, float4 v) { st4(st + L::b(0), rr, c, v); });
         } else {
             for_k32(BM, x, ldx, m0, M, kb * 32, K, tid, [&](int rr, int c, float4 v) {
-                st4(st, rr, c, tf32x4(posx4(v)));
-                st4(st + TILE128, rr, c, tf32x4(negx4(v)));
+                st4(st + L::a(0), rr, c, tf32x4(posx4(v)));
+                st4(st + L::a(1), rr, c, tf32x4(negx4(v)));
             });
-            for_k32(BN, (const float*)wa, K, n0, N, kb * 32, K, tid, [&](int rr, int c, float4 v) { st4(st + 2 * TILE128, rr, c, v); });
-            for_k32(BN, (const float*)wb, K, n0, N, kb * 32, K, tid, [&](int rr, int c, float4 v) { st4(st + 3 * TILE128, rr, c, v); });
-        }
-    }
-    __device__ void mma(uint32_t st, int wg, float (&acc)[1][BN / 2], uint32_t sd) const {
-        const uint32_t aoff = (uint32_t)wg * 64u * 128u;
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            const uint64_t o = (uint64_t)(2 * k);
-            if (BF) wgmma_bf16(acc[0], sdesc(st + aoff) + o, sdesc(st + TILE128) + o, (k == 0) ? sd : 1u);
-            else if (SINGLE) wgmma_tf32(acc[0], sdesc(st + aoff) + o, sdesc(st + TILE128) + o, (k == 0) ? sd : 1u);
-            else {
-                wgmma_tf32(acc[0], sdesc(st + aoff) + o, sdesc(st + 2 * TILE128) + o, (k == 0) ? sd : 1u);
-                wgmma_tf32(acc[0], sdesc(st + TILE128 + aoff) + o, sdesc(st + 3 * TILE128) + o, 1u);
-            }
+            for_k32(BN, (const float*)wa, K, n0, N, kb * 32, K, tid, [&](int rr, int c, float4 v) { st4(st + L::b(0), rr, c, v); });
+            for_k32(BN, (const float*)wb, K, n0, N, kb * 32, K, tid, [&](int rr, int c, float4 v) { st4(st + L::b(1), rr, c, v); });
         }
     }
     __device__ void epilogue(float (&acc)[1][BN / 2], int m0, int n0, int, int tid) const {
@@ -292,9 +347,10 @@ struct ZsProb : NoScale {
 // KIND 0: S and W+-^T TF32 fp32 ; 1: bf16 ; 2: block-scaled fp16 S (scale per row and 128 k) with row-scaled fp16 W+-^T
 template <int KIND>
 struct ZrProb {
-    static constexpr int BN = (KIND == 2) ? 64 : 128, NACC = 2, CHUNK = (KIND == 2) ? 2 : 0;
-    static constexpr int BT = BN * 128;
-    static constexpr int STAGE = TILE128 + 2 * BT;
+    static constexpr int BN = (KIND == 2) ? 64 : 128, CHUNK = (KIND == 2) ? 2 : 0;
+    static constexpr int FMT = KIND == 0 ? OP_TF32 : KIND == 1 ? OP_BF16 : OP_F16;
+    using PRODS = Prods<Pr<0, 0, 0>, Pr<1, 0, 1>>;           // S W+ and S W- into their own accumulators
+    using L = Stage<PRODS, BN>;
     static constexpr bool COL_FAST = true;
     int M, N, K;
     const void* s; const void* wp; const void* wn;     // S [M, K] (row stride K), W+^T / W-^T [N, K]
@@ -305,24 +361,13 @@ struct ZrProb {
     __device__ float chunk_scale(int row, int ch, int) const { return (KIND == 2 && row < M) ? rs[(long long)row * rs_ld + ch] : 1.f; }
     __device__ void load(uint8_t* st, int kb, int m0, int n0, int, int tid) const {
         if (KIND) {
-            copy_k16(st, BM, (const uint16_t*)s, K, m0, M, kb * 64, tid);
-            copy_k16(st + TILE128, BN, (const uint16_t*)wp, K, n0, N, kb * 64, tid);
-            copy_k16(st + TILE128 + BT, BN, (const uint16_t*)wn, K, n0, N, kb * 64, tid);
+            copy_k16(st + L::a(0), BM, (const uint16_t*)s, K, m0, M, kb * 64, tid);
+            copy_k16(st + L::b(0), BN, (const uint16_t*)wp, K, n0, N, kb * 64, tid);
+            copy_k16(st + L::b(1), BN, (const uint16_t*)wn, K, n0, N, kb * 64, tid);
         } else {
-            for_k32(BM, (const float*)s, K, m0, M, kb * 32, K, tid, [&](int r, int c, float4 v) { st4(st, r, c, v); });
-            for_k32(BN, (const float*)wp, K, n0, N, kb * 32, K, tid, [&](int r, int c, float4 v) { st4(st + TILE128, r, c, v); });
-            for_k32(BN, (const float*)wn, K, n0, N, kb * 32, K, tid, [&](int r, int c, float4 v) { st4(st + TILE128 + BT, r, c, v); });
-        }
-    }
-    __device__ void mma(uint32_t st, int wg, float (&acc)[2][BN / 2], uint32_t sd) const {
-        const uint64_t a = sdesc(st + (uint32_t)wg * 64u * 128u), b0 = sdesc(st + TILE128), b1 = sdesc(st + TILE128 + BT);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            const uint64_t o = (uint64_t)(2 * k);
-            const uint32_t d = (k == 0) ? sd : 1u;
-            if (KIND == 0) { wgmma_tf32(acc[0], a + o, b0 + o, d); wgmma_tf32(acc[1], a + o, b1 + o, d); }
-            else if (KIND == 1) { wgmma_bf16(acc[0], a + o, b0 + o, d); wgmma_bf16(acc[1], a + o, b1 + o, d); }
-            else { wgmma_f16(acc[0], a + o, b0 + o, d); wgmma_f16(acc[1], a + o, b1 + o, d); }
+            for_k32(BM, (const float*)s, K, m0, M, kb * 32, K, tid, [&](int r, int c, float4 v) { st4(st + L::a(0), r, c, v); });
+            for_k32(BN, (const float*)wp, K, n0, N, kb * 32, K, tid, [&](int r, int c, float4 v) { st4(st + L::b(0), r, c, v); });
+            for_k32(BN, (const float*)wn, K, n0, N, kb * 32, K, tid, [&](int r, int c, float4 v) { st4(st + L::b(1), r, c, v); });
         }
     }
     __device__ void epilogue(float (&acc)[2][BN / 2], int m0, int n0, int, int tid) const {
@@ -367,105 +412,59 @@ __device__ __forceinline__ void lin_store(const LinOut& o, int row, int col, flo
     if (EPI == TE_TC_EPI_BIAS_GELU || EPI == TE_TC_EPI_BIAS_ADD) *reinterpret_cast<float2*>(o.C2 + (long long)row * o.ldc2 + col) = y2;
 }
 
-// ---- fp32-grade Linear, 3xTF32: C = A B^T ~ A_hi B_hi^T + A_lo B_hi^T + A_hi B_lo^T (A split on load, B pre-split) -------
-template <int EPI>
-struct Lin3Prob : NoScale {
-    static constexpr int BN = 128, NACC = 1, CHUNK = 4;
-    static constexpr int STAGE = 4 * TILE128;
-    static constexpr bool COL_FAST = true;
-    int K;
-    const float* a; long long lda; const float* bh; const float* bl;
+// ---- Linear GEMMs: C = epi(A B^T), B = the weight copy [N, K] K-major --------------------------------------------------
+// LIN_3XTF32: fp32 grade, A split on load into tf32 hi / lo, B pre-split; Split3 in chunks of 4 k-blocks.
+// LIN_TF32:   single pass (activation-gradient backward): tf32(A) B^T, B rounded once.
+// LIN_F16X3:  fp32 grade on block-scaled fp16 operands (te_common.cuh): A and B pre-split into hi / lo, Split3.
+// LIN_F16:    single pass on the fp16 hi parts.
+// The fp16 forms take one chunk = 128 k = one scale block of A; the columns carry the row scale of B.
+enum { LIN_3XTF32 = 0, LIN_TF32 = 1, LIN_F16X3 = 2, LIN_F16 = 3 };
+struct LinArgs {
+    int K, rs_ld;
+    const void* a; const void* a_lo; long long lda;  // fp32 A [M, K] (row stride lda), or the fp16 hi / lo of A (row stride K)
+    const void* b; const void* b_lo;                 // tf32 or fp16 hi / lo of B
+    const float* rs; const float* cs;                // fp16 forms: the scales of A [M, rs_ld] and of the rows of B [N]
     LinOut o;
-    __device__ int kblocks() const { return K / 32; }
-    __device__ void load(uint8_t* st, int kb, int m0, int n0, int, int tid) const {
-        for_k32(BM, a, lda, m0, o.M, kb * 32, K, tid, [&](int r, int c, float4 v) { st_split(st, st + TILE128, r, c, v); });
-        for_k32(BN, bh, K, n0, o.N, kb * 32, K, tid, [&](int r, int c, float4 v) { st4(st + 2 * TILE128, r, c, v); });
-        for_k32(BN, bl, K, n0, o.N, kb * 32, K, tid, [&](int r, int c, float4 v) { st4(st + 3 * TILE128, r, c, v); });
-    }
-    __device__ void mma(uint32_t st, int wg, float (&acc)[1][BN / 2], uint32_t sd) const {
-        const uint32_t aoff = (uint32_t)wg * 64u * 128u;
-        const uint64_t ah = sdesc(st + aoff), al = sdesc(st + TILE128 + aoff), bhd = sdesc(st + 2 * TILE128), bld = sdesc(st + 3 * TILE128);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            const uint64_t q = (uint64_t)(2 * k);
-            wgmma_tf32(acc[0], al + q, bhd + q, (k == 0) ? sd : 1u);          // small terms first
-            wgmma_tf32(acc[0], ah + q, bld + q, 1u);
-            wgmma_tf32(acc[0], ah + q, bhd + q, 1u);
-        }
-    }
-    __device__ void epilogue(float (&acc)[1][BN / 2], int m0, int n0, int, int tid) const {
-#pragma unroll
-        for (int j = 0; j < BN / 2; j += 2) lin_store<EPI>(o, m0 + frag_row(tid, j), n0 + frag_col(tid, j), acc[0][j], acc[0][j + 1]);
-    }
 };
-
-// ---- single-pass TF32 Linear (activation-gradient backward): C = tf32(A) B^T, B rounded once ---------------------------
-template <int EPI>
-struct Lin1Prob : NoScale {
-    static constexpr int BN = 128, NACC = 1, CHUNK = 0;
-    static constexpr int STAGE = 2 * TILE128;
+// with CUDA 12.9, a 136-byte LinArgs made nvcc read the kernel parameter through a generic pointer, at four more registers
+// in the 3xTF32 kernels; at 128 bytes it is read like the other problems' parameters
+static_assert(sizeof(LinArgs) <= 128, "LinArgs: keep the kernel parameter within 128 bytes");
+template <int EPI, int FORM>
+struct LinProb : LinArgs {
+    static constexpr bool F16 = FORM == LIN_F16X3 || FORM == LIN_F16, SPLIT = FORM == LIN_3XTF32 || FORM == LIN_F16X3;
+    static constexpr int BN = 128, CHUNK = F16 ? 2 : SPLIT ? 4 : 0, FMT = F16 ? OP_F16 : OP_TF32;
+    using PRODS = std::conditional_t<SPLIT, Split3, One>;
+    using L = Stage<PRODS, BN>;
     static constexpr bool COL_FAST = true;
-    int K;
-    const float* a; long long lda; const float* b;
-    LinOut o;
-    __device__ int kblocks() const { return K / 32; }
+    __device__ int kblocks() const { return K / (F16 ? 64 : 32); }
+    __device__ float chunk_scale(int row, int ch, int) const {
+        if constexpr (F16) return row < o.M ? rs[(long long)row * rs_ld + ch] : 1.f;
+        else return 1.f;
+    }
     __device__ void load(uint8_t* st, int kb, int m0, int n0, int, int tid) const {
-        for_k32(BM, a, lda, m0, o.M, kb * 32, K, tid, [&](int r, int c, float4 v) { st4(st, r, c, tf32x4(v)); });
-        for_k32(BN, b, K, n0, o.N, kb * 32, K, tid, [&](int r, int c, float4 v) { st4(st + TILE128, r, c, v); });
-    }
-    __device__ void mma(uint32_t st, int wg, float (&acc)[1][BN / 2], uint32_t sd) const {
-        const uint64_t a0 = sdesc(st + (uint32_t)wg * 64u * 128u), b0 = sdesc(st + TILE128);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) wgmma_tf32(acc[0], a0 + (uint64_t)(2 * k), b0 + (uint64_t)(2 * k), (k == 0) ? sd : 1u);
-    }
-    __device__ void epilogue(float (&acc)[1][BN / 2], int m0, int n0, int, int tid) const {
-#pragma unroll
-        for (int j = 0; j < BN / 2; j += 2)
-            lin_store<EPI, true>(o, m0 + frag_row(tid, j), n0 + frag_col(tid, j), acc[0][j], acc[0][j + 1]);
-    }
-};
-
-// ---- fp16-split Linear: block-scaled fp16 operands (te_common.cuh).  TERMS 3: hi*hi + lo*hi + hi*lo (fp32 grade);
-//      TERMS 1: hi*hi (single pass).  One chunk = 128 k = one activation scale block; the columns carry the weight row scale.
-template <int EPI, int TERMS>
-struct F16Prob {
-    static constexpr int BN = 128, NACC = 1, CHUNK = 2;
-    static constexpr int STAGE = (TERMS == 3 ? 4 : 2) * TILE128;
-    static constexpr bool COL_FAST = true;
-    int K;
-    const __half* ah; const __half* al; const __half* bh; const __half* bl;
-    const float* rs; int rs_ld; const float* cs;
-    LinOut o;
-    __device__ int kblocks() const { return K / 64; }
-    __device__ float chunk_scale(int row, int ch, int) const { return row < o.M ? rs[(long long)row * rs_ld + ch] : 1.f; }
-    __device__ void load(uint8_t* st, int kb, int m0, int n0, int, int tid) const {
-        copy_k16(st, BM, (const uint16_t*)ah, K, m0, o.M, kb * 64, tid);
-        copy_k16(st + TILE128, BN, (const uint16_t*)bh, K, n0, o.N, kb * 64, tid);
-        if (TERMS == 3) {
-            copy_k16(st + 2 * TILE128, BM, (const uint16_t*)al, K, m0, o.M, kb * 64, tid);
-            copy_k16(st + 3 * TILE128, BN, (const uint16_t*)bl, K, n0, o.N, kb * 64, tid);
-        }
-    }
-    __device__ void mma(uint32_t st, int wg, float (&acc)[1][BN / 2], uint32_t sd) const {
-        const uint32_t aoff = (uint32_t)wg * 64u * 128u;
-        const uint64_t a0 = sdesc(st + aoff), b0 = sdesc(st + TILE128), a1 = sdesc(st + 2 * TILE128 + aoff), b1 = sdesc(st + 3 * TILE128);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            const uint64_t q = (uint64_t)(2 * k);
-            if (TERMS == 3) {
-                wgmma_f16(acc[0], a1 + q, b0 + q, (k == 0) ? sd : 1u);
-                wgmma_f16(acc[0], a0 + q, b1 + q, 1u);
-                wgmma_f16(acc[0], a0 + q, b0 + q, 1u);
-            } else {
-                wgmma_f16(acc[0], a0 + q, b0 + q, (k == 0) ? sd : 1u);
+        if constexpr (F16) {
+            copy_k16(st + L::a(0), BM, (const uint16_t*)a, K, m0, o.M, kb * 64, tid);
+            copy_k16(st + L::b(0), BN, (const uint16_t*)b, K, n0, o.N, kb * 64, tid);
+            if constexpr (SPLIT) {
+                copy_k16(st + L::a(1), BM, (const uint16_t*)a_lo, K, m0, o.M, kb * 64, tid);
+                copy_k16(st + L::b(1), BN, (const uint16_t*)b_lo, K, n0, o.N, kb * 64, tid);
             }
+        } else if constexpr (SPLIT) {
+            for_k32(BM, (const float*)a, lda, m0, o.M, kb * 32, K, tid, [&](int r, int c, float4 v) { st_split(st + L::a(0), st + L::a(1), r, c, v); });
+            for_k32(BN, (const float*)b, K, n0, o.N, kb * 32, K, tid, [&](int r, int c, float4 v) { st4(st + L::b(0), r, c, v); });
+            for_k32(BN, (const float*)b_lo, K, n0, o.N, kb * 32, K, tid, [&](int r, int c, float4 v) { st4(st + L::b(1), r, c, v); });
+        } else {
+            for_k32(BM, (const float*)a, lda, m0, o.M, kb * 32, K, tid, [&](int r, int c, float4 v) { st4(st + L::a(0), r, c, tf32x4(v)); });
+            for_k32(BN, (const float*)b, K, n0, o.N, kb * 32, K, tid, [&](int r, int c, float4 v) { st4(st + L::b(0), r, c, v); });
         }
     }
     __device__ void epilogue(float (&acc)[1][BN / 2], int m0, int n0, int, int tid) const {
 #pragma unroll
         for (int j = 0; j < BN / 2; j += 2) {
             const int col = n0 + frag_col(tid, j);
-            lin_store<EPI>(o, m0 + frag_row(tid, j), col, acc[0][j] * cs[col], acc[0][j + 1] * cs[col + 1]);   // exact scaling
+            if constexpr (F16)                                          // exact scaling
+                lin_store<EPI>(o, m0 + frag_row(tid, j), col, acc[0][j] * cs[col], acc[0][j + 1] * cs[col + 1]);
+            else lin_store<EPI, FORM == LIN_TF32>(o, m0 + frag_row(tid, j), col, acc[0][j], acc[0][j + 1]);
         }
     }
 };
@@ -474,9 +473,9 @@ struct F16Prob {
 enum { AT_STORE = 0, AT_MUL = 1, AT_SD = 2, AT_SOFTMAX = 3, AT_RESID = 4 };
 template <int EPI, bool SP, int BN_>
 struct NnProb : NoScale {
-    static constexpr int BN = BN_, NACC = 1, CHUNK = 0;
-    static constexpr int BT = BN * 128;
-    static constexpr int STAGE = SP ? TILE128 + BT : 2 * (TILE128 + BT);
+    static constexpr int BN = BN_, CHUNK = 0, FMT = OP_TF32;
+    using PRODS = std::conditional_t<SP, One, Split3>;
+    using L = Stage<PRODS, BN>;
     static constexpr bool COL_FAST = false;
     int N, H, dh, ld_out, batch;
     const float* a; long long lda; const float* b; long long ldb;
@@ -487,28 +486,13 @@ struct NnProb : NoScale {
         const long long rows = (long long)batch * N;
         const int k0 = h * dh + kb * 32, kend = h * dh + dh;
         if (SP) {
-            for_k32(BM, a, lda, (long long)s * N + m0, rows, k0, kend, tid, [&](int r, int c, float4 v) { st4(st, r, c, tf32x4(v)); });
-            for_k32(BN, b, ldb, (long long)s * N + n0, rows, k0, kend, tid, [&](int r, int c, float4 v) { st4(st + TILE128, r, c, tf32x4(v)); });
+            for_k32(BM, a, lda, (long long)s * N + m0, rows, k0, kend, tid, [&](int r, int c, float4 v) { st4(st + L::a(0), r, c, tf32x4(v)); });
+            for_k32(BN, b, ldb, (long long)s * N + n0, rows, k0, kend, tid, [&](int r, int c, float4 v) { st4(st + L::b(0), r, c, tf32x4(v)); });
         } else {
-            for_k32(BM, a, lda, (long long)s * N + m0, rows, k0, kend, tid, [&](int r, int c, float4 v) { st_split(st, st + TILE128, r, c, v); });
+            for_k32(BM, a, lda, (long long)s * N + m0, rows, k0, kend, tid,
+                    [&](int r, int c, float4 v) { st_split(st + L::a(0), st + L::a(1), r, c, v); });
             for_k32(BN, b, ldb, (long long)s * N + n0, rows, k0, kend, tid,
-                    [&](int r, int c, float4 v) { st_split(st + 2 * TILE128, st + 2 * TILE128 + BT, r, c, v); });
-        }
-    }
-    __device__ void mma(uint32_t st, int wg, float (&acc)[1][BN / 2], uint32_t sd) const {
-        const uint32_t aoff = (uint32_t)wg * 64u * 128u;
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            const uint64_t q = (uint64_t)(2 * k);
-            if (SP) {
-                wgmma_tf32(acc[0], sdesc(st + aoff) + q, sdesc(st + TILE128) + q, (k == 0) ? sd : 1u);
-            } else {
-                const uint64_t ah = sdesc(st + aoff), al = sdesc(st + TILE128 + aoff), bhd = sdesc(st + 2 * TILE128),
-                               bld = sdesc(st + 2 * TILE128 + BT);
-                wgmma_tf32(acc[0], al + q, bhd + q, (k == 0) ? sd : 1u);
-                wgmma_tf32(acc[0], ah + q, bld + q, 1u);
-                wgmma_tf32(acc[0], ah + q, bhd + q, 1u);
-            }
+                    [&](int r, int c, float4 v) { st_split(st + L::b(0), st + L::b(1), r, c, v); });
         }
     }
     __device__ void epilogue(float (&acc)[1][BN / 2], int m0, int n0, int bh, int tid) const {
@@ -573,9 +557,9 @@ struct NnProb : NoScale {
 //   X is MN-major (transposed on load).  a_shared: A indexed by the batch only (dense rollout product, "heads" = column tiles).
 template <int AMN, int EPI, bool SP, int BN_>
 struct NkProb : NoScale {
-    static constexpr int BN = BN_, NACC = 1, CHUNK = SP ? 0 : 4;
-    static constexpr int BT = BN * 128;
-    static constexpr int STAGE = SP ? TILE128 + BT : 2 * (TILE128 + BT);
+    static constexpr int BN = BN_, CHUNK = SP ? 0 : 4, FMT = OP_TF32;
+    using PRODS = std::conditional_t<SP, One, Split3>;
+    using L = Stage<PRODS, BN>;
     static constexpr bool COL_FAST = false;
     int N, H, NP, ld_out, n_out, n_pad, a_shared;
     const float* map; const float* X; long long ldx;
@@ -592,28 +576,12 @@ struct NkProb : NoScale {
         const int s = bh / H, h = bh % H;
         const float* xb = X + (long long)s * N * ldx;
         if (SP) {
-            load_a(kb, m0, bh, tid, [&](int r, int c, float4 v) { st4(st, r, c, tf32x4(v)); });
-            for_mn32(BN, xb, ldx, h * BN, n_pad, kb * 32, N, tid, [&](int r, int c, float4 v) { st4(st + TILE128, r, c, tf32x4(v)); });
+            load_a(kb, m0, bh, tid, [&](int r, int c, float4 v) { st4(st + L::a(0), r, c, tf32x4(v)); });
+            for_mn32(BN, xb, ldx, h * BN, n_pad, kb * 32, N, tid, [&](int r, int c, float4 v) { st4(st + L::b(0), r, c, tf32x4(v)); });
         } else {
-            load_a(kb, m0, bh, tid, [&](int r, int c, float4 v) { st_split(st, st + TILE128, r, c, v); });
+            load_a(kb, m0, bh, tid, [&](int r, int c, float4 v) { st_split(st + L::a(0), st + L::a(1), r, c, v); });
             for_mn32(BN, xb, ldx, h * BN, n_pad, kb * 32, N, tid,
-                     [&](int r, int c, float4 v) { st_split(st + 2 * TILE128, st + 2 * TILE128 + BT, r, c, v); });
-        }
-    }
-    __device__ void mma(uint32_t st, int wg, float (&acc)[1][BN / 2], uint32_t sd) const {
-        const uint32_t aoff = (uint32_t)wg * 64u * 128u;
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            const uint64_t q = (uint64_t)(2 * k);
-            if (SP) {
-                wgmma_tf32(acc[0], sdesc(st + aoff) + q, sdesc(st + TILE128) + q, (k == 0) ? sd : 1u);
-            } else {
-                const uint64_t ah = sdesc(st + aoff), al = sdesc(st + TILE128 + aoff), bhd = sdesc(st + 2 * TILE128),
-                               bld = sdesc(st + 2 * TILE128 + BT);
-                wgmma_tf32(acc[0], al + q, bhd + q, (k == 0) ? sd : 1u);
-                wgmma_tf32(acc[0], ah + q, bld + q, 1u);
-                wgmma_tf32(acc[0], ah + q, bhd + q, 1u);
-            }
+                     [&](int r, int c, float4 v) { st_split(st + L::b(0), st + L::b(1), r, c, v); });
         }
     }
     __device__ void epilogue(float (&acc)[1][BN / 2], int m0, int, int bh, int tid) const {
@@ -652,7 +620,7 @@ template <class P>
 int launch(const P& p, dim3 grid, cudaStream_t st) {
     const int col_fast = P::COL_FAST && grid.x <= 65535;
     if (col_fast) grid = dim3(grid.y, grid.x, grid.z);
-    constexpr int SMEM = 2 * P::STAGE + 1024;
+    constexpr int SMEM = 2 * P::L::BYTES + 1024;
     // cudaFuncAttributeMaxDynamicSharedMemorySize is per device: one bit per device ordinal
     static unsigned long long done = 0;
     int dev = 0;
@@ -673,9 +641,7 @@ inline unsigned mtiles(long long M) { return (unsigned)((M + BM - 1) / BM); }
 
 // ---- weight preparation: W [out,in] -> the derived operand copies of te_gemm_tc.h ------------------------------------
 __global__ void prepare_weights_kernel(const float* __restrict__ w, float* __restrict__ d, int out_f, int in_f) {
-    const long long n = (long long)out_f * in_f;
-    float *wp = d, *wn = d + n, *wpt = d + 2 * n, *wnt = d + 3 * n, *wh = d + 4 * n, *wl = d + 5 * n, *wth = d + 6 * n,
-          *wtl = d + 7 * n, *wa = d + 8 * n;
+    const TeDerived<float> dv(d, in_f, out_f);
     __shared__ float tile[32][33];
     const int bx = blockIdx.x * 32, by = blockIdx.y * 32;      // bx: in index, by: out index
     for (int i = threadIdx.y; i < 32; i += blockDim.y) {
@@ -684,13 +650,13 @@ __global__ void prepare_weights_kernel(const float* __restrict__ w, float* __res
         if (o < out_f && c < in_f) {
             const long long idx = (long long)o * in_f + c;
             v = w[idx];
-            wp[idx] = to_tf32(fmaxf(v, 0.f));
-            wn[idx] = to_tf32(fminf(v, 0.f));
+            dv.wp[idx] = to_tf32(fmaxf(v, 0.f));
+            dv.wn[idx] = to_tf32(fminf(v, 0.f));
             const float hi = to_tf32(v);
-            wh[idx] = hi;
-            wl[idx] = to_tf32(v - hi);
-            wa[idx] = to_tf32(fabsf(v));
-            reinterpret_cast<__nv_bfloat16*>(d + 11 * n)[idx] = __float2bfloat16_rn(fabsf(v));      // bf16(|W|): bf16 S1 kernel
+            dv.wh[idx] = hi;
+            dv.wl[idx] = to_tf32(v - hi);
+            dv.wabs[idx] = to_tf32(fabsf(v));
+            dv.bf_wabs[idx] = __float2bfloat16_rn(fabsf(v));
         }
         tile[i][threadIdx.x] = v;
     }
@@ -700,14 +666,13 @@ __global__ void prepare_weights_kernel(const float* __restrict__ w, float* __res
         if (o < out_f && c < in_f) {
             const float v = tile[threadIdx.x][i];
             const long long idx = (long long)c * out_f + o;
-            wpt[idx] = to_tf32(fmaxf(v, 0.f));
-            wnt[idx] = to_tf32(fminf(v, 0.f));
-            __nv_bfloat16* bp = reinterpret_cast<__nv_bfloat16*>(d + 9 * n);
-            bp[idx] = __float2bfloat16_rn(fmaxf(v, 0.f));
-            bp[n + idx] = __float2bfloat16_rn(fminf(v, 0.f));
+            dv.wpt[idx] = to_tf32(fmaxf(v, 0.f));
+            dv.wnt[idx] = to_tf32(fminf(v, 0.f));
+            dv.bf_wpt[idx] = __float2bfloat16_rn(fmaxf(v, 0.f));
+            dv.bf_wnt[idx] = __float2bfloat16_rn(fminf(v, 0.f));
             const float hi = to_tf32(v);
-            wth[idx] = hi;
-            wtl[idx] = to_tf32(v - hi);
+            dv.wth[idx] = hi;
+            dv.wtl[idx] = to_tf32(v - hi);
         }
     }
 }
@@ -791,23 +756,30 @@ unsigned stride_blocks(long long work, int per_block) {
     return (unsigned)(b < 1 ? 1 : b);
 }
 
-template <int EPI>
-int lin3(const float* a, long long lda, const float* bh, const float* bl, int K, const LinOut& o, cudaStream_t st) {
-    Lin3Prob<EPI> p;
-    p.K = K; p.a = a; p.lda = lda; p.bh = bh; p.bl = bl; p.o = o;
-    return launch(p, dim3(mtiles(o.M), o.N / 128), st);
+// The Linear GEMM of one operand form with the epilogue epi: the forward epilogues (STORE, BIAS, BIAS_GELU, BIAS_ADD) when
+// FWD, else the backward ones (STORE, GELU_BWD).  C [rows, N] = epi(A B^T); bias / e0 / y2 as in te_gemm_tc.h.
+template <int EPI, int FORM>
+int lin_launch(const LinArgs& args, cudaStream_t st) {
+    LinProb<EPI, FORM> p;
+    static_cast<LinArgs&>(p) = args;
+    return launch(p, dim3(mtiles(args.o.M), args.o.N / 128), st);
 }
-template <int EPI, int TERMS>
-int f16(const __half* ah, const __half* al, const __half* bh, const __half* bl, const float* rs, const float* cs, int K,
-        const LinOut& o, cudaStream_t st) {
-    F16Prob<EPI, TERMS> p;
-    p.K = K; p.ah = ah; p.al = al; p.bh = bh; p.bl = bl; p.rs = rs; p.rs_ld = (K + 127) / 128; p.cs = cs; p.o = o;
-    return launch(p, dim3(mtiles(o.M), o.N / 128), st);
-}
-LinOut lin_out(long long rows, int N, const float* bias, const float* e0, float* y, float* y2) {
-    LinOut o;
-    o.M = (int)rows; o.N = N; o.bias = bias; o.E = e0; o.lde = N; o.C = y; o.ldc = N; o.C2 = y2; o.ldc2 = N;
-    return o;
+template <int FORM, bool FWD>
+int linear(int K, const void* a, const void* a_lo, long long lda, const void* b, const void* b_lo, const float* rs,
+           const float* cs, long long rows, int N, const float* bias, const float* e0, float* y, float* y2, int epi,
+           const char* who, cudaStream_t st) {
+    LinArgs g;
+    g.K = K; g.a = a; g.a_lo = a_lo; g.lda = lda; g.b = b; g.b_lo = b_lo; g.rs = rs; g.rs_ld = (K + 127) / 128; g.cs = cs;
+    g.o.M = (int)rows; g.o.N = N; g.o.bias = bias; g.o.E = e0; g.o.lde = N; g.o.C = y; g.o.ldc = N; g.o.C2 = y2; g.o.ldc2 = N;
+    switch (epi) {
+        case TE_TC_EPI_STORE: return lin_launch<TE_TC_EPI_STORE, FORM>(g, st);
+        case TE_TC_EPI_BIAS: if constexpr (FWD) return lin_launch<TE_TC_EPI_BIAS, FORM>(g, st); break;
+        case TE_TC_EPI_BIAS_GELU: if constexpr (FWD) return lin_launch<TE_TC_EPI_BIAS_GELU, FORM>(g, st); break;
+        case TE_TC_EPI_BIAS_ADD: if constexpr (FWD) return lin_launch<TE_TC_EPI_BIAS_ADD, FORM>(g, st); break;
+        case TE_TC_EPI_GELU_BWD: if constexpr (!FWD) return lin_launch<TE_TC_EPI_GELU_BWD, FORM>(g, st); break;
+    }
+    te_set_last_error((std::string(who) + ": unsupported epilogue").c_str());
+    return TE_ERR_UNSUPPORTED;
 }
 
 // S = sd(R, Z) [rows, out] on the z+ S kernel.  Single-pass: wa = |W| (xabs = bf16(|x|) with BF); two-pass: wa / wb = W+ / W-.
@@ -829,23 +801,19 @@ int zs(const float* x, long long ldx, const void* xabs, const void* wa, const vo
 // =====================================================================================================================
 // public entry points (te_gemm_tc.h)
 // =====================================================================================================================
-long long te_tc_derived_floats(int in_features, int out_features) { return 16LL * in_features * out_features; }
+long long te_tc_derived_floats(int in_features, int out_features) { return TeDerived<float>::floats(in_features, out_features); }
 
 int te_tc_prepare_weights(const float* w, float* derived, int in_features, int out_features, cudaStream_t st) {
     dim3 grid((in_features + 31) / 32, (out_features + 31) / 32), block(32, 8);
     prepare_weights_kernel<<<grid, block, 0, st>>>(w, derived, out_features, in_features);
     TE_CUDA_CHECK_LAUNCH();
-    const long long n = (long long)in_features * out_features;
-    if (in_features % 8 == 0 && in_features >= 8 && a16(w))        // row-scaled fp16 split: [hi | lo | 2^-f] from 11.5 n
-        TE_TRY(te_tc_rowsplit_f16(w, in_features, out_features, in_features, derived + 11 * n + n / 2, derived + 12 * n,
-                                  derived + 12 * n + n / 2, st));
+    const TeDerived<float> dv(derived, in_features, out_features);
+    if (in_features % 8 == 0 && in_features >= 8 && a16(w))        // row-scaled fp16 split of W
+        TE_TRY(te_tc_rowsplit_f16(w, in_features, out_features, in_features, dv.h_w, dv.l_w, dv.s_w, st));
     if (out_features % 8 == 0 && in_features >= 2) {               // single-pass fp16 operands from the TF32-rounded transposes [in, out]
-        TE_TRY(te_tc_rowsplit_f16(derived + 6 * n, out_features, in_features, out_features, derived + 13 * n, nullptr,
-                                  derived + 13 * n + n / 2, st));
-        TE_TRY(te_tc_rowsplit_f16(derived + 2 * n, out_features, in_features, out_features, derived + 14 * n, nullptr,
-                                  derived + 15 * n, st));
-        TE_TRY(te_tc_rowsplit_f16(derived + 3 * n, out_features, in_features, out_features, derived + 14 * n + n / 2, nullptr,
-                                  derived + 15 * n + in_features, st));
+        TE_TRY(te_tc_rowsplit_f16(dv.wth, out_features, in_features, out_features, dv.h_wt, nullptr, dv.s_wt, st));
+        TE_TRY(te_tc_rowsplit_f16(dv.wpt, out_features, in_features, out_features, dv.h_wpt, nullptr, dv.s_wpt, st));
+        TE_TRY(te_tc_rowsplit_f16(dv.wnt, out_features, in_features, out_features, dv.h_wnt, nullptr, dv.s_wnt, st));
     }
     return TE_OK;
 }
@@ -882,13 +850,13 @@ bool te_tc_zplus_supported(long long rows, int in_features, int out_features, lo
 int te_tc_zplus_s1(const float* x, long long ldx, float* xabs, const float* derived, const float* r, long long ldr,
                    const float* y, long long ldy, const float* bias, float* s_out, long long rows, int in_features,
                    int out_features, cudaStream_t st, bool bf16, float* s16, float* s16_scale) {
-    const long long n = (long long)in_features * out_features;
+    const TeDerived<const float> dv(derived, in_features, out_features);
     if (ldx % 4 != 0 || !a16(x) || !a16(r) || !a16(y) || ldr % 2 != 0 || ldy % 2 != 0) {
         te_set_last_error("te_tc_zplus_s1: alignment");
         return TE_ERR_ARG;
     }
     void* o = s16 ? (void*)s16 : (void*)s_out;
-    auto run = [&](auto zs_fn, const float* wa) {
+    auto run = [&](auto zs_fn, const void* wa) {
         return zs_fn(x, ldx, xabs, wa, nullptr, r, ldr, y, ldy, bias, o, s16_scale, rows, in_features, out_features, st);
     };
     if (bf16 && in_features % 64 == 0) {
@@ -896,24 +864,24 @@ int te_tc_zplus_s1(const float* x, long long ldx, float* xabs, const float* deri
         abs_bf16_kernel<<<stride_blocks(rows * (in_features / 4), 256), 256, 0, st>>>(
             x, ldx, reinterpret_cast<__nv_bfloat16*>(xabs), rows, in_features / 4);
         TE_CUDA_CHECK_LAUNCH();
-        return s16 ? run(zs<true, true, ZO_F16S>, derived + 11 * n) : run(zs<true, true, ZO_F32>, derived + 11 * n);
+        return s16 ? run(zs<true, true, ZO_F16S>, dv.bf_wabs) : run(zs<true, true, ZO_F32>, dv.bf_wabs);
     }
-    return s16 ? run(zs<true, false, ZO_F16S>, derived + 8 * n) : run(zs<true, false, ZO_F32>, derived + 8 * n);
+    return s16 ? run(zs<true, false, ZO_F16S>, dv.wabs) : run(zs<true, false, ZO_F32>, dv.wabs);
 }
 
 int te_tc_zplus_r(const float* s, const float* derived, const float* x, long long ldx, float* out, long long ld_out,
                   long long rows, int in_features, int out_features, cudaStream_t st) {
-    const long long n = (long long)in_features * out_features;
+    const TeDerived<const float> dv(derived, in_features, out_features);
     ZrProb<0> p;
     memset(&p, 0, sizeof(p));
     p.M = (int)rows; p.N = in_features; p.K = out_features;
-    p.s = s; p.wp = derived + 2 * n; p.wn = derived + 3 * n; p.x = x; p.ldx = ldx; p.out = out; p.ldo = ld_out;
+    p.s = s; p.wp = dv.wpt; p.wn = dv.wnt; p.x = x; p.ldx = ldx; p.out = out; p.ldo = ld_out;
     return launch(p, dim3(mtiles(rows), in_features / 128), st);
 }
 
 int te_tc_zplus_r16(const float* s, float* split, float* scale, const float* derived, const float* x, long long ldx, float* out,
                     long long ld_out, long long rows, int in_features, int out_features, cudaStream_t st) {
-    const long long n = (long long)in_features * out_features;
+    const TeDerived<const float> dv(derived, in_features, out_features);
     if (!a16(split) || !scale || !a16(derived) || !a16(x) || !a16(out) || ldx % 4 != 0 || ld_out % 4 != 0) {
         te_set_last_error("te_tc_zplus_r16: bad operands");
         return TE_ERR_ARG;
@@ -921,8 +889,8 @@ int te_tc_zplus_r16(const float* s, float* split, float* scale, const float* der
     if (s) TE_TRY(te_tc_blocksplit_f16(s, out_features, rows, out_features, split, scale, st, true));
     ZrProb<2> p;
     p.M = (int)rows; p.N = in_features; p.K = out_features;
-    p.s = split; p.wp = derived + 14 * n; p.wn = derived + 14 * n + n / 2;
-    p.rs = scale; p.rs_ld = (out_features + 127) / 128; p.cp = derived + 15 * n; p.cn = derived + 15 * n + in_features;
+    p.s = split; p.wp = dv.h_wpt; p.wn = dv.h_wnt;
+    p.rs = scale; p.rs_ld = (out_features + 127) / 128; p.cp = dv.s_wpt; p.cn = dv.s_wnt;
     p.x = x; p.ldx = ldx; p.out = out; p.ldo = ld_out;
     return launch(p, dim3(mtiles(rows), in_features / 64), st);
 }
@@ -935,7 +903,7 @@ int te_tc_zplus_linear_relprop(const float* x, long long ldx, const float* deriv
         te_set_last_error("te_gemm_tc: operands must be 16-byte aligned");
         return TE_ERR_ARG;
     }
-    const long long n = (long long)in_features * out_features;
+    const TeDerived<const float> dv(derived, in_features, out_features);
     const bool single = y && a16(y) && ldy % 4 == 0 && (!bias || a16(bias));
     const bool rb = zv.r_bf16 && (out_features % 64 == 0);          // S as bf16, R kernel with bf16 operands
     if (!rb && single && xabs && a16(xabs)) {
@@ -953,9 +921,9 @@ int te_tc_zplus_linear_relprop(const float* x, long long ldx, const float* deriv
     }
     // S = sd(R, Z) [rows, out]: single-pass from y, or two-pass
     auto run = [&](auto zs_fn) {
-        return single ? zs_fn(x, ldx, nullptr, derived + 8 * n, nullptr, r, ldr, y, ldy, bias, s_scratch, nullptr, rows,
+        return single ? zs_fn(x, ldx, nullptr, dv.wabs, nullptr, r, ldr, y, ldy, bias, s_scratch, nullptr, rows,
                               in_features, out_features, st)
-                      : zs_fn(x, ldx, nullptr, derived, derived + n, r, ldr, nullptr, 0, nullptr, s_scratch, nullptr, rows,
+                      : zs_fn(x, ldx, nullptr, dv.wp, dv.wn, r, ldr, nullptr, 0, nullptr, s_scratch, nullptr, rows,
                               in_features, out_features, st);
     };
     if (single) TE_TRY(rb ? run(zs<true, false, ZO_BF16>) : run(zs<true, false, ZO_F32>));
@@ -964,7 +932,7 @@ int te_tc_zplus_linear_relprop(const float* x, long long ldx, const float* deriv
         ZrProb<1> p;
         memset(&p, 0, sizeof(p));
         p.M = (int)rows; p.N = in_features; p.K = out_features;
-        p.s = s_scratch; p.wp = derived + 9 * n; p.wn = (const __nv_bfloat16*)(derived + 9 * n) + n;
+        p.s = s_scratch; p.wp = dv.bf_wpt; p.wn = dv.bf_wnt;
         p.x = x; p.ldx = ldx; p.out = out; p.ldo = ld_out;
         return launch(p, dim3(mtiles(rows), in_features / 128), st);
     }
@@ -978,56 +946,35 @@ bool te_tc_gemm3x_supported(long long rows, int K, int N, long long lda) {
 
 int te_tc_linear_fwd(const float* x, long long ldx, const float* derived, int in_features, int out_features, const float* bias,
                      float* y, float* y2, const float* e0, long long rows, int epi, cudaStream_t st) {
-    const long long n = (long long)in_features * out_features;
     if (!a16(x) || !a16(derived) || !a16(y) || (y2 && !a16(y2)) || (e0 && !a16(e0)) || (bias && !a16(bias))) {
         te_set_last_error("te_tc_linear_fwd: operands must be 16-byte aligned");
         return TE_ERR_ARG;
     }
-    const LinOut o = lin_out(rows, out_features, bias, e0, y, y2);
-    const float *bh = derived + 4 * n, *bl = derived + 5 * n;
-    switch (epi) {
-        case TE_TC_EPI_STORE: return lin3<TE_TC_EPI_STORE>(x, ldx, bh, bl, in_features, o, st);
-        case TE_TC_EPI_BIAS: return lin3<TE_TC_EPI_BIAS>(x, ldx, bh, bl, in_features, o, st);
-        case TE_TC_EPI_BIAS_GELU: return lin3<TE_TC_EPI_BIAS_GELU>(x, ldx, bh, bl, in_features, o, st);
-        case TE_TC_EPI_BIAS_ADD: return lin3<TE_TC_EPI_BIAS_ADD>(x, ldx, bh, bl, in_features, o, st);
-    }
-    te_set_last_error("te_tc_linear_fwd: unsupported epilogue");
-    return TE_ERR_UNSUPPORTED;
+    const TeDerived<const float> dv(derived, in_features, out_features);
+    return linear<LIN_3XTF32, true>(in_features, x, nullptr, ldx, dv.wh, dv.wl, nullptr, nullptr, rows, out_features, bias, e0, y,
+                                    y2, epi, "te_tc_linear_fwd", st);
 }
 
 int te_tc_linear_bwd(const float* dy, const float* derived, int in_features, int out_features, float* dx, const float* e0,
                      long long rows, int epi, cudaStream_t st) {
-    const long long n = (long long)in_features * out_features;
     if (!a16(dy) || !a16(derived) || !a16(dx) || (e0 && !a16(e0))) {
         te_set_last_error("te_tc_linear_bwd: operands must be 16-byte aligned");
         return TE_ERR_ARG;
     }
-    const LinOut o = lin_out(rows, in_features, nullptr, e0, dx, nullptr);
-    if (epi == TE_TC_EPI_STORE) return lin3<TE_TC_EPI_STORE>(dy, out_features, derived + 6 * n, derived + 7 * n, out_features, o, st);
-    if (epi == TE_TC_EPI_GELU_BWD) return lin3<TE_TC_EPI_GELU_BWD>(dy, out_features, derived + 6 * n, derived + 7 * n, out_features, o, st);
-    te_set_last_error("te_tc_linear_bwd: unsupported epilogue");
-    return TE_ERR_UNSUPPORTED;
+    const TeDerived<const float> dv(derived, in_features, out_features);
+    return linear<LIN_3XTF32, false>(out_features, dy, nullptr, out_features, dv.wth, dv.wtl, nullptr, nullptr, rows, in_features,
+                                     nullptr, e0, dx, nullptr, epi, "te_tc_linear_bwd", st);
 }
 
 int te_tc_linear_bwd_tf32(const float* dy, long long lddy, const float* derived, int in_features, int out_features, float* dx,
                           const float* e0, long long rows, int epi, cudaStream_t st) {
-    const long long n = (long long)in_features * out_features;
     if (!a16(dy) || lddy % 4 != 0 || !a16(derived) || !a16(dx) || (e0 && !a16(e0))) {
         te_set_last_error("te_tc_linear_bwd_tf32: operands must be 16-byte aligned");
         return TE_ERR_ARG;
     }
-    const LinOut o = lin_out(rows, in_features, nullptr, e0, dx, nullptr);
-    const dim3 grid(mtiles(rows), in_features / 128);
-    if (epi == TE_TC_EPI_STORE) {
-        Lin1Prob<TE_TC_EPI_STORE> p; p.K = out_features; p.a = dy; p.lda = lddy; p.b = derived + 6 * n; p.o = o;
-        return launch(p, grid, st);
-    }
-    if (epi == TE_TC_EPI_GELU_BWD) {
-        Lin1Prob<TE_TC_EPI_GELU_BWD> p; p.K = out_features; p.a = dy; p.lda = lddy; p.b = derived + 6 * n; p.o = o;
-        return launch(p, grid, st);
-    }
-    te_set_last_error("te_tc_linear_bwd_tf32: unsupported epilogue");
-    return TE_ERR_UNSUPPORTED;
+    const TeDerived<const float> dv(derived, in_features, out_features);
+    return linear<LIN_TF32, false>(out_features, dy, nullptr, lddy, dv.wth, nullptr, nullptr, nullptr, rows, in_features, nullptr,
+                                   e0, dx, nullptr, epi, "te_tc_linear_bwd_tf32", st);
 }
 
 bool te_tc_fwd16_supported(long long rows, int K, int N, long long lda) {
@@ -1037,7 +984,6 @@ bool te_tc_fwd16_supported(long long rows, int K, int N, long long lda) {
 int te_tc_linear_fwd16(const float* x, long long ldx, float* split, float* scale, const float* derived, int in_features,
                        int out_features, const float* bias, float* y, float* y2, const float* e0, long long rows, int epi,
                        cudaStream_t st, float* split_out, float* scale_out) {
-    const long long n = (long long)in_features * out_features;
     if (!a16(split) || !scale || !a16(derived) || !a16(y) || (y2 && !a16(y2)) || (e0 && !a16(e0)) || (bias && !a16(bias)) ||
         (split_out && (!a16(split_out) || !scale_out || !y2 || epi != TE_TC_EPI_BIAS_GELU))) {
         te_set_last_error("te_tc_linear_fwd16: bad operands");
@@ -1046,40 +992,24 @@ int te_tc_linear_fwd16(const float* x, long long ldx, float* split, float* scale
     const __half* ah = reinterpret_cast<const __half*>(split);
     const __half* al = ah + rows * in_features;
     if (x) TE_TRY(te_tc_blocksplit_f16(x, ldx, rows, in_features, split, scale, st));
-    const __half* bh = reinterpret_cast<const __half*>(derived + 11 * n + n / 2);
-    const __half* bl = reinterpret_cast<const __half*>(derived + 12 * n);
-    const float* cs = derived + 12 * n + n / 2;
-    const LinOut o = lin_out(rows, out_features, bias, e0, y, y2);
-    switch (epi) {
-        case TE_TC_EPI_STORE: return f16<TE_TC_EPI_STORE, 3>(ah, al, bh, bl, scale, cs, in_features, o, st);
-        case TE_TC_EPI_BIAS: return f16<TE_TC_EPI_BIAS, 3>(ah, al, bh, bl, scale, cs, in_features, o, st);
-        case TE_TC_EPI_BIAS_GELU:
-            TE_TRY((f16<TE_TC_EPI_BIAS_GELU, 3>(ah, al, bh, bl, scale, cs, in_features, o, st)));
-            // the next Linear's A operand: the block-scaled split of y2 = gelu(y)
-            if (split_out) return te_tc_blocksplit_f16(y2, out_features, rows, out_features, split_out, scale_out, st);
-            return TE_OK;
-        case TE_TC_EPI_BIAS_ADD: return f16<TE_TC_EPI_BIAS_ADD, 3>(ah, al, bh, bl, scale, cs, in_features, o, st);
-    }
-    te_set_last_error("te_tc_linear_fwd16: unsupported epilogue");
-    return TE_ERR_UNSUPPORTED;
+    const TeDerived<const float> dv(derived, in_features, out_features);
+    TE_TRY((linear<LIN_F16X3, true>(in_features, ah, al, in_features, dv.h_w, dv.l_w, scale, dv.s_w, rows, out_features, bias, e0,
+                                    y, y2, epi, "te_tc_linear_fwd16", st)));
+    // the next Linear's A operand (BIAS_GELU only): the block-scaled split of y2 = gelu(y)
+    if (split_out) return te_tc_blocksplit_f16(y2, out_features, rows, out_features, split_out, scale_out, st);
+    return TE_OK;
 }
 
 int te_tc_linear_bwd16(const float* dy, long long lddy, float* split, float* scale, const float* derived, int in_features,
                        int out_features, float* dx, const float* e0, long long rows, int epi, cudaStream_t st) {
-    const long long n = (long long)in_features * out_features;
     if (!a16(split) || !scale || !a16(derived) || !a16(dx) || (e0 && !a16(e0))) {
         te_set_last_error("te_tc_linear_bwd16: bad operands");
         return TE_ERR_ARG;
     }
     if (dy) TE_TRY(te_tc_blocksplit_f16(dy, lddy, rows, out_features, split, scale, st, true));
-    const __half* ah = reinterpret_cast<const __half*>(split);
-    const __half* bt = reinterpret_cast<const __half*>(derived + 13 * n);
-    const float* cs = derived + 13 * n + n / 2;
-    const LinOut o = lin_out(rows, in_features, nullptr, e0, dx, nullptr);
-    if (epi == TE_TC_EPI_GELU_BWD) return f16<TE_TC_EPI_GELU_BWD, 1>(ah, nullptr, bt, nullptr, scale, cs, out_features, o, st);
-    if (epi == TE_TC_EPI_STORE) return f16<TE_TC_EPI_STORE, 1>(ah, nullptr, bt, nullptr, scale, cs, out_features, o, st);
-    te_set_last_error("te_tc_linear_bwd16: unsupported epilogue");
-    return TE_ERR_UNSUPPORTED;
+    const TeDerived<const float> dv(derived, in_features, out_features);
+    return linear<LIN_F16, false>(out_features, split, nullptr, out_features, dv.h_wt, nullptr, scale, dv.s_wt, rows, in_features,
+                                  nullptr, e0, dx, nullptr, epi, "te_tc_linear_bwd16", st);
 }
 
 // ---- attention-shaped contractions -------------------------------------------------------------------------------------

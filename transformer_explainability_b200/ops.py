@@ -60,6 +60,22 @@ def _workspace(nbytes, device):
     return torch.empty((nbytes + 255) // 256 * 64, dtype=torch.float32, device=device)   # 256-byte multiple
 
 
+def _up64(n):
+    return (n + 63) // 64 * 64
+
+
+def _tc_scratch(w, device, s=0, operand=0, split=None):
+    """The scratch of the tensor-core stand-alone entry points for the weight w [out, in], laid out as include/te_b200.h
+    documents it: [s floats of S, rounded up to 64 | 16 * in * out derived weight copies | operand floats], or with
+    split = (rows, cols, hi_only) the fp16 split of a [rows, cols] operand, rounded up to 64, and its rows * ceil(cols / 128)
+    block scales in place of the operand."""
+    n = _up64(s) + 16 * w.numel() + operand
+    if split is not None:
+        rows, cols, hi_only = split
+        n += _up64(rows * cols // 2 if hi_only else rows * cols) + rows * ((cols + 127) // 128)
+    return torch.empty(n, device=device, dtype=torch.float32)
+
+
 @_on_device
 def linear_forward(x, w, bias=None, tensor_cores=False, f16_split=False):
     """y = x W^T + b.  tensor_cores: fp32-grade 3xTF32 split on the tensor cores (shapes that do not qualify fall back);
@@ -69,8 +85,7 @@ def linear_forward(x, w, bias=None, tensor_cores=False, f16_split=False):
         raise ValueError("linear_forward: x [...,in], w [out,in], bias [out] expected")
     rows = x.numel() // x.shape[-1]
     y = torch.empty(*x.shape[:-1], w.shape[0], device=x.device, dtype=torch.float32)
-    nscratch = 16 * w.numel() + ((x.numel() + 63) // 64 * 64 + rows * ((x.shape[-1] + 127) // 128) if f16_split else 0)
-    scratch = torch.empty(nscratch, device=x.device, dtype=torch.float32) if tensor_cores else None
+    scratch = _tc_scratch(w, x.device, split=(rows, x.shape[-1], False) if f16_split else None) if tensor_cores else None
     flags = (_lib.FLAG_LINEAR_TENSOR_CORES if tensor_cores else 0) | (_lib.FLAG_LINEAR_F16_SPLIT if f16_split else 0)
     check(_lib.load().te_linear_forward_ex(ptr(x), ptr(w), ptr(bias), ptr(y), ptr(scratch), rows, x.shape[-1], w.shape[0],
                                            flags, _stream()),
@@ -100,7 +115,7 @@ def linear_backward(dy, w, tensor_cores=False):
         raise ValueError("linear_backward: dy [...,out], w [out,in] expected")
     rows = dy.numel() // dy.shape[-1]
     dx = torch.empty(*dy.shape[:-1], w.shape[1], device=dy.device, dtype=torch.float32)
-    scratch = torch.empty(16 * w.numel(), device=dy.device, dtype=torch.float32) if tensor_cores else None
+    scratch = _tc_scratch(w, dy.device) if tensor_cores else None
     check(_lib.load().te_linear_backward_ex(ptr(dy), ptr(w), ptr(dx), ptr(scratch), rows, w.shape[1], w.shape[0],
                                             _lib.FLAG_LINEAR_TENSOR_CORES if tensor_cores else 0, _stream()),
           "te_linear_backward_ex")
@@ -115,8 +130,7 @@ def linear_backward_f16(dy, w):
         raise ValueError("linear_backward_f16: dy [...,out], w [out,in] expected")
     rows = dy.numel() // dy.shape[-1]
     dx = torch.empty(*dy.shape[:-1], w.shape[1], device=dy.device, dtype=torch.float32)
-    n = 16 * w.numel() + (dy.numel() // 2 + 63) // 64 * 64 + rows * ((w.shape[0] + 127) // 128)
-    scratch = torch.empty(n, device=dy.device, dtype=torch.float32)
+    scratch = _tc_scratch(w, dy.device, split=(rows, w.shape[0], True))
     check(_lib.load().te_linear_backward_ex(ptr(dy), ptr(w), ptr(dx), ptr(scratch), rows, w.shape[1], w.shape[0],
                                             _lib.FLAG_LINEAR_TENSOR_CORES | _lib.FLAG_BACKWARD_F16, _stream()),
           "te_linear_backward_ex")
@@ -131,7 +145,7 @@ def linear_backward_tf32(dy, w):
         raise ValueError("linear_backward_tf32: dy [...,out], w [out,in] expected")
     rows = dy.numel() // dy.shape[-1]
     dx = torch.empty(*dy.shape[:-1], w.shape[1], device=dy.device, dtype=torch.float32)
-    scratch = torch.empty(16 * w.numel(), device=dy.device, dtype=torch.float32)
+    scratch = _tc_scratch(w, dy.device)
     check(_lib.load().te_linear_backward_ex(ptr(dy), ptr(w), ptr(dx), ptr(scratch), rows, w.shape[1], w.shape[0],
                                             _lib.FLAG_LINEAR_TENSOR_CORES | _lib.FLAG_BACKWARD_TF32, _stream()),
           "te_linear_backward_ex")
@@ -162,8 +176,7 @@ def linear_forward_epi(x, w, bias=None, e0=None, epi="bias", family="simt"):
     flags = LINEAR_FAMILIES[family]
     y = torch.empty(rows, N, device=x.device, dtype=torch.float32)
     y2 = torch.empty_like(y) if epi in ("bias_gelu", "bias_add") else None
-    nscratch = 16 * w.numel() + ((rows * K + 63) // 64 * 64 + rows * ((K + 127) // 128) if family == "f16_split" else 0)
-    scratch = torch.empty(nscratch, device=x.device, dtype=torch.float32) if flags else None
+    scratch = _tc_scratch(w, x.device, split=(rows, K, False) if family == "f16_split" else None) if flags else None
     check(_lib.load().te_linear_forward_epi(ptr(x), ptr(w), ptr(bias), ptr(e0), ptr(y), ptr(y2), ptr(scratch), rows, K, N,
                                             LINEAR_EPI[epi], flags, _stream()), "te_linear_forward_epi")
     return y, y2
@@ -178,8 +191,7 @@ def linear_backward_epi(dy, w, e0=None, epi="store", family="simt"):
     rows, K, N = dy.shape[0], w.shape[0], w.shape[1]
     flags = LINEAR_FAMILIES[family]
     dx = torch.empty(rows, N, device=dy.device, dtype=torch.float32)
-    nscratch = 16 * w.numel() + ((rows * K // 2 + 63) // 64 * 64 + rows * ((K + 127) // 128) if family == "f16" else 0)
-    scratch = torch.empty(nscratch, device=dy.device, dtype=torch.float32) if flags else None
+    scratch = _tc_scratch(w, dy.device, split=(rows, K, True) if family == "f16" else None) if flags else None
     check(_lib.load().te_linear_backward_epi(ptr(dy), ptr(w), ptr(e0), ptr(dx), ptr(scratch), rows, N, K, LINEAR_EPI[epi],
                                              flags, _stream()), "te_linear_backward_epi")
     return dx
@@ -209,7 +221,7 @@ def tc_zplus_s(x, w, r, y, bias=None, f16=False, bf16=False):
     if x.dim() != 2 or w.dim() != 2 or w.shape[1] != x.shape[1] or r.shape != y.shape or r.shape != (x.shape[0], w.shape[0]):
         raise ValueError("tc_zplus_s: x [rows,in], w [out,in], r / y [rows,out] expected")
     rows, K, N = x.shape[0], x.shape[1], w.shape[0]
-    scratch = torch.empty(16 * w.numel() + rows * K, device=x.device, dtype=torch.float32)
+    scratch = _tc_scratch(w, x.device, operand=rows * K)
     s = None if f16 else torch.empty(rows, N, device=x.device, dtype=torch.float32)
     s16 = torch.empty(rows, N, device=x.device, dtype=torch.float16) if f16 else None
     sc = torch.full((rows, N // 128), float("nan"), device=x.device, dtype=torch.float32) if f16 else None
@@ -265,10 +277,10 @@ def linear_relprop(x, w, r, tensor_cores=False, y=None, bias=None, bf16=False, v
         raise ValueError("linear_relprop: x [...,in], w [out,in], r / y [...,out], bias [out] expected")
     rows = x.numel() // x.shape[-1]
     out = torch.empty_like(x)
-    nscratch = rows * w.shape[0]
     if tensor_cores:
-        nscratch = (nscratch + 63) // 64 * 64 + 16 * w.numel() + x.numel()
-    scratch = torch.empty(nscratch, device=x.device, dtype=torch.float32)
+        scratch = _tc_scratch(w, x.device, s=rows * w.shape[0], operand=x.numel())
+    else:
+        scratch = torch.empty(rows * w.shape[0], device=x.device, dtype=torch.float32)
     flags = _lib.FLAG_ZPLUS_TENSOR_CORES if tensor_cores else 0
     if r_f16:
         flags |= _lib.FLAG_ZPLUS_R_F16
