@@ -65,7 +65,14 @@ extern "C" {
                                          * (TE_FLAG_BACKWARD_TF32): same 11 significant bits, twice the tensor rate */
 #define TE_FLAG_RULES_LRP 512u         /* the rule library of modules/layers_lrp.py (baselines/ViT/ViT_orig_LRP.py) instead of
                                          modules/layers_ours.py: Linear divides its two halves by their OWN denominators
-                                         (layers_lrp.py:199-200), Add has no ratio normalisation (:98-100).  fp32 SIMT rules. */
+                                         (layers_lrp.py:199-200), Add has no ratio normalisation (:98-100).  fp32 SIMT rules
+                                         unless TE_FLAG_RULES_LRP_TC.  te_vit_attribute (ViT_orig_LRP) and te_bert_attribute
+                                         (BERT_cls_lrp.py on BERT_orig_lrp.py; also the attention-mask Add) */
+#define TE_FLAG_RULES_LRP_TC 32768u      /* with TE_FLAG_RULES_LRP (read only together with it): both halves of its Linear rule,
+                                          * S = sd(R, x+- W+-^T) and x+- * (S W+-), as single-pass TF32 wgmma GEMMs (needs
+                                          * `derived`).  Each denominator is a sum of non-negative products, so TF32 operands
+                                          * cost no cancellation; an exact zero stays exactly zero.  The bf16 / fp16 flags
+                                          * (TE_FLAG_ZPLUS_BF16, _S1_BF16, _R_F16) do not apply to this rule. */
 #define TE_FLAG_RELPROP_TO_INPUT 8u   /* finish the lowest block as well: relevance at the encoder input (what
                                          model.relprop() returns in the reference) is left in tensor "relevance_in" */
 
@@ -213,8 +220,10 @@ TE_API int te_bert_tensor(const te_bert_config* cfg, int batch, int seq, void* w
  * that each rule can be parity-tested against the reference layer class it replaces.
  * ---------------------------------------------------------------------------------------------- */
 /* Linear.relprop, alpha=1 (layers_ours.py:207-230): x [rows,in], w [out,in], r [rows,out] -> out [rows,in].
- * flags & TE_FLAG_RULES_LRP: the layers_lrp variant (modules/layers_lrp.py:187-210, separate denominators).
- * scratch: rows*out floats; with TE_FLAG_ZPLUS_TENSOR_CORES: round_up(rows*out,64) + 16*in*out floats. */
+ * flags & TE_FLAG_RULES_LRP: the layers_lrp variant (modules/layers_lrp.py:187-210, separate denominators), on the
+ * tensor cores with TE_FLAG_RULES_LRP_TC as well (in, out multiples of 128; other shapes run the fp32 SIMT rule).
+ * scratch: rows*out floats; with TE_FLAG_ZPLUS_TENSOR_CORES (layers_ours) or TE_FLAG_RULES_LRP | TE_FLAG_RULES_LRP_TC:
+ * round_up(rows*out,64) + 16*in*out floats. */
 TE_API int te_linear_relprop(const float* x, const float* w, const float* r, float* out, float* scratch, int rows,
                       int in_features, int out_features, unsigned flags, void* stream);
 /* Same rule with the Linear's saved forward output y = x W^T + bias [rows,out] supplied (what the engines do): with

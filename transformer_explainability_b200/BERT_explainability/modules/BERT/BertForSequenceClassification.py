@@ -115,6 +115,7 @@ class BertForSequenceClassification(nn.Module):
         self._engine = None
         self._weights_version = None
         self.engine_flags = 0
+        self._rule_flags = 0                   # BERT_cls_lrp sets TE_FLAG_RULES_LRP (the modules/layers_lrp.py rule library)
         std = getattr(config, "initializer_range", 0.02)
         for m in self.modules():                                   # transformers' _init_weights
             if isinstance(m, (nn.Linear, nn.Embedding)):
@@ -141,13 +142,14 @@ class BertForSequenceClassification(nn.Module):
         if dev.type != "cuda":
             raise RuntimeError("the CUDA engine has no CPU path: move the model to a CUDA device (model.cuda())")
         v = self._version()
+        flags = self.engine_flags | getattr(self, "_rule_flags", 0)
         if self._engine is None or self._engine.device != dev:
-            self._engine = BertEngine(self._cfg, device=dev, flags=self.engine_flags)
+            self._engine = BertEngine(self._cfg, device=dev, flags=flags)
             self._weights_version = None
         if self._weights_version != v:
             self._engine.load_state_dict(self.state_dict())
             self._weights_version = v
-        self._engine.flags = self.engine_flags
+        self._engine.flags = flags
         return self._engine
 
     def _engine_tensor(self, name, layer):

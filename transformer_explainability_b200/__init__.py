@@ -47,6 +47,12 @@ def install_aliases(extra=True):
                     "transformer_explainability_b200.BERT_explainability.modules.BERT.ExplanationGenerator",
                 "BERT_explainability.modules.BERT.BertForSequenceClassification":
                     "transformer_explainability_b200.BERT_explainability.modules.BERT.BertForSequenceClassification",
+                "BERT_explainability.modules.layers_lrp":
+                    "transformer_explainability_b200.BERT_explainability.modules.layers_lrp",
+                "BERT_explainability.modules.BERT.BERT_orig_lrp":
+                    "transformer_explainability_b200.BERT_explainability.modules.BERT.BERT_orig_lrp",
+                "BERT_explainability.modules.BERT.BERT_cls_lrp":
+                    "transformer_explainability_b200.BERT_explainability.modules.BERT.BERT_cls_lrp",
             })
         except ImportError:
             pass

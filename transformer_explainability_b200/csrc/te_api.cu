@@ -195,15 +195,17 @@ extern "C" int te_linear_backward_ex(const float* dy, const float* w, float* dx,
 extern "C" int te_linear_relprop(const float* x, const float* w, const float* r, float* out, float* scratch, int rows,
                                  int in_features, int out_features, unsigned flags, void* stream) {
     REQ(x && w && r && out && scratch && rows > 0 && in_features > 0 && out_features > 0, "te_linear_relprop: bad argument");
-    if (flags & TE_FLAG_RULES_LRP)
-        return te_zplus_linear_relprop_lrp(x, in_features, w, r, out_features, out, scratch, rows, in_features, out_features,
-                                           ST(stream));
+    const bool lrp = (flags & TE_FLAG_RULES_LRP) != 0;
+    const unsigned tc_flag = lrp ? TE_FLAG_RULES_LRP_TC : TE_FLAG_ZPLUS_TENSOR_CORES;
     const float* derived = nullptr;
-    if ((flags & TE_FLAG_ZPLUS_TENSOR_CORES) && te_tc_zplus_supported(rows, in_features, out_features, in_features)) {
+    if ((flags & tc_flag) && te_tc_zplus_supported(rows, in_features, out_features, in_features)) {
         const TcScratch c = tc_scratch(scratch, (long long)rows * out_features, in_features, out_features, 0);
         TE_TRY(te_tc_prepare_weights(w, c.derived, in_features, out_features, ST(stream)));
         derived = c.derived;
     }
+    if (lrp)
+        return te_zplus_linear_relprop_lrp(x, in_features, w, derived, r, out_features, out, scratch, rows, in_features,
+                                           out_features, ST(stream));
     return te_zplus_linear_relprop(x, in_features, w, derived, r, out, scratch, rows, in_features, out_features,
                                    ST(stream));
 }

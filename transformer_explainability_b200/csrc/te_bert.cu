@@ -343,10 +343,21 @@ extern "C" int te_bert_attribute(const te_bert_config* cfg, const float* weights
     // ---- relprop -----------------------------------------------------------------------------------------------
     float* R = ws.tD[0]; float* R1 = ws.tD[1]; float* R2 = ws.tD[2]; float* R3 = ws.tD[3];
     float* RF = ws.tF[0]; float* SF = ws.tF[1]; float* S = ws.t3D[0]; float* Rqkv = ws.t3D[1];
+    // Linear / Add rules of the selected rule library: layers_ours, or with TE_FLAG_RULES_LRP layers_lrp (BERT_cls_lrp.py on
+    // BERT_orig_lrp.py: Linear with separate denominators, Add = RelPropSimple, also for the attention-mask Add).  dw is set
+    // for the z+ rules with TE_FLAG_ZPLUS_TENSOR_CORES, for the layers_lrp rule with TE_FLAG_RULES_LRP_TC.
+    const bool lrpv = (flags & TE_FLAG_RULES_LRP) != 0;
+    double* addp = lrpv ? nullptr : ws.addpart;
+    auto lin = [&](const float* x, long long ldx, const float* wt, const float* dwt, const float* r, long long ldr, float* out,
+                   float* sbuf, long long rows, int in, int outf, const float* y, long long ldy, const float* bias,
+                   long long ld_out, float* xabs) -> int {
+        if (lrpv) return te_zplus_linear_relprop_lrp(x, ldx, wt, dwt, r, ldr, out, sbuf, rows, in, outf, st, ld_out);
+        return te_zplus_linear_relprop_ldr(x, ldx, wt, dwt, r, ldr, out, sbuf, rows, in, outf, st, y, ldy, bias, sel.zv, ld_out, xabs);
+    };
     // classifier.relprop (X = pooled) ; dropout / Tanh identity ; pooler.dense.relprop (X = first token) ; pool
-    TE_TRY(te_zplus_linear_relprop(ws.pooled, d.D, w.clsw, nullptr, ws.seed, ws.rpool, ws.shead, d.B, d.D, d.C, st));
-    TE_TRY(te_zplus_linear_relprop(ws.h_last, (long long)d.N * d.D, w.poolw, nullptr, ws.rpool, ws.rfirst, ws.shead, d.B,
-                                   d.D, d.D, st));
+    TE_TRY(lin(ws.pooled, d.D, w.clsw, nullptr, ws.seed, d.C, ws.rpool, ws.shead, d.B, d.D, d.C, nullptr, 0, nullptr, 0, nullptr));
+    TE_TRY(lin(ws.h_last, (long long)d.N * d.D, w.poolw, nullptr, ws.rpool, d.D, ws.rfirst, ws.shead, d.B, d.D, d.D, nullptr, 0,
+               nullptr, 0, nullptr));
     TE_TRY(te_launch_index_select_relprop(ws.h_last, ws.rfirst, nullptr, R, d.B, d.N, d.D, st));
 
     for (int l = d.L - 1; l >= sel.low; --l) {
@@ -355,34 +366,35 @@ extern "C" int te_bert_attribute(const te_bert_config* cfg, const float* weights
         const DerivedW dw = bind_derived(d, sel.dbase, l);
         // BertOutput.relprop :474-487 ; BertIntermediate.relprop :451-456 ; BertLayer.clone
         // top layer: relevance is non-zero only in the first token's row (pooler, BERT.py:181-190) and every rule down
-        // to the attention-output dense rule is row-wise -> its three z+ rules run on the B first-token rows only (exact)
+        // to the attention-output dense rule is row-wise (both libraries) -> its three Linear rules run on the B
+        // first-token rows only (exact)
         const bool top = (l == d.L - 1) && te_engine_cls_rows();
         const long long zr = top ? d.B : d.M;
         const long long sD = top ? (long long)d.N * d.D : d.D, sF = top ? (long long)d.N * d.F : d.F;
-        TE_TRY(te_launch_add_relprop(a.d2, a.ao, R, R1, R2, ws.addpart, d.B, (long long)d.N * d.D, st));
-        TE_TRY(te_zplus_linear_relprop_ldr(a.g, sF, lw.w2, dw.w2, R1, sD, RF, S, zr, d.F, d.D, st, a.d2, sD, lw.b2, sel.zv, sF, SF));
-        TE_TRY(te_zplus_linear_relprop_ldr(a.ao, sD, lw.w1, dw.w1, RF, sF, R1, SF, zr, d.D, d.F, st, a.hpre, sF, lw.b1, sel.zv, sD, S));
+        TE_TRY(te_launch_add_relprop(a.d2, a.ao, R, R1, R2, addp, d.B, (long long)d.N * d.D, st));
+        TE_TRY(lin(a.g, sF, lw.w2, dw.w2, R1, sD, RF, S, zr, d.F, d.D, a.d2, sD, lw.b2, sF, SF));
+        TE_TRY(lin(a.ao, sD, lw.w1, dw.w1, RF, sF, R1, SF, zr, d.D, d.F, a.hpre, sF, lw.b1, sD, S));
         TE_TRY(te_launch_clone_relprop(a.ao, R1, R2, nullptr, R, MD, st));
         // BertSelfOutput.relprop :427-434
-        TE_TRY(te_launch_add_relprop(a.d1, a.h, R, R1, R2, ws.addpart, d.B, (long long)d.N * d.D, st));
+        TE_TRY(te_launch_add_relprop(a.d1, a.h, R, R1, R2, addp, d.B, (long long)d.N * d.D, st));
         if (top) TE_TRY(te_launch_fill(R3, 0.f, MD, st));
-        TE_TRY(te_zplus_linear_relprop_ldr(a.ctx, sD, lw.ow, dw.o, R1, sD, R3, S, zr, d.D, d.D, st, a.d1, sD, lw.ob, sel.zv, sD, S + MD));
+        TE_TRY(lin(a.ctx, sD, lw.ow, dw.o, R1, sD, R3, S, zr, d.D, d.D, a.d1, sD, lw.ob, sD, S + MD));
         // BertSelfAttention.relprop :367-409: matmul2 rule -> attn_cam (:380), cam_v
         const bool last = (l == sel.low && !(flags & TE_FLAG_RELPROP_TO_INPUT));
         TE_TRY(attn_relprop_pv(sel, d.B, d.H, d.N, d.NP, d.dh, a.qkv, a.P, R3, a.ctx, S, a.cam, Rqkv, last, st));
         if (last) break;
-        // add([scores, mask]).relprop : scores = q k^T / sqrt(d) recomputed ; relevance renormalised  :386-388
+        // add([scores, mask]).relprop : scores = q k^T / sqrt(d) recomputed ; relevance renormalised (layers_ours)  :386-388
         TE_TRY(attn_nn(sel.atc, d.B, d.H, d.N, d.NP, d.dh, a.qkv, 3 * d.D, a.qkv + d.D, 3 * d.D, ws.tA[0], nullptr, scale,
                        TE_EPI_STORE, st));
-        TE_TRY(te_launch_add_relprop_keymask(ws.tA[0], ws.maskadd, a.cam, ws.tA[1], ws.addpart, d.B, d.H, d.N, d.NP, st));
+        TE_TRY(te_launch_add_relprop_keymask(ws.tA[0], ws.maskadd, a.cam, ws.tA[1], addp, d.B, d.H, d.N, d.NP, st));
         // matmul1 rule on the unscaled product -> cam_q, cam_k
         TE_TRY(attn_relprop_qk(sel, d.B, d.H, d.N, d.NP, d.dh, a.qkv, ws.tA[1], ws.tA[0], Rqkv, st));
-        // query / key / value z+ rules (separate Linears), Clone(3), Clone(2)
-        TE_TRY(te_zplus_linear_relprop_ldr(a.h, d.D, lw.qkvw, dw.q, Rqkv, 3 * d.D, R, S, d.M, d.D, d.D, st, a.qkv, 3 * d.D, lw.qkvb, sel.zv, 0, S + MD));
-        TE_TRY(te_zplus_linear_relprop_ldr(a.h, d.D, lw.qkvw + DD, dw.k, Rqkv + d.D, 3 * d.D, R1, S, d.M, d.D, d.D, st, a.qkv + d.D, 3 * d.D,
-                                           lw.qkvb + d.D, sel.zv, 0, S + MD));
-        TE_TRY(te_zplus_linear_relprop_ldr(a.h, d.D, lw.qkvw + 2 * DD, dw.v, Rqkv + 2 * d.D, 3 * d.D, R3, S, d.M, d.D, d.D, st,
-                                           a.qkv + 2 * d.D, 3 * d.D, lw.qkvb + 2 * d.D, sel.zv, 0, S + MD));
+        // query / key / value Linear rules (separate Linears), Clone(3), Clone(2)
+        TE_TRY(lin(a.h, d.D, lw.qkvw, dw.q, Rqkv, 3 * d.D, R, S, d.M, d.D, d.D, a.qkv, 3 * d.D, lw.qkvb, 0, S + MD));
+        TE_TRY(lin(a.h, d.D, lw.qkvw + DD, dw.k, Rqkv + d.D, 3 * d.D, R1, S, d.M, d.D, d.D, a.qkv + d.D, 3 * d.D, lw.qkvb + d.D, 0,
+                   S + MD));
+        TE_TRY(lin(a.h, d.D, lw.qkvw + 2 * DD, dw.v, Rqkv + 2 * d.D, 3 * d.D, R3, S, d.M, d.D, d.D, a.qkv + 2 * d.D, 3 * d.D,
+                   lw.qkvb + 2 * d.D, 0, S + MD));
         TE_TRY(te_launch_clone_relprop(a.h, R, R1, R3, SF, MD, st));                      // self.clone (3-way)
         TE_TRY(te_launch_clone_relprop(a.h, SF, R2, nullptr, R, MD, st));                 // attention.clone
     }

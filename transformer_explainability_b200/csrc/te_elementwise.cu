@@ -706,7 +706,8 @@ __global__ void add_keymask_scale_kernel(const float* __restrict__ x1, const flo
                                          const double* __restrict__ partial, int HN, int N, int ld) {
     const int b = blockIdx.y;
     __shared__ float fa_s;
-    if (threadIdx.x == 0) {
+    if (threadIdx.x == 0 && partial == nullptr) fa_s = 1.f;      // layers_lrp variant: no ratio normalisation
+    else if (threadIdx.x == 0) {
         double A = 0, Bs = 0, rho = 0;
         const double* q = partial + (long long)b * TE_ADD_SPLIT * 3;
         for (int i = 0; i < TE_ADD_SPLIT; ++i) { A += q[i * 3]; Bs += q[i * 3 + 1]; rho += q[i * 3 + 2]; }
@@ -957,8 +958,10 @@ int te_launch_add2(const float* a, const float* b, float* out, long long n, cuda
 int te_launch_add_relprop_keymask(const float* x1, const float* keymask, const float* r, float* r1, double* partial,
                                   int B, int H, int N, int ld, cudaStream_t st) {
     TE_REQ(B <= 65535, "add_relprop_keymask: batch too large for one launch");
-    add_keymask_reduce_kernel<<<dim3(TE_ADD_SPLIT, B), kThreads, 0, st>>>(x1, keymask, r, partial, H * N, N, ld);
-    TE_CUDA_CHECK_LAUNCH();
+    if (partial) {                            // null: Add of modules/layers_lrp.py (RelPropSimple) — x1 * S only
+        add_keymask_reduce_kernel<<<dim3(TE_ADD_SPLIT, B), kThreads, 0, st>>>(x1, keymask, r, partial, H * N, N, ld);
+        TE_CUDA_CHECK_LAUNCH();
+    }
     int gx = (H * N + 7) / 8;
     gx = gx > 64 ? 64 : gx;
     add_keymask_scale_kernel<<<dim3(gx, B), kThreads, 0, st>>>(x1, keymask, r, r1, partial, H * N, N, ld);

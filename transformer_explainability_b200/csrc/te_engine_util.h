@@ -151,7 +151,8 @@ static inline int attn_nk(bool tc, int B, int H, int N, int NP, int dh, const fl
 // TE_FLAG_RULES_LRP, TE_FLAG_RELPROP_TO_INPUT) are read where they are used.
 struct Select {
     const float* lbase;   // derived weights of the forward / backward Linears (TE_FLAG_LINEAR_TENSOR_CORES), else NULL
-    const float* dbase;   // derived weights of the z+ rules (TE_FLAG_ZPLUS_TENSOR_CORES), else NULL
+    const float* dbase;   // derived weights of the Linear relevance rules: the z+ rules (TE_FLAG_ZPLUS_TENSOR_CORES), or with
+                          // TE_FLAG_RULES_LRP the layers_lrp rule (TE_FLAG_RULES_LRP_TC); else NULL
     bool atc;             // attention contractions on tensor cores (TE_FLAG_ATTN_TENSOR_CORES)
     bool btf;             // single-pass TF32 backward Linears and attention gradients (TE_FLAG_BACKWARD_TF32)
     bool rtf;             // single-pass TF32 relevance-side attention contractions (TE_FLAG_RELPROP_TF32)
@@ -174,12 +175,15 @@ static inline long long bwd_scale_floats(long long rows, int out) { return rows 
 static inline int decode_flags(Select& s, const char* fn, unsigned flags, const float* derived, int start_layer, bool zplus,
                                Lent bwd_split = {nullptr, 0}, Lent bwd_scale = {nullptr, 0}, long long rows = 0,
                                int widest_out = 0) {
-    if ((flags & (TE_FLAG_LINEAR_TENSOR_CORES | (zplus ? TE_FLAG_ZPLUS_TENSOR_CORES : 0u))) && !derived) {
+    // the tensor-core flag of the Linear rule of the selected rule library: layers_ours (z+) or layers_lrp
+    const bool lrp = (flags & TE_FLAG_RULES_LRP) != 0;
+    const unsigned rule_tc = lrp ? (flags & TE_FLAG_RULES_LRP_TC) : (flags & TE_FLAG_ZPLUS_TENSOR_CORES);
+    if (((flags & (TE_FLAG_LINEAR_TENSOR_CORES | (zplus ? TE_FLAG_ZPLUS_TENSOR_CORES : 0u))) || (zplus && rule_tc)) && !derived) {
         te_set_last_error((std::string(fn) + ": tensor-core flags need the derived weight buffer").c_str());
         return TE_ERR_ARG;
     }
     s.lbase = (flags & TE_FLAG_LINEAR_TENSOR_CORES) ? derived : nullptr;
-    s.dbase = (flags & TE_FLAG_ZPLUS_TENSOR_CORES) ? derived : nullptr;
+    s.dbase = rule_tc ? derived : nullptr;
     s.atc = (flags & TE_FLAG_ATTN_TENSOR_CORES) != 0;
     s.btf = (flags & TE_FLAG_BACKWARD_TF32) != 0;
     s.rtf = (flags & TE_FLAG_RELPROP_TF32) != 0;

@@ -61,6 +61,12 @@ int te_tc_zplus_linear_relprop(const float* x, long long ldx, const float* deriv
                                float* out, float* s_scratch, long long rows, int in_features, int out_features, cudaStream_t st,
                                const float* y, long long ldy, const float* bias, ZplusVariant zv, long long ld_out,
                                float* xabs);
+// Linear.relprop of the layers_lrp library (te_zplus_linear_relprop_lrp) on single-pass TF32 wgmma: for each half in turn,
+// S = sd(R, x+- W+-^T) into s_scratch [rows, out], then out (+)= x+- * (S W+-).  Row strides ldx, ldr, ld_out; shapes as
+// te_tc_zplus_supported.
+int te_tc_lrp_linear_relprop(const float* x, long long ldx, const float* derived, const float* r, long long ldr, float* out,
+                             long long ld_out, float* s_scratch, long long rows, int in_features, int out_features,
+                             cudaStream_t st);
 
 // fp32-grade (3xTF32 split) Linear GEMMs; epilogues mirror the SIMT ones
 enum { TE_TC_EPI_STORE = 0, TE_TC_EPI_BIAS = 1, TE_TC_EPI_BIAS_GELU = 2, TE_TC_EPI_BIAS_ADD = 3, TE_TC_EPI_GELU_BWD = 4 };

@@ -83,5 +83,6 @@ int te_launch_tanh(const float* x, float* y, long long n, cudaStream_t st);
 int te_launch_tanh_bwd(const float* dy, const float* y, float* dx, long long n, cudaStream_t st);
 int te_launch_add2(const float* a, const float* b, float* out, long long n, cudaStream_t st);
 // Add.relprop for add([scores, key-broadcast mask]); only the scores' relevance is produced.
+// partial == NULL selects the layers_lrp variant: r1 = x1 * sd(r, x1 + mask), no ratio normalisation.
 int te_launch_add_relprop_keymask(const float* x1, const float* keymask, const float* r, float* r1, double* partial,
                                   int B, int H, int N, int ld, cudaStream_t st);

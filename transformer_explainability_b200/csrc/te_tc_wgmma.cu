@@ -14,7 +14,7 @@
 //   the stage layout and the wgmma sequence of every k-block follow from those (Stage, issue below).
 //
 // Problems (structs below): the z+ rule's two contractions (two-pass S, single-pass S1, R; TF32, bf16 and block-scaled fp16
-// operand forms), the Linear GEMMs (3xTF32, single-pass TF32, fp16 split, single-pass fp16), the attention-shaped N x N and
+// operand forms), the two halves of the layers_lrp Linear rule (single-pass TF32), the Linear GEMMs (3xTF32, single-pass TF32, fp16 split, single-pass fp16), the attention-shaped N x N and
 // token-reduced N x d contractions and the dense rollout product.
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -383,6 +383,67 @@ struct ZrProb {
             }
             *reinterpret_cast<float2*>(out + (long long)row * ldo + col) =
                 make_float2(fmaxf(xv.x, 0.f) * ap.x + fminf(xv.x, 0.f) * an.x, fmaxf(xv.y, 0.f) * ap.y + fminf(xv.y, 0.f) * an.y);
+        }
+    }
+};
+
+// ---- Linear rule of the layers_lrp library: each half over its own denominator --------------------------------------
+// S half:  S = sd(R, x+- W+-^T), TF32-rounded fp32 [M, N] (A = tf32(x+) or tf32(x-) transformed on load, B = W+ / W-).
+// Both factors of every product share a sign, so the denominator is a sum of non-negative terms: no cancellation, and it
+// is exactly 0 (S = 0) only when every term is.
+template <bool NEG>
+struct LrpSProb : NoScale {
+    static constexpr int BN = 128, CHUNK = 0, FMT = OP_TF32;
+    using PRODS = One;
+    using L = Stage<PRODS, BN>;
+    static constexpr bool COL_FAST = true;
+    int M, N, K;
+    const float* x; long long ldx; const float* w;      // w: W+ or W- (tf32) [N, K]
+    const float* r; long long ldr; float* out;           // out: S [M, N], row stride N
+    __device__ int kblocks() const { return K / 32; }
+    __device__ void load(uint8_t* st, int kb, int m0, int n0, int, int tid) const {
+        for_k32(BM, x, ldx, m0, M, kb * 32, K, tid, [&](int rr, int c, float4 v) { st4(st + L::a(0), rr, c, tf32x4(NEG ? negx4(v) : posx4(v))); });
+        for_k32(BN, w, K, n0, N, kb * 32, K, tid, [&](int rr, int c, float4 v) { st4(st + L::b(0), rr, c, v); });
+    }
+    __device__ void epilogue(float (&acc)[1][BN / 2], int m0, int n0, int, int tid) const {
+#pragma unroll
+        for (int j = 0; j < BN / 2; j += 2) {
+            const int row = m0 + frag_row(tid, j), col = n0 + frag_col(tid, j);
+            if (row >= M) continue;
+            const float2 rr = *reinterpret_cast<const float2*>(r + (long long)row * ldr + col);
+            *reinterpret_cast<float2*>(out + (long long)row * N + col) =
+                make_float2(to_tf32(te_sd(rr.x, acc[0][j])), to_tf32(te_sd(rr.y, acc[0][j + 1])));
+        }
+    }
+};
+// R half:  out = x+ * (S W+)  (NEG false),  out += x- * (S W-)  (NEG true).  A = S [M, K], B = W+^T / W-^T [N, K].
+template <bool NEG>
+struct LrpRProb : NoScale {
+    static constexpr int BN = 128, CHUNK = 0, FMT = OP_TF32;
+    using PRODS = One;
+    using L = Stage<PRODS, BN>;
+    static constexpr bool COL_FAST = true;
+    int M, N, K;
+    const float* s; const float* wt;
+    const float* x; long long ldx; float* out; long long ldo;
+    __device__ int kblocks() const { return K / 32; }
+    __device__ void load(uint8_t* st, int kb, int m0, int n0, int, int tid) const {
+        for_k32(BM, s, K, m0, M, kb * 32, K, tid, [&](int rr, int c, float4 v) { st4(st + L::a(0), rr, c, v); });
+        for_k32(BN, wt, K, n0, N, kb * 32, K, tid, [&](int rr, int c, float4 v) { st4(st + L::b(0), rr, c, v); });
+    }
+    __device__ void epilogue(float (&acc)[1][BN / 2], int m0, int n0, int, int tid) const {
+#pragma unroll
+        for (int j = 0; j < BN / 2; j += 2) {
+            const int row = m0 + frag_row(tid, j), col = n0 + frag_col(tid, j);
+            if (row >= M) continue;
+            const float2 xv = *reinterpret_cast<const float2*>(x + (long long)row * ldx + col);
+            float2* o = reinterpret_cast<float2*>(out + (long long)row * ldo + col);
+            if (NEG) {
+                const float2 prev = *o;
+                *o = make_float2(prev.x + fminf(xv.x, 0.f) * acc[0][j], prev.y + fminf(xv.y, 0.f) * acc[0][j + 1]);
+            } else {
+                *o = make_float2(fmaxf(xv.x, 0.f) * acc[0][j], fmaxf(xv.y, 0.f) * acc[0][j + 1]);
+            }
         }
     }
 };
@@ -937,6 +998,34 @@ int te_tc_zplus_linear_relprop(const float* x, long long ldx, const float* deriv
         return launch(p, dim3(mtiles(rows), in_features / 128), st);
     }
     return te_tc_zplus_r(s_scratch, derived, x, ldx, out, ld_out, rows, in_features, out_features, st);
+}
+
+namespace {
+template <bool NEG>
+int lrp_half(const float* x, long long ldx, const TeDerived<const float>& dv, const float* r, long long ldr, float* out,
+             long long ld_out, float* s, long long rows, int in_features, int out_features, cudaStream_t st) {
+    LrpSProb<NEG> ps;
+    ps.M = (int)rows; ps.N = out_features; ps.K = in_features;
+    ps.x = x; ps.ldx = ldx; ps.w = NEG ? dv.wn : dv.wp; ps.r = r; ps.ldr = ldr; ps.out = s;
+    TE_TRY(launch(ps, dim3(mtiles(rows), out_features / 128), st));
+    LrpRProb<NEG> pr;
+    pr.M = (int)rows; pr.N = in_features; pr.K = out_features;
+    pr.s = s; pr.wt = NEG ? dv.wnt : dv.wpt; pr.x = x; pr.ldx = ldx; pr.out = out; pr.ldo = ld_out;
+    return launch(pr, dim3(mtiles(rows), in_features / 128), st);
+}
+}  // namespace
+
+int te_tc_lrp_linear_relprop(const float* x, long long ldx, const float* derived, const float* r, long long ldr, float* out,
+                             long long ld_out, float* s_scratch, long long rows, int in_features, int out_features,
+                             cudaStream_t st) {
+    if (!a16(x) || !a16(derived) || !a16(r) || !a16(out) || !a16(s_scratch) || ldx % 4 != 0 || ldr % 4 != 0 || ld_out % 4 != 0) {
+        te_set_last_error("te_tc_lrp_linear_relprop: operands must be 16-byte aligned");
+        return TE_ERR_ARG;
+    }
+    const TeDerived<const float> dv(derived, in_features, out_features);
+    // the two halves in sequence through the one S buffer: x+ first (writes out), then x- (adds to it)
+    TE_TRY(lrp_half<false>(x, ldx, dv, r, ldr, out, ld_out, s_scratch, rows, in_features, out_features, st));
+    return lrp_half<true>(x, ldx, dv, r, ldr, out, ld_out, s_scratch, rows, in_features, out_features, st);
 }
 
 // ---- Linear GEMMs ---------------------------------------------------------------------------------------------------

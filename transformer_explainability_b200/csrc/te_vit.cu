@@ -367,11 +367,12 @@ extern "C" int te_vit_attribute(const te_vit_config* cfg, const float* weights, 
     float* R = ws.tD[0]; float* R1 = ws.tD[1]; float* R2 = ws.tD[2]; float* R3 = ws.tD[3];
     float* RF = ws.tF[0]; float* SF = ws.tF[1]; float* S = ws.t3D[0]; float* Rqkv = ws.t3D[1]; float* S1 = ws.tA;
     // head.relprop (z+), pool.relprop (IndexSelect), norm.relprop (identity)
-    // z+ rule / Add rule of the selected rule library (layers_ours, or layers_lrp with TE_FLAG_RULES_LRP)
+    // z+ rule / Add rule of the selected rule library (layers_ours, or layers_lrp with TE_FLAG_RULES_LRP; dwt is then set
+    // only with TE_FLAG_RULES_LRP_TC)
     auto zrule = [&](const float* x, long long ldx, const float* wt, const float* dwt, const float* r, long long ldr, float* out,
                      float* sbuf, long long rows, int in, int outf, const float* y, long long ldy, const float* bias,
                      long long ld_out, float* xabs) -> int {
-        if (lrpv) return te_zplus_linear_relprop_lrp(x, ldx, wt, r, ldr, out, sbuf, rows, in, outf, st);
+        if (lrpv) return te_zplus_linear_relprop_lrp(x, ldx, wt, dwt, r, ldr, out, sbuf, rows, in, outf, st, ld_out);
         return te_zplus_linear_relprop_ldr(x, ldx, wt, dwt, r, ldr, out, sbuf, rows, in, outf, st, y, ldy, bias, sel.zv, ld_out, xabs);
     };
     auto addrule = [&](const float* x1, const float* x2, const float* r, float* r1, float* r2) -> int {

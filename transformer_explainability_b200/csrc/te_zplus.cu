@@ -44,10 +44,17 @@ int te_zplus_linear_relprop_ldr(const float* x, long long ldx, const float* w, c
     return TE_OK;
 }
 
-int te_zplus_linear_relprop_lrp(const float* x, long long ldx, const float* w, const float* r, long long ldr, float* out,
-                                float* s_scratch, long long rows, int in_features, int out_features, cudaStream_t st) {
+int te_zplus_linear_relprop_lrp(const float* x, long long ldx, const float* w, const float* w_derived, const float* r,
+                                long long ldr, float* out, float* s_scratch, long long rows, int in_features, int out_features,
+                                cudaStream_t st, long long ld_out) {
     if (rows <= 0) return TE_OK;
-    if (rows > 0x7fffffffLL || ldx > 0x7fffffffLL || ldr > 0x7fffffffLL) { te_set_last_error("zplus_lrp: overflow"); return TE_ERR_ARG; }
+    if (ld_out == 0) ld_out = in_features;
+    if (rows > 0x7fffffffLL || ldx > 0x7fffffffLL || ldr > 0x7fffffffLL || ld_out > 0x7fffffffLL) {
+        te_set_last_error("zplus_lrp: overflow");
+        return TE_ERR_ARG;
+    }
+    if (w_derived && te_tc_zplus_supported(rows, in_features, out_features, ldx) && ldr % 4 == 0 && ld_out % 4 == 0)
+        return te_tc_lrp_linear_relprop(x, ldx, w_derived, r, ldr, out, ld_out, s_scratch, rows, in_features, out_features, st);
     TeGemm p;
     memset(&p, 0, sizeof(p));
     p.nb1 = p.nb2 = 1; p.alpha = 1.f;
@@ -57,7 +64,7 @@ int te_zplus_linear_relprop_lrp(const float* x, long long ldx, const float* w, c
         p.E0 = r; p.lde0 = (int)ldr; p.M = (int)rows; p.N = out_features; p.K = in_features;
         TE_TRY(te_gemm_launch(p, TE_L_K, TE_L_K, half ? TE_XF_AB_NEG : TE_XF_AB_POS, TE_EPI_SD, st));
         // R_in (+)= x+- * (S_half W+-)
-        p.A = s_scratch; p.lda = out_features; p.B = w; p.ldb = in_features; p.C = out; p.ldc = in_features;
+        p.A = s_scratch; p.lda = out_features; p.B = w; p.ldb = in_features; p.C = out; p.ldc = (int)ld_out;
         p.E0 = x; p.lde0 = (int)ldx; p.M = (int)rows; p.N = in_features; p.K = out_features;
         TE_TRY(te_gemm_launch(p, TE_L_K, TE_L_MN, half ? TE_XF_B_NEG : TE_XF_B_POS, half ? TE_EPI_MULNEG_ACC : TE_EPI_MULPOS, st));
     }

@@ -30,6 +30,10 @@ int te_zplus_linear_relprop_ldr(const float* x, long long ldx, const float* w, c
 // token rows — the CLS rows of the top block, the only rows whose relevance is non-zero there (SURVEY.md 8a).
 
 // Linear.relprop of the layers_lrp baseline variant (modules/layers_lrp.py:187-210, alpha=1): S1 = sd(R, x+ W+^T),
-// S2 = sd(R, x- W-^T) (separate denominators), R_in = x+ * (S1 W+) + x- * (S2 W-).  fp32 SIMT; s_scratch [rows, out].
-int te_zplus_linear_relprop_lrp(const float* x, long long ldx, const float* w, const float* r, long long ldr, float* out,
-                                float* s_scratch, long long rows, int in_features, int out_features, cudaStream_t st);
+// S2 = sd(R, x- W-^T) (separate denominators), R_in = x+ * (S1 W+) + x- * (S2 W-).  s_scratch [rows, out] holds S1, then S2.
+// w_derived: the te_tc_prepare_weights() copies of w, or NULL.  When given (and the shape qualifies) both halves run on
+// single-pass TF32 wgmma (TE_FLAG_RULES_LRP_TC; every denominator is a sum of non-negative products); otherwise fp32 SIMT.
+// ld_out: row stride of out (0 = in_features), for the strided row subsets of te_zplus_linear_relprop_ldr.
+int te_zplus_linear_relprop_lrp(const float* x, long long ldx, const float* w, const float* w_derived, const float* r,
+                                long long ldr, float* out, float* s_scratch, long long rows, int in_features, int out_features,
+                                cudaStream_t st, long long ld_out = 0);

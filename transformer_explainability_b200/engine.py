@@ -79,7 +79,7 @@ class ViTEngine:
     @_on_engine_device
     def _derived(self, flags):
         """W+/W-/W+^T/W-^T TF32 copies for the tensor-core z+ path (built once per weight load)."""
-        if not (flags & _lib.FLAG_TENSOR_CORES):
+        if not (flags & (_lib.FLAG_TENSOR_CORES | _lib.FLAG_RULES_LRP_TC)):
             return None
         if self.derived is None:
             n = check(self.lib.te_vit_derived_total(ctypes.byref(self.cfg)), "te_vit_derived_total")
@@ -326,7 +326,7 @@ class BertEngine:
 
     @_on_engine_device
     def _derived(self, flags):
-        if not (flags & _lib.FLAG_TENSOR_CORES):
+        if not (flags & (_lib.FLAG_TENSOR_CORES | _lib.FLAG_RULES_LRP_TC)):
             return None
         if self.derived is None:
             n = check(self.lib.te_bert_derived_total(ctypes.byref(self.cfg)), "te_bert_derived_total")

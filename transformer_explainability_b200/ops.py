@@ -270,13 +270,20 @@ def tc_attention_nk(amap, np_, amn, x, ldx, batch, heads, n, out, ld_out, e=None
 def linear_relprop(x, w, r, tensor_cores=False, y=None, bias=None, bf16=False, variant="ours", r_f16=False):
     """``Linear.relprop`` (layers_ours.py:207-230): x [...,in], w [out,in], r [...,out] -> [...,in].
     y / bias: the layer's saved forward output (and bias) — lets the tensor-core path form the denominator in one pass.
-    variant="lrp": the rule of ``modules/layers_lrp.py:187-210`` (separate denominators; fp32 SIMT)."""
+    variant="lrp": the rule of ``modules/layers_lrp.py:187-210`` (separate denominators; fp32 SIMT); variant="lrp_tc": the
+    same rule on single-pass TF32 tensor cores (TE_FLAG_RULES_LRP_TC; in / out multiples of 128, other shapes run the SIMT
+    rule; tensor_cores, y, bias, bf16 and r_f16 do not apply to either)."""
     _req(x, w, r, y, bias)
     if (w.dim() != 2 or x.shape[-1] != w.shape[1] or r.shape[-1] != w.shape[0] or r.shape[:-1] != x.shape[:-1]
             or (y is not None and y.shape != r.shape) or (bias is not None and bias.numel() != w.shape[0])):
         raise ValueError("linear_relprop: x [...,in], w [out,in], r / y [...,out], bias [out] expected")
     rows = x.numel() // x.shape[-1]
     out = torch.empty_like(x)
+    if variant == "lrp_tc":
+        scratch = _tc_scratch(w, x.device, s=rows * w.shape[0])
+        check(_lib.load().te_linear_relprop(ptr(x), ptr(w), ptr(r), ptr(out), ptr(scratch), rows, x.shape[-1], w.shape[0],
+                                            _lib.FLAG_RULES_LRP | _lib.FLAG_RULES_LRP_TC, _stream()), "te_linear_relprop")
+        return out
     if tensor_cores:
         scratch = _tc_scratch(w, x.device, s=rows * w.shape[0], operand=x.numel())
     else:
@@ -291,7 +298,7 @@ def linear_relprop(x, w, r, tensor_cores=False, y=None, bias=None, bf16=False, v
     if variant == "lrp":
         flags, y = _lib.FLAG_RULES_LRP, None
     elif variant != "ours":
-        raise ValueError("variant: 'ours' or 'lrp'")
+        raise ValueError("variant: 'ours', 'lrp' or 'lrp_tc'")
     if y is not None:
         check(_lib.load().te_linear_relprop_ex(ptr(x), ptr(w), ptr(bias), ptr(y), ptr(r), ptr(out), ptr(scratch), rows,
                                                x.shape[-1], w.shape[0], flags, _stream()), "te_linear_relprop_ex")
