@@ -264,10 +264,10 @@ BERT_GENERATORS = [("LRP", dict(start_layer=0)), ("LRP", dict(start_layer=1)), (
 BERT_FORWARD_ONLY = ("attn_last_layer", "rollout")
 
 
-def _bert_setup(seed, dim, heads, inter, cases, n=3, seq=130):
+def _bert_setup(seed, dim, heads, inter, cases, n=3, seq=130, c_qkv=3.0):
     params, heads = obert.init_params(seed=seed, vocab=1000, max_pos=512, dim=dim, depth=3, heads=heads, inter=inter,
                                       rand_affine=True)
-    params = conditioned.condition_bert(params)
+    params = conditioned.condition_bert(params, c_qkv=c_qkv)
     g = torch.Generator().manual_seed(seed + 1)
     ids = torch.randint(5, 1000, (n, seq), generator=g)
     ids[:, 0], ids[:, -1] = 101, 102

@@ -350,6 +350,11 @@ GELU_GRAD_EXACT = 3e-7
 GELU_GRAD_FAST = 6e-7
 
 
+def elem_err(out, ref, scale):
+    """largest |out - ref| over the element's own scale (fp64 ref and scale): the measure LIN_BOUND bounds"""
+    return ((out.double() - ref).abs() / scale).max().item()
+
+
 def _gelu64(y):
     return 0.5 * y * (1 + torch.erf(y / 2 ** 0.5))
 
@@ -386,7 +391,7 @@ def test_linear_forward_epilogues(rows, K):
         for epi in ("bias_gelu", "bias_add"):
             y, y2 = ops.linear_forward_epi(x, w, b, e0 if epi == "bias_add" else None, epi=epi, family=family)
             torch.cuda.synchronize()
-            ey = ((y.double() - y64).abs() / scale).max().item()
+            ey = elem_err(y, y64, scale)
             if epi == "bias_gelu":      # |GELU'| <= 1.13, plus the fp32 GELU itself
                 e2 = ((y2.double() - _gelu64(y64)).abs() / (1.13 * scale)).max().item()
                 b2 = bound + 5e-7

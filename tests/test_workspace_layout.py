@@ -54,7 +54,9 @@ def _check(ext, uses):
 
 
 VIT = [dict(embed_dim=256, num_heads=4, mlp_ratio=r) for r in (0.5, 1.0, 1.5, 2.0, 4.0)] + \
-      [dict(embed_dim=256, num_heads=4, mlp_ratio=1.0, distilled=True), dict(), dict(embed_dim=768, mlp_ratio=1.0)]
+      [dict(embed_dim=256, num_heads=4, mlp_ratio=1.0, distilled=True), dict(), dict(embed_dim=768, mlp_ratio=1.0)] + \
+      [dict(embed_dim=192, num_heads=3), dict(embed_dim=384, num_heads=6), dict(embed_dim=384, num_heads=6, distilled=True),
+       dict(embed_dim=384, num_heads=12), dict(embed_dim=384, num_heads=8), dict(img_size=384)]     # tests/test_gpu_model_geometries.py
 
 
 @pytest.mark.parametrize("kw", VIT, ids=lambda kw: "-".join("%s%s" % (k, v) for k, v in kw.items()) or "vit_b16")
@@ -78,7 +80,10 @@ def test_vit_lent_regions_cover_their_uses(kw, batch):
 
 
 BERT = [dict(hidden_size=256, num_attention_heads=4, intermediate_size=f) for f in (128, 256, 384, 512, 1024)] + \
-       [dict(), dict(intermediate_size=768)]
+       [dict(), dict(intermediate_size=768)] + \
+       [dict(hidden_size=128, num_attention_heads=2, intermediate_size=512),
+        dict(hidden_size=384, num_attention_heads=12, intermediate_size=1536),
+        dict(hidden_size=512, num_attention_heads=8, intermediate_size=2048)]         # tests/test_gpu_model_geometries.py
 
 
 @pytest.mark.parametrize("kw", BERT, ids=lambda kw: "-".join("%s%s" % (k, v) for k, v in kw.items()) or "bert_base")
