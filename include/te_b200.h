@@ -138,6 +138,13 @@ TE_API int te_vit_forward(const te_vit_config* cfg, const float* weights, const 
 TE_API int te_vit_attribute(const te_vit_config* cfg, const float* weights, const float* derived, int batch, int* index,
                      int start_layer, unsigned flags, float* maps, void* workspace, long long workspace_bytes,
                      void* stream);
+/* Same with model.relprop(cam, alpha=alpha) (ViT_LRP.py:324, any method): every Linear.relprop of the rule library applies
+ * the LRP-alpha-beta rule with beta = alpha - 1 (layers_ours.py:207-230, layers_lrp.py:187-210), R_in = alpha * act -
+ * beta * inh, the inhibitor half running after the activator through the same scratch (the workspace size is unchanged).
+ * alpha = 1 is exactly te_vit_attribute.  The other rules do not depend on alpha.  A non-finite alpha returns TE_ERR_ARG. */
+TE_API int te_vit_attribute_alpha(const te_vit_config* cfg, const float* weights, const float* derived, int batch, int* index,
+                                  int start_layer, float alpha, unsigned flags, float* maps, void* workspace,
+                                  long long workspace_bytes, void* stream);
 
 /* te_vit_forward + te_vit_attribute: one call per batch = LRP.generate_LRP for `batch` independent inputs. */
 TE_API int te_vit_explain(const te_vit_config* cfg, const float* weights, const float* derived, const float* images,
@@ -205,6 +212,11 @@ TE_API int te_bert_forward(const te_bert_config* cfg, const float* weights, cons
 TE_API int te_bert_attribute(const te_bert_config* cfg, const float* weights, const float* derived, int batch, int seq,
                       int* index, int start_layer, unsigned flags, float* maps, void* workspace,
                       long long workspace_bytes, void* stream);
+/* Same with model.relprop(cam, alpha=alpha) (BertForSequenceClassification.py:83-88): the LRP-alpha-beta Linear rule as for
+ * te_vit_attribute_alpha.  alpha = 1 is exactly te_bert_attribute; a non-finite alpha returns TE_ERR_ARG. */
+TE_API int te_bert_attribute_alpha(const te_bert_config* cfg, const float* weights, const float* derived, int batch, int seq,
+                                   int* index, int start_layer, float alpha, unsigned flags, float* maps, void* workspace,
+                                   long long workspace_bytes, void* stream);
 TE_API int te_bert_explain(const te_bert_config* cfg, const float* weights, const float* derived,
                     const long long* input_ids, const long long* attention_mask, int batch, int seq, int* index,
                     int start_layer, unsigned flags, float* maps, float* logits, void* workspace,
@@ -234,6 +246,14 @@ TE_API int te_linear_relprop(const float* x, const float* w, const float* r, flo
 TE_API int te_linear_relprop_ex(const float* x, const float* w, const float* bias, const float* y, const float* r,
                          float* out, float* scratch, int rows, int in_features, int out_features, unsigned flags,
                          void* stream);
+/* Linear.relprop(R, alpha) for any finite alpha: the LRP-alpha-beta rule, beta = alpha - 1, R_in = alpha * act - beta * inh
+ * (layers_ours.py:207-230; with TE_FLAG_RULES_LRP layers_lrp.py:187-210).  inh is act with the weight signs swapped:
+ * x+ * (S_i W-) + x- * (S_i W+) with S_i = sd(R, x+ W-^T + x- W+^T) (layers_lrp: each of the four products over its own
+ * denominator).  y == NULL: te_linear_relprop (bias ignored); y != NULL: te_linear_relprop_ex.  Scratch sizes as there.
+ * alpha = 1 is exactly those entries; a non-finite alpha returns TE_ERR_ARG. */
+TE_API int te_linear_relprop_alpha(const float* x, const float* w, const float* bias, const float* y, const float* r,
+                                   float* out, float* scratch, int rows, int in_features, int out_features, float alpha,
+                                   unsigned flags, void* stream);
 /* Add.relprop (layers_ours.py:97-120) per sample: x1,x2,r [batch,per_sample] -> r1,r2.
  * scratch: batch*48 doubles; scratch == NULL selects the layers_lrp variant (modules/layers_lrp.py:48-60,98-100:
  * r1 = x1*sd(r, x1+x2), r2 = x2*sd(r, x1+x2), no ratio normalisation). */

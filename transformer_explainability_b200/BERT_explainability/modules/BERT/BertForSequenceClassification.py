@@ -167,10 +167,9 @@ class BertForSequenceClassification(nn.Module):
 
     def relprop(self, cam=None, **kwargs):
         """``relprop`` (:83-88): relevance at the encoder input [B,S,D]; leaves attn_cam / attn_gradients of every
-        layer readable through ``layer.attention.self.get_attn_cam()`` ... like the reference."""
-        if kwargs.get("alpha", 1) != 1:
-            raise NotImplementedError("only alpha=1 is implemented (the only value the reference passes)")
+        layer readable through ``layer.attention.self.get_attn_cam()`` ... like the reference.  ``alpha`` (default 1)
+        selects the LRP-alpha-beta rule, beta = alpha - 1, in every Linear.relprop."""
         eng = self.engine()
         index = cam.argmax(dim=-1).to(torch.int32) if cam is not None else None
-        eng.attribute(index=index, start_layer=0, flags=eng.flags | _lib.FLAG_RELPROP_TO_INPUT)
+        eng.attribute(index=index, start_layer=0, flags=eng.flags | _lib.FLAG_RELPROP_TO_INPUT, alpha=kwargs.get("alpha", 1))
         return eng.tensor("relevance_in")

@@ -4,7 +4,7 @@ import torch
 import torch.nn as nn
 
 from transformer_explainability_b200.modules.layers_ours import *            # noqa: F401,F403
-from transformer_explainability_b200.modules.layers_ours import RelProp, RelPropSimple, _check_alpha, _c, _mix
+from transformer_explainability_b200.modules.layers_ours import RelProp, RelPropSimple, _c, _mix
 from transformer_explainability_b200.modules import layers_ours as _base
 from transformer_explainability_b200 import ops
 
@@ -20,7 +20,6 @@ class MatMul(RelPropSimple):
         return torch.matmul(*inputs)
 
     def relprop(self, R, alpha):
-        _check_alpha(alpha)
         a, b = self.X
         if a.shape[-1] == a.shape[-2] == b.shape[-2] and R.shape == torch.Size(list(a.shape[:-1]) + [b.shape[-1]]) \
                 and a.shape[-1] != b.shape[-1]:

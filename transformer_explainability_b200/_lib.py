@@ -67,6 +67,7 @@ PROTOTYPES = {
     "te_vit_derived_total": (c_ll, [_CFG]),
     "te_vit_prepare_derived": (c_int, [_CFG, _P, _P, _P]),
     "te_vit_attribute": (c_int, [_CFG, _P, _P, c_int, _P, c_int, c_uint, _P, _P, c_ll, _P]),
+    "te_vit_attribute_alpha": (c_int, [_CFG, _P, _P, c_int, _P, c_int, c_float, c_uint, _P, _P, c_ll, _P]),
     "te_vit_explain": (c_int, [_CFG, _P, _P, _P, c_int, _P, c_int, c_uint, _P, _P, _P, c_ll, _P]),
     "te_vit_tensor": (c_int, [_CFG, c_int, _P, c_char_p, c_int, ctypes.POINTER(_P), ctypes.POINTER(c_ll),
                               ctypes.POINTER(c_ll)]),
@@ -83,11 +84,13 @@ PROTOTYPES = {
     "te_bert_workspace_bytes": (c_ll, [_BCFG, c_int, c_int]),
     "te_bert_forward": (c_int, [_BCFG, _P, _P, _P, _P, c_int, c_int, c_uint, _P, _P, c_ll, _P]),
     "te_bert_attribute": (c_int, [_BCFG, _P, _P, c_int, c_int, _P, c_int, c_uint, _P, _P, c_ll, _P]),
+    "te_bert_attribute_alpha": (c_int, [_BCFG, _P, _P, c_int, c_int, _P, c_int, c_float, c_uint, _P, _P, c_ll, _P]),
     "te_bert_explain": (c_int, [_BCFG, _P, _P, _P, _P, c_int, c_int, _P, c_int, c_uint, _P, _P, _P, c_ll, _P]),
     "te_bert_tensor": (c_int, [_BCFG, c_int, c_int, _P, c_char_p, c_int, ctypes.POINTER(_P), ctypes.POINTER(c_ll),
                                ctypes.POINTER(c_ll)]),
     "te_linear_relprop": (c_int, [_P, _P, _P, _P, _P, c_int, c_int, c_int, c_uint, _P]),
     "te_linear_relprop_ex": (c_int, [_P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_uint, _P]),
+    "te_linear_relprop_alpha": (c_int, [_P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_float, c_uint, _P]),
     "te_add_relprop": (c_int, [_P, _P, _P, _P, _P, _P, c_int, c_ll, _P]),
     "te_clone_relprop": (c_int, [_P, _P, _P, _P, _P, c_ll, _P]),
     "te_matmul_av_relprop": (c_int, [_P, _P, _P, _P, _P, _P, c_int, c_int, c_int, _P]),

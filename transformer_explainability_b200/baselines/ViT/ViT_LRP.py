@@ -200,25 +200,25 @@ class VisionTransformer(nn.Module):
     def relprop(self, cam=None, method="transformer_attribution", is_ablation=False, start_layer=0, **kwargs):
         """``ViT_LRP.py:324-398``.  ``cam`` is the one-hot class-relevance seed [B,C] (``generate_LRP`` passes
         the same one-hot it back-propagates, ViT_explanation_generator.py:31-40); the engine derives the class
-        index from it and runs gradient + relprop + rollout in one call."""
-        if kwargs.get("alpha", 1) != 1:
-            raise NotImplementedError("only alpha=1 is implemented (the only value the reference passes)")
+        index from it and runs gradient + relprop + rollout in one call.  ``alpha`` (default 1) selects the
+        LRP-alpha-beta rule, beta = alpha - 1, in every Linear.relprop, for every method that runs the relprop."""
+        alpha = kwargs.get("alpha", 1)
         eng = self.engine()
         index = cam.argmax(dim=-1).to(torch.int32) if cam is not None else None
         first = 2 if self.distilled else 1
         if method in ("transformer_attribution", "grad"):
-            maps, _ = eng.attribute(index=index, start_layer=start_layer)
+            maps, _ = eng.attribute(index=index, start_layer=start_layer, alpha=alpha)
             return maps
         if method == "full":                                   # :337-343: relevance of every pixel, channels summed
-            return eng.relprop_pixels(index=index)
+            return eng.relprop_pixels(index=index, alpha=alpha)
         # secondary methods (:345-398): head reductions of the saved per-block tensors
         if method == "rollout":                                # attn_cam of every block -> rollout
-            eng.attribute(index=index, start_layer=0, flags=eng.flags | _lib.FLAG_KEEP_ALL_CAMS)
+            eng.attribute(index=index, start_layer=0, flags=eng.flags | _lib.FLAG_KEEP_ALL_CAMS, alpha=alpha)
             cams = [ops.head_reduce(blk.attn.get_attn_cam(), mode="relu_mean") for blk in self.blocks]
             return compute_rollout_attention(cams, start_layer=start_layer)[:, 0, first:]
         if method in ("last_layer", "second_layer"):
             l = len(self.blocks) - 1 if method == "last_layer" else 1
-            eng.attribute(index=index, start_layer=l)          # the relprop stops at attn_cam of block l
+            eng.attribute(index=index, start_layer=l, alpha=alpha)     # the relprop stops at attn_cam of block l
             attn = self.blocks[l].attn
             c = ops.head_reduce(attn.get_attn_cam(), attn.get_attn_gradients() if is_ablation else None, mode="relu_mean")
             return c[:, 0, first:]

@@ -192,29 +192,28 @@ extern "C" int te_linear_backward_ex(const float* dy, const float* w, float* dx,
                                  ST(stream));
 }
 
-extern "C" int te_linear_relprop(const float* x, const float* w, const float* r, float* out, float* scratch, int rows,
-                                 int in_features, int out_features, unsigned flags, void* stream) {
-    REQ(x && w && r && out && scratch && rows > 0 && in_features > 0 && out_features > 0, "te_linear_relprop: bad argument");
-    const bool lrp = (flags & TE_FLAG_RULES_LRP) != 0;
-    const unsigned tc_flag = lrp ? TE_FLAG_RULES_LRP_TC : TE_FLAG_ZPLUS_TENSOR_CORES;
+extern "C" int te_linear_relprop_alpha(const float* x, const float* w, const float* bias, const float* y, const float* r,
+                                       float* out, float* scratch, int rows, int in_features, int out_features, float alpha,
+                                       unsigned flags, void* stream) {
+    REQ(x && w && r && out && scratch && rows > 0 && in_features > 0 && out_features > 0,
+        "te_linear_relprop_alpha: bad argument");
+    REQ(isfinite(alpha), "te_linear_relprop_alpha: alpha must be finite");
     const float* derived = nullptr;
-    if ((flags & tc_flag) && te_tc_zplus_supported(rows, in_features, out_features, in_features)) {
-        const TcScratch c = tc_scratch(scratch, (long long)rows * out_features, in_features, out_features, 0);
-        TE_TRY(te_tc_prepare_weights(w, c.derived, in_features, out_features, ST(stream)));
-        derived = c.derived;
+    if (!y) {                                            // te_linear_relprop: either rule library, two-pass denominator
+        const bool lrp = (flags & TE_FLAG_RULES_LRP) != 0;
+        const unsigned tc_flag = lrp ? TE_FLAG_RULES_LRP_TC : TE_FLAG_ZPLUS_TENSOR_CORES;
+        if ((flags & tc_flag) && te_tc_zplus_supported(rows, in_features, out_features, in_features)) {
+            const TcScratch c = tc_scratch(scratch, (long long)rows * out_features, in_features, out_features, 0);
+            TE_TRY(te_tc_prepare_weights(w, c.derived, in_features, out_features, ST(stream)));
+            derived = c.derived;
+        }
+        if (lrp)
+            return te_zplus_linear_relprop_lrp(x, in_features, w, derived, r, out_features, out, scratch, rows, in_features,
+                                               out_features, ST(stream), 0, alpha);
+        return te_zplus_linear_relprop_ldr(x, in_features, w, derived, r, out_features, out, scratch, rows, in_features,
+                                           out_features, ST(stream), nullptr, 0, nullptr, {}, 0, nullptr, alpha);
     }
-    if (lrp)
-        return te_zplus_linear_relprop_lrp(x, in_features, w, derived, r, out_features, out, scratch, rows, in_features,
-                                           out_features, ST(stream));
-    return te_zplus_linear_relprop(x, in_features, w, derived, r, out, scratch, rows, in_features, out_features,
-                                   ST(stream));
-}
-
-extern "C" int te_linear_relprop_ex(const float* x, const float* w, const float* bias, const float* y, const float* r,
-                                    float* out, float* scratch, int rows, int in_features, int out_features,
-                                    unsigned flags, void* stream) {
-    REQ(x && w && r && out && scratch && rows > 0 && in_features > 0 && out_features > 0, "te_linear_relprop_ex: bad argument");
-    const float* derived = nullptr;
+    // te_linear_relprop_ex: the layers_ours rule with the saved forward output (single-pass tensor-core denominator)
     float* xabs = nullptr;
     if ((flags & TE_FLAG_ZPLUS_TENSOR_CORES) && te_tc_zplus_supported(rows, in_features, out_features, in_features)) {
         const TcScratch c = tc_scratch(scratch, (long long)rows * out_features, in_features, out_features, 0);   // operand: |x|
@@ -223,7 +222,19 @@ extern "C" int te_linear_relprop_ex(const float* x, const float* w, const float*
         xabs = c.op;
     }
     return te_zplus_linear_relprop_ldr(x, in_features, w, derived, r, out_features, out, scratch, rows, in_features,
-                                       out_features, ST(stream), y, out_features, bias, te_zplus_from_flags(flags), 0, xabs);
+                                       out_features, ST(stream), y, out_features, bias, te_zplus_from_flags(flags), 0, xabs,
+                                       alpha);
+}
+
+extern "C" int te_linear_relprop(const float* x, const float* w, const float* r, float* out, float* scratch, int rows,
+                                 int in_features, int out_features, unsigned flags, void* stream) {
+    return te_linear_relprop_alpha(x, w, nullptr, nullptr, r, out, scratch, rows, in_features, out_features, 1.f, flags, stream);
+}
+
+extern "C" int te_linear_relprop_ex(const float* x, const float* w, const float* bias, const float* y, const float* r,
+                                    float* out, float* scratch, int rows, int in_features, int out_features,
+                                    unsigned flags, void* stream) {
+    return te_linear_relprop_alpha(x, w, bias, y, r, out, scratch, rows, in_features, out_features, 1.f, flags, stream);
 }
 
 extern "C" int te_add_relprop(const float* x1, const float* x2, const float* r, float* r1, float* r2, void* scratch,

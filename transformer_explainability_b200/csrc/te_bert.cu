@@ -292,8 +292,16 @@ extern "C" int te_bert_forward(const te_bert_config* cfg, const float* weights, 
 extern "C" int te_bert_attribute(const te_bert_config* cfg, const float* weights, const float* derived, int batch,
                                  int seq, int* index, int start_layer, unsigned flags, float* maps, void* workspace,
                                  long long workspace_bytes, void* stream) {
+    return te_bert_attribute_alpha(cfg, weights, derived, batch, seq, index, start_layer, 1.f, flags, maps, workspace,
+                                   workspace_bytes, stream);
+}
+
+extern "C" int te_bert_attribute_alpha(const te_bert_config* cfg, const float* weights, const float* derived, int batch,
+                                       int seq, int* index, int start_layer, float alpha, unsigned flags, float* maps,
+                                       void* workspace, long long workspace_bytes, void* stream) {
     Dims d; Workspace ws;
     TE_TRY(check_ws(cfg, batch, seq, workspace, workspace_bytes, d, ws));
+    if (!isfinite(alpha)) { te_set_last_error("te_bert_attribute: alpha must be finite"); return TE_ERR_ARG; }
     if (!weights || !index || (!maps && !(flags & TE_FLAG_GRADIENTS_ONLY))) { te_set_last_error("te_bert_attribute: null pointer"); return TE_ERR_ARG; }
     if (start_layer < 0 || start_layer >= d.L) { te_set_last_error("te_bert_attribute: start_layer out of range"); return TE_ERR_ARG; }
     // fp16 backward split of dy in tF[1], block scales in t3D[1] (idle until the relprop)
@@ -345,14 +353,16 @@ extern "C" int te_bert_attribute(const te_bert_config* cfg, const float* weights
     float* RF = ws.tF[0]; float* SF = ws.tF[1]; float* S = ws.t3D[0]; float* Rqkv = ws.t3D[1];
     // Linear / Add rules of the selected rule library: layers_ours, or with TE_FLAG_RULES_LRP layers_lrp (BERT_cls_lrp.py on
     // BERT_orig_lrp.py: Linear with separate denominators, Add = RelPropSimple, also for the attention-mask Add).  dw is set
-    // for the z+ rules with TE_FLAG_ZPLUS_TENSOR_CORES, for the layers_lrp rule with TE_FLAG_RULES_LRP_TC.
+    // for the z+ rules with TE_FLAG_ZPLUS_TENSOR_CORES, for the layers_lrp rule with TE_FLAG_RULES_LRP_TC.  alpha != 1: the
+    // alpha-beta Linear rule of either library.
     const bool lrpv = (flags & TE_FLAG_RULES_LRP) != 0;
     double* addp = lrpv ? nullptr : ws.addpart;
     auto lin = [&](const float* x, long long ldx, const float* wt, const float* dwt, const float* r, long long ldr, float* out,
                    float* sbuf, long long rows, int in, int outf, const float* y, long long ldy, const float* bias,
                    long long ld_out, float* xabs) -> int {
-        if (lrpv) return te_zplus_linear_relprop_lrp(x, ldx, wt, dwt, r, ldr, out, sbuf, rows, in, outf, st, ld_out);
-        return te_zplus_linear_relprop_ldr(x, ldx, wt, dwt, r, ldr, out, sbuf, rows, in, outf, st, y, ldy, bias, sel.zv, ld_out, xabs);
+        if (lrpv) return te_zplus_linear_relprop_lrp(x, ldx, wt, dwt, r, ldr, out, sbuf, rows, in, outf, st, ld_out, alpha);
+        return te_zplus_linear_relprop_ldr(x, ldx, wt, dwt, r, ldr, out, sbuf, rows, in, outf, st, y, ldy, bias, sel.zv, ld_out, xabs,
+                                           alpha);
     };
     // classifier.relprop (X = pooled) ; dropout / Tanh identity ; pooler.dense.relprop (X = first token) ; pool
     TE_TRY(lin(ws.pooled, d.D, w.clsw, nullptr, ws.seed, d.C, ws.rpool, ws.shead, d.B, d.D, d.C, nullptr, 0, nullptr, 0, nullptr));

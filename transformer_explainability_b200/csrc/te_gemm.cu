@@ -70,9 +70,9 @@ __device__ __forceinline__ void epilogue4(const TeGemm& p, float* __restrict__ C
     if (row >= p.M || col >= p.N) return;
     const int nv = min(4, p.N - col);
     float e[4] = {0.f, 0.f, 0.f, 0.f}, c[4] = {0.f, 0.f, 0.f, 0.f}, o[4], o2[4] = {0.f, 0.f, 0.f, 0.f};
-    constexpr bool needE = (EPI == TE_EPI_BIAS_ADD || EPI == TE_EPI_GELU_BWD || EPI == TE_EPI_SD ||
-                            EPI == TE_EPI_MUL || EPI == TE_EPI_MULPOS || EPI == TE_EPI_MULNEG_ACC);
-    constexpr bool needC = (EPI == TE_EPI_MULNEG_ACC || EPI == TE_EPI_ACCUM);
+    constexpr bool needE = (EPI == TE_EPI_BIAS_ADD || EPI == TE_EPI_GELU_BWD || EPI == TE_EPI_SD || EPI == TE_EPI_SD_SCALED ||
+                            EPI == TE_EPI_MUL || EPI == TE_EPI_MULPOS || EPI == TE_EPI_MULNEG_ACC || EPI == TE_EPI_MULPOS_ACC);
+    constexpr bool needC = (EPI == TE_EPI_MULNEG_ACC || EPI == TE_EPI_MULPOS_ACC || EPI == TE_EPI_ACCUM);
     constexpr bool hasC2 = (EPI == TE_EPI_BIAS_GELU || EPI == TE_EPI_BIAS_ADD);
     const long long co = (long long)row * p.ldc + col;
     if (needE) {
@@ -102,9 +102,11 @@ __device__ __forceinline__ void epilogue4(const TeGemm& p, float* __restrict__ C
         else if (EPI == TE_EPI_BIAS_ADD) { o[j] = a + bj; o2[j] = e[j] + o[j]; }
         else if (EPI == TE_EPI_GELU_BWD) o[j] = a * te_gelu_grad(e[j]);
         else if (EPI == TE_EPI_SD) o[j] = te_sd(e[j], p.alpha * a);
+        else if (EPI == TE_EPI_SD_SCALED) o[j] = p.scale * te_sd(e[j], p.alpha * a);
         else if (EPI == TE_EPI_MUL) o[j] = p.alpha * a * e[j];
         else if (EPI == TE_EPI_MULPOS) o[j] = fmaxf(e[j], 0.f) * a;
         else if (EPI == TE_EPI_MULNEG_ACC) o[j] = c[j] + fminf(e[j], 0.f) * a;
+        else if (EPI == TE_EPI_MULPOS_ACC) o[j] = c[j] + fmaxf(e[j], 0.f) * a;
         else o[j] = c[j] + p.alpha * a;   // ACCUM
     }
     if (nv == 4 && p.vecC) *reinterpret_cast<float4*>(C + co) = make_float4(o[0], o[1], o[2], o[3]);
@@ -141,7 +143,8 @@ __global__ void __launch_bounds__(256, (TM == 8) ? 2 : 3) te_gemm_kernel(const T
     const float* __restrict__ E0 = p.E0 ? p.E0 + b1 * p.sE1 + b2 * p.sE2 : nullptr;
 
     const int T = (p.K + BK - 1) / BK;
-    const int ntiles = (XF == TE_XF_AB_POSNEG) ? 2 * T : T;
+    constexpr bool KCAT = (XF == TE_XF_AB_POSNEG || XF == TE_XF_AB_NEGPOS);   // K-concatenated: two phases over K
+    const int ntiles = KCAT ? 2 * T : T;
 
     float acc[TM][TM];
 #pragma unroll
@@ -153,14 +156,17 @@ __global__ void __launch_bounds__(256, (TM == 8) ? 2 : 3) te_gemm_kernel(const T
 
     auto gload = [&](int t) {
         int k0 = t * BK, amode = 0, bmode = 0;
-        if (XF == TE_XF_AB_POSNEG) {
+        if (KCAT) {
             const int ph = (t >= T) ? 1 : 0;
             k0 = (t - ph * T) * BK;
-            amode = bmode = ph + 1;
+            amode = ph + 1;
+            bmode = (XF == TE_XF_AB_POSNEG) ? ph + 1 : 2 - ph;    // NEGPOS: x+ with W-, then x- with W+
         } else if (XF == TE_XF_B_POS) bmode = 1;
         else if (XF == TE_XF_B_NEG) bmode = 2;
         else if (XF == TE_XF_AB_POS) amode = bmode = 1;         // x+ W+^T  (layers_lrp Linear rule: separate denominators)
         else if (XF == TE_XF_AB_NEG) amode = bmode = 2;         // x- W-^T
+        else if (XF == TE_XF_A_POS_B_NEG) { amode = 1; bmode = 2; }   // x+ W-^T  (layers_lrp inhibitor half)
+        else if (XF == TE_XF_A_NEG_B_POS) { amode = 2; bmode = 1; }   // x- W+^T
 #pragma unroll
         for (int i = 0; i < NLD; ++i) {
             ra[i] = clamp4(load_tile4<TM, ALAY>(A, p.lda, p.M, p.K, m0, k0, tid + i * 256, p.vecA), amode);
@@ -242,6 +248,9 @@ int launch_tm(const TeGemm& p, cudaStream_t st) {
 
 #define TE_CASE(AL, BL, X, E) \
     if (alay == AL && blay == BL && xf == X && epi == E) return launch_tm<AL, BL, X, E>(p, st);
+// small tiles only: at 128 x 128 these variants spill under the two-CTA register cap
+#define TE_CASE4(AL, BL, X, E) \
+    if (alay == AL && blay == BL && xf == X && epi == E) return launch_one<4, AL, BL, X, E>(p, st);
 
 int te_gemm_launch(TeGemm p, int alay, int blay, int xf, int epi, cudaStream_t st) {
     if (p.M <= 0 || p.N <= 0 || p.K <= 0 || p.nb1 <= 0 || p.nb2 <= 0) return TE_OK;
@@ -268,6 +277,15 @@ int te_gemm_launch(TeGemm p, int alay, int blay, int xf, int epi, cudaStream_t s
     TE_CASE(TE_L_K, TE_L_K, TE_XF_AB_NEG, TE_EPI_SD)
     TE_CASE(TE_L_K, TE_L_MN, TE_XF_B_POS, TE_EPI_MULPOS)
     TE_CASE(TE_L_K, TE_L_MN, TE_XF_B_NEG, TE_EPI_MULNEG_ACC)
+    // relprop, alpha-beta rule (alpha != 1): S scaled by alpha / -beta, the inhibitor half with the weight signs swapped
+    TE_CASE4(TE_L_K, TE_L_K, TE_XF_AB_POSNEG, TE_EPI_SD_SCALED)
+    TE_CASE4(TE_L_K, TE_L_K, TE_XF_AB_NEGPOS, TE_EPI_SD_SCALED)
+    TE_CASE4(TE_L_K, TE_L_K, TE_XF_AB_POS, TE_EPI_SD_SCALED)
+    TE_CASE4(TE_L_K, TE_L_K, TE_XF_AB_NEG, TE_EPI_SD_SCALED)
+    TE_CASE4(TE_L_K, TE_L_K, TE_XF_A_POS_B_NEG, TE_EPI_SD_SCALED)
+    TE_CASE4(TE_L_K, TE_L_K, TE_XF_A_NEG_B_POS, TE_EPI_SD_SCALED)
+    TE_CASE4(TE_L_K, TE_L_MN, TE_XF_B_NEG, TE_EPI_MULPOS_ACC)
+    TE_CASE4(TE_L_K, TE_L_MN, TE_XF_B_POS, TE_EPI_MULNEG_ACC)
     TE_CASE(TE_L_K, TE_L_K, TE_XF_NONE, TE_EPI_SD)
     TE_CASE(TE_L_K, TE_L_K, TE_XF_NONE, TE_EPI_MUL)
     TE_CASE(TE_L_MN, TE_L_MN, TE_XF_NONE, TE_EPI_MUL)

@@ -16,7 +16,12 @@
 #include "te_common.cuh"
 
 enum { TE_L_K = 0, TE_L_MN = 1 };
-enum { TE_XF_NONE = 0, TE_XF_AB_POSNEG = 1, TE_XF_B_POS = 2, TE_XF_B_NEG = 3, TE_XF_AB_POS = 4, TE_XF_AB_NEG = 5 };
+// AB_POSNEG: [A+ | A-] [B+ | B-]^T (the reduction runs over both halves) ; AB_NEGPOS: [A+ | A-] [B- | B+]^T (the inhibitor
+// denominator of the alpha-beta rule) ; A_POS_B_NEG / A_NEG_B_POS: the mixed-sign products of the layers_lrp inhibitor half
+enum {
+    TE_XF_NONE = 0, TE_XF_AB_POSNEG = 1, TE_XF_B_POS = 2, TE_XF_B_NEG = 3, TE_XF_AB_POS = 4, TE_XF_AB_NEG = 5,
+    TE_XF_AB_NEGPOS = 6, TE_XF_A_POS_B_NEG = 7, TE_XF_A_NEG_B_POS = 8
+};
 enum {
     TE_EPI_STORE = 0,      // C = alpha*acc
     TE_EPI_BIAS = 1,       // C = acc + bias[n]
@@ -27,7 +32,9 @@ enum {
     TE_EPI_MUL = 6,        // C = alpha * acc * E0
     TE_EPI_MULPOS = 7,     // C  = max(E0,0) * acc
     TE_EPI_MULNEG_ACC = 8, // C += min(E0,0) * acc
-    TE_EPI_ACCUM = 9       // C += alpha*acc
+    TE_EPI_ACCUM = 9,      // C += alpha*acc
+    TE_EPI_SD_SCALED = 10, // C = scale * safe_divide(E0, alpha*acc)
+    TE_EPI_MULPOS_ACC = 11 // C += max(E0,0) * acc
 };
 
 struct TeGemm {
@@ -37,6 +44,7 @@ struct TeGemm {
     long long sA1, sA2, sB1, sB2, sC1, sC2, sE1, sE2, sD1, sD2;   // D = C2
     int nb1, nb2;
     float alpha;
+    float scale;                          // TE_EPI_SD_SCALED only
     int vecA, vecB, vecC, vecC2, vecE;   // filled by te_gemm_launch
 };
 

@@ -60,13 +60,15 @@ int te_tc_prepare_weights(const float* w, float* derived, int in_features, int o
 int te_tc_zplus_linear_relprop(const float* x, long long ldx, const float* derived, const float* r, long long ldr,
                                float* out, float* s_scratch, long long rows, int in_features, int out_features, cudaStream_t st,
                                const float* y, long long ldy, const float* bias, ZplusVariant zv, long long ld_out,
-                               float* xabs);
+                               float* xabs, float alpha = 1.f);
+// alpha != 1 (the alpha-beta rule of te_zplus.h): the inhibitor half follows the activator through s_scratch, the same kernels
+// with the weight operands swapped, the single-pass S kernel with the |x| |W|^T term negated and the R kernel accumulating.
 // Linear.relprop of the layers_lrp library (te_zplus_linear_relprop_lrp) on single-pass TF32 wgmma: for each half in turn,
 // S = sd(R, x+- W+-^T) into s_scratch [rows, out], then out (+)= x+- * (S W+-).  Row strides ldx, ldr, ld_out; shapes as
-// te_tc_zplus_supported.
+// te_tc_zplus_supported.  alpha != 1: the inhibitor products x+ W-, x- W+ follow, every S scaled by alpha or -beta.
 int te_tc_lrp_linear_relprop(const float* x, long long ldx, const float* derived, const float* r, long long ldr, float* out,
                              long long ld_out, float* s_scratch, long long rows, int in_features, int out_features,
-                             cudaStream_t st);
+                             cudaStream_t st, float alpha = 1.f);
 
 // fp32-grade (3xTF32 split) Linear GEMMs; epilogues mirror the SIMT ones
 enum { TE_TC_EPI_STORE = 0, TE_TC_EPI_BIAS = 1, TE_TC_EPI_BIAS_GELU = 2, TE_TC_EPI_BIAS_ADD = 3, TE_TC_EPI_GELU_BWD = 4 };
@@ -96,7 +98,7 @@ int te_tc_linear_bwd16(const float* dy, long long lddy, float* split, float* sca
                        int out_features, float* dx, const float* e0, long long rows, int epi, cudaStream_t st);
 // R_in = x+ (S W+) + x- (S W-): split / scale hold the hi-only split of S [rows, out] (s != NULL: pre-pass here)
 int te_tc_zplus_r16(const float* s, float* split, float* scale, const float* derived, const float* x, long long ldx, float* out,
-                    long long ld_out, long long rows, int in_features, int out_features, cudaStream_t st);
+                    long long ld_out, long long rows, int in_features, int out_features, cudaStream_t st, bool inh = false);
 
 // attention-shaped N x N contractions (Q K^T, dctx V^T, S2 V^T), fp32-grade 3xTF32, head slices in place
 enum { TE_TC_ATTN_STORE = 0, TE_TC_ATTN_MUL = 1, TE_TC_ATTN_SD = 2, TE_TC_ATTN_SOFTMAX = 3 };   // SOFTMAX: N <= 256
@@ -121,10 +123,13 @@ int te_tc_bmm_nk_resid(const float* A, const float* J, const float* rowscale, fl
 // xabs: scratch [rows, in] for bf16(|x|), the A operand of the bf16 single-pass S kernel
 int te_tc_zplus_s1(const float* x, long long ldx, float* xabs, const float* derived, const float* r, long long ldr,
                    const float* y, long long ldy, const float* bias, float* s_out, long long rows, int in_features,
-                   int out_features, cudaStream_t st, bool bf16 = false, float* s16 = nullptr, float* s16_scale = nullptr);
+                   int out_features, cudaStream_t st, bool bf16 = false, float* s16 = nullptr, float* s16_scale = nullptr,
+                   float s_scale = 1.f, bool inh = false);
 // s16 / s16_scale: when given, S leaves as hi-only block-scaled fp16 [rows, out] (+ [rows, out/128] scales) — the A operand of
-// te_tc_zplus_r16 — instead of fp32 in s_out
+// te_tc_zplus_r16 — instead of fp32 in s_out.  s_scale: S = s_scale * sd(R, Z) ; inh: the inhibitor denominator
+// ((y - bias) - |x| |W|^T) / 2 of the alpha-beta rule.
+// inh (te_tc_zplus_r, te_tc_zplus_r16): the inhibitor half, out += x+ (S W-) + x- (S W+)
 int te_tc_zplus_r(const float* s, const float* derived, const float* x, long long ldx, float* out, long long ld_out,
-                  long long rows, int in_features, int out_features, cudaStream_t st);
+                  long long rows, int in_features, int out_features, cudaStream_t st, bool inh = false);
 int te_tc_linear_bwd_tf32(const float* dy, long long lddy, const float* derived, int in_features, int out_features, float* dx,
                           const float* e0, long long rows, int epi, cudaStream_t st);

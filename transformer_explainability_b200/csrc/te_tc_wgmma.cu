@@ -258,6 +258,9 @@ struct NoScale {
 // ---- z+ rule, first contraction: S = sd(R, Z) ---------------------------------------------------------------------
 // Z two-pass:    x+ W+^T + x- W-^T                        (A tiles x+ / x- transformed on load, B = W+ / W-)
 // Z single-pass: ((y - bias) + |x| |W|^T) / 2             (the saved forward output y = x W^T + bias)
+// The inhibitor half of the alpha-beta rule swaps the weight signs: two-pass with B = W- / W+ (wa / wb), single-pass with
+// zsign = -1, Z = ((y - bias) - |x| |W|^T) / 2 == x+ W-^T + x- W+^T.  S leaves as sscale * sd(R, Z) (alpha or -beta; 1 for
+// the plain z+ rule).
 // OUT: 0 = S as TF32-rounded fp32, 1 = bf16, 2 = hi-only block-scaled fp16 (one 2^-e per row and 128 columns)
 enum { ZO_F32 = 0, ZO_BF16 = 1, ZO_F16S = 2 };
 template <bool SINGLE, bool BF, int OUT>
@@ -272,6 +275,7 @@ struct ZsProb : NoScale {
     const void* wa; const void* wb;         // SINGLE: |W| (tf32 or bf16) ; else W+ / W- (tf32) [N, K]
     const float* r; long long ldr; const float* y; long long ldy; const float* bias;
     void* out; long long ldo; float* hs;    // hs: ZO_F16S block scales [M, N / 128]
+    float sscale, zsign;                    // S = sscale * sd(R, Z) ; SINGLE: sign of the |x| |W|^T term
 
     __device__ int kblocks() const { return K / (BF ? 64 : 32); }
     __device__ void load(uint8_t* st, int kb, int m0, int n0, int, int tid) const {
@@ -305,13 +309,14 @@ struct ZsProb : NoScale {
                     const float2 yy = *reinterpret_cast<const float2*>(y + (long long)row * ldy + col);
                     const float2 bb = bias ? *reinterpret_cast<const float2*>(bias + col) : make_float2(0.f, 0.f);
                     // x+ W+^T + x- W-^T == (x W^T + |x| |W|^T) / 2 ; a negative result is cancellation noise of a sum of
-                    // non-negative terms
-                    z.x = fmaxf(0.5f * ((yy.x - bb.x) + z.x), 0.f);
-                    z.y = fmaxf(0.5f * ((yy.y - bb.y) + z.y), 0.f);
+                    // non-negative terms (zsign = -1: x+ W-^T + x- W+^T == (x W^T - |x| |W|^T) / 2, a sum of non-positive terms)
+                    z.x = 0.5f * ((yy.x - bb.x) + zsign * z.x);
+                    z.y = 0.5f * ((yy.y - bb.y) + zsign * z.y);
+                    z = zsign > 0.f ? make_float2(fmaxf(z.x, 0.f), fmaxf(z.y, 0.f)) : make_float2(fminf(z.x, 0.f), fminf(z.y, 0.f));
                 }
             }
-            sv[j] = te_sd(rr.x, z.x);
-            sv[j + 1] = te_sd(rr.y, z.y);
+            sv[j] = sscale * te_sd(rr.x, z.x);
+            sv[j + 1] = sscale * te_sd(rr.y, z.y);
             if (OUT == ZO_F16S) rmax[(j >> 1) & 1] = fmaxf(rmax[(j >> 1) & 1], fmaxf(fabsf(sv[j]), fabsf(sv[j + 1])));
             if (row >= M) continue;
             if (OUT == ZO_F32) {
@@ -345,6 +350,8 @@ struct ZsProb : NoScale {
 
 // ---- z+ rule, second contraction: R_in = x+ (S W+) + x- (S W-) --------------------------------------------------------
 // KIND 0: S and W+-^T TF32 fp32 ; 1: bf16 ; 2: block-scaled fp16 S (scale per row and 128 k) with row-scaled fp16 W+-^T
+// The inhibitor half of the alpha-beta rule passes the weights swapped (wp = W-^T, wn = W+^T and their scales) with accum
+// set: R_in += x+ (S W-) + x- (S W+).
 template <int KIND>
 struct ZrProb {
     static constexpr int BN = (KIND == 2) ? 64 : 128, CHUNK = (KIND == 2) ? 2 : 0;
@@ -356,6 +363,7 @@ struct ZrProb {
     const void* s; const void* wp; const void* wn;     // S [M, K] (row stride K), W+^T / W-^T [N, K]
     const float* rs; int rs_ld; const float* cp; const float* cn;   // KIND 2: scales of S, of the rows of W+^T / W-^T
     const float* x; long long ldx; float* out; long long ldo;
+    int accum;                                                      // add into out instead of overwriting it
 
     __device__ int kblocks() const { return K / (KIND ? 64 : 32); }
     __device__ float chunk_scale(int row, int ch, int) const { return (KIND == 2 && row < M) ? rs[(long long)row * rs_ld + ch] : 1.f; }
@@ -381,8 +389,13 @@ struct ZrProb {
                 ap.x *= cp[col]; ap.y *= cp[col + 1];
                 an.x *= cn[col]; an.y *= cn[col + 1];
             }
-            *reinterpret_cast<float2*>(out + (long long)row * ldo + col) =
-                make_float2(fmaxf(xv.x, 0.f) * ap.x + fminf(xv.x, 0.f) * an.x, fmaxf(xv.y, 0.f) * ap.y + fminf(xv.y, 0.f) * an.y);
+            float2* o = reinterpret_cast<float2*>(out + (long long)row * ldo + col);
+            float2 v = make_float2(fmaxf(xv.x, 0.f) * ap.x + fminf(xv.x, 0.f) * an.x, fmaxf(xv.y, 0.f) * ap.y + fminf(xv.y, 0.f) * an.y);
+            if (accum) {
+                const float2 prev = *o;
+                v = make_float2(prev.x + v.x, prev.y + v.y);
+            }
+            *o = v;
         }
     }
 };
@@ -390,7 +403,9 @@ struct ZrProb {
 // ---- Linear rule of the layers_lrp library: each half over its own denominator --------------------------------------
 // S half:  S = sd(R, x+- W+-^T), TF32-rounded fp32 [M, N] (A = tf32(x+) or tf32(x-) transformed on load, B = W+ / W-).
 // Both factors of every product share a sign, so the denominator is a sum of non-negative terms: no cancellation, and it
-// is exactly 0 (S = 0) only when every term is.
+// is exactly 0 (S = 0) only when every term is.  The inhibitor products of the alpha-beta rule pair x+ with W- and x- with
+// W+ (w is a runtime operand; NEG is the sign of x only): sums of non-positive terms, equally well conditioned.
+// S leaves scaled by sscale (alpha, -beta, or 1 for the plain rule).
 template <bool NEG>
 struct LrpSProb : NoScale {
     static constexpr int BN = 128, CHUNK = 0, FMT = OP_TF32;
@@ -400,6 +415,7 @@ struct LrpSProb : NoScale {
     int M, N, K;
     const float* x; long long ldx; const float* w;      // w: W+ or W- (tf32) [N, K]
     const float* r; long long ldr; float* out;           // out: S [M, N], row stride N
+    float sscale;
     __device__ int kblocks() const { return K / 32; }
     __device__ void load(uint8_t* st, int kb, int m0, int n0, int, int tid) const {
         for_k32(BM, x, ldx, m0, M, kb * 32, K, tid, [&](int rr, int c, float4 v) { st4(st + L::a(0), rr, c, tf32x4(NEG ? negx4(v) : posx4(v))); });
@@ -412,11 +428,12 @@ struct LrpSProb : NoScale {
             if (row >= M) continue;
             const float2 rr = *reinterpret_cast<const float2*>(r + (long long)row * ldr + col);
             *reinterpret_cast<float2*>(out + (long long)row * N + col) =
-                make_float2(to_tf32(te_sd(rr.x, acc[0][j])), to_tf32(te_sd(rr.y, acc[0][j + 1])));
+                make_float2(to_tf32(sscale * te_sd(rr.x, acc[0][j])), to_tf32(sscale * te_sd(rr.y, acc[0][j + 1])));
         }
     }
 };
-// R half:  out = x+ * (S W+)  (NEG false),  out += x- * (S W-)  (NEG true).  A = S [M, K], B = W+^T / W-^T [N, K].
+// R half:  out = x+ * (S W+)  (NEG false),  out += x- * (S W-)  (NEG true).  A = S [M, K], B = W+^T / W-^T [N, K] (W-^T /
+// W+^T for the inhibitor products).  accum: the NEG false half adds into out as well (every product after the first).
 template <bool NEG>
 struct LrpRProb : NoScale {
     static constexpr int BN = 128, CHUNK = 0, FMT = OP_TF32;
@@ -426,6 +443,7 @@ struct LrpRProb : NoScale {
     int M, N, K;
     const float* s; const float* wt;
     const float* x; long long ldx; float* out; long long ldo;
+    int accum;
     __device__ int kblocks() const { return K / 32; }
     __device__ void load(uint8_t* st, int kb, int m0, int n0, int, int tid) const {
         for_k32(BM, s, K, m0, M, kb * 32, K, tid, [&](int rr, int c, float4 v) { st4(st + L::a(0), rr, c, v); });
@@ -441,6 +459,9 @@ struct LrpRProb : NoScale {
             if (NEG) {
                 const float2 prev = *o;
                 *o = make_float2(prev.x + fminf(xv.x, 0.f) * acc[0][j], prev.y + fminf(xv.y, 0.f) * acc[0][j + 1]);
+            } else if (accum) {
+                const float2 prev = *o;
+                *o = make_float2(prev.x + fmaxf(xv.x, 0.f) * acc[0][j], prev.y + fmaxf(xv.y, 0.f) * acc[0][j + 1]);
             } else {
                 *o = make_float2(fmaxf(xv.x, 0.f) * acc[0][j], fmaxf(xv.y, 0.f) * acc[0][j + 1]);
             }
@@ -848,12 +869,13 @@ int linear(int K, const void* a, const void* a_lo, long long lda, const void* b,
 template <bool SINGLE, bool BF, int OUT>
 int zs(const float* x, long long ldx, const void* xabs, const void* wa, const void* wb, const float* r, long long ldr,
        const float* y, long long ldy, const float* bias, void* out, float* hs, long long rows, int in_features, int out_features,
-       cudaStream_t st) {
+       cudaStream_t st, float s_scale, bool inh) {
     ZsProb<SINGLE, BF, OUT> p;
     p.M = (int)rows; p.N = out_features; p.K = in_features;
     p.x = x; p.ldx = ldx; p.xabs = xabs; p.wa = wa; p.wb = wb;
     p.r = r; p.ldr = ldr; p.y = y; p.ldy = ldy; p.bias = bias;
     p.out = out; p.ldo = out_features; p.hs = hs;
+    p.sscale = s_scale; p.zsign = inh ? -1.f : 1.f;
     return launch(p, dim3(mtiles(p.M), p.N / 128), st);
 }
 
@@ -910,7 +932,7 @@ bool te_tc_zplus_supported(long long rows, int in_features, int out_features, lo
 }
 int te_tc_zplus_s1(const float* x, long long ldx, float* xabs, const float* derived, const float* r, long long ldr,
                    const float* y, long long ldy, const float* bias, float* s_out, long long rows, int in_features,
-                   int out_features, cudaStream_t st, bool bf16, float* s16, float* s16_scale) {
+                   int out_features, cudaStream_t st, bool bf16, float* s16, float* s16_scale, float s_scale, bool inh) {
     const TeDerived<const float> dv(derived, in_features, out_features);
     if (ldx % 4 != 0 || !a16(x) || !a16(r) || !a16(y) || ldr % 2 != 0 || ldy % 2 != 0) {
         te_set_last_error("te_tc_zplus_s1: alignment");
@@ -918,7 +940,8 @@ int te_tc_zplus_s1(const float* x, long long ldx, float* xabs, const float* deri
     }
     void* o = s16 ? (void*)s16 : (void*)s_out;
     auto run = [&](auto zs_fn, const void* wa) {
-        return zs_fn(x, ldx, xabs, wa, nullptr, r, ldr, y, ldy, bias, o, s16_scale, rows, in_features, out_features, st);
+        return zs_fn(x, ldx, xabs, wa, nullptr, r, ldr, y, ldy, bias, o, s16_scale, rows, in_features, out_features, st, s_scale,
+                     inh);
     };
     if (bf16 && in_features % 64 == 0) {
         if (!a16(xabs)) { te_set_last_error("te_tc_zplus_s1: alignment"); return TE_ERR_ARG; }
@@ -931,17 +954,18 @@ int te_tc_zplus_s1(const float* x, long long ldx, float* xabs, const float* deri
 }
 
 int te_tc_zplus_r(const float* s, const float* derived, const float* x, long long ldx, float* out, long long ld_out,
-                  long long rows, int in_features, int out_features, cudaStream_t st) {
+                  long long rows, int in_features, int out_features, cudaStream_t st, bool inh) {
     const TeDerived<const float> dv(derived, in_features, out_features);
     ZrProb<0> p;
     memset(&p, 0, sizeof(p));
     p.M = (int)rows; p.N = in_features; p.K = out_features;
-    p.s = s; p.wp = dv.wpt; p.wn = dv.wnt; p.x = x; p.ldx = ldx; p.out = out; p.ldo = ld_out;
+    p.s = s; p.wp = inh ? dv.wnt : dv.wpt; p.wn = inh ? dv.wpt : dv.wnt; p.x = x; p.ldx = ldx; p.out = out; p.ldo = ld_out;
+    p.accum = inh;
     return launch(p, dim3(mtiles(rows), in_features / 128), st);
 }
 
 int te_tc_zplus_r16(const float* s, float* split, float* scale, const float* derived, const float* x, long long ldx, float* out,
-                    long long ld_out, long long rows, int in_features, int out_features, cudaStream_t st) {
+                    long long ld_out, long long rows, int in_features, int out_features, cudaStream_t st, bool inh) {
     const TeDerived<const float> dv(derived, in_features, out_features);
     if (!a16(split) || !scale || !a16(derived) || !a16(x) || !a16(out) || ldx % 4 != 0 || ld_out % 4 != 0) {
         te_set_last_error("te_tc_zplus_r16: bad operands");
@@ -950,20 +974,18 @@ int te_tc_zplus_r16(const float* s, float* split, float* scale, const float* der
     if (s) TE_TRY(te_tc_blocksplit_f16(s, out_features, rows, out_features, split, scale, st, true));
     ZrProb<2> p;
     p.M = (int)rows; p.N = in_features; p.K = out_features;
-    p.s = split; p.wp = dv.h_wpt; p.wn = dv.h_wnt;
-    p.rs = scale; p.rs_ld = (out_features + 127) / 128; p.cp = dv.s_wpt; p.cn = dv.s_wnt;
-    p.x = x; p.ldx = ldx; p.out = out; p.ldo = ld_out;
+    p.s = split; p.wp = inh ? dv.h_wnt : dv.h_wpt; p.wn = inh ? dv.h_wpt : dv.h_wnt;
+    p.rs = scale; p.rs_ld = (out_features + 127) / 128; p.cp = inh ? dv.s_wnt : dv.s_wpt; p.cn = inh ? dv.s_wpt : dv.s_wnt;
+    p.x = x; p.ldx = ldx; p.out = out; p.ldo = ld_out; p.accum = inh;
     return launch(p, dim3(mtiles(rows), in_features / 64), st);
 }
 
-int te_tc_zplus_linear_relprop(const float* x, long long ldx, const float* derived, const float* r, long long ldr,
-                               float* out, float* s_scratch, long long rows, int in_features, int out_features, cudaStream_t st,
-                               const float* y, long long ldy, const float* bias, ZplusVariant zv, long long ld_out, float* xabs) {
-    if (ld_out == 0) ld_out = in_features;
-    if (!a16(x) || !a16(derived) || !a16(r) || !a16(out) || !a16(s_scratch)) {
-        te_set_last_error("te_gemm_tc: operands must be 16-byte aligned");
-        return TE_ERR_ARG;
-    }
+namespace {
+// One half of the z+ / alpha-beta rule: S = s_scale * sd(R, Z) into s_scratch, then out = x+ (S W+) + x- (S W-); the inhibitor
+// half (inh) swaps the weight signs in both contractions and adds into out.
+int zplus_half(const float* x, long long ldx, const float* derived, const float* r, long long ldr, float* out, float* s_scratch,
+               long long rows, int in_features, int out_features, cudaStream_t st, const float* y, long long ldy,
+               const float* bias, ZplusVariant zv, long long ld_out, float* xabs, float s_scale, bool inh) {
     const TeDerived<const float> dv(derived, in_features, out_features);
     const bool single = y && a16(y) && ldy % 4 == 0 && (!bias || a16(bias));
     const bool rb = zv.r_bf16 && (out_features % 64 == 0);          // S as bf16, R kernel with bf16 operands
@@ -973,19 +995,20 @@ int te_tc_zplus_linear_relprop(const float* x, long long ldx, const float* deriv
             // ([rows, out] fp16, then the [rows, out/128] scales: rows*out floats hold both)
             float* s16_scale = s_scratch + ((rows * out_features / 2 + 63) & ~63LL);
             TE_TRY(te_tc_zplus_s1(x, ldx, xabs, derived, r, ldr, y, ldy, bias, nullptr, rows, in_features, out_features, st,
-                                  zv.s1_bf16, s_scratch, s16_scale));
-            return te_tc_zplus_r16(nullptr, s_scratch, s16_scale, derived, x, ldx, out, ld_out, rows, in_features, out_features, st);
+                                  zv.s1_bf16, s_scratch, s16_scale, s_scale, inh));
+            return te_tc_zplus_r16(nullptr, s_scratch, s16_scale, derived, x, ldx, out, ld_out, rows, in_features, out_features, st,
+                                   inh);
         }
         TE_TRY(te_tc_zplus_s1(x, ldx, xabs, derived, r, ldr, y, ldy, bias, s_scratch, rows, in_features, out_features, st,
-                              zv.s1_bf16));
-        return te_tc_zplus_r(s_scratch, derived, x, ldx, out, ld_out, rows, in_features, out_features, st);
+                              zv.s1_bf16, nullptr, nullptr, s_scale, inh));
+        return te_tc_zplus_r(s_scratch, derived, x, ldx, out, ld_out, rows, in_features, out_features, st, inh);
     }
-    // S = sd(R, Z) [rows, out]: single-pass from y, or two-pass
+    // S = s_scale * sd(R, Z) [rows, out]: single-pass from y, or two-pass
     auto run = [&](auto zs_fn) {
         return single ? zs_fn(x, ldx, nullptr, dv.wabs, nullptr, r, ldr, y, ldy, bias, s_scratch, nullptr, rows,
-                              in_features, out_features, st)
-                      : zs_fn(x, ldx, nullptr, dv.wp, dv.wn, r, ldr, nullptr, 0, nullptr, s_scratch, nullptr, rows,
-                              in_features, out_features, st);
+                              in_features, out_features, st, s_scale, inh)
+                      : zs_fn(x, ldx, nullptr, inh ? dv.wn : dv.wp, inh ? dv.wp : dv.wn, r, ldr, nullptr, 0, nullptr, s_scratch,
+                              nullptr, rows, in_features, out_features, st, s_scale, inh);
     };
     if (single) TE_TRY(rb ? run(zs<true, false, ZO_BF16>) : run(zs<true, false, ZO_F32>));
     else TE_TRY(rb ? run(zs<false, false, ZO_BF16>) : run(zs<false, false, ZO_F32>));
@@ -993,39 +1016,66 @@ int te_tc_zplus_linear_relprop(const float* x, long long ldx, const float* deriv
         ZrProb<1> p;
         memset(&p, 0, sizeof(p));
         p.M = (int)rows; p.N = in_features; p.K = out_features;
-        p.s = s_scratch; p.wp = dv.bf_wpt; p.wn = dv.bf_wnt;
-        p.x = x; p.ldx = ldx; p.out = out; p.ldo = ld_out;
+        p.s = s_scratch; p.wp = inh ? dv.bf_wnt : dv.bf_wpt; p.wn = inh ? dv.bf_wpt : dv.bf_wnt;
+        p.x = x; p.ldx = ldx; p.out = out; p.ldo = ld_out; p.accum = inh;
         return launch(p, dim3(mtiles(rows), in_features / 128), st);
     }
-    return te_tc_zplus_r(s_scratch, derived, x, ldx, out, ld_out, rows, in_features, out_features, st);
+    return te_tc_zplus_r(s_scratch, derived, x, ldx, out, ld_out, rows, in_features, out_features, st, inh);
+}
+}  // namespace
+
+int te_tc_zplus_linear_relprop(const float* x, long long ldx, const float* derived, const float* r, long long ldr,
+                               float* out, float* s_scratch, long long rows, int in_features, int out_features, cudaStream_t st,
+                               const float* y, long long ldy, const float* bias, ZplusVariant zv, long long ld_out, float* xabs,
+                               float alpha) {
+    if (ld_out == 0) ld_out = in_features;
+    if (!a16(x) || !a16(derived) || !a16(r) || !a16(out) || !a16(s_scratch)) {
+        te_set_last_error("te_gemm_tc: operands must be 16-byte aligned");
+        return TE_ERR_ARG;
+    }
+    // activator (alpha = 1: the z+ rule, S unscaled), then for beta != 0 the inhibitor through the same S buffer
+    const float beta = alpha - 1.f;
+    TE_TRY(zplus_half(x, ldx, derived, r, ldr, out, s_scratch, rows, in_features, out_features, st, y, ldy, bias, zv, ld_out, xabs,
+                      alpha, false));
+    if (beta == 0.f) return TE_OK;
+    return zplus_half(x, ldx, derived, r, ldr, out, s_scratch, rows, in_features, out_features, st, y, ldy, bias, zv, ld_out, xabs,
+                      -beta, true);
 }
 
 namespace {
+// one product of the layers_lrp rule: x+ (NEG false) or x- (NEG true) with the weight w (w [out, in], wt its transpose);
+// S = s_scale * sd(R, x+- w^T), out (+)= x+- * (S w)
 template <bool NEG>
-int lrp_half(const float* x, long long ldx, const TeDerived<const float>& dv, const float* r, long long ldr, float* out,
-             long long ld_out, float* s, long long rows, int in_features, int out_features, cudaStream_t st) {
+int lrp_half(const float* x, long long ldx, const float* w, const float* wt, const float* r, long long ldr, float* out,
+             long long ld_out, float* s, long long rows, int in_features, int out_features, cudaStream_t st, float s_scale,
+             bool accum) {
     LrpSProb<NEG> ps;
     ps.M = (int)rows; ps.N = out_features; ps.K = in_features;
-    ps.x = x; ps.ldx = ldx; ps.w = NEG ? dv.wn : dv.wp; ps.r = r; ps.ldr = ldr; ps.out = s;
+    ps.x = x; ps.ldx = ldx; ps.w = w; ps.r = r; ps.ldr = ldr; ps.out = s; ps.sscale = s_scale;
     TE_TRY(launch(ps, dim3(mtiles(rows), out_features / 128), st));
     LrpRProb<NEG> pr;
     pr.M = (int)rows; pr.N = in_features; pr.K = out_features;
-    pr.s = s; pr.wt = NEG ? dv.wnt : dv.wpt; pr.x = x; pr.ldx = ldx; pr.out = out; pr.ldo = ld_out;
+    pr.s = s; pr.wt = wt; pr.x = x; pr.ldx = ldx; pr.out = out; pr.ldo = ld_out; pr.accum = accum;
     return launch(pr, dim3(mtiles(rows), in_features / 128), st);
 }
 }  // namespace
 
 int te_tc_lrp_linear_relprop(const float* x, long long ldx, const float* derived, const float* r, long long ldr, float* out,
                              long long ld_out, float* s_scratch, long long rows, int in_features, int out_features,
-                             cudaStream_t st) {
+                             cudaStream_t st, float alpha) {
     if (!a16(x) || !a16(derived) || !a16(r) || !a16(out) || !a16(s_scratch) || ldx % 4 != 0 || ldr % 4 != 0 || ld_out % 4 != 0) {
         te_set_last_error("te_tc_lrp_linear_relprop: operands must be 16-byte aligned");
         return TE_ERR_ARG;
     }
     const TeDerived<const float> dv(derived, in_features, out_features);
-    // the two halves in sequence through the one S buffer: x+ first (writes out), then x- (adds to it)
-    TE_TRY(lrp_half<false>(x, ldx, dv, r, ldr, out, ld_out, s_scratch, rows, in_features, out_features, st));
-    return lrp_half<true>(x, ldx, dv, r, ldr, out, ld_out, s_scratch, rows, in_features, out_features, st);
+    // the products in sequence through the one S buffer: x+ W+ first (writes out), then x- W- (adds to it); for beta != 0
+    // the inhibitor's x+ W-, x- W+ add to it as well, S scaled by alpha for the activator and -beta for the inhibitor
+    const float beta = alpha - 1.f;
+    TE_TRY(lrp_half<false>(x, ldx, dv.wp, dv.wpt, r, ldr, out, ld_out, s_scratch, rows, in_features, out_features, st, alpha, false));
+    TE_TRY(lrp_half<true>(x, ldx, dv.wn, dv.wnt, r, ldr, out, ld_out, s_scratch, rows, in_features, out_features, st, alpha, true));
+    if (beta == 0.f) return TE_OK;
+    TE_TRY(lrp_half<false>(x, ldx, dv.wn, dv.wnt, r, ldr, out, ld_out, s_scratch, rows, in_features, out_features, st, -beta, true));
+    return lrp_half<true>(x, ldx, dv.wp, dv.wpt, r, ldr, out, ld_out, s_scratch, rows, in_features, out_features, st, -beta, true);
 }
 
 // ---- Linear GEMMs ---------------------------------------------------------------------------------------------------

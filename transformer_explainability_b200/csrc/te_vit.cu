@@ -309,8 +309,16 @@ extern "C" int te_vit_prepare_derived(const te_vit_config* cfg, const float* wei
 extern "C" int te_vit_attribute(const te_vit_config* cfg, const float* weights, const float* derived, int batch,
                                 int* index, int start_layer, unsigned flags, float* maps, void* workspace,
                                 long long workspace_bytes, void* stream) {
+    return te_vit_attribute_alpha(cfg, weights, derived, batch, index, start_layer, 1.f, flags, maps, workspace, workspace_bytes,
+                                  stream);
+}
+
+extern "C" int te_vit_attribute_alpha(const te_vit_config* cfg, const float* weights, const float* derived, int batch,
+                                      int* index, int start_layer, float alpha, unsigned flags, float* maps, void* workspace,
+                                      long long workspace_bytes, void* stream) {
     Dims d; Workspace ws;
     TE_TRY(check_ws(cfg, batch, workspace, workspace_bytes, d, ws));
+    if (!isfinite(alpha)) { te_set_last_error("te_vit_attribute: alpha must be finite"); return TE_ERR_ARG; }
     if (!weights || !index || (!maps && !(flags & TE_FLAG_GRADIENTS_ONLY))) { te_set_last_error("te_vit_attribute: null pointer"); return TE_ERR_ARG; }
     if (start_layer < 0 || start_layer >= d.L) { te_set_last_error("te_vit_attribute: start_layer out of range"); return TE_ERR_ARG; }
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
@@ -368,12 +376,13 @@ extern "C" int te_vit_attribute(const te_vit_config* cfg, const float* weights, 
     float* RF = ws.tF[0]; float* SF = ws.tF[1]; float* S = ws.t3D[0]; float* Rqkv = ws.t3D[1]; float* S1 = ws.tA;
     // head.relprop (z+), pool.relprop (IndexSelect), norm.relprop (identity)
     // z+ rule / Add rule of the selected rule library (layers_ours, or layers_lrp with TE_FLAG_RULES_LRP; dwt is then set
-    // only with TE_FLAG_RULES_LRP_TC)
+    // only with TE_FLAG_RULES_LRP_TC); alpha != 1: the alpha-beta Linear rule of either library
     auto zrule = [&](const float* x, long long ldx, const float* wt, const float* dwt, const float* r, long long ldr, float* out,
                      float* sbuf, long long rows, int in, int outf, const float* y, long long ldy, const float* bias,
                      long long ld_out, float* xabs) -> int {
-        if (lrpv) return te_zplus_linear_relprop_lrp(x, ldx, wt, dwt, r, ldr, out, sbuf, rows, in, outf, st, ld_out);
-        return te_zplus_linear_relprop_ldr(x, ldx, wt, dwt, r, ldr, out, sbuf, rows, in, outf, st, y, ldy, bias, sel.zv, ld_out, xabs);
+        if (lrpv) return te_zplus_linear_relprop_lrp(x, ldx, wt, dwt, r, ldr, out, sbuf, rows, in, outf, st, ld_out, alpha);
+        return te_zplus_linear_relprop_ldr(x, ldx, wt, dwt, r, ldr, out, sbuf, rows, in, outf, st, y, ldy, bias, sel.zv, ld_out, xabs,
+                                           alpha);
     };
     auto addrule = [&](const float* x1, const float* x2, const float* r, float* r1, float* r2) -> int {
         return te_launch_add_relprop(x1, x2, r, r1, r2, lrpv ? nullptr : ws.addpart, d.B, (long long)d.N * d.D, st);

@@ -1,5 +1,9 @@
 // z+ rule of Linear.relprop (modules/layers_ours.py:207-230, alpha=1):
 //   Z = x+ W+^T + x- W-^T ; S = safe_divide(R, Z) ; R_in = x+ * (S W+) + x- * (S W-)
+// alpha-beta rule (alpha != 1, beta = alpha - 1): R_in = alpha * act - beta * inh, act the z+ result above and inh the same
+// rule with the weight signs swapped: S_i = sd(R, x+ W-^T + x- W+^T), inh = x+ * (S_i W-) + x- * (S_i W+).  The drivers run
+// the inhibitor half after the activator half through the same s_scratch, with alpha and -beta folded into S, adding into
+// out.  alpha = 1 launches exactly the z+ rule.  A non-finite alpha returns TE_ERR_ARG.
 #pragma once
 #include "te_common.cuh"
 
@@ -23,7 +27,7 @@ int te_zplus_linear_relprop_ldr(const float* x, long long ldx, const float* w, c
                                 long long ldr, float* out, float* s_scratch, long long rows, int in_features,
                                 int out_features, cudaStream_t st, const float* y = nullptr, long long ldy = 0,
                                 const float* bias = nullptr, ZplusVariant zv = {}, long long ld_out = 0,
-                                float* xabs = nullptr);
+                                float* xabs = nullptr, float alpha = 1.f);
 // xabs: scratch [rows, in] (the |x| operand of the single-pass S kernel); without it the tensor-core path uses the two-pass
 // S kernel.
 // ld_out: row stride of out (0 = in_features).  With row strides on x, r, y and out the rule runs on a strided subset of
@@ -31,9 +35,11 @@ int te_zplus_linear_relprop_ldr(const float* x, long long ldx, const float* w, c
 
 // Linear.relprop of the layers_lrp baseline variant (modules/layers_lrp.py:187-210, alpha=1): S1 = sd(R, x+ W+^T),
 // S2 = sd(R, x- W-^T) (separate denominators), R_in = x+ * (S1 W+) + x- * (S2 W-).  s_scratch [rows, out] holds S1, then S2.
+// alpha != 1: R_in = alpha * act - beta * inh with inh = x+ * (sd(R, x+ W-^T) W-) + x- * (sd(R, x- W+^T) W+), its two products
+// run after the activator's through the same s_scratch.
 // w_derived: the te_tc_prepare_weights() copies of w, or NULL.  When given (and the shape qualifies) both halves run on
 // single-pass TF32 wgmma (TE_FLAG_RULES_LRP_TC; every denominator is a sum of non-negative products); otherwise fp32 SIMT.
 // ld_out: row stride of out (0 = in_features), for the strided row subsets of te_zplus_linear_relprop_ldr.
 int te_zplus_linear_relprop_lrp(const float* x, long long ldx, const float* w, const float* w_derived, const float* r,
                                 long long ldr, float* out, float* s_scratch, long long rows, int in_features, int out_features,
-                                cudaStream_t st, long long ld_out = 0);
+                                cudaStream_t st, long long ld_out = 0, float alpha = 1.f);

@@ -133,12 +133,13 @@ class ViTEngine:
         return logits
 
     @_on_engine_device
-    def relprop_pixels(self, index=None, per_channel=False, flags=None):
+    def relprop_pixels(self, index=None, per_channel=False, flags=None, alpha=1.0):
         """``method="full"`` (ViT_LRP.py:337-343) on the activations of the last ``forward``: the relprop is run to
         the encoder input, through ``self.add`` and the patch convolution's z^B rule.  Returns the relevance of every
-        pixel, [B,H,W] (channels summed, what the reference returns) or [B,C,H,W] with ``per_channel``."""
+        pixel, [B,H,W] (channels summed, what the reference returns) or [B,C,H,W] with ``per_channel``.
+        alpha: as for ``attribute`` (the z^B rule of the patch convolution does not depend on it)."""
         fl = (self.flags if flags is None else flags) | _lib.FLAG_RELPROP_TO_INPUT
-        self.attribute(index=index, start_layer=0, flags=fl)
+        self.attribute(index=index, start_layer=0, flags=fl, alpha=alpha)
         b = self.last_batch
         images = getattr(self, "_last_images", None)
         if images is None or images.shape[0] != b:
@@ -152,9 +153,10 @@ class ViTEngine:
         return out
 
     @_on_engine_device
-    def attribute(self, index=None, start_layer=0, flags=None):
+    def attribute(self, index=None, start_layer=0, flags=None, alpha=1.0):
         """Backward + relprop + rollout on the activations of the last ``forward``.
-        Returns (maps [B,N-prefix], index [B] int32)."""
+        Returns (maps [B,N-prefix], index [B] int32).  alpha: ``model.relprop(..., alpha=alpha)``, the LRP-alpha-beta rule
+        (beta = alpha - 1) in every Linear.relprop; 1 is the z+ rule every generator uses."""
         b = self.last_batch
         if b <= 0:
             raise RuntimeError("attribute() needs a preceding forward()")
@@ -162,9 +164,9 @@ class ViTEngine:
         idx = self._index_tensor(index, b)
         maps = torch.empty(b, self.tokens - self.prefix, dtype=torch.float32, device=self.device)
         fl = self.flags if flags is None else flags
-        check(self.lib.te_vit_attribute(ctypes.byref(self.cfg), ptr(self.weights), ptr(self._derived(fl)), b, ptr(idx),
-                                        int(start_layer), fl, ptr(maps), ptr(ws), ws.numel() * 4, self._stream()),
-              "te_vit_attribute")
+        check(self.lib.te_vit_attribute_alpha(ctypes.byref(self.cfg), ptr(self.weights), ptr(self._derived(fl)), b, ptr(idx),
+                                              int(start_layer), float(alpha), fl, ptr(maps), ptr(ws), ws.numel() * 4,
+                                              self._stream()), "te_vit_attribute_alpha")
         return maps, idx
 
     @_on_engine_device
@@ -379,7 +381,9 @@ class BertEngine:
         return logits
 
     @_on_engine_device
-    def attribute(self, index=None, start_layer=11, flags=None):
+    def attribute(self, index=None, start_layer=11, flags=None, alpha=1.0):
+        """Backward + relprop + normalised rollout on the activations of the last ``forward``; alpha as for
+        ``ViTEngine.attribute``.  Returns (maps [B,S], index [B] int32)."""
         b, s = self.last
         if b <= 0:
             raise RuntimeError("attribute() needs a preceding forward()")
@@ -387,9 +391,9 @@ class BertEngine:
         idx = ViTEngine._index_tensor(self, index, b)
         maps = torch.empty(b, s, dtype=torch.float32, device=self.device)
         fl = self.flags if flags is None else flags
-        check(self.lib.te_bert_attribute(ctypes.byref(self.cfg), ptr(self.weights), ptr(self._derived(fl)), b, s, ptr(idx),
-                                         int(start_layer), fl, ptr(maps), ptr(ws), ws.numel() * 4, self._stream()),
-              "te_bert_attribute")
+        check(self.lib.te_bert_attribute_alpha(ctypes.byref(self.cfg), ptr(self.weights), ptr(self._derived(fl)), b, s,
+                                               ptr(idx), int(start_layer), float(alpha), fl, ptr(maps), ptr(ws),
+                                               ws.numel() * 4, self._stream()), "te_bert_attribute_alpha")
         return maps, idx
 
     @_on_engine_device

@@ -3,7 +3,7 @@
 ``RelPropSimple``, no ratio normalisation, ``:98-100``); every ``relprop`` is one C-ABI call."""
 from transformer_explainability_b200 import ops
 from .layers_ours import *                                            # noqa: F401,F403
-from .layers_ours import RelPropSimple, RelProp, _c, _check_alpha, nn, torch
+from .layers_ours import RelPropSimple, RelProp, _c, nn, torch
 
 __all__ = ['forward_hook', 'Clone', 'Add', 'Cat', 'ReLU', 'GELU', 'Dropout', 'BatchNorm2d', 'Linear', 'MaxPool2d',
            'AdaptiveAvgPool2d', 'AvgPool2d', 'Conv2d', 'Sequential', 'safe_divide', 'einsum', 'Softmax', 'IndexSelect',
@@ -15,7 +15,6 @@ class Add(RelPropSimple):
         return torch.add(*inputs)
 
     def relprop(self, R, alpha):
-        _check_alpha(alpha)
         a, b = self.X
         if b.shape != a.shape:
             raise NotImplementedError("broadcast Add.relprop is not on the ViT_orig_LRP path")
@@ -24,5 +23,4 @@ class Add(RelPropSimple):
 
 class Linear(nn.Linear, RelProp):
     def relprop(self, R, alpha):
-        _check_alpha(alpha)
-        return ops.linear_relprop(_c(self.X), _c(self.weight), _c(R), variant="lrp")
+        return ops.linear_relprop(_c(self.X), _c(self.weight), _c(R), variant="lrp", alpha=alpha)

@@ -2,7 +2,8 @@
 protocol, but every rule runs as an sm_90a CUDA kernel through the C ABI (``ops``) instead of a
 re-forward + ``torch.autograd.grad``.
 
-Only alpha=1 is supported (the only value any caller of the reference passes).  Layers whose
+``Linear.relprop(R, alpha)`` applies the LRP-alpha-beta rule with beta = alpha - 1 (``layers_ours.py:207-230``); every
+other rule does not depend on alpha and ignores it, as in the reference.  Layers whose
 relprop is the identity in the reference (Softmax, LayerNorm, GELU, Dropout, ReLU —
 ``layers_ours.py:45-46,67-80``) stay the identity.  Layers that are not on the
 transformer-attribution path (Conv2d, BatchNorm2d, pools, Cat, AddEye) keep their forward and raise
@@ -32,11 +33,6 @@ def forward_hook(self, input, output):
     else:
         self.X = input[0].detach()
     self.Y = output
-
-
-def _check_alpha(alpha):
-    if alpha != 1:
-        raise NotImplementedError("only alpha=1 (z+ rule) is implemented; the reference never passes another value")
 
 
 def _c(t):
@@ -84,7 +80,6 @@ class Add(RelPropSimple):
         return torch.add(*inputs)
 
     def relprop(self, R, alpha):
-        _check_alpha(alpha)
         a, b = self.X
         if b.shape != a.shape:
             raise NotImplementedError("broadcast Add.relprop is handled inside the BERT engine")
@@ -101,7 +96,6 @@ class einsum(RelPropSimple):
         return torch.einsum(self.equation, *operands)
 
     def relprop(self, R, alpha):
-        _check_alpha(alpha)
         a, b = self.X
         if self.equation == 'bhij,bhjd->bhid':
             return list(ops.matmul_av_relprop(_c(a), _c(b), _c(R)))
@@ -117,7 +111,6 @@ class IndexSelect(RelProp):
         return torch.index_select(inputs, dim, indices)
 
     def relprop(self, R, alpha):
-        _check_alpha(alpha)
         if self.dim != 1 or int(self.indices) != 0:
             raise NotImplementedError("IndexSelect.relprop: only dim=1, index 0 (the CLS pool) is implemented")
         return ops.index_select_relprop(_c(self.X), _c(R))
@@ -129,7 +122,6 @@ class Clone(RelProp):
         return [input for _ in range(num)]
 
     def relprop(self, R, alpha):
-        _check_alpha(alpha)
         return ops.clone_relprop(_c(self.X), [_c(r) for r in R])
 
 
@@ -156,15 +148,13 @@ class BatchNorm2d(nn.BatchNorm2d, RelProp):
 
 class Linear(nn.Linear, RelProp):
     def relprop(self, R, alpha):
-        _check_alpha(alpha)
-        return ops.linear_relprop(_c(self.X), _c(self.weight), _c(R))
+        return ops.linear_relprop(_c(self.X), _c(self.weight), _c(R), alpha=alpha)
 
 
 class Conv2d(nn.Conv2d, RelProp):
     def relprop(self, R, alpha):
         """``layers_ours.py:242-259``, 3-channel (z^B) branch, for the patch-embedding geometry the reference uses it
         with (kernel == stride, no padding, ``ViT_LRP.py:228``): R [B,D,H/P,W/P] -> [B,3,H,W]."""
-        _check_alpha(alpha)
         x = self.X
         k, st = self.kernel_size, self.stride
         if x.shape[1] != 3 or k != st or k[0] != k[1] or tuple(self.padding) != (0, 0) or x.shape[2] != x.shape[3]:

@@ -1,7 +1,7 @@
 """Stand-alone LRP rules and rollout on CUDA tensors (thin wrappers over the C ABI).
 
 Each function is the CUDA counterpart of one ``relprop`` of the reference's
-``modules/layers_ours.py`` (alpha=1); see ``include/te_b200.h`` for the citations.
+``modules/layers_ours.py``; see ``include/te_b200.h`` for the citations.  Only the Linear rule depends on alpha.
 All inputs must be contiguous fp32 CUDA tensors; there is no CPU path.
 """
 import torch
@@ -267,12 +267,14 @@ def tc_attention_nk(amap, np_, amn, x, ldx, batch, heads, n, out, ld_out, e=None
 
 
 @_on_device
-def linear_relprop(x, w, r, tensor_cores=False, y=None, bias=None, bf16=False, variant="ours", r_f16=False):
-    """``Linear.relprop`` (layers_ours.py:207-230): x [...,in], w [out,in], r [...,out] -> [...,in].
+def linear_relprop(x, w, r, tensor_cores=False, y=None, bias=None, bf16=False, variant="ours", r_f16=False, alpha=1.0):
+    """``Linear.relprop(R, alpha)`` (layers_ours.py:207-230): x [...,in], w [out,in], r [...,out] -> [...,in].
     y / bias: the layer's saved forward output (and bias) — lets the tensor-core path form the denominator in one pass.
     variant="lrp": the rule of ``modules/layers_lrp.py:187-210`` (separate denominators; fp32 SIMT); variant="lrp_tc": the
     same rule on single-pass TF32 tensor cores (TE_FLAG_RULES_LRP_TC; in / out multiples of 128, other shapes run the SIMT
-    rule; tensor_cores, y, bias, bf16 and r_f16 do not apply to either)."""
+    rule; tensor_cores, y, bias, bf16 and r_f16 do not apply to either).
+    alpha: the LRP-alpha-beta rule, beta = alpha - 1: alpha * activator - beta * inhibitor relevance (the inhibitor is the
+    same rule with the weight signs swapped); alpha=1 is the z+ rule.  A non-finite alpha raises."""
     _req(x, w, r, y, bias)
     if (w.dim() != 2 or x.shape[-1] != w.shape[1] or r.shape[-1] != w.shape[0] or r.shape[:-1] != x.shape[:-1]
             or (y is not None and y.shape != r.shape) or (bias is not None and bias.numel() != w.shape[0])):
@@ -281,8 +283,10 @@ def linear_relprop(x, w, r, tensor_cores=False, y=None, bias=None, bf16=False, v
     out = torch.empty_like(x)
     if variant == "lrp_tc":
         scratch = _tc_scratch(w, x.device, s=rows * w.shape[0])
-        check(_lib.load().te_linear_relprop(ptr(x), ptr(w), ptr(r), ptr(out), ptr(scratch), rows, x.shape[-1], w.shape[0],
-                                            _lib.FLAG_RULES_LRP | _lib.FLAG_RULES_LRP_TC, _stream()), "te_linear_relprop")
+        check(_lib.load().te_linear_relprop_alpha(ptr(x), ptr(w), None, None, ptr(r), ptr(out), ptr(scratch), rows,
+                                                  x.shape[-1], w.shape[0], float(alpha),
+                                                  _lib.FLAG_RULES_LRP | _lib.FLAG_RULES_LRP_TC, _stream()),
+              "te_linear_relprop_alpha")
         return out
     if tensor_cores:
         scratch = _tc_scratch(w, x.device, s=rows * w.shape[0], operand=x.numel())
@@ -299,12 +303,10 @@ def linear_relprop(x, w, r, tensor_cores=False, y=None, bias=None, bf16=False, v
         flags, y = _lib.FLAG_RULES_LRP, None
     elif variant != "ours":
         raise ValueError("variant: 'ours', 'lrp' or 'lrp_tc'")
-    if y is not None:
-        check(_lib.load().te_linear_relprop_ex(ptr(x), ptr(w), ptr(bias), ptr(y), ptr(r), ptr(out), ptr(scratch), rows,
-                                               x.shape[-1], w.shape[0], flags, _stream()), "te_linear_relprop_ex")
-    else:
-        check(_lib.load().te_linear_relprop(ptr(x), ptr(w), ptr(r), ptr(out), ptr(scratch), rows, x.shape[-1], w.shape[0],
-                                            flags, _stream()), "te_linear_relprop")
+    # y None: the two-pass rule (te_linear_relprop); y given: the single-pass form (te_linear_relprop_ex)
+    check(_lib.load().te_linear_relprop_alpha(ptr(x), ptr(w), ptr(bias) if y is not None else None, ptr(y), ptr(r), ptr(out),
+                                              ptr(scratch), rows, x.shape[-1], w.shape[0], float(alpha), flags, _stream()),
+          "te_linear_relprop_alpha")
     return out
 
 
