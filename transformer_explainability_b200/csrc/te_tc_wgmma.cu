@@ -1,12 +1,15 @@
 // Tensor-core GEMMs of the engines on Hopper (sm_90a): every contraction of te_gemm_tc.h runs on ONE kernel template,
 // wg_kernel<P>, built on wgmma.mma_async with fp32 accumulators in registers.
 //
-//   CTA = 2 warpgroups (256 threads), tile BM = 128 rows (64 per warpgroup) x P::BN columns.
+//   Two consumer warpgroups (threads 0..255), tile BM = 128 rows (64 per warpgroup) x P::BN columns.
 //   Operand tiles are K-major, one 128-byte row per tile row (32 tf32 / 64 fp16 / bf16 elements), in the 128-byte
-//   swizzled layout wgmma reads (16-byte chunk c of row r at r * 128 + ((c ^ (r % 8)) << 4)).  Every thread of the CTA
-//   loads its share of the next k-block from global memory into registers, applies the problem's element transform
-//   (TF32 rounding, |x|, x+ / x-, hi / lo split, transposition of MN-major sources) and stores it into the other of two
-//   shared-memory stages while the wgmmas of the current k-block run.
+//   swizzled layout wgmma reads (16-byte chunk c of row r at r * 128 + ((c ^ (r % 8)) << 4)).  Two mainloops:
+//   P::TMA (operands stored ready to use, or needing only TF32 rounding of A): persistent CTAs with a third, producer
+//   warpgroup whose one thread feeds a ring of up to 8 shared-memory stages by TMA behind full / empty mbarriers
+//   (tma_tiles).  Otherwise every thread of a 256-thread CTA loads its share of the next k-block from global memory into
+//   registers, applies the problem's element transform (TF32 rounding, |x|, x+ / x-, hi / lo split, transposition of
+//   MN-major sources) and stores it into the other of two shared-memory stages while the wgmmas of the current k-block
+//   run (reg_tile).  Both issue the same wgmmas in the same order per tile.
 //   P::CHUNK > 0: the reduction is cut into chunks of CHUNK k-blocks; each chunk accumulates in its own registers and is
 //   added into fp32 sums with round-to-nearest adds (optionally times a per-row power-of-two block scale), so a long
 //   reduction does not ride on the tensor core's accumulator rounding and block-scaled fp16 operands get their scale.
@@ -39,6 +42,34 @@ __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
+
+// mbarriers (CTA scope), TMA tile loads, warpgroup register hand-over
+__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
+}
+__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory"); }
+// returns once the phase of parity `parity` has completed (a fresh barrier counts its phase of parity 1 as completed)
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
+    uint32_t done;
+    do {
+        asm volatile("{\n.reg .pred p;\nmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}\n"
+                     : "=r"(done) : "r"(bar), "r"(parity) : "memory");
+    } while (!done);
+}
+// the box of map at (k, row) into shared memory at dst; completes its bytes on bar
+__device__ __forceinline__ void tma_load(uint32_t dst, const CUtensorMap* map, int k, int row, uint32_t bar) {
+    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
+                 ::"r"(dst), "l"((uint64_t)map), "r"(k), "r"(row), "r"(bar) : "memory");
+}
+__device__ __forceinline__ void bar_named(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 
 __device__ __forceinline__ float to_tf32(float x) {
     uint32_t u;
@@ -175,17 +206,6 @@ __device__ __forceinline__ void for_mn32(int rows, const float* __restrict__ bas
         f(r, c, make_float4(e[0], e[1], e[2], e[3]));
     }
 }
-// 16-bit source, K-major, row stride ld elements, K % 8 == 0: straight copy
-__device__ __forceinline__ void copy_k16(uint8_t* tile, int rows, const uint16_t* __restrict__ base, long long ld, long long row0,
-                                         long long nrows, int k0, int tid) {
-    for (int idx = tid; idx < rows * 8; idx += NTHREADS) {
-        const int r = idx >> 3, c = idx & 7;
-        const long long gr = row0 + r;
-        uint4 v = make_uint4(0u, 0u, 0u, 0u);
-        if (gr < nrows) v = *reinterpret_cast<const uint4*>(base + gr * ld + k0 + 8 * c);
-        *reinterpret_cast<uint4*>(tile + swz(r, c)) = v;
-    }
-}
 __device__ __forceinline__ void st4(uint8_t* tile, int r, int c, float4 v) { *reinterpret_cast<float4*>(tile + swz(r, c)) = v; }
 // hi / lo split of a chunk into two tiles: hi = tf32(v), lo = tf32(v - hi)
 __device__ __forceinline__ void st_split(uint8_t* hi, uint8_t* lo, int r, int c, float4 v) {
@@ -200,27 +220,47 @@ __device__ __forceinline__ int frag_row(int tid, int j) { return 64 * (tid >> 7)
 __device__ __forceinline__ int frag_col(int tid, int j) { return 8 * (j >> 2) + 2 * (tid & 3) + (j & 1); }
 
 // ---- the kernel -----------------------------------------------------------------------------------------------------
+// The TMA problems' tensor maps, one per stage tile (A tiles, then B tiles), and their tile grid.
+struct TmaArgs {
+    CUtensorMap map[4];
+    int mtiles, ntiles;
+};
+constexpr int NTHREADS_TMA = 384, SMEM_MAX = 227 * 1024;
+// stages of a TMA problem: as many as fit next to the 1024-byte alignment slack and the barriers, at most 8
+__host__ __device__ constexpr int tma_stages(int bytes) { return (SMEM_MAX - 1024 - 128) / bytes < 8 ? (SMEM_MAX - 1024 - 128) / bytes : 8; }
+
+// chunk fold: tot += acc times the per-row block scale of chunk ch
+template <class P, int NA, int NR, int NT, int NTR>
+__device__ __forceinline__ void fold(const P& p, float (&acc)[NA][NR], float (&tot)[NT][NTR], int m0, int ch, int z, int tid) {
+    const float s0 = p.chunk_scale(m0 + frag_row(tid, 0), ch, z), s1 = p.chunk_scale(m0 + frag_row(tid, 2), ch, z);
+#pragma unroll
+    for (int a = 0; a < NA; ++a)
+#pragma unroll
+        for (int j = 0; j < NR; ++j) tot[a][j] = fmaf(acc[a][j], ((j >> 1) & 1) ? s1 : s0, tot[a][j]);
+}
+template <int NA, int NR>
+__device__ __forceinline__ void zero(float (&v)[NA][NR]) {
+#pragma unroll
+    for (int a = 0; a < NA; ++a)
+#pragma unroll
+        for (int j = 0; j < NR; ++j) v[a][j] = 0.f;
+}
+
+// Register mainloop: all 256 threads load the next k-block (with the problem's element transform) into the other of two
+// stages while the current k-block's wgmmas run; one tile per CTA.
 template <class P>
-__global__ void __launch_bounds__(NTHREADS, 1) wg_kernel(const P p, int col_fast) {
+__device__ __forceinline__ void reg_tile(const P& p, uint8_t* smem, int col_fast) {
     constexpr int NR = P::BN / 2;
     constexpr int NA = P::PRODS::NACC;
     constexpr int STAGE = P::L::BYTES;
     constexpr int NT = P::CHUNK ? NA : 1, NTR = P::CHUNK ? NR : 1;
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     const int tid = threadIdx.x, wg = tid >> 7;
     const int m0 = (col_fast ? blockIdx.y : blockIdx.x) * BM, n0 = (col_fast ? blockIdx.x : blockIdx.y) * P::BN;
     const int z = blockIdx.z;
     float acc[NA][NR];
     float tot[NT][NTR];
-#pragma unroll
-    for (int a = 0; a < NA; ++a)
-#pragma unroll
-        for (int j = 0; j < NR; ++j) acc[a][j] = 0.f;
-#pragma unroll
-    for (int a = 0; a < NT; ++a)
-#pragma unroll
-        for (int j = 0; j < NTR; ++j) tot[a][j] = 0.f;
+    zero(acc);
+    zero(tot);
 
     const int kb = p.kblocks();
     p.load(smem, 0, m0, n0, z, tid);
@@ -233,16 +273,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) wg_kernel(const P p, int col_fast
         wg_commit();
         if (it + 1 < kb) p.load(smem + ((it + 1) & 1) * STAGE, it + 1, m0, n0, z, tid);
         wg_wait0();
-        if constexpr (P::CHUNK > 0) {
-            if ((it + 1) % P::CHUNK == 0 || it + 1 == kb) {
-                const int ch = it / P::CHUNK;
-                const float s0 = p.chunk_scale(m0 + frag_row(tid, 0), ch, z), s1 = p.chunk_scale(m0 + frag_row(tid, 2), ch, z);
-#pragma unroll
-                for (int a = 0; a < NA; ++a)
-#pragma unroll
-                    for (int j = 0; j < NR; ++j) tot[a][j] = fmaf(acc[a][j], ((j >> 1) & 1) ? s1 : s0, tot[a][j]);
-            }
-        }
+        if constexpr (P::CHUNK > 0)
+            if ((it + 1) % P::CHUNK == 0 || it + 1 == kb) fold(p, acc, tot, m0, it / P::CHUNK, z, tid);
         fence_proxy_async();
         __syncthreads();
     }
@@ -250,9 +282,120 @@ __global__ void __launch_bounds__(NTHREADS, 1) wg_kernel(const P p, int col_fast
     else p.epilogue(acc, m0, n0, z, tid);
 }
 
+// TMA mainloop on persistent CTAs.  Warpgroups 0 and 1 (threads 0..255, the same rows and fragments as the register
+// mainloop) consume; warpgroup 2 produces: one thread issues the TMA boxes of every stage tile into a ring of S stages,
+// each with a full barrier (the producer's expect_tx, completed by the TMA bytes) and an empty barrier (one arrive per
+// consumer warp once the stage's wgmmas have retired).  Tile t = blockIdx.x, blockIdx.x + gridDim.x, ... is decoded
+// column-fastest, and the producer runs into the next tile's k-blocks while the consumers run the epilogue.
+// Consumers keep one k-block's wgmmas in flight (wait_group 1) and wait for all only before a chunk fold and the epilogue;
+// wgmmas into one accumulator execute in issue order, so every tile's sums are those of the register mainloop.
+// P::AFIX: A tile 0 lands raw fp32 and each consumer warpgroup applies P::fix_a to its own 64 rows in place.
+template <class P>
+__device__ __forceinline__ void tma_tiles(const P& p, const TmaArgs& ta, uint8_t* smem) {
+    using L = typename P::L;
+    constexpr int NR = P::BN / 2;
+    constexpr int NA = P::PRODS::NACC;
+    constexpr int STAGE = L::BYTES, S = tma_stages(STAGE);
+    constexpr int NT = P::CHUNK ? NA : 1, NTR = P::CHUNK ? NR : 1;
+    constexpr int KE = P::FMT == OP_TF32 ? 32 : 64;          // elements in a 128-byte row
+    static_assert(S >= 2, "a TMA problem needs two stages");
+    __shared__ __align__(8) uint64_t bars[2 * S];            // full[S], then empty[S]
+    const int tid = threadIdx.x, wg = tid >> 7;
+    const uint32_t full0 = smem_u32(bars), empty0 = full0 + 8u * S, st0 = smem_u32(smem);
+    if (tid == 0) {
+        for (int s = 0; s < S; ++s) {
+            mbar_init(full0 + 8u * s, 1);
+            mbar_init(empty0 + 8u * s, 8);
+        }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    const int kb = p.kblocks(), ntiles = ta.mtiles * ta.ntiles;
+    int stage = 0;
+    uint32_t phase = 0;
+
+    if (wg == 2) {
+        setmaxnreg_dec<40>();
+        if (tid != 2 * 128) return;
+        for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
+            const int m0 = (t / ta.ntiles) * BM, n0 = (t % ta.ntiles) * P::BN;
+            for (int it = 0; it < kb; ++it) {
+                mbar_wait(empty0 + 8u * stage, phase ^ 1u);
+                const uint32_t full = full0 + 8u * stage, st = st0 + (uint32_t)stage * STAGE;
+                mbar_expect_tx(full, STAGE);
+#pragma unroll
+                for (int i = 0; i < L::NTA; ++i) tma_load(st + L::a(i), &ta.map[i], it * KE, m0, full);
+#pragma unroll
+                for (int j = 0; j < L::NTB; ++j) tma_load(st + L::b(j), &ta.map[L::NTA + j], it * KE, n0, full);
+                if (++stage == S) { stage = 0; phase ^= 1u; }
+            }
+        }
+        return;
+    }
+
+    setmaxnreg_inc<232>();
+    float acc[NA][NR];
+    float tot[NT][NTR];
+    auto release = [&](int s) {
+        if ((tid & 31) == 0) mbar_arrive(empty0 + 8u * s);
+    };
+    for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
+        const int m0 = (t / ta.ntiles) * BM, n0 = (t % ta.ntiles) * P::BN;
+        zero(acc);
+        zero(tot);
+        int pend = -1;                                        // the stage whose wgmmas are still in flight
+        for (int it = 0; it < kb; ++it) {
+            mbar_wait(full0 + 8u * stage, phase);
+            const uint32_t st = st0 + (uint32_t)stage * STAGE;
+            if constexpr (P::AFIX) {
+                float4* a = reinterpret_cast<float4*>(smem + (uint32_t)stage * STAGE + L::a(0) + (uint32_t)wg * 64u * 128u);
+#pragma unroll
+                for (int i = tid & 127; i < 64 * 8; i += 128) a[i] = P::fix_a(a[i]);
+                fence_proxy_async();
+                bar_named(1 + wg, 128);
+            }
+            const bool fresh = P::CHUNK ? (it % P::CHUNK == 0) : (it == 0);
+            wg_fence();
+            issue<P>(st, wg, acc, fresh ? 0u : 1u);
+            wg_commit();
+            const bool last = it + 1 == kb;
+            if (last || (P::CHUNK ? (it + 1) % P::CHUNK == 0 : false)) {
+                wg_wait0();
+                if (pend >= 0) release(pend);
+                release(stage);
+                pend = -1;
+                if constexpr (P::CHUNK > 0) fold(p, acc, tot, m0, it / P::CHUNK, 0, tid);
+            } else {
+                wg_wait1();
+                if (pend >= 0) release(pend);
+                pend = stage;
+            }
+            if (++stage == S) { stage = 0; phase ^= 1u; }
+        }
+        if constexpr (P::CHUNK > 0) p.epilogue(tot, m0, n0, 0, tid);
+        else p.epilogue(acc, m0, n0, 0, tid);
+    }
+}
+
+template <class P>
+__global__ void __launch_bounds__(P::TMA ? NTHREADS_TMA : NTHREADS, 1)
+    wg_kernel(const P p, const __grid_constant__ TmaArgs ta, int col_fast) {
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+    if constexpr (P::TMA) tma_tiles(p, ta, smem);
+    else reg_tile(p, smem, col_fast);
+}
+
 // unit block scale for the plain chunked problems
 struct NoScale {
     __device__ __forceinline__ float chunk_scale(int, int, int) const { return 1.f; }
+};
+
+// Problems with P::TMA run the TMA mainloop; tile(i) names the K-major global source of stage tile i (A tiles, then B
+// tiles): rows x cols elements at row stride ld.  The others load through registers (P::load).
+struct TmaTile {
+    const void* base;
+    long long rows, cols, ld;
 };
 
 // ---- z+ rule, first contraction: S = sd(R, Z) ---------------------------------------------------------------------
@@ -269,6 +412,8 @@ struct ZsProb : NoScale {
     using PRODS = std::conditional_t<SINGLE, One, Prods<Pr<0, 0, 0>, Pr<0, 1, 1>>>;    // two-pass: x+ W+^T, then x- W-^T
     using L = Stage<PRODS, BN>;
     static constexpr bool COL_FAST = true;
+    // single-pass: TMA (A = bf16(|x|), or raw x made tf32(|x|) in shared memory); two-pass: x+ / x- formed on load
+    static constexpr bool TMA = SINGLE, AFIX = SINGLE && !BF;
     int M, N, K;
     const float* x; long long ldx;
     const void* xabs;                       // BF: bf16(|x|) [M, K]
@@ -278,23 +423,18 @@ struct ZsProb : NoScale {
     float sscale, zsign;                    // S = sscale * sd(R, Z) ; SINGLE: sign of the |x| |W|^T term
 
     __device__ int kblocks() const { return K / (BF ? 64 : 32); }
+    __device__ static float4 fix_a(float4 v) { return tf32x4(absx4(v)); }
+    TmaTile tile(int i) const {
+        if (i == 0) return BF ? TmaTile{xabs, M, K, K} : TmaTile{x, M, K, ldx};
+        return TmaTile{wa, N, K, K};
+    }
     __device__ void load(uint8_t* st, int kb, int m0, int n0, int, int tid) const {
-        if (BF) {
-            copy_k16(st + L::a(0), BM, (const uint16_t*)xabs, K, m0, M, kb * 64, tid);
-            copy_k16(st + L::b(0), BN, (const uint16_t*)wa, K, n0, N, kb * 64, tid);
-            return;
-        }
-        if (SINGLE) {
-            for_k32(BM, x, ldx, m0, M, kb * 32, K, tid, [&](int rr, int c, float4 v) { st4(st + L::a(0), rr, c, tf32x4(absx4(v))); });
-            for_k32(BN, (const float*)wa, K, n0, N, kb * 32, K, tid, [&](int rr, int c, float4 v) { st4(st + L::b(0), rr, c, v); });
-        } else {
-            for_k32(BM, x, ldx, m0, M, kb * 32, K, tid, [&](int rr, int c, float4 v) {
-                st4(st + L::a(0), rr, c, tf32x4(posx4(v)));
-                st4(st + L::a(1), rr, c, tf32x4(negx4(v)));
-            });
-            for_k32(BN, (const float*)wa, K, n0, N, kb * 32, K, tid, [&](int rr, int c, float4 v) { st4(st + L::b(0), rr, c, v); });
-            for_k32(BN, (const float*)wb, K, n0, N, kb * 32, K, tid, [&](int rr, int c, float4 v) { st4(st + L::b(1), rr, c, v); });
-        }
+        for_k32(BM, x, ldx, m0, M, kb * 32, K, tid, [&](int rr, int c, float4 v) {
+            st4(st + L::a(0), rr, c, tf32x4(posx4(v)));
+            st4(st + L::a(1), rr, c, tf32x4(negx4(v)));
+        });
+        for_k32(BN, (const float*)wa, K, n0, N, kb * 32, K, tid, [&](int rr, int c, float4 v) { st4(st + L::b(0), rr, c, v); });
+        for_k32(BN, (const float*)wb, K, n0, N, kb * 32, K, tid, [&](int rr, int c, float4 v) { st4(st + L::b(1), rr, c, v); });
     }
     __device__ void epilogue(float (&acc)[1][BN / 2], int m0, int n0, int, int tid) const {
         float sv[BN / 2];
@@ -358,7 +498,7 @@ struct ZrProb {
     static constexpr int FMT = KIND == 0 ? OP_TF32 : KIND == 1 ? OP_BF16 : OP_F16;
     using PRODS = Prods<Pr<0, 0, 0>, Pr<1, 0, 1>>;           // S W+ and S W- into their own accumulators
     using L = Stage<PRODS, BN>;
-    static constexpr bool COL_FAST = true;
+    static constexpr bool TMA = true, AFIX = false;
     int M, N, K;
     const void* s; const void* wp; const void* wn;     // S [M, K] (row stride K), W+^T / W-^T [N, K]
     const float* rs; int rs_ld; const float* cp; const float* cn;   // KIND 2: scales of S, of the rows of W+^T / W-^T
@@ -367,17 +507,7 @@ struct ZrProb {
 
     __device__ int kblocks() const { return K / (KIND ? 64 : 32); }
     __device__ float chunk_scale(int row, int ch, int) const { return (KIND == 2 && row < M) ? rs[(long long)row * rs_ld + ch] : 1.f; }
-    __device__ void load(uint8_t* st, int kb, int m0, int n0, int, int tid) const {
-        if (KIND) {
-            copy_k16(st + L::a(0), BM, (const uint16_t*)s, K, m0, M, kb * 64, tid);
-            copy_k16(st + L::b(0), BN, (const uint16_t*)wp, K, n0, N, kb * 64, tid);
-            copy_k16(st + L::b(1), BN, (const uint16_t*)wn, K, n0, N, kb * 64, tid);
-        } else {
-            for_k32(BM, (const float*)s, K, m0, M, kb * 32, K, tid, [&](int r, int c, float4 v) { st4(st + L::a(0), r, c, v); });
-            for_k32(BN, (const float*)wp, K, n0, N, kb * 32, K, tid, [&](int r, int c, float4 v) { st4(st + L::b(0), r, c, v); });
-            for_k32(BN, (const float*)wn, K, n0, N, kb * 32, K, tid, [&](int r, int c, float4 v) { st4(st + L::b(1), r, c, v); });
-        }
-    }
+    TmaTile tile(int i) const { return i == 0 ? TmaTile{s, M, K, K} : TmaTile{i == 1 ? wp : wn, N, K, K}; }
     __device__ void epilogue(float (&acc)[2][BN / 2], int m0, int n0, int, int tid) const {
 #pragma unroll
         for (int j = 0; j < BN / 2; j += 2) {
@@ -411,7 +541,7 @@ struct LrpSProb : NoScale {
     static constexpr int BN = 128, CHUNK = 0, FMT = OP_TF32;
     using PRODS = One;
     using L = Stage<PRODS, BN>;
-    static constexpr bool COL_FAST = true;
+    static constexpr bool COL_FAST = true, TMA = false, AFIX = false;
     int M, N, K;
     const float* x; long long ldx; const float* w;      // w: W+ or W- (tf32) [N, K]
     const float* r; long long ldr; float* out;           // out: S [M, N], row stride N
@@ -439,16 +569,13 @@ struct LrpRProb : NoScale {
     static constexpr int BN = 128, CHUNK = 0, FMT = OP_TF32;
     using PRODS = One;
     using L = Stage<PRODS, BN>;
-    static constexpr bool COL_FAST = true;
+    static constexpr bool TMA = true, AFIX = false;
     int M, N, K;
     const float* s; const float* wt;
     const float* x; long long ldx; float* out; long long ldo;
     int accum;
     __device__ int kblocks() const { return K / 32; }
-    __device__ void load(uint8_t* st, int kb, int m0, int n0, int, int tid) const {
-        for_k32(BM, s, K, m0, M, kb * 32, K, tid, [&](int rr, int c, float4 v) { st4(st + L::a(0), rr, c, v); });
-        for_k32(BN, wt, K, n0, N, kb * 32, K, tid, [&](int rr, int c, float4 v) { st4(st + L::b(0), rr, c, v); });
-    }
+    TmaTile tile(int i) const { return i == 0 ? TmaTile{s, M, K, K} : TmaTile{wt, N, K, K}; }
     __device__ void epilogue(float (&acc)[1][BN / 2], int m0, int n0, int, int tid) const {
 #pragma unroll
         for (int j = 0; j < BN / 2; j += 2) {
@@ -518,27 +645,22 @@ struct LinProb : LinArgs {
     using PRODS = std::conditional_t<SPLIT, Split3, One>;
     using L = Stage<PRODS, BN>;
     static constexpr bool COL_FAST = true;
+    // the fp16 forms and the single-pass TF32 form (A rounded in shared memory) on TMA; 3xTF32 splits A on load
+    static constexpr bool TMA = FORM != LIN_3XTF32, AFIX = FORM == LIN_TF32;
     __device__ int kblocks() const { return K / (F16 ? 64 : 32); }
     __device__ float chunk_scale(int row, int ch, int) const {
         if constexpr (F16) return row < o.M ? rs[(long long)row * rs_ld + ch] : 1.f;
         else return 1.f;
     }
+    __device__ static float4 fix_a(float4 v) { return tf32x4(v); }
+    TmaTile tile(int i) const {
+        if (i < L::NTA) return TmaTile{i == 0 ? a : a_lo, o.M, K, F16 ? K : lda};
+        return TmaTile{i == L::NTA ? b : b_lo, o.N, K, K};
+    }
     __device__ void load(uint8_t* st, int kb, int m0, int n0, int, int tid) const {
-        if constexpr (F16) {
-            copy_k16(st + L::a(0), BM, (const uint16_t*)a, K, m0, o.M, kb * 64, tid);
-            copy_k16(st + L::b(0), BN, (const uint16_t*)b, K, n0, o.N, kb * 64, tid);
-            if constexpr (SPLIT) {
-                copy_k16(st + L::a(1), BM, (const uint16_t*)a_lo, K, m0, o.M, kb * 64, tid);
-                copy_k16(st + L::b(1), BN, (const uint16_t*)b_lo, K, n0, o.N, kb * 64, tid);
-            }
-        } else if constexpr (SPLIT) {
-            for_k32(BM, (const float*)a, lda, m0, o.M, kb * 32, K, tid, [&](int r, int c, float4 v) { st_split(st + L::a(0), st + L::a(1), r, c, v); });
-            for_k32(BN, (const float*)b, K, n0, o.N, kb * 32, K, tid, [&](int r, int c, float4 v) { st4(st + L::b(0), r, c, v); });
-            for_k32(BN, (const float*)b_lo, K, n0, o.N, kb * 32, K, tid, [&](int r, int c, float4 v) { st4(st + L::b(1), r, c, v); });
-        } else {
-            for_k32(BM, (const float*)a, lda, m0, o.M, kb * 32, K, tid, [&](int r, int c, float4 v) { st4(st + L::a(0), r, c, tf32x4(v)); });
-            for_k32(BN, (const float*)b, K, n0, o.N, kb * 32, K, tid, [&](int r, int c, float4 v) { st4(st + L::b(0), r, c, v); });
-        }
+        for_k32(BM, (const float*)a, lda, m0, o.M, kb * 32, K, tid, [&](int r, int c, float4 v) { st_split(st + L::a(0), st + L::a(1), r, c, v); });
+        for_k32(BN, (const float*)b, K, n0, o.N, kb * 32, K, tid, [&](int r, int c, float4 v) { st4(st + L::b(0), r, c, v); });
+        for_k32(BN, (const float*)b_lo, K, n0, o.N, kb * 32, K, tid, [&](int r, int c, float4 v) { st4(st + L::b(1), r, c, v); });
     }
     __device__ void epilogue(float (&acc)[1][BN / 2], int m0, int n0, int, int tid) const {
 #pragma unroll
@@ -558,7 +680,7 @@ struct NnProb : NoScale {
     static constexpr int BN = BN_, CHUNK = 0, FMT = OP_TF32;
     using PRODS = std::conditional_t<SP, One, Split3>;
     using L = Stage<PRODS, BN>;
-    static constexpr bool COL_FAST = false;
+    static constexpr bool COL_FAST = false, TMA = false, AFIX = false;
     int N, H, dh, ld_out, batch;
     const float* a; long long lda; const float* b; long long ldb;
     const float* E; float* out; float alpha;
@@ -642,7 +764,7 @@ struct NkProb : NoScale {
     static constexpr int BN = BN_, CHUNK = SP ? 0 : 4, FMT = OP_TF32;
     using PRODS = std::conditional_t<SP, One, Split3>;
     using L = Stage<PRODS, BN>;
-    static constexpr bool COL_FAST = false;
+    static constexpr bool COL_FAST = false, TMA = false, AFIX = false;
     int N, H, NP, ld_out, n_out, n_pad, a_shared;
     const float* map; const float* X; long long ldx;
     const float* rowscale; const float* E; float* out; float alpha;
@@ -693,29 +815,86 @@ struct NkProb : NoScale {
 // ---- launch ---------------------------------------------------------------------------------------------------------
 inline bool a16(const void* p) { return ((uintptr_t)p & 15u) == 0; }
 
-// grid: (m-tiles, column tiles, z).  P::COL_FAST problems (the Linear-rule GEMMs) are launched with the column tile in
-// blockIdx.x, so that consecutively scheduled CTAs share an A panel and the panel is read from HBM about once instead of
-// once per column tile; the weights, at most a few tens of MB, stay in L2.  More than 65535 m-tiles do not fit in grid.y:
-// those launches keep the m-tile in blockIdx.x, which is why the order is a kernel argument.  The tiles and their
-// arithmetic do not change.
+int sm_count() {
+    static int sms[64];
+    int dev = 0;
+    cudaGetDevice(&dev);
+    int& n = sms[dev & 63];
+    if (n == 0 && cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) n = 1;
+    return n;
+}
+
+// cuTensorMapEncodeTiled through the runtime's driver entry point (the library links only the runtime)
+using EncodeTiled = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                 const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                 CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+EncodeTiled encode_tiled() {
+    static const EncodeTiled fn = [] {
+        void* f = nullptr;
+        cudaDriverEntryPointQueryResult q;
+        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &q) != cudaSuccess ||
+            q != cudaDriverEntryPointSuccess)
+            return (EncodeTiled) nullptr;
+        return (EncodeTiled)f;
+    }();
+    return fn;
+}
+// The map of one stage tile: boxes of 128 bytes (one swizzled row) x box_rows rows, 128-byte swizzle (the layout swz() and
+// sdesc() describe), rows and columns past the source filled with zeros.  TMA needs a 16-byte-aligned base and a row
+// stride that is a multiple of 16 bytes.
+bool encode_tile(CUtensorMap* map, const TmaTile& t, int esize, int box_rows) {
+    const EncodeTiled fn = encode_tiled();
+    if (!fn || ((uintptr_t)t.base & 15u) || (t.ld * esize) % 16 != 0 || t.rows < 1 || t.cols < 1) return false;
+    const cuuint64_t dims[2] = {(cuuint64_t)t.cols, (cuuint64_t)t.rows}, strides[1] = {(cuuint64_t)(t.ld * esize)};
+    const cuuint32_t box[2] = {(cuuint32_t)(128 / esize), (cuuint32_t)box_rows}, estr[2] = {1, 1};
+    return fn(map, esize == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_UINT16, 2, const_cast<void*>(t.base), dims,
+              strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
+// grid: (m-tiles, column tiles, z).
+// P::TMA problems run min(tiles, SMs) persistent CTAs of 384 threads that walk the tiles column-fastest (tma_tiles).
+// The others run one CTA of 256 threads per tile.  P::COL_FAST problems are launched with the column tile in blockIdx.x,
+// so that consecutively scheduled CTAs share an A panel and the panel is read from HBM about once instead of once per
+// column tile; the weights, at most a few tens of MB, stay in L2.  More than 65535 m-tiles do not fit in grid.y: those
+// launches keep the m-tile in blockIdx.x, which is why the order is a kernel argument.  The tiles and their arithmetic do
+// not change.
 template <class P>
 int launch(const P& p, dim3 grid, cudaStream_t st) {
-    const int col_fast = P::COL_FAST && grid.x <= 65535;
-    if (col_fast) grid = dim3(grid.y, grid.x, grid.z);
-    constexpr int SMEM = 2 * P::L::BYTES + 1024;
+    TmaArgs ta;
+    memset(&ta, 0, sizeof(ta));
+    int col_fast = 0, threads = NTHREADS, smem = 2 * P::L::BYTES + 1024;
+    if constexpr (P::TMA) {
+        constexpr int ESIZE = P::FMT == OP_TF32 ? 4 : 2;
+        for (int i = 0; i < P::L::NTA + P::L::NTB; ++i)
+            if (!encode_tile(&ta.map[i], p.tile(i), ESIZE, i < P::L::NTA ? BM : P::BN)) {
+                te_set_last_error("te_tc: cannot encode a TMA tensor map (16-byte-aligned base and row stride required)");
+                return TE_ERR_ARG;
+            }
+        const long long tiles = (long long)grid.x * grid.y;
+        if (grid.z != 1 || tiles > INT32_MAX) { te_set_last_error("te_tc: grid too large for one launch"); return TE_ERR_ARG; }
+        ta.mtiles = (int)grid.x;
+        ta.ntiles = (int)grid.y;
+        grid = dim3((unsigned)std::min<long long>(tiles, sm_count()));
+        threads = NTHREADS_TMA;
+        smem = tma_stages(P::L::BYTES) * P::L::BYTES + 1024;
+    } else {
+        col_fast = P::COL_FAST && grid.x <= 65535;
+        if (col_fast) grid = dim3(grid.y, grid.x, grid.z);
+    }
     // cudaFuncAttributeMaxDynamicSharedMemorySize is per device: one bit per device ordinal
     static unsigned long long done = 0;
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess) { te_set_last_error("te_tc: cudaGetDevice failed"); return TE_ERR_CUDA; }
     if (!(done & (1ull << (dev & 63)))) {
-        if (cudaFuncSetAttribute(wg_kernel<P>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM) != cudaSuccess) {
+        if (cudaFuncSetAttribute(wg_kernel<P>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) {
             te_set_last_error("te_tc: cannot raise dynamic shared memory");
             return TE_ERR_CUDA;
         }
         done |= 1ull << (dev & 63);
     }
     if (grid.y > 65535 || grid.z > 65535) { te_set_last_error("te_tc: grid too large for one launch"); return TE_ERR_ARG; }
-    wg_kernel<P><<<grid, NTHREADS, SMEM, st>>>(p, col_fast);
+    wg_kernel<P><<<grid, threads, smem, st>>>(p, ta, col_fast);
     TE_CUDA_CHECK_LAUNCH();
     return TE_OK;
 }
@@ -827,13 +1006,8 @@ __global__ void abs_bf16_kernel(const float* __restrict__ x, long long ldx, __nv
 }
 // grid of a grid-stride elementwise pass: at most 16 blocks per SM
 unsigned stride_blocks(long long work, int per_block) {
-    static int sms[64];
-    int dev = 0;
-    cudaGetDevice(&dev);
-    int& n = sms[dev & 63];
-    if (n == 0 && cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) n = 1;
     long long b = (work + per_block - 1) / per_block;
-    const long long cap = (long long)n * 16;
+    const long long cap = (long long)sm_count() * 16;
     if (b > cap) b = cap;
     return (unsigned)(b < 1 ? 1 : b);
 }
