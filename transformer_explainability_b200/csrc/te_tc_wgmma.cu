@@ -4,12 +4,12 @@
 //   Two consumer warpgroups (threads 0..255), tile BM = 128 rows (64 per warpgroup) x P::BN columns.
 //   Operand tiles are K-major, one 128-byte row per tile row (32 tf32 / 64 fp16 / bf16 elements), in the 128-byte
 //   swizzled layout wgmma reads (16-byte chunk c of row r at r * 128 + ((c ^ (r % 8)) << 4)).  Two mainloops:
-//   P::TMA (operands stored ready to use, or needing only TF32 rounding of A): persistent CTAs with a third, producer
-//   warpgroup whose one thread feeds a ring of up to 8 shared-memory stages by TMA behind full / empty mbarriers
-//   (tma_tiles).  Otherwise every thread of a 256-thread CTA loads its share of the next k-block from global memory into
-//   registers, applies the problem's element transform (TF32 rounding, |x|, x+ / x-, hi / lo split, transposition of
-//   MN-major sources) and stores it into the other of two shared-memory stages while the wgmmas of the current k-block
-//   run (reg_tile).  Both issue the same wgmmas in the same order per tile.
+//   P::TMA: persistent CTAs with a third, producer warpgroup whose one thread feeds a ring of up to 8 shared-memory stages
+//   by TMA behind full / empty mbarriers, and the consumers apply the problem's operand transform (TF32 rounding, |x|,
+//   hi / lo split, transposition of MN-major sources) in shared memory (tma_tiles).  Otherwise every thread of a
+//   256-thread CTA loads its share of the next k-block from global memory into registers, applies the transform (x+ / x-,
+//   hi / lo split) and stores it into the other of two shared-memory stages while the wgmmas of the current k-block run
+//   (reg_tile).  Both issue the same wgmmas in the same order per tile.
 //   P::CHUNK > 0: the reduction is cut into chunks of CHUNK k-blocks; each chunk accumulates in its own registers and is
 //   added into fp32 sums with round-to-nearest adds (optionally times a per-row power-of-two block scale), so a long
 //   reduction does not ride on the tensor core's accumulator rounding and block-scaled fp16 operands get their scale.
@@ -64,6 +64,11 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
 __device__ __forceinline__ void tma_load(uint32_t dst, const CUtensorMap* map, int k, int row, uint32_t bar) {
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
                  ::"r"(dst), "l"((uint64_t)map), "r"(k), "r"(row), "r"(bar) : "memory");
+}
+// the same for a 3-D map at (x, y, z)
+__device__ __forceinline__ void tma_load3(uint32_t dst, const CUtensorMap* map, int x, int y, int z, uint32_t bar) {
+    asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];"
+                 ::"r"(dst), "l"((uint64_t)map), "r"(x), "r"(y), "r"(z), "r"(bar) : "memory");
 }
 __device__ __forceinline__ void bar_named(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
 template <int N>
@@ -128,13 +133,15 @@ using One = Prods<Pr<0, 0, 0>>;
 // A = [hi | lo], B = [hi | lo]: hi*hi + lo*hi + hi*lo, the small terms first (3xTF32 and the three-term fp16 split)
 using Split3 = Prods<Pr<0, 1, 0>, Pr<0, 0, 1>, Pr<0, 0, 0>>;
 
-// A stage: the problem's A tiles (BM rows each), then its B tiles (BN rows each); a(i) / b(j) are byte offsets in it.
-template <class PRODS, int BN>
+// A stage: the problem's A tiles (BM rows each), then its B tiles (BN rows each), then LAND bytes where TMA lands MN-major
+// sources before the consumers transpose them into the tiles; a(i) / b(j) / land() are byte offsets in it.
+template <class PRODS, int BN, int LAND = 0>
 struct Stage {
     static constexpr int NTA = PRODS::NTA, NTB = PRODS::NTB;
-    static constexpr int BYTES = NTA * TILE128 + NTB * BN * 128;
+    static constexpr int BYTES = NTA * TILE128 + NTB * BN * 128 + LAND;
     __host__ __device__ static constexpr uint32_t a(int i) { return (uint32_t)i * TILE128; }
     __host__ __device__ static constexpr uint32_t b(int j) { return (uint32_t)(NTA * TILE128 + j * BN * 128); }
+    __host__ __device__ static constexpr uint32_t land() { return (uint32_t)(NTA * TILE128 + NTB * BN * 128); }
 };
 
 enum { OP_TF32 = 0, OP_BF16 = 1, OP_F16 = 2 };
@@ -188,24 +195,6 @@ __device__ __forceinline__ void for_k32(int rows, const float* __restrict__ base
         f(r, c, v);
     }
 }
-// fp32 source, MN-major: tile row r = source column col0 + r (valid below ncols), chunk c = source rows k0 + 4c .. +3 (valid
-// below K).  Consecutive threads take consecutive columns (coalesced).
-template <class F>
-__device__ __forceinline__ void for_mn32(int rows, const float* __restrict__ base, long long ld, int col0, int ncols, int k0,
-                                         int K, int tid, F f) {
-    for (int idx = tid; idx < rows * 8; idx += NTHREADS) {
-        const int r = idx % rows, c = idx / rows;
-        const int col = col0 + r;
-        const int k = k0 + 4 * c;
-        float e[4] = {0.f, 0.f, 0.f, 0.f};
-        if (col < ncols) {
-#pragma unroll
-            for (int u = 0; u < 4; ++u)
-                if (k + u < K) e[u] = base[(long long)(k + u) * ld + col];
-        }
-        f(r, c, make_float4(e[0], e[1], e[2], e[3]));
-    }
-}
 __device__ __forceinline__ void st4(uint8_t* tile, int r, int c, float4 v) { *reinterpret_cast<float4*>(tile + swz(r, c)) = v; }
 // hi / lo split of a chunk into two tiles: hi = tf32(v), lo = tf32(v - hi)
 __device__ __forceinline__ void st_split(uint8_t* hi, uint8_t* lo, int r, int c, float4 v) {
@@ -214,17 +203,72 @@ __device__ __forceinline__ void st_split(uint8_t* hi, uint8_t* lo, int r, int c,
     st4(lo, r, c, tf32x4(subx4(v, h)));
 }
 
+// ---- operand transforms in shared memory (TMA mainloop), rows r0 .. r0 + n - 1 of a tile by thread t of nt ------------
+// The swizzle permutes the chunks within a row, so an element-wise transform walks the rows' 16-byte chunks in order.
+// In place: v = f(v).
+template <class F>
+__device__ __forceinline__ void map_rows(uint8_t* tile, int r0, int n, int t, int nt, F f) {
+    float4* a = reinterpret_cast<float4*>(tile + r0 * 128);
+    for (int i = t; i < n * 8; i += nt) a[i] = f(a[i]);
+}
+// hi / lo split in place: the raw value landed in hi; the same arithmetic as st_split
+__device__ __forceinline__ void split_rows(uint8_t* hi, uint8_t* lo, int r0, int n, int t, int nt) {
+    float4* h = reinterpret_cast<float4*>(hi + r0 * 128);
+    float4* l = reinterpret_cast<float4*>(lo + r0 * 128);
+    for (int i = t; i < n * 8; i += nt) {
+        const float4 v = h[i], vh = tf32x4(v);
+        h[i] = vh;
+        l[i] = tf32x4(subx4(v, vh));
+    }
+}
+// Transposition of an MN-major source.  It lands as boxes of 32 source rows (k) x 32 fp32 (tile rows), 128-byte swizzled
+// like a tile (element (k, m) of a box at k * 128 + ((m / 4) ^ (k % 8)) * 16 + (m % 4) * 4), box j holding tile rows
+// 32 j .. 32 j + 31.  Chunk c of tile row r is (k = 4c .. 4c + 3, m = r): f(r, c, v) stores it.  Consecutive threads take
+// consecutive rows, so a warp's four loads of one k each hit 32 different banks and each quarter-warp's float4 stores
+// (rows r .. r + 7, one chunk) hit 8 different 16-byte bank groups.
+template <class F>
+__device__ __forceinline__ void transpose_rows(const uint8_t* land, int r0, int n, int t, int nt, F f) {
+    for (int i = t; i < n * 8; i += nt) {
+        const int r = r0 + i % n, c = i / n, m = r & 31;
+        const uint8_t* box = land + (r >> 5) * 4096 + (m & 3) * 4;
+        float e[4];
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+            const int k = 4 * c + u;
+            e[u] = *reinterpret_cast<const float*>(box + k * 128 + (((m >> 2) ^ (k & 7)) << 4));
+        }
+        f(r, c, make_float4(e[0], e[1], e[2], e[3]));
+    }
+}
+// The stores of a transposed chunk into a single-pass (TF32-rounded) or split (hi / lo) tile pair
+template <bool SP>
+__device__ __forceinline__ auto put_tf32(uint8_t* hi, uint8_t* lo) {
+    return [=](int r, int c, float4 v) {
+        if (SP) st4(hi, r, c, tf32x4(v));
+        else st_split(hi, lo, r, c, v);
+    };
+}
+// An operand that landed K-major: TF32-rounded (SP) or split into hi / lo in place
+template <bool SP>
+__device__ __forceinline__ void fix_tf32(uint8_t* hi, uint8_t* lo, int r0, int n, int t, int nt) {
+    if (SP) map_rows(hi, r0, n, t, nt, [](float4 v) { return tf32x4(v); });
+    else split_rows(hi, lo, r0, n, t, nt);
+}
+
 // ---- accumulator fragments: element j of a warpgroup's m64nN accumulator sits at
 //      row = 16 * warp + lane / 4 + 8 * ((j / 2) % 2), column = 8 * (j / 4) + 2 * (lane % 4) + j % 2 --------------------
 __device__ __forceinline__ int frag_row(int tid, int j) { return 64 * (tid >> 7) + 16 * ((tid >> 5) & 3) + ((tid & 31) >> 2) + 8 * ((j >> 1) & 1); }
 __device__ __forceinline__ int frag_col(int tid, int j) { return 8 * (j >> 2) + 2 * (tid & 3) + (j & 1); }
 
 // ---- the kernel -----------------------------------------------------------------------------------------------------
-// The TMA problems' tensor maps, one per stage tile (A tiles, then B tiles), and their tile grid.
+// The TMA problems' tensor maps, one per source (A tiles, then B tiles), and their tile grid: nz batches (the attention
+// problems' sample x head) of mtiles x ntiles tiles.
 struct TmaArgs {
     CUtensorMap map[4];
-    int mtiles, ntiles;
+    int mtiles, ntiles, nz;
 };
+// what the consumers of a TMA problem transform in shared memory before the wgmmas read a stage (P::FIX, P::fix)
+enum { FIX_NONE = 0, FIX_A = 1, FIX_AB = 2 };
 constexpr int NTHREADS_TMA = 384, SMEM_MAX = 227 * 1024;
 // stages of a TMA problem: as many as fit next to the 1024-byte alignment slack and the barriers, at most 8
 __host__ __device__ constexpr int tma_stages(int bytes) { return (SMEM_MAX - 1024 - 128) / bytes < 8 ? (SMEM_MAX - 1024 - 128) / bytes : 8; }
@@ -284,12 +328,15 @@ __device__ __forceinline__ void reg_tile(const P& p, uint8_t* smem, int col_fast
 
 // TMA mainloop on persistent CTAs.  Warpgroups 0 and 1 (threads 0..255, the same rows and fragments as the register
 // mainloop) consume; warpgroup 2 produces: one thread issues the TMA boxes of every stage tile into a ring of S stages,
-// each with a full barrier (the producer's expect_tx, completed by the TMA bytes) and an empty barrier (one arrive per
-// consumer warp once the stage's wgmmas have retired).  Tile t = blockIdx.x, blockIdx.x + gridDim.x, ... is decoded
-// column-fastest, and the producer runs into the next tile's k-blocks while the consumers run the epilogue.
+// each with a full barrier (the producer's expect_tx in P::produce, completed by the TMA bytes) and an empty barrier (one
+// arrive per consumer warp once the stage's wgmmas have retired).  Tile t = blockIdx.x, blockIdx.x + gridDim.x, ... is
+// decoded batch-major, then column-fastest (the tiles of one batch are adjacent, so its operand panels are reused from L2),
+// and the producer runs into the next tile's k-blocks while the consumers run the epilogue.
 // Consumers keep one k-block's wgmmas in flight (wait_group 1) and wait for all only before a chunk fold and the epilogue;
 // wgmmas into one accumulator execute in issue order, so every tile's sums are those of the register mainloop.
-// P::AFIX: A tile 0 lands raw fp32 and each consumer warpgroup applies P::fix_a to its own 64 rows in place.
+// P::FIX: the stage lands raw and the consumers run P::fix on it (TF32 rounding, hi / lo split, transposition of MN-major
+// sources): FIX_A, each consumer warpgroup its own 64 rows of A behind its own named barrier; FIX_AB, in addition the B tiles
+// shared by both warpgroups, their rows split over all 256 consumer threads, behind one 256-thread named barrier.
 template <class P>
 __device__ __forceinline__ void tma_tiles(const P& p, const TmaArgs& ta, uint8_t* smem) {
     using L = typename P::L;
@@ -297,7 +344,6 @@ __device__ __forceinline__ void tma_tiles(const P& p, const TmaArgs& ta, uint8_t
     constexpr int NA = P::PRODS::NACC;
     constexpr int STAGE = L::BYTES, S = tma_stages(STAGE);
     constexpr int NT = P::CHUNK ? NA : 1, NTR = P::CHUNK ? NR : 1;
-    constexpr int KE = P::FMT == OP_TF32 ? 32 : 64;          // elements in a 128-byte row
     static_assert(S >= 2, "a TMA problem needs two stages");
     __shared__ __align__(8) uint64_t bars[2 * S];            // full[S], then empty[S]
     const int tid = threadIdx.x, wg = tid >> 7;
@@ -310,23 +356,25 @@ __device__ __forceinline__ void tma_tiles(const P& p, const TmaArgs& ta, uint8_t
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
-    const int kb = p.kblocks(), ntiles = ta.mtiles * ta.ntiles;
+    const int kb = p.kblocks(), per_z = ta.mtiles * ta.ntiles, ntiles = ta.nz * per_z;
     int stage = 0;
     uint32_t phase = 0;
+    auto decode = [&](int t, int& m0, int& n0, int& z) {
+        z = t / per_z;
+        const int r = t - z * per_z;
+        m0 = (r / ta.ntiles) * BM;
+        n0 = (r % ta.ntiles) * P::BN;
+    };
 
     if (wg == 2) {
         setmaxnreg_dec<40>();
         if (tid != 2 * 128) return;
         for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
-            const int m0 = (t / ta.ntiles) * BM, n0 = (t % ta.ntiles) * P::BN;
+            int m0, n0, z;
+            decode(t, m0, n0, z);
             for (int it = 0; it < kb; ++it) {
                 mbar_wait(empty0 + 8u * stage, phase ^ 1u);
-                const uint32_t full = full0 + 8u * stage, st = st0 + (uint32_t)stage * STAGE;
-                mbar_expect_tx(full, STAGE);
-#pragma unroll
-                for (int i = 0; i < L::NTA; ++i) tma_load(st + L::a(i), &ta.map[i], it * KE, m0, full);
-#pragma unroll
-                for (int j = 0; j < L::NTB; ++j) tma_load(st + L::b(j), &ta.map[L::NTA + j], it * KE, n0, full);
+                p.produce(ta, st0 + (uint32_t)stage * STAGE, full0 + 8u * stage, it, m0, n0, z);
                 if (++stage == S) { stage = 0; phase ^= 1u; }
             }
         }
@@ -340,19 +388,19 @@ __device__ __forceinline__ void tma_tiles(const P& p, const TmaArgs& ta, uint8_t
         if ((tid & 31) == 0) mbar_arrive(empty0 + 8u * s);
     };
     for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
-        const int m0 = (t / ta.ntiles) * BM, n0 = (t % ta.ntiles) * P::BN;
+        int m0, n0, z;
+        decode(t, m0, n0, z);
         zero(acc);
         zero(tot);
         int pend = -1;                                        // the stage whose wgmmas are still in flight
         for (int it = 0; it < kb; ++it) {
             mbar_wait(full0 + 8u * stage, phase);
             const uint32_t st = st0 + (uint32_t)stage * STAGE;
-            if constexpr (P::AFIX) {
-                float4* a = reinterpret_cast<float4*>(smem + (uint32_t)stage * STAGE + L::a(0) + (uint32_t)wg * 64u * 128u);
-#pragma unroll
-                for (int i = tid & 127; i < 64 * 8; i += 128) a[i] = P::fix_a(a[i]);
+            if constexpr (P::FIX != FIX_NONE) {
+                p.fix(smem + (uint32_t)stage * STAGE, wg, tid);
                 fence_proxy_async();
-                bar_named(1 + wg, 128);
+                if constexpr (P::FIX == FIX_A) bar_named(1 + wg, 128);
+                else bar_named(3, 256);
             }
             const bool fresh = P::CHUNK ? (it % P::CHUNK == 0) : (it == 0);
             wg_fence();
@@ -364,7 +412,7 @@ __device__ __forceinline__ void tma_tiles(const P& p, const TmaArgs& ta, uint8_t
                 if (pend >= 0) release(pend);
                 release(stage);
                 pend = -1;
-                if constexpr (P::CHUNK > 0) fold(p, acc, tot, m0, it / P::CHUNK, 0, tid);
+                if constexpr (P::CHUNK > 0) fold(p, acc, tot, m0, it / P::CHUNK, z, tid);
             } else {
                 wg_wait1();
                 if (pend >= 0) release(pend);
@@ -372,8 +420,8 @@ __device__ __forceinline__ void tma_tiles(const P& p, const TmaArgs& ta, uint8_t
             }
             if (++stage == S) { stage = 0; phase ^= 1u; }
         }
-        if constexpr (P::CHUNK > 0) p.epilogue(tot, m0, n0, 0, tid);
-        else p.epilogue(acc, m0, n0, 0, tid);
+        if constexpr (P::CHUNK > 0) p.epilogue(tot, m0, n0, z, tid);
+        else p.epilogue(acc, m0, n0, z, tid);
     }
 }
 
@@ -391,12 +439,33 @@ struct NoScale {
     __device__ __forceinline__ float chunk_scale(int, int, int) const { return 1.f; }
 };
 
-// Problems with P::TMA run the TMA mainloop; tile(i) names the K-major global source of stage tile i (A tiles, then B
-// tiles): rows x cols elements at row stride ld.  The others load through registers (P::load).
+// Problems with P::TMA run the TMA mainloop; tile(i) names the global source of tensor map i (A tiles, then B tiles): rows x
+// cols elements at row stride ld, read in boxes of 128 bytes x box_rows rows, with count > 0 a third dimension of count such
+// matrices at stride cstride (elements).  P::produce issues a stage's boxes from the P::NMAPS maps.  The others load through
+// registers (P::load).
 struct TmaTile {
     const void* base;
     long long rows, cols, ld;
+    int box_rows;
+    long long count = 0, cstride = 0;
 };
+// P::produce of the problems whose stage tiles are all K-major boxes of 2-D maps at (k-block, tile row): A tile i from
+// map i at row m0, B tile j from map NTA + j at row n0
+template <class P>
+__device__ __forceinline__ void produce_tiles(const TmaArgs& ta, uint32_t st, uint32_t bar, int it, int m0, int n0) {
+    using L = typename P::L;
+    constexpr int KE = P::FMT == OP_TF32 ? 32 : 64;          // elements in a 128-byte row
+    mbar_expect_tx(bar, L::BYTES);
+#pragma unroll
+    for (int i = 0; i < L::NTA; ++i) tma_load(st + L::a(i), &ta.map[i], it * KE, m0, bar);
+#pragma unroll
+    for (int j = 0; j < L::NTB; ++j) tma_load(st + L::b(j), &ta.map[L::NTA + j], it * KE, n0, bar);
+}
+#define TE_PRODUCE_TILES(P)                                                                                      \
+    static constexpr int NMAPS = L::NTA + L::NTB;                                                                \
+    __device__ void produce(const TmaArgs& ta, uint32_t st, uint32_t bar, int it, int m0, int n0, int) const { \
+        produce_tiles<P>(ta, st, bar, it, m0, n0);                                                               \
+    }
 
 // ---- z+ rule, first contraction: S = sd(R, Z) ---------------------------------------------------------------------
 // Z two-pass:    x+ W+^T + x- W-^T                        (A tiles x+ / x- transformed on load, B = W+ / W-)
@@ -413,7 +482,8 @@ struct ZsProb : NoScale {
     using L = Stage<PRODS, BN>;
     static constexpr bool COL_FAST = true;
     // single-pass: TMA (A = bf16(|x|), or raw x made tf32(|x|) in shared memory); two-pass: x+ / x- formed on load
-    static constexpr bool TMA = SINGLE, AFIX = SINGLE && !BF;
+    static constexpr bool TMA = SINGLE;
+    static constexpr int FIX = SINGLE && !BF ? FIX_A : FIX_NONE;
     int M, N, K;
     const float* x; long long ldx;
     const void* xabs;                       // BF: bf16(|x|) [M, K]
@@ -423,10 +493,13 @@ struct ZsProb : NoScale {
     float sscale, zsign;                    // S = sscale * sd(R, Z) ; SINGLE: sign of the |x| |W|^T term
 
     __device__ int kblocks() const { return K / (BF ? 64 : 32); }
-    __device__ static float4 fix_a(float4 v) { return tf32x4(absx4(v)); }
+    __device__ void fix(uint8_t* st, int wg, int tid) const {
+        map_rows(st + L::a(0), 64 * wg, 64, tid & 127, 128, [](float4 v) { return tf32x4(absx4(v)); });
+    }
+    TE_PRODUCE_TILES(ZsProb)
     TmaTile tile(int i) const {
-        if (i == 0) return BF ? TmaTile{xabs, M, K, K} : TmaTile{x, M, K, ldx};
-        return TmaTile{wa, N, K, K};
+        if (i == 0) return BF ? TmaTile{xabs, M, K, K, BM} : TmaTile{x, M, K, ldx, BM};
+        return TmaTile{wa, N, K, K, BN};
     }
     __device__ void load(uint8_t* st, int kb, int m0, int n0, int, int tid) const {
         for_k32(BM, x, ldx, m0, M, kb * 32, K, tid, [&](int rr, int c, float4 v) {
@@ -498,7 +571,8 @@ struct ZrProb {
     static constexpr int FMT = KIND == 0 ? OP_TF32 : KIND == 1 ? OP_BF16 : OP_F16;
     using PRODS = Prods<Pr<0, 0, 0>, Pr<1, 0, 1>>;           // S W+ and S W- into their own accumulators
     using L = Stage<PRODS, BN>;
-    static constexpr bool TMA = true, AFIX = false;
+    static constexpr bool TMA = true;
+    static constexpr int FIX = FIX_NONE;
     int M, N, K;
     const void* s; const void* wp; const void* wn;     // S [M, K] (row stride K), W+^T / W-^T [N, K]
     const float* rs; int rs_ld; const float* cp; const float* cn;   // KIND 2: scales of S, of the rows of W+^T / W-^T
@@ -506,8 +580,9 @@ struct ZrProb {
     int accum;                                                      // add into out instead of overwriting it
 
     __device__ int kblocks() const { return K / (KIND ? 64 : 32); }
+    TE_PRODUCE_TILES(ZrProb)
     __device__ float chunk_scale(int row, int ch, int) const { return (KIND == 2 && row < M) ? rs[(long long)row * rs_ld + ch] : 1.f; }
-    TmaTile tile(int i) const { return i == 0 ? TmaTile{s, M, K, K} : TmaTile{i == 1 ? wp : wn, N, K, K}; }
+    TmaTile tile(int i) const { return i == 0 ? TmaTile{s, M, K, K, BM} : TmaTile{i == 1 ? wp : wn, N, K, K, BN}; }
     __device__ void epilogue(float (&acc)[2][BN / 2], int m0, int n0, int, int tid) const {
 #pragma unroll
         for (int j = 0; j < BN / 2; j += 2) {
@@ -541,7 +616,7 @@ struct LrpSProb : NoScale {
     static constexpr int BN = 128, CHUNK = 0, FMT = OP_TF32;
     using PRODS = One;
     using L = Stage<PRODS, BN>;
-    static constexpr bool COL_FAST = true, TMA = false, AFIX = false;
+    static constexpr bool COL_FAST = true, TMA = false;
     int M, N, K;
     const float* x; long long ldx; const float* w;      // w: W+ or W- (tf32) [N, K]
     const float* r; long long ldr; float* out;           // out: S [M, N], row stride N
@@ -569,13 +644,15 @@ struct LrpRProb : NoScale {
     static constexpr int BN = 128, CHUNK = 0, FMT = OP_TF32;
     using PRODS = One;
     using L = Stage<PRODS, BN>;
-    static constexpr bool TMA = true, AFIX = false;
+    static constexpr bool TMA = true;
+    static constexpr int FIX = FIX_NONE;
     int M, N, K;
     const float* s; const float* wt;
     const float* x; long long ldx; float* out; long long ldo;
     int accum;
     __device__ int kblocks() const { return K / 32; }
-    TmaTile tile(int i) const { return i == 0 ? TmaTile{s, M, K, K} : TmaTile{wt, N, K, K}; }
+    TE_PRODUCE_TILES(LrpRProb)
+    TmaTile tile(int i) const { return i == 0 ? TmaTile{s, M, K, K, BM} : TmaTile{wt, N, K, K, BN}; }
     __device__ void epilogue(float (&acc)[1][BN / 2], int m0, int n0, int, int tid) const {
 #pragma unroll
         for (int j = 0; j < BN / 2; j += 2) {
@@ -646,16 +723,20 @@ struct LinProb : LinArgs {
     using L = Stage<PRODS, BN>;
     static constexpr bool COL_FAST = true;
     // the fp16 forms and the single-pass TF32 form (A rounded in shared memory) on TMA; 3xTF32 splits A on load
-    static constexpr bool TMA = FORM != LIN_3XTF32, AFIX = FORM == LIN_TF32;
+    static constexpr bool TMA = FORM != LIN_3XTF32;
+    static constexpr int FIX = FORM == LIN_TF32 ? FIX_A : FIX_NONE;
     __device__ int kblocks() const { return K / (F16 ? 64 : 32); }
     __device__ float chunk_scale(int row, int ch, int) const {
         if constexpr (F16) return row < o.M ? rs[(long long)row * rs_ld + ch] : 1.f;
         else return 1.f;
     }
-    __device__ static float4 fix_a(float4 v) { return tf32x4(v); }
+    __device__ void fix(uint8_t* st, int wg, int tid) const {
+        map_rows(st + L::a(0), 64 * wg, 64, tid & 127, 128, [](float4 v) { return tf32x4(v); });
+    }
+    TE_PRODUCE_TILES(LinProb)
     TmaTile tile(int i) const {
-        if (i < L::NTA) return TmaTile{i == 0 ? a : a_lo, o.M, K, F16 ? K : lda};
-        return TmaTile{i == L::NTA ? b : b_lo, o.N, K, K};
+        if (i < L::NTA) return TmaTile{i == 0 ? a : a_lo, o.M, K, F16 ? K : lda, BM};
+        return TmaTile{i == L::NTA ? b : b_lo, o.N, K, K, BN};
     }
     __device__ void load(uint8_t* st, int kb, int m0, int n0, int, int tid) const {
         for_k32(BM, (const float*)a, lda, m0, o.M, kb * 32, K, tid, [&](int r, int c, float4 v) { st_split(st + L::a(0), st + L::a(1), r, c, v); });
@@ -680,24 +761,28 @@ struct NnProb : NoScale {
     static constexpr int BN = BN_, CHUNK = 0, FMT = OP_TF32;
     using PRODS = std::conditional_t<SP, One, Split3>;
     using L = Stage<PRODS, BN>;
-    static constexpr bool COL_FAST = false, TMA = false, AFIX = false;
+    // A and B land raw in their (hi) tiles from 2-D maps over the packed [batch * N, H * dh] rows; a 32-column box never
+    // leaves head h (dh is 32 or 64).  Rows past a sample's N are the next sample's (zeros past the tensor): they reach only
+    // the output rows and columns the epilogue masks.
+    static constexpr bool TMA = true;
+    static constexpr int FIX = FIX_AB;
     int N, H, dh, ld_out, batch;
     const float* a; long long lda; const float* b; long long ldb;
     const float* E; float* out; float alpha;
     __device__ int kblocks() const { return dh / 32; }
-    __device__ void load(uint8_t* st, int kb, int m0, int n0, int bh, int tid) const {
-        const int s = bh / H, h = bh % H;
-        const long long rows = (long long)batch * N;
-        const int k0 = h * dh + kb * 32, kend = h * dh + dh;
-        if (SP) {
-            for_k32(BM, a, lda, (long long)s * N + m0, rows, k0, kend, tid, [&](int r, int c, float4 v) { st4(st + L::a(0), r, c, tf32x4(v)); });
-            for_k32(BN, b, ldb, (long long)s * N + n0, rows, k0, kend, tid, [&](int r, int c, float4 v) { st4(st + L::b(0), r, c, tf32x4(v)); });
-        } else {
-            for_k32(BM, a, lda, (long long)s * N + m0, rows, k0, kend, tid,
-                    [&](int r, int c, float4 v) { st_split(st + L::a(0), st + L::a(1), r, c, v); });
-            for_k32(BN, b, ldb, (long long)s * N + n0, rows, k0, kend, tid,
-                    [&](int r, int c, float4 v) { st_split(st + L::b(0), st + L::b(1), r, c, v); });
-        }
+    static constexpr int NMAPS = 2;
+    TmaTile tile(int i) const {
+        return i == 0 ? TmaTile{a, (long long)batch * N, H * dh, lda, BM} : TmaTile{b, (long long)batch * N, H * dh, ldb, BN};
+    }
+    __device__ void produce(const TmaArgs& ta, uint32_t st, uint32_t bar, int kb, int m0, int n0, int bh) const {
+        const int s = bh / H, k = (bh % H) * dh + kb * 32;
+        mbar_expect_tx(bar, TILE128 + BN * 128);
+        tma_load(st + L::a(0), &ta.map[0], k, s * N + m0, bar);
+        tma_load(st + L::b(0), &ta.map[1], k, s * N + n0, bar);
+    }
+    __device__ void fix(uint8_t* st, int wg, int tid) const {
+        fix_tf32<SP>(st + L::a(0), st + L::a(1), 64 * wg, 64, tid & 127, 128);
+        fix_tf32<SP>(st + L::b(0), st + L::b(1), 0, BN, tid, 256);
     }
     __device__ void epilogue(float (&acc)[1][BN / 2], int m0, int n0, int bh, int tid) const {
         const int ncols = (N + 3) & ~3;                  // the row padding up to a multiple of 4 is written as zeros
@@ -735,13 +820,20 @@ struct NnProb : NoScale {
                 *reinterpret_cast<float2*>(out + ((long long)bh * N + r) * ld_out + col) = make_float2(acc[0][j] * inv, acc[0][j + 1] * inv);
             }
         } else {
+        // E of the whole fragment is loaded before the first store, so that its loads are in flight together (out may alias E)
+        float2 ef[BN / 4];
+#pragma unroll
+        for (int j = 0; j < BN / 2; j += 2) {
+            const int r = m0 + frag_row(tid, j), col = n0 + frag_col(tid, j);
+            ef[j / 2] = (EPI != AT_STORE && r < N && col < ncols)
+                            ? *reinterpret_cast<const float2*>(E + ((long long)bh * N + r) * ld_out + col) : make_float2(0.f, 0.f);
+        }
 #pragma unroll
         for (int j = 0; j < BN / 2; j += 2) {
             const int r = m0 + frag_row(tid, j), col = n0 + frag_col(tid, j);
             if (r >= N || col >= ncols) continue;
             const long long off = ((long long)bh * N + r) * ld_out + col;
-            float2 e = make_float2(0.f, 0.f);
-            if (EPI != AT_STORE) e = *reinterpret_cast<const float2*>(E + off);
+            const float2 e = ef[j / 2];
             float v[2] = {alpha * acc[0][j], alpha * acc[0][j + 1]};
             const float ee[2] = {e.x, e.y};
 #pragma unroll
@@ -757,52 +849,67 @@ struct NnProb : NoScale {
 };
 
 // ---- token-reduced N x d contraction: out[b, m, h*BN + d] = epi(alpha * sum_k A_h[m,k] X[b, k, h*BN + d]) ----------------
-//   AMN 0: A_h[m,k] = map[bh][m][k] (K-major) ; AMN 1: A_h[m,k] = map[bh][k][m] (MN-major, transposed on load)
-//   X is MN-major (transposed on load).  a_shared: A indexed by the batch only (dense rollout product, "heads" = column tiles).
+//   AMN 0: A_h[m,k] = map[bh][m][k] (K-major) ; AMN 1: A_h[m,k] = map[bh][k][m] (MN-major, transposed in shared memory)
+//   X is MN-major (transposed in shared memory).  a_shared: A indexed by the batch only (dense rollout product, "heads" =
+//   column tiles).
+// The map is a 3-D tensor map of inner extent N (not NP) at row stride NP, so keys and rows >= N land as zeros in every bh
+// and the pad columns are never read; X is one over [batch, N, ld] of inner extent n_pad: tokens >= N and columns >= n_pad
+// land as zeros.  The MN-major sources land as 32 x 32 boxes behind the tiles (Stage::land: A's four boxes when AMN, then
+// X's BN / 32).
 template <int AMN, int EPI, bool SP, int BN_>
 struct NkProb : NoScale {
     static constexpr int BN = BN_, CHUNK = SP ? 0 : 4, FMT = OP_TF32;
     using PRODS = std::conditional_t<SP, One, Split3>;
-    using L = Stage<PRODS, BN>;
-    static constexpr bool COL_FAST = false, TMA = false, AFIX = false;
-    int N, H, NP, ld_out, n_out, n_pad, a_shared;
+    static constexpr int LAND_A = AMN ? BM * 128 : 0, LAND_X = BN * 128;
+    using L = Stage<PRODS, BN, LAND_A + LAND_X>;
+    static constexpr bool TMA = true;
+    static constexpr int FIX = FIX_AB;
+    int N, H, NP, ld_out, n_out, n_pad, a_shared, batch;
     const float* map; const float* X; long long ldx;
     const float* rowscale; const float* E; float* out; float alpha;
     __device__ int kblocks() const { return (N + 31) / 32; }
-    template <class F>
-    __device__ __forceinline__ void load_a(int kb, int m0, int bh, int tid, F f) const {
-        const int s = bh / H;
-        const float* base = map + (long long)(a_shared ? s : bh) * N * NP;
-        if (AMN == 0) for_k32(BM, base, NP, m0, N, kb * 32, N, tid, f);
-        else for_mn32(BM, base, NP, m0, N, kb * 32, N, tid, f);
+    static constexpr int NMAPS = 2;
+    TmaTile tile(int i) const {
+        if (i == 0) return TmaTile{map, N, N, NP, AMN ? 32 : BM, (long long)batch * (a_shared ? 1 : H), (long long)N * NP};
+        return TmaTile{X, N, n_pad, ldx, 32, batch, (long long)N * ldx};
     }
-    __device__ void load(uint8_t* st, int kb, int m0, int, int bh, int tid) const {
-        const int s = bh / H, h = bh % H;
-        const float* xb = X + (long long)s * N * ldx;
-        if (SP) {
-            load_a(kb, m0, bh, tid, [&](int r, int c, float4 v) { st4(st + L::a(0), r, c, tf32x4(v)); });
-            for_mn32(BN, xb, ldx, h * BN, n_pad, kb * 32, N, tid, [&](int r, int c, float4 v) { st4(st + L::b(0), r, c, tf32x4(v)); });
-        } else {
-            load_a(kb, m0, bh, tid, [&](int r, int c, float4 v) { st_split(st + L::a(0), st + L::a(1), r, c, v); });
-            for_mn32(BN, xb, ldx, h * BN, n_pad, kb * 32, N, tid,
-                     [&](int r, int c, float4 v) { st_split(st + L::b(0), st + L::b(1), r, c, v); });
-        }
+    __device__ void produce(const TmaArgs& ta, uint32_t st, uint32_t bar, int kb, int m0, int, int bh) const {
+        const int s = bh / H, h = bh % H, za = a_shared ? s : bh;
+        mbar_expect_tx(bar, (AMN ? LAND_A : TILE128) + LAND_X);
+        if (AMN == 0) tma_load3(st + L::a(0), &ta.map[0], kb * 32, m0, za, bar);
+#pragma unroll
+        for (int j = 0; j < LAND_A / 4096; ++j) tma_load3(st + L::land() + j * 4096, &ta.map[0], m0 + 32 * j, kb * 32, za, bar);
+#pragma unroll
+        for (int j = 0; j < LAND_X / 4096; ++j)
+            tma_load3(st + L::land() + LAND_A + j * 4096, &ta.map[1], h * BN + 32 * j, kb * 32, s, bar);
+    }
+    __device__ void fix(uint8_t* st, int wg, int tid) const {
+        if (AMN) transpose_rows(st + L::land(), 64 * wg, 64, tid & 127, 128, put_tf32<SP>(st + L::a(0), st + L::a(1)));
+        else fix_tf32<SP>(st + L::a(0), st + L::a(1), 64 * wg, 64, tid & 127, 128);
+        transpose_rows(st + L::land() + LAND_A, 0, BN, tid, 256, put_tf32<SP>(st + L::b(0), st + L::b(1)));
     }
     __device__ void epilogue(float (&acc)[1][BN / 2], int m0, int, int bh, int tid) const {
         const int s = bh / H, h = bh % H;
+        // E of the whole fragment is loaded before the first store, so that its loads are in flight together (out may alias E)
+        float2 ef[BN / 4];
+#pragma unroll
+        for (int j = 0; j < BN / 2; j += 2) {
+            const int m = m0 + frag_row(tid, j), gcol = h * BN + frag_col(tid, j);
+            ef[j / 2] = (EPI != AT_STORE && m < N && gcol < n_pad)
+                            ? *reinterpret_cast<const float2*>(E + ((long long)s * N + m) * ld_out + gcol) : make_float2(0.f, 0.f);
+        }
 #pragma unroll
         for (int j = 0; j < BN / 2; j += 2) {
             const int m = m0 + frag_row(tid, j), gcol = h * BN + frag_col(tid, j);
             if (m >= N || gcol >= n_pad) continue;
             const long long off = ((long long)s * N + m) * ld_out + gcol;
             float v[2] = {alpha * acc[0][j], alpha * acc[0][j + 1]};
+            const float2 e = ef[j / 2];
             if (EPI == AT_MUL) {
-                const float2 e = *reinterpret_cast<const float2*>(E + off);
                 v[0] *= e.x; v[1] *= e.y;
             } else if (EPI == AT_RESID) {
                 // the identity's share of the rollout step, added in fp32: out = A J + diag(rowscale) J
                 const float rsc = rowscale ? rowscale[(long long)s * N + m] : 1.f;
-                const float2 e = *reinterpret_cast<const float2*>(E + off);
                 v[0] += rsc * e.x; v[1] += rsc * e.y;
             }
             if (gcol >= n_out) v[0] = 0.f;
@@ -839,21 +946,25 @@ EncodeTiled encode_tiled() {
     }();
     return fn;
 }
-// The map of one stage tile: boxes of 128 bytes (one swizzled row) x box_rows rows, 128-byte swizzle (the layout swz() and
-// sdesc() describe), rows and columns past the source filled with zeros.  TMA needs a 16-byte-aligned base and a row
-// stride that is a multiple of 16 bytes.
-bool encode_tile(CUtensorMap* map, const TmaTile& t, int esize, int box_rows) {
+// The map of a source: boxes of 128 bytes (one swizzled row) x box_rows rows (x 1 matrix), 128-byte swizzle (the layout swz()
+// and sdesc() describe), rows, columns and matrices past the source filled with zeros.  TMA needs a 16-byte-aligned base and
+// strides that are multiples of 16 bytes.
+bool encode_tile(CUtensorMap* map, const TmaTile& t, int esize) {
     const EncodeTiled fn = encode_tiled();
-    if (!fn || ((uintptr_t)t.base & 15u) || (t.ld * esize) % 16 != 0 || t.rows < 1 || t.cols < 1) return false;
-    const cuuint64_t dims[2] = {(cuuint64_t)t.cols, (cuuint64_t)t.rows}, strides[1] = {(cuuint64_t)(t.ld * esize)};
-    const cuuint32_t box[2] = {(cuuint32_t)(128 / esize), (cuuint32_t)box_rows}, estr[2] = {1, 1};
-    return fn(map, esize == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_UINT16, 2, const_cast<void*>(t.base), dims,
-              strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+    const int rank = t.count > 0 ? 3 : 2;
+    if (!fn || ((uintptr_t)t.base & 15u) || (t.ld * esize) % 16 != 0 || (t.cstride * esize) % 16 != 0 || t.rows < 1 || t.cols < 1)
+        return false;
+    const cuuint64_t dims[3] = {(cuuint64_t)t.cols, (cuuint64_t)t.rows, (cuuint64_t)t.count};
+    const cuuint64_t strides[2] = {(cuuint64_t)(t.ld * esize), (cuuint64_t)(t.cstride * esize)};
+    const cuuint32_t box[3] = {(cuuint32_t)(128 / esize), (cuuint32_t)t.box_rows, 1}, estr[3] = {1, 1, 1};
+    return fn(map, esize == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_UINT16, rank, const_cast<void*>(t.base),
+              dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+              CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-// grid: (m-tiles, column tiles, z).
-// P::TMA problems run min(tiles, SMs) persistent CTAs of 384 threads that walk the tiles column-fastest (tma_tiles).
+// grid: (m-tiles, column tiles, batches).
+// P::TMA problems run min(tiles, SMs) persistent CTAs of 384 threads that walk the tiles batch-major, then column-fastest
+// (tma_tiles).
 // The others run one CTA of 256 threads per tile.  P::COL_FAST problems are launched with the column tile in blockIdx.x,
 // so that consecutively scheduled CTAs share an A panel and the panel is read from HBM about once instead of once per
 // column tile; the weights, at most a few tens of MB, stay in L2.  More than 65535 m-tiles do not fit in grid.y: those
@@ -866,15 +977,17 @@ int launch(const P& p, dim3 grid, cudaStream_t st) {
     int col_fast = 0, threads = NTHREADS, smem = 2 * P::L::BYTES + 1024;
     if constexpr (P::TMA) {
         constexpr int ESIZE = P::FMT == OP_TF32 ? 4 : 2;
-        for (int i = 0; i < P::L::NTA + P::L::NTB; ++i)
-            if (!encode_tile(&ta.map[i], p.tile(i), ESIZE, i < P::L::NTA ? BM : P::BN)) {
-                te_set_last_error("te_tc: cannot encode a TMA tensor map (16-byte-aligned base and row stride required)");
+        static_assert(P::NMAPS <= 4, "TmaArgs holds four tensor maps");
+        for (int i = 0; i < P::NMAPS; ++i)
+            if (!encode_tile(&ta.map[i], p.tile(i), ESIZE)) {
+                te_set_last_error("te_tc: cannot encode a TMA tensor map (16-byte-aligned base and strides required)");
                 return TE_ERR_ARG;
             }
-        const long long tiles = (long long)grid.x * grid.y;
-        if (grid.z != 1 || tiles > INT32_MAX) { te_set_last_error("te_tc: grid too large for one launch"); return TE_ERR_ARG; }
+        const long long tiles = (long long)grid.x * grid.y * grid.z;
+        if (tiles > INT32_MAX) { te_set_last_error("te_tc: grid too large for one launch"); return TE_ERR_ARG; }
         ta.mtiles = (int)grid.x;
         ta.ntiles = (int)grid.y;
+        ta.nz = (int)grid.z;
         grid = dim3((unsigned)std::min<long long>(tiles, sm_count()));
         threads = NTHREADS_TMA;
         smem = tma_stages(P::L::BYTES) * P::L::BYTES + 1024;
@@ -1347,7 +1460,7 @@ template <int AMN, int EPI, bool SP, int BN>
 int nk(const float* map, int NP, const float* X, long long ldx, int batch, int H, int N, float* out, int ld_out, int n_out,
        int n_pad, int a_shared, const float* rowscale, const float* E, float alpha, cudaStream_t st) {
     NkProb<AMN, EPI, SP, BN> p;
-    p.N = N; p.H = H; p.NP = NP; p.ld_out = ld_out; p.n_out = n_out; p.n_pad = n_pad; p.a_shared = a_shared;
+    p.N = N; p.H = H; p.NP = NP; p.ld_out = ld_out; p.n_out = n_out; p.n_pad = n_pad; p.a_shared = a_shared; p.batch = batch;
     p.map = map; p.X = X; p.ldx = ldx; p.rowscale = rowscale; p.E = E; p.out = out; p.alpha = alpha;
     return launch(p, dim3(mtiles(N), 1, (unsigned)(batch * H)), st);
 }
