@@ -155,6 +155,10 @@ TE_API int te_vit_explain(const te_vit_config* cfg, const float* weights, const 
  * (ViT_LRP.py:102-130).  name in {"attn","attn_grad","attn_cam","qkv","x_in","ctx","logits","rollout_mats"}, and the
  * scratch regions of the last attribute call, "tmp_d0".."tmp_d3" [B,N,D], "tmp_f0","tmp_f1" [B,N,F], "tmp_3d0","tmp_3d1"
  * [B,N,3D] (diagnostics; a region may be larger than its view).
+ * Test / diagnostic taps, views of the saved forward activations (named after the oracle's cache keys), per layer:
+ * "xn1","attn_out","x_mid","xn2","mlp_out" [B,N,D], "h" (fc1 output before the GELU), "g" [B,N,F], "mean1","rstd1",
+ * "mean2","rstd2" [B,N]; per model: "x_last" (the last block's output), "x_final_norm" [B,N,D].  attribute() leaves
+ * every saved forward activation as the forward wrote it.
  * Returns a device pointer, 4 dims and 4 element strides (unused dims are 1).  Host-only address arithmetic: nothing on
  * the device is read. */
 TE_API int te_vit_tensor(const te_vit_config* cfg, int batch, void* workspace, const char* name, int layer,
@@ -223,7 +227,11 @@ TE_API int te_bert_explain(const te_bert_config* cfg, const float* weights, cons
                     long long workspace_bytes, void* stream);
 /* get_attn / get_attn_gradients / get_attn_cam of BertSelfAttention (BERT.py:281-297):
  * name in {"attn","attn_grad","attn_cam","hidden","logits","relevance_in"} and the scratch regions "tmp_d0".."tmp_d3",
- * "tmp_f0","tmp_f1", "tmp_3d0","tmp_3d1" as for te_vit_tensor. */
+ * "tmp_f0","tmp_f1", "tmp_3d0","tmp_3d1" as for te_vit_tensor.
+ * Test / diagnostic taps, views of the saved forward activations, per layer: "qkv" [B,S,3D], "ctx", "d1" (attention
+ * output dense), "s1" (= d1 + hidden, the input of the attention-output LayerNorm), "ao" (its output), "d2" (output
+ * dense), "s2" (= d2 + ao) [B,S,D], "hpre" (intermediate dense before the GELU), "g" [B,S,F], "mean1","rstd1","mean2",
+ * "rstd2" [B,S]; per model: "h_last" [B,S,D], "pooled" [B,D]. */
 TE_API int te_bert_tensor(const te_bert_config* cfg, int batch, int seq, void* workspace, const char* name, int layer,
                    float** ptr, long long dims[4], long long strides[4]);
 

@@ -43,6 +43,29 @@ def _merge(t):
     return t.permute(0, 2, 1, 3).reshape(b, n, h * d)
 
 
+def layer_forward(p, dm, i, h, ext_mask):
+    """``BertLayer.forward`` (``:498-519``) of layer ``i`` on its input ``h`` [B,S,D] with the additive mask ``ext_mask``:
+    returns (output, the layer's cache)."""
+    L = "bert.encoder.layer.%d." % i
+    dh = dm.dim // dm.heads
+    c = {"h": h}
+    q = _heads(F.linear(h, p[L + "attention.self.query.weight"], p[L + "attention.self.query.bias"]), dm.heads)
+    k = _heads(F.linear(h, p[L + "attention.self.key.weight"], p[L + "attention.self.key.bias"]), dm.heads)
+    v = _heads(F.linear(h, p[L + "attention.self.value.weight"], p[L + "attention.self.value.bias"]), dm.heads)
+    scores = (q @ k.transpose(-1, -2)) / math.sqrt(dh)
+    masked = scores + ext_mask
+    probs = masked.softmax(dim=-1)
+    ctx = _merge(probs @ v)
+    d1 = F.linear(ctx, p[L + "attention.output.dense.weight"], p[L + "attention.output.dense.bias"])
+    ao = F.layer_norm(d1 + h, (dm.dim,), p[L + "attention.output.LayerNorm.weight"],
+                      p[L + "attention.output.LayerNorm.bias"], dm.eps)
+    g = F.gelu(F.linear(ao, p[L + "intermediate.dense.weight"], p[L + "intermediate.dense.bias"]))
+    d2 = F.linear(g, p[L + "output.dense.weight"], p[L + "output.dense.bias"])
+    h = F.layer_norm(d2 + ao, (dm.dim,), p[L + "output.LayerNorm.weight"], p[L + "output.LayerNorm.bias"], dm.eps)
+    c.update(q=q, k=k, v=v, scores=scores, probs=probs, ctx=ctx, d1=d1, ao=ao, g=g, d2=d2)
+    return h, c
+
+
 def forward(params, input_ids, attention_mask, num_heads, need_grad=False):
     p = params
     dm = BertDims(params, num_heads)
@@ -57,25 +80,9 @@ def forward(params, input_ids, attention_mask, num_heads, need_grad=False):
     if need_grad:
         h = h.detach().requires_grad_(True)
     ext_mask = (1.0 - attention_mask[:, None, None, :].to(dtype)) * -10000.0       # transformers 3.5.1
-    dh = dm.dim // dm.heads
     cache = {"dims": dm, "layers": [], "ext_mask": ext_mask}
     for i in range(dm.depth):
-        L = "bert.encoder.layer.%d." % i
-        c = {"h": h}
-        q = _heads(F.linear(h, p[L + "attention.self.query.weight"], p[L + "attention.self.query.bias"]), dm.heads)
-        k = _heads(F.linear(h, p[L + "attention.self.key.weight"], p[L + "attention.self.key.bias"]), dm.heads)
-        v = _heads(F.linear(h, p[L + "attention.self.value.weight"], p[L + "attention.self.value.bias"]), dm.heads)
-        scores = (q @ k.transpose(-1, -2)) / math.sqrt(dh)
-        masked = scores + ext_mask
-        probs = masked.softmax(dim=-1)
-        ctx = _merge(probs @ v)
-        d1 = F.linear(ctx, p[L + "attention.output.dense.weight"], p[L + "attention.output.dense.bias"])
-        ao = F.layer_norm(d1 + h, (dm.dim,), p[L + "attention.output.LayerNorm.weight"],
-                          p[L + "attention.output.LayerNorm.bias"], dm.eps)
-        g = F.gelu(F.linear(ao, p[L + "intermediate.dense.weight"], p[L + "intermediate.dense.bias"]))
-        d2 = F.linear(g, p[L + "output.dense.weight"], p[L + "output.dense.bias"])
-        h = F.layer_norm(d2 + ao, (dm.dim,), p[L + "output.LayerNorm.weight"], p[L + "output.LayerNorm.bias"], dm.eps)
-        c.update(q=q, k=k, v=v, scores=scores, probs=probs, ctx=ctx, d1=d1, ao=ao, g=g, d2=d2)
+        h, c = layer_forward(p, dm, i, h, ext_mask)
         cache["layers"].append(c)
     cache["h_last"] = h
     first = h[:, 0]

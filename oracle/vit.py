@@ -48,6 +48,28 @@ def _merge_heads(t):
     return t.permute(0, 2, 1, 3).reshape(b, n, h * d)           # 'b h n d -> b n (h d)'
 
 
+def block_forward(p, cfg, i, t):
+    """``Block.forward`` (``:196-201``) of block ``i`` on its input ``t`` [B,N,D]: returns (output, the block's cache)."""
+    pre = "blocks.%d." % i
+    scale = (cfg.dim // cfg.heads) ** -0.5
+    c = {"x_in": t}
+    xn1 = F.layer_norm(t, (cfg.dim,), p[pre + "norm1.weight"], p[pre + "norm1.bias"], cfg.eps_block)
+    qkv = F.linear(xn1, p[pre + "attn.qkv.weight"], p.get(pre + "attn.qkv.bias"))
+    q, k, v = [_split_heads(u, cfg.heads) for u in qkv.chunk(3, dim=-1)]   # '(qkv h d)'
+    dots = (q @ k.transpose(-1, -2)) * scale
+    attn = dots.softmax(dim=-1)
+    ctx = _merge_heads(attn @ v)
+    attn_out = F.linear(ctx, p[pre + "attn.proj.weight"], p[pre + "attn.proj.bias"])
+    x_mid = t + attn_out
+    xn2 = F.layer_norm(x_mid, (cfg.dim,), p[pre + "norm2.weight"], p[pre + "norm2.bias"], cfg.eps_block)
+    hpre = F.linear(xn2, p[pre + "mlp.fc1.weight"], p[pre + "mlp.fc1.bias"])
+    g = F.gelu(hpre)
+    mlp_out = F.linear(g, p[pre + "mlp.fc2.weight"], p[pre + "mlp.fc2.bias"])
+    c.update(xn1=xn1, q=q, k=k, v=v, attn=attn, ctx=ctx, attn_out=attn_out, x_mid=x_mid,
+             xn2=xn2, g=g, mlp_out=mlp_out)
+    return x_mid + mlp_out, c
+
+
 def forward(params, x, num_heads, need_grad=False, norm_eps=None):
     """Returns (logits [B,C], cache).  ``cache`` holds every tensor the relprop needs.
     ``norm_eps``: one epsilon for every LayerNorm (the ``ViT_new`` factories, ``ViT_new.py:226-254``)."""
@@ -67,25 +89,8 @@ def forward(params, x, num_heads, need_grad=False, norm_eps=None):
     if need_grad:
         t = t.detach().requires_grad_(True)     # puts every attn tensor on an autograd graph
     cache = {"cfg": cfg, "blocks": [], "tokens_pre_pos": tokens_pre_pos.detach(), "image": x}
-    scale = (cfg.dim // cfg.heads) ** -0.5
     for i in range(cfg.depth):
-        pre = "blocks.%d." % i
-        c = {"x_in": t}
-        xn1 = F.layer_norm(t, (cfg.dim,), p[pre + "norm1.weight"], p[pre + "norm1.bias"], cfg.eps_block)
-        qkv = F.linear(xn1, p[pre + "attn.qkv.weight"], p.get(pre + "attn.qkv.bias"))
-        q, k, v = [_split_heads(u, cfg.heads) for u in qkv.chunk(3, dim=-1)]   # '(qkv h d)'
-        dots = (q @ k.transpose(-1, -2)) * scale
-        attn = dots.softmax(dim=-1)
-        ctx = _merge_heads(attn @ v)
-        attn_out = F.linear(ctx, p[pre + "attn.proj.weight"], p[pre + "attn.proj.bias"])
-        x_mid = t + attn_out
-        xn2 = F.layer_norm(x_mid, (cfg.dim,), p[pre + "norm2.weight"], p[pre + "norm2.bias"], cfg.eps_block)
-        hpre = F.linear(xn2, p[pre + "mlp.fc1.weight"], p[pre + "mlp.fc1.bias"])
-        g = F.gelu(hpre)
-        mlp_out = F.linear(g, p[pre + "mlp.fc2.weight"], p[pre + "mlp.fc2.bias"])
-        t = x_mid + mlp_out
-        c.update(xn1=xn1, q=q, k=k, v=v, attn=attn, ctx=ctx, attn_out=attn_out, x_mid=x_mid,
-                 xn2=xn2, g=g, mlp_out=mlp_out)
+        t, c = block_forward(p, cfg, i, t)
         cache["blocks"].append(c)
     xf = F.layer_norm(t, (cfg.dim,), p["norm.weight"], p["norm.bias"], cfg.eps_final)
     cache["x_final_norm"] = xf

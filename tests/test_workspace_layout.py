@@ -103,6 +103,75 @@ def test_bert_lent_regions_cover_their_uses(kw, batch, seq):
     _check(ext, uses)
 
 
+# ---- the saved-activation taps: documented views, inside the workspace, disjoint --------------------------------------------
+SCRATCH = ["tmp_d%d" % i for i in range(4)] + ["tmp_f0", "tmp_f1", "tmp_3d0", "tmp_3d1"]
+
+
+def _tap(fn, cfg, shape, name, layer):
+    p, dims, strides = ctypes.c_void_p(), (ctypes.c_longlong * 4)(), (ctypes.c_longlong * 4)()
+    rc = fn(ctypes.byref(cfg), *shape, ctypes.c_void_p(FAKE_WS), name.encode(), layer, ctypes.byref(p), dims, strides)
+    assert rc == 0, name
+    return p.value, tuple(dims), tuple(strides)
+
+
+def _rows(B, N, W):
+    """[B, N, W] row-major, padded to four dims"""
+    return (B, N, W, 1), (N * W, W, 1, 1)
+
+
+def _check_taps(fn, cfg, shape, nbytes, per_layer, per_model, depth):
+    """every tap has its documented dims / strides, lies inside the workspace, and no two saved taps (nor a saved tap and
+    the lent scratch) share a byte"""
+    spans = []
+    for layer, table in [(l, per_layer) for l in range(depth)] + [(0, per_model)]:
+        for name, (dims, strides) in table.items():
+            p, d, s = _tap(fn, cfg, shape, name, layer)
+            assert (d, s) == (dims, strides), "%s[%d]: dims %s strides %s" % (name, layer, d, s)
+            extent = 1 + sum((n - 1) * st for n, st in zip(d, s))
+            assert FAKE_WS <= p and p + 4 * extent <= FAKE_WS + nbytes, "%s[%d] outside the workspace" % (name, layer)
+            spans.append((p, p + 4 * extent, "%s[%d]" % (name, layer)))
+    for name in SCRATCH:
+        p, d, s = _tap(fn, cfg, shape, name, 0)
+        spans.append((p, p + 4 * (1 + sum((n - 1) * st for n, st in zip(d, s))), name))
+    spans.sort()
+    for (a0, a1, an), (b0, b1, bn) in zip(spans, spans[1:]):
+        assert a1 <= b0, "%s overlaps %s" % (an, bn)
+
+
+@pytest.mark.parametrize("kw", VIT, ids=lambda kw: "-".join("%s%s" % (k, v) for k, v in kw.items()) or "vit_b16")
+@pytest.mark.parametrize("batch", [1, 3])
+def test_vit_taps_in_bounds_and_disjoint(kw, batch):
+    lib = _lib.load()
+    cfg = vit_config(**kw)
+    B, D, F, H, C = batch, cfg.dim, cfg.mlp_dim, cfg.heads, cfg.num_classes
+    N = (cfg.img_size // cfg.patch_size) ** 2 + (2 if cfg.distilled else 1)
+    NP = (N + 3) & ~3
+    att = ((B, H, N, N), (H * N * NP, N * NP, NP, 1))
+    per_layer = dict(attn=att, attn_grad=att, attn_cam=att, qkv=_rows(B, N, 3 * D), h=_rows(B, N, F), g=_rows(B, N, F))
+    per_layer.update({n: _rows(B, N, D) for n in ("x_in", "xn1", "ctx", "attn_out", "x_mid", "xn2", "mlp_out")})
+    per_layer.update({n: ((B, N, 1, 1), (N, 1, 1, 1)) for n in ("mean1", "rstd1", "mean2", "rstd2")})
+    per_model = dict(x_last=_rows(B, N, D), x_final_norm=_rows(B, N, D), logits=((B, C, 1, 1), (C, 1, 1, 1)),
+                     rollout_mats=((cfg.depth, B, N, N), (B * N * NP, N * NP, NP, 1)))
+    nbytes = lib.te_vit_workspace_bytes(ctypes.byref(cfg), batch)
+    _check_taps(lib.te_vit_tensor, cfg, (batch,), nbytes, per_layer, per_model, cfg.depth)
+
+
+@pytest.mark.parametrize("kw", BERT, ids=lambda kw: "-".join("%s%s" % (k, v) for k, v in kw.items()) or "bert_base")
+@pytest.mark.parametrize("batch,seq", [(1, 130), (3, 512)])
+def test_bert_taps_in_bounds_and_disjoint(kw, batch, seq):
+    lib = _lib.load()
+    cfg = bert_config(**kw)
+    B, N, D, F, H, C = batch, seq, cfg.hidden, cfg.intermediate, cfg.heads, cfg.num_labels
+    NP = (N + 3) & ~3
+    att = ((B, H, N, N), (H * N * NP, N * NP, NP, 1))
+    per_layer = dict(attn=att, attn_grad=att, attn_cam=att, qkv=_rows(B, N, 3 * D), hpre=_rows(B, N, F), g=_rows(B, N, F))
+    per_layer.update({n: _rows(B, N, D) for n in ("hidden", "ctx", "d1", "s1", "ao", "d2", "s2")})
+    per_layer.update({n: ((B, N, 1, 1), (N, 1, 1, 1)) for n in ("mean1", "rstd1", "mean2", "rstd2")})
+    per_model = dict(h_last=_rows(B, N, D), pooled=((B, D, 1, 1), (D, 1, 1, 1)), logits=((B, C, 1, 1), (C, 1, 1, 1)))
+    nbytes = lib.te_bert_workspace_bytes(ctypes.byref(cfg), batch, seq)
+    _check_taps(lib.te_bert_tensor, cfg, (batch, seq), nbytes, per_layer, per_model, cfg.layers)
+
+
 # te_*_workspace_bytes of the benchmarked configurations (batch 1 and the benchmarked batch), as laid out before the
 # lent regions were sized by their uses: with F = 4D every use fits in M*F, so the size must not move
 BASELINE_BYTES = [

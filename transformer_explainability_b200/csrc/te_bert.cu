@@ -443,6 +443,9 @@ extern "C" int te_bert_tensor(const te_bert_config* cfg, int batch, int seq, voi
         return set(ws.tF[n[5] - '0'], d.B, d.N, d.F, 1, (long long)d.N * d.F, d.F, 1, 1);
     if (n.rfind("tmp_3d", 0) == 0 && n.size() == 7 && n[6] >= '0' && n[6] <= '1')
         return set(ws.t3D[n[6] - '0'], d.B, d.N, 3LL * d.D, 1, (long long)d.N * 3 * d.D, 3LL * d.D, 1, 1);
+    const long long ND = (long long)d.N * d.D, NF = (long long)d.N * d.F;
+    if (n == "h_last") return set(ws.h_last, d.B, d.N, d.D, 1, ND, d.D, 1, 1);
+    if (n == "pooled") return set(ws.pooled, d.B, d.D, 1, 1, d.D, 1, 1, 1);
     if (layer < 0 || layer >= d.L) { te_set_last_error("te_bert_tensor: layer out of range"); return TE_ERR_ARG; }
     LayerAct& a = ws.layer[layer];
     const long long hs = (long long)d.N * d.NP, bs = hs * d.H;
@@ -450,6 +453,15 @@ extern "C" int te_bert_tensor(const te_bert_config* cfg, int batch, int seq, voi
     if (n == "attn_grad") return set(a.G, d.B, d.H, d.N, d.N, bs, hs, d.NP, 1);
     if (n == "attn_cam") return set(a.cam, d.B, d.H, d.N, d.N, bs, hs, d.NP, 1);
     if (n == "hidden") return set(a.h, d.B, d.N, d.D, 1, (long long)d.N * d.D, d.D, 1, 1);
+    // the rest of the saved forward activations of the layer (views only: test / diagnostic taps)
+    if (n == "qkv") return set(a.qkv, d.B, d.N, 3LL * d.D, 1, 3 * ND, 3LL * d.D, 1, 1);
+    float* rowD = n == "ctx" ? a.ctx : n == "d1" ? a.d1 : n == "s1" ? a.s1 : n == "ao" ? a.ao : n == "d2" ? a.d2
+                : n == "s2" ? a.s2 : nullptr;
+    if (rowD) return set(rowD, d.B, d.N, d.D, 1, ND, d.D, 1, 1);
+    float* rowF = n == "hpre" ? a.hpre : n == "g" ? a.g : nullptr;
+    if (rowF) return set(rowF, d.B, d.N, d.F, 1, NF, d.F, 1, 1);
+    float* row1 = n == "mean1" ? a.mean1 : n == "rstd1" ? a.rstd1 : n == "mean2" ? a.mean2 : n == "rstd2" ? a.rstd2 : nullptr;
+    if (row1) return set(row1, d.B, d.N, 1, 1, d.N, 1, 1, 1);
     te_set_last_error("te_bert_tensor: unknown tensor name");
     return TE_ERR_ARG;
 }

@@ -488,6 +488,9 @@ extern "C" int te_vit_tensor(const te_vit_config* cfg, int batch, void* workspac
     if (n == "logits") return set(ws.logits, d.B, d.C, 1, 1, d.C, 1, 1, 1);
     if (n == "relevance_in") return set(ws.tD[0], d.B, d.N, d.D, 1, (long long)d.N * d.D, d.D, 1, 1);
     if (n == "rollout_mats") return set(ws.mats, d.L, d.B, d.N, d.N, (long long)d.B * d.N * d.NP, (long long)d.N * d.NP, d.NP, 1);
+    const long long ND = (long long)d.N * d.D, NF = (long long)d.N * d.F;
+    if (n == "x_last") return set(ws.x_last, d.B, d.N, d.D, 1, ND, d.D, 1, 1);
+    if (n == "x_final_norm") return set(ws.xf, d.B, d.N, d.D, 1, ND, d.D, 1, 1);
     // scratch of the last attribute() call (debug / diagnostics): tmp_d0..3 [B,N,D], tmp_f0..1 [B,N,F], tmp_3d0..1 [B,N,3D]
     if (n.rfind("tmp_d", 0) == 0 && n.size() == 6 && n[5] >= '0' && n[5] <= '3')
         return set(ws.tD[n[5] - '0'], d.B, d.N, d.D, 1, (long long)d.N * d.D, d.D, 1, 1);
@@ -504,6 +507,14 @@ extern "C" int te_vit_tensor(const te_vit_config* cfg, int batch, void* workspac
     if (n == "qkv") return set(a.qkv, d.B, d.N, 3LL * d.D, 1, (long long)d.N * 3 * d.D, 3LL * d.D, 1, 1);
     if (n == "x_in") return set(a.x_in, d.B, d.N, d.D, 1, (long long)d.N * d.D, d.D, 1, 1);
     if (n == "ctx") return set(a.ctx, d.B, d.N, d.D, 1, (long long)d.N * d.D, d.D, 1, 1);
+    // the rest of the saved forward activations of the block (views only: test / diagnostic taps)
+    float* rowD = n == "xn1" ? a.xn1 : n == "attn_out" ? a.attn_out : n == "x_mid" ? a.x_mid : n == "xn2" ? a.xn2
+                : n == "mlp_out" ? a.mlp_out : nullptr;
+    if (rowD) return set(rowD, d.B, d.N, d.D, 1, ND, d.D, 1, 1);
+    float* rowF = n == "h" ? a.h : n == "g" ? a.g : nullptr;
+    if (rowF) return set(rowF, d.B, d.N, d.F, 1, NF, d.F, 1, 1);
+    float* row1 = n == "mean1" ? a.mean1 : n == "rstd1" ? a.rstd1 : n == "mean2" ? a.mean2 : n == "rstd2" ? a.rstd2 : nullptr;
+    if (row1) return set(row1, d.B, d.N, 1, 1, d.N, 1, 1, 1);
     te_set_last_error("te_vit_tensor: unknown tensor name");
     return TE_ERR_ARG;
 }
