@@ -432,6 +432,32 @@ TE_API long long te_pr_curve_workspace_bytes(long long n);
 TE_API int te_pr_curve(const unsigned* keys, long long n, float* thresholds, long long* tps, long long* fps, long long* count,
                        void* workspace, long long workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * ERASER rationale evaluation  (BERT_rationale_benchmark/models/pipeline/bert_pipeline.py:96-138,547-582;
+ * BERT_rationale_benchmark/metrics.py:111-215)
+ * ---------------------------------------------------------------------------------------------- */
+#define TE_ERASER_MAX_WORDS 1024
+#define TE_ERASER_MAX_KS 64
+#define TE_ERASER_MAX_THRESHOLDS 8
+/* Workspace of te_eraser_rationales for `words` word ranges and `spans` truth spans over `batch` documents. */
+TE_API long long te_eraser_workspace_bytes(int batch, long long words, long long spans);
+/* Per document b of maps [batch, seq] (device, padded rows), over its W = word_offsets[b+1] - word_offsets[b] words
+ * (W <= TE_ERASER_MAX_WORDS) and its truth spans [span_offsets[b], span_offsets[b+1]):
+ *   word_scores[w] = max over the word's pieces p in [first, last] (piece_ranges [words, 2]) of clamp(maps[b, p], min=0); a
+ *     NaN piece makes the word NaN (np.max);
+ *   the words are ranked NaN first, then by descending score, then by ascending word index (-0 == +0: the order key of
+ *     te_perturb_images); order[b, r] = the word at rank r for r < min(kmax, W), -1 up to kmax = ks[nk-1];
+ *   counts [batch, nk, 3 + nthr] (int32), over the first n = min(ks[i], W) ranks: n, tok_hits = words inside any truth
+ *     span (start <= w < end), span_hits = words whose one-word span [w, w+1) is a truth span, and per threshold t
+ *     iou_hits = words whose best IoU (1 / len of the shortest truth span holding w, 0 if none; fp64) is >= thresholds[t].
+ * word_offsets, piece_ranges, span_offsets, spans [.., 2], ks (non-decreasing, nk <= TE_ERASER_MAX_KS) and thresholds
+ * (fp64, nthr <= TE_ERASER_MAX_THRESHOLDS) are host arrays, validated before anything is launched: every piece range must
+ * satisfy 0 <= first <= last < seq and every span 0 <= start <= end, else TE_ERR_ARG. */
+TE_API int te_eraser_rationales(const float* maps, int batch, int seq, const int* word_offsets, const int* piece_ranges,
+                                const int* span_offsets, const int* spans, const int* ks, int nk, const double* thresholds,
+                                int nthr, float* word_scores, int* order, int* counts, void* workspace,
+                                long long workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -125,10 +125,15 @@ PROTOTYPES = {
     "te_seg_metrics": (c_int, [_P, _P, c_int, c_int, c_int, c_float, _P, _P, _P, _P, _P, _P, _P, _P, c_ll, _P]),
     "te_pr_curve_workspace_bytes": (c_ll, [c_ll]),
     "te_pr_curve": (c_int, [_P, c_ll, _P, _P, _P, _P, _P, c_ll, _P]),
+    "te_eraser_workspace_bytes": (c_ll, [c_int, c_ll, c_ll]),
+    "te_eraser_rationales": (c_int, [_P, c_int, c_int, _P, _P, _P, _P, _P, c_int, _P, c_int, _P, _P, _P, _P, c_ll, _P]),
 }
 
 PERTURB_MAX_STEPS = 64          # TE_PERTURB_MAX_STEPS
 PERTURB_MAX_CHANNELS = 16       # TE_PERTURB_MAX_CHANNELS
+ERASER_MAX_WORDS = 1024         # TE_ERASER_MAX_WORDS
+ERASER_MAX_KS = 64              # TE_ERASER_MAX_KS
+ERASER_MAX_THRESHOLDS = 8       # TE_ERASER_MAX_THRESHOLDS
 
 _lib = None
 

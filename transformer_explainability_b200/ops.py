@@ -605,3 +605,55 @@ def pr_curve(sorted_keys):
           "te_pr_curve")
     k = int(count.item())
     return thr[:k], tps[:k], fps[:k]
+
+
+# ---- ERASER rationale evaluation (BERT_rationale_benchmark/models/pipeline/bert_pipeline.py, metrics.py) ---------------------
+def _host_i32(a, what, cols=None):
+    import numpy as np
+    a = np.ascontiguousarray(np.asarray(a, dtype=np.int64).reshape(-1, cols) if cols else np.asarray(a, dtype=np.int64))
+    if a.size and (a.min() < -2 ** 31 or a.max() >= 2 ** 31):
+        raise ValueError("eraser_rationales: %s outside the int32 range" % what)
+    return np.ascontiguousarray(a.astype(np.int32))
+
+
+@_on_device
+def eraser_rationales(maps, piece_ranges, word_offsets, spans, span_offsets, ks, thresholds=(0.5,)):
+    """Per document b of maps [B, S] (padded rows, fp32 CUDA): the word scores (max of the clamped map over each word's
+    inclusive piece range ``piece_ranges[word_offsets[b]:word_offsets[b+1]]``), the top-kmax word order (NaN first, then
+    descending score, then ascending word index) and per k the counts (n_pred, tok_hits, span_hits, iou_hits per
+    threshold) against the truth spans ``spans[span_offsets[b]:span_offsets[b+1]]`` of (start, end) word indices
+    (see include/te_b200.h: te_eraser_rationales).  The ranges, spans, offsets, ks and thresholds are host sequences.
+    Returns a dict of CUDA tensors: ``word_scores`` fp32 [words], ``order`` int32 [B, max(ks)] (-1 past the last word),
+    ``counts`` int32 [B, len(ks), 3 + len(thresholds)]."""
+    import numpy as np
+    _req(maps)
+    if maps.dim() != 2:
+        raise ValueError("eraser_rationales: maps [B, S] expected")
+    B, S = maps.shape
+    woff = _host_i32(word_offsets, "word_offsets")
+    soff = _host_i32(span_offsets, "span_offsets")
+    if woff.shape != (B + 1,) or soff.shape != (B + 1,):
+        raise ValueError("eraser_rationales: word_offsets and span_offsets need B + 1 = %d entries" % (B + 1))
+    ranges = _host_i32(piece_ranges, "piece_ranges", 2)
+    sp = _host_i32(spans, "spans", 2)
+    if len(ranges) != int(woff[-1]) or len(sp) != int(soff[-1]):
+        raise ValueError("eraser_rationales: %d piece ranges / %d spans, the offsets end at %d / %d"
+                         % (len(ranges), len(sp), woff[-1], soff[-1]))
+    ks = [int(k) for k in ks]
+    thr = np.ascontiguousarray(np.asarray([float(t) for t in thresholds], dtype=np.float64))
+    if not 0 < len(ks) <= _lib.ERASER_MAX_KS or len(thr) > _lib.ERASER_MAX_THRESHOLDS:
+        raise ValueError("eraser_rationales: 1..%d ks and at most %d thresholds expected"
+                         % (_lib.ERASER_MAX_KS, _lib.ERASER_MAX_THRESHOLDS))
+    lib = _lib.load()
+    ws = _workspace(check(lib.te_eraser_workspace_bytes(B, len(ranges), len(sp)), "te_eraser_workspace_bytes"), maps.device)
+    dev = maps.device
+    out = {"word_scores": torch.empty(len(ranges), device=dev, dtype=torch.float32),
+           "order": torch.empty(B, max(max(ks), 0), device=dev, dtype=torch.int32),
+           "counts": torch.empty(B, len(ks), 3 + len(thr), device=dev, dtype=torch.int32)}
+    ks_c = (_lib.c_int * len(ks))(*ks)
+    host = lambda a: a.ctypes.data_as(_lib.c_void_p) if a.size else None      # noqa: E731
+    check(lib.te_eraser_rationales(ptr(maps), B, S, host(woff), host(ranges), host(soff), host(sp), ks_c, len(ks), host(thr),
+                                   len(thr), ptr(out["word_scores"]) if len(ranges) else None,
+                                   ptr(out["order"]) if max(ks) > 0 else None, ptr(out["counts"]), ptr(ws), ws.numel() * 4,
+                                   _stream()), "te_eraser_rationales")
+    return out
