@@ -397,6 +397,9 @@ TE_API int te_perturb_images(const float* images, const float* saliency, int bat
  * p_target gives -inf, an underflowed p_second +inf; a target outside [0, classes) gives NaN). */
 TE_API int te_logit_stats(const float* logits, const int* target, int rows, int classes, int* pred, float* max_logit,
                           float* max_prob, float* dissim, void* stream);
+/* Per row of logits [rows, classes] (classes >= 1): probs = the fp32 softmax, with torch.softmax's arithmetic (the row
+ * maximum subtracted, expf, the sum, one division per entry).  A row holding a NaN gives a NaN row. */
+TE_API int te_class_probs(const float* logits, int rows, int classes, float* probs, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Segmentation evaluation  (baselines/ViT/imagenet_seg_eval.py:212-277,312-314; utils/metrices.py)
@@ -457,6 +460,26 @@ TE_API int te_eraser_rationales(const float* maps, int batch, int seq, const int
                                 const int* span_offsets, const int* spans, const int* ks, int nk, const double* thresholds,
                                 int nthr, float* word_scores, int* order, int* counts, void* workspace,
                                 long long workspace_bytes, void* stream);
+
+/* ERASER faithfulness inputs (metrics.py:284-364: comprehensiveness, sufficiency and their AOPC bins) */
+#define TE_ERASER_MAX_SELECTIONS 64
+#define TE_ERASER_MAX_SEQ 8192
+/* Workspace of te_eraser_reduce_inputs for `words` word ranges over `batch` documents and `selections` sizes. */
+TE_API long long te_eraser_reduce_workspace_bytes(int batch, long long words, int selections);
+/* Per document b of maps [batch, seq] (device, padded rows) and input_ids [batch, seq] (int64, device), with its length
+ * lengths[b] (the row is [CLS] p_1 ... p_n [SEP] at positions 0 .. lengths[b] - 1) and its W words (piece ranges as for
+ * te_eraser_rationales): the words are ranked exactly as te_eraser_rationales ranks them, each inner piece carries the
+ * smallest rank of the words whose range holds it, and for each selection size n = n_select[b, j] (0 <= n <= W):
+ *   out_ids[b, j, 0] (comprehensiveness) = [CLS], every inner piece (positions 1 .. lengths[b] - 2) of rank >= n, [SEP];
+ *   out_ids[b, j, 1] (sufficiency)       = [CLS], every inner piece of rank < n, [SEP];
+ * both in position order and zero past their lengths out_len[b, j, 0 / 1] (int32; the two sum to lengths[b] + 2).
+ * lengths, word_offsets, piece_ranges and n_select [batch, selections] are host arrays, validated before anything is
+ * launched: 2 <= lengths[b] <= seq, every range 1 <= first <= last <= lengths[b] - 2, W <= TE_ERASER_MAX_WORDS,
+ * 0 <= n <= W, selections <= TE_ERASER_MAX_SELECTIONS and seq <= TE_ERASER_MAX_SEQ, else TE_ERR_ARG. */
+TE_API int te_eraser_reduce_inputs(const float* maps, const long long* input_ids, int batch, int seq, const int* lengths,
+                                   const int* word_offsets, const int* piece_ranges, const int* n_select, int selections,
+                                   long long* out_ids, int* out_len, void* workspace, long long workspace_bytes,
+                                   void* stream);
 
 #ifdef __cplusplus
 }

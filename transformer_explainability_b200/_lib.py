@@ -127,6 +127,9 @@ PROTOTYPES = {
     "te_pr_curve": (c_int, [_P, c_ll, _P, _P, _P, _P, _P, c_ll, _P]),
     "te_eraser_workspace_bytes": (c_ll, [c_int, c_ll, c_ll]),
     "te_eraser_rationales": (c_int, [_P, c_int, c_int, _P, _P, _P, _P, _P, c_int, _P, c_int, _P, _P, _P, _P, c_ll, _P]),
+    "te_eraser_reduce_workspace_bytes": (c_ll, [c_int, c_ll, c_int]),
+    "te_eraser_reduce_inputs": (c_int, [_P, _P, c_int, c_int, _P, _P, _P, _P, c_int, _P, _P, _P, c_ll, _P]),
+    "te_class_probs": (c_int, [_P, c_int, c_int, _P, _P]),
 }
 
 PERTURB_MAX_STEPS = 64          # TE_PERTURB_MAX_STEPS
@@ -134,6 +137,8 @@ PERTURB_MAX_CHANNELS = 16       # TE_PERTURB_MAX_CHANNELS
 ERASER_MAX_WORDS = 1024         # TE_ERASER_MAX_WORDS
 ERASER_MAX_KS = 64              # TE_ERASER_MAX_KS
 ERASER_MAX_THRESHOLDS = 8       # TE_ERASER_MAX_THRESHOLDS
+ERASER_MAX_SELECTIONS = 64      # TE_ERASER_MAX_SELECTIONS
+ERASER_MAX_SEQ = 8192           # TE_ERASER_MAX_SEQ
 
 _lib = None
 

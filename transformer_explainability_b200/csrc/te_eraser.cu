@@ -3,6 +3,9 @@
 //     (NaN propagates); the words are ranked NaN first, then by descending score, then by ascending word index (the order
 //     key of te_perturb_images); the first kmax ranks are written out, and per k the counts of the predicted words that
 //     metrics.py's hard-rationale scores need come from prefix sums along that order.
+//   * reduce_kernel: one block per document, the ranking of eraser_kernel; each piece is marked with the smallest rank of
+//     the words holding it, and per selection size n the pieces of the first n ranks (sufficiency) and the other inner
+//     pieces (comprehensiveness) are compacted, between the document's [CLS] and [SEP], by one block scan.
 // The ragged host arrays (word piece ranges, truth spans, their offsets) are validated on the host and copied into the
 // workspace, so no index the caller passes is read from the map before it has been checked.
 #include "../../include/te_b200.h"
@@ -28,6 +31,36 @@ __device__ __forceinline__ uint32_t order_key(float v) {
     return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
 }
 
+// Score and rank the W words of one document (map row m, inclusive piece ranges): word_scores[w] (may be null) = the max
+// of the clamped map over the word's pieces (NaN propagates), sword[r] = the word at rank r.  Ends with a block barrier.
+__device__ __forceinline__ void rank_words(const float* __restrict__ m, const int2* __restrict__ ranges, int W,
+                                           float* __restrict__ word_scores, unsigned long long* skey, int* sword) {
+    for (int w = threadIdx.x; w < W; w += blockDim.x) {
+        const int2 r = ranges[w];
+        float s = 0.f;
+        bool nan = false, first = true;
+        for (int p = r.x; p <= r.y; ++p) {
+            float v = m[p];
+            if (v != v) { nan = true; continue; }
+            v = v < 0.f ? 0.f : v;                                 // clamp(min=0)
+            s = first ? v : fmaxf(s, v);
+            first = false;
+        }
+        if (nan) s = __int_as_float(0x7fc00000);
+        if (word_scores) word_scores[w] = s;
+        skey[w] = ((unsigned long long)(~order_key(s)) << 32) | (unsigned)w;   // ascending = ranking order
+    }
+    __syncthreads();
+    // rank = number of smaller keys (all keys are distinct)
+    for (int w = threadIdx.x; w < W; w += blockDim.x) {
+        const unsigned long long k = skey[w];
+        int rank = 0;
+        for (int u = 0; u < W; ++u) rank += skey[u] < k;
+        sword[rank] = w;
+    }
+    __syncthreads();
+}
+
 __global__ void __launch_bounds__(kThreads) eraser_kernel(
         const float* __restrict__ maps, int seq, const int* __restrict__ word_off, const int2* __restrict__ ranges,
         const int* __restrict__ span_off, const int2* __restrict__ spans, EraserParams prm, float* __restrict__ word_scores,
@@ -41,31 +74,7 @@ __global__ void __launch_bounds__(kThreads) eraser_kernel(
     const float* m = maps + (long long)b * seq;
     const int nind = 2 + prm.nthr;
 
-    // word scores and ranking keys
-    for (int w = threadIdx.x; w < W; w += kThreads) {
-        const int2 r = ranges[w0 + w];
-        float s = 0.f;
-        bool nan = false, first = true;
-        for (int p = r.x; p <= r.y; ++p) {
-            float v = m[p];
-            if (v != v) { nan = true; continue; }
-            v = v < 0.f ? 0.f : v;                                 // clamp(min=0)
-            s = first ? v : fmaxf(s, v);
-            first = false;
-        }
-        if (nan) s = __int_as_float(0x7fc00000);
-        word_scores[w0 + w] = s;
-        skey[w] = ((unsigned long long)(~order_key(s)) << 32) | (unsigned)w;
-    }
-    __syncthreads();
-    // rank = number of smaller keys (all keys are distinct)
-    for (int w = threadIdx.x; w < W; w += kThreads) {
-        const unsigned long long k = skey[w];
-        int rank = 0;
-        for (int u = 0; u < W; ++u) rank += skey[u] < k;
-        sword[rank] = w;
-    }
-    __syncthreads();
+    rank_words(m, ranges + w0, W, word_scores + w0, skey, sword);
     int* ord = order + (long long)b * prm.kmax;
     for (int r = threadIdx.x; r < prm.kmax; r += kThreads) ord[r] = r < W ? sword[r] : -1;
 
@@ -113,6 +122,73 @@ __global__ void __launch_bounds__(kThreads) eraser_kernel(
         const int i = e / ncol, c = e - i * ncol;
         const int n = min(prm.k[i], W);
         counts[((long long)b * prm.nk + i) * ncol + c] = c == 0 ? n : (n > 0 ? (int)sind[c - 1][n - 1] : 0);
+    }
+}
+
+// Reduced rows of document b for each selection size n = n_select[b, j]: every inner piece p in [1, len - 2] whose
+// smallest holding rank is < n goes to the sufficiency row, every other inner piece to the comprehensiveness row, both in
+// position order between the document's first ([CLS]) and last ([SEP]) token; zeros past each row's length.
+__global__ void __launch_bounds__(kThreads) reduce_kernel(
+        const float* __restrict__ maps, const long long* __restrict__ ids, int seq, const int* __restrict__ lens,
+        const int* __restrict__ word_off, const int2* __restrict__ ranges, const int* __restrict__ n_select, int J,
+        long long* __restrict__ out_ids, int* __restrict__ out_len) {
+    __shared__ unsigned long long skey[TE_ERASER_MAX_WORDS];
+    __shared__ int sword[TE_ERASER_MAX_WORDS];
+    __shared__ int swarp[kWarps];
+    extern __shared__ int pmin[];                                  // [seq]: smallest rank of the words holding each piece
+    const int b = blockIdx.x;
+    const int w0 = word_off[b], W = word_off[b + 1] - w0;
+    const int len = lens[b];
+    const long long* row = ids + (long long)b * seq;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+
+    for (int p = threadIdx.x; p < len; p += kThreads) pmin[p] = 0x7fffffff;
+    rank_words(maps + (long long)b * seq, ranges + w0, W, nullptr, skey, sword);
+    for (int r = threadIdx.x; r < W; r += kThreads) {
+        const int2 rg = ranges[w0 + sword[r]];
+        for (int p = rg.x; p <= rg.y; ++p) atomicMin(&pmin[p], r);
+    }
+    __syncthreads();
+    const long long cls = row[0], sep = row[len - 1];
+    for (int j = 0; j < J; ++j) {
+        const int n = n_select[b * J + j];
+        long long* comp = out_ids + (((long long)b * J + j) * 2) * seq;
+        long long* suff = comp + seq;
+        int carry = 0;                                             // rationale pieces before the current tile
+        for (int t0 = 1; t0 <= len - 2; t0 += kThreads) {
+            const int p = t0 + threadIdx.x;
+            const bool in = p <= len - 2;
+            const bool sel = in && pmin[p] < n;
+            const unsigned ball = __ballot_sync(0xffffffffu, sel);
+            if (lane == 0) swarp[warp] = __popc(ball);
+            __syncthreads();
+            int before = carry, total = carry;
+            for (int u = 0; u < kWarps; ++u) {
+                before += u < warp ? swarp[u] : 0;
+                total += swarp[u];
+            }
+            before += __popc(ball & ((1u << lane) - 1u));
+            if (in) {
+                if (sel) suff[1 + before] = row[p];
+                else comp[p - before] = row[p];                    // 1 + (p - 1 - before)
+            }
+            carry = total;
+            __syncthreads();                                       // swarp is rewritten by the next tile
+        }
+        const int R = carry;
+        const int lc = len - R, ls = 2 + R;
+        for (int p = threadIdx.x; p < seq; p += kThreads) {
+            if (p >= lc) comp[p] = 0;
+            if (p >= ls) suff[p] = 0;
+        }
+        if (threadIdx.x == 0) {
+            comp[0] = cls;
+            comp[lc - 1] = sep;
+            suff[0] = cls;
+            suff[ls - 1] = sep;
+            out_len[(b * J + j) * 2] = lc;
+            out_len[(b * J + j) * 2 + 1] = ls;
+        }
     }
 }
 
@@ -188,6 +264,63 @@ extern "C" int te_eraser_rationales(const float* maps, int batch, int seq, const
         return TE_ERR_CUDA;
     }
     eraser_kernel<<<batch, kThreads, 0, st>>>(maps, seq, d_woff, d_ranges, d_soff, d_spans, prm, word_scores, order, counts);
+    TE_CUDA_CHECK_LAUNCH();
+    return TE_OK;
+}
+
+extern "C" long long te_eraser_reduce_workspace_bytes(int batch, long long words, int selections) {
+    if (batch <= 0 || words < 0 || words > 0x7fffffffLL || selections <= 0) return TE_ERR_ARG;
+    return up256(4LL * (batch + 1)) + up256(8 * words) + up256(4LL * batch) + up256(4LL * batch * selections);
+}
+
+extern "C" int te_eraser_reduce_inputs(const float* maps, const long long* input_ids, int batch, int seq, const int* lengths,
+                                       const int* word_offsets, const int* piece_ranges, const int* n_select, int selections,
+                                       long long* out_ids, int* out_len, void* workspace, long long workspace_bytes,
+                                       void* stream) {
+    REQ(maps && input_ids && lengths && word_offsets && n_select && out_ids && out_len,
+        "te_eraser_reduce_inputs: null argument");
+    REQ(batch > 0 && batch <= 65535, "te_eraser_reduce_inputs: batch must lie in 1..65535");
+    REQ(seq >= 2 && seq <= TE_ERASER_MAX_SEQ, "te_eraser_reduce_inputs: seq outside 2..TE_ERASER_MAX_SEQ");
+    REQ(selections > 0 && selections <= TE_ERASER_MAX_SELECTIONS,
+        "te_eraser_reduce_inputs: selections outside 1..TE_ERASER_MAX_SELECTIONS");
+    REQ(word_offsets[0] == 0, "te_eraser_reduce_inputs: word offsets must start at 0");
+    for (int b = 0; b < batch; ++b) {
+        const long long nw = (long long)word_offsets[b + 1] - word_offsets[b];
+        REQ(nw >= 0 && nw <= TE_ERASER_MAX_WORDS, "te_eraser_reduce_inputs: a document holds 0..TE_ERASER_MAX_WORDS words");
+        REQ(lengths[b] >= 2 && lengths[b] <= seq, "te_eraser_reduce_inputs: every length must lie in 2..seq");
+        for (long long w = word_offsets[b]; w < word_offsets[b + 1]; ++w)
+            REQ(piece_ranges[2 * w] >= 1 && piece_ranges[2 * w] <= piece_ranges[2 * w + 1] &&
+                piece_ranges[2 * w + 1] <= lengths[b] - 2,
+                "te_eraser_reduce_inputs: every piece range [first, last] must satisfy 1 <= first <= last <= length - 2");
+        for (int j = 0; j < selections; ++j)
+            REQ(n_select[(long long)b * selections + j] >= 0 && n_select[(long long)b * selections + j] <= nw,
+                "te_eraser_reduce_inputs: every selection size must lie in 0..W of its document");
+    }
+    const long long words = word_offsets[batch];
+    REQ(words == 0 || piece_ranges, "te_eraser_reduce_inputs: null piece ranges");
+    REQ(workspace && (((uintptr_t)workspace) & 255u) == 0, "te_eraser_reduce_inputs: workspace null or not 256-byte aligned");
+    if (te_eraser_reduce_workspace_bytes(batch, words, selections) > workspace_bytes) {
+        te_set_last_error("te_eraser_reduce_inputs: workspace too small");
+        return TE_ERR_WORKSPACE;
+    }
+    char* p = static_cast<char*>(workspace);
+    int* d_woff = reinterpret_cast<int*>(p);
+    p += up256(4LL * (batch + 1));
+    int2* d_ranges = reinterpret_cast<int2*>(p);
+    p += up256(8 * words);
+    int* d_lens = reinterpret_cast<int*>(p);
+    p += up256(4LL * batch);
+    int* d_nsel = reinterpret_cast<int*>(p);
+    cudaStream_t st = ST(stream);
+    if (cudaMemcpyAsync(d_woff, word_offsets, 4 * (size_t)(batch + 1), cudaMemcpyHostToDevice, st) != cudaSuccess ||
+        (words && cudaMemcpyAsync(d_ranges, piece_ranges, 8 * (size_t)words, cudaMemcpyHostToDevice, st) != cudaSuccess) ||
+        cudaMemcpyAsync(d_lens, lengths, 4 * (size_t)batch, cudaMemcpyHostToDevice, st) != cudaSuccess ||
+        cudaMemcpyAsync(d_nsel, n_select, 4 * (size_t)batch * selections, cudaMemcpyHostToDevice, st) != cudaSuccess) {
+        te_set_last_error("te_eraser_reduce_inputs: copy of the host arrays failed");
+        return TE_ERR_CUDA;
+    }
+    reduce_kernel<<<batch, kThreads, 4 * (size_t)seq, st>>>(maps, input_ids, seq, d_lens, d_woff, d_ranges, d_nsel,
+                                                             selections, out_ids, out_len);
     TE_CUDA_CHECK_LAUNCH();
     return TE_OK;
 }

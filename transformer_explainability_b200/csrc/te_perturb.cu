@@ -3,6 +3,7 @@
 //     uint32 keys of the saliency finds, for every step, the key threshold T and the index cut among the keys equal to T
 //     (ties broken by ascending pixel index); a grid-wide stream then writes out[S,B,C,P] from one read of x and s.
 //   * te_logit_stats: arg-max / max logit / max softmax probability / log(p_target / p_second), one warp per row.
+//   * te_class_probs: the fp32 softmax of each row, one warp per row.
 #include "../../include/te_b200.h"
 #include "te_kernels.h"
 
@@ -225,6 +226,23 @@ __global__ void logit_stats_kernel(const float* __restrict__ logits, const int* 
     }
 }
 
+// one warp per row of logits [R, K]: torch.softmax (maximum subtracted, expf, sum, divide); fmaxf skips a NaN, whose
+// expf term then makes the sum and every probability of the row NaN
+__global__ void class_probs_kernel(const float* __restrict__ logits, int R, int K, float* __restrict__ probs) {
+    const int lane = threadIdx.x & 31;
+    const int r = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (r >= R) return;
+    const float* l = logits + (long long)r * K;
+    float m = -INFINITY;
+    for (int j = lane; j < K; j += 32) m = fmaxf(m, l[j]);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    float sum = 0.f;
+    for (int j = lane; j < K; j += 32) sum += expf(l[j] - m);
+    sum = te_warp_sum(sum);
+    for (int j = lane; j < K; j += 32) probs[(long long)r * K + j] = expf(l[j] - m) / sum;
+}
+
 }  // namespace
 
 #define ST(s) reinterpret_cast<cudaStream_t>(s)
@@ -284,6 +302,15 @@ extern "C" int te_logit_stats(const float* logits, const int* target, int rows, 
     const int warps = kThreads / 32;
     logit_stats_kernel<<<(rows + warps - 1) / warps, kThreads, 0, ST(stream)>>>(logits, target, rows, classes, pred, max_logit,
                                                                                  max_prob, dissim);
+    TE_CUDA_CHECK_LAUNCH();
+    return TE_OK;
+}
+
+extern "C" int te_class_probs(const float* logits, int rows, int classes, float* probs, void* stream) {
+    REQ(logits && probs, "te_class_probs: null argument");
+    REQ(rows > 0 && classes >= 1, "te_class_probs: rows > 0 and classes >= 1 expected");
+    const int warps = kThreads / 32;
+    class_probs_kernel<<<(rows + warps - 1) / warps, kThreads, 0, ST(stream)>>>(logits, rows, classes, probs);
     TE_CUDA_CHECK_LAUNCH();
     return TE_OK;
 }

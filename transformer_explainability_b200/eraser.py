@@ -26,9 +26,19 @@ Deviations from the reference (DESIGN.md §1):
  * one annotation per document and split (the pipeline keys its predictions by docid: two annotations of one document would
    merge into one key), and every annotation needs an evidence; otherwise ``ValueError``;
  * soft-token metrics (AUPRC, AP) are not computed.
+
+With ``faithfulness=True`` (CLI ``--faithfulness``) the same pass also measures ``metrics.py``'s faithfulness
+(``score_classifications``, ``:255-364``): per batch one more engine forward gives the original logits, one
+``te_eraser_reduce_inputs`` call builds the comprehensiveness (rationale words removed) and sufficiency (only the rationale
+words kept) rows of every selection size, the rows run through the engine forward in length-sorted chunks, and
+``te_class_probs`` turns each chunk's logits into probabilities on the device.  The selection sizes, the default k and the
+row layout are defined in DESIGN.md §1; the result lines go to ``faithfulness_results.jsonl`` and ``metrics.py``'s
+``classification_scores`` dict to ``faithfulness_scores.json``.
 """
 import argparse
+import functools
 import json
+import math
 import os
 from dataclasses import dataclass
 from typing import FrozenSet, Optional, Tuple, Union
@@ -36,7 +46,10 @@ from typing import FrozenSet, Optional, Tuple, Union
 import numpy as np
 import torch
 
+from . import _lib
+
 KS = tuple(range(5, 85, 5))
+AOPC_THRESHOLDS = (0.01, 0.05, 0.1, 0.2, 0.5)              # metrics.py --aopc_thresholds
 SPECIAL_PIECES = ("[CLS]", "[SEP]", "[UNK]", "[PAD]")
 METHODS = ("transformer_attribution", "partial_lrp", "last_attn", "attn_gradcam", "lrp", "rollout")
 METHOD_FOLDER = {"transformer_attribution": "ours", "partial_lrp": "partial_lrp", "last_attn": "last_attn",
@@ -313,9 +326,133 @@ def hard_scores(truth, docids, counts, orders, thresholds=(0.5,)):
             "token_prf": _prf(truth.token_keys, truth.n_tokens, token_pred, pred_order)}
 
 
+# ---- faithfulness: selection sizes and metrics.py's score_classifications --------------------------------------------------
+def select_count(fraction, W):
+    """The number of words selected at fraction f in (0, 1] of W words: min(W, max(1, floor(f * W + 0.5)))."""
+    return min(W, max(1, int(math.floor(fraction * W + 0.5))))
+
+
+def human_fraction(annotations, docids, word_counts, truth):
+    """The default k fraction: the mean over the split's documents of (words < W covered by a truth span) / W."""
+    fr = []
+    for a, d, W in zip(annotations, docids, word_counts):
+        covered = set(t for s, e in truth.spans_by_key.get((a.annotation_id, d), []) for t in range(s, min(e, W)))
+        fr.append(len(covered) / W if W else 0.0)
+    return sum(fr) / len(fr)
+
+
+def _log_ratio(x, y):
+    """log(x / y) as scipy.special.rel_entr takes it: log1p((x - y) / y) for 0.5 < x / y < 2, else log(x / y)."""
+    r = x / y
+    return math.log1p((x - y) / y) if 0.5 < r < 2 else math.log(r)
+
+
+def _entropy(pk, qk=None):
+    """scipy.stats.entropy of one distribution (or the KL divergence of pk from qk): both normalised, -x log x (0 at 0)
+    or x log(x / y) (0 at x = 0, inf at y = 0 < x) with rel_entr's log, summed with numpy."""
+    pk = np.asarray(pk, dtype=np.float64)
+    pk = pk / np.sum(pk, axis=0, keepdims=True)
+    if qk is None:
+        vec = [x if x != x else -x * math.log(x) if x > 0 else 0.0 if x == 0 else -math.inf for x in pk.tolist()]
+    else:
+        qk = np.asarray(qk, dtype=np.float64)
+        qk = qk / np.sum(qk, axis=0, keepdims=True)
+        vec = [math.nan if x != x or y != y else x * _log_ratio(x, y) if x > 0 and y > 0 else 0.0 if x == 0 and y >= 0
+               else math.inf for x, y in zip(pk.tolist(), qk.tolist())]
+    return np.sum(np.asarray(vec, dtype=np.float64))
+
+
+def _classification_report(truth, pred, names):
+    """sklearn's ``classification_report(truth, pred, output_dict=True, target_names=names)`` for the labels
+    0 .. len(names) - 1, each of which occurs in truth; a zero division gives 0 (sklearn's ``zero_division="warn"``)."""
+    truth, pred = np.asarray(truth), np.asarray(pred)
+    tp = np.array([np.sum((truth == l) & (pred == l)) for l in range(len(names))], dtype=np.int64)
+    n_pred = np.array([np.sum(pred == l) for l in range(len(names))], dtype=np.int64)
+    n_true = np.array([np.sum(truth == l) for l in range(len(names))], dtype=np.int64)
+
+    def div(a, b):
+        a, b = np.asarray(a, dtype=np.float64), np.asarray(b, dtype=np.float64)
+        return np.where(b == 0, 0.0, a / np.where(b == 0, 1.0, b))
+    cols = {"precision": div(tp, n_pred), "recall": div(tp, n_true), "f1-score": div(2.0 * tp, 1.0 * n_true + n_pred)}
+    out = {name: dict({k: float(v[i]) for k, v in cols.items()}, support=float(n_true[i])) for i, name in enumerate(names)}
+    out["accuracy"] = float(div(tp.sum(), n_pred.sum()))
+    out["macro avg"] = dict({k: float(np.average(v)) for k, v in cols.items()}, support=float(np.sum(n_true)))
+    out["weighted avg"] = dict({k: float(np.average(v, weights=n_true)) for k, v in cols.items()},
+                               support=float(np.sum(n_true)))
+    return out
+
+
+def classification_scores_from_probs(annotations, class_names, pred, probs, comp, suff, thresholds, aopc_thresholds):
+    """``metrics.py``'s ``score_classifications`` (``:284-364``) for one result line per annotation, in annotation order:
+    pred [N] predicted class indices, probs [N, C] (``classification_scores``), comp / suff [N, 1 + T, C] (the main k,
+    then one entry per value of ``thresholds``: ``thresholded_scores``), classes in the order of ``class_names``.  The
+    averages and their Python float / numpy arithmetic are the reference's, so the values are its values; ``labels`` is
+    rebuilt as the reference builds it (``list(set(...))``, whose order follows the hash seed)."""
+    probs = np.asarray(probs, dtype=np.float64)
+    comp, suff = np.asarray(comp, dtype=np.float64), np.asarray(suff, dtype=np.float64)
+    labels = list(set(a.classification for a in annotations))
+    label_to_int = {l: i for i, l in enumerate(labels)}
+    truth = [label_to_int[a.classification] for a in annotations]
+    predicted = [label_to_int[class_names[int(p)]] for p in pred]
+    rows = range(len(annotations))
+    beta0 = [float(probs[i, int(pred[i])]) for i in rows]
+    cols = [1 + t for t in sorted(range(len(thresholds)), key=lambda t: thresholds[t]) if thresholds[t] in aopc_thresholds]
+    if len(cols) != len(aopc_thresholds):
+        raise ValueError("every AOPC threshold needs its own thresholded scores")
+    out = {"accuracy": float(np.average(np.asarray(truth) == np.asarray(predicted))),
+           "prf": _classification_report(truth, predicted, labels)}
+    for name, red in (("comprehensiveness", comp), ("sufficiency", suff)):
+        out[name] = np.average([beta0[i] - float(red[i, 0, int(pred[i])]) for i in rows])
+        out[name + "_entropy"] = np.average([_entropy(probs[i].tolist()) - _entropy(red[i, 0].tolist()) for i in rows])
+        out[name + "_kl"] = np.average([_entropy(red[i, 0].tolist(), probs[i].tolist()) for i in rows])
+        points = np.array([[beta0[i] - float(red[i, c, int(pred[i])]) for c in cols] for i in rows])
+        out[name + "_aopc"] = np.average(points)
+        out[name + "_aopc_points"] = np.average(points, axis=0).tolist()
+    out["aopc_thresholds"] = list(aopc_thresholds)
+    return out
+
+
+def faithfulness_lines(annotations, docids, class_names, pred, probs, comp, suff, thresholds, selected):
+    """One ``metrics.py`` result line per annotation (keyed by its own annotation id): the main-k words as
+    ``hard_rationale_predictions``, ``classification``, ``classification_scores``, the main-k comprehensiveness and
+    sufficiency scores and one ``thresholded_scores`` entry per threshold."""
+    def scores(p):
+        return {c: float(v) for c, v in zip(class_names, p)}
+    out = []
+    for i, (a, d) in enumerate(zip(annotations, docids)):
+        out.append(json.dumps({
+            "annotation_id": a.annotation_id,
+            "rationales": [{"docid": d, "hard_rationale_predictions": [{"start_token": int(w), "end_token": int(w) + 1}
+                                                                       for w in selected[i]]}],
+            "classification": class_names[int(pred[i])], "classification_scores": scores(probs[i]),
+            "comprehensiveness_classification_scores": scores(comp[i][0]),
+            "sufficiency_classification_scores": scores(suff[i][0]),
+            "thresholded_scores": [{"threshold": float(t), "comprehensiveness_classification_scores": scores(comp[i][1 + j]),
+                                    "sufficiency_classification_scores": scores(suff[i][1 + j])}
+                                   for j, t in enumerate(thresholds)]}))
+    return out
+
+
+def _generator_model(generator_method):
+    f = generator_method
+    while isinstance(f, functools.partial):
+        f = f.func
+    model = getattr(getattr(f, "__self__", None), "model", None)
+    if model is None or not hasattr(model, "engine"):
+        raise ValueError("faithfulness needs a Generator method bound to a façade BERT model (its engine runs the "
+                         "forwards of the reduced inputs)")
+    return model
+
+
+def _check_fraction(f, what):
+    if not (isinstance(f, float) and 0.0 < f <= 1.0):
+        raise ValueError("%s must lie in (0, 1], got %r" % (what, f))
+
+
 # ---- the evaluation ---------------------------------------------------------------------------------------------------------
 def eraser_eval(generator_method, documents, annotations, encodings, evidence_classes, batch_size=8, ks=KS,
-                iou_thresholds=(0.5,), pad_id=0, device=None, same_length=None):
+                iou_thresholds=(0.5,), pad_id=0, device=None, same_length=None, faithfulness=False,
+                aopc_thresholds=AOPC_THRESHOLDS, k_fraction=None, faith_chunk=None):
     """The test loop of the pipeline (``bert_pipeline.py:456-582``) and ``metrics.py``'s hard scores on the engine.
 
     generator_method: a bound ``Generator`` method (``generate_LRP`` keeps its ``start_layer = 11``), called as
@@ -325,7 +462,15 @@ def eraser_eval(generator_method, documents, annotations, encodings, evidence_cl
     only holds documents of one token length (no padding); it defaults to on for ``generate_attn_gradcam``, whose gradient
     weights and min-max normalisation run over the whole [S, S] map, padded query rows included.
     Returns {"docids": [...], "word_ranges", "order" [docs, max(ks)] (-1 past the last word), "counts" [docs, len(ks),
-    3 + len(iou_thresholds)], "lines" {k: [...]}, "scores" {k: metrics dict}}, all in dataset order."""
+    3 + len(iou_thresholds)], "lines" {k: [...]}, "scores" {k: metrics dict}}, all in dataset order.
+
+    With ``faithfulness`` (the generator must be bound to a façade model, whose engine runs the forwards) the same maps
+    also give ``metrics.py``'s faithfulness at the fractions (k_fraction, *aopc_thresholds) of each document's words
+    (``k_fraction`` defaults to ``human_fraction``); the reduced rows run in length-sorted chunks of at most
+    ``faith_chunk`` rows (default: the engine's ``max_chunk`` at the chunk's length).  The other keys are unchanged, and
+    a key "faithfulness" holds {"fractions", "n_select" [docs, 1 + T], "pred" [docs], "logits" [docs, C], "probs"
+    [docs, C], "comp" / "suff" [docs, 1 + T, C] (fp32 probabilities), "lines", "scores", "real_tokens",
+    "padded_tokens"}."""
     ks = tuple(int(k) for k in ks)
     docids = [annotation_docid(a) for a in annotations]
     if len(set(docids)) != len(docids):
@@ -344,6 +489,30 @@ def eraser_eval(generator_method, documents, annotations, encodings, evidence_cl
     if same_length is None:
         name = getattr(getattr(generator_method, "func", generator_method), "__name__", "")
         same_length = name == "generate_attn_gradcam"
+    ks_run = ks
+    if faithfulness:
+        fracs = [float(f) for f in aopc_thresholds]
+        for f in fracs:
+            _check_fraction(f, "an AOPC threshold")
+        if not fracs:
+            raise ValueError("faithfulness needs at least one AOPC threshold")
+        if k_fraction is None:
+            k_fraction = human_fraction(annotations, docids, [len(ranges[d]) for d in docids], truth)
+        _check_fraction(float(k_fraction), "k_fraction")
+        fracs = [float(k_fraction)] + fracs
+        J = len(fracs)
+        nsel = np.array([[select_count(f, len(ranges[d])) for f in fracs] for d in docids], dtype=np.int64).reshape(n, J)
+        eng = _generator_model(generator_method).engine()
+        names = [c for c, _ in sorted(evidence_classes.items(), key=lambda kv: kv[1])]
+        C = eng.cfg.num_labels
+        # device rows, in the order they are produced: [probs of the originals | of the reduced rows | original logits]
+        buf = torch.empty(n * (1 + 2 * J) + n, C, dtype=torch.float32, device=device)
+        orig_slot = np.zeros(n, dtype=np.int64)
+        red_slot = np.zeros((n, J, 2), dtype=np.int64)
+        n_orig, slot, real_tok, padded_tok = 0, n, 0, 0
+        selected = [None] * n
+        kfull = max(kmax, int(nsel[:, 0].max()) if n else 0)
+        ks_run = ks + ((kfull,) if kfull > kmax else ())
     by_len = sorted(range(n), key=lambda i: len(encodings[docids[i]][0]))
     batches = []
     for i in by_len:
@@ -365,28 +534,80 @@ def eraser_eval(generator_method, documents, annotations, encodings, evidence_cl
             woff.append(len(wr))
             sp.extend(truth.spans_by_key.get((d, d), []))
             soff.append(len(sp))
-        maps = generator_method(input_ids=ids.to(device), attention_mask=mask.to(device),
+        ids_d, mask_d = ids.to(device), mask.to(device)
+        maps = generator_method(input_ids=ids_d, attention_mask=mask_d,
                                 index=torch.as_tensor([targets[i] for i in idx], device=device))
-        res = ops.eraser_rationales(maps.reshape(len(idx), S).to(torch.float32).contiguous(), wr, woff, sp, soff, ks,
-                                    iou_thresholds)
-        host = torch.cat([res["order"].reshape(len(idx), -1), res["counts"].reshape(len(idx), -1)], dim=1).cpu().numpy()
+        maps = maps.reshape(len(idx), S).to(torch.float32).contiguous()
+        res = ops.eraser_rationales(maps, wr, woff, sp, soff, ks_run, iou_thresholds)
+        parts = [res["order"].reshape(len(idx), -1), res["counts"].reshape(len(idx), -1)]
+        if faithfulness:
+            B, o = len(idx), n_orig
+            logits = eng.forward(ids_d, mask_d)
+            buf[n * (1 + 2 * J) + o:n * (1 + 2 * J) + o + B].copy_(logits)
+            ops.class_probs(logits, out=buf[o:o + B])
+            orig_slot[idx] = np.arange(o, o + B)
+            n_orig += B
+            red = ops.eraser_reduce_inputs(maps, ids_d, [len(encodings[docids[i]][0]) for i in idx], wr, woff, nsel[idx])
+            parts.append(red["lengths"].reshape(B, -1).to(parts[0].dtype))
+        host = torch.cat(parts, dim=1).cpu().numpy()
+        kr = ks_run[-1]
         order[idx] = host[:, :kmax]
-        counts[idx] = host[:, kmax:].reshape(len(idx), len(ks), ncol)
+        counts[idx] = host[:, kr:kr + len(ks) * ncol].reshape(len(idx), len(ks), ncol)
+        if faithfulness:
+            for r, i in enumerate(idx):
+                selected[i] = host[r, :nsel[i, 0]].tolist()
+            lens = host[:, kr + len(ks_run) * ncol:].reshape(-1)          # [B * J * 2], rows (document, selection, kind)
+            rows = sorted(range(len(lens)), key=lambda q: -int(lens[q]))  # longest first: each chunk's first row sets S
+            flat = red["ids"].reshape(len(lens), S)
+            s0 = 0
+            while s0 < len(rows):
+                L = int(lens[rows[s0]])
+                chunk = rows[s0:s0 + (faith_chunk or eng.max_chunk(L))]
+                sel = torch.as_tensor(chunk, device=device)
+                x = flat.index_select(0, sel)[:, :L].contiguous()
+                m = (torch.arange(L, device=device)[None, :] <
+                     torch.as_tensor(lens[chunk], device=device)[:, None]).to(torch.int64)
+                ops.class_probs(eng.forward(x, m), out=buf[slot:slot + len(chunk)])
+                for q_i, q in enumerate(chunk):
+                    r, rest = divmod(q, 2 * J)
+                    red_slot[idx[r], rest // 2, rest % 2] = slot + q_i
+                slot += len(chunk)
+                real_tok += int(lens[chunk].sum())
+                padded_tok += len(chunk) * L
+                s0 += len(chunk)
     lines = rationale_lines(docids, ks=ks, order=order)
     scores = {k: hard_scores(truth, docids, counts[:, i], order, iou_thresholds) for i, k in enumerate(ks)}
-    return {"docids": docids, "word_ranges": [ranges[d] for d in docids], "order": order, "counts": counts,
-            "lines": lines, "scores": scores}
+    out = {"docids": docids, "word_ranges": [ranges[d] for d in docids], "order": order, "counts": counts,
+           "lines": lines, "scores": scores}
+    if faithfulness:
+        allp = buf.cpu().numpy()
+        logits = allp[n * (1 + 2 * J) + orig_slot]
+        pred = np.argmax(logits, axis=1)                                # the first maximum
+        probs, comp, suff = allp[orig_slot], allp[red_slot[:, :, 0]], allp[red_slot[:, :, 1]]
+        thr = fracs[1:]
+        out["faithfulness"] = {
+            "fractions": fracs, "n_select": nsel, "pred": pred, "logits": logits, "probs": probs, "comp": comp,
+            "suff": suff, "lines": faithfulness_lines(annotations, docids, names, pred, probs, comp, suff, thr, selected),
+            "scores": classification_scores_from_probs(annotations, names, pred, probs, comp, suff, thr, thr),
+            "real_tokens": real_tok, "padded_tokens": padded_tok}
+    return out
 
 
 def write_results(results, folder):
     """``identifier_results_{k}.json`` (the pipeline's files) and ``scores_{k}.json`` (``metrics.py``'s ``--score_file``
-    layout: indent 4, sorted keys) under ``folder``."""
+    layout: indent 4, sorted keys) under ``folder``; with faithfulness results also ``faithfulness_results.jsonl``
+    (``metrics.py``'s results format) and ``faithfulness_scores.json`` (its ``classification_scores`` dict)."""
     os.makedirs(folder, exist_ok=True)
     for k, lines in results["lines"].items():
         with open(os.path.join(folder, "identifier_results_%d.json" % k), "w") as f:
             f.write("".join(line + "\n" for line in lines))
         with open(os.path.join(folder, "scores_%d.json" % k), "w") as f:
             json.dump(results["scores"][k], f, indent=4, sort_keys=True)
+    if "faithfulness" in results:
+        with open(os.path.join(folder, "faithfulness_results.jsonl"), "w") as f:
+            f.write("".join(line + "\n" for line in results["faithfulness"]["lines"]))
+        with open(os.path.join(folder, "faithfulness_scores.json"), "w") as f:
+            json.dump(results["faithfulness"]["scores"], f, indent=4, sort_keys=True)
 
 
 # ---- command line ---------------------------------------------------------------------------------------------------------
@@ -402,6 +623,13 @@ def build_parser():
                    help="classifier weights (default: output_dir/classifier/classifier.pt, where the pipeline saves them)")
     p.add_argument("--batch-size", dest="batch_size", type=int, default=8)
     p.add_argument("--iou-thresholds", dest="iou_thresholds", type=float, nargs="+", default=[0.5])
+    p.add_argument("--faithfulness", action="store_true",
+                   help="also measure comprehensiveness, sufficiency and their AOPC (metrics.py score_classifications)")
+    p.add_argument("--aopc-thresholds", dest="aopc_thresholds", type=float, nargs="+", default=list(AOPC_THRESHOLDS),
+                   help="fractions of each document's words for the AOPC bins (metrics.py --aopc_thresholds)")
+    p.add_argument("--k-fraction", dest="k_fraction", type=float, default=None,
+                   help="fraction of words removed / kept for the main comprehensiveness and sufficiency (default: the "
+                        "split's mean fraction of words inside a human rationale)")
     return p
 
 
@@ -412,6 +640,12 @@ def parse_args(argv=None):
         p.error("--batch-size must be at least 1")
     if not 1 <= len(args.iou_thresholds) <= 8:
         p.error("--iou-thresholds takes 1 to 8 values")
+    if not 1 <= len(args.aopc_thresholds) < _lib.ERASER_MAX_SELECTIONS:
+        p.error("--aopc-thresholds takes 1 to %d values" % (_lib.ERASER_MAX_SELECTIONS - 1))
+    if any(not 0.0 < f <= 1.0 for f in args.aopc_thresholds) or len(set(args.aopc_thresholds)) != len(args.aopc_thresholds):
+        p.error("--aopc-thresholds takes distinct fractions in (0, 1]")
+    if args.k_fraction is not None and not 0.0 < args.k_fraction <= 1.0:
+        p.error("--k-fraction must lie in (0, 1]")
     if args.state_dict is None:
         args.state_dict = os.path.join(args.output_dir, "classifier", "classifier.pt")
     return args
@@ -451,11 +685,18 @@ def main(argv=None):
     evidence_classes = {c: i for i, c in enumerate(classes)}
     gen = build_generator(args.method, params["bert_dir"], len(classes), args.state_dict)
     res = eraser_eval(gen, documents, annotations, encodings, evidence_classes, batch_size=args.batch_size,
-                      iou_thresholds=args.iou_thresholds)
+                      iou_thresholds=args.iou_thresholds, faithfulness=args.faithfulness,
+                      aopc_thresholds=args.aopc_thresholds, k_fraction=args.k_fraction)
     write_results(res, os.path.join(args.output_dir, METHOD_FOLDER[args.method]))
     for k in KS:
         print("top-%d token F1 %.4f (instance macro %.4f)" % (k, res["scores"][k]["token_prf"]["instance_micro"]["f1"],
                                                               res["scores"][k]["token_prf"]["instance_macro"]["f1"]))
+    if args.faithfulness:
+        f = res["faithfulness"]["scores"]
+        print("k fraction %.4f: comprehensiveness %.4f, sufficiency %.4f" % (res["faithfulness"]["fractions"][0],
+                                                                            f["comprehensiveness"], f["sufficiency"]))
+        print("AOPC over %s: comprehensiveness %.4f, sufficiency %.4f" % (f["aopc_thresholds"], f["comprehensiveness_aopc"],
+                                                                         f["sufficiency_aopc"]))
     return res
 
 

@@ -529,6 +529,22 @@ def logit_stats(logits, target):
     return pred, max_logit, max_prob, dissim
 
 
+@_on_device
+def class_probs(logits, out=None):
+    """The fp32 softmax of each row of logits [R, K] (see include/te_b200.h: te_class_probs); ``out`` [R, K] fp32 may be
+    given (a view into a larger buffer, contiguous)."""
+    _req(logits)
+    if logits.dim() != 2 or logits.shape[0] == 0:
+        raise ValueError("class_probs: logits [R, K] with R > 0 expected")
+    out = torch.empty_like(logits) if out is None else out
+    _req(out)
+    if out.shape != logits.shape or out.device != logits.device:
+        raise ValueError("class_probs: out must be [R, K] on the logits' device")
+    R, K = logits.shape
+    check(_lib.load().te_class_probs(ptr(logits), R, K, ptr(out), _stream()), "te_class_probs")
+    return out
+
+
 # ---- segmentation evaluation (baselines/ViT/imagenet_seg_eval.py) ----------------------------------------------------------
 def _req_u32(t, what):
     if not (t.is_cuda and t.dtype in (torch.int32, torch.uint32) and t.is_contiguous()):
@@ -608,11 +624,11 @@ def pr_curve(sorted_keys):
 
 
 # ---- ERASER rationale evaluation (BERT_rationale_benchmark/models/pipeline/bert_pipeline.py, metrics.py) ---------------------
-def _host_i32(a, what, cols=None):
+def _host_i32(a, what, cols=None, op="eraser_rationales"):
     import numpy as np
     a = np.ascontiguousarray(np.asarray(a, dtype=np.int64).reshape(-1, cols) if cols else np.asarray(a, dtype=np.int64))
     if a.size and (a.min() < -2 ** 31 or a.max() >= 2 ** 31):
-        raise ValueError("eraser_rationales: %s outside the int32 range" % what)
+        raise ValueError("%s: %s outside the int32 range" % (op, what))
     return np.ascontiguousarray(a.astype(np.int32))
 
 
@@ -656,4 +672,43 @@ def eraser_rationales(maps, piece_ranges, word_offsets, spans, span_offsets, ks,
                                    len(thr), ptr(out["word_scores"]) if len(ranges) else None,
                                    ptr(out["order"]) if max(ks) > 0 else None, ptr(out["counts"]), ptr(ws), ws.numel() * 4,
                                    _stream()), "te_eraser_rationales")
+    return out
+
+
+@_on_device
+def eraser_reduce_inputs(maps, input_ids, lengths, piece_ranges, word_offsets, n_select):
+    """The comprehensiveness and sufficiency rows of each document b of maps [B, S] (fp32 CUDA) and input_ids [B, S]
+    (int64 CUDA) for each selection size ``n_select[b][j]`` (host [B, J], 0 <= n <= W): the words are ranked as
+    ``eraser_rationales`` ranks them; the sufficiency row is [CLS], the inner pieces held by a word of the first n ranks,
+    [SEP]; the comprehensiveness row is [CLS], the other inner pieces, [SEP] (see include/te_b200.h:
+    te_eraser_reduce_inputs).  lengths [B], the ranges and offsets are host sequences.  Returns a dict of CUDA tensors:
+    ``ids`` int64 [B, J, 2, S] (comprehensiveness, sufficiency; zero past each length), ``lengths`` int32 [B, J, 2]."""
+    _req(maps)
+    if maps.dim() != 2:
+        raise ValueError("eraser_reduce_inputs: maps [B, S] expected")
+    B, S = maps.shape
+    if not (input_ids.is_cuda and input_ids.dtype == torch.int64 and input_ids.is_contiguous()) or \
+            input_ids.shape != maps.shape or input_ids.device != maps.device:
+        raise ValueError("eraser_reduce_inputs: input_ids int64 [B, S] contiguous on the maps' device expected")
+    op = "eraser_reduce_inputs"
+    lens = _host_i32(lengths, "lengths", op=op)
+    woff = _host_i32(word_offsets, "word_offsets", op=op)
+    nsel = _host_i32(n_select, "n_select", op=op)
+    if lens.shape != (B,) or woff.shape != (B + 1,):
+        raise ValueError("eraser_reduce_inputs: lengths need B = %d and word_offsets B + 1 entries" % B)
+    if nsel.ndim != 2 or nsel.shape[0] != B or not 0 < nsel.shape[1] <= _lib.ERASER_MAX_SELECTIONS:
+        raise ValueError("eraser_reduce_inputs: n_select [B, J] with 1 <= J <= %d expected" % _lib.ERASER_MAX_SELECTIONS)
+    ranges = _host_i32(piece_ranges, "piece_ranges", 2, op=op)
+    if len(ranges) != int(woff[-1]):
+        raise ValueError("eraser_reduce_inputs: %d piece ranges, the offsets end at %d" % (len(ranges), woff[-1]))
+    J = nsel.shape[1]
+    lib = _lib.load()
+    ws = _workspace(check(lib.te_eraser_reduce_workspace_bytes(B, len(ranges), J), "te_eraser_reduce_workspace_bytes"),
+                    maps.device)
+    out = {"ids": torch.empty(B, J, 2, S, device=maps.device, dtype=torch.int64),
+           "lengths": torch.empty(B, J, 2, device=maps.device, dtype=torch.int32)}
+    host = lambda a: a.ctypes.data_as(_lib.c_void_p) if a.size else None      # noqa: E731
+    check(lib.te_eraser_reduce_inputs(ptr(maps), ptr(input_ids), B, S, host(lens), host(woff), host(ranges), host(nsel), J,
+                                      ptr(out["ids"]), ptr(out["lengths"]), ptr(ws), ws.numel() * 4, _stream()),
+          "te_eraser_reduce_inputs")
     return out
