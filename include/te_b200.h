@@ -134,19 +134,17 @@ TE_API int te_vit_forward(const te_vit_config* cfg, const float* weights, const 
  * method="transformer_attribution" (ViT_LRP.py:324-369) on the activations te_vit_forward left behind:
  * arg-max (where index[b] < 0), one-hot, class gradient of every attention map, LRP relprop through
  * every block >= start_layer, relu(grad*cam) head-mean, +I, rollout, row 0 without the prefix token(s).
- * index [batch] int32 in/out (device); maps [batch, tokens-prefix] (device). */
-TE_API int te_vit_attribute(const te_vit_config* cfg, const float* weights, const float* derived, int batch, int* index,
-                     int start_layer, unsigned flags, float* maps, void* workspace, long long workspace_bytes,
-                     void* stream);
-/* Same with model.relprop(cam, alpha=alpha) (ViT_LRP.py:324, any method): every Linear.relprop of the rule library applies
+ * index [batch] int32 in/out (device); maps [batch, tokens-prefix] (device).
+ * alpha: model.relprop(cam, alpha=alpha) (ViT_LRP.py:324, any method): every Linear.relprop of the rule library applies
  * the LRP-alpha-beta rule with beta = alpha - 1 (layers_ours.py:207-230, layers_lrp.py:187-210), R_in = alpha * act -
- * beta * inh, the inhibitor half running after the activator through the same scratch (the workspace size is unchanged).
- * alpha = 1 is exactly te_vit_attribute.  The other rules do not depend on alpha.  A non-finite alpha returns TE_ERR_ARG. */
-TE_API int te_vit_attribute_alpha(const te_vit_config* cfg, const float* weights, const float* derived, int batch, int* index,
-                                  int start_layer, float alpha, unsigned flags, float* maps, void* workspace,
-                                  long long workspace_bytes, void* stream);
+ * beta * inh, the inhibitor half running after the activator through the same scratch (the workspace size does not depend
+ * on alpha).  alpha = 1 is the z+ rule every generator uses.  The other rules do not depend on alpha.  A non-finite alpha
+ * returns TE_ERR_ARG. */
+TE_API int te_vit_attribute(const te_vit_config* cfg, const float* weights, const float* derived, int batch, int* index,
+                            int start_layer, float alpha, unsigned flags, float* maps, void* workspace,
+                            long long workspace_bytes, void* stream);
 
-/* te_vit_forward + te_vit_attribute: one call per batch = LRP.generate_LRP for `batch` independent inputs. */
+/* te_vit_forward + te_vit_attribute (alpha = 1): one call per batch = LRP.generate_LRP for `batch` independent inputs. */
 TE_API int te_vit_explain(const te_vit_config* cfg, const float* weights, const float* derived, const float* images,
                    int batch, int* index, int start_layer, unsigned flags, float* maps, float* logits, void* workspace,
                    long long workspace_bytes, void* stream);
@@ -166,16 +164,13 @@ TE_API int te_vit_tensor(const te_vit_config* cfg, int batch, void* workspace, c
 /* method="full" (ViT_LRP.py:337-343): relevance carried through ``self.add`` (tokens + pos_embed), ``[:, 1:]``,
  * PatchEmbed.relprop (:238-242) and the z^B rule of the patch convolution (layers_ours.py:242-259).
  * Call after te_vit_forward + te_vit_attribute(flags | TE_FLAG_RELPROP_TO_INPUT) on the same workspace and images.
+ * flags: those of that te_vit_attribute call; TE_FLAG_RULES_LRP selects the layers_lrp Add rule for self.add.relprop
+ * (baselines/ViT/ViT_orig_LRP.py, method="full").
  * pixel_maps [batch, img, img] (channels summed — what relprop returns) and / or pixel_relevance
  * [batch, in_chans, img, img] (Conv2d.relprop's own output) are written when non-NULL. */
 TE_API int te_vit_relprop_pixels(const te_vit_config* cfg, const float* weights, const float* images, int batch,
-                          float* pixel_maps, float* pixel_relevance, void* workspace, long long workspace_bytes,
-                          void* stream);
-/* Same with the engine flags of the preceding te_vit_attribute call: TE_FLAG_RULES_LRP selects the layers_lrp Add rule for
- * self.add.relprop (baselines/ViT/ViT_orig_LRP.py, method="full"). */
-TE_API int te_vit_relprop_pixels_ex(const te_vit_config* cfg, const float* weights, const float* images, int batch,
-                                    unsigned flags, float* pixel_maps, float* pixel_relevance, void* workspace,
-                                    long long workspace_bytes, void* stream);
+                                 unsigned flags, float* pixel_maps, float* pixel_relevance, void* workspace,
+                                 long long workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * BERT sequence classifier  (BERT_explainability/modules/BERT/BertForSequenceClassification.py:12-88,
@@ -212,15 +207,12 @@ TE_API int te_bert_forward(const te_bert_config* cfg, const float* weights, cons
 /* The rest of Generator.generate_LRP (ExplanationGenerator.py:33-59): arg-max (index[b] < 0), one-hot, class
  * gradient of every attention_probs, relprop (BertForSequenceClassification.relprop), relu(grad*cam) head mean,
  * +I, row-normalised rollout from start_layer, row 0 with element 0 replaced by the row minimum.
- * maps [batch, seq]. */
+ * maps [batch, seq].  alpha: model.relprop(cam, alpha=alpha) (BertForSequenceClassification.py:83-88), the LRP-alpha-beta
+ * Linear rule as for te_vit_attribute; a non-finite alpha returns TE_ERR_ARG. */
 TE_API int te_bert_attribute(const te_bert_config* cfg, const float* weights, const float* derived, int batch, int seq,
-                      int* index, int start_layer, unsigned flags, float* maps, void* workspace,
-                      long long workspace_bytes, void* stream);
-/* Same with model.relprop(cam, alpha=alpha) (BertForSequenceClassification.py:83-88): the LRP-alpha-beta Linear rule as for
- * te_vit_attribute_alpha.  alpha = 1 is exactly te_bert_attribute; a non-finite alpha returns TE_ERR_ARG. */
-TE_API int te_bert_attribute_alpha(const te_bert_config* cfg, const float* weights, const float* derived, int batch, int seq,
-                                   int* index, int start_layer, float alpha, unsigned flags, float* maps, void* workspace,
-                                   long long workspace_bytes, void* stream);
+                             int* index, int start_layer, float alpha, unsigned flags, float* maps, void* workspace,
+                             long long workspace_bytes, void* stream);
+/* te_bert_forward + te_bert_attribute (alpha = 1). */
 TE_API int te_bert_explain(const te_bert_config* cfg, const float* weights, const float* derived,
                     const long long* input_ids, const long long* attention_mask, int batch, int seq, int* index,
                     int start_layer, unsigned flags, float* maps, float* logits, void* workspace,
@@ -239,29 +231,23 @@ TE_API int te_bert_tensor(const te_bert_config* cfg, int batch, int seq, void* w
  * Stand-alone LRP rules (modules/layers_ours.py) — the same kernels the engine chains, exported so
  * that each rule can be parity-tested against the reference layer class it replaces.
  * ---------------------------------------------------------------------------------------------- */
-/* Linear.relprop, alpha=1 (layers_ours.py:207-230): x [rows,in], w [out,in], r [rows,out] -> out [rows,in].
- * flags & TE_FLAG_RULES_LRP: the layers_lrp variant (modules/layers_lrp.py:187-210, separate denominators), on the
- * tensor cores with TE_FLAG_RULES_LRP_TC as well (in, out multiples of 128; other shapes run the fp32 SIMT rule).
+/* Linear.relprop(R, alpha) (layers_ours.py:207-230): x [rows,in], w [out,in], r [rows,out] -> out [rows,in].
+ * alpha: the LRP-alpha-beta rule for any finite alpha, beta = alpha - 1, R_in = alpha * act - beta * inh; inh is act with the
+ * weight signs swapped: x+ * (S_i W-) + x- * (S_i W+) with S_i = sd(R, x+ W-^T + x- W+^T).  alpha = 1 is the z+ rule; a
+ * non-finite alpha returns TE_ERR_ARG.
+ * y / bias: the Linear's saved forward output y = x W^T + bias [rows,out] (what the engines do; bias may be NULL, no bias),
+ * or y = NULL.  With y and TE_FLAG_ZPLUS_TENSOR_CORES the denominator is formed in ONE tensor-core pass through the exact
+ * identity x+ W+^T + x- W-^T == ((y - bias) + |x| |W|^T) / 2, and the variant flags TE_FLAG_ZPLUS_BF16, _S1_BF16 and _R_F16
+ * apply; without y the denominator takes two passes and those flags are not read.
+ * flags & TE_FLAG_RULES_LRP: the layers_lrp variant (modules/layers_lrp.py:187-210, separate denominators: each of the
+ * four products over its own), which does not read y / bias; on the tensor cores with TE_FLAG_RULES_LRP_TC as well (in, out
+ * multiples of 128; other shapes run the fp32 SIMT rule).
  * scratch: rows*out floats; with TE_FLAG_ZPLUS_TENSOR_CORES (layers_ours) or TE_FLAG_RULES_LRP | TE_FLAG_RULES_LRP_TC:
- * round_up(rows*out,64) + 16*in*out floats. */
-TE_API int te_linear_relprop(const float* x, const float* w, const float* r, float* out, float* scratch, int rows,
-                      int in_features, int out_features, unsigned flags, void* stream);
-/* Same rule with the Linear's saved forward output y = x W^T + bias [rows,out] supplied (what the engines do): with
- * TE_FLAG_ZPLUS_TENSOR_CORES the denominator is then formed in ONE tensor-core pass through the exact identity
- * x+ W+^T + x- W-^T == ((y - bias) + |x| |W|^T) / 2.  bias may be NULL (no bias).
- * scratch: rows*out floats; with TE_FLAG_ZPLUS_TENSOR_CORES: round_up(rows*out,64) + 16*in*out + rows*in floats
- * (S, the derived weight copies, the tf32(|x|) operand of the single-pass kernel). */
-TE_API int te_linear_relprop_ex(const float* x, const float* w, const float* bias, const float* y, const float* r,
-                         float* out, float* scratch, int rows, int in_features, int out_features, unsigned flags,
-                         void* stream);
-/* Linear.relprop(R, alpha) for any finite alpha: the LRP-alpha-beta rule, beta = alpha - 1, R_in = alpha * act - beta * inh
- * (layers_ours.py:207-230; with TE_FLAG_RULES_LRP layers_lrp.py:187-210).  inh is act with the weight signs swapped:
- * x+ * (S_i W-) + x- * (S_i W+) with S_i = sd(R, x+ W-^T + x- W+^T) (layers_lrp: each of the four products over its own
- * denominator).  y == NULL: te_linear_relprop (bias ignored); y != NULL: te_linear_relprop_ex.  Scratch sizes as there.
- * alpha = 1 is exactly those entries; a non-finite alpha returns TE_ERR_ARG. */
-TE_API int te_linear_relprop_alpha(const float* x, const float* w, const float* bias, const float* y, const float* r,
-                                   float* out, float* scratch, int rows, int in_features, int out_features, float alpha,
-                                   unsigned flags, void* stream);
+ * round_up(rows*out,64) + 16*in*out floats (S, the derived weight copies), + rows*in floats with y (the tf32(|x|) operand of
+ * the single-pass kernel). */
+TE_API int te_linear_relprop(const float* x, const float* w, const float* bias, const float* y, const float* r, float* out,
+                             float* scratch, int rows, int in_features, int out_features, float alpha, unsigned flags,
+                             void* stream);
 /* Add.relprop (layers_ours.py:97-120) per sample: x1,x2,r [batch,per_sample] -> r1,r2.
  * scratch: batch*48 doubles; scratch == NULL selects the layers_lrp variant (modules/layers_lrp.py:48-60,98-100:
  * r1 = x1*sd(r, x1+x2), r2 = x2*sd(r, x1+x2), no ratio normalisation). */
@@ -316,37 +302,29 @@ TE_API int te_attribution_rollout(const float* grad, const float* cam, int layer
 TE_API int te_compute_rollout_attention(const float* mats, int layers, int batch, int n, int start_layer, int normalize,
                                  float* joint, void* workspace, long long workspace_bytes, void* stream);
 
-/* Plain Linear GEMMs — exported for kernel unit tests only.  flags & TE_FLAG_LINEAR_TENSOR_CORES selects the
- * wgmma 3xTF32 path (scratch: 16*in*out floats for the derived weight copies; may be NULL otherwise); with
- * TE_FLAG_LINEAR_F16_SPLIT as well, te_linear_forward_ex runs the fp16-split kernel (scratch: 16*in*out +
- * round_up(rows*in,64) + rows*ceil(in/128) floats).  te_linear_backward_ex with TE_FLAG_BACKWARD_F16 as well: scratch
- * 16*in*out + round_up(rows*out/2,64) + rows*ceil(out/128) floats. */
-TE_API int te_linear_forward(const float* x, const float* w, const float* bias, float* y, int rows, int in_features,
-                      int out_features, void* stream);
-TE_API int te_linear_forward_ex(const float* x, const float* w, const float* bias, float* y, float* scratch, int rows,
-                         int in_features, int out_features, unsigned flags, void* stream);
 /* The operand format of the fp16-split forward Linear (TE_FLAG_LINEAR_F16_SPLIT) — exported for unit tests of the format: x [rows, cols]
  * -> hi, lo fp16 [rows, cols] (hi = fp16(2^e x), lo = fp16(2^e x - hi)) and scale_inv [rows, ceil(cols / 128)] = 2^-e, one e per row
  * and 128 columns chosen so that 2^e max|x| lies in [2^14, 2^15) (e = 0 for an all-zero or non-finite block).  cols % 4 == 0. */
 TE_API int te_f16_block_split(const float* x, int rows, int cols, void* hi, void* lo, float* scale_inv, void* stream);
-TE_API int te_linear_backward_ex(const float* dy, const float* w, float* dx, float* scratch, int rows, int in_features,
-                          int out_features, unsigned flags, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Diagnostic entry points — exported for kernel unit tests only.  Each runs the named tensor-core kernel (or kernel family)
  * directly: a shape or epilogue that kernel does not take returns TE_ERR_UNSUPPORTED with a te_last_error() message, never a
  * fall-back to another kernel, so a call that succeeds has run the kernel it asked for.
  * ---------------------------------------------------------------------------------------------- */
-/* Linear GEMMs with their fused epilogues, through the engines' own kernel selection.  epi: 0 STORE (y = x W^T), 1 BIAS (+ bias),
- * 2 BIAS_GELU (y2 = erf-GELU(y) as well), 3 BIAS_ADD (y2 = e0 + y as well); backward 0 STORE (dx = dy W), 4 GELU_BWD
- * (dx = (dy W) * GELU'(e0)).  e0 / y2 share the row stride of y (dx).  flags select the family: 0 fp32 SIMT;
- * TE_FLAG_LINEAR_TENSOR_CORES 3xTF32; + TE_FLAG_LINEAR_F16_SPLIT (forward) fp16 split; + TE_FLAG_BACKWARD_TF32 / TE_FLAG_BACKWARD_F16
- * (backward) single-pass TF32 / fp16.  scratch as for te_linear_forward_ex / te_linear_backward_ex. */
-TE_API int te_linear_forward_epi(const float* x, const float* w, const float* bias, const float* e0, float* y, float* y2,
-                                 float* scratch, int rows, int in_features, int out_features, int epi, unsigned flags,
-                                 void* stream);
-TE_API int te_linear_backward_epi(const float* dy, const float* w, const float* e0, float* dx, float* scratch, int rows,
-                                  int in_features, int out_features, int epi, unsigned flags, void* stream);
+/* Linear GEMMs with their fused epilogues, through the engines' own kernel selection: forward y = x W^T, x [rows,in],
+ * w [out,in]; backward dx = dy W, dy [rows,out].  epi: 0 STORE (y = x W^T), 1 BIAS (+ bias), 2 BIAS_GELU (y2 = erf-GELU(y)
+ * as well), 3 BIAS_ADD (y2 = e0 + y as well); backward 0 STORE (dx = dy W), 4 GELU_BWD (dx = (dy W) * GELU'(e0)).  e0 / y2
+ * share the row stride of y (dx).  flags select the family: 0 fp32 SIMT; TE_FLAG_LINEAR_TENSOR_CORES 3xTF32;
+ * + TE_FLAG_LINEAR_F16_SPLIT (forward) fp16 split; + TE_FLAG_BACKWARD_TF32 / TE_FLAG_BACKWARD_F16 (backward) single-pass
+ * TF32 / fp16.  scratch (may be NULL for SIMT): 16*in*out floats for the derived weight copies; with the fp16 split
+ * + round_up(rows*in,64) + rows*ceil(in/128) floats; with TE_FLAG_BACKWARD_F16 + round_up(rows*out/2,64) + rows*ceil(out/128)
+ * floats. */
+TE_API int te_linear_forward(const float* x, const float* w, const float* bias, const float* e0, float* y, float* y2,
+                             float* scratch, int rows, int in_features, int out_features, int epi, unsigned flags,
+                             void* stream);
+TE_API int te_linear_backward(const float* dy, const float* w, const float* e0, float* dx, float* scratch, int rows,
+                              int in_features, int out_features, int epi, unsigned flags, void* stream);
 /* LayerNorm over the last dimension of x [rows, D] (D % 4 == 0) that also emits the fp16-split operand of y in the format of
  * te_f16_block_split: y [rows, D], mean / rstd [rows] (each may be NULL), hi, lo fp16 [rows, D] with lo == hi + rows*D,
  * scale_inv [rows, ceil(D / 128)]. */

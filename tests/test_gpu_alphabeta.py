@@ -7,16 +7,12 @@
   tests/test_gpu_tc.py), the layers_lrp rule on SIMT 1e-5 and on TF32 tensor cores 3e-3.
 - Conservation per row: sum R_in = sum R for layers_ours at every alpha (alpha - beta = 1); the layers_lrp row sums equal
   its alpha = 1 row sums.
-- alpha = 1 through the new entries is bit-identical to the old entries (every rule path; the ViT-B- and BERT-width
-  engines at flags 0 and 7475).
 - Engines at alpha = 2 against the fp64 oracle on the conditioned 3-block models of tests/test_gpu_methods_tc.py (its
   builders, FLAG_SETS, tol() and regime gate): every ViT method that reads the relprop, DeiT-distilled, ViT_orig_LRP
   (layers_lrp on SIMT and on tensor cores), BERT and BERT_cls_lrp relevance_in and attn_cam taps.
 - The facades: Linear.relprop(R, alpha) of both libraries is ops.linear_relprop(alpha=...), model.relprop(alpha=2) is the
   engine's attribute(alpha=2), the alpha-independent rules ignore alpha, a NaN alpha raises.
 """
-import ctypes
-
 import pytest
 import torch
 
@@ -116,69 +112,6 @@ def test_non_finite_alpha_raises():
         for bad in (float("nan"), float("inf")):
             with pytest.raises(_lib.TeError):
                 ops.linear_relprop(xd, wd, rd, alpha=bad, **kw)
-
-
-# ---- alpha = 1 through the new entries == the old entries -------------------------------------------------------------
-def test_alpha_one_is_bit_identical_to_the_old_entries():
-    lib = _lib.load()
-    st = ops._stream()
-    for rows, inf, outf in VIT_SHAPES[:2] + SIMT_SHAPES[:1]:
-        x, w, b, r = (t.cuda() for t in _inputs(rows, inf, outf, 9))
-        y = ops.linear_forward(x, w, b)
-        scratch = ops._tc_scratch(w, x.device, s=rows * outf, operand=x.numel())
-        for flags in (0, _lib.FLAG_ZPLUS_TENSOR_CORES, _lib.FLAG_ZPLUS_TENSOR_CORES | _lib.FLAG_ZPLUS_BF16,
-                      _lib.FLAG_ZPLUS_TENSOR_CORES | _lib.FLAG_ZPLUS_S1_BF16,
-                      _lib.FLAG_ZPLUS_TENSOR_CORES | _lib.FLAG_ZPLUS_S1_BF16 | _lib.FLAG_ZPLUS_R_F16,
-                      _lib.FLAG_RULES_LRP, _lib.FLAG_RULES_LRP | _lib.FLAG_RULES_LRP_TC):
-            old, new = torch.empty_like(x), torch.empty_like(x)
-            P = _lib.ptr
-            _lib.check(lib.te_linear_relprop(P(x), P(w), P(r), P(old), P(scratch), rows, inf, outf, flags, st))
-            _lib.check(lib.te_linear_relprop_alpha(P(x), P(w), None, None, P(r), P(new), P(scratch), rows, inf, outf, 1.0,
-                                                   flags, st))
-            assert torch.equal(old, new), ("plain", flags)
-            if flags & _lib.FLAG_RULES_LRP:
-                continue
-            _lib.check(lib.te_linear_relprop_ex(P(x), P(w), P(b), P(y), P(r), P(old), P(scratch), rows, inf, outf, flags, st))
-            _lib.check(lib.te_linear_relprop_alpha(P(x), P(w), P(b), P(y), P(r), P(new), P(scratch), rows, inf, outf, 1.0,
-                                                   flags, st))
-            assert torch.equal(old, new), ("ex", flags)
-
-
-def _old_vit_attribute(eng, flags):
-    b = eng.last_batch
-    ws = eng._workspace(b)
-    idx = torch.full((b,), -1, dtype=torch.int32, device=eng.device)
-    maps = torch.empty(b, eng.tokens - eng.prefix, dtype=torch.float32, device=eng.device)
-    _lib.check(eng.lib.te_vit_attribute(ctypes.byref(eng.cfg), _lib.ptr(eng.weights), _lib.ptr(eng._derived(flags)), b,
-                                        _lib.ptr(idx), 0, flags, _lib.ptr(maps), _lib.ptr(ws), ws.numel() * 4, eng._stream()))
-    return maps
-
-
-def test_engines_alpha_one_bit_identical(vit_b, bert_b):
-    for flags in (0, _lib.FLAG_BENCH_DEFAULT):
-        model = mtc._vit_model(vit_b)
-        model.engine_flags = flags
-        x = vit_b["x"].cuda()
-        model(x)
-        eng = model.engine()
-        fl = flags | _lib.FLAG_RELPROP_TO_INPUT
-        old = _old_vit_attribute(eng, fl)
-        new, _ = eng.attribute(flags=fl, alpha=1.0)
-        assert torch.equal(old, new), flags
-        bm = _bert_model(bert_b, "ours")
-        bm.engine_flags = flags
-        ids, mask = bert_b["ids"].cuda(), bert_b["mask"].cuda()
-        bm(ids, mask)
-        be = bm.engine()
-        b, s = be.last
-        ws = be._workspace(b, s)
-        idx = torch.full((b,), -1, dtype=torch.int32, device=be.device)
-        maps = torch.empty(b, s, dtype=torch.float32, device=be.device)
-        _lib.check(be.lib.te_bert_attribute(ctypes.byref(be.cfg), _lib.ptr(be.weights), _lib.ptr(be._derived(fl)), b, s,
-                                            _lib.ptr(idx), 0, fl, _lib.ptr(maps), _lib.ptr(ws), ws.numel() * 4, be._stream()))
-        r_old = be.tensor("relevance_in").clone()
-        new, _ = be.attribute(start_layer=0, flags=fl, alpha=1.0)
-        assert torch.equal(maps, new) and torch.equal(r_old, be.tensor("relevance_in")), flags
 
 
 # ---- engines at alpha = 2 against fp64 -----------------------------------------------------------------------------------

@@ -335,7 +335,7 @@ def test_f16_block_split_format_bit_exact():
     assert np.array_equal(lo.cpu().numpy().view(np.uint16)[ok], rl.view(np.uint16)[ok])
 
 
-# ---- fused Linear epilogues of every kernel family (te_linear_forward_epi / te_linear_backward_epi: no fall-back) -----------
+# ---- fused Linear epilogues of every kernel family (te_linear_forward / te_linear_backward: no fall-back) -------------------
 # Bounds per element, relative to the element's own scale |x||W|^T (+ |bias|): fp32 SIMT 3e-6 (test_tc_3xtf32_linear_is_fp32_grade),
 # 3xTF32 and the fp16 split 1.5e-8 * K + 2e-6 (same test; the fp16 split keeps the 3xTF32 operand precision), single-pass
 # TF32 / fp16 2e-3 (test_tc_persistent_pair_kernels).
@@ -460,6 +460,32 @@ def test_linear_epilogue_entry_points_do_not_fall_back():
     assert ex.value.status == _lib.TE_ERR_UNSUPPORTED
     y, _ = ops.linear_forward_epi(x, torch.randn(64, 96, device="cuda"), None, epi="store", family="simt")
     assert torch.isfinite(y).all()
+
+
+def test_linear_convenience_functions_fall_back_family_by_family():
+    """linear_forward / linear_backward / _f16 / _tf32 fall back where the family they ask for does not take the shape:
+    forward fp16 split -> 3xTF32 -> SIMT, backward fp16 or single-pass TF32 -> 3xTF32 -> SIMT.  Each result is bit-identical
+    to the strict entry point run on the family it should land on: width 64 (BERT-tiny) for every tensor-core family,
+    K = 96 (3xTF32 takes it, the fp16 kernels do not) and K = 128 (every family takes it)."""
+    from transformer_explainability_b200 import ops
+    g = torch.Generator(device="cuda").manual_seed(7)
+    rows = 77
+    for K, N, f16_lands, tc_lands in ((96, 64, "simt", "simt"), (96, 128, "3xtf32", "3xtf32"),
+                                      (128, 128, "f16_split", "3xtf32")):
+        x = torch.randn(rows, K, generator=g, device="cuda")
+        w = torch.randn(N, K, generator=g, device="cuda") * 0.05
+        b = torch.randn(N, generator=g, device="cuda")
+        for got, family in ((ops.linear_forward(x, w, b, tensor_cores=True), tc_lands),
+                            (ops.linear_forward(x, w, b, tensor_cores=True, f16_split=True), f16_lands)):
+            want, _ = ops.linear_forward_epi(x, w, b, epi="bias", family=family)
+            assert torch.equal(got, want), ("forward", K, N, family)
+    for K, N, f16_lands, tf32_lands, tc_lands in ((96, 64, "simt", "simt", "simt"), (96, 128, "3xtf32", "tf32", "3xtf32"),
+                                                  (128, 128, "f16", "tf32", "3xtf32")):
+        dy = torch.randn(rows, K, generator=g, device="cuda")
+        w = torch.randn(K, N, generator=g, device="cuda") * 0.05
+        for got, family in ((ops.linear_backward(dy, w, tensor_cores=True), tc_lands),
+                            (ops.linear_backward_f16(dy, w), f16_lands), (ops.linear_backward_tf32(dy, w), tf32_lands)):
+            assert torch.equal(got, ops.linear_backward_epi(dy, w, epi="store", family=family)), ("backward", K, N, family)
 
 
 # ---- the other producers of the fp16-split operand format ----------------------------------------------------------------

@@ -66,14 +66,12 @@ PROTOTYPES = {
     "te_vit_forward": (c_int, [_CFG, _P, _P, _P, c_int, c_uint, _P, _P, c_ll, _P]),
     "te_vit_derived_total": (c_ll, [_CFG]),
     "te_vit_prepare_derived": (c_int, [_CFG, _P, _P, _P]),
-    "te_vit_attribute": (c_int, [_CFG, _P, _P, c_int, _P, c_int, c_uint, _P, _P, c_ll, _P]),
-    "te_vit_attribute_alpha": (c_int, [_CFG, _P, _P, c_int, _P, c_int, c_float, c_uint, _P, _P, c_ll, _P]),
+    "te_vit_attribute": (c_int, [_CFG, _P, _P, c_int, _P, c_int, c_float, c_uint, _P, _P, c_ll, _P]),
     "te_vit_explain": (c_int, [_CFG, _P, _P, _P, c_int, _P, c_int, c_uint, _P, _P, _P, c_ll, _P]),
     "te_vit_tensor": (c_int, [_CFG, c_int, _P, c_char_p, c_int, ctypes.POINTER(_P), ctypes.POINTER(c_ll),
                               ctypes.POINTER(c_ll)]),
     "te_set_option": (c_int, [c_char_p, c_int]),
-    "te_vit_relprop_pixels": (c_int, [_CFG, _P, _P, c_int, _P, _P, _P, c_ll, _P]),
-    "te_vit_relprop_pixels_ex": (c_int, [_CFG, _P, _P, c_int, c_uint, _P, _P, _P, c_ll, _P]),
+    "te_vit_relprop_pixels": (c_int, [_CFG, _P, _P, c_int, c_uint, _P, _P, _P, c_ll, _P]),
     "te_bert_num_weights": (c_int, [_BCFG]),
     "te_bert_weight_name": (c_char_p, [_BCFG, c_int]),
     "te_bert_weight_numel": (c_ll, [_BCFG, c_int]),
@@ -83,14 +81,11 @@ PROTOTYPES = {
     "te_bert_prepare_derived": (c_int, [_BCFG, _P, _P, _P]),
     "te_bert_workspace_bytes": (c_ll, [_BCFG, c_int, c_int]),
     "te_bert_forward": (c_int, [_BCFG, _P, _P, _P, _P, c_int, c_int, c_uint, _P, _P, c_ll, _P]),
-    "te_bert_attribute": (c_int, [_BCFG, _P, _P, c_int, c_int, _P, c_int, c_uint, _P, _P, c_ll, _P]),
-    "te_bert_attribute_alpha": (c_int, [_BCFG, _P, _P, c_int, c_int, _P, c_int, c_float, c_uint, _P, _P, c_ll, _P]),
+    "te_bert_attribute": (c_int, [_BCFG, _P, _P, c_int, c_int, _P, c_int, c_float, c_uint, _P, _P, c_ll, _P]),
     "te_bert_explain": (c_int, [_BCFG, _P, _P, _P, _P, c_int, c_int, _P, c_int, c_uint, _P, _P, _P, c_ll, _P]),
     "te_bert_tensor": (c_int, [_BCFG, c_int, c_int, _P, c_char_p, c_int, ctypes.POINTER(_P), ctypes.POINTER(c_ll),
                                ctypes.POINTER(c_ll)]),
-    "te_linear_relprop": (c_int, [_P, _P, _P, _P, _P, c_int, c_int, c_int, c_uint, _P]),
-    "te_linear_relprop_ex": (c_int, [_P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_uint, _P]),
-    "te_linear_relprop_alpha": (c_int, [_P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_float, c_uint, _P]),
+    "te_linear_relprop": (c_int, [_P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_float, c_uint, _P]),
     "te_add_relprop": (c_int, [_P, _P, _P, _P, _P, _P, c_int, c_ll, _P]),
     "te_clone_relprop": (c_int, [_P, _P, _P, _P, _P, c_ll, _P]),
     "te_matmul_av_relprop": (c_int, [_P, _P, _P, _P, _P, _P, c_int, c_int, c_int, _P]),
@@ -105,12 +100,9 @@ PROTOTYPES = {
     "te_attribution_rollout": (c_int, [_P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_uint, _P, _P, _P,
                                        c_ll, _P]),
     "te_compute_rollout_attention": (c_int, [_P, c_int, c_int, c_int, c_int, c_int, _P, _P, c_ll, _P]),
-    "te_linear_forward": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, _P]),
-    "te_linear_forward_ex": (c_int, [_P, _P, _P, _P, _P, c_int, c_int, c_int, c_uint, _P]),
-    "te_linear_backward_ex": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_uint, _P]),
     "te_f16_block_split": (c_int, [_P, c_int, c_int, _P, _P, _P, _P]),
-    "te_linear_forward_epi": (c_int, [_P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_uint, _P]),
-    "te_linear_backward_epi": (c_int, [_P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_uint, _P]),
+    "te_linear_forward": (c_int, [_P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_uint, _P]),
+    "te_linear_backward": (c_int, [_P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_uint, _P]),
     "te_layernorm_split": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_float, _P]),
     "te_tc_zplus_s": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_uint, _P]),
     "te_tc_attention_nn": (c_int, [_P, c_ll, _P, c_ll, c_int, c_int, c_int, c_int, _P, c_int, _P, c_float, c_int, c_int, _P]),

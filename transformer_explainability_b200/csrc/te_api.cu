@@ -19,7 +19,7 @@ void te_count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
 extern "C" long long te_kernel_launch_count(void) { return g_launches.load(); }
 
 extern "C" const char* te_last_error(void) { return g_last_error.c_str(); }
-extern "C" int te_version(void) { return 100; }
+extern "C" int te_version(void) { return 101; }
 
 #define ST(s) reinterpret_cast<cudaStream_t>(s)
 #define REQ(c, msg) do { if (!(c)) { te_set_last_error(msg); return TE_ERR_ARG; } } while (0)
@@ -29,15 +29,6 @@ static TeGemm g0(int nb) {
     memset(&p, 0, sizeof(p));
     p.nb1 = nb; p.nb2 = 1; p.alpha = 1.f;
     return p;
-}
-
-extern "C" int te_linear_forward(const float* x, const float* w, const float* bias, float* y, int rows,
-                                 int in_features, int out_features, void* stream) {
-    REQ(x && w && y && rows > 0 && in_features > 0 && out_features > 0, "te_linear_forward: bad argument");
-    TeGemm p = g0(1);
-    p.A = x; p.lda = in_features; p.B = w; p.ldb = in_features; p.C = y; p.ldc = out_features; p.bias = bias;
-    p.M = rows; p.N = out_features; p.K = in_features;
-    return te_gemm_launch(p, TE_L_K, TE_L_K, TE_XF_NONE, TE_EPI_BIAS, ST(stream));
 }
 
 // The scratch of the stand-alone tensor-core entry points, in the layouts include/te_b200.h documents:
@@ -53,72 +44,59 @@ static TcScratch tc_scratch(float* scratch, long long s_floats, int in_features,
     return c;
 }
 
-// forward Linear with the kernel family the flags select.  strict: a tensor-core family that does not take the shape is an
-// error; otherwise every tensor-core path takes the shapes of the 3xTF32 kernel and the derived copies are made only when one is
-// taken.  With TE_FLAG_LINEAR_F16_SPLIT the operand is the fp16 hi, lo split of x (rows*in floats).
-static int linear_forward_flags(const float* x, const float* w, const float* bias, const float* e0, float* y, float* y2,
-                                float* scratch, int rows, int in_features, int out_features, int epi, unsigned flags,
-                                bool strict, cudaStream_t st) {
-    const bool tc = (flags & TE_FLAG_LINEAR_TENSOR_CORES) && scratch &&
-                    (strict || te_tc_gemm3x_supported(rows, in_features, out_features, in_features));
+// The Linear entries run the family the flags name or return TE_ERR_UNSUPPORTED before anything is launched.  The derived
+// weight copies start the scratch; with TE_FLAG_LINEAR_F16_SPLIT the operand region holds the fp16 hi, lo split of x
+// (rows*in floats), with TE_FLAG_BACKWARD_F16 the fp16 hi part of dy (rows*out/2 floats).
+extern "C" int te_linear_forward(const float* x, const float* w, const float* bias, const float* e0, float* y, float* y2,
+                                 float* scratch, int rows, int in_features, int out_features, int epi, unsigned flags,
+                                 void* stream) {
+    REQ(x && w && y && rows > 0 && in_features > 0 && out_features > 0, "te_linear_forward: bad argument");
+    REQ(epi >= TE_EPI_STORE && epi <= TE_EPI_BIAS_ADD, "te_linear_forward: epilogue must be STORE, BIAS, BIAS_GELU or BIAS_ADD");
+    REQ(y2 || (epi != TE_EPI_BIAS_GELU && epi != TE_EPI_BIAS_ADD), "te_linear_forward: BIAS_GELU / BIAS_ADD need y2");
+    REQ(e0 || epi != TE_EPI_BIAS_ADD, "te_linear_forward: BIAS_ADD needs e0");
+    REQ(!(flags & ~(TE_FLAG_LINEAR_TENSOR_CORES | TE_FLAG_LINEAR_F16_SPLIT)), "te_linear_forward: unknown family flags");
+    const bool tc = (flags & TE_FLAG_LINEAR_TENSOR_CORES) != 0, f16 = (flags & TE_FLAG_LINEAR_F16_SPLIT) != 0;
+    REQ(!f16 || tc, "te_linear_forward: TE_FLAG_LINEAR_F16_SPLIT needs TE_FLAG_LINEAR_TENSOR_CORES");
+    REQ(scratch || !tc, "te_linear_forward: the tensor-core families need scratch");
+    if (f16 && !te_tc_fwd16_supported(rows, in_features, out_features, in_features))
+        return te_util::no_fallback("te_linear_forward: the fp16-split kernel does not take this shape");
+    if (tc && !te_tc_gemm3x_supported(rows, in_features, out_features, in_features))
+        return te_util::no_fallback("te_linear_forward: the 3xTF32 kernel does not take this shape");
+    cudaStream_t st = ST(stream);
     if (tc) TE_TRY(te_tc_prepare_weights(w, scratch, in_features, out_features, st));
     te_util::F16Split fs = {nullptr, nullptr, false, nullptr, nullptr};
-    if (tc && (flags & TE_FLAG_LINEAR_F16_SPLIT)) {
+    if (f16) {
         const TcScratch c = tc_scratch(scratch, 0, in_features, out_features, (long long)rows * in_features);
         fs.split = c.op; fs.scale = c.scale;
     }
     return te_util::linear_fwd_tc(tc ? scratch : nullptr, x, in_features, w, bias, y, y2, e0, rows, in_features, out_features,
-                                  epi, st, &fs, strict);
+                                  epi, st, &fs);
 }
 
-// activation-gradient backward Linear, same selection.  With TE_FLAG_BACKWARD_F16 the operand is the fp16 hi part of dy
-// (rows*out/2 floats).
-static int linear_backward_flags(const float* dy, const float* w, const float* e0, float* dx, float* scratch, int rows,
-                                 int in_features, int out_features, int epi, unsigned flags, bool strict, cudaStream_t st) {
-    const bool tc = (flags & TE_FLAG_LINEAR_TENSOR_CORES) && scratch &&
-                    (strict || te_tc_gemm3x_supported(rows, out_features, in_features, out_features));
+extern "C" int te_linear_backward(const float* dy, const float* w, const float* e0, float* dx, float* scratch, int rows,
+                                  int in_features, int out_features, int epi, unsigned flags, void* stream) {
+    REQ(dy && w && dx && rows > 0 && in_features > 0 && out_features > 0, "te_linear_backward: bad argument");
+    REQ(epi == TE_EPI_STORE || epi == TE_EPI_GELU_BWD, "te_linear_backward: epilogue must be STORE or GELU_BWD");
+    REQ(e0 || epi != TE_EPI_GELU_BWD, "te_linear_backward: GELU_BWD needs e0");
+    REQ(!(flags & ~(TE_FLAG_LINEAR_TENSOR_CORES | TE_FLAG_BACKWARD_TF32 | TE_FLAG_BACKWARD_F16)),
+        "te_linear_backward: unknown family flags");
+    const bool tc = (flags & TE_FLAG_LINEAR_TENSOR_CORES) != 0, f16 = (flags & TE_FLAG_BACKWARD_F16) != 0;
+    REQ(!(flags & (TE_FLAG_BACKWARD_TF32 | TE_FLAG_BACKWARD_F16)) || tc,
+        "te_linear_backward: the single-pass families need TE_FLAG_LINEAR_TENSOR_CORES");
+    REQ(scratch || !tc, "te_linear_backward: the tensor-core families need scratch");
+    if (f16 && !te_tc_fwd16_supported(rows, out_features, in_features, out_features))
+        return te_util::no_fallback("te_linear_backward: the single-pass fp16 kernel does not take this shape");
+    if (tc && !te_tc_gemm3x_supported(rows, out_features, in_features, out_features))
+        return te_util::no_fallback("te_linear_backward: the 3xTF32 / single-pass TF32 kernels do not take this shape");
+    cudaStream_t st = ST(stream);
     if (tc) TE_TRY(te_tc_prepare_weights(w, scratch, in_features, out_features, st));
     te_util::F16Split fs = {nullptr, nullptr, false, nullptr, nullptr};
-    if (tc && (flags & TE_FLAG_BACKWARD_F16)) {
+    if (f16) {
         const TcScratch c = tc_scratch(scratch, 0, in_features, out_features, (long long)rows * out_features / 2);
         fs.split = c.op; fs.scale = c.scale;
     }
     return te_util::linear_bwd_tc(tc ? scratch : nullptr, dy, w, dx, e0, rows, in_features, out_features, epi, st,
-                                  (flags & TE_FLAG_BACKWARD_TF32) != 0, &fs, strict);
-}
-
-extern "C" int te_linear_forward_ex(const float* x, const float* w, const float* bias, float* y, float* scratch, int rows,
-                                    int in_features, int out_features, unsigned flags, void* stream) {
-    REQ(x && w && y && rows > 0 && in_features > 0 && out_features > 0, "te_linear_forward_ex: bad argument");
-    return linear_forward_flags(x, w, bias, nullptr, y, nullptr, scratch, rows, in_features, out_features, TE_EPI_BIAS, flags,
-                                false, ST(stream));
-}
-
-extern "C" int te_linear_forward_epi(const float* x, const float* w, const float* bias, const float* e0, float* y, float* y2,
-                                     float* scratch, int rows, int in_features, int out_features, int epi, unsigned flags,
-                                     void* stream) {
-    REQ(x && w && y && rows > 0 && in_features > 0 && out_features > 0, "te_linear_forward_epi: bad argument");
-    REQ(epi >= TE_EPI_STORE && epi <= TE_EPI_BIAS_ADD, "te_linear_forward_epi: epilogue must be STORE, BIAS, BIAS_GELU or BIAS_ADD");
-    REQ(y2 || (epi != TE_EPI_BIAS_GELU && epi != TE_EPI_BIAS_ADD), "te_linear_forward_epi: BIAS_GELU / BIAS_ADD need y2");
-    REQ(e0 || epi != TE_EPI_BIAS_ADD, "te_linear_forward_epi: BIAS_ADD needs e0");
-    REQ(!(flags & ~(TE_FLAG_LINEAR_TENSOR_CORES | TE_FLAG_LINEAR_F16_SPLIT)), "te_linear_forward_epi: unknown family flags");
-    REQ(!(flags & TE_FLAG_LINEAR_F16_SPLIT) || (flags & TE_FLAG_LINEAR_TENSOR_CORES),
-        "te_linear_forward_epi: TE_FLAG_LINEAR_F16_SPLIT needs TE_FLAG_LINEAR_TENSOR_CORES");
-    REQ(scratch || !(flags & TE_FLAG_LINEAR_TENSOR_CORES), "te_linear_forward_epi: the tensor-core families need scratch");
-    return linear_forward_flags(x, w, bias, e0, y, y2, scratch, rows, in_features, out_features, epi, flags, true, ST(stream));
-}
-
-extern "C" int te_linear_backward_epi(const float* dy, const float* w, const float* e0, float* dx, float* scratch, int rows,
-                                      int in_features, int out_features, int epi, unsigned flags, void* stream) {
-    REQ(dy && w && dx && rows > 0 && in_features > 0 && out_features > 0, "te_linear_backward_epi: bad argument");
-    REQ(epi == TE_EPI_STORE || epi == TE_EPI_GELU_BWD, "te_linear_backward_epi: epilogue must be STORE or GELU_BWD");
-    REQ(e0 || epi != TE_EPI_GELU_BWD, "te_linear_backward_epi: GELU_BWD needs e0");
-    REQ(!(flags & ~(TE_FLAG_LINEAR_TENSOR_CORES | TE_FLAG_BACKWARD_TF32 | TE_FLAG_BACKWARD_F16)),
-        "te_linear_backward_epi: unknown family flags");
-    REQ(!(flags & (TE_FLAG_BACKWARD_TF32 | TE_FLAG_BACKWARD_F16)) || (flags & TE_FLAG_LINEAR_TENSOR_CORES),
-        "te_linear_backward_epi: the single-pass families need TE_FLAG_LINEAR_TENSOR_CORES");
-    REQ(scratch || !(flags & TE_FLAG_LINEAR_TENSOR_CORES), "te_linear_backward_epi: the tensor-core families need scratch");
-    return linear_backward_flags(dy, w, e0, dx, scratch, rows, in_features, out_features, epi, flags, true, ST(stream));
+                                  (flags & TE_FLAG_BACKWARD_TF32) != 0, &fs);
 }
 
 extern "C" int te_layernorm_split(const float* x, const float* w, const float* b, float* y, float* mean, float* rstd, void* hi,
@@ -185,56 +163,25 @@ extern "C" int te_f16_block_split(const float* x, int rows, int cols, void* hi, 
     return te_tc_blocksplit_f16(x, cols, rows, cols, reinterpret_cast<float*>(hi), scale_inv, ST(stream));
 }
 
-extern "C" int te_linear_backward_ex(const float* dy, const float* w, float* dx, float* scratch, int rows, int in_features,
-                                     int out_features, unsigned flags, void* stream) {
-    REQ(dy && w && dx && rows > 0 && in_features > 0 && out_features > 0, "te_linear_backward_ex: bad argument");
-    return linear_backward_flags(dy, w, nullptr, dx, scratch, rows, in_features, out_features, TE_EPI_STORE, flags, false,
-                                 ST(stream));
-}
-
-extern "C" int te_linear_relprop_alpha(const float* x, const float* w, const float* bias, const float* y, const float* r,
-                                       float* out, float* scratch, int rows, int in_features, int out_features, float alpha,
-                                       unsigned flags, void* stream) {
-    REQ(x && w && r && out && scratch && rows > 0 && in_features > 0 && out_features > 0,
-        "te_linear_relprop_alpha: bad argument");
-    REQ(isfinite(alpha), "te_linear_relprop_alpha: alpha must be finite");
+extern "C" int te_linear_relprop(const float* x, const float* w, const float* bias, const float* y, const float* r, float* out,
+                                 float* scratch, int rows, int in_features, int out_features, float alpha, unsigned flags,
+                                 void* stream) {
+    REQ(x && w && r && out && scratch && rows > 0 && in_features > 0 && out_features > 0, "te_linear_relprop: bad argument");
+    REQ(isfinite(alpha), "te_linear_relprop: alpha must be finite");
+    const bool lrp = (flags & TE_FLAG_RULES_LRP) != 0;
     const float* derived = nullptr;
-    if (!y) {                                            // te_linear_relprop: either rule library, two-pass denominator
-        const bool lrp = (flags & TE_FLAG_RULES_LRP) != 0;
-        const unsigned tc_flag = lrp ? TE_FLAG_RULES_LRP_TC : TE_FLAG_ZPLUS_TENSOR_CORES;
-        if ((flags & tc_flag) && te_tc_zplus_supported(rows, in_features, out_features, in_features)) {
-            const TcScratch c = tc_scratch(scratch, (long long)rows * out_features, in_features, out_features, 0);
-            TE_TRY(te_tc_prepare_weights(w, c.derived, in_features, out_features, ST(stream)));
-            derived = c.derived;
-        }
-        if (lrp)
-            return te_zplus_linear_relprop_lrp(x, in_features, w, derived, r, out_features, out, scratch, rows, in_features,
-                                               out_features, ST(stream), 0, alpha);
-        return te_zplus_linear_relprop_ldr(x, in_features, w, derived, r, out_features, out, scratch, rows, in_features,
-                                           out_features, ST(stream), nullptr, 0, nullptr, {}, 0, nullptr, alpha);
-    }
-    // te_linear_relprop_ex: the layers_ours rule with the saved forward output (single-pass tensor-core denominator)
     float* xabs = nullptr;
-    if ((flags & TE_FLAG_ZPLUS_TENSOR_CORES) && te_tc_zplus_supported(rows, in_features, out_features, in_features)) {
+    if ((flags & (lrp ? TE_FLAG_RULES_LRP_TC : TE_FLAG_ZPLUS_TENSOR_CORES)) &&
+        te_tc_zplus_supported(rows, in_features, out_features, in_features)) {
         const TcScratch c = tc_scratch(scratch, (long long)rows * out_features, in_features, out_features, 0);   // operand: |x|
         TE_TRY(te_tc_prepare_weights(w, c.derived, in_features, out_features, ST(stream)));
         derived = c.derived;
-        xabs = c.op;
+        if (y) xabs = c.op;
     }
-    return te_zplus_linear_relprop_ldr(x, in_features, w, derived, r, out_features, out, scratch, rows, in_features,
-                                       out_features, ST(stream), y, out_features, bias, te_zplus_from_flags(flags), 0, xabs,
-                                       alpha);
-}
-
-extern "C" int te_linear_relprop(const float* x, const float* w, const float* r, float* out, float* scratch, int rows,
-                                 int in_features, int out_features, unsigned flags, void* stream) {
-    return te_linear_relprop_alpha(x, w, nullptr, nullptr, r, out, scratch, rows, in_features, out_features, 1.f, flags, stream);
-}
-
-extern "C" int te_linear_relprop_ex(const float* x, const float* w, const float* bias, const float* y, const float* r,
-                                    float* out, float* scratch, int rows, int in_features, int out_features,
-                                    unsigned flags, void* stream) {
-    return te_linear_relprop_alpha(x, w, bias, y, r, out, scratch, rows, in_features, out_features, 1.f, flags, stream);
+    // without y the z+ rule runs its two-pass form, to which the bf16 / fp16 variant flags do not apply
+    return te_linear_rule_relprop(lrp, x, in_features, w, derived, r, out_features, out, scratch, rows, in_features, out_features,
+                                  ST(stream), y, out_features, bias, y ? te_zplus_from_flags(flags) : ZplusVariant{}, 0, xabs,
+                                  alpha);
 }
 
 extern "C" int te_add_relprop(const float* x1, const float* x2, const float* r, float* r1, float* r2, void* scratch,

@@ -289,16 +289,9 @@ extern "C" int te_bert_forward(const te_bert_config* cfg, const float* weights, 
 // =====================================================================================================
 // attribute = class-gradient backward + relprop + normalised rollout   (Generator.generate_LRP :33-59)
 // =====================================================================================================
-extern "C" int te_bert_attribute(const te_bert_config* cfg, const float* weights, const float* derived, int batch,
-                                 int seq, int* index, int start_layer, unsigned flags, float* maps, void* workspace,
+extern "C" int te_bert_attribute(const te_bert_config* cfg, const float* weights, const float* derived, int batch, int seq,
+                                 int* index, int start_layer, float alpha, unsigned flags, float* maps, void* workspace,
                                  long long workspace_bytes, void* stream) {
-    return te_bert_attribute_alpha(cfg, weights, derived, batch, seq, index, start_layer, 1.f, flags, maps, workspace,
-                                   workspace_bytes, stream);
-}
-
-extern "C" int te_bert_attribute_alpha(const te_bert_config* cfg, const float* weights, const float* derived, int batch,
-                                       int seq, int* index, int start_layer, float alpha, unsigned flags, float* maps,
-                                       void* workspace, long long workspace_bytes, void* stream) {
     Dims d; Workspace ws;
     TE_TRY(check_ws(cfg, batch, seq, workspace, workspace_bytes, d, ws));
     if (!isfinite(alpha)) { te_set_last_error("te_bert_attribute: alpha must be finite"); return TE_ERR_ARG; }
@@ -355,19 +348,12 @@ extern "C" int te_bert_attribute_alpha(const te_bert_config* cfg, const float* w
     // BERT_orig_lrp.py: Linear with separate denominators, Add = RelPropSimple, also for the attention-mask Add).  dw is set
     // for the z+ rules with TE_FLAG_ZPLUS_TENSOR_CORES, for the layers_lrp rule with TE_FLAG_RULES_LRP_TC.  alpha != 1: the
     // alpha-beta Linear rule of either library.
-    const bool lrpv = (flags & TE_FLAG_RULES_LRP) != 0;
-    double* addp = lrpv ? nullptr : ws.addpart;
-    auto lin = [&](const float* x, long long ldx, const float* wt, const float* dwt, const float* r, long long ldr, float* out,
-                   float* sbuf, long long rows, int in, int outf, const float* y, long long ldy, const float* bias,
-                   long long ld_out, float* xabs) -> int {
-        if (lrpv) return te_zplus_linear_relprop_lrp(x, ldx, wt, dwt, r, ldr, out, sbuf, rows, in, outf, st, ld_out, alpha);
-        return te_zplus_linear_relprop_ldr(x, ldx, wt, dwt, r, ldr, out, sbuf, rows, in, outf, st, y, ldy, bias, sel.zv, ld_out, xabs,
-                                           alpha);
-    };
+    double* addp = sel.lrp ? nullptr : ws.addpart;
     // classifier.relprop (X = pooled) ; dropout / Tanh identity ; pooler.dense.relprop (X = first token) ; pool
-    TE_TRY(lin(ws.pooled, d.D, w.clsw, nullptr, ws.seed, d.C, ws.rpool, ws.shead, d.B, d.D, d.C, nullptr, 0, nullptr, 0, nullptr));
-    TE_TRY(lin(ws.h_last, (long long)d.N * d.D, w.poolw, nullptr, ws.rpool, d.D, ws.rfirst, ws.shead, d.B, d.D, d.D, nullptr, 0,
-               nullptr, 0, nullptr));
+    TE_TRY(te_linear_rule_relprop(sel.lrp, ws.pooled, d.D, w.clsw, nullptr, ws.seed, d.C, ws.rpool, ws.shead, d.B, d.D, d.C, st,
+                                  nullptr, 0, nullptr, sel.zv, 0, nullptr, alpha));
+    TE_TRY(te_linear_rule_relprop(sel.lrp, ws.h_last, (long long)d.N * d.D, w.poolw, nullptr, ws.rpool, d.D, ws.rfirst, ws.shead,
+                                  d.B, d.D, d.D, st, nullptr, 0, nullptr, sel.zv, 0, nullptr, alpha));
     TE_TRY(te_launch_index_select_relprop(ws.h_last, ws.rfirst, nullptr, R, d.B, d.N, d.D, st));
 
     for (int l = d.L - 1; l >= sel.low; --l) {
@@ -382,13 +368,16 @@ extern "C" int te_bert_attribute_alpha(const te_bert_config* cfg, const float* w
         const long long zr = top ? d.B : d.M;
         const long long sD = top ? (long long)d.N * d.D : d.D, sF = top ? (long long)d.N * d.F : d.F;
         TE_TRY(te_launch_add_relprop(a.d2, a.ao, R, R1, R2, addp, d.B, (long long)d.N * d.D, st));
-        TE_TRY(lin(a.g, sF, lw.w2, dw.w2, R1, sD, RF, S, zr, d.F, d.D, a.d2, sD, lw.b2, sF, SF));
-        TE_TRY(lin(a.ao, sD, lw.w1, dw.w1, RF, sF, R1, SF, zr, d.D, d.F, a.hpre, sF, lw.b1, sD, S));
+        TE_TRY(te_linear_rule_relprop(sel.lrp, a.g, sF, lw.w2, dw.w2, R1, sD, RF, S, zr, d.F, d.D, st, a.d2, sD, lw.b2, sel.zv, sF,
+                                      SF, alpha));
+        TE_TRY(te_linear_rule_relprop(sel.lrp, a.ao, sD, lw.w1, dw.w1, RF, sF, R1, SF, zr, d.D, d.F, st, a.hpre, sF, lw.b1, sel.zv,
+                                      sD, S, alpha));
         TE_TRY(te_launch_clone_relprop(a.ao, R1, R2, nullptr, R, MD, st));
         // BertSelfOutput.relprop :427-434
         TE_TRY(te_launch_add_relprop(a.d1, a.h, R, R1, R2, addp, d.B, (long long)d.N * d.D, st));
         if (top) TE_TRY(te_launch_fill(R3, 0.f, MD, st));
-        TE_TRY(lin(a.ctx, sD, lw.ow, dw.o, R1, sD, R3, S, zr, d.D, d.D, a.d1, sD, lw.ob, sD, S + MD));
+        TE_TRY(te_linear_rule_relprop(sel.lrp, a.ctx, sD, lw.ow, dw.o, R1, sD, R3, S, zr, d.D, d.D, st, a.d1, sD, lw.ob, sel.zv, sD,
+                                      S + MD, alpha));
         // BertSelfAttention.relprop :367-409: matmul2 rule -> attn_cam (:380), cam_v
         const bool last = (l == sel.low && !(flags & TE_FLAG_RELPROP_TO_INPUT));
         TE_TRY(attn_relprop_pv(sel, d.B, d.H, d.N, d.NP, d.dh, a.qkv, a.P, R3, a.ctx, S, a.cam, Rqkv, last, st));
@@ -400,11 +389,12 @@ extern "C" int te_bert_attribute_alpha(const te_bert_config* cfg, const float* w
         // matmul1 rule on the unscaled product -> cam_q, cam_k
         TE_TRY(attn_relprop_qk(sel, d.B, d.H, d.N, d.NP, d.dh, a.qkv, ws.tA[1], ws.tA[0], Rqkv, st));
         // query / key / value Linear rules (separate Linears), Clone(3), Clone(2)
-        TE_TRY(lin(a.h, d.D, lw.qkvw, dw.q, Rqkv, 3 * d.D, R, S, d.M, d.D, d.D, a.qkv, 3 * d.D, lw.qkvb, 0, S + MD));
-        TE_TRY(lin(a.h, d.D, lw.qkvw + DD, dw.k, Rqkv + d.D, 3 * d.D, R1, S, d.M, d.D, d.D, a.qkv + d.D, 3 * d.D, lw.qkvb + d.D, 0,
-                   S + MD));
-        TE_TRY(lin(a.h, d.D, lw.qkvw + 2 * DD, dw.v, Rqkv + 2 * d.D, 3 * d.D, R3, S, d.M, d.D, d.D, a.qkv + 2 * d.D, 3 * d.D,
-                   lw.qkvb + 2 * d.D, 0, S + MD));
+        TE_TRY(te_linear_rule_relprop(sel.lrp, a.h, d.D, lw.qkvw, dw.q, Rqkv, 3 * d.D, R, S, d.M, d.D, d.D, st, a.qkv, 3 * d.D,
+                                      lw.qkvb, sel.zv, 0, S + MD, alpha));
+        TE_TRY(te_linear_rule_relprop(sel.lrp, a.h, d.D, lw.qkvw + DD, dw.k, Rqkv + d.D, 3 * d.D, R1, S, d.M, d.D, d.D, st,
+                                      a.qkv + d.D, 3 * d.D, lw.qkvb + d.D, sel.zv, 0, S + MD, alpha));
+        TE_TRY(te_linear_rule_relprop(sel.lrp, a.h, d.D, lw.qkvw + 2 * DD, dw.v, Rqkv + 2 * d.D, 3 * d.D, R3, S, d.M, d.D, d.D, st,
+                                      a.qkv + 2 * d.D, 3 * d.D, lw.qkvb + 2 * d.D, sel.zv, 0, S + MD, alpha));
         TE_TRY(te_launch_clone_relprop(a.h, R, R1, R3, SF, MD, st));                      // self.clone (3-way)
         TE_TRY(te_launch_clone_relprop(a.h, SF, R2, nullptr, R, MD, st));                 // attention.clone
     }
@@ -422,7 +412,7 @@ extern "C" int te_bert_explain(const te_bert_config* cfg, const float* weights, 
                                long long workspace_bytes, void* stream) {
     TE_TRY(te_bert_forward(cfg, weights, derived, input_ids, attention_mask, batch, seq, flags, logits, workspace,
                            workspace_bytes, stream));
-    return te_bert_attribute(cfg, weights, derived, batch, seq, index, start_layer, flags, maps, workspace, workspace_bytes,
+    return te_bert_attribute(cfg, weights, derived, batch, seq, index, start_layer, 1.f, flags, maps, workspace, workspace_bytes,
                              stream);
 }
 

@@ -839,8 +839,8 @@ int te_launch_clone_relprop(const float* x, const float* r1, const float* r2, co
     TE_CUDA_CHECK_LAUNCH();
     return TE_OK;
 }
-int te_launch_add_relprop_ex(const float* x1, const float* x2, long long x2_sample_stride, const float* r, float* r1,
-                             float* r2, double* partial, int B, long long per_sample, cudaStream_t st) {
+int te_launch_add_relprop_strided(const float* x1, const float* x2, long long x2_sample_stride, const float* r, float* r1,
+                                  float* r2, double* partial, int B, long long per_sample, cudaStream_t st) {
     TE_REQ(per_sample % 4 == 0 && x2_sample_stride % 4 == 0, "add_relprop: per-sample size % 4 != 0");
     TE_REQ(B <= 65535, "add_relprop: batch too large for one launch");
     const long long per4 = per_sample / 4, x2s4 = x2_sample_stride / 4;
@@ -856,7 +856,7 @@ int te_launch_add_relprop_ex(const float* x1, const float* x2, long long x2_samp
 }
 int te_launch_add_relprop(const float* x1, const float* x2, const float* r, float* r1, float* r2, double* partial,
                           int B, long long per_sample, cudaStream_t st) {
-    return te_launch_add_relprop_ex(x1, x2, per_sample, r, r1, r2, partial, B, per_sample, st);
+    return te_launch_add_relprop_strided(x1, x2, per_sample, r, r1, r2, partial, B, per_sample, st);
 }
 int te_launch_index_select_relprop(const float* x, const float* r_tok0, const float* r_tok1, float* out, int B,
                                    int N, int D, cudaStream_t st) {

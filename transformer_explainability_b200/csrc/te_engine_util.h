@@ -46,8 +46,8 @@ static inline int linear_bwd(const float* dy, const float* w, float* dx, const f
     return te_gemm_launch(p, TE_L_K, TE_L_MN, TE_XF_NONE, epi, st);
 }
 
-// strict: a requested kernel family that does not take the shape / epilogue is an error (TE_ERR_UNSUPPORTED), not a fall-back to
-// the next family — what the diagnostic entry points te_linear_forward_epi / te_linear_backward_epi need
+// a requested kernel family that does not take the shape / epilogue is an error (TE_ERR_UNSUPPORTED), not a fall-back to the
+// next family — what the diagnostic entry points need
 static inline int no_fallback(const char* msg) {
     te_set_last_error(msg);
     return TE_ERR_UNSUPPORTED;
@@ -60,32 +60,26 @@ static inline int no_fallback(const char* msg) {
 struct F16Split { float* split; float* scale; bool ready; float* split_out; float* scale_out; };
 static inline int linear_fwd_tc(const float* dw, const float* x, int lda, const float* w, const float* bias, float* y,
                                 float* y2, const float* e0, long long M, int in, int out, int epi, cudaStream_t st,
-                                const F16Split* fs = nullptr, bool strict = false) {
+                                const F16Split* fs = nullptr) {
     const bool f16 = dw && fs && fs->split;
     if (f16 && epi != TE_EPI_GELU_BWD && te_tc_fwd16_supported(M, in, out, lda))
         return te_tc_linear_fwd16(fs->ready ? nullptr : x, lda, fs->split, fs->scale, dw, in, out, bias, y, y2, e0, M, epi, st,
                                   epi == TE_EPI_BIAS_GELU ? fs->split_out : nullptr, epi == TE_EPI_BIAS_GELU ? fs->scale_out : nullptr);
-    if (strict && f16) return no_fallback("linear forward: the fp16-split kernel does not take this shape / epilogue");
     if (dw && te_tc_gemm3x_supported(M, in, out, lda))
         return te_tc_linear_fwd(x, lda, dw, in, out, bias, y, y2, e0, M, epi, st);      // epilogue ids coincide
-    if (strict && dw) return no_fallback("linear forward: the 3xTF32 kernel does not take this shape");
     return linear_fwd(x, lda, w, bias, y, y2, e0, M, in, out, epi, st);
 }
 // tf32: single-pass TF32 wgmma kernel (TE_FLAG_BACKWARD_TF32) instead of the 3xTF32 split
 // fs: hi-only split scratch of dy (M*out/2 floats + M*ceil(out/128)) -> single-pass fp16 kernel (TE_FLAG_BACKWARD_F16)
 static inline int linear_bwd_tc(const float* dw, const float* dy, const float* w, float* dx, const float* e0, long long M,
-                                int in, int out, int epi, cudaStream_t st, bool tf32 = false, const F16Split* fs = nullptr,
-                                bool strict = false) {
+                                int in, int out, int epi, cudaStream_t st, bool tf32 = false, const F16Split* fs = nullptr) {
     const bool f16 = dw && fs && fs->split, single_epi = epi == TE_EPI_STORE || epi == TE_EPI_GELU_BWD;
     if (f16 && single_epi && te_tc_fwd16_supported(M, out, in, out))
         return te_tc_linear_bwd16(fs->ready ? nullptr : dy, out, fs->split, fs->scale, dw, in, out, dx, e0, M, epi, st);
-    if (strict && f16) return no_fallback("linear backward: the single-pass fp16 kernel does not take this shape / epilogue");
     if (dw && tf32 && single_epi && te_tc_gemm3x_supported(M, out, in, out))
         return te_tc_linear_bwd_tf32(dy, out, dw, in, out, dx, e0, M, epi, st);
-    if (strict && dw && tf32) return no_fallback("linear backward: the single-pass TF32 kernel does not take this shape / epilogue");
     if (dw && te_tc_gemm3x_supported(M, out, in, out))
         return te_tc_linear_bwd(dy, dw, in, out, dx, e0, M, epi, st);
-    if (strict && dw) return no_fallback("linear backward: the 3xTF32 kernel does not take this shape");
     return linear_bwd(dy, w, dx, e0, M, in, out, epi, st);
 }
 
@@ -148,7 +142,7 @@ static inline int attn_nk(bool tc, int B, int H, int N, int NP, int dh, const fl
 
 // ---- kernel selection ------------------------------------------------------------------------------------------------
 // What the engine flags select for one te_*_forward / te_*_attribute call.  The model-specific modes (TE_FLAG_GRADIENTS_ONLY,
-// TE_FLAG_RULES_LRP, TE_FLAG_RELPROP_TO_INPUT) are read where they are used.
+// TE_FLAG_RELPROP_TO_INPUT) are read where they are used.
 struct Select {
     const float* lbase;   // derived weights of the forward / backward Linears (TE_FLAG_LINEAR_TENSOR_CORES), else NULL
     const float* dbase;   // derived weights of the Linear relevance rules: the z+ rules (TE_FLAG_ZPLUS_TENSOR_CORES), or with
@@ -158,6 +152,7 @@ struct Select {
     bool rtf;             // single-pass TF32 relevance-side attention contractions (TE_FLAG_RELPROP_TF32)
     bool f16;             // fp16-split forward Linears requested (TE_FLAG_LINEAR_F16_SPLIT); f16_forward() checks the shapes
     F16Split bfs;         // single-pass fp16 backward Linears (TE_FLAG_BACKWARD_F16): hi-only split of dy; split NULL = off
+    bool lrp;             // rule library of modules/layers_lrp.py instead of layers_ours (TE_FLAG_RULES_LRP)
     ZplusVariant zv;      // bf16 / fp16 variants of the tensor-core z+ rule
     int low;              // lowest block the relprop must reach
 };
@@ -194,6 +189,7 @@ static inline int decode_flags(Select& s, const char* fn, unsigned flags, const 
         return TE_ERR_WORKSPACE;
     }
     s.bfs = {bf16 ? bwd_split.ptr : nullptr, bwd_scale.ptr, false, nullptr, nullptr};
+    s.lrp = lrp;
     s.zv = te_zplus_from_flags(flags);
     s.low = (flags & (TE_FLAG_KEEP_ALL_CAMS | TE_FLAG_RELPROP_TO_INPUT)) ? 0 : start_layer;
     return TE_OK;

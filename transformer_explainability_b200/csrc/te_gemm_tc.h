@@ -56,7 +56,7 @@ long long te_tc_derived_floats(int in_features, int out_features);
 int te_tc_prepare_weights(const float* w, float* derived, int in_features, int out_features, cudaStream_t st);
 // y / bias (optional): the Linear's saved forward output y = x W^T + bias [rows, out] (row stride ldy).  When given,
 // Z is formed in ONE pass as ((y - bias) + |x| |W|^T) / 2  ==  x+ W+^T + x- W-^T  (exact identity), halving the S kernel.
-// zv, ld_out, xabs: as in te_zplus_linear_relprop_ldr (te_zplus.h).
+// zv, ld_out, xabs: as in te_zplus_linear_relprop (te_zplus.h).
 int te_tc_zplus_linear_relprop(const float* x, long long ldx, const float* derived, const float* r, long long ldr,
                                float* out, float* s_scratch, long long rows, int in_features, int out_features, cudaStream_t st,
                                const float* y, long long ldy, const float* bias, ZplusVariant zv, long long ld_out,

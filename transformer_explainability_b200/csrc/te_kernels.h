@@ -39,8 +39,8 @@ int te_launch_add_relprop(const float* x1, const float* x2, const float* r, floa
                           int B, long long per_sample, cudaStream_t st);
 // partial == NULL selects the layers_lrp variant (modules/layers_lrp.py:48-60,98-100): r1 = x1*sd(r,x1+x2), r2 = x2*sd(...)
 // same with x2 addressed as x2 + b*x2_sample_stride (0: one tensor shared by every sample, e.g. pos_embed); r2 may be null
-int te_launch_add_relprop_ex(const float* x1, const float* x2, long long x2_sample_stride, const float* r, float* r1,
-                             float* r2, double* partial, int B, long long per_sample, cudaStream_t st);
+int te_launch_add_relprop_strided(const float* x1, const float* x2, long long x2_sample_stride, const float* r, float* r1,
+                                  float* r2, double* partial, int B, long long per_sample, cudaStream_t st);
 // ---- first layer: Conv2d z^B rule behind PatchEmbed.relprop (te_patch_relprop.cu) ------------------
 long long te_patch_relprop_scratch_floats(int B, int C, int img, int P, int D);
 // r: relevance of the patch tokens, row (b, p) at r + b*r_sample_stride + p*D.  r_pixels [B,C,img,img] and / or

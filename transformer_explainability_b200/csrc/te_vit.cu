@@ -306,16 +306,9 @@ extern "C" int te_vit_prepare_derived(const te_vit_config* cfg, const float* wei
     return TE_OK;
 }
 
-extern "C" int te_vit_attribute(const te_vit_config* cfg, const float* weights, const float* derived, int batch,
-                                int* index, int start_layer, unsigned flags, float* maps, void* workspace,
+extern "C" int te_vit_attribute(const te_vit_config* cfg, const float* weights, const float* derived, int batch, int* index,
+                                int start_layer, float alpha, unsigned flags, float* maps, void* workspace,
                                 long long workspace_bytes, void* stream) {
-    return te_vit_attribute_alpha(cfg, weights, derived, batch, index, start_layer, 1.f, flags, maps, workspace, workspace_bytes,
-                                  stream);
-}
-
-extern "C" int te_vit_attribute_alpha(const te_vit_config* cfg, const float* weights, const float* derived, int batch,
-                                      int* index, int start_layer, float alpha, unsigned flags, float* maps, void* workspace,
-                                      long long workspace_bytes, void* stream) {
     Dims d; Workspace ws;
     TE_TRY(check_ws(cfg, batch, workspace, workspace_bytes, d, ws));
     if (!isfinite(alpha)) { te_set_last_error("te_vit_attribute: alpha must be finite"); return TE_ERR_ARG; }
@@ -330,7 +323,6 @@ extern "C" int te_vit_attribute_alpha(const te_vit_config* cfg, const float* wei
     te_util::Select sel;
     TE_TRY(te_util::decode_flags(sel, "te_vit_attribute", flags, derived, start_layer, true, {ws.tF[1], ws.nF[1]},
                                  {ws.t3D[1], M3D}, d.M, std::max(3 * d.D, d.F)));
-    const bool lrpv = (flags & TE_FLAG_RULES_LRP) != 0;         // rule library of modules/layers_lrp.py (ViT_orig_LRP.py)
 
     // ---- class index and seeds  (ViT_explanation_generator.py:28-35) ---------------------------
     TE_TRY(te_launch_argmax(ws.logits, index, d.B, d.C, /*only_negative=*/1, st));
@@ -375,23 +367,16 @@ extern "C" int te_vit_attribute_alpha(const te_vit_config* cfg, const float* wei
     float* R = ws.tD[0]; float* R1 = ws.tD[1]; float* R2 = ws.tD[2]; float* R3 = ws.tD[3];
     float* RF = ws.tF[0]; float* SF = ws.tF[1]; float* S = ws.t3D[0]; float* Rqkv = ws.t3D[1]; float* S1 = ws.tA;
     // head.relprop (z+), pool.relprop (IndexSelect), norm.relprop (identity)
-    // z+ rule / Add rule of the selected rule library (layers_ours, or layers_lrp with TE_FLAG_RULES_LRP; dwt is then set
-    // only with TE_FLAG_RULES_LRP_TC); alpha != 1: the alpha-beta Linear rule of either library
-    auto zrule = [&](const float* x, long long ldx, const float* wt, const float* dwt, const float* r, long long ldr, float* out,
-                     float* sbuf, long long rows, int in, int outf, const float* y, long long ldy, const float* bias,
-                     long long ld_out, float* xabs) -> int {
-        if (lrpv) return te_zplus_linear_relprop_lrp(x, ldx, wt, dwt, r, ldr, out, sbuf, rows, in, outf, st, ld_out, alpha);
-        return te_zplus_linear_relprop_ldr(x, ldx, wt, dwt, r, ldr, out, sbuf, rows, in, outf, st, y, ldy, bias, sel.zv, ld_out, xabs,
-                                           alpha);
-    };
+    // Linear rule / Add rule of the selected rule library (layers_ours, or layers_lrp with TE_FLAG_RULES_LRP; the derived
+    // weights are then set only with TE_FLAG_RULES_LRP_TC); alpha != 1: the alpha-beta Linear rule of either library
     auto addrule = [&](const float* x1, const float* x2, const float* r, float* r1, float* r2) -> int {
-        return te_launch_add_relprop(x1, x2, r, r1, r2, lrpv ? nullptr : ws.addpart, d.B, (long long)d.N * d.D, st);
+        return te_launch_add_relprop(x1, x2, r, r1, r2, sel.lrp ? nullptr : ws.addpart, d.B, (long long)d.N * d.D, st);
     };
-    TE_TRY(zrule(ws.xf, (long long)d.N * d.D, w.headw, nullptr, ws.seed, d.C, ws.rhead0, ws.shead, d.B, d.D, d.C, nullptr, 0,
-                 nullptr, 0, nullptr));
+    TE_TRY(te_linear_rule_relprop(sel.lrp, ws.xf, (long long)d.N * d.D, w.headw, nullptr, ws.seed, d.C, ws.rhead0, ws.shead, d.B,
+                                  d.D, d.C, st, nullptr, 0, nullptr, sel.zv, 0, nullptr, alpha));
     if (cfg->distilled)
-        TE_TRY(zrule(ws.xf + d.D, (long long)d.N * d.D, w.headdw, nullptr, ws.seed, d.C, ws.rhead1, ws.shead, d.B, d.D, d.C,
-                     nullptr, 0, nullptr, 0, nullptr));
+        TE_TRY(te_linear_rule_relprop(sel.lrp, ws.xf + d.D, (long long)d.N * d.D, w.headdw, nullptr, ws.seed, d.C, ws.rhead1,
+                                      ws.shead, d.B, d.D, d.C, st, nullptr, 0, nullptr, sel.zv, 0, nullptr, alpha));
     TE_TRY(te_launch_index_select_relprop(ws.xf, ws.rhead0, cfg->distilled ? ws.rhead1 : nullptr, R, d.B, d.N, d.D, st));
 
     for (int l = d.L - 1; l >= sel.low; --l) {
@@ -403,23 +388,27 @@ extern "C" int te_vit_attribute_alpha(const te_vit_config* cfg, const float* wei
         // and every rule down to the proj rule is row-wise: Add / Clone map a zero row to a zero row, the z+ rule computes
         // each output row from the same input row.  So the three z+ rules of the top block run on the B pooled rows only
         // (row stride N*D / N*F) — exact (SURVEY.md 8a "structural savings"), bit-identical rows, 1/N of the work.
-        const bool top = (l == d.L - 1) && !cfg->distilled && !lrpv && te_engine_cls_rows();
+        const bool top = (l == d.L - 1) && !cfg->distilled && !sel.lrp && te_engine_cls_rows();
         const long long zr = top ? d.B : d.M;                          // rows the z+ rules of this block touch
         const long long sD = top ? (long long)d.N * d.D : d.D, sF = top ? (long long)d.N * d.F : d.F;
         TE_TRY(addrule(a.x_mid, a.mlp_out, R, R1, R2));                                                            // add2
-        TE_TRY(zrule(a.g, sF, bw.fc2w, dw.fc2, R2, sD, RF, S, zr, d.F, d.D, a.mlp_out, sD, bw.fc2b, sF, SF));      // fc2 ; GELU id
-        TE_TRY(zrule(a.xn2, sD, bw.fc1w, dw.fc1, RF, sF, R2, SF, zr, d.D, d.F, a.h, sF, bw.fc1b, sD, S));          // fc1 ; norm2 id
+        TE_TRY(te_linear_rule_relprop(sel.lrp, a.g, sF, bw.fc2w, dw.fc2, R2, sD, RF, S, zr, d.F, d.D, st, a.mlp_out, sD, bw.fc2b,
+                                      sel.zv, sF, SF, alpha));                                                    // fc2 ; GELU id
+        TE_TRY(te_linear_rule_relprop(sel.lrp, a.xn2, sD, bw.fc1w, dw.fc1, RF, sF, R2, SF, zr, d.D, d.F, st, a.h, sF, bw.fc1b,
+                                      sel.zv, sD, S, alpha));                                                     // fc1 ; norm2 id
         TE_TRY(te_launch_clone_relprop(a.x_mid, R1, R2, nullptr, R, MD, st));                                      // clone2
         TE_TRY(addrule(a.x_in, a.attn_out, R, R1, R2));                                                            // add1
         // Attention.relprop :154-177
         if (top) TE_TRY(te_launch_fill(R3, 0.f, MD, st));                                   // rows the strided rule does not write
-        TE_TRY(zrule(a.ctx, sD, bw.projw, dw.proj, R2, sD, R3, S, zr, d.D, d.D, a.attn_out, sD, bw.projb, sD, S + MD));   // proj
+        TE_TRY(te_linear_rule_relprop(sel.lrp, a.ctx, sD, bw.projw, dw.proj, R2, sD, R3, S, zr, d.D, d.D, st, a.attn_out, sD,
+                                      bw.projb, sel.zv, sD, S + MD, alpha));                                      // proj
         // matmul2 rule -> attn_cam (:160-165), cam_v ; matmul1 rule -> cam_q, cam_k (:170-173)
         const bool last = (l == sel.low && !(flags & TE_FLAG_RELPROP_TO_INPUT));      // nothing below attn_cam is consumed
         TE_TRY(te_util::attn_relprop_pv(sel, d.B, d.H, d.N, d.NP, d.dh, a.qkv, a.P, R3, a.ctx, S, a.cam, Rqkv, last, st));
         if (last) break;
         TE_TRY(te_util::attn_relprop_qk(sel, d.B, d.H, d.N, d.NP, d.dh, a.qkv, a.cam, S1, Rqkv, st));
-        TE_TRY(zrule(a.xn1, d.D, bw.qkvw, dw.qkv, Rqkv, 3 * d.D, R2, S, d.M, d.D, 3 * d.D, a.qkv, 3 * d.D, bw.qkvb, 0, RF));   // qkv ; norm1 id
+        TE_TRY(te_linear_rule_relprop(sel.lrp, a.xn1, d.D, bw.qkvw, dw.qkv, Rqkv, 3 * d.D, R2, S, d.M, d.D, 3 * d.D, st, a.qkv,
+                                      3 * d.D, bw.qkvb, sel.zv, 0, RF, alpha));                                   // qkv ; norm1 id
         TE_TRY(te_launch_clone_relprop(a.x_in, R1, R2, nullptr, R, MD, st));                                       // clone1
     }
 
@@ -437,15 +426,8 @@ extern "C" int te_vit_attribute_alpha(const te_vit_config* cfg, const float* wei
 // Precondition: te_vit_forward + te_vit_attribute(flags | TE_FLAG_RELPROP_TO_INPUT) on this workspace and these images.
 // ================================================================================================
 extern "C" int te_vit_relprop_pixels(const te_vit_config* cfg, const float* weights, const float* images, int batch,
-                                     float* pixel_maps, float* pixel_relevance, void* workspace, long long workspace_bytes,
-                                     void* stream) {
-    return te_vit_relprop_pixels_ex(cfg, weights, images, batch, 0u, pixel_maps, pixel_relevance, workspace, workspace_bytes,
-                                    stream);
-}
-
-extern "C" int te_vit_relprop_pixels_ex(const te_vit_config* cfg, const float* weights, const float* images, int batch,
-                                        unsigned flags, float* pixel_maps, float* pixel_relevance, void* workspace,
-                                        long long workspace_bytes, void* stream) {
+                                     unsigned flags, float* pixel_maps, float* pixel_relevance, void* workspace,
+                                     long long workspace_bytes, void* stream) {
     Dims d; Workspace ws;
     TE_TRY(check_ws(cfg, batch, workspace, workspace_bytes, d, ws));
     if (!weights || !images || (!pixel_maps && !pixel_relevance)) { te_set_last_error("te_vit_relprop_pixels: null pointer"); return TE_ERR_ARG; }
@@ -462,8 +444,8 @@ extern "C" int te_vit_relprop_pixels_ex(const te_vit_config* cfg, const float* w
                       d.D, TE_EPI_BIAS, st));
     TE_TRY(te_launch_assemble_tokens(patch_out, w.cls, w.dist, nullptr, tokens, d.B, d.N, d.D, d.prefix, st));
     // self.add.relprop: x2 = pos_embed, shared by every sample; only the tokens' share is consumed
-    TE_TRY(te_launch_add_relprop_ex(tokens, w.pos, 0, R, Rtok, nullptr, (flags & TE_FLAG_RULES_LRP) ? nullptr : ws.addpart, d.B,
-                                    (long long)d.N * d.D, st));
+    TE_TRY(te_launch_add_relprop_strided(tokens, w.pos, 0, R, Rtok, nullptr, (flags & TE_FLAG_RULES_LRP) ? nullptr : ws.addpart,
+                                         d.B, (long long)d.N * d.D, st));
     // cam[:, 1:] -> PatchEmbed.relprop (:238-242) -> Conv2d z^B rule -> sum over channels
     return te_patch_relprop_run(images, w.patchw, Rtok + (long long)d.prefix * d.D, (long long)d.N * d.D, d.B, d.Cin, d.img,
                                 d.P, d.D, ws.pix, pixel_relevance, pixel_maps, st);
@@ -473,7 +455,7 @@ extern "C" int te_vit_explain(const te_vit_config* cfg, const float* weights, co
                               int batch, int* index, int start_layer, unsigned flags, float* maps, float* logits,
                               void* workspace, long long workspace_bytes, void* stream) {
     TE_TRY(te_vit_forward(cfg, weights, derived, images, batch, flags, logits, workspace, workspace_bytes, stream));
-    return te_vit_attribute(cfg, weights, derived, batch, index, start_layer, flags, maps, workspace, workspace_bytes,
+    return te_vit_attribute(cfg, weights, derived, batch, index, start_layer, 1.f, flags, maps, workspace, workspace_bytes,
                             stream);
 }
 

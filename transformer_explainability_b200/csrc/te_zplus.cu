@@ -11,16 +11,9 @@ ZplusVariant te_zplus_from_flags(unsigned flags) {
 }
 
 int te_zplus_linear_relprop(const float* x, long long ldx, const float* w, const float* w_derived, const float* r,
-                            float* out, float* s_scratch, long long rows, int in_features, int out_features,
-                            cudaStream_t st) {
-    return te_zplus_linear_relprop_ldr(x, ldx, w, w_derived, r, out_features, out, s_scratch, rows, in_features,
-                                       out_features, st);
-}
-
-int te_zplus_linear_relprop_ldr(const float* x, long long ldx, const float* w, const float* w_derived, const float* r,
-                                long long ldr, float* out, float* s_scratch, long long rows, int in_features,
-                                int out_features, cudaStream_t st, const float* y, long long ldy, const float* bias, ZplusVariant zv,
-                                long long ld_out, float* xabs, float alpha) {
+                            long long ldr, float* out, float* s_scratch, long long rows, int in_features,
+                            int out_features, cudaStream_t st, const float* y, long long ldy, const float* bias, ZplusVariant zv,
+                            long long ld_out, float* xabs, float alpha) {
     if (rows <= 0) return TE_OK;
     if (ld_out == 0) ld_out = in_features;
     if (!isfinite(alpha)) { te_set_last_error("zplus: alpha must be finite"); return TE_ERR_ARG; }
@@ -97,4 +90,15 @@ int te_zplus_linear_relprop_lrp(const float* x, long long ldx, const float* w, c
         TE_TRY(te_gemm_launch(p, TE_L_K, TE_L_MN, h.r_xf, h.r_epi, st));
     }
     return TE_OK;
+}
+
+int te_linear_rule_relprop(bool lrp, const float* x, long long ldx, const float* w, const float* w_derived, const float* r,
+                           long long ldr, float* out, float* s_scratch, long long rows, int in_features, int out_features,
+                           cudaStream_t st, const float* y, long long ldy, const float* bias, ZplusVariant zv,
+                           long long ld_out, float* xabs, float alpha) {
+    if (lrp)
+        return te_zplus_linear_relprop_lrp(x, ldx, w, w_derived, r, ldr, out, s_scratch, rows, in_features, out_features, st,
+                                           ld_out, alpha);
+    return te_zplus_linear_relprop(x, ldx, w, w_derived, r, ldr, out, s_scratch, rows, in_features, out_features, st, y, ldy,
+                                   bias, zv, ld_out, xabs, alpha);
 }

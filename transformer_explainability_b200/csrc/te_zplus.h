@@ -14,20 +14,17 @@
 struct ZplusVariant { bool r_bf16, s1_bf16, r_f16; };
 ZplusVariant te_zplus_from_flags(unsigned flags);
 
-// x [rows, in] with row stride ldx ; w [out, in] ; r [rows, out] ; out [rows, in] ; s_scratch [rows, out].
+// x [rows, in] with row stride ldx ; w [out, in] ; r [rows, out] with row stride ldr (a column slice of a packed
+// [rows, 3*out] relevance tensor) ; out [rows, in] ; s_scratch [rows, out].
 // w_derived: the te_tc_prepare_weights() copies of w, or NULL.  When given (and the shape qualifies) both
 // contractions run on wgmma tensor cores (TF32 inputs, fp32 accumulate); otherwise — and as the checker —
 // the fp32 SIMT path.
-int te_zplus_linear_relprop(const float* x, long long ldx, const float* w, const float* w_derived, const float* r,
-                            float* out, float* s_scratch, long long rows, int in_features, int out_features,
-                            cudaStream_t st);
-// same with an explicit row stride for r (a column slice of a packed [rows, 3*out] relevance tensor)
 // y / bias: the Linear's saved forward output and bias (optional; enables the single-pass tensor-core S kernel)
-int te_zplus_linear_relprop_ldr(const float* x, long long ldx, const float* w, const float* w_derived, const float* r,
-                                long long ldr, float* out, float* s_scratch, long long rows, int in_features,
-                                int out_features, cudaStream_t st, const float* y = nullptr, long long ldy = 0,
-                                const float* bias = nullptr, ZplusVariant zv = {}, long long ld_out = 0,
-                                float* xabs = nullptr, float alpha = 1.f);
+int te_zplus_linear_relprop(const float* x, long long ldx, const float* w, const float* w_derived, const float* r,
+                            long long ldr, float* out, float* s_scratch, long long rows, int in_features,
+                            int out_features, cudaStream_t st, const float* y = nullptr, long long ldy = 0,
+                            const float* bias = nullptr, ZplusVariant zv = {}, long long ld_out = 0,
+                            float* xabs = nullptr, float alpha = 1.f);
 // xabs: scratch [rows, in] (the |x| operand of the single-pass S kernel); without it the tensor-core path uses the two-pass
 // S kernel.
 // ld_out: row stride of out (0 = in_features).  With row strides on x, r, y and out the rule runs on a strided subset of
@@ -39,7 +36,14 @@ int te_zplus_linear_relprop_ldr(const float* x, long long ldx, const float* w, c
 // run after the activator's through the same s_scratch.
 // w_derived: the te_tc_prepare_weights() copies of w, or NULL.  When given (and the shape qualifies) both halves run on
 // single-pass TF32 wgmma (TE_FLAG_RULES_LRP_TC; every denominator is a sum of non-negative products); otherwise fp32 SIMT.
-// ld_out: row stride of out (0 = in_features), for the strided row subsets of te_zplus_linear_relprop_ldr.
+// ld_out: row stride of out (0 = in_features), for the strided row subsets of te_zplus_linear_relprop.
 int te_zplus_linear_relprop_lrp(const float* x, long long ldx, const float* w, const float* w_derived, const float* r,
                                 long long ldr, float* out, float* s_scratch, long long rows, int in_features, int out_features,
                                 cudaStream_t st, long long ld_out = 0, float alpha = 1.f);
+
+// The Linear rule of the selected rule library: lrp (TE_FLAG_RULES_LRP) runs te_zplus_linear_relprop_lrp, which does not
+// read y, ldy, bias, zv or xabs; otherwise te_zplus_linear_relprop (layers_ours).  The other arguments go to either as given.
+int te_linear_rule_relprop(bool lrp, const float* x, long long ldx, const float* w, const float* w_derived, const float* r,
+                           long long ldr, float* out, float* s_scratch, long long rows, int in_features, int out_features,
+                           cudaStream_t st, const float* y, long long ldy, const float* bias, ZplusVariant zv,
+                           long long ld_out, float* xabs, float alpha);

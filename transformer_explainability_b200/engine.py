@@ -31,8 +31,11 @@ def vit_config(img_size=224, patch_size=16, in_chans=3, num_classes=1000, embed_
                        int(embed_dim * mlp_ratio), int(bool(distilled)), eps_block, eps_final)
 
 
-class ViTEngine:
-    """Runs ``generate_LRP(method='transformer_attribution')`` for batches of independent inputs."""
+class _Engine:
+    """Host state the ViT and BERT engines share: the flat frozen-weight buffer described by the library's weight table, the
+    derived tensor-core weight copies, and the workspace of the last shape.  ``_prefix`` names the model's C entry points."""
+    _prefix = None
+    _optional = ()                  # weight names a state_dict may leave out (zeros)
 
     def __init__(self, cfg, state_dict=None, device=None, flags=0):
         if not torch.cuda.is_available():
@@ -42,50 +45,48 @@ class ViTEngine:
         self.cfg = cfg
         self.device = torch.device(device if device is not None else "cuda:%d" % torch.cuda.current_device())
         self.flags = flags
-        n = check(self.lib.te_vit_num_weights(ctypes.byref(cfg)), "te_vit_num_weights")
-        self.weight_table = []
-        for i in range(n):
-            self.weight_table.append((self.lib.te_vit_weight_name(ctypes.byref(cfg), i).decode(),
-                                      self.lib.te_vit_weight_numel(ctypes.byref(cfg), i),
-                                      self.lib.te_vit_weight_offset(ctypes.byref(cfg), i)))
-        total = check(self.lib.te_vit_weight_total(ctypes.byref(cfg)), "te_vit_weight_total")
+        c = ctypes.byref(cfg)
+        n = check(self._fn("num_weights")(c), self._prefix + "num_weights")
+        self.weight_table = [(self._fn("weight_name")(c, i).decode(), self._fn("weight_numel")(c, i),
+                              self._fn("weight_offset")(c, i)) for i in range(n)]
+        total = check(self._fn("weight_total")(c), self._prefix + "weight_total")
         self.weights = torch.zeros(total, dtype=torch.float32, device=self.device)
         self.derived = None                      # tensor-core weight copies, built on demand
         self._ws = None
-        self._ws_batch = 0
-        self.tokens = (cfg.img_size // cfg.patch_size) ** 2 + (2 if cfg.distilled else 1)
-        self.prefix = 2 if cfg.distilled else 1
-        self.last_batch = 0
+        self._ws_key = None
         if state_dict is not None:
             self.load_state_dict(state_dict)
+
+    def _fn(self, name):
+        return getattr(self.lib, self._prefix + name)
 
     # ---- weights ------------------------------------------------------------------------------
     @_on_engine_device
     def load_state_dict(self, sd):
-        """Pack a reference-keyed ``state_dict`` (timm ViT names) into the flat device buffer."""
+        """Pack a reference-keyed ``state_dict`` into the flat device buffer."""
         host = torch.zeros(self.weights.numel(), dtype=torch.float32)
         for name, numel, off in self.weight_table:
             if name not in sd:
-                if name.endswith("qkv.bias"):
-                    continue                          # qkv_bias=False models: zeros
+                if name.endswith(self._optional):
+                    continue
                 raise KeyError("state_dict is missing %r" % name)
             t = sd[name].detach().to(torch.float32).reshape(-1).cpu()
             if t.numel() != numel:
                 raise ValueError("%s: expected %d values, got %d" % (name, numel, t.numel()))
             host[off:off + numel] = t
-        self.weights.copy_(host, non_blocking=False)
+        self.weights.copy_(host)
         self.derived = None
 
     @_on_engine_device
     def _derived(self, flags):
-        """W+/W-/W+^T/W-^T TF32 copies for the tensor-core z+ path (built once per weight load)."""
+        """W+/W-/W+^T/W-^T TF32 copies for the tensor-core paths (built once per weight load)."""
         if not (flags & (_lib.FLAG_TENSOR_CORES | _lib.FLAG_RULES_LRP_TC)):
             return None
         if self.derived is None:
-            n = check(self.lib.te_vit_derived_total(ctypes.byref(self.cfg)), "te_vit_derived_total")
+            n = check(self._fn("derived_total")(ctypes.byref(self.cfg)), self._prefix + "derived_total")
             self.derived = torch.empty(n, dtype=torch.float32, device=self.device)
-            check(self.lib.te_vit_prepare_derived(ctypes.byref(self.cfg), ptr(self.weights), ptr(self.derived),
-                                                  self._stream()), "te_vit_prepare_derived")
+            check(self._fn("prepare_derived")(ctypes.byref(self.cfg), ptr(self.weights), ptr(self.derived), self._stream()),
+                  self._prefix + "prepare_derived")
         return self.derived
 
     def broadcast_weights(self, src=0, group=None):
@@ -93,29 +94,73 @@ class ViTEngine:
         import torch.distributed as dist
         dist.broadcast(self.weights, src=src, group=group)
 
-    # ---- workspace ----------------------------------------------------------------------------
-    def workspace_bytes(self, batch):
-        return check(self.lib.te_vit_workspace_bytes(ctypes.byref(self.cfg), batch), "te_vit_workspace_bytes")
+    # ---- workspace: shape = (batch,) for ViT, (batch, seq) for BERT -----------------------------
+    def _workspace_bytes(self, *shape):
+        return check(self._fn("workspace_bytes")(ctypes.byref(self.cfg), *shape), self._prefix + "workspace_bytes")
 
-    def _workspace(self, batch):
-        if self._ws is None or self._ws_batch != batch:
+    def _shaped_workspace(self, *shape):
+        if self._ws is None or self._ws_key != shape:
             self._ws = None
-            nbytes = self.workspace_bytes(batch)
-            self._ws = torch.empty(nbytes // 4, dtype=torch.float32, device=self.device)
-            self._ws_batch = batch
+            self._ws = torch.empty(self._workspace_bytes(*shape) // 4, dtype=torch.float32, device=self.device)
+            self._ws_key = shape
         return self._ws
 
-    def max_chunk(self, limit=None, reserve_bytes=4 << 30):
-        """Largest per-call batch whose workspace fits in free HBM (activations of all blocks are kept)."""
+    def _max_batch(self, limit, reserve_bytes, *rest):
         free, _ = torch.cuda.mem_get_info(self.device)
         if self._ws is not None:
             free += self._ws.numel() * 4
-        per = self.workspace_bytes(2) - self.workspace_bytes(1)
+        per = self._workspace_bytes(2, *rest) - self._workspace_bytes(1, *rest)
         b = max(1, int((free - reserve_bytes) // max(per, 1)))
         return min(b, limit) if limit else b
 
     def _stream(self):
         return ctypes.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+
+    def _index_tensor(self, index, b):
+        if index is None:
+            return torch.full((b,), -1, dtype=torch.int32, device=self.device)
+        t = torch.as_tensor(index, device=self.device).reshape(-1).to(torch.int32)
+        if t.numel() == 1 and b > 1:
+            t = t.expand(b)
+        if t.numel() != b:
+            raise ValueError("index must have one entry per sample")
+        return t.contiguous().clone()
+
+    def _view(self, name, layer, *shape):
+        """The strided view of workspace tensor ``name`` that ``<prefix>tensor`` describes."""
+        ws = self._shaped_workspace(*shape)
+        p = ctypes.c_void_p()
+        dims = (ctypes.c_longlong * 4)()
+        strides = (ctypes.c_longlong * 4)()
+        check(self._fn("tensor")(ctypes.byref(self.cfg), *shape, ptr(ws), name.encode(), layer, ctypes.byref(p), dims, strides),
+              self._prefix + "tensor")
+        off = (p.value - ws.data_ptr()) // 4
+        nd = 4
+        while nd > 2 and dims[nd - 1] == 1:
+            nd -= 1
+        return torch.as_strided(ws, [int(dims[i]) for i in range(nd)], [int(strides[i]) for i in range(nd)], off)
+
+
+class ViTEngine(_Engine):
+    """Runs ``generate_LRP(method='transformer_attribution')`` for batches of independent inputs."""
+    _prefix = "te_vit_"
+    _optional = ("qkv.bias",)       # qkv_bias=False models: zeros
+
+    def __init__(self, cfg, state_dict=None, device=None, flags=0):
+        super().__init__(cfg, state_dict, device, flags)
+        self.tokens = (cfg.img_size // cfg.patch_size) ** 2 + (2 if cfg.distilled else 1)
+        self.prefix = 2 if cfg.distilled else 1
+        self.last_batch = 0
+
+    def workspace_bytes(self, batch):
+        return self._workspace_bytes(batch)
+
+    def _workspace(self, batch):
+        return self._shaped_workspace(batch)
+
+    def max_chunk(self, limit=None, reserve_bytes=4 << 30):
+        """Largest per-call batch whose workspace fits in free HBM (activations of all blocks are kept)."""
+        return self._max_batch(limit, reserve_bytes)
 
     # ---- the three calls ------------------------------------------------------------------------
     @_on_engine_device
@@ -147,9 +192,9 @@ class ViTEngine:
         ws = self._workspace(b)
         c, s = self.cfg.in_chans, self.cfg.img_size
         out = torch.empty((b, c, s, s) if per_channel else (b, s, s), dtype=torch.float32, device=self.device)
-        check(self.lib.te_vit_relprop_pixels_ex(ctypes.byref(self.cfg), ptr(self.weights), ptr(images), b, fl,
-                                                None if per_channel else ptr(out), ptr(out) if per_channel else None,
-                                                ptr(ws), ws.numel() * 4, self._stream()), "te_vit_relprop_pixels_ex")
+        check(self.lib.te_vit_relprop_pixels(ctypes.byref(self.cfg), ptr(self.weights), ptr(images), b, fl,
+                                             None if per_channel else ptr(out), ptr(out) if per_channel else None,
+                                             ptr(ws), ws.numel() * 4, self._stream()), "te_vit_relprop_pixels")
         return out
 
     @_on_engine_device
@@ -164,9 +209,9 @@ class ViTEngine:
         idx = self._index_tensor(index, b)
         maps = torch.empty(b, self.tokens - self.prefix, dtype=torch.float32, device=self.device)
         fl = self.flags if flags is None else flags
-        check(self.lib.te_vit_attribute_alpha(ctypes.byref(self.cfg), ptr(self.weights), ptr(self._derived(fl)), b, ptr(idx),
-                                              int(start_layer), float(alpha), fl, ptr(maps), ptr(ws), ws.numel() * 4,
-                                              self._stream()), "te_vit_attribute_alpha")
+        check(self.lib.te_vit_attribute(ctypes.byref(self.cfg), ptr(self.weights), ptr(self._derived(fl)), b, ptr(idx),
+                                        int(start_layer), float(alpha), fl, ptr(maps), ptr(ws), ws.numel() * 4, self._stream()),
+              "te_vit_attribute")
         return maps, idx
 
     @_on_engine_device
@@ -250,30 +295,9 @@ class ViTEngine:
             return st["maps"], st["idx"], st["logits"]
         return st["maps"], st["idx"]
 
-    def _index_tensor(self, index, b):
-        if index is None:
-            return torch.full((b,), -1, dtype=torch.int32, device=self.device)
-        t = torch.as_tensor(index, device=self.device).reshape(-1).to(torch.int32)
-        if t.numel() == 1 and b > 1:
-            t = t.expand(b)
-        if t.numel() != b:
-            raise ValueError("index must have one entry per sample")
-        return t.contiguous().clone()
-
     # ---- accessors (get_attn / get_attn_gradients / get_attn_cam ..., ViT_LRP.py:102-130) ---------
     def tensor(self, name, layer=0):
-        b = self.last_batch
-        ws = self._workspace(b)
-        p = ctypes.c_void_p()
-        dims = (ctypes.c_longlong * 4)()
-        strides = (ctypes.c_longlong * 4)()
-        check(self.lib.te_vit_tensor(ctypes.byref(self.cfg), b, ptr(ws), name.encode(), layer, ctypes.byref(p), dims,
-                                     strides), "te_vit_tensor")
-        off = (p.value - ws.data_ptr()) // 4
-        nd = 4
-        while nd > 2 and dims[nd - 1] == 1:
-            nd -= 1
-        return torch.as_strided(ws, [int(dims[i]) for i in range(nd)], [int(strides[i]) for i in range(nd)], off)
+        return self._view(name, layer, self.last_batch)
 
 
 def bert_config(vocab_size=30522, max_position_embeddings=512, type_vocab_size=2, hidden_size=768,
@@ -284,79 +308,23 @@ def bert_config(vocab_size=30522, max_position_embeddings=512, type_vocab_size=2
                         num_attention_heads, intermediate_size, num_labels, layer_norm_eps)
 
 
-class BertEngine:
+class BertEngine(_Engine):
     """``Generator.generate_LRP`` (BERT_explainability/modules/BERT/ExplanationGenerator.py:28-59) for batches of
     independent sequences of one length."""
+    _prefix = "te_bert_"
 
     def __init__(self, cfg, state_dict=None, device=None, flags=0):
-        if not torch.cuda.is_available():
-            raise RuntimeError("transformer_explainability_b200 needs a CUDA device (H100, sm_90a); "
-                               "there is no CPU fallback")
-        self.lib = _lib.load()
-        self.cfg = cfg
-        self.device = torch.device(device if device is not None else "cuda:%d" % torch.cuda.current_device())
-        self.flags = flags
-        n = check(self.lib.te_bert_num_weights(ctypes.byref(cfg)), "te_bert_num_weights")
-        self.weight_table = [(self.lib.te_bert_weight_name(ctypes.byref(cfg), i).decode(),
-                              self.lib.te_bert_weight_numel(ctypes.byref(cfg), i),
-                              self.lib.te_bert_weight_offset(ctypes.byref(cfg), i)) for i in range(n)]
-        total = check(self.lib.te_bert_weight_total(ctypes.byref(cfg)), "te_bert_weight_total")
-        self.weights = torch.zeros(total, dtype=torch.float32, device=self.device)
-        self.derived = None
-        self._ws = None
-        self._ws_key = None
+        super().__init__(cfg, state_dict, device, flags)
         self.last = (0, 0)
-        if state_dict is not None:
-            self.load_state_dict(state_dict)
-
-    @_on_engine_device
-    def load_state_dict(self, sd):
-        host = torch.zeros(self.weights.numel(), dtype=torch.float32)
-        for name, numel, off in self.weight_table:
-            if name not in sd:
-                raise KeyError("state_dict is missing %r" % name)
-            t = sd[name].detach().to(torch.float32).reshape(-1).cpu()
-            if t.numel() != numel:
-                raise ValueError("%s: expected %d values, got %d" % (name, numel, t.numel()))
-            host[off:off + numel] = t
-        self.weights.copy_(host)
-        self.derived = None
-
-    def broadcast_weights(self, src=0, group=None):
-        import torch.distributed as dist
-        dist.broadcast(self.weights, src=src, group=group)
-
-    @_on_engine_device
-    def _derived(self, flags):
-        if not (flags & (_lib.FLAG_TENSOR_CORES | _lib.FLAG_RULES_LRP_TC)):
-            return None
-        if self.derived is None:
-            n = check(self.lib.te_bert_derived_total(ctypes.byref(self.cfg)), "te_bert_derived_total")
-            self.derived = torch.empty(n, dtype=torch.float32, device=self.device)
-            check(self.lib.te_bert_prepare_derived(ctypes.byref(self.cfg), ptr(self.weights), ptr(self.derived),
-                                                   self._stream()), "te_bert_prepare_derived")
-        return self.derived
 
     def workspace_bytes(self, batch, seq):
-        return check(self.lib.te_bert_workspace_bytes(ctypes.byref(self.cfg), batch, seq), "te_bert_workspace_bytes")
+        return self._workspace_bytes(batch, seq)
 
     def _workspace(self, batch, seq):
-        if self._ws is None or self._ws_key != (batch, seq):
-            self._ws = None
-            self._ws = torch.empty(self.workspace_bytes(batch, seq) // 4, dtype=torch.float32, device=self.device)
-            self._ws_key = (batch, seq)
-        return self._ws
+        return self._shaped_workspace(batch, seq)
 
     def max_chunk(self, seq, limit=None, reserve_bytes=4 << 30):
-        free, _ = torch.cuda.mem_get_info(self.device)
-        if self._ws is not None:
-            free += self._ws.numel() * 4
-        per = self.workspace_bytes(2, seq) - self.workspace_bytes(1, seq)
-        b = max(1, int((free - reserve_bytes) // max(per, 1)))
-        return min(b, limit) if limit else b
-
-    def _stream(self):
-        return ctypes.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+        return self._max_batch(limit, reserve_bytes, seq)
 
     def _ids(self, input_ids, attention_mask):
         if not input_ids.is_cuda and input_ids.numel() and (int(input_ids.min()) < 0 or
@@ -388,12 +356,12 @@ class BertEngine:
         if b <= 0:
             raise RuntimeError("attribute() needs a preceding forward()")
         ws = self._workspace(b, s)
-        idx = ViTEngine._index_tensor(self, index, b)
+        idx = self._index_tensor(index, b)
         maps = torch.empty(b, s, dtype=torch.float32, device=self.device)
         fl = self.flags if flags is None else flags
-        check(self.lib.te_bert_attribute_alpha(ctypes.byref(self.cfg), ptr(self.weights), ptr(self._derived(fl)), b, s,
-                                               ptr(idx), int(start_layer), float(alpha), fl, ptr(maps), ptr(ws),
-                                               ws.numel() * 4, self._stream()), "te_bert_attribute_alpha")
+        check(self.lib.te_bert_attribute(ctypes.byref(self.cfg), ptr(self.weights), ptr(self._derived(fl)), b, s, ptr(idx),
+                                         int(start_layer), float(alpha), fl, ptr(maps), ptr(ws), ws.numel() * 4,
+                                         self._stream()), "te_bert_attribute")
         return maps, idx
 
     @_on_engine_device
@@ -403,7 +371,7 @@ class BertEngine:
         B, S = ids.shape
         chunk = min(B, chunk or self.max_chunk(S, limit=B))
         maps = torch.empty(B, S, dtype=torch.float32, device=self.device)
-        idx_all = ViTEngine._index_tensor(self, index, B)
+        idx_all = self._index_tensor(index, B)
         logits = torch.empty(B, self.cfg.num_labels, dtype=torch.float32, device=self.device) if return_logits else None
         fl = self.flags if flags is None else flags
         derived = self._derived(fl)
@@ -420,15 +388,4 @@ class BertEngine:
         return maps, idx_all
 
     def tensor(self, name, layer=0):
-        b, s = self.last
-        ws = self._workspace(b, s)
-        p = ctypes.c_void_p()
-        dims = (ctypes.c_longlong * 4)()
-        strides = (ctypes.c_longlong * 4)()
-        check(self.lib.te_bert_tensor(ctypes.byref(self.cfg), b, s, ptr(ws), name.encode(), layer, ctypes.byref(p), dims,
-                                      strides), "te_bert_tensor")
-        off = (p.value - ws.data_ptr()) // 4
-        nd = 4
-        while nd > 2 and dims[nd - 1] == 1:
-            nd -= 1
-        return torch.as_strided(ws, [int(dims[i]) for i in range(nd)], [int(strides[i]) for i in range(nd)], off)
+        return self._view(name, layer, *self.last)

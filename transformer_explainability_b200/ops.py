@@ -76,6 +76,60 @@ def _tc_scratch(w, device, s=0, operand=0, split=None):
     return torch.empty(n, device=device, dtype=torch.float32)
 
 
+# ---- Linear GEMMs: te_linear_forward / te_linear_backward run the kernel family named or return TE_ERR_UNSUPPORTED ----------
+LINEAR_FAMILIES = {
+    "simt": 0,
+    "3xtf32": _lib.FLAG_LINEAR_TENSOR_CORES,
+    "f16_split": _lib.FLAG_LINEAR_TENSOR_CORES | _lib.FLAG_LINEAR_F16_SPLIT,          # forward only
+    "tf32": _lib.FLAG_LINEAR_TENSOR_CORES | _lib.FLAG_BACKWARD_TF32,                  # backward only
+    "f16": _lib.FLAG_LINEAR_TENSOR_CORES | _lib.FLAG_BACKWARD_F16,                    # backward only
+}
+LINEAR_EPI = {"store": 0, "bias": 1, "bias_gelu": 2, "bias_add": 3, "gelu_bwd": 4}
+ATTN_EPI = {"store": 0, "mul": 1, "sd": 2, "softmax": 3}
+# where the convenience functions fall back to when a family does not take the shape (every shape the fp16 kernels take,
+# 3xTF32 takes as well)
+_STEP_DOWN = {"f16_split": "3xtf32", "f16": "3xtf32", "tf32": "3xtf32", "3xtf32": "simt"}
+
+
+def _linear_call(fn, args, epi, family, fall_back):
+    """fn(*args, epi, the family's flags, stream); with fall_back a family that returns TE_ERR_UNSUPPORTED steps down."""
+    while True:
+        status = fn(*args, LINEAR_EPI[epi], LINEAR_FAMILIES[family], _stream())
+        if not (fall_back and status == _lib.TE_ERR_UNSUPPORTED):
+            return check(status, fn.__name__)
+        family = _STEP_DOWN[family]
+
+
+def _linear_forward(x, w, bias, e0, epi, family, fall_back):
+    """x [rows,in] -> (y [rows,out], y2 or None), see linear_forward_epi."""
+    rows, K, N = x.shape[0], x.shape[1], w.shape[0]
+    y = torch.empty(rows, N, device=x.device, dtype=torch.float32)
+    y2 = torch.empty_like(y) if epi in ("bias_gelu", "bias_add") else None
+    scratch = _tc_scratch(w, x.device, split=(rows, K, False) if family == "f16_split" else None) if family != "simt" else None
+    _linear_call(_lib.load().te_linear_forward, (ptr(x), ptr(w), ptr(bias), ptr(e0), ptr(y), ptr(y2), ptr(scratch), rows, K, N),
+                 epi, family, fall_back)
+    return y, y2
+
+
+def _linear_backward(dy, w, e0, epi, family, fall_back):
+    """dy [rows,out] -> dx [rows,in], see linear_backward_epi."""
+    rows, K, N = dy.shape[0], w.shape[0], w.shape[1]
+    dx = torch.empty(rows, N, device=dy.device, dtype=torch.float32)
+    scratch = _tc_scratch(w, dy.device, split=(rows, K, True) if family == "f16" else None) if family != "simt" else None
+    _linear_call(_lib.load().te_linear_backward, (ptr(dy), ptr(w), ptr(e0), ptr(dx), ptr(scratch), rows, N, K), epi, family,
+                 fall_back)
+    return dx
+
+
+def _linear_backward_any(what, dy, w, family):
+    """dy [...,out] -> dx [...,in] on the family, falling back where it does not take the shape."""
+    _req(dy, w)
+    if w.dim() != 2 or dy.shape[-1] != w.shape[0]:
+        raise ValueError("%s: dy [...,out], w [out,in] expected" % what)
+    dx = _linear_backward(dy.reshape(-1, dy.shape[-1]), w, None, "store", family, True)
+    return dx.view(*dy.shape[:-1], w.shape[1])
+
+
 @_on_device
 def linear_forward(x, w, bias=None, tensor_cores=False, f16_split=False):
     """y = x W^T + b.  tensor_cores: fp32-grade 3xTF32 split on the tensor cores (shapes that do not qualify fall back);
@@ -83,14 +137,9 @@ def linear_forward(x, w, bias=None, tensor_cores=False, f16_split=False):
     _req(x, w, bias)
     if w.dim() != 2 or x.shape[-1] != w.shape[1] or (bias is not None and bias.numel() != w.shape[0]):
         raise ValueError("linear_forward: x [...,in], w [out,in], bias [out] expected")
-    rows = x.numel() // x.shape[-1]
-    y = torch.empty(*x.shape[:-1], w.shape[0], device=x.device, dtype=torch.float32)
-    scratch = _tc_scratch(w, x.device, split=(rows, x.shape[-1], False) if f16_split else None) if tensor_cores else None
-    flags = (_lib.FLAG_LINEAR_TENSOR_CORES if tensor_cores else 0) | (_lib.FLAG_LINEAR_F16_SPLIT if f16_split else 0)
-    check(_lib.load().te_linear_forward_ex(ptr(x), ptr(w), ptr(bias), ptr(y), ptr(scratch), rows, x.shape[-1], w.shape[0],
-                                           flags, _stream()),
-          "te_linear_forward_ex")
-    return y
+    family = ("f16_split" if f16_split else "3xtf32") if tensor_cores else "simt"
+    y, _ = _linear_forward(x.reshape(-1, x.shape[-1]), w, bias, None, "bias", family, True)
+    return y.view(*x.shape[:-1], w.shape[0])
 
 
 @_on_device
@@ -110,61 +159,23 @@ def f16_block_split(x):
 @_on_device
 def linear_backward(dy, w, tensor_cores=False):
     """dx = dy W  (activation gradient of a Linear; no dW on this path)."""
-    _req(dy, w)
-    if w.dim() != 2 or dy.shape[-1] != w.shape[0]:
-        raise ValueError("linear_backward: dy [...,out], w [out,in] expected")
-    rows = dy.numel() // dy.shape[-1]
-    dx = torch.empty(*dy.shape[:-1], w.shape[1], device=dy.device, dtype=torch.float32)
-    scratch = _tc_scratch(w, dy.device) if tensor_cores else None
-    check(_lib.load().te_linear_backward_ex(ptr(dy), ptr(w), ptr(dx), ptr(scratch), rows, w.shape[1], w.shape[0],
-                                            _lib.FLAG_LINEAR_TENSOR_CORES if tensor_cores else 0, _stream()),
-          "te_linear_backward_ex")
-    return dx
+    return _linear_backward_any("linear_backward", dy, w, "3xtf32" if tensor_cores else "simt")
 
 
 @_on_device
 def linear_backward_f16(dy, w):
     """dx = dy W as a single-pass fp16 GEMM (block-scaled fp16 gradient, row-scaled fp16 weights; TE_FLAG_BACKWARD_F16)."""
-    _req(dy, w)
-    if w.dim() != 2 or dy.shape[-1] != w.shape[0]:
-        raise ValueError("linear_backward_f16: dy [...,out], w [out,in] expected")
-    rows = dy.numel() // dy.shape[-1]
-    dx = torch.empty(*dy.shape[:-1], w.shape[1], device=dy.device, dtype=torch.float32)
-    scratch = _tc_scratch(w, dy.device, split=(rows, w.shape[0], True))
-    check(_lib.load().te_linear_backward_ex(ptr(dy), ptr(w), ptr(dx), ptr(scratch), rows, w.shape[1], w.shape[0],
-                                            _lib.FLAG_LINEAR_TENSOR_CORES | _lib.FLAG_BACKWARD_F16, _stream()),
-          "te_linear_backward_ex")
-    return dx
+    return _linear_backward_any("linear_backward_f16", dy, w, "f16")
 
 
 @_on_device
 def linear_backward_tf32(dy, w):
     """dx = dy W as a single-pass TF32 wgmma GEMM (what TE_FLAG_BACKWARD_TF32 selects)."""
-    _req(dy, w)
-    if w.dim() != 2 or dy.shape[-1] != w.shape[0]:
-        raise ValueError("linear_backward_tf32: dy [...,out], w [out,in] expected")
-    rows = dy.numel() // dy.shape[-1]
-    dx = torch.empty(*dy.shape[:-1], w.shape[1], device=dy.device, dtype=torch.float32)
-    scratch = _tc_scratch(w, dy.device)
-    check(_lib.load().te_linear_backward_ex(ptr(dy), ptr(w), ptr(dx), ptr(scratch), rows, w.shape[1], w.shape[0],
-                                            _lib.FLAG_LINEAR_TENSOR_CORES | _lib.FLAG_BACKWARD_TF32, _stream()),
-          "te_linear_backward_ex")
-    return dx
+    return _linear_backward_any("linear_backward_tf32", dy, w, "tf32")
 
 
 # ---- diagnostic wrappers of the kernels (include/te_b200.h: "Diagnostic entry points"): no fall-back, a shape the requested
 # kernel does not take raises TeError with status TE_ERR_UNSUPPORTED -------------------------------------------------------
-LINEAR_FAMILIES = {
-    "simt": 0,
-    "3xtf32": _lib.FLAG_LINEAR_TENSOR_CORES,
-    "f16_split": _lib.FLAG_LINEAR_TENSOR_CORES | _lib.FLAG_LINEAR_F16_SPLIT,          # forward only
-    "tf32": _lib.FLAG_LINEAR_TENSOR_CORES | _lib.FLAG_BACKWARD_TF32,                  # backward only
-    "f16": _lib.FLAG_LINEAR_TENSOR_CORES | _lib.FLAG_BACKWARD_F16,                    # backward only
-}
-LINEAR_EPI = {"store": 0, "bias": 1, "bias_gelu": 2, "bias_add": 3, "gelu_bwd": 4}
-ATTN_EPI = {"store": 0, "mul": 1, "sd": 2, "softmax": 3}
-
-
 @_on_device
 def linear_forward_epi(x, w, bias=None, e0=None, epi="bias", family="simt"):
     """y = x W^T (+ bias) with a fused epilogue on the kernel family named (LINEAR_FAMILIES) -> (y, y2); y2 is None unless
@@ -172,14 +183,7 @@ def linear_forward_epi(x, w, bias=None, e0=None, epi="bias", family="simt"):
     _req(x, w, bias, e0)
     if x.dim() != 2 or w.dim() != 2 or w.shape[1] != x.shape[1] or (e0 is not None and e0.shape != (x.shape[0], w.shape[0])):
         raise ValueError("linear_forward_epi: x [rows,in], w [out,in], e0 [rows,out] expected")
-    rows, K, N = x.shape[0], x.shape[1], w.shape[0]
-    flags = LINEAR_FAMILIES[family]
-    y = torch.empty(rows, N, device=x.device, dtype=torch.float32)
-    y2 = torch.empty_like(y) if epi in ("bias_gelu", "bias_add") else None
-    scratch = _tc_scratch(w, x.device, split=(rows, K, False) if family == "f16_split" else None) if flags else None
-    check(_lib.load().te_linear_forward_epi(ptr(x), ptr(w), ptr(bias), ptr(e0), ptr(y), ptr(y2), ptr(scratch), rows, K, N,
-                                            LINEAR_EPI[epi], flags, _stream()), "te_linear_forward_epi")
-    return y, y2
+    return _linear_forward(x, w, bias, e0, epi, family, False)
 
 
 @_on_device
@@ -188,13 +192,7 @@ def linear_backward_epi(dy, w, e0=None, epi="store", family="simt"):
     _req(dy, w, e0)
     if dy.dim() != 2 or w.dim() != 2 or dy.shape[1] != w.shape[0] or (e0 is not None and e0.shape != (dy.shape[0], w.shape[1])):
         raise ValueError("linear_backward_epi: dy [rows,out], w [out,in], e0 [rows,in] expected")
-    rows, K, N = dy.shape[0], w.shape[0], w.shape[1]
-    flags = LINEAR_FAMILIES[family]
-    dx = torch.empty(rows, N, device=dy.device, dtype=torch.float32)
-    scratch = _tc_scratch(w, dy.device, split=(rows, K, True) if family == "f16" else None) if flags else None
-    check(_lib.load().te_linear_backward_epi(ptr(dy), ptr(w), ptr(e0), ptr(dx), ptr(scratch), rows, N, K, LINEAR_EPI[epi],
-                                             flags, _stream()), "te_linear_backward_epi")
-    return dx
+    return _linear_backward(dy, w, e0, epi, family, False)
 
 
 @_on_device
@@ -283,10 +281,9 @@ def linear_relprop(x, w, r, tensor_cores=False, y=None, bias=None, bf16=False, v
     out = torch.empty_like(x)
     if variant == "lrp_tc":
         scratch = _tc_scratch(w, x.device, s=rows * w.shape[0])
-        check(_lib.load().te_linear_relprop_alpha(ptr(x), ptr(w), None, None, ptr(r), ptr(out), ptr(scratch), rows,
-                                                  x.shape[-1], w.shape[0], float(alpha),
-                                                  _lib.FLAG_RULES_LRP | _lib.FLAG_RULES_LRP_TC, _stream()),
-              "te_linear_relprop_alpha")
+        check(_lib.load().te_linear_relprop(ptr(x), ptr(w), None, None, ptr(r), ptr(out), ptr(scratch), rows, x.shape[-1],
+                                            w.shape[0], float(alpha), _lib.FLAG_RULES_LRP | _lib.FLAG_RULES_LRP_TC, _stream()),
+              "te_linear_relprop")
         return out
     if tensor_cores:
         scratch = _tc_scratch(w, x.device, s=rows * w.shape[0], operand=x.numel())
@@ -303,10 +300,10 @@ def linear_relprop(x, w, r, tensor_cores=False, y=None, bias=None, bf16=False, v
         flags, y = _lib.FLAG_RULES_LRP, None
     elif variant != "ours":
         raise ValueError("variant: 'ours', 'lrp' or 'lrp_tc'")
-    # y None: the two-pass rule (te_linear_relprop); y given: the single-pass form (te_linear_relprop_ex)
-    check(_lib.load().te_linear_relprop_alpha(ptr(x), ptr(w), ptr(bias) if y is not None else None, ptr(y), ptr(r), ptr(out),
-                                              ptr(scratch), rows, x.shape[-1], w.shape[0], float(alpha), flags, _stream()),
-          "te_linear_relprop_alpha")
+    # y None: the two-pass rule; y given: the single-pass form
+    check(_lib.load().te_linear_relprop(ptr(x), ptr(w), ptr(bias) if y is not None else None, ptr(y), ptr(r), ptr(out),
+                                        ptr(scratch), rows, x.shape[-1], w.shape[0], float(alpha), flags, _stream()),
+          "te_linear_relprop")
     return out
 
 
