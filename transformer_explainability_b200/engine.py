@@ -2,8 +2,15 @@
 
 The engine is the CUDA replacement for the stateful hook machinery of the reference
 (``modules/layers_ours.py:16-27`` forward hooks, ``retain_graph=True`` autograd graph): it owns one
-flat fp32 weight buffer (the unit of the single NCCL broadcast) and one activation workspace per
-stream, and issues O(1) launches per block per BATCH through the C ABI.
+flat fp32 weight buffer (the unit of the single NCCL broadcast), the tensor-core copies derived from it, and one
+activation workspace (of the last shape), and issues O(1) launches per block per BATCH through the C ABI.
+
+Every public call launches on the caller's current stream.  Calls to one engine are ordered in the order they are
+issued, whatever their streams: each call ends by recording an event, and a call on another stream first waits on it,
+so the state the later call leaves (workspace, ``tensor()`` views, ``attribute()`` inputs) is what stays.  The
+workspace and the derived weights are marked as used by every stream that ran on them (``record_stream``), so a reshape
+never hands their memory out while another stream's work still reads it.  Calls to one engine therefore never overlap
+on the device; two engines are independent.
 """
 import ctypes
 import functools
@@ -17,11 +24,25 @@ from ._lib import TeVitConfig, check, ptr
 def _on_engine_device(fn):
     """Make the engine's device current for the duration of the call: the C library launches on the current device
     and neither it nor ``torch.cuda.current_stream(dev)`` switches devices (a model moved to ``cuda:1`` without
-    ``torch.cuda.set_device(1)`` would otherwise fail with an invalid resource handle)."""
+    ``torch.cuda.set_device(1)`` would otherwise fail with an invalid resource handle).  The call is ordered after the
+    engine's previous call on any stream (the module docstring); not while a CUDA graph is being captured, where an
+    event of outside work cannot be waited on and the graph's own order applies."""
     @functools.wraps(fn)
     def wrapped(self, *args, **kwargs):
         with torch.cuda.device(self.device):
-            return fn(self, *args, **kwargs)
+            stream = torch.cuda.current_stream(self.device)
+            if torch.cuda.is_current_stream_capturing():
+                return fn(self, *args, **kwargs)
+            if self._done_stream is not None and self._done_stream != stream:
+                stream.wait_event(self._done)
+            try:
+                return fn(self, *args, **kwargs)
+            finally:
+                for t in (self._ws, self.derived):
+                    if t is not None:
+                        t.record_stream(stream)
+                self._done.record(stream)
+                self._done_stream = stream
     return wrapped
 
 
@@ -54,6 +75,8 @@ class _Engine:
         self.derived = None                      # tensor-core weight copies, built on demand
         self._ws = None
         self._ws_key = None
+        self._done = torch.cuda.Event()          # recorded at the end of every public call
+        self._done_stream = None
         if state_dict is not None:
             self.load_state_dict(state_dict)
 
@@ -75,24 +98,32 @@ class _Engine:
                 raise ValueError("%s: expected %d values, got %d" % (name, numel, t.numel()))
             host[off:off + numel] = t
         self.weights.copy_(host)
-        self.derived = None
+        self._prepare_derived()
+
+    def _prepare_derived(self):
+        """Re-derive the tensor-core copies from the weights, in place: once built, the derived buffer keeps its address,
+        so the CUDA graphs of ``explain_graphed`` that captured it stay valid after a weight reload."""
+        if self.derived is not None:
+            check(self._fn("prepare_derived")(ctypes.byref(self.cfg), ptr(self.weights), ptr(self.derived), self._stream()),
+                  self._prefix + "prepare_derived")
 
     @_on_engine_device
     def _derived(self, flags):
-        """W+/W-/W+^T/W-^T TF32 copies for the tensor-core paths (built once per weight load)."""
+        """W+/W-/W+^T/W-^T TF32 copies for the tensor-core paths (built on first use, kept current by every weight load)."""
         if not (flags & (_lib.FLAG_TENSOR_CORES | _lib.FLAG_RULES_LRP_TC)):
             return None
         if self.derived is None:
             n = check(self._fn("derived_total")(ctypes.byref(self.cfg)), self._prefix + "derived_total")
             self.derived = torch.empty(n, dtype=torch.float32, device=self.device)
-            check(self._fn("prepare_derived")(ctypes.byref(self.cfg), ptr(self.weights), ptr(self.derived), self._stream()),
-                  self._prefix + "prepare_derived")
+            self._prepare_derived()
         return self.derived
 
+    @_on_engine_device
     def broadcast_weights(self, src=0, group=None):
-        """The one collective of the path: NCCL broadcast of the flat frozen-weight buffer."""
+        """The one collective of the path: NCCL broadcast of the flat frozen-weight buffer (the derived copies follow)."""
         import torch.distributed as dist
         dist.broadcast(self.weights, src=src, group=group)
+        self._prepare_derived()
 
     # ---- workspace: shape = (batch,) for ViT, (batch, seq) for BERT -----------------------------
     def _workspace_bytes(self, *shape):
@@ -261,7 +292,8 @@ class ViTEngine(_Engine):
                       idx_in=torch.full((B,), -1, dtype=torch.int32, device=self.device),
                       idx=torch.full((B,), -1, dtype=torch.int32, device=self.device),
                       maps=torch.empty(B, self.tokens - self.prefix, dtype=torch.float32, device=self.device),
-                      logits=torch.empty(B, self.cfg.num_classes, dtype=torch.float32, device=self.device), ws=ws)
+                      logits=torch.empty(B, self.cfg.num_classes, dtype=torch.float32, device=self.device), ws=ws,
+                      derived=derived)
             st["images"].copy_(images)
 
             def run():
@@ -282,7 +314,10 @@ class ViTEngine(_Engine):
             st["graph"] = graph
             g[key] = st
         st = g[key]
-        if st["ws"] is not self._ws:                         # the workspace was re-allocated for another batch size
+        # every pointer the graph captured besides its own buffers: the weights and the derived copies are rewritten in
+        # place by a weight load, but the workspace is re-allocated for another batch size and the derived copies may
+        # have been dropped (e.g. to free memory)
+        if st["ws"] is not self._ws or st["derived"] is not self._derived(fl):
             del g[key]
             return self.explain_graphed(images, index=index, start_layer=start_layer, flags=flags,
                                         return_logits=return_logits)
