@@ -459,6 +459,35 @@ TE_API int te_eraser_reduce_inputs(const float* maps, const long long* input_ids
                                    long long* out_ids, int* out_len, void* workspace, long long workspace_bytes,
                                    void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Input preparation  (baselines/ViT/generate_visualizations.py:194-199: Resize((224, 224)) + ToTensor() on PIL images)
+ * Pillow's 8-bit bilinear resize (ImagingResample, support 1): per axis scale = in / out, fs = max(scale, 1), and for output
+ * index i, center = (i + 0.5) scale, xmin = max((int)(center - fs + 0.5), 0), n = min((int)(center + fs + 0.5), in) - xmin,
+ * weights tri((j + xmin - center + 0.5) * (1 / fs)) divided by their (double) sum, as int32 (int)(+-0.5 + w 2^22).  Each pass starts
+ * an int32 accumulator at 2^21, sums u8 * k and clips to uint8 (>= 255 << 22: 255, <= 0: 0, else >> 22); the first pass's
+ * uint8 result feeds the second.  The horizontal pass runs first, except when h > 100 w and out_h < h (Pillow 12's
+ * Image.resize then resizes vertically first).
+ * ---------------------------------------------------------------------------------------------- */
+#define TE_PREPARE_MAX_SIDE 16384
+#define TE_PREPARE_MAX_OUT 4096
+/* Host only: the table of one axis resized from in_size (1..TE_PREPARE_MAX_SIDE) to out_size (1..TE_PREPARE_MAX_OUT)
+ * samples.  Returns ksize = 2 ceil(max(in / out, 1)) + 1 (or TE_ERR_ARG); when k and bounds are given, k [out_size, ksize]
+ * receives the int32 weights (zero past n) and bounds [out_size, 2] the pairs (xmin, n). */
+TE_API int te_resize_coeffs(int in_size, int out_size, int* k, int* bounds);
+/* Workspace of te_prepare_images for `batch` images no taller than max_in_h and no wider than max_in_w. */
+TE_API long long te_prepare_images_workspace_bytes(int batch, int max_in_h, int max_in_w, int out_h, int out_w);
+/* A ragged batch of RGB uint8 images, each HWC and contiguous at byte offsets[b] of packed (device, packed_bytes long),
+ * of sizes [batch, 2] = (h, w) (host; sides 1..TE_PREPARE_MAX_SIDE), resized to out_h x out_w (1..TE_PREPARE_MAX_OUT) as
+ * Pillow's Image.resize((out_w, out_h), BILINEAR) does, bit for bit:
+ *   out01 [batch, 3, out_h, out_w]    = u8 / 255.f (IEEE division): ToTensor() of the resized image;
+ *   out_norm [batch, 3, out_h, out_w] = (out01 - mean[c]) / std[c] in fp32 (host mean / std [3], finite, std != 0).
+ * Either output may be NULL (not both).  sizes and offsets are validated before anything is launched: every image must lie
+ * inside packed, else TE_ERR_ARG.  One host-to-device copy (image descriptors and the tables of te_resize_coeffs) and two
+ * launches per batch, whatever the image sizes. */
+TE_API int te_prepare_images(const unsigned char* packed, long long packed_bytes, int batch, const int* sizes,
+                             const long long* offsets, int out_h, int out_w, const float* mean, const float* std,
+                             float* out01, float* out_norm, void* workspace, long long workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

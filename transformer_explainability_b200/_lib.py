@@ -122,6 +122,9 @@ PROTOTYPES = {
     "te_eraser_reduce_workspace_bytes": (c_ll, [c_int, c_ll, c_int]),
     "te_eraser_reduce_inputs": (c_int, [_P, _P, c_int, c_int, _P, _P, _P, _P, c_int, _P, _P, _P, c_ll, _P]),
     "te_class_probs": (c_int, [_P, c_int, c_int, _P, _P]),
+    "te_resize_coeffs": (c_int, [c_int, c_int, _P, _P]),
+    "te_prepare_images_workspace_bytes": (c_ll, [c_int, c_int, c_int, c_int, c_int]),
+    "te_prepare_images": (c_int, [_P, c_ll, c_int, _P, _P, c_int, c_int, _P, _P, _P, _P, _P, c_ll, _P]),
 }
 
 PERTURB_MAX_STEPS = 64          # TE_PERTURB_MAX_STEPS
@@ -131,6 +134,8 @@ ERASER_MAX_KS = 64              # TE_ERASER_MAX_KS
 ERASER_MAX_THRESHOLDS = 8       # TE_ERASER_MAX_THRESHOLDS
 ERASER_MAX_SELECTIONS = 64      # TE_ERASER_MAX_SELECTIONS
 ERASER_MAX_SEQ = 8192           # TE_ERASER_MAX_SEQ
+PREPARE_MAX_SIDE = 16384        # TE_PREPARE_MAX_SIDE
+PREPARE_MAX_OUT = 4096          # TE_PREPARE_MAX_OUT
 
 _lib = None
 

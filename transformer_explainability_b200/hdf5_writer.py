@@ -15,7 +15,21 @@ II.A, III.A-D, IV.A.1-2).  ``h5py.File(path)['vis'][i]`` does not depend on the 
 unchanged.  This image ships no HDF5 library at all: the emitter is checked against the specification by the independent
 reader ``read_minimal_hdf5`` (``tests/test_hdf5_writer.py``), not against libhdf5 — stated here, in DESIGN.md and in the
 test.
+
+The command is the reference script itself: it explains every image of an ImageNet validation folder and writes
+``visualizations/{method}/{vis_class}/{ablation}/results.hdf5`` (``visualizations/{method}/index_{class_id}`` for
+``--vis-class index``), the directory ``python -m transformer_explainability_b200.perturbation`` reads.
+
+    python -m transformer_explainability_b200.hdf5_writer --method transformer_attribution \\
+        --imagenet-validation-path /data/imagenet --state-dict vit_base_patch16_224.pth --batch-size 32
+
+The images are decoded on the host by PIL (the bits torchvision's ``pil_loader`` gives the reference), packed per batch
+into one pinned buffer, and resized and scaled to [0, 1] on the GPU by ``ops.prepare_images``, bit for bit
+``Resize((224, 224)) + ToTensor()`` of the reference.  Deviations from the script (DESIGN.md §1): ``--method`` is required
+(the reference's default is not among its choices); an existing ``results.hdf5`` in the target directory is replaced;
+``--vis-class index`` explains the top class, as the reference does; every sample is min-max normalised on its own.
 """
+import argparse
 import os
 import struct
 import tempfile
@@ -320,3 +334,101 @@ def compute_saliency_and_save(loader, method_dir, method, lrp=None, baselines=No
                     b, 1, data.shape[-2], data.shape[-1])
             out.append(images, vis.detach().cpu().numpy(), target.detach().cpu().numpy())
     return out.path
+
+
+# ---- command line: generate_visualizations.py ----------------------------------------------------------------------------
+METHODS = ("rollout", "lrp", "transformer_attribution", "full_lrp", "lrp_last_layer", "attn_last_layer", "attn_gradcam")
+# the façade model whose generator each method uses in generate_visualizations.py:180-192; only that one is built
+MODEL_KIND = {"rollout": "new", "attn_gradcam": "new", "lrp": "lrp", "transformer_attribution": "lrp",
+              "attn_last_layer": "lrp", "full_lrp": "orig", "lrp_last_layer": "orig"}
+
+
+def read_rgb(path):
+    """torchvision's ``pil_loader`` (``Image.open(f).convert("RGB")``), returning the decoded HWC uint8 array."""
+    from PIL import Image
+    with open(path, "rb") as f:
+        return np.array(Image.open(f).convert("RGB"))
+
+
+def pack_images(batch):
+    """Collate of (HWC uint8 RGB array, target) samples -> (packed uint8 [sum of 3 h w], sizes int32 [B, 2] = (h, w),
+    offsets int64 [B], targets int64 [B]): the images one after another in batch order, ``ops.prepare_images``' input."""
+    import torch
+    arrays = [np.ascontiguousarray(a, dtype=np.uint8) for a, _ in batch]
+    for a in arrays:
+        if a.ndim != 3 or a.shape[2] != 3:
+            raise ValueError("pack_images: HWC RGB images expected, got shape %s" % (a.shape,))
+    sizes = np.array([a.shape[:2] for a in arrays], dtype=np.int32).reshape(-1, 2)
+    offsets = np.concatenate([[0], np.cumsum([a.size for a in arrays])[:-1]]).astype(np.int64)
+    packed = torch.from_numpy(np.concatenate([a.reshape(-1) for a in arrays]))
+    targets = torch.tensor([int(t) for _, t in batch], dtype=torch.int64)
+    return packed, torch.from_numpy(sizes), torch.from_numpy(offsets), targets
+
+
+def imagenet_val_loader(path, batch_size, num_workers=4):
+    """The reference's ``ImageNet(path, split='val')`` in its sample order, decoded by ``read_rgb`` in ``num_workers``
+    processes and packed by ``pack_images`` into pinned host buffers."""
+    import torch
+    from torchvision.datasets import ImageNet
+    ds = ImageNet(path, split="val", loader=read_rgb)
+    return torch.utils.data.DataLoader(ds, batch_size=batch_size, shuffle=False, num_workers=num_workers,
+                                       collate_fn=pack_images, pin_memory=torch.cuda.is_available())
+
+
+def prepared_batches(loader, device="cuda", size=224):
+    """(images [B, 3, size, size] fp32 in [0, 1] on ``device``, targets [B]) per packed batch of ``loader``: the copy of
+    the pinned batch does not block the host, and ``ops.prepare_images`` resizes it on the device."""
+    from . import ops
+    for packed, sizes, offsets, target in loader:
+        out01, _ = ops.prepare_images(packed.to(device, non_blocking=True), sizes.numpy(), offsets.numpy(), (size, size))
+        yield out01, target
+
+
+def build_parser():
+    from .perturbation import str2bool
+    p = argparse.ArgumentParser(description="Explain an ImageNet validation folder into results.hdf5")
+    p.add_argument("--batch-size", type=int, default=1)
+    p.add_argument("--method", type=str, required=True, choices=METHODS)
+    p.add_argument("--lmd", type=float, default=10, help="accepted for compatibility; unused, as in the reference")
+    p.add_argument("--vis-class", type=str, default="top", choices=["top", "target", "index"])
+    p.add_argument("--class-id", type=int, default=0, help="names the output directory of --vis-class index")
+    for flag in ("--cls-agn", "--no-ia", "--no-fx", "--no-fgx", "--no-m", "--no-reg"):
+        p.add_argument(flag, action="store_true", default=False, help="accepted for compatibility; unused")
+    p.add_argument("--is-ablation", type=str2bool, default=False)
+    p.add_argument("--imagenet-validation-path", type=str, required=True,
+                   help="directory holding meta.bin and val/{wnid}/*.JPEG (torchvision's ImageNet layout)")
+    p.add_argument("--state-dict", type=str, default=None,
+                   help="ViT-B/16 weights (timm key names); pretrained weights are not downloaded")
+    p.add_argument("--root", type=str, default=None,
+                   help="directory holding visualizations/ (default: the current directory)")
+    p.add_argument("--num-workers", type=int, default=4, help="decoding processes")
+    return p
+
+
+def parse_args(argv=None):
+    p = build_parser()
+    args = p.parse_args(argv)
+    if args.batch_size < 1:
+        p.error("--batch-size must be at least 1")
+    if args.num_workers < 0:
+        p.error("--num-workers must not be negative")
+    return args
+
+
+def main(argv=None):
+    args = parse_args(argv)
+    from . import perturbation, segmentation
+    method_dir = perturbation.vis_method_dir(args, args.root or os.getcwd())
+    os.makedirs(method_dir, exist_ok=True)
+    if os.path.exists(os.path.join(method_dir, "results.hdf5")):
+        os.remove(os.path.join(method_dir, "results.hdf5"))
+    lrp, orig_lrp, baselines = segmentation.build_generators(args.method, args.state_dict, kind=MODEL_KIND[args.method])
+    loader = imagenet_val_loader(args.imagenet_validation_path, args.batch_size, args.num_workers)
+    path = compute_saliency_and_save(prepared_batches(loader), method_dir, args.method, lrp=lrp, baselines=baselines,
+                                     orig_lrp=orig_lrp, vis_class=args.vis_class, is_ablation=args.is_ablation)
+    print(path)
+    return path
+
+
+if __name__ == "__main__":
+    main()

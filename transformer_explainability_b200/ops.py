@@ -709,3 +709,37 @@ def eraser_reduce_inputs(maps, input_ids, lengths, piece_ranges, word_offsets, n
                                       ptr(out["ids"]), ptr(out["lengths"]), ptr(ws), ws.numel() * 4, _stream()),
           "te_eraser_reduce_inputs")
     return out
+
+
+# ---- input preparation (baselines/ViT/generate_visualizations.py: Resize((224, 224)) + ToTensor()) ---------------------------
+@_on_device
+def prepare_images(packed_u8, sizes, offsets, out_hw=(224, 224), mean=None, std=None):
+    """A ragged batch of decoded RGB images, HWC uint8 each, packed into the 1-D uint8 CUDA tensor ``packed_u8`` at byte
+    ``offsets[b]`` with ``sizes[b] = (h, w)`` (host sequences), resized to ``out_hw`` exactly as
+    ``PIL.Image.resize((w, h), BILINEAR)`` does (see include/te_b200.h: te_prepare_images).  Returns ``(out01, out_norm)``:
+    fp32 CUDA [B, 3, h, w], out01 = ``ToTensor()`` of the resized image and out_norm = (out01 - mean) / std, None unless
+    ``mean`` and ``std`` (three values each) are given."""
+    import numpy as np
+    if not (packed_u8.is_cuda and packed_u8.dtype == torch.uint8 and packed_u8.dim() == 1 and packed_u8.is_contiguous()):
+        raise ValueError("prepare_images: packed_u8 must be a contiguous 1-D uint8 CUDA tensor")
+    sz = _host_i32(sizes, "sizes", 2, op="prepare_images")
+    off = np.ascontiguousarray(np.asarray(offsets, dtype=np.int64).reshape(-1))
+    B = len(sz)
+    if B == 0 or off.shape != (B,):
+        raise ValueError("prepare_images: sizes [B, 2] and offsets [B] with B >= 1 expected")
+    if (mean is None) != (std is None) or (mean is not None and (len(mean) != 3 or len(std) != 3)):
+        raise ValueError("prepare_images: mean and std are given together, three values each")
+    oh, ow = (int(v) for v in out_hw)
+    lib = _lib.load()
+    nbytes = check(lib.te_prepare_images_workspace_bytes(B, int(sz[:, 0].max()), int(sz[:, 1].max()), oh, ow),
+                   "te_prepare_images_workspace_bytes")
+    dev = packed_u8.device
+    ws = _workspace(nbytes, dev)
+    out01 = torch.empty(B, 3, oh, ow, device=dev, dtype=torch.float32)
+    out_norm = None if mean is None else torch.empty_like(out01)
+    mean_c = None if mean is None else (_lib.c_float * 3)(*[float(m) for m in mean])
+    std_c = None if std is None else (_lib.c_float * 3)(*[float(s) for s in std])
+    host = lambda a: a.ctypes.data_as(_lib.c_void_p)      # noqa: E731
+    check(lib.te_prepare_images(ptr(packed_u8), packed_u8.numel(), B, host(sz), host(off), oh, ow, mean_c, std_c, ptr(out01),
+                                ptr(out_norm), ptr(ws), ws.numel() * 4, _stream()), "te_prepare_images")
+    return out01, out_norm

@@ -278,10 +278,11 @@ def make_experiment_dir(runs):
     return d
 
 
-def build_generators(method, state_dict=None, device="cuda"):
-    """(lrp, orig_lrp, baselines) with only the façade model ``method`` needs."""
+def build_generators(method, state_dict=None, device="cuda", kind=None):
+    """(lrp, orig_lrp, baselines) with only the façade model ``method`` needs: ``kind`` "new" (``ViT_new``), "lrp"
+    (``ViT_LRP``) or "orig" (``ViT_orig_LRP``), by default the one this evaluation uses for ``method``."""
     from .baselines.ViT.ViT_explanation_generator import LRP, Baselines
-    kind = _MODEL[method]
+    kind = kind or _MODEL[method]
     if kind == "new":
         from .baselines.ViT.ViT_new import vit_base_patch16_224 as make
     elif kind == "lrp":
