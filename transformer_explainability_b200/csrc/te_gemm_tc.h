@@ -121,6 +121,7 @@ int te_tc_bmm_nk_resid(const float* A, const float* J, const float* rowscale, fl
 
 // z+ rule contractions and the single-pass TF32 backward Linear (shapes: te_tc_gemm3x_supported)
 // xabs: scratch [rows, in] for bf16(|x|), the A operand of the bf16 single-pass S kernel
+// r / y: 16-byte-aligned bases, ldr and ldy multiples of 4 (the S kernel loads their tiles by TMA)
 int te_tc_zplus_s1(const float* x, long long ldx, float* xabs, const float* derived, const float* r, long long ldr,
                    const float* y, long long ldy, const float* bias, float* s_out, long long rows, int in_features,
                    int out_features, cudaStream_t st, bool bf16 = false, float* s16 = nullptr, float* s16_scale = nullptr,

@@ -263,15 +263,32 @@ __device__ __forceinline__ int frag_col(int tid, int j) { return 8 * (j >> 2) + 
 // ---- the kernel -----------------------------------------------------------------------------------------------------
 // The TMA problems' tensor maps, one per source (A tiles, then B tiles), and their tile grid: nz batches (the attention
 // problems' sample x head) of mtiles x ntiles tiles.
+// After the P::NMAPS stage maps come the P::EPI_MAPS maps of the epilogue operands.
+constexpr int TMA_MAPS = 5;
 struct TmaArgs {
-    CUtensorMap map[4];
+    CUtensorMap map[TMA_MAPS];
     int mtiles, ntiles, nz;
 };
 // what the consumers of a TMA problem transform in shared memory before the wgmmas read a stage (P::FIX, P::fix)
 enum { FIX_NONE = 0, FIX_A = 1, FIX_AB = 2 };
 constexpr int NTHREADS_TMA = 384, SMEM_MAX = 227 * 1024;
-// stages of a TMA problem: as many as fit next to the 1024-byte alignment slack and the barriers, at most 8
-__host__ __device__ constexpr int tma_stages(int bytes) { return (SMEM_MAX - 1024 - 128) / bytes < 8 ? (SMEM_MAX - 1024 - 128) / bytes : 8; }
+// stages of a TMA problem: as many as fit next to its epilogue buffer (epi bytes), the 1024-byte alignment slack and the
+// barriers, at most 8
+__host__ __device__ constexpr int tma_stages(int bytes, int epi) {
+    return (SMEM_MAX - 1024 - 256 - epi) / bytes < 8 ? (SMEM_MAX - 1024 - 256 - epi) / bytes : 8;
+}
+
+// ---- epilogue operands (TMA mainloop) ---------------------------------------------------------------------------------
+// A problem's P::EPI_MAPS fp32 operands of the output's shape ([rows, cols] at a row stride, e.g. R and y of the z+ S
+// kernel) are loaded per tile by the producer into an epilogue buffer behind the stages: each operand's BM x BN tile at
+// (m0, n0) as BN / 32 boxes of 32 columns x BM rows, 128-byte swizzled like an operand tile, so that a warp's float2 reads
+// of a fragment (8 rows x 32 bytes) hit every bank group at most twice.
+template <class P>
+__host__ __device__ constexpr int epi_bytes() { return P::EPI_MAPS * BM * P::BN * 4; }
+// the float2 at columns c, c + 1 (c even) of tile-local row r of the epilogue operand tile at t
+__device__ __forceinline__ float2 epi_f2(const uint8_t* t, int r, int c) {
+    return *reinterpret_cast<const float2*>(t + (c >> 5) * (BM * 128) + swz(r, (c & 31) >> 2) + (c & 3) * 4);
+}
 
 // chunk fold: tot += acc times the per-row block scale of chunk ch
 template <class P, int NA, int NR, int NT, int NTR>
@@ -322,8 +339,8 @@ __device__ __forceinline__ void reg_tile(const P& p, uint8_t* smem, int col_fast
         fence_proxy_async();
         __syncthreads();
     }
-    if constexpr (P::CHUNK > 0) p.epilogue(tot, m0, n0, z, tid);
-    else p.epilogue(acc, m0, n0, z, tid);
+    if constexpr (P::CHUNK > 0) p.epilogue(tot, m0, n0, z, tid, nullptr);
+    else p.epilogue(acc, m0, n0, z, tid, nullptr);
 }
 
 // TMA mainloop on persistent CTAs.  Warpgroups 0 and 1 (threads 0..255, the same rows and fragments as the register
@@ -337,22 +354,29 @@ __device__ __forceinline__ void reg_tile(const P& p, uint8_t* smem, int col_fast
 // P::FIX: the stage lands raw and the consumers run P::fix on it (TF32 rounding, hi / lo split, transposition of MN-major
 // sources): FIX_A, each consumer warpgroup its own 64 rows of A behind its own named barrier; FIX_AB, in addition the B tiles
 // shared by both warpgroups, their rows split over all 256 consumer threads, behind one 256-thread named barrier.
+// P::EPI_MAPS > 0: the producer also loads the tile's epilogue operands into the epilogue buffer behind the stages, with its
+// own full barrier (expect_tx) and empty barrier (one arrive per consumer warp after the epilogue).  It issues them once the
+// first min(S, kb) k-blocks of the tile are issued, where it would next wait for a stage the consumers free only after the
+// previous tile's epilogue, so the one buffer costs the stage ring no prefetch; the operands land during the mainloop.
 template <class P>
 __device__ __forceinline__ void tma_tiles(const P& p, const TmaArgs& ta, uint8_t* smem) {
     using L = typename P::L;
     constexpr int NR = P::BN / 2;
     constexpr int NA = P::PRODS::NACC;
-    constexpr int STAGE = L::BYTES, S = tma_stages(STAGE);
+    constexpr int STAGE = L::BYTES, EPI = epi_bytes<P>(), S = tma_stages(STAGE, EPI);
     constexpr int NT = P::CHUNK ? NA : 1, NTR = P::CHUNK ? NR : 1;
     static_assert(S >= 2, "a TMA problem needs two stages");
-    __shared__ __align__(8) uint64_t bars[2 * S];            // full[S], then empty[S]
+    __shared__ __align__(8) uint64_t bars[2 * S + 2];        // full[S], empty[S], then the epilogue buffer's full, empty
     const int tid = threadIdx.x, wg = tid >> 7;
     const uint32_t full0 = smem_u32(bars), empty0 = full0 + 8u * S, st0 = smem_u32(smem);
+    const uint32_t efull = full0 + 16u * S, eempty = efull + 8u, ebuf = st0 + (uint32_t)S * STAGE;
     if (tid == 0) {
         for (int s = 0; s < S; ++s) {
             mbar_init(full0 + 8u * s, 1);
             mbar_init(empty0 + 8u * s, 8);
         }
+        mbar_init(efull, 1);
+        mbar_init(eempty, 8);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
@@ -369,6 +393,7 @@ __device__ __forceinline__ void tma_tiles(const P& p, const TmaArgs& ta, uint8_t
     if (wg == 2) {
         setmaxnreg_dec<40>();
         if (tid != 2 * 128) return;
+        uint32_t ephase = 0;
         for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
             int m0, n0, z;
             decode(t, m0, n0, z);
@@ -376,6 +401,19 @@ __device__ __forceinline__ void tma_tiles(const P& p, const TmaArgs& ta, uint8_t
                 mbar_wait(empty0 + 8u * stage, phase ^ 1u);
                 p.produce(ta, st0 + (uint32_t)stage * STAGE, full0 + 8u * stage, it, m0, n0, z);
                 if (++stage == S) { stage = 0; phase ^= 1u; }
+                if constexpr (EPI > 0) {
+                    if (it == min(S, kb) - 1) {
+                        mbar_wait(eempty, ephase ^ 1u);
+                        mbar_expect_tx(efull, EPI);
+#pragma unroll
+                        for (int i = 0; i < P::EPI_MAPS; ++i)
+#pragma unroll
+                            for (int b = 0; b < P::BN / 32; ++b)
+                                tma_load(ebuf + (uint32_t)(i * BM * P::BN * 4 + b * BM * 128), &ta.map[P::NMAPS + i], n0 + 32 * b,
+                                         m0, efull);
+                        ephase ^= 1u;
+                    }
+                }
             }
         }
         return;
@@ -387,41 +425,55 @@ __device__ __forceinline__ void tma_tiles(const P& p, const TmaArgs& ta, uint8_t
     auto release = [&](int s) {
         if ((tid & 31) == 0) mbar_arrive(empty0 + 8u * s);
     };
+    // the wgmmas of the next k-block (sd = 0 starts the sums) on the next stage, committed as one group
+    auto consume = [&](uint32_t sd) {
+        mbar_wait(full0 + 8u * stage, phase);
+        if constexpr (P::FIX != FIX_NONE) {
+            p.fix(smem + (uint32_t)stage * STAGE, wg, tid);
+            fence_proxy_async();
+            if constexpr (P::FIX == FIX_A) bar_named(1 + wg, 128);
+            else bar_named(3, 256);
+        }
+        wg_fence();
+        issue<P>(st0 + (uint32_t)stage * STAGE, wg, acc, sd);
+        wg_commit();
+    };
+    auto next = [&] {
+        if (++stage == S) { stage = 0; phase ^= 1u; }
+    };
+    constexpr int CH = P::CHUNK;
+    uint32_t ephase = 0;
     for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
         int m0, n0, z;
         decode(t, m0, n0, z);
         zero(acc);
         zero(tot);
-        int pend = -1;                                        // the stage whose wgmmas are still in flight
-        for (int it = 0; it < kb; ++it) {
-            mbar_wait(full0 + 8u * stage, phase);
-            const uint32_t st = st0 + (uint32_t)stage * STAGE;
-            if constexpr (P::FIX != FIX_NONE) {
-                p.fix(smem + (uint32_t)stage * STAGE, wg, tid);
-                fence_proxy_async();
-                if constexpr (P::FIX == FIX_A) bar_named(1 + wg, 128);
-                else bar_named(3, 256);
-            }
-            const bool fresh = P::CHUNK ? (it % P::CHUNK == 0) : (it == 0);
-            wg_fence();
-            issue<P>(st, wg, acc, fresh ? 0u : 1u);
-            wg_commit();
-            const bool last = it + 1 == kb;
-            if (last || (P::CHUNK ? (it + 1) % P::CHUNK == 0 : false)) {
-                wg_wait0();
-                if (pend >= 0) release(pend);
-                release(stage);
-                pend = -1;
-                if constexpr (P::CHUNK > 0) fold(p, acc, tot, m0, it / P::CHUNK, z, tid);
-            } else {
+        // One chunk (the whole reduction when CHUNK = 0) per pass: its first k-block starts the sums, the steady state
+        // waits for all but the newest group and releases the previous stage, and only the chunk's end waits for all.
+        // No branch inside the k-loop selects between the two waits, so ptxas keeps the one group in flight.
+        for (int k0 = 0; k0 < kb; k0 += CH ? CH : kb) {
+            const int k1 = CH ? min(k0 + CH, kb) : kb;
+            consume(0u);
+            for (int it = k0 + 1; it < k1; ++it) {
+                const int prev = stage;
+                next();
+                consume(1u);
                 wg_wait1();
-                if (pend >= 0) release(pend);
-                pend = stage;
+                release(prev);
             }
-            if (++stage == S) { stage = 0; phase ^= 1u; }
+            wg_wait0();
+            release(stage);
+            next();
+            if constexpr (CH > 0) fold(p, acc, tot, m0, k0 / CH, z, tid);
         }
-        if constexpr (P::CHUNK > 0) p.epilogue(tot, m0, n0, z, tid);
-        else p.epilogue(acc, m0, n0, z, tid);
+        if constexpr (EPI > 0) mbar_wait(efull, ephase);
+        if constexpr (P::CHUNK > 0) p.epilogue(tot, m0, n0, z, tid, smem + (uint32_t)S * STAGE);
+        else p.epilogue(acc, m0, n0, z, tid, smem + (uint32_t)S * STAGE);
+        if constexpr (EPI > 0) {
+            __syncwarp();                                     // the warp's reads of the buffer are done
+            if ((tid & 31) == 0) mbar_arrive(eempty);
+            ephase ^= 1u;
+        }
     }
 }
 
@@ -484,6 +536,7 @@ struct ZsProb : NoScale {
     // single-pass: TMA (A = bf16(|x|), or raw x made tf32(|x|) in shared memory); two-pass: x+ / x- formed on load
     static constexpr bool TMA = SINGLE;
     static constexpr int FIX = SINGLE && !BF ? FIX_A : FIX_NONE;
+    static constexpr int EPI_MAPS = SINGLE ? 2 : 0;            // R and y, staged by the producer
     int M, N, K;
     const float* x; long long ldx;
     const void* xabs;                       // BF: bf16(|x|) [M, K]
@@ -499,7 +552,8 @@ struct ZsProb : NoScale {
     TE_PRODUCE_TILES(ZsProb)
     TmaTile tile(int i) const {
         if (i == 0) return BF ? TmaTile{xabs, M, K, K, BM} : TmaTile{x, M, K, ldx, BM};
-        return TmaTile{wa, N, K, K, BN};
+        if (i == 1) return TmaTile{wa, N, K, K, BN};
+        return i == 2 ? TmaTile{r, M, N, ldr, BM} : TmaTile{y, M, N, ldy, BM};
     }
     __device__ void load(uint8_t* st, int kb, int m0, int n0, int, int tid) const {
         for_k32(BM, x, ldx, m0, M, kb * 32, K, tid, [&](int rr, int c, float4 v) {
@@ -509,7 +563,9 @@ struct ZsProb : NoScale {
         for_k32(BN, (const float*)wa, K, n0, N, kb * 32, K, tid, [&](int rr, int c, float4 v) { st4(st + L::b(0), rr, c, v); });
         for_k32(BN, (const float*)wb, K, n0, N, kb * 32, K, tid, [&](int rr, int c, float4 v) { st4(st + L::b(1), rr, c, v); });
     }
-    __device__ void epilogue(float (&acc)[1][BN / 2], int m0, int n0, int, int tid) const {
+    // Single-pass: R and y come from the epilogue buffer (eb), bias from global memory; the whole fragment's S is computed
+    // before the first store.  Two-pass (register mainloop): R from global memory.
+    __device__ void epilogue(float (&acc)[1][BN / 2], int m0, int n0, int, int tid, const uint8_t* eb) const {
         float sv[BN / 2];
         float rmax[2] = {0.f, 0.f};
 #pragma unroll
@@ -517,9 +573,10 @@ struct ZsProb : NoScale {
             const int row = m0 + frag_row(tid, j), col = n0 + frag_col(tid, j);
             float2 rr = make_float2(0.f, 0.f), z = make_float2(acc[0][j], acc[0][j + 1]);
             if (row < M) {
-                rr = *reinterpret_cast<const float2*>(r + (long long)row * ldr + col);
+                rr = SINGLE ? epi_f2(eb, frag_row(tid, j), frag_col(tid, j))
+                            : *reinterpret_cast<const float2*>(r + (long long)row * ldr + col);
                 if (SINGLE) {
-                    const float2 yy = *reinterpret_cast<const float2*>(y + (long long)row * ldy + col);
+                    const float2 yy = epi_f2(eb + BM * BN * 4, frag_row(tid, j), frag_col(tid, j));
                     const float2 bb = bias ? *reinterpret_cast<const float2*>(bias + col) : make_float2(0.f, 0.f);
                     // x+ W+^T + x- W-^T == (x W^T + |x| |W|^T) / 2 ; a negative result is cancellation noise of a sum of
                     // non-negative terms (zsign = -1: x+ W-^T + x- W+^T == (x W^T - |x| |W|^T) / 2, a sum of non-positive terms)
@@ -531,6 +588,10 @@ struct ZsProb : NoScale {
             sv[j] = sscale * te_sd(rr.x, z.x);
             sv[j + 1] = sscale * te_sd(rr.y, z.y);
             if (OUT == ZO_F16S) rmax[(j >> 1) & 1] = fmaxf(rmax[(j >> 1) & 1], fmaxf(fabsf(sv[j]), fabsf(sv[j + 1])));
+        }
+#pragma unroll
+        for (int j = 0; j < BN / 2; j += 2) {
+            const int row = m0 + frag_row(tid, j), col = n0 + frag_col(tid, j);
             if (row >= M) continue;
             if (OUT == ZO_F32) {
                 *reinterpret_cast<float2*>((float*)out + (long long)row * ldo + col) = make_float2(to_tf32(sv[j]), to_tf32(sv[j + 1]));
@@ -572,7 +633,7 @@ struct ZrProb {
     using PRODS = Prods<Pr<0, 0, 0>, Pr<1, 0, 1>>;           // S W+ and S W- into their own accumulators
     using L = Stage<PRODS, BN>;
     static constexpr bool TMA = true;
-    static constexpr int FIX = FIX_NONE;
+    static constexpr int FIX = FIX_NONE, EPI_MAPS = 1;           // x, staged by the producer
     int M, N, K;
     const void* s; const void* wp; const void* wn;     // S [M, K] (row stride K), W+^T / W-^T [N, K]
     const float* rs; int rs_ld; const float* cp; const float* cn;   // KIND 2: scales of S, of the rows of W+^T / W-^T
@@ -582,25 +643,36 @@ struct ZrProb {
     __device__ int kblocks() const { return K / (KIND ? 64 : 32); }
     TE_PRODUCE_TILES(ZrProb)
     __device__ float chunk_scale(int row, int ch, int) const { return (KIND == 2 && row < M) ? rs[(long long)row * rs_ld + ch] : 1.f; }
-    TmaTile tile(int i) const { return i == 0 ? TmaTile{s, M, K, K, BM} : TmaTile{i == 1 ? wp : wn, N, K, K, BN}; }
-    __device__ void epilogue(float (&acc)[2][BN / 2], int m0, int n0, int, int tid) const {
+    TmaTile tile(int i) const {
+        if (i == 0) return TmaTile{s, M, K, K, BM};
+        return i < 3 ? TmaTile{i == 1 ? wp : wn, N, K, K, BN} : TmaTile{x, M, N, ldx, BM};
+    }
+    // x comes from the epilogue buffer (eb), the column scales from global memory.  Accumulating, each thread reads the
+    // out elements it then writes, from global memory: out is not staged (it may alias x, and the value read must be the
+    // one the previous launch left), and its reads are done for the whole fragment into acc[0] before the first store.
+    __device__ void epilogue(float (&acc)[2][BN / 2], int m0, int n0, int, int tid, const uint8_t* eb) const {
 #pragma unroll
         for (int j = 0; j < BN / 2; j += 2) {
             const int row = m0 + frag_row(tid, j), col = n0 + frag_col(tid, j);
             if (row >= M) continue;
-            const float2 xv = *reinterpret_cast<const float2*>(x + (long long)row * ldx + col);
+            const float2 xv = epi_f2(eb, frag_row(tid, j), frag_col(tid, j));
             float2 ap = make_float2(acc[0][j], acc[0][j + 1]), an = make_float2(acc[1][j], acc[1][j + 1]);
             if (KIND == 2) {
                 ap.x *= cp[col]; ap.y *= cp[col + 1];
                 an.x *= cn[col]; an.y *= cn[col + 1];
             }
-            float2* o = reinterpret_cast<float2*>(out + (long long)row * ldo + col);
             float2 v = make_float2(fmaxf(xv.x, 0.f) * ap.x + fminf(xv.x, 0.f) * an.x, fmaxf(xv.y, 0.f) * ap.y + fminf(xv.y, 0.f) * an.y);
             if (accum) {
-                const float2 prev = *o;
+                const float2 prev = *reinterpret_cast<const float2*>(out + (long long)row * ldo + col);
                 v = make_float2(prev.x + v.x, prev.y + v.y);
             }
-            *o = v;
+            acc[0][j] = v.x;
+            acc[0][j + 1] = v.y;
+        }
+#pragma unroll
+        for (int j = 0; j < BN / 2; j += 2) {
+            const int row = m0 + frag_row(tid, j), col = n0 + frag_col(tid, j);
+            if (row < M) *reinterpret_cast<float2*>(out + (long long)row * ldo + col) = make_float2(acc[0][j], acc[0][j + 1]);
         }
     }
 };
@@ -626,7 +698,7 @@ struct LrpSProb : NoScale {
         for_k32(BM, x, ldx, m0, M, kb * 32, K, tid, [&](int rr, int c, float4 v) { st4(st + L::a(0), rr, c, tf32x4(NEG ? negx4(v) : posx4(v))); });
         for_k32(BN, w, K, n0, N, kb * 32, K, tid, [&](int rr, int c, float4 v) { st4(st + L::b(0), rr, c, v); });
     }
-    __device__ void epilogue(float (&acc)[1][BN / 2], int m0, int n0, int, int tid) const {
+    __device__ void epilogue(float (&acc)[1][BN / 2], int m0, int n0, int, int tid, const uint8_t*) const {
 #pragma unroll
         for (int j = 0; j < BN / 2; j += 2) {
             const int row = m0 + frag_row(tid, j), col = n0 + frag_col(tid, j);
@@ -645,30 +717,41 @@ struct LrpRProb : NoScale {
     using PRODS = One;
     using L = Stage<PRODS, BN>;
     static constexpr bool TMA = true;
-    static constexpr int FIX = FIX_NONE;
+    static constexpr int FIX = FIX_NONE, EPI_MAPS = 1;           // x, staged by the producer
     int M, N, K;
     const float* s; const float* wt;
     const float* x; long long ldx; float* out; long long ldo;
     int accum;
     __device__ int kblocks() const { return K / 32; }
     TE_PRODUCE_TILES(LrpRProb)
-    TmaTile tile(int i) const { return i == 0 ? TmaTile{s, M, K, K, BM} : TmaTile{wt, N, K, K, BN}; }
-    __device__ void epilogue(float (&acc)[1][BN / 2], int m0, int n0, int, int tid) const {
+    TmaTile tile(int i) const {
+        return i == 0 ? TmaTile{s, M, K, K, BM} : i == 1 ? TmaTile{wt, N, K, K, BN} : TmaTile{x, M, N, ldx, BM};
+    }
+    // x from the epilogue buffer, out read as in ZrProb (accumulating products: global memory, whole fragment first)
+    __device__ void epilogue(float (&acc)[1][BN / 2], int m0, int n0, int, int tid, const uint8_t* eb) const {
 #pragma unroll
         for (int j = 0; j < BN / 2; j += 2) {
             const int row = m0 + frag_row(tid, j), col = n0 + frag_col(tid, j);
             if (row >= M) continue;
-            const float2 xv = *reinterpret_cast<const float2*>(x + (long long)row * ldx + col);
-            float2* o = reinterpret_cast<float2*>(out + (long long)row * ldo + col);
+            const float2 xv = epi_f2(eb, frag_row(tid, j), frag_col(tid, j));
+            const float2* o = reinterpret_cast<const float2*>(out + (long long)row * ldo + col);
+            float2 v;
             if (NEG) {
                 const float2 prev = *o;
-                *o = make_float2(prev.x + fminf(xv.x, 0.f) * acc[0][j], prev.y + fminf(xv.y, 0.f) * acc[0][j + 1]);
+                v = make_float2(prev.x + fminf(xv.x, 0.f) * acc[0][j], prev.y + fminf(xv.y, 0.f) * acc[0][j + 1]);
             } else if (accum) {
                 const float2 prev = *o;
-                *o = make_float2(prev.x + fmaxf(xv.x, 0.f) * acc[0][j], prev.y + fmaxf(xv.y, 0.f) * acc[0][j + 1]);
+                v = make_float2(prev.x + fmaxf(xv.x, 0.f) * acc[0][j], prev.y + fmaxf(xv.y, 0.f) * acc[0][j + 1]);
             } else {
-                *o = make_float2(fmaxf(xv.x, 0.f) * acc[0][j], fmaxf(xv.y, 0.f) * acc[0][j + 1]);
+                v = make_float2(fmaxf(xv.x, 0.f) * acc[0][j], fmaxf(xv.y, 0.f) * acc[0][j + 1]);
             }
+            acc[0][j] = v.x;
+            acc[0][j + 1] = v.y;
+        }
+#pragma unroll
+        for (int j = 0; j < BN / 2; j += 2) {
+            const int row = m0 + frag_row(tid, j), col = n0 + frag_col(tid, j);
+            if (row < M) *reinterpret_cast<float2*>(out + (long long)row * ldo + col) = make_float2(acc[0][j], acc[0][j + 1]);
         }
     }
 };
@@ -679,22 +762,31 @@ struct LinOut {
     const float* bias; const float* E; long long lde;
     float* C; long long ldc; float* C2; long long ldc2;
 };
+// The Linear epilogue of a fragment in two passes: lin_value forms y from the product and the operands read before any
+// store (bias; E of GELU_BWD), then lin_store writes y and the second output (gelu(y), or E + y for BIAS_ADD).  e(): the
+// fragment's float2 of E (the epilogue buffer on the TMA mainloop).
 // v: the product for columns col, col + 1 (already scaled)
-template <int EPI, bool FAST_GRAD = false>
-__device__ __forceinline__ void lin_store(const LinOut& o, int row, int col, float v0, float v1) {
-    if (row >= o.M) return;
+template <int EPI, bool FAST_GRAD, class EF>
+__device__ __forceinline__ float2 lin_value(const LinOut& o, int col, float v0, float v1, EF e) {
     float2 b = make_float2(0.f, 0.f);
     if ((EPI == TE_TC_EPI_BIAS || EPI == TE_TC_EPI_BIAS_GELU || EPI == TE_TC_EPI_BIAS_ADD) && o.bias)
         b = *reinterpret_cast<const float2*>(o.bias + col);
-    float2 y = make_float2(v0 + b.x, v1 + b.y), y2 = make_float2(0.f, 0.f);
-    if (EPI == TE_TC_EPI_BIAS_GELU) y2 = make_float2(te_gelu(y.x), te_gelu(y.y));
-    if (EPI == TE_TC_EPI_BIAS_ADD || EPI == TE_TC_EPI_GELU_BWD) {
-        const float2 e = *reinterpret_cast<const float2*>(o.E + (long long)row * o.lde + col);
-        if (EPI == TE_TC_EPI_BIAS_ADD) y2 = make_float2(e.x + y.x, e.y + y.y);
-        else if (FAST_GRAD) y = make_float2(v0 * te_gelu_grad_fast(e.x), v1 * te_gelu_grad_fast(e.y));
-        else y = make_float2(v0 * te_gelu_grad(e.x), v1 * te_gelu_grad(e.y));
+    if (EPI == TE_TC_EPI_GELU_BWD) {
+        const float2 ev = e();
+        if (FAST_GRAD) return make_float2(v0 * te_gelu_grad_fast(ev.x), v1 * te_gelu_grad_fast(ev.y));
+        return make_float2(v0 * te_gelu_grad(ev.x), v1 * te_gelu_grad(ev.y));
     }
+    return make_float2(v0 + b.x, v1 + b.y);
+}
+template <int EPI, class EF>
+__device__ __forceinline__ void lin_store(const LinOut& o, int row, int col, float2 y, EF e) {
     *reinterpret_cast<float2*>(o.C + (long long)row * o.ldc + col) = y;
+    float2 y2 = make_float2(0.f, 0.f);
+    if (EPI == TE_TC_EPI_BIAS_GELU) y2 = make_float2(te_gelu(y.x), te_gelu(y.y));
+    if (EPI == TE_TC_EPI_BIAS_ADD) {
+        const float2 ev = e();
+        y2 = make_float2(ev.x + y.x, ev.y + y.y);
+    }
     if (EPI == TE_TC_EPI_BIAS_GELU || EPI == TE_TC_EPI_BIAS_ADD) *reinterpret_cast<float2*>(o.C2 + (long long)row * o.ldc2 + col) = y2;
 }
 
@@ -725,6 +817,8 @@ struct LinProb : LinArgs {
     // the fp16 forms and the single-pass TF32 form (A rounded in shared memory) on TMA; 3xTF32 splits A on load
     static constexpr bool TMA = FORM != LIN_3XTF32;
     static constexpr int FIX = FORM == LIN_TF32 ? FIX_A : FIX_NONE;
+    // E of BIAS_ADD / GELU_BWD, staged by the producer on the TMA mainloop
+    static constexpr int EPI_MAPS = TMA && (EPI == TE_TC_EPI_BIAS_ADD || EPI == TE_TC_EPI_GELU_BWD) ? 1 : 0;
     __device__ int kblocks() const { return K / (F16 ? 64 : 32); }
     __device__ float chunk_scale(int row, int ch, int) const {
         if constexpr (F16) return row < o.M ? rs[(long long)row * rs_ld + ch] : 1.f;
@@ -736,21 +830,38 @@ struct LinProb : LinArgs {
     TE_PRODUCE_TILES(LinProb)
     TmaTile tile(int i) const {
         if (i < L::NTA) return TmaTile{i == 0 ? a : a_lo, o.M, K, F16 ? K : lda, BM};
-        return TmaTile{i == L::NTA ? b : b_lo, o.N, K, K, BN};
+        if (i < NMAPS) return TmaTile{i == L::NTA ? b : b_lo, o.N, K, K, BN};
+        return TmaTile{o.E, o.M, o.N, o.lde, BM};
     }
     __device__ void load(uint8_t* st, int kb, int m0, int n0, int, int tid) const {
         for_k32(BM, (const float*)a, lda, m0, o.M, kb * 32, K, tid, [&](int r, int c, float4 v) { st_split(st + L::a(0), st + L::a(1), r, c, v); });
         for_k32(BN, (const float*)b, K, n0, o.N, kb * 32, K, tid, [&](int r, int c, float4 v) { st4(st + L::b(0), r, c, v); });
         for_k32(BN, (const float*)b_lo, K, n0, o.N, kb * 32, K, tid, [&](int r, int c, float4 v) { st4(st + L::b(1), r, c, v); });
     }
-    __device__ void epilogue(float (&acc)[1][BN / 2], int m0, int n0, int, int tid) const {
+    // E from the epilogue buffer (eb) on the TMA mainloop, from global memory on the register mainloop (3xTF32); bias and
+    // the column scales from global memory, before the first store
+    __device__ void epilogue(float (&acc)[1][BN / 2], int m0, int n0, int, int tid, const uint8_t* eb) const {
 #pragma unroll
         for (int j = 0; j < BN / 2; j += 2) {
-            const int col = n0 + frag_col(tid, j);
+            const int row = m0 + frag_row(tid, j), col = n0 + frag_col(tid, j);
+            if (row >= o.M) continue;
+            auto e = [&] { return efrag(eb, tid, j, row, col); };
+            float2 y;
             if constexpr (F16)                                          // exact scaling
-                lin_store<EPI>(o, m0 + frag_row(tid, j), col, acc[0][j] * cs[col], acc[0][j + 1] * cs[col + 1]);
-            else lin_store<EPI, FORM == LIN_TF32>(o, m0 + frag_row(tid, j), col, acc[0][j], acc[0][j + 1]);
+                y = lin_value<EPI, false>(o, col, acc[0][j] * cs[col], acc[0][j + 1] * cs[col + 1], e);
+            else y = lin_value<EPI, FORM == LIN_TF32>(o, col, acc[0][j], acc[0][j + 1], e);
+            acc[0][j] = y.x;
+            acc[0][j + 1] = y.y;
         }
+#pragma unroll
+        for (int j = 0; j < BN / 2; j += 2) {
+            const int row = m0 + frag_row(tid, j), col = n0 + frag_col(tid, j);
+            if (row < o.M) lin_store<EPI>(o, row, col, make_float2(acc[0][j], acc[0][j + 1]), [&] { return efrag(eb, tid, j, row, col); });
+        }
+    }
+    __device__ float2 efrag(const uint8_t* eb, int tid, int j, int row, int col) const {
+        if constexpr (EPI_MAPS > 0) return epi_f2(eb, frag_row(tid, j), frag_col(tid, j));
+        else return *reinterpret_cast<const float2*>(o.E + (long long)row * o.lde + col);
     }
 };
 
@@ -765,7 +876,7 @@ struct NnProb : NoScale {
     // leaves head h (dh is 32 or 64).  Rows past a sample's N are the next sample's (zeros past the tensor): they reach only
     // the output rows and columns the epilogue masks.
     static constexpr bool TMA = true;
-    static constexpr int FIX = FIX_AB;
+    static constexpr int FIX = FIX_AB, EPI_MAPS = 0;
     int N, H, dh, ld_out, batch;
     const float* a; long long lda; const float* b; long long ldb;
     const float* E; float* out; float alpha;
@@ -784,7 +895,7 @@ struct NnProb : NoScale {
         fix_tf32<SP>(st + L::a(0), st + L::a(1), 64 * wg, 64, tid & 127, 128);
         fix_tf32<SP>(st + L::b(0), st + L::b(1), 0, BN, tid, 256);
     }
-    __device__ void epilogue(float (&acc)[1][BN / 2], int m0, int n0, int bh, int tid) const {
+    __device__ void epilogue(float (&acc)[1][BN / 2], int m0, int n0, int bh, int tid, const uint8_t*) const {
         const int ncols = (N + 3) & ~3;                  // the row padding up to a multiple of 4 is written as zeros
         if constexpr (EPI == AT_SOFTMAX) {
             // softmax(alpha * A B^T) over the key axis: the tile holds every key (N <= BN); a row's values sit in one quad
@@ -863,7 +974,7 @@ struct NkProb : NoScale {
     static constexpr int LAND_A = AMN ? BM * 128 : 0, LAND_X = BN * 128;
     using L = Stage<PRODS, BN, LAND_A + LAND_X>;
     static constexpr bool TMA = true;
-    static constexpr int FIX = FIX_AB;
+    static constexpr int FIX = FIX_AB, EPI_MAPS = 0;
     int N, H, NP, ld_out, n_out, n_pad, a_shared, batch;
     const float* map; const float* X; long long ldx;
     const float* rowscale; const float* E; float* out; float alpha;
@@ -888,7 +999,7 @@ struct NkProb : NoScale {
         else fix_tf32<SP>(st + L::a(0), st + L::a(1), 64 * wg, 64, tid & 127, 128);
         transpose_rows(st + L::land() + LAND_A, 0, BN, tid, 256, put_tf32<SP>(st + L::b(0), st + L::b(1)));
     }
-    __device__ void epilogue(float (&acc)[1][BN / 2], int m0, int, int bh, int tid) const {
+    __device__ void epilogue(float (&acc)[1][BN / 2], int m0, int, int bh, int tid, const uint8_t*) const {
         const int s = bh / H, h = bh % H;
         // E of the whole fragment is loaded before the first store, so that its loads are in flight together (out may alias E)
         float2 ef[BN / 4];
@@ -977,9 +1088,9 @@ int launch(const P& p, dim3 grid, cudaStream_t st) {
     int col_fast = 0, threads = NTHREADS, smem = 2 * P::L::BYTES + 1024;
     if constexpr (P::TMA) {
         constexpr int ESIZE = P::FMT == OP_TF32 ? 4 : 2;
-        static_assert(P::NMAPS <= 4, "TmaArgs holds four tensor maps");
-        for (int i = 0; i < P::NMAPS; ++i)
-            if (!encode_tile(&ta.map[i], p.tile(i), ESIZE)) {
+        static_assert(P::NMAPS + P::EPI_MAPS <= TMA_MAPS, "TmaArgs holds TMA_MAPS tensor maps");
+        for (int i = 0; i < P::NMAPS + P::EPI_MAPS; ++i)        // the epilogue operands are fp32
+            if (!encode_tile(&ta.map[i], p.tile(i), i < P::NMAPS ? ESIZE : 4)) {
                 te_set_last_error("te_tc: cannot encode a TMA tensor map (16-byte-aligned base and strides required)");
                 return TE_ERR_ARG;
             }
@@ -990,7 +1101,7 @@ int launch(const P& p, dim3 grid, cudaStream_t st) {
         ta.nz = (int)grid.z;
         grid = dim3((unsigned)std::min<long long>(tiles, sm_count()));
         threads = NTHREADS_TMA;
-        smem = tma_stages(P::L::BYTES) * P::L::BYTES + 1024;
+        smem = tma_stages(P::L::BYTES, epi_bytes<P>()) * P::L::BYTES + epi_bytes<P>() + 1024;
     } else {
         col_fast = P::COL_FAST && grid.x <= 65535;
         if (col_fast) grid = dim3(grid.y, grid.x, grid.z);
@@ -1221,7 +1332,7 @@ int te_tc_zplus_s1(const float* x, long long ldx, float* xabs, const float* deri
                    const float* y, long long ldy, const float* bias, float* s_out, long long rows, int in_features,
                    int out_features, cudaStream_t st, bool bf16, float* s16, float* s16_scale, float s_scale, bool inh) {
     const TeDerived<const float> dv(derived, in_features, out_features);
-    if (ldx % 4 != 0 || !a16(x) || !a16(r) || !a16(y) || ldr % 2 != 0 || ldy % 2 != 0) {
+    if (ldx % 4 != 0 || !a16(x) || !a16(r) || !a16(y) || ldr % 4 != 0 || ldy % 4 != 0) {   // R, y: TMA-encodable
         te_set_last_error("te_tc_zplus_s1: alignment");
         return TE_ERR_ARG;
     }
