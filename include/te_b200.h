@@ -459,6 +459,31 @@ TE_API int te_eraser_reduce_inputs(const float* maps, const long long* input_ids
                                    long long* out_ids, int* out_len, void* workspace, long long workspace_bytes,
                                    void* stream);
 
+/* ERASER soft-token scores (metrics.py:217-253: score_soft_tokens) */
+/* Workspace of te_eraser_soft_scores for `spans` truth spans over `batch` documents. */
+TE_API long long te_eraser_soft_workspace_bytes(int batch, long long spans);
+/* Per document b, over its W = word_offsets[b+1] - word_offsets[b] word scores word_scores[word_offsets[b] ..] (device,
+ * the layout te_eraser_rationales writes; W <= TE_ERASER_MAX_WORDS), its truth spans [span_offsets[b], span_offsets[b+1])
+ * (word w < W is positive iff some span has start <= w < end) and its tail tail_counts[b] = (positives, negatives) of
+ * the words past truncation, which score 0:
+ *   the soft prediction is the W scores followed by the tail's zeros; the words are ranked as te_eraser_rationales ranks
+ *   them, bit-equal scores (-0 == +0) form one tie group, and the tail joins the group of score 0 (or follows the last
+ *   group when no word scores 0).  With P positives and N negatives in all and each group's cumulative (tps, fps) in
+ *   descending score order (sklearn's _binary_clf_curve), in fp64:
+ *   scores[b, 0] = auc(recall, precision) of precision_recall_curve (recall tps / P, or 1 when P = 0; precision
+ *     tps / (tps + fps); the point (0, 1) first), the trapezoid area;
+ *   scores[b, 1] = average_precision_score: the sum over groups of (recall step) * precision;
+ *   scores[b, 2] = roc_auc_score: the trapezoid area under (fps / N, tps / P) from (0, 0), from an integer sum
+ *     (roc_curve's dropped collinear points change only its rounding); NaN when P = 0 or N = 0;
+ *   flags[b, 0] = 1 when P = 0 or N = 0 (a single-class document), flags[b, 1] = 1 when a word score is NaN or
+ *     negative: then all three scores are NaN and only flags[b, 0] is meaningful besides.
+ * word_offsets, span_offsets, spans [.., 2] and tail_counts [batch, 2] are host arrays, validated before anything is
+ * launched: offsets from 0, W <= TE_ERASER_MAX_WORDS, every span 0 <= start <= end, tail counts >= 0 with sum <= 2^30, and
+ * W + the tail >= 1 per document, else TE_ERR_ARG. */
+TE_API int te_eraser_soft_scores(const float* word_scores, int batch, const int* word_offsets, const int* span_offsets,
+                                 const int* spans, const int* tail_counts, double* scores, int* flags, void* workspace,
+                                 long long workspace_bytes, void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Input preparation  (baselines/ViT/generate_visualizations.py:194-199: Resize((224, 224)) + ToTensor() on PIL images)
  * Pillow's 8-bit bilinear resize (ImagingResample, support 1): per axis scale = in / out, fs = max(scale, 1), and for output

@@ -6,6 +6,8 @@
 //   * reduce_kernel: one block per document, the ranking of eraser_kernel; each piece is marked with the smallest rank of
 //     the words holding it, and per selection size n the pieces of the first n ranks (sufficiency) and the other inner
 //     pieces (comprehensiveness) are compacted, between the document's [CLS] and [SEP], by one block scan.
+//   * soft_kernel: one block per document, the ranking of eraser_kernel over given word scores; the tie groups' cumulative
+//     (tps, fps) come from one warp scan, and metrics.py's soft-token areas (:217-253) are reduced in fp64.
 // The ragged host arrays (word piece ranges, truth spans, their offsets) are validated on the host and copied into the
 // workspace, so no index the caller passes is read from the map before it has been checked.
 #include "../../include/te_b200.h"
@@ -31,11 +33,28 @@ __device__ __forceinline__ uint32_t order_key(float v) {
     return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
 }
 
+// Rank the W words of one document by the scores score(w): skey[w] = (~order_key << 32) | w, sword[r] = the word at rank r
+// (NaN first, then descending score, then ascending word index).  Ends with a block barrier.
+template <class Score>
+__device__ __forceinline__ void rank_scores(Score score, int W, unsigned long long* skey, int* sword) {
+    for (int w = threadIdx.x; w < W; w += blockDim.x)
+        skey[w] = ((unsigned long long)(~order_key(score(w))) << 32) | (unsigned)w;   // ascending = ranking order
+    __syncthreads();
+    // rank = number of smaller keys (all keys are distinct)
+    for (int w = threadIdx.x; w < W; w += blockDim.x) {
+        const unsigned long long k = skey[w];
+        int rank = 0;
+        for (int u = 0; u < W; ++u) rank += skey[u] < k;
+        sword[rank] = w;
+    }
+    __syncthreads();
+}
+
 // Score and rank the W words of one document (map row m, inclusive piece ranges): word_scores[w] (may be null) = the max
-// of the clamped map over the word's pieces (NaN propagates), sword[r] = the word at rank r.  Ends with a block barrier.
+// of the clamped map over the word's pieces (NaN propagates), ranked by rank_scores.  Ends with a block barrier.
 __device__ __forceinline__ void rank_words(const float* __restrict__ m, const int2* __restrict__ ranges, int W,
                                            float* __restrict__ word_scores, unsigned long long* skey, int* sword) {
-    for (int w = threadIdx.x; w < W; w += blockDim.x) {
+    rank_scores([&](int w) {
         const int2 r = ranges[w];
         float s = 0.f;
         bool nan = false, first = true;
@@ -48,17 +67,8 @@ __device__ __forceinline__ void rank_words(const float* __restrict__ m, const in
         }
         if (nan) s = __int_as_float(0x7fc00000);
         if (word_scores) word_scores[w] = s;
-        skey[w] = ((unsigned long long)(~order_key(s)) << 32) | (unsigned)w;   // ascending = ranking order
-    }
-    __syncthreads();
-    // rank = number of smaller keys (all keys are distinct)
-    for (int w = threadIdx.x; w < W; w += blockDim.x) {
-        const unsigned long long k = skey[w];
-        int rank = 0;
-        for (int u = 0; u < W; ++u) rank += skey[u] < k;
-        sword[rank] = w;
-    }
-    __syncthreads();
+        return s;
+    }, W, skey, sword);
 }
 
 __global__ void __launch_bounds__(kThreads) eraser_kernel(
@@ -192,6 +202,125 @@ __global__ void __launch_bounds__(kThreads) reduce_kernel(
     }
 }
 
+// score_soft_tokens' three areas of document b (metrics.py:217-253) from its W word scores and its tail (tail[b] = the
+// positive and negative words past truncation, which score 0): the words are ranked by rank_scores, so bit-equal scores
+// (-0 == +0) are contiguous; a warp scan of (positive, tie-group end) along the ranks gives each group's cumulative
+// (tps, fps), _binary_clf_curve's points; the tail joins the last group when it scores 0, else follows it as its own
+// group (the scores are >= 0); the areas are summed per group in fp64 and reduced over the block.
+__global__ void __launch_bounds__(kThreads) soft_kernel(
+        const float* __restrict__ word_scores, const int* __restrict__ word_off, const int* __restrict__ span_off,
+        const int2* __restrict__ spans, const int2* __restrict__ tail, double* __restrict__ scores, int* __restrict__ flags) {
+    __shared__ unsigned long long skey[TE_ERASER_MAX_WORDS];
+    __shared__ int sword[TE_ERASER_MAX_WORDS];
+    __shared__ int sscan[TE_ERASER_MAX_WORDS];                     // positive | group end << 16, then inclusive prefix sums
+    __shared__ long long gtp[TE_ERASER_MAX_WORDS + 1], gfp[TE_ERASER_MAX_WORDS + 1];   // cumulative counts per tie group
+    __shared__ double sred[2][kWarps];
+    __shared__ long long sroc[kWarps];
+    __shared__ int sG, sbad;
+    const int b = blockIdx.x;
+    const int w0 = word_off[b], W = word_off[b + 1] - w0;
+    const int s0 = span_off[b], S = span_off[b + 1] - s0;
+    const float* s = word_scores + w0;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (threadIdx.x == 0) sbad = 0;
+    __syncthreads();
+    rank_scores([&](int w) {
+        const float v = s[w];
+        if (!(v >= 0.f)) sbad = 1;                                 // NaN or negative: no soft scores
+        return v;
+    }, W, skey, sword);
+    const auto group_end = [&](int r) {
+        return r == W - 1 || (unsigned)(skey[sword[r]] >> 32) != (unsigned)(skey[sword[r + 1]] >> 32);
+    };
+    for (int r = threadIdx.x; r < W; r += kThreads) {
+        const int w = sword[r];
+        int pos = 0;
+        for (int j = 0; j < S; ++j) {
+            const int2 t = spans[s0 + j];
+            pos |= t.x <= w && w < t.y;
+        }
+        sscan[r] = pos | (int)group_end(r) << 16;
+    }
+    __syncthreads();
+    if (warp == 0) {                                               // lane l owns ranks [l*C, (l+1)*C)
+        const int C = (W + 31) / 32;
+        const int r0 = lane * C, r1 = min(W, r0 + C);
+        int sum = 0;
+        for (int r = r0; r < r1; ++r) sum += sscan[r];
+        int incl = sum;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const int u = __shfl_up_sync(0xffffffffu, incl, o);
+            if (lane >= o) incl += u;
+        }
+        int run = incl - sum;
+        for (int r = r0; r < r1; ++r) { run += sscan[r]; sscan[r] = run; }
+    }
+    __syncthreads();
+    for (int r = threadIdx.x; r < W; r += kThreads) {
+        if (!group_end(r)) continue;
+        const int g = (sscan[r] >> 16) - 1, tp = sscan[r] & 0xffff;
+        gtp[g] = tp;
+        gfp[g] = r + 1 - tp;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int G = W ? sscan[W - 1] >> 16 : 0;
+        const long long tp = G ? gtp[G - 1] : 0, fp = G ? gfp[G - 1] : 0;
+        if (tail[b].x + tail[b].y > 0) {
+            if (!(G && (unsigned)(skey[sword[W - 1]] >> 32) == ~order_key(0.f))) ++G;
+            gtp[G - 1] = tp + tail[b].x;
+            gfp[G - 1] = fp + tail[b].y;
+        }
+        sG = G;
+    }
+    __syncthreads();
+    const int G = sG;                                              // >= 1: W + tail >= 1 is checked on the host
+    const long long P = gtp[G - 1], N = gfp[G - 1];
+    // precision_recall_curve's points (recall tp / P, 1 without positives; precision tp / (tp + fp)) after the point
+    // (0, 1): auc(recall, precision) is their trapezoid area, average_precision_score the step area; roc_curve's points
+    // (fp / N, tp / P) after (0, 0): roc_auc_score's trapezoid area, summed in integers
+    double pr = 0.0, ap = 0.0;
+    long long roc = 0;
+    for (int g = threadIdx.x; g < G; g += kThreads) {
+        const long long tp = gtp[g], fp = gfp[g];
+        const long long tq = g ? gtp[g - 1] : 0, fq = g ? gfp[g - 1] : 0;
+        const double p = (double)tp / (double)(tp + fp), q = g ? (double)tq / (double)(tq + fq) : 1.0;
+        const double r = P ? (double)tp / (double)P : 1.0, rq = g ? (P ? (double)tq / (double)P : 1.0) : 0.0;
+        pr += (r - rq) * (p + q) / 2.0;
+        ap += (r - rq) * p;
+        roc += (fp - fq) * (tp + tq);
+    }
+#pragma unroll
+    for (int o = 16; o; o >>= 1) {
+        pr += __shfl_down_sync(0xffffffffu, pr, o);
+        ap += __shfl_down_sync(0xffffffffu, ap, o);
+        roc += __shfl_down_sync(0xffffffffu, roc, o);
+    }
+    if (lane == 0) {
+        sred[0][warp] = pr;
+        sred[1][warp] = ap;
+        sroc[warp] = roc;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        pr = ap = 0.0;
+        roc = 0;
+        for (int u = 0; u < kWarps; ++u) {
+            pr += sred[0][u];
+            ap += sred[1][u];
+            roc += sroc[u];
+        }
+        const bool single = P == 0 || N == 0;
+        const double nan = __longlong_as_double(0x7ff8000000000000LL);
+        scores[3 * b] = sbad ? nan : pr;
+        scores[3 * b + 1] = sbad ? nan : ap;
+        scores[3 * b + 2] = sbad || single ? nan : (double)roc / (2.0 * (double)P * (double)N);
+        flags[2 * b] = single;
+        flags[2 * b + 1] = sbad;
+    }
+}
+
 }  // namespace
 
 #define ST(s) reinterpret_cast<cudaStream_t>(s)
@@ -321,6 +450,57 @@ extern "C" int te_eraser_reduce_inputs(const float* maps, const long long* input
     }
     reduce_kernel<<<batch, kThreads, 4 * (size_t)seq, st>>>(maps, input_ids, seq, d_lens, d_woff, d_ranges, d_nsel,
                                                              selections, out_ids, out_len);
+    TE_CUDA_CHECK_LAUNCH();
+    return TE_OK;
+}
+
+extern "C" long long te_eraser_soft_workspace_bytes(int batch, long long spans) {
+    if (batch <= 0 || spans < 0 || spans > 0x7fffffffLL) return TE_ERR_ARG;
+    return 2 * up256(4LL * (batch + 1)) + up256(8 * spans) + up256(8LL * batch);
+}
+
+extern "C" int te_eraser_soft_scores(const float* word_scores, int batch, const int* word_offsets, const int* span_offsets,
+                                     const int* spans, const int* tail_counts, double* scores, int* flags, void* workspace,
+                                     long long workspace_bytes, void* stream) {
+    REQ(word_offsets && span_offsets && tail_counts && scores && flags, "te_eraser_soft_scores: null argument");
+    REQ(batch > 0 && batch <= 65535, "te_eraser_soft_scores: batch must lie in 1..65535");
+    REQ(word_offsets[0] == 0 && span_offsets[0] == 0, "te_eraser_soft_scores: offsets must start at 0");
+    for (int b = 0; b < batch; ++b) {
+        const long long nw = (long long)word_offsets[b + 1] - word_offsets[b];
+        REQ(nw >= 0 && nw <= TE_ERASER_MAX_WORDS, "te_eraser_soft_scores: a document holds 0..TE_ERASER_MAX_WORDS words");
+        REQ(span_offsets[b + 1] >= span_offsets[b], "te_eraser_soft_scores: span offsets must be non-decreasing");
+        const long long tp = tail_counts[2 * b], tn = tail_counts[2 * b + 1];
+        REQ(tp >= 0 && tn >= 0 && tp + tn <= (1 << 30), "te_eraser_soft_scores: tail counts must lie in 0..2^30");
+        REQ(nw + tp + tn >= 1, "te_eraser_soft_scores: a document needs a word or a tail word");
+    }
+    const long long words = word_offsets[batch], nspans = span_offsets[batch];
+    REQ(words == 0 || word_scores, "te_eraser_soft_scores: null word scores");
+    REQ(nspans == 0 || spans, "te_eraser_soft_scores: null spans");
+    for (long long j = 0; j < nspans; ++j)
+        REQ(spans[2 * j] >= 0 && spans[2 * j] <= spans[2 * j + 1],
+            "te_eraser_soft_scores: every truth span (start, end) must satisfy 0 <= start <= end");
+    REQ(workspace && (((uintptr_t)workspace) & 255u) == 0, "te_eraser_soft_scores: workspace null or not 256-byte aligned");
+    if (te_eraser_soft_workspace_bytes(batch, nspans) > workspace_bytes) {
+        te_set_last_error("te_eraser_soft_scores: workspace too small");
+        return TE_ERR_WORKSPACE;
+    }
+    char* p = static_cast<char*>(workspace);
+    int* d_woff = reinterpret_cast<int*>(p);
+    p += up256(4LL * (batch + 1));
+    int* d_soff = reinterpret_cast<int*>(p);
+    p += up256(4LL * (batch + 1));
+    int2* d_spans = reinterpret_cast<int2*>(p);
+    p += up256(8 * nspans);
+    int2* d_tail = reinterpret_cast<int2*>(p);
+    cudaStream_t st = ST(stream);
+    if (cudaMemcpyAsync(d_woff, word_offsets, 4 * (size_t)(batch + 1), cudaMemcpyHostToDevice, st) != cudaSuccess ||
+        cudaMemcpyAsync(d_soff, span_offsets, 4 * (size_t)(batch + 1), cudaMemcpyHostToDevice, st) != cudaSuccess ||
+        (nspans && cudaMemcpyAsync(d_spans, spans, 8 * (size_t)nspans, cudaMemcpyHostToDevice, st) != cudaSuccess) ||
+        cudaMemcpyAsync(d_tail, tail_counts, 8 * (size_t)batch, cudaMemcpyHostToDevice, st) != cudaSuccess) {
+        te_set_last_error("te_eraser_soft_scores: copy of the host arrays failed");
+        return TE_ERR_CUDA;
+    }
+    soft_kernel<<<batch, kThreads, 0, st>>>(word_scores, d_woff, d_soff, d_spans, d_tail, scores, flags);
     TE_CUDA_CHECK_LAUNCH();
     return TE_OK;
 }

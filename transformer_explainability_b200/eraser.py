@@ -24,8 +24,7 @@ Deviations from the reference (DESIGN.md §1):
    the gradients and min-max normalises over the whole [S, S] map, padded query rows included, so its batches only hold
    documents of one length;
  * one annotation per document and split (the pipeline keys its predictions by docid: two annotations of one document would
-   merge into one key), and every annotation needs an evidence; otherwise ``ValueError``;
- * soft-token metrics (AUPRC, AP) are not computed.
+   merge into one key), and every annotation needs an evidence; otherwise ``ValueError``.
 
 With ``faithfulness=True`` (CLI ``--faithfulness``) the same pass also measures ``metrics.py``'s faithfulness
 (``score_classifications``, ``:255-364``): per batch one more engine forward gives the original logits, one
@@ -34,12 +33,21 @@ words kept) rows of every selection size, the rows run through the engine forwar
 ``te_class_probs`` turns each chunk's logits into probabilities on the device.  The selection sizes, the default k and the
 row layout are defined in DESIGN.md §1; the result lines go to ``faithfulness_results.jsonl`` and ``metrics.py``'s
 ``classification_scores`` dict to ``faithfulness_scores.json``.
+
+With ``tokens_to_flip=True`` (CLI ``--tokens-to-flip``, with ``--faithfulness``) each batch also searches, in rounds of
+``flip_chunk`` selection sizes, for each document's smallest k whose comprehensiveness row changes the prediction
+(``te_eraser_reduce_inputs`` rows, the chunked engine forward, ``te_logit_stats``' argmax): the ``tokens_to_flip`` field of
+``faithfulness_results.jsonl`` and ``tokens_to_flip.json``.  With ``soft_scores=True`` (CLI ``--soft-scores``) one
+``te_eraser_soft_scores`` call per batch scores the word scores, followed by a 0 per word past truncation, as
+``metrics.py``'s soft predictions (``score_soft_tokens``: AUPRC, average precision, ROC AUC): ``soft_results.jsonl`` and
+``soft_scores.json``.  Both are defined in DESIGN.md §1.
 """
 import argparse
 import functools
 import json
 import math
 import os
+import warnings
 from dataclasses import dataclass
 from typing import FrozenSet, Optional, Tuple, Union
 
@@ -412,15 +420,17 @@ def classification_scores_from_probs(annotations, class_names, pred, probs, comp
     return out
 
 
-def faithfulness_lines(annotations, docids, class_names, pred, probs, comp, suff, thresholds, selected):
+def faithfulness_lines(annotations, docids, class_names, pred, probs, comp, suff, thresholds, selected, tokens_to_flip=None):
     """One ``metrics.py`` result line per annotation (keyed by its own annotation id): the main-k words as
     ``hard_rationale_predictions``, ``classification``, ``classification_scores``, the main-k comprehensiveness and
-    sufficiency scores and one ``thresholded_scores`` entry per threshold."""
+    sufficiency scores and one ``thresholded_scores`` entry per threshold; with ``tokens_to_flip`` (one int per
+    annotation) also that field, last."""
     def scores(p):
         return {c: float(v) for c, v in zip(class_names, p)}
     out = []
     for i, (a, d) in enumerate(zip(annotations, docids)):
-        out.append(json.dumps({
+        extra = {} if tokens_to_flip is None else {"tokens_to_flip": int(tokens_to_flip[i])}
+        out.append(json.dumps(dict({
             "annotation_id": a.annotation_id,
             "rationales": [{"docid": d, "hard_rationale_predictions": [{"start_token": int(w), "end_token": int(w) + 1}
                                                                        for w in selected[i]]}],
@@ -429,8 +439,125 @@ def faithfulness_lines(annotations, docids, class_names, pred, probs, comp, suff
             "sufficiency_classification_scores": scores(suff[i][0]),
             "thresholded_scores": [{"threshold": float(t), "comprehensiveness_classification_scores": scores(comp[i][1 + j]),
                                     "sufficiency_classification_scores": scores(suff[i][1 + j])}
-                                   for j, t in enumerate(thresholds)]}))
+                                   for j, t in enumerate(thresholds)]}, **extra)))
     return out
+
+
+def flip_scores(annotations, docids, n_words, tokens, flipped):
+    """``tokens_to_flip.json``: the mean fraction of the document's words, as ``metrics.py`` averages it (``:337-346``:
+    tokens / document words per annotation, ``np.average``), the number of documents that never flipped and the
+    per-document values, in annotation order."""
+    frac = [int(t) / int(n) for t, n in zip(tokens, n_words)]
+    return {"tokens_to_flip": np.average(frac), "never_flipped": int(len(flipped) - np.count_nonzero(flipped)),
+            "documents": [{"annotation_id": a.annotation_id, "docid": d, "tokens_to_flip": int(t), "words": int(n),
+                           "fraction": f, "flipped": bool(fl)}
+                          for a, d, t, n, f, fl in zip(annotations, docids, tokens, n_words, frac, flipped)]}
+
+
+# ---- soft-token scores: metrics.py's score_soft_tokens ----------------------------------------------------------------------
+def soft_truth(truth, annotation, docid, W, n_words):
+    """(the truth spans of (annotation id, docid), (positives, negatives) past the W scored words): the truth side of
+    ``PositionScoredDocument.from_results`` for a document of n_words words.  A span past the document raises
+    ``ValueError`` (the reference's truth vector has no room for it)."""
+    spans = truth.spans_by_key.get((annotation.annotation_id, docid), [])
+    if any(e > n_words for _, e in spans):
+        raise ValueError("annotation %r: a truth span ends past document %r's %d words"
+                         % (annotation.annotation_id, docid, n_words))
+    pos = len(set(t for s, e in spans for t in range(max(s, W), e)))
+    return spans, (pos, n_words - W - pos)
+
+
+def soft_token_scores(per_doc, single_class):
+    """``score_soft_tokens``' dict (``metrics.py:217-253``) from the per-document (AUPRC, AP, ROC AUC) rows and
+    single-class flags, in annotation order: AUPRC averaged over every document, AP and ROC AUC over the documents that
+    hold both classes (``_score_aggregator(..., True)``; none: numpy's mean of nothing, NaN)."""
+    if len(per_doc) == 0:
+        return {"auprc": 0.0, "average_precision": 0.0, "roc_auc_score": 0.0}
+    per_doc = np.asarray(per_doc, dtype=np.float64)
+    keep = [i for i in range(len(per_doc)) if not single_class[i]]
+    with warnings.catch_warnings():
+        warnings.simplefilter("ignore")
+        return {"auprc": np.average(per_doc[:, 0].tolist()), "average_precision": np.average(per_doc[keep, 1].tolist()),
+                "roc_auc_score": np.average(per_doc[keep, 2].tolist())}
+
+
+def soft_lines(annotations, docids, word_scores, n_words):
+    """One ``metrics.py`` result line per annotation: ``soft_rationale_predictions`` = the W fp32 word scores, then a 0
+    for each word past truncation (one score per document word, as ``PositionScoredDocument.from_results`` asserts)."""
+    return [json.dumps({"annotation_id": a.annotation_id, "rationales": [{"docid": d, "soft_rationale_predictions":
+                                                                          [float(x) for x in s] + [0.0] * (n - len(s))}]})
+            for a, d, s, n in zip(annotations, docids, word_scores, n_words)]
+
+
+def _sorted_chunks(eng, flat, lens, rows, cap, device):
+    """The rows ``rows`` of flat [R, S] (host lengths ``lens[q]``), longest first, through the engine forward in padded
+    chunks of at most ``cap`` rows (default: the engine's ``max_chunk`` at the chunk's length): yields (chunk, L, logits)."""
+    rows = sorted(rows, key=lambda q: -int(lens[q]))               # longest first: each chunk's first row sets S
+    s0 = 0
+    while s0 < len(rows):
+        L = int(lens[rows[s0]])
+        chunk = rows[s0:s0 + (cap or eng.max_chunk(L))]
+        sel = torch.as_tensor(chunk, device=device)
+        x = flat.index_select(0, sel)[:, :L].contiguous()
+        m = (torch.arange(L, device=device)[None, :] <
+             torch.as_tensor(lens[chunk], device=device)[:, None]).to(torch.int64)
+        yield chunk, L, eng.forward(x, m)
+        s0 += len(chunk)
+
+
+def _flip_search(eng, maps, ids, lens, ranges, woff, orders, pred0, n_words, flip_chunk, cap):
+    """Tokens to flip of one batch (DESIGN.md §1): in rounds, every unfinished document b runs the comprehensiveness
+    rows of its next ``flip_chunk`` selection sizes (``te_eraser_reduce_inputs``; their lengths follow on the host from
+    the full word order ``orders[b]``), in length-sorted chunks, and ``te_logit_stats`` gives their argmax; one copy of
+    the round's predictions finds each document's first flip.  Returns (tokens [B], flipped [B], rows, real tokens,
+    padded tokens)."""
+    from . import ops
+    B, device = len(lens), maps.device
+    W = np.diff(np.asarray(woff))
+    comp_len = []                                                  # comp_len[b][k - 1]: the row length at selection k
+    for b in range(B):
+        seen, cl = set(), []
+        for w in orders[b][:W[b]]:
+            a, e = ranges[woff[b] + int(w)]
+            seen.update(range(a, e + 1))
+            cl.append(lens[b] - len(seen))
+        comp_len.append(cl)
+    nxt = [1] * B
+    tokens = [None if W[b] else n_words[b] for b in range(B)]
+    flipped = [False] * B
+    n_rows = real = padded = 0
+    while any(t is None for t in tokens):
+        live = [b for b in range(B) if tokens[b] is None]
+        J = min(flip_chunk, max(W[b] - nxt[b] + 1 for b in live))
+        nsel = np.zeros((B, J), dtype=np.int64)
+        rows, rlen = [], np.zeros(B * J * 2, dtype=np.int64)
+        for b in live:
+            for j, k in enumerate(range(nxt[b], min(nxt[b] + J, W[b] + 1))):
+                nsel[b, j] = k
+                rows.append((b * J + j) * 2)
+                rlen[rows[-1]] = comp_len[b][k - 1]
+        red = ops.eraser_reduce_inputs(maps, ids, lens, ranges, woff, nsel)
+        flat = red["ids"].reshape(B * J * 2, -1)
+        pred = torch.empty(len(rows), dtype=torch.int32, device=device)
+        slot, s = {}, 0
+        for chunk, L, logits in _sorted_chunks(eng, flat, rlen, rows, cap, device):
+            pred[s:s + len(chunk)] = ops.logit_stats(logits, torch.zeros(len(chunk), dtype=torch.int32, device=device))[0]
+            slot.update((q, s + i) for i, q in enumerate(chunk))
+            s += len(chunk)
+            real += int(rlen[chunk].sum())
+            padded += len(chunk) * L
+        n_rows += len(rows)
+        ph = pred.cpu().numpy()
+        for b in live:
+            ks = range(nxt[b], min(nxt[b] + J, W[b] + 1))
+            hit = next((k for j, k in enumerate(ks) if ph[slot[(b * J + j) * 2]] != pred0[b]), None)
+            if hit is not None:
+                tokens[b], flipped[b] = hit, True
+            else:
+                nxt[b] += len(ks)
+                if nxt[b] > W[b]:
+                    tokens[b] = n_words[b]
+    return tokens, flipped, n_rows, real, padded
 
 
 def _generator_model(generator_method):
@@ -452,7 +579,8 @@ def _check_fraction(f, what):
 # ---- the evaluation ---------------------------------------------------------------------------------------------------------
 def eraser_eval(generator_method, documents, annotations, encodings, evidence_classes, batch_size=8, ks=KS,
                 iou_thresholds=(0.5,), pad_id=0, device=None, same_length=None, faithfulness=False,
-                aopc_thresholds=AOPC_THRESHOLDS, k_fraction=None, faith_chunk=None):
+                aopc_thresholds=AOPC_THRESHOLDS, k_fraction=None, faith_chunk=None, soft_scores=False,
+                tokens_to_flip=False, flip_chunk=16):
     """The test loop of the pipeline (``bert_pipeline.py:456-582``) and ``metrics.py``'s hard scores on the engine.
 
     generator_method: a bound ``Generator`` method (``generate_LRP`` keeps its ``start_layer = 11``), called as
@@ -470,11 +598,23 @@ def eraser_eval(generator_method, documents, annotations, encodings, evidence_cl
     ``faith_chunk`` rows (default: the engine's ``max_chunk`` at the chunk's length).  The other keys are unchanged, and
     a key "faithfulness" holds {"fractions", "n_select" [docs, 1 + T], "pred" [docs], "logits" [docs, C], "probs"
     [docs, C], "comp" / "suff" [docs, 1 + T, C] (fp32 probabilities), "lines", "scores", "real_tokens",
-    "padded_tokens"}."""
+    "padded_tokens"}.
+
+    With ``soft_scores`` the same word scores also give ``metrics.py``'s soft-token scores (one ``te_eraser_soft_scores``
+    call per batch), in a key "soft": {"per_document" [docs, 3] (AUPRC, AP, ROC AUC), "single_class" [docs], "lines",
+    "scores"}; a NaN word score raises ``ValueError``.  With ``tokens_to_flip`` (needs ``faithfulness``) each batch's
+    maps also drive the tokens-to-flip search (DESIGN.md §1) in rounds of ``flip_chunk`` selection sizes per document;
+    "faithfulness" gains "tokens_to_flip" [docs], "flipped" [docs], "flip_scores" (``tokens_to_flip.json``),
+    "flip_rows", "flip_real_tokens" and "flip_padded_tokens", and its lines the ``tokens_to_flip`` field."""
     ks = tuple(int(k) for k in ks)
+    if tokens_to_flip and not faithfulness:
+        raise ValueError("tokens_to_flip needs faithfulness (metrics.py reads it with the classification fields)")
+    if tokens_to_flip and not 1 <= int(flip_chunk) <= _lib.ERASER_MAX_SELECTIONS:
+        raise ValueError("flip_chunk must lie in 1..%d" % _lib.ERASER_MAX_SELECTIONS)
     docids = [annotation_docid(a) for a in annotations]
     if len(set(docids)) != len(docids):
         raise ValueError("two annotations of the split share a document; the pipeline keys its predictions by docid")
+    n_words = [len(documents[d].split()) for d in docids]
     truth = TruthIndex(annotations)
     ranges = {d: word_piece_ranges(documents[d].split(), encodings[d][1]) for d in set(docids)}
     targets = [evidence_classes[a.classification] for a in annotations]
@@ -512,7 +652,19 @@ def eraser_eval(generator_method, documents, annotations, encodings, evidence_cl
         n_orig, slot, real_tok, padded_tok = 0, n, 0, 0
         selected = [None] * n
         kfull = max(kmax, int(nsel[:, 0].max()) if n else 0)
+        if tokens_to_flip:                                          # the search needs every document's full order
+            if C < 2:
+                raise ValueError("tokens_to_flip needs at least two classes")
+            kfull = max([kfull] + [len(ranges[d]) for d in docids])
+            flip_tok = np.zeros(n, dtype=np.int64)
+            flipped = np.zeros(n, dtype=bool)
+            flip_stats = [0, 0, 0]
         ks_run = ks + ((kfull,) if kfull > kmax else ())
+    if soft_scores:
+        soft_doc = np.zeros((n, 3), dtype=np.float64)
+        single = np.zeros(n, dtype=bool)
+        soft_words = [None] * n
+        soft_truths = [soft_truth(truth, a, d, len(ranges[d]), nw) for a, d, nw in zip(annotations, docids, n_words)]
     by_len = sorted(range(n), key=lambda i: len(encodings[docids[i]][0]))
     batches = []
     for i in by_len:
@@ -540,6 +692,13 @@ def eraser_eval(generator_method, documents, annotations, encodings, evidence_cl
         maps = maps.reshape(len(idx), S).to(torch.float32).contiguous()
         res = ops.eraser_rationales(maps, wr, woff, sp, soff, ks_run, iou_thresholds)
         parts = [res["order"].reshape(len(idx), -1), res["counts"].reshape(len(idx), -1)]
+        if soft_scores:
+            ssp, ssoff = [], [0]
+            for i in idx:
+                ssp.extend(soft_truths[i][0])
+                ssoff.append(len(ssp))
+            soft = ops.eraser_soft_scores(res["word_scores"], woff, ssp, ssoff, [soft_truths[i][1] for i in idx])
+            parts += [soft["scores"].view(torch.int32).reshape(len(idx), 6), soft["flags"]]
         if faithfulness:
             B, o = len(idx), n_orig
             logits = eng.forward(ids_d, mask_d)
@@ -547,34 +706,45 @@ def eraser_eval(generator_method, documents, annotations, encodings, evidence_cl
             ops.class_probs(logits, out=buf[o:o + B])
             orig_slot[idx] = np.arange(o, o + B)
             n_orig += B
-            red = ops.eraser_reduce_inputs(maps, ids_d, [len(encodings[docids[i]][0]) for i in idx], wr, woff, nsel[idx])
+            tok_lens = [len(encodings[docids[i]][0]) for i in idx]
+            red = ops.eraser_reduce_inputs(maps, ids_d, tok_lens, wr, woff, nsel[idx])
             parts.append(red["lengths"].reshape(B, -1).to(parts[0].dtype))
+            if tokens_to_flip:                                      # te_logit_stats' pred: the first maximum
+                parts.append(ops.logit_stats(logits, torch.zeros(B, dtype=torch.int32, device=device))[0][:, None])
         host = torch.cat(parts, dim=1).cpu().numpy()
         kr = ks_run[-1]
         order[idx] = host[:, :kmax]
         counts[idx] = host[:, kr:kr + len(ks) * ncol].reshape(len(idx), len(ks), ncol)
+        c0 = kr + len(ks_run) * ncol
+        if soft_scores:
+            soft_doc[idx] = np.ascontiguousarray(host[:, c0:c0 + 6]).view(np.float64)
+            single[idx] = host[:, c0 + 6] != 0
+            bad = [docids[i] for r, i in enumerate(idx) if host[r, c0 + 7]]
+            if bad:
+                raise ValueError("document %r has a NaN word score; metrics.py's soft-token scores (sklearn) reject NaN"
+                                 % bad[0])
+            ws_host = res["word_scores"].cpu().numpy()
+            for r, i in enumerate(idx):
+                soft_words[i] = ws_host[woff[r]:woff[r + 1]]
+            c0 += 8
         if faithfulness:
             for r, i in enumerate(idx):
                 selected[i] = host[r, :nsel[i, 0]].tolist()
-            lens = host[:, kr + len(ks_run) * ncol:].reshape(-1)          # [B * J * 2], rows (document, selection, kind)
-            rows = sorted(range(len(lens)), key=lambda q: -int(lens[q]))  # longest first: each chunk's first row sets S
+            lens = host[:, c0:c0 + 2 * J].reshape(-1)                    # [B * J * 2], rows (document, selection, kind)
             flat = red["ids"].reshape(len(lens), S)
-            s0 = 0
-            while s0 < len(rows):
-                L = int(lens[rows[s0]])
-                chunk = rows[s0:s0 + (faith_chunk or eng.max_chunk(L))]
-                sel = torch.as_tensor(chunk, device=device)
-                x = flat.index_select(0, sel)[:, :L].contiguous()
-                m = (torch.arange(L, device=device)[None, :] <
-                     torch.as_tensor(lens[chunk], device=device)[:, None]).to(torch.int64)
-                ops.class_probs(eng.forward(x, m), out=buf[slot:slot + len(chunk)])
+            for chunk, L, logits_c in _sorted_chunks(eng, flat, lens, range(len(lens)), faith_chunk, device):
+                ops.class_probs(logits_c, out=buf[slot:slot + len(chunk)])
                 for q_i, q in enumerate(chunk):
                     r, rest = divmod(q, 2 * J)
                     red_slot[idx[r], rest // 2, rest % 2] = slot + q_i
                 slot += len(chunk)
                 real_tok += int(lens[chunk].sum())
                 padded_tok += len(chunk) * L
-                s0 += len(chunk)
+            if tokens_to_flip:                                      # the batch's maps stay on the device until it ends
+                t, fl, *st = _flip_search(eng, maps, ids_d, tok_lens, wr, woff, host[:, :kr], host[:, c0 + 2 * J],
+                                          [n_words[i] for i in idx], int(flip_chunk), faith_chunk)
+                flip_tok[idx], flipped[idx] = t, fl
+                flip_stats = [a + b for a, b in zip(flip_stats, st)]
     lines = rationale_lines(docids, ks=ks, order=order)
     scores = {k: hard_scores(truth, docids, counts[:, i], order, iou_thresholds) for i, k in enumerate(ks)}
     out = {"docids": docids, "word_ranges": [ranges[d] for d in docids], "order": order, "counts": counts,
@@ -587,16 +757,28 @@ def eraser_eval(generator_method, documents, annotations, encodings, evidence_cl
         thr = fracs[1:]
         out["faithfulness"] = {
             "fractions": fracs, "n_select": nsel, "pred": pred, "logits": logits, "probs": probs, "comp": comp,
-            "suff": suff, "lines": faithfulness_lines(annotations, docids, names, pred, probs, comp, suff, thr, selected),
+            "suff": suff, "lines": faithfulness_lines(annotations, docids, names, pred, probs, comp, suff, thr, selected,
+                                                      flip_tok if tokens_to_flip else None),
             "scores": classification_scores_from_probs(annotations, names, pred, probs, comp, suff, thr, thr),
             "real_tokens": real_tok, "padded_tokens": padded_tok}
+        if tokens_to_flip:
+            out["faithfulness"].update({
+                "tokens_to_flip": flip_tok, "flipped": flipped,
+                "flip_scores": flip_scores(annotations, docids, n_words, flip_tok, flipped), "flip_rows": flip_stats[0],
+                "flip_real_tokens": flip_stats[1], "flip_padded_tokens": flip_stats[2]})
+    if soft_scores:
+        out["soft"] = {"per_document": soft_doc, "single_class": single,
+                       "lines": soft_lines(annotations, docids, soft_words, n_words),
+                       "scores": soft_token_scores(soft_doc, single)}
     return out
 
 
 def write_results(results, folder):
     """``identifier_results_{k}.json`` (the pipeline's files) and ``scores_{k}.json`` (``metrics.py``'s ``--score_file``
     layout: indent 4, sorted keys) under ``folder``; with faithfulness results also ``faithfulness_results.jsonl``
-    (``metrics.py``'s results format) and ``faithfulness_scores.json`` (its ``classification_scores`` dict)."""
+    (``metrics.py``'s results format) and ``faithfulness_scores.json`` (its ``classification_scores`` dict), with
+    tokens to flip also ``tokens_to_flip.json``; with soft scores ``soft_results.jsonl`` and ``soft_scores.json``
+    (``score_soft_tokens``' dict)."""
     os.makedirs(folder, exist_ok=True)
     for k, lines in results["lines"].items():
         with open(os.path.join(folder, "identifier_results_%d.json" % k), "w") as f:
@@ -608,6 +790,14 @@ def write_results(results, folder):
             f.write("".join(line + "\n" for line in results["faithfulness"]["lines"]))
         with open(os.path.join(folder, "faithfulness_scores.json"), "w") as f:
             json.dump(results["faithfulness"]["scores"], f, indent=4, sort_keys=True)
+        if "flip_scores" in results["faithfulness"]:
+            with open(os.path.join(folder, "tokens_to_flip.json"), "w") as f:
+                json.dump(results["faithfulness"]["flip_scores"], f, indent=4, sort_keys=True)
+    if "soft" in results:
+        with open(os.path.join(folder, "soft_results.jsonl"), "w") as f:
+            f.write("".join(line + "\n" for line in results["soft"]["lines"]))
+        with open(os.path.join(folder, "soft_scores.json"), "w") as f:
+            json.dump(results["soft"]["scores"], f, indent=4, sort_keys=True)
 
 
 # ---- command line ---------------------------------------------------------------------------------------------------------
@@ -630,6 +820,11 @@ def build_parser():
     p.add_argument("--k-fraction", dest="k_fraction", type=float, default=None,
                    help="fraction of words removed / kept for the main comprehensiveness and sufficiency (default: the "
                         "split's mean fraction of words inside a human rationale)")
+    p.add_argument("--soft-scores", dest="soft_scores", action="store_true",
+                   help="also score the word scores as soft predictions (metrics.py score_soft_tokens: AUPRC, AP, ROC AUC)")
+    p.add_argument("--tokens-to-flip", dest="tokens_to_flip", action="store_true",
+                   help="also find each document's tokens to flip: the fewest best-ranked words whose removal changes "
+                        "the prediction (needs --faithfulness)")
     return p
 
 
@@ -646,6 +841,8 @@ def parse_args(argv=None):
         p.error("--aopc-thresholds takes distinct fractions in (0, 1]")
     if args.k_fraction is not None and not 0.0 < args.k_fraction <= 1.0:
         p.error("--k-fraction must lie in (0, 1]")
+    if args.tokens_to_flip and not args.faithfulness:
+        p.error("--tokens-to-flip needs --faithfulness")
     if args.state_dict is None:
         args.state_dict = os.path.join(args.output_dir, "classifier", "classifier.pt")
     return args
@@ -686,7 +883,8 @@ def main(argv=None):
     gen = build_generator(args.method, params["bert_dir"], len(classes), args.state_dict)
     res = eraser_eval(gen, documents, annotations, encodings, evidence_classes, batch_size=args.batch_size,
                       iou_thresholds=args.iou_thresholds, faithfulness=args.faithfulness,
-                      aopc_thresholds=args.aopc_thresholds, k_fraction=args.k_fraction)
+                      aopc_thresholds=args.aopc_thresholds, k_fraction=args.k_fraction, soft_scores=args.soft_scores,
+                      tokens_to_flip=args.tokens_to_flip)
     write_results(res, os.path.join(args.output_dir, METHOD_FOLDER[args.method]))
     for k in KS:
         print("top-%d token F1 %.4f (instance macro %.4f)" % (k, res["scores"][k]["token_prf"]["instance_micro"]["f1"],
@@ -697,6 +895,13 @@ def main(argv=None):
                                                                             f["comprehensiveness"], f["sufficiency"]))
         print("AOPC over %s: comprehensiveness %.4f, sufficiency %.4f" % (f["aopc_thresholds"], f["comprehensiveness_aopc"],
                                                                          f["sufficiency_aopc"]))
+    if args.tokens_to_flip:
+        t = res["faithfulness"]["flip_scores"]
+        print("tokens to flip: mean fraction %.4f, %d of %d documents never flipped" % (
+            t["tokens_to_flip"], t["never_flipped"], len(t["documents"])))
+    if args.soft_scores:
+        s = res["soft"]["scores"]
+        print("soft tokens: AUPRC %.4f, AP %.4f, ROC AUC %.4f" % (s["auprc"], s["average_precision"], s["roc_auc_score"]))
     return res
 
 

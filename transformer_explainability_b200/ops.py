@@ -711,6 +711,41 @@ def eraser_reduce_inputs(maps, input_ids, lengths, piece_ranges, word_offsets, n
     return out
 
 
+@_on_device
+def eraser_soft_scores(word_scores, word_offsets, spans, span_offsets, tail_counts):
+    """``metrics.py``'s soft-token scores of each document b: its word scores ``word_scores[word_offsets[b]:
+    word_offsets[b+1]]`` (fp32 CUDA, as ``eraser_rationales`` returns them) followed by its tail of
+    ``tail_counts[b] = (positives, negatives)`` words past truncation, which score 0, against the truth spans
+    ``spans[span_offsets[b]:span_offsets[b+1]]`` of (start, end) word indices (see include/te_b200.h:
+    te_eraser_soft_scores).  The offsets, spans and tail counts are host sequences.  Returns a dict of CUDA tensors:
+    ``scores`` fp64 [B, 3] (AUPRC, average precision, ROC AUC), ``flags`` int32 [B, 2] (single class, NaN or negative
+    score)."""
+    if not (word_scores.is_cuda and word_scores.dtype == torch.float32 and word_scores.dim() == 1 and
+            word_scores.is_contiguous()):
+        raise ValueError("eraser_soft_scores: word_scores fp32 [words] contiguous on a CUDA device expected")
+    op = "eraser_soft_scores"
+    woff = _host_i32(word_offsets, "word_offsets", op=op)
+    soff = _host_i32(span_offsets, "span_offsets", op=op)
+    tails = _host_i32(tail_counts, "tail_counts", 2, op=op)
+    B = len(woff) - 1
+    if B < 1 or soff.shape != (B + 1,) or tails.shape != (B, 2):
+        raise ValueError("eraser_soft_scores: word_offsets and span_offsets need B + 1 entries and tail_counts [B, 2]")
+    sp = _host_i32(spans, "spans", 2, op=op)
+    if int(woff[-1]) != word_scores.numel() or len(sp) != int(soff[-1]):
+        raise ValueError("eraser_soft_scores: %d word scores / %d spans, the offsets end at %d / %d"
+                         % (word_scores.numel(), len(sp), woff[-1], soff[-1]))
+    lib = _lib.load()
+    dev = word_scores.device
+    ws = _workspace(check(lib.te_eraser_soft_workspace_bytes(B, len(sp)), "te_eraser_soft_workspace_bytes"), dev)
+    out = {"scores": torch.empty(B, 3, device=dev, dtype=torch.float64),
+           "flags": torch.empty(B, 2, device=dev, dtype=torch.int32)}
+    host = lambda a: a.ctypes.data_as(_lib.c_void_p) if a.size else None      # noqa: E731
+    check(lib.te_eraser_soft_scores(ptr(word_scores) if word_scores.numel() else None, B, host(woff), host(soff), host(sp),
+                                    host(tails), ptr(out["scores"]), ptr(out["flags"]), ptr(ws), ws.numel() * 4,
+                                    _stream()), "te_eraser_soft_scores")
+    return out
+
+
 # ---- input preparation (baselines/ViT/generate_visualizations.py: Resize((224, 224)) + ToTensor()) ---------------------------
 @_on_device
 def prepare_images(packed_u8, sizes, offsets, out_hw=(224, 224), mean=None, std=None):
