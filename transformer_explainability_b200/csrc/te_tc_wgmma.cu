@@ -633,7 +633,9 @@ struct ZrProb {
     using PRODS = Prods<Pr<0, 0, 0>, Pr<1, 0, 1>>;           // S W+ and S W- into their own accumulators
     using L = Stage<PRODS, BN>;
     static constexpr bool TMA = true;
-    static constexpr int FIX = FIX_NONE, EPI_MAPS = 1;           // x, staged by the producer
+    // x, staged by the producer, except for KIND 0: its 64 KB buffer would cost it one of four 48 KB stages, and the TF32
+    // kernel runs faster with the stage and x read from global memory in the epilogue
+    static constexpr int FIX = FIX_NONE, EPI_MAPS = KIND == 0 ? 0 : 1;
     int M, N, K;
     const void* s; const void* wp; const void* wn;     // S [M, K] (row stride K), W+^T / W-^T [N, K]
     const float* rs; int rs_ld; const float* cp; const float* cn;   // KIND 2: scales of S, of the rows of W+^T / W-^T
@@ -647,15 +649,17 @@ struct ZrProb {
         if (i == 0) return TmaTile{s, M, K, K, BM};
         return i < 3 ? TmaTile{i == 1 ? wp : wn, N, K, K, BN} : TmaTile{x, M, N, ldx, BM};
     }
-    // x comes from the epilogue buffer (eb), the column scales from global memory.  Accumulating, each thread reads the
-    // out elements it then writes, from global memory: out is not staged (it may alias x, and the value read must be the
-    // one the previous launch left), and its reads are done for the whole fragment into acc[0] before the first store.
+    // x comes from the epilogue buffer (eb), or for KIND 0 from global memory, the column scales from global memory.
+    // Accumulating, each thread reads the out elements it then writes, from global memory: out is not staged (it may alias
+    // x, and the value read must be the one the previous launch left).  All reads of the fragment are done into acc[0]
+    // before the first store.
     __device__ void epilogue(float (&acc)[2][BN / 2], int m0, int n0, int, int tid, const uint8_t* eb) const {
 #pragma unroll
         for (int j = 0; j < BN / 2; j += 2) {
             const int row = m0 + frag_row(tid, j), col = n0 + frag_col(tid, j);
             if (row >= M) continue;
-            const float2 xv = epi_f2(eb, frag_row(tid, j), frag_col(tid, j));
+            const float2 xv = EPI_MAPS ? epi_f2(eb, frag_row(tid, j), frag_col(tid, j))
+                                       : *reinterpret_cast<const float2*>(x + (long long)row * ldx + col);
             float2 ap = make_float2(acc[0][j], acc[0][j + 1]), an = make_float2(acc[1][j], acc[1][j + 1]);
             if (KIND == 2) {
                 ap.x *= cp[col]; ap.y *= cp[col + 1];
@@ -810,15 +814,22 @@ static_assert(sizeof(LinArgs) <= 128, "LinArgs: keep the kernel parameter within
 template <int EPI, int FORM>
 struct LinProb : LinArgs {
     static constexpr bool F16 = FORM == LIN_F16X3 || FORM == LIN_F16, SPLIT = FORM == LIN_3XTF32 || FORM == LIN_F16X3;
-    static constexpr int BN = 128, CHUNK = F16 ? 2 : SPLIT ? 4 : 0, FMT = F16 ? OP_F16 : OP_TF32;
+    // The single-pass TF32 STORE form (one accumulator, no epilogue buffer) takes 256 columns: 48 KB per stage (4 stages)
+    // for twice the MMAs of a 32 KB stage at 128, and the tf32(A) fix serves twice the columns.  The others stay at 128:
+    // the chunked forms' acc + tot, and GELU_BWD's E buffer, would not fit at 256.  The epilogue guards the columns past N
+    // (N a multiple of 128).
+    static constexpr int BN = FORM == LIN_TF32 && EPI == TE_TC_EPI_STORE ? 256 : 128;
+    static constexpr int CHUNK = F16 ? 2 : SPLIT ? 4 : 0, FMT = F16 ? OP_F16 : OP_TF32;
     using PRODS = std::conditional_t<SPLIT, Split3, One>;
     using L = Stage<PRODS, BN>;
     static constexpr bool COL_FAST = true;
     // the fp16 forms and the single-pass TF32 form (A rounded in shared memory) on TMA; 3xTF32 splits A on load
     static constexpr bool TMA = FORM != LIN_3XTF32;
     static constexpr int FIX = FORM == LIN_TF32 ? FIX_A : FIX_NONE;
-    // E of BIAS_ADD / GELU_BWD, staged by the producer on the TMA mainloop
-    static constexpr int EPI_MAPS = TMA && (EPI == TE_TC_EPI_BIAS_ADD || EPI == TE_TC_EPI_GELU_BWD) ? 1 : 0;
+    // E of GELU_BWD, staged by the producer on the TMA mainloop.  E of BIAS_ADD (the fp16-split forward, 64 KB stages) is
+    // read from global memory before the first store: its 64 KB buffer would cost it one of three stages, and that form
+    // runs faster with the stage.
+    static constexpr int EPI_MAPS = TMA && EPI == TE_TC_EPI_GELU_BWD ? 1 : 0;
     __device__ int kblocks() const { return K / (F16 ? 64 : 32); }
     __device__ float chunk_scale(int row, int ch, int) const {
         if constexpr (F16) return row < o.M ? rs[(long long)row * rs_ld + ch] : 1.f;
@@ -838,13 +849,18 @@ struct LinProb : LinArgs {
         for_k32(BN, (const float*)b, K, n0, o.N, kb * 32, K, tid, [&](int r, int c, float4 v) { st4(st + L::b(0), r, c, v); });
         for_k32(BN, (const float*)b_lo, K, n0, o.N, kb * 32, K, tid, [&](int r, int c, float4 v) { st4(st + L::b(1), r, c, v); });
     }
-    // E from the epilogue buffer (eb) on the TMA mainloop, from global memory on the register mainloop (3xTF32); bias and
-    // the column scales from global memory, before the first store
+    // E from the epilogue buffer (eb) when staged, else from global memory; bias, the column scales and an unstaged E of
+    // BIAS_ADD from global memory, for the whole fragment before the first store (C2 may alias E)
     __device__ void epilogue(float (&acc)[1][BN / 2], int m0, int n0, int, int tid, const uint8_t* eb) const {
+        // the fragment's elements inside the output (at BN = 128 every column is)
+        auto inside = [&](int row, int col) { return row < o.M && (BN == 128 || col < o.N); };
+        constexpr bool E_FIRST = EPI == TE_TC_EPI_BIAS_ADD && EPI_MAPS == 0;
+        float2 ef[E_FIRST ? BN / 4 : 1];
 #pragma unroll
         for (int j = 0; j < BN / 2; j += 2) {
             const int row = m0 + frag_row(tid, j), col = n0 + frag_col(tid, j);
-            if (row >= o.M) continue;
+            if (!inside(row, col)) continue;
+            if constexpr (E_FIRST) ef[j / 2] = efrag(eb, tid, j, row, col);
             auto e = [&] { return efrag(eb, tid, j, row, col); };
             float2 y;
             if constexpr (F16)                                          // exact scaling
@@ -856,7 +872,11 @@ struct LinProb : LinArgs {
 #pragma unroll
         for (int j = 0; j < BN / 2; j += 2) {
             const int row = m0 + frag_row(tid, j), col = n0 + frag_col(tid, j);
-            if (row < o.M) lin_store<EPI>(o, row, col, make_float2(acc[0][j], acc[0][j + 1]), [&] { return efrag(eb, tid, j, row, col); });
+            if (inside(row, col))
+                lin_store<EPI>(o, row, col, make_float2(acc[0][j], acc[0][j + 1]), [&] {
+                    if constexpr (E_FIRST) return ef[j / 2];
+                    else return efrag(eb, tid, j, row, col);
+                });
         }
     }
     __device__ float2 efrag(const uint8_t* eb, int tid, int j, int row, int col) const {
@@ -1240,9 +1260,10 @@ unsigned stride_blocks(long long work, int per_block) {
 // FWD, else the backward ones (STORE, GELU_BWD).  C [rows, N] = epi(A B^T); bias / e0 / y2 as in te_gemm_tc.h.
 template <int EPI, int FORM>
 int lin_launch(const LinArgs& args, cudaStream_t st) {
-    LinProb<EPI, FORM> p;
+    using P = LinProb<EPI, FORM>;
+    P p;
     static_cast<LinArgs&>(p) = args;
-    return launch(p, dim3(mtiles(args.o.M), args.o.N / 128), st);
+    return launch(p, dim3(mtiles(args.o.M), (args.o.N + P::BN - 1) / P::BN), st);
 }
 template <int FORM, bool FWD>
 int linear(int K, const void* a, const void* a_lo, long long lda, const void* b, const void* b_lo, const float* rs,
