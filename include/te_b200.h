@@ -276,15 +276,18 @@ TE_API int te_patch_embed_relprop(const float* images, const float* weight, cons
                            long long workspace_bytes, void* stream);
 
 /* generate_visualization's tensor part (example.ipynb:57-60): maps [batch, grid*grid] -> reshape grid x grid -> bilinear
- * x scale (align_corners=False) -> per-sample min-max normalisation -> out [batch, grid*scale, grid*scale]. */
+ * x scale (align_corners=False) -> per-sample min-max normalisation -> out [batch, grid*scale, grid*scale].  As with the
+ * notebook's t.min() / t.max(), a NaN in a sample's map makes all of that sample NaN, and a constant map gives 0 / 0 = NaN. */
 TE_API int te_relevance_heatmap(const float* maps, int batch, int grid, int scale, float* out, void* stream);
 /* Head reductions of attention-shaped tensors [batch, heads, n, ld] -> out [batch, n, n] (contiguous), the building
  * block of the secondary methods (ViT_LRP.py:345-398; ViT_explanation_generator.py:51-83; BERT
  * ExplanationGenerator.py:61-155):   v_h = a_h (* g_h if g) (* head_w[b,h] if head_w);
- *   mode 0: mean_h v_h          mode 1: mean_h relu(v_h)  ("clamp(min=0).mean")      mode 2: relu(mean_h v_h). */
+ *   mode 0: mean_h v_h          mode 1: mean_h relu(v_h)  ("clamp(min=0).mean")      mode 2: relu(mean_h v_h).
+ * g has a's layout (row stride ld), head_w is [batch, heads]; the pad columns [n, ld) are never read. */
 TE_API int te_head_reduce(const float* a, const float* g, const float* head_w, int batch, int heads, int n, int ld, int mode,
                    float* out, void* stream);
-/* out[b,h] = mean of g[b,h, r0:r1, c0:c1]  (``grad.mean(dim=[1,2])`` of the GradCAM baselines). */
+/* out[b,h] = mean of g[b,h, r0:r1, c0:c1]  (``grad.mean(dim=[1,2])`` of the GradCAM baselines); the region must satisfy
+ * 0 <= r0 < r1 <= n and 0 <= c0 < c1 <= n, else TE_ERR_ARG before anything is launched. */
 TE_API int te_head_region_mean(const float* g, int batch, int heads, int n, int ld, int r0, int r1, int c0, int c1, float* out,
                         void* stream);
 

@@ -506,12 +506,15 @@ __global__ void aggregate_layers_vec_kernel(const float* __restrict__ G0, const 
 
 // generate_visualization (example.ipynb:57-60): [g,g] relevance -> bilinear x scale (align_corners=False, the arithmetic of
 // torch.nn.functional.interpolate(mode='bilinear', scale_factor=scale)) -> per-sample min-max.  One block per sample.
+// fminf / fmaxf skip NaN, so a NaN flag rides along the reduction: like torch's t.min() / t.max(), a NaN anywhere in the
+// up-sampled map makes the minimum, hence every normalised pixel, NaN.
 __global__ void relevance_heatmap_kernel(const float* __restrict__ maps, float* __restrict__ out, int g, int scale) {
     const int G = g * scale, total = G * G;
     const float* m = maps + (long long)blockIdx.x * g * g;
     float* o = out + (long long)blockIdx.x * total;
     const float rs = 1.0f / (float)scale;
     float mn = INFINITY, mx = -INFINITY;
+    int nan = 0;
     for (int p = threadIdx.x; p < total; p += blockDim.x) {
         const int y = p / G, x = p % G;
         const float sy = fmaxf(rs * ((float)y + 0.5f) - 0.5f, 0.f), sx = fmaxf(rs * ((float)x + 0.5f) - 0.5f, 0.f);
@@ -521,17 +524,20 @@ __global__ void relevance_heatmap_kernel(const float* __restrict__ maps, float* 
         const float v = ly0 * (lx0 * m[y0 * g + x0] + lx1 * m[y0 * g + x1]) + ly1 * (lx0 * m[y1 * g + x0] + lx1 * m[y1 * g + x1]);
         o[p] = v;
         mn = fminf(mn, v); mx = fmaxf(mx, v);
+        nan |= v != v;
     }
     __shared__ float smn[kThreads / 32], smx[kThreads / 32], bmn, bmx;
+    __shared__ int snan[kThreads / 32];
     for (int s = 16; s > 0; s >>= 1) {
         mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, s));
         mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, s));
+        nan |= __shfl_xor_sync(0xffffffffu, nan, s);
     }
-    if ((threadIdx.x & 31) == 0) { smn[threadIdx.x >> 5] = mn; smx[threadIdx.x >> 5] = mx; }
+    if ((threadIdx.x & 31) == 0) { smn[threadIdx.x >> 5] = mn; smx[threadIdx.x >> 5] = mx; snan[threadIdx.x >> 5] = nan; }
     __syncthreads();
     if (threadIdx.x == 0) {
-        for (int i = 1; i < kThreads / 32; ++i) { mn = fminf(mn, smn[i]); mx = fmaxf(mx, smx[i]); }
-        bmn = mn; bmx = mx;
+        for (int i = 1; i < kThreads / 32; ++i) { mn = fminf(mn, smn[i]); mx = fmaxf(mx, smx[i]); nan |= snan[i]; }
+        bmn = nan ? NAN : mn; bmx = mx;
     }
     __syncthreads();
     const float lo = bmn, range = bmx - bmn;

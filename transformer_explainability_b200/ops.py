@@ -398,13 +398,16 @@ def head_reduce(a, g=None, head_weight=None, mode="mean"):
     """Reduce an attention-shaped tensor over its heads: a [B,H,N,N] (optionally * g, * head_weight[B,H]) -> [B,N,N].
     mode: "mean" | "relu_mean" (``clamp(min=0).mean(heads)``) | "mean_relu" (``mean(heads).clamp(min=0)``)."""
     a, ld = _attn_layout(a)
+    B, H, N, _ = a.shape
     if g is not None:
+        _same_shape("head_reduce", a, g)
         g, ldg = _attn_layout(g)
         if ldg != ld:
-            a, g, ld = a.contiguous(), g.contiguous(), a.shape[-1]
-    B, H, N, _ = a.shape
+            a, g, ld = a.contiguous(), g.contiguous(), N
     if head_weight is not None:
         _req(head_weight)
+        if head_weight.shape != (B, H):
+            raise ValueError("head_reduce: head_weight %s, expected [B,H] = %s" % (tuple(head_weight.shape), (B, H)))
     out = torch.empty(B, N, N, device=a.device, dtype=torch.float32)
     m = {"mean": 0, "relu_mean": 1, "mean_relu": 2}[mode]
     check(_lib.load().te_head_reduce(ptr(a), ptr(g), ptr(head_weight), B, H, N, ld, m, ptr(out), _stream()),

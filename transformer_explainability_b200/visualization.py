@@ -10,9 +10,11 @@ import torch
 def relevance_to_heatmap(maps, grid=14, scale=16):
     """[B, grid*grid] -> min-max normalised [B, grid*scale, grid*scale] (device tensor) through the engine's kernel
     (``te_relevance_heatmap``, one block per sample).  CUDA tensors only: there is no host path."""
-    b = maps.shape[0]
     if not maps.is_cuda:
         raise ValueError("relevance_to_heatmap needs a CUDA tensor (no CPU fallback)")
+    if maps.dim() != 2 or maps.shape[1] != grid * grid:
+        raise ValueError("relevance_to_heatmap: maps %s, expected [B, grid*grid] = [B, %d]" % (tuple(maps.shape), grid * grid))
+    b = maps.shape[0]
     from . import _lib
     m = maps.detach().to(torch.float32).contiguous()
     out = torch.empty(b, grid * scale, grid * scale, device=m.device, dtype=torch.float32)
