@@ -279,6 +279,18 @@ TE_API int te_patch_embed_relprop(const float* images, const float* weight, cons
  * x scale (align_corners=False) -> per-sample min-max normalisation -> out [batch, grid*scale, grid*scale].  As with the
  * notebook's t.min() / t.max(), a NaN in a sample's map makes all of that sample NaN, and a constant map gives 0 / 0 = NaN. */
 TE_API int te_relevance_heatmap(const float* maps, int batch, int grid, int scale, float* out, void* stream);
+/* The notebooks' JET overlay (Transformer_explainability.ipynb: generate_visualization, show_cam_on_image), bit for bit the
+ * numpy / cv2 sequence per sample: images [batch, 3, h, w] fp32 (the normalised input), heat [batch, h, w] fp32 (min-max
+ * normalised, e.g. te_relevance_heatmap's output) -> out [batch, h, w, 3] uint8 BGR:
+ *   img = (x - min) / (max - min) over the sample;  u = (uint8)(255.f * heat) (truncation, NaN -> 0);
+ *   otsu: t = cv2's THRESH_OTSU value of u (fp64, getThreshVal_Otsu_8u), thresholds[b] = t when thresholds is not NULL,
+ *         u = u > t ? 255 : 0;
+ *   cam = JET_BGR[u] / 255.f + img (BGR colour channel k plus RGB image channel k, as the notebook adds them);
+ *   out[y, x, 2 - k] = (uint8)(255.f * (cam_k / max(cam))) (truncation, NaN -> 0: a constant image renders as 0).
+ * batch >= 1, h, w >= 1 (3 h w < 2^31), images / heat / out non-NULL and otsu 0 or 1, else TE_ERR_ARG before anything is
+ * launched.  One launch, no workspace. */
+TE_API int te_render_overlay(const float* images, const float* heat, int batch, int h, int w, int otsu, unsigned char* out,
+                             int* thresholds, void* stream);
 /* Head reductions of attention-shaped tensors [batch, heads, n, ld] -> out [batch, n, n] (contiguous), the building
  * block of the secondary methods (ViT_LRP.py:345-398; ViT_explanation_generator.py:51-83; BERT
  * ExplanationGenerator.py:61-155):   v_h = a_h (* g_h if g) (* head_w[b,h] if head_w);

@@ -94,6 +94,7 @@ PROTOTYPES = {
     "te_patch_embed_relprop_workspace_bytes": (c_ll, [c_int, c_int, c_int, c_int, c_int]),
     "te_patch_embed_relprop": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, c_int, _P, _P, _P, c_ll, _P]),
     "te_relevance_heatmap": (c_int, [_P, c_int, c_int, c_int, _P, _P]),
+    "te_render_overlay": (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P, _P, _P]),
     "te_head_reduce": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, c_int, _P, _P]),
     "te_head_region_mean": (c_int, [_P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P]),
     "te_rollout_workspace_bytes": (c_ll, [c_int, c_int, c_int]),
