@@ -75,6 +75,15 @@ extern "C" {
                                           * (TE_FLAG_ZPLUS_BF16, _S1_BF16, _R_F16) do not apply to this rule. */
 #define TE_FLAG_RELPROP_TO_INPUT 8u   /* finish the lowest block as well: relevance at the encoder input (what
                                          model.relprop() returns in the reference) is left in tensor "relevance_in" */
+#define TE_FLAG_ATTN_GRAD_ROLLOUT 65536u /* te_*_attribute explains with the LRP-free gradient-weighted attention rollout of
+                                          * Chefer, Gur, Wolf (ICCV 2021) instead of transformer_attribution: the class-gradient
+                                          * backward down to start_layer, then the rollout of mean_h relu(G * P) + I with the
+                                          * attention probabilities P in place of attn_cam, no row normalisation; ViT maps
+                                          * R[0, prefix:], BERT maps R[0, :] with element 0 set to 0.  No relprop runs: attn_cam,
+                                          * the relprop scratch and "relevance_in" are not written, and the rule-library and
+                                          * relprop-only precision flags (RULES_LRP*, ZPLUS_*, RELPROP_TF32) change nothing.
+                                          * Combined with TE_FLAG_GRADIENTS_ONLY, _KEEP_ALL_CAMS or _RELPROP_TO_INPUT, or with
+                                          * alpha != 1, te_*_attribute returns TE_ERR_ARG. */
 
 TE_API const char* te_last_error(void);
 /* Process-wide tuning switches (not part of the reference surface).

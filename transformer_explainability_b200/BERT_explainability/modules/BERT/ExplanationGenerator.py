@@ -79,6 +79,15 @@ class Generator:
         cam[:, 0, 0] = 0
         return cam[:, 0]
 
+    def generate_attn_grad_rollout(self, input_ids, attention_mask, index=None, start_layer=0):
+        """The LRP-free gradient-weighted attention rollout of Chefer, Gur, Wolf (ICCV 2021): for l = start_layer .. L-1,
+        R <- R + mean_h relu(dy_c/dA_l * A_l) R from R = I, row 0 with [0] = 0 as the comparison generators above.
+        [B,S] -> [B,S]; padded positions come out exactly 0."""
+        eng = self.model.engine()
+        maps, _ = eng.explain(input_ids, attention_mask, index=index, start_layer=start_layer,
+                              flags=eng.flags | _lib.FLAG_ATTN_GRAD_ROLLOUT)
+        return maps
+
     def generate_LRP_batched(self, input_ids, attention_mask=None, index=None, start_layer=11, chunk=None,
                              return_index=False):
         """B independent sequences of equal length in one engine call: [B,S] -> [B,S]."""

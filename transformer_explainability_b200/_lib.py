@@ -43,6 +43,7 @@ FLAG_LINEAR_F16_SPLIT = 4096
 FLAG_ZPLUS_R_F16 = 8192
 FLAG_BACKWARD_F16 = 16384
 FLAG_RULES_LRP_TC = 32768       # with FLAG_RULES_LRP: its Linear rule on TF32 tensor cores (needs the derived weights too)
+FLAG_ATTN_GRAD_ROLLOUT = 65536  # attribute() explains with the LRP-free gradient-weighted attention rollout (ICCV 2021)
 FLAG_TENSOR_CORES = FLAG_ZPLUS_TENSOR_CORES | FLAG_LINEAR_TENSOR_CORES      # the ones that need derived weights
 FLAG_ALL_FAST = FLAG_TENSOR_CORES | FLAG_ATTN_TENSOR_CORES | FLAG_ROLLOUT_FUSED
 # what bench.py runs by default: updated as faster selections pass the parity tests (tests/test_gpu_parity_full.py)

@@ -36,6 +36,15 @@ class LRP:
         maps, idx = self.model.engine().explain(input, index=index, start_layer=start_layer, chunk=chunk)
         return (maps, idx) if return_index else maps
 
+    def generate_attn_grad_rollout(self, input, index=None, start_layer=0):
+        """The LRP-free gradient-weighted attention rollout of Chefer, Gur, Wolf (ICCV 2021): for l = start_layer .. L-1,
+        R <- R + mean_h relu(dy_c/dA_l * A_l) R from R = I, row 0 without the prefix token(s).  [B,3,H,W] -> [B,N-prefix];
+        ``index`` as for ``generate_LRP`` (arg-max when None).  The model's rule-library and relprop precision flags are
+        accepted and change nothing: no relprop runs."""
+        eng = self.model.engine()
+        maps, _ = eng.explain(input, index=index, start_layer=start_layer, flags=eng.flags | _lib.FLAG_ATTN_GRAD_ROLLOUT)
+        return maps
+
 
 class Baselines:
     """``ViT_explanation_generator.py:45-83`` for a ``baselines.ViT.ViT_new`` (or ``ViT_LRP``) model."""

@@ -295,11 +295,13 @@ extern "C" int te_bert_attribute(const te_bert_config* cfg, const float* weights
     Dims d; Workspace ws;
     TE_TRY(check_ws(cfg, batch, seq, workspace, workspace_bytes, d, ws));
     if (!isfinite(alpha)) { te_set_last_error("te_bert_attribute: alpha must be finite"); return TE_ERR_ARG; }
+    TE_TRY(te_util::check_grad_rollout("te_bert_attribute", flags, alpha));
+    const bool grad_rollout = (flags & TE_FLAG_ATTN_GRAD_ROLLOUT) != 0;
     if (!weights || !index || (!maps && !(flags & TE_FLAG_GRADIENTS_ONLY))) { te_set_last_error("te_bert_attribute: null pointer"); return TE_ERR_ARG; }
     if (start_layer < 0 || start_layer >= d.L) { te_set_last_error("te_bert_attribute: start_layer out of range"); return TE_ERR_ARG; }
     // fp16 backward split of dy in tF[1], block scales in t3D[1] (idle until the relprop)
     Select sel;
-    TE_TRY(decode_flags(sel, "te_bert_attribute", flags, derived, start_layer, true, {ws.tF[1], ws.nF[1]},
+    TE_TRY(decode_flags(sel, "te_bert_attribute", flags, derived, start_layer, !grad_rollout, {ws.tF[1], ws.nF[1]},
                         {ws.t3D[1], d.M * 3LL * d.D}, d.M, std::max(3 * d.D, d.F)));
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     Weights w;
@@ -340,6 +342,21 @@ extern "C" int te_bert_attribute(const te_bert_config* cfg, const float* weights
     }
 
     if (flags & TE_FLAG_GRADIENTS_ONLY) return TE_OK;      // attention-GradCAM baseline: gradients are all it reads
+    // P and G of a layer are carved side by side in every layer's slice, so one layer stride serves both operands
+    const long long layer_stride = d.L > 1 ? (long long)(ws.layer[1].G - ws.layer[0].G) : 0;
+    if (grad_rollout) {
+        // gradient-weighted attention rollout: mean_h relu(G * P) + I chained from start_layer, no relprop, no row
+        // normalisation; row 0 with element 0 set to 0 (the reference's BERT comparison generators).  Padded keys have
+        // P = 0 and padded queries G = 0, so padded entries come out exactly 0.
+        TE_TRY(te_rollout_layers(ws.layer[0].G, ws.layer[0].P, layer_stride, d.L, d.B, d.H, d.N, d.NP, d.NP, start_layer,
+                                 /*normalize=*/0, flags, ws.mats, ws.joint[0], ws.joint[1], nullptr, maps, /*first=*/0,
+                                 /*bert_fix=*/0, st));
+        if (cudaMemset2DAsync(maps, sizeof(float) * d.N, 0, sizeof(float), d.B, st) != cudaSuccess) {
+            te_set_last_error("te_bert_attribute: clearing element 0 of the maps failed");
+            return TE_ERR_CUDA;
+        }
+        return TE_OK;
+    }
 
     // ---- relprop -----------------------------------------------------------------------------------------------
     float* R = ws.tD[0]; float* R1 = ws.tD[1]; float* R2 = ws.tD[2]; float* R3 = ws.tD[3];
@@ -400,9 +417,9 @@ extern "C" int te_bert_attribute(const te_bert_config* cfg, const float* weights
     }
 
     // ---- aggregation + normalised rollout, row 0 with [0] = min   (ExplanationGenerator.py:47-59) ---------------
-    TE_TRY(te_rollout_layers(ws.layer[0].G, ws.layer[0].cam, d.L > 1 ? (long long)(ws.layer[1].G - ws.layer[0].G) : 0,
-                             d.L, d.B, d.H, d.N, d.NP, d.NP, start_layer, /*normalize=*/1, flags, ws.mats, ws.joint[0],
-                             ws.joint[1], nullptr, maps, /*first=*/0, /*bert_fix=*/1, st));
+    TE_TRY(te_rollout_layers(ws.layer[0].G, ws.layer[0].cam, layer_stride, d.L, d.B, d.H, d.N, d.NP, d.NP, start_layer,
+                             /*normalize=*/1, flags, ws.mats, ws.joint[0], ws.joint[1], nullptr, maps, /*first=*/0,
+                             /*bert_fix=*/1, st));
     return TE_OK;
 }
 

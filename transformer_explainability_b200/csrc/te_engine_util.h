@@ -195,6 +195,24 @@ static inline int decode_flags(Select& s, const char* fn, unsigned flags, const 
     return TE_OK;
 }
 
+// TE_FLAG_ATTN_GRAD_ROLLOUT runs no relprop: the modes that stop before it or carry it further, and the alpha-beta rule,
+// have nothing to act on, so asking for them together is an error rather than a silently ignored bit
+static inline int check_grad_rollout(const char* fn, unsigned flags, float alpha) {
+    if (!(flags & TE_FLAG_ATTN_GRAD_ROLLOUT)) return TE_OK;
+    const char* clash = (flags & TE_FLAG_GRADIENTS_ONLY) ? "TE_FLAG_GRADIENTS_ONLY"
+                      : (flags & TE_FLAG_KEEP_ALL_CAMS) ? "TE_FLAG_KEEP_ALL_CAMS"
+                      : (flags & TE_FLAG_RELPROP_TO_INPUT) ? "TE_FLAG_RELPROP_TO_INPUT" : nullptr;
+    if (clash) {
+        te_set_last_error((std::string(fn) + ": TE_FLAG_ATTN_GRAD_ROLLOUT does not combine with " + clash).c_str());
+        return TE_ERR_ARG;
+    }
+    if (alpha != 1.f) {
+        te_set_last_error((std::string(fn) + ": TE_FLAG_ATTN_GRAD_ROLLOUT runs no relprop, alpha must be 1").c_str());
+        return TE_ERR_ARG;
+    }
+    return TE_OK;
+}
+
 // fp16-split forward Linears (te_tc_wgmma.cu) of a block with D-wide inputs and an F-wide GELU layer: the block-scaled split
 // of the D-wide inputs lives in a (+ scales a_scale), that of the GELU output in b (+ b_scale), buffers the engine lends while
 // they are idle.  LayerNorm emits the split of what it produces (qkv and fc1 inputs); the attention context goes through the

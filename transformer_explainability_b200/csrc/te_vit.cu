@@ -312,6 +312,8 @@ extern "C" int te_vit_attribute(const te_vit_config* cfg, const float* weights, 
     Dims d; Workspace ws;
     TE_TRY(check_ws(cfg, batch, workspace, workspace_bytes, d, ws));
     if (!isfinite(alpha)) { te_set_last_error("te_vit_attribute: alpha must be finite"); return TE_ERR_ARG; }
+    TE_TRY(te_util::check_grad_rollout("te_vit_attribute", flags, alpha));
+    const bool grad_rollout = (flags & TE_FLAG_ATTN_GRAD_ROLLOUT) != 0;
     if (!weights || !index || (!maps && !(flags & TE_FLAG_GRADIENTS_ONLY))) { te_set_last_error("te_vit_attribute: null pointer"); return TE_ERR_ARG; }
     if (start_layer < 0 || start_layer >= d.L) { te_set_last_error("te_vit_attribute: start_layer out of range"); return TE_ERR_ARG; }
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
@@ -321,7 +323,7 @@ extern "C" int te_vit_attribute(const te_vit_config* cfg, const float* weights, 
     const long long MD = d.M * d.D, M3D = d.M * 3LL * d.D;
     // fp16 backward split of dy in tF[1], block scales in t3D[1] (idle until the relprop)
     te_util::Select sel;
-    TE_TRY(te_util::decode_flags(sel, "te_vit_attribute", flags, derived, start_layer, true, {ws.tF[1], ws.nF[1]},
+    TE_TRY(te_util::decode_flags(sel, "te_vit_attribute", flags, derived, start_layer, !grad_rollout, {ws.tF[1], ws.nF[1]},
                                  {ws.t3D[1], M3D}, d.M, std::max(3 * d.D, d.F)));
 
     // ---- class index and seeds  (ViT_explanation_generator.py:28-35) ---------------------------
@@ -362,6 +364,12 @@ extern "C" int te_vit_attribute(const te_vit_config* cfg, const float* weights, 
     }
 
     if (flags & TE_FLAG_GRADIENTS_ONLY) return TE_OK;      // attention-GradCAM baseline: gradients are all it reads
+    // P and G of a layer are carved side by side in every layer's slice, so one layer stride serves both operands
+    const long long layer_stride = d.L > 1 ? (long long)(ws.layer[1].G - ws.layer[0].G) : 0;
+    if (grad_rollout)       // gradient-weighted attention rollout: mean_h relu(G * P) + I chained from start_layer, no relprop
+        return te_rollout_layers(ws.layer[0].G, ws.layer[0].P, layer_stride, d.L, d.B, d.H, d.N, d.NP, d.NP, start_layer,
+                                 /*normalize=*/0, flags, ws.mats, ws.joint[0], ws.joint[1], nullptr, maps, d.prefix,
+                                 /*bert_fix=*/0, st);
 
     // ---- relprop  (VisionTransformer.relprop :324-331) --------------------------------------------
     float* R = ws.tD[0]; float* R1 = ws.tD[1]; float* R2 = ws.tD[2]; float* R3 = ws.tD[3];
@@ -413,8 +421,7 @@ extern "C" int te_vit_attribute(const te_vit_config* cfg, const float* weights, 
     }
 
     // ---- aggregation + rollout  (:357-368) ---------------------------------------------------------
-    TE_TRY(te_rollout_layers(ws.layer[0].G, ws.layer[0].cam,
-                             d.L > 1 ? (long long)(ws.layer[1].G - ws.layer[0].G) : 0, d.L, d.B, d.H, d.N, d.NP, d.NP,
+    TE_TRY(te_rollout_layers(ws.layer[0].G, ws.layer[0].cam, layer_stride, d.L, d.B, d.H, d.N, d.NP, d.NP,
                              start_layer, /*normalize=*/0, flags, ws.mats, ws.joint[0], ws.joint[1], nullptr, maps,
                              d.prefix, /*bert_fix=*/0, st));
     return TE_OK;

@@ -69,6 +69,12 @@ METHOD_GENERATOR = {"transformer_attribution": ("ours", "generate_LRP"),
                     "attn_gradcam": ("cls_lrp", "generate_attn_gradcam"),
                     "lrp": ("cls_lrp", "generate_full_lrp"),
                     "rollout": ("cls_lrp", "generate_rollout")}
+# one more choice besides the pipeline's METHODS: the LRP-free gradient-weighted attention rollout of the authors'
+# follow-up paper (Chefer, Gur, Wolf, ICCV 2021) on the BertForSequenceClassification model.  Padded keys and queries
+# contribute exactly nothing to it, so it takes length-sorted padded batches like transformer_attribution.
+FOLLOW_UP_FOLDER = {"attn_grad_rollout": "attn_grad_rollout"}
+FOLLOW_UP_GENERATOR = {"attn_grad_rollout": ("ours", "generate_attn_grad_rollout")}
+CHOICES = METHODS + tuple(FOLLOW_UP_GENERATOR)
 
 
 def topk_rationales(scores, ks=KS):
@@ -807,7 +813,7 @@ def build_parser():
     p.add_argument("--output_dir", dest="output_dir", required=True)
     p.add_argument("--model_params", dest="model_params", required=True,
                    help="the pipeline's JSON parameters (bert_vocab, bert_dir, max_length, evidence_classifier.classes)")
-    p.add_argument("--method", default="transformer_attribution", choices=METHODS)
+    p.add_argument("--method", default="transformer_attribution", choices=CHOICES)
     p.add_argument("--split", default="test")
     p.add_argument("--state-dict", dest="state_dict", default=None,
                    help="classifier weights (default: output_dir/classifier/classifier.pt, where the pipeline saves them)")
@@ -852,7 +858,7 @@ def build_generator(method, bert_dir, num_labels, state_dict=None, device="cuda"
     """The bound ``Generator`` method of ``method`` on the one façade model it needs (``:422-448``)."""
     import transformers
     from .BERT_explainability.modules.BERT.ExplanationGenerator import Generator
-    kind, fn = METHOD_GENERATOR[method]
+    kind, fn = {**METHOD_GENERATOR, **FOLLOW_UP_GENERATOR}[method]
     if kind == "ours":
         from .BERT_explainability.modules.BERT.BertForSequenceClassification import BertForSequenceClassification
     else:
@@ -885,7 +891,7 @@ def main(argv=None):
                       iou_thresholds=args.iou_thresholds, faithfulness=args.faithfulness,
                       aopc_thresholds=args.aopc_thresholds, k_fraction=args.k_fraction, soft_scores=args.soft_scores,
                       tokens_to_flip=args.tokens_to_flip)
-    write_results(res, os.path.join(args.output_dir, METHOD_FOLDER[args.method]))
+    write_results(res, os.path.join(args.output_dir, {**METHOD_FOLDER, **FOLLOW_UP_FOLDER}[args.method]))
     for k in KS:
         print("top-%d token F1 %.4f (instance macro %.4f)" % (k, res["scores"][k]["token_prf"]["instance_micro"]["f1"],
                                                               res["scores"][k]["token_prf"]["instance_macro"]["f1"]))

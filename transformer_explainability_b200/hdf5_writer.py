@@ -315,6 +315,8 @@ def compute_saliency_and_save(loader, method_dir, method, lrp=None, baselines=No
                 res = lrp.generate_LRP_batched(x, start_layer=1, index=index)
             elif method == "transformer_attribution":
                 res = lrp.generate_LRP_batched(x, start_layer=1, index=index)       # method="grad" is the legacy alias
+            elif method == "attn_grad_rollout":
+                res = lrp.generate_attn_grad_rollout(x, index=index)
             elif method == "full_lrp":
                 res = (orig_lrp or lrp).generate_LRP(x, method="full", index=index)
             elif method == "lrp_last_layer":
@@ -341,6 +343,10 @@ METHODS = ("rollout", "lrp", "transformer_attribution", "full_lrp", "lrp_last_la
 # the façade model whose generator each method uses in generate_visualizations.py:180-192; only that one is built
 MODEL_KIND = {"rollout": "new", "attn_gradcam": "new", "lrp": "lrp", "transformer_attribution": "lrp",
               "attn_last_layer": "lrp", "full_lrp": "orig", "lrp_last_layer": "orig"}
+# one more choice besides the script's METHODS: the LRP-free gradient-weighted attention rollout of the authors' follow-up
+# paper (Chefer, Gur, Wolf, ICCV 2021) on the ViT_LRP model, written to visualizations/attn_grad_rollout/...
+FOLLOW_UP_KIND = {"attn_grad_rollout": "lrp"}
+CHOICES = METHODS + tuple(FOLLOW_UP_KIND)
 
 
 def read_rgb(path):
@@ -388,7 +394,7 @@ def build_parser():
     from .perturbation import str2bool
     p = argparse.ArgumentParser(description="Explain an ImageNet validation folder into results.hdf5")
     p.add_argument("--batch-size", type=int, default=1)
-    p.add_argument("--method", type=str, required=True, choices=METHODS)
+    p.add_argument("--method", type=str, required=True, choices=CHOICES)
     p.add_argument("--lmd", type=float, default=10, help="accepted for compatibility; unused, as in the reference")
     p.add_argument("--vis-class", type=str, default="top", choices=["top", "target", "index"])
     p.add_argument("--class-id", type=int, default=0, help="names the output directory of --vis-class index")
@@ -422,7 +428,8 @@ def main(argv=None):
     os.makedirs(method_dir, exist_ok=True)
     if os.path.exists(os.path.join(method_dir, "results.hdf5")):
         os.remove(os.path.join(method_dir, "results.hdf5"))
-    lrp, orig_lrp, baselines = segmentation.build_generators(args.method, args.state_dict, kind=MODEL_KIND[args.method])
+    kind = {**MODEL_KIND, **FOLLOW_UP_KIND}[args.method]
+    lrp, orig_lrp, baselines = segmentation.build_generators(args.method, args.state_dict, kind=kind)
     loader = imagenet_val_loader(args.imagenet_validation_path, args.batch_size, args.num_workers)
     path = compute_saliency_and_save(prepared_batches(loader), method_dir, args.method, lrp=lrp, baselines=baselines,
                                      orig_lrp=orig_lrp, vis_class=args.vis_class, is_ablation=args.is_ablation)

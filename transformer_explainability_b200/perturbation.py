@@ -222,7 +222,8 @@ def str2bool(v):
 
 
 METHODS = ['rollout', 'lrp', 'transformer_attribution', 'full_lrp', 'v_gradcam', 'lrp_last_layer', 'lrp_second_layer',
-           'gradcam', 'attn_last_layer', 'attn_gradcam', 'input_grads']
+           'gradcam', 'attn_last_layer', 'attn_gradcam', 'input_grads',
+           'attn_grad_rollout']      # the LRP-free gradient-weighted attention rollout (Chefer, Gur, Wolf, ICCV 2021)
 
 
 def build_parser():

@@ -32,8 +32,12 @@ from . import ops
 from .perturbation import str2bool
 
 METHODS = ("rollout", "transformer_attribution", "full_lrp", "lrp_last_layer", "attn_last_layer", "attn_gradcam")
+# the methods of the reference script are METHODS; one more choice is the LRP-free gradient-weighted attention rollout of
+# the authors' follow-up paper (Chefer, Gur, Wolf, ICCV 2021), so that both papers' methods compare on one engine
+FOLLOW_UP_METHODS = ("attn_grad_rollout",)
+CHOICES = METHODS + FOLLOW_UP_METHODS
 _MODEL = {"rollout": "new", "attn_gradcam": "new", "transformer_attribution": "lrp", "full_lrp": "orig",
-          "lrp_last_layer": "orig", "attn_last_layer": "orig"}
+          "lrp_last_layer": "orig", "attn_last_layer": "orig", "attn_grad_rollout": "lrp"}
 
 
 # ---- data ----------------------------------------------------------------------------------------------------------------
@@ -92,8 +96,8 @@ class ImagenetSegmentation(torch.utils.data.Dataset):
 
 # ---- the evaluation ------------------------------------------------------------------------------------------------------
 def check_method(method):
-    if method not in METHODS:
-        raise ValueError("unknown segmentation method %r (expected one of %s)" % (method, ", ".join(METHODS)))
+    if method not in CHOICES:
+        raise ValueError("unknown segmentation method %r (expected one of %s)" % (method, ", ".join(CHOICES)))
 
 
 def explain(method, x, lrp=None, orig_lrp=None, baselines=None, is_ablation=False):
@@ -107,6 +111,8 @@ def explain(method, x, lrp=None, orig_lrp=None, baselines=None, is_ablation=Fals
         res = gen.generate_rollout(x, start_layer=1)
     elif method == "transformer_attribution":
         res = gen.generate_LRP_batched(x, start_layer=1)
+    elif method == "attn_grad_rollout":
+        res = gen.generate_attn_grad_rollout(x)
     elif method == "full_lrp":
         res = gen.generate_LRP(x, method="full")
     elif method == "lrp_last_layer":
@@ -237,7 +243,7 @@ def build_parser():
     p = argparse.ArgumentParser(description="ImageNet-segmentation evaluation of the ViT explanation methods")
     p.add_argument("--arc", type=str, default="vgg", metavar="N", help="model architecture (names the run directory)")
     p.add_argument("--train_dataset", type=str, default="imagenet", metavar="N", help="names the run directory")
-    p.add_argument("--method", type=str, required=True, choices=METHODS)
+    p.add_argument("--method", type=str, required=True, choices=CHOICES)
     p.add_argument("--thr", type=float, default=0., help="threshold of the PR-curve scores")
     p.add_argument("--K", type=int, default=1, help="accepted for compatibility; unused, as in the reference")
     p.add_argument("--save-img", action="store_true", default=False, help="not supported")

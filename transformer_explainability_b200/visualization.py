@@ -86,22 +86,43 @@ def show_cam_on_image(img, mask):
     return cam / np.max(cam)
 
 
-def generate_visualization(attribution_generator, original_image, class_index=None, start_layer=0, use_thresholding=False):
+# transformer_attribution (the notebooks' method) or the LRP-free gradient-weighted attention rollout of the authors'
+# follow-up paper (Chefer, Gur, Wolf, ICCV 2021)
+METHODS = ("transformer_attribution", "attn_grad_rollout")
+
+
+def _check_method(method):
+    if method not in METHODS:
+        raise ValueError("unknown visualization method %r (expected one of %s)" % (method, ", ".join(METHODS)))
+
+
+def generate_visualization(attribution_generator, original_image, class_index=None, start_layer=0, use_thresholding=False,
+                           method="transformer_attribution"):
     """``example.ipynb:55-66`` / ``Transformer_explainability.ipynb``: original_image [3,224,224] -> uint8 overlay
-    [224,224,3] (numpy), with the notebook's ``use_thresholding`` switch."""
+    [224,224,3] (numpy), with the notebook's ``use_thresholding`` switch; ``method`` one of ``METHODS``."""
+    _check_method(method)
     dev = next(attribution_generator.model.parameters()).device
     x = original_image.unsqueeze(0).to(dev)
-    maps = attribution_generator.generate_LRP(x, method="transformer_attribution", index=class_index,
-                                              start_layer=start_layer).detach()
+    if method == "attn_grad_rollout":
+        maps = attribution_generator.generate_attn_grad_rollout(x, index=class_index, start_layer=start_layer)
+    else:
+        maps = attribution_generator.generate_LRP(x, method="transformer_attribution", index=class_index,
+                                                  start_layer=start_layer).detach()
     return render_overlays(x, relevance_to_heatmap(maps), use_thresholding)[0].cpu().numpy()
 
 
-def generate_visualizations(attribution_generator, images, class_index=None, start_layer=0, use_thresholding=False):
+def generate_visualizations(attribution_generator, images, class_index=None, start_layer=0, use_thresholding=False,
+                            method="transformer_attribution"):
     """``generate_visualization`` for a batch: images [B,3,224,224] -> uint8 CUDA [B,224,224,3].  One engine call
-    (``generate_LRP_batched``) for the maps, one ``te_relevance_heatmap`` and one ``te_render_overlay``."""
+    (``generate_LRP_batched`` or ``generate_attn_grad_rollout``) for the maps, one ``te_relevance_heatmap`` and one
+    ``te_render_overlay``."""
+    _check_method(method)
     dev = next(attribution_generator.model.parameters()).device
     x = images.to(dev, torch.float32)
-    maps = attribution_generator.generate_LRP_batched(x, index=class_index, start_layer=start_layer)
+    if method == "attn_grad_rollout":
+        maps = attribution_generator.generate_attn_grad_rollout(x, index=class_index, start_layer=start_layer)
+    else:
+        maps = attribution_generator.generate_LRP_batched(x, index=class_index, start_layer=start_layer)
     return render_overlays(x, relevance_to_heatmap(maps), use_thresholding)
 
 
@@ -169,19 +190,23 @@ def build_model(name, state_dict=None, device="cuda"):
     return model.to(device).eval()
 
 
-def render_batch(model, packed, sizes, offsets, transform, class_indices=(), use_thresholding=False):
+def render_batch(model, packed, sizes, offsets, transform, class_indices=(), use_thresholding=False,
+                 method="transformer_attribution"):
     """One batch of the command on the device: (overlays uint8 [B, K, 224, 224, 3], classes int64 [B, K], top-5 indices
     [B, k], logits [B, k], probabilities [B, k]) on the host after one device-to-host copy; K = 1 + len(class_indices),
-    column 0 the predicted class."""
+    column 0 the predicted class.  ``method``: one of ``METHODS``."""
+    from . import _lib
+    _check_method(method)
     x, _ = prepare_batch(packed, sizes, offsets, transform)
     eng = model.engine()
+    flags = eng.flags | (_lib.FLAG_ATTN_GRAD_ROLLOUT if method == "attn_grad_rollout" else 0)
     logits = eng.forward(x)
     b = x.shape[0]
     pred = logits.argmax(dim=-1)
     cols = [pred] + [torch.full((b,), int(c), device=pred.device, dtype=pred.dtype) for c in class_indices]
     overlays = []
     for idx in cols:
-        maps, _ = eng.attribute(index=idx.to(torch.int32))
+        maps, _ = eng.attribute(index=idx.to(torch.int32), flags=flags)
         overlays.append(render_overlays(x, relevance_to_heatmap(maps), use_thresholding))
     k = min(5, logits.shape[1])
     top = logits.topk(k, dim=1)[1]
@@ -197,7 +222,7 @@ def render_batch(model, packed, sizes, offsets, transform, class_indices=(), use
 
 
 def run(model, paths, output_dir, class_indices=(), use_thresholding=False, transform="center-crop", batch_size=16,
-        timings=None):
+        timings=None, method="transformer_attribution"):
     """The command on already-parsed arguments; returns the written PNG paths.  ``timings`` (a dict) accumulates the
     seconds spent decoding, on the device (ending in the copy to the host) and encoding PNGs."""
     from PIL import Image
@@ -214,7 +239,7 @@ def run(model, paths, output_dir, class_indices=(), use_thresholding=False, tran
         packed, sizes, offsets, _ = hdf5_writer.pack_images([(hdf5_writer.read_rgb(p), 0) for p in chunk])
         t1 = time.perf_counter()
         img, cls, idx, logit, prob = render_batch(model, packed.to(dev), sizes.numpy(), offsets.numpy(), transform,
-                                                  class_indices, use_thresholding)
+                                                  class_indices, use_thresholding, method)
         t2 = time.perf_counter()
         for i, p in enumerate(chunk):
             stem = os.path.splitext(os.path.basename(p))[0]
@@ -246,6 +271,9 @@ def build_parser():
     p.add_argument("--transform", choices=("center-crop", "resize"), default=None,
                    help="Resize(256) + CenterCrop(224) (default for the ViT models) or Resize((224, 224)) (default for DeiT)")
     p.add_argument("--batch-size", type=int, default=16)
+    p.add_argument("--method", choices=METHODS, default="transformer_attribution",
+                   help="the explanation method rendered: transformer_attribution (the notebooks') or the LRP-free "
+                        "gradient-weighted attention rollout")
     return p
 
 
@@ -265,7 +293,7 @@ def main(argv=None):
     if any(not 0 <= c < model.num_classes for c in args.class_index):
         raise SystemExit("--class-index must lie in 0..%d" % (model.num_classes - 1))
     written = run(model, image_paths(args.images), args.output_dir, args.class_index, args.use_thresholding,
-                  args.transform, args.batch_size)
+                  args.transform, args.batch_size, method=args.method)
     print("%d overlays in %s" % (len(written), args.output_dir))
     return written
 
