@@ -508,6 +508,18 @@ TE_API int te_eraser_soft_scores(const float* word_scores, int batch, const int*
                                  const int* spans, const int* tail_counts, double* scores, int* flags, void* workspace,
                                  long long workspace_bytes, void* stream);
 
+/* ERASER LaTeX heat maps (bert_pipeline.py:49-93: the colour weights generate() prints, :551-561: its inputs) */
+/* Per row b of maps [batch, seq] (device, padded rows), over its first L = lengths[b] entries a (lengths: device int32,
+ * 1 <= L <= seq; the caller checks them, the kernel clips them to [0, seq]):
+ *   a = clamp(a, min=0) when clamp (NaN stays NaN);  mn, mx = min(a), max(a), NaN if any entry is NaN (torch.min / max);
+ *   w = 0 everywhere when mx == mn, else w = (100 * (a - mn)) / (mx - mn), each operation one IEEE fp32 rounding
+ *   (__fsub_rn, __fmul_rn, __fdiv_rn, no contraction); then w < 1 -> 0 (NaN stays NaN);
+ *   out[b, :L] = w, out[b, L:seq] = 0.  maps[b, L:] is never read.
+ * batch in 1..65535, seq >= 1, maps / lengths / out non-NULL, clamp 0 or 1, else TE_ERR_ARG before anything is launched.
+ * One launch (a block per row), no workspace. */
+TE_API int te_eraser_latex_weights(const float* maps, int batch, int seq, const int* lengths, int clamp, float* out,
+                                   void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Input preparation  (baselines/ViT/generate_visualizations.py:194-199: Resize((224, 224)) + ToTensor() on PIL images)
  * Pillow's 8-bit bilinear resize (ImagingResample, support 1): per axis scale = in / out, fs = max(scale, 1), and for output

@@ -126,6 +126,7 @@ PROTOTYPES = {
     "te_class_probs": (c_int, [_P, c_int, c_int, _P, _P]),
     "te_eraser_soft_workspace_bytes": (c_ll, [c_int, c_ll]),
     "te_eraser_soft_scores": (c_int, [_P, c_int, _P, _P, _P, _P, _P, _P, _P, c_ll, _P]),
+    "te_eraser_latex_weights": (c_int, [_P, c_int, c_int, _P, c_int, _P, _P]),
     "te_resize_coeffs": (c_int, [c_int, c_int, _P, _P]),
     "te_prepare_images_workspace_bytes": (c_ll, [c_int, c_int, c_int, c_int, c_int]),
     "te_prepare_images": (c_int, [_P, c_ll, c_int, _P, _P, c_int, c_int, _P, _P, _P, _P, _P, c_ll, _P]),

@@ -8,6 +8,8 @@
 //     pieces (comprehensiveness) are compacted, between the document's [CLS] and [SEP], by one block scan.
 //   * soft_kernel: one block per document, the ranking of eraser_kernel over given word scores; the tie groups' cumulative
 //     (tps, fps) come from one warp scan, and metrics.py's soft-token areas (:217-253) are reduced in fp64.
+//   * latex_kernel: one block per row, the colour weights of bert_pipeline.py's generate() (:49-56): the row's NaN-aware
+//     min / max by a block reduction, then the reference's fp32 operations in its order with explicit IEEE roundings.
 // The ragged host arrays (word piece ranges, truth spans, their offsets) are validated on the host and copied into the
 // workspace, so no index the caller passes is read from the map before it has been checked.
 #include "../../include/te_b200.h"
@@ -321,6 +323,58 @@ __global__ void __launch_bounds__(kThreads) soft_kernel(
     }
 }
 
+constexpr int kLatexThreads = 256;
+
+// generate()'s weights of row b: a = the first L entries (clamped at 0 when clamp; NaN stays); mn / mx = min / max of a,
+// NaN when any entry is NaN, as torch.min / torch.max; w = 0 for a constant row (mx == mn, false for NaN), else
+// (100 * (a - mn)) / (mx - mn) with one fp32 rounding per operation; w < 1 -> 0; zeros past L.
+__global__ void __launch_bounds__(kLatexThreads) latex_kernel(const float* __restrict__ maps, int seq,
+                                                              const int* __restrict__ lengths, int clamp,
+                                                              float* __restrict__ out) {
+    __shared__ float smn[kLatexThreads / 32], smx[kLatexThreads / 32];
+    __shared__ int snan[kLatexThreads / 32];
+    const int b = blockIdx.x;
+    const int L = min(max(lengths[b], 0), seq);
+    const float* row = maps + (long long)b * seq;
+    float* o = out + (long long)b * seq;
+    const float inf = __int_as_float(0x7f800000);
+    float mn = inf, mx = -inf;
+    int nan = 0;
+    for (int p = threadIdx.x; p < L; p += kLatexThreads) {
+        float v = row[p];
+        if (clamp && v < 0.f) v = 0.f;
+        if (v != v) nan = 1;
+        else { mn = fminf(mn, v); mx = fmaxf(mx, v); }
+    }
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int s = 16; s; s >>= 1) {
+        mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, s));
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, s));
+        nan |= __shfl_xor_sync(0xffffffffu, nan, s);
+    }
+    if (lane == 0) { smn[warp] = mn; smx[warp] = mx; snan[warp] = nan; }
+    __syncthreads();
+    mn = smn[0]; mx = smx[0]; nan = snan[0];
+    for (int u = 1; u < kLatexThreads / 32; ++u) {
+        mn = fminf(mn, smn[u]);
+        mx = fmaxf(mx, smx[u]);
+        nan |= snan[u];
+    }
+    if (nan) mn = mx = __int_as_float(0x7fc00000);
+    const float range = __fsub_rn(mx, mn);
+    for (int p = threadIdx.x; p < seq; p += kLatexThreads) {
+        float w = 0.f;
+        if (p < L && !(mx == mn)) {
+            float v = row[p];
+            if (clamp && v < 0.f) v = 0.f;
+            w = __fdiv_rn(__fmul_rn(100.f, __fsub_rn(v, mn)), range);
+            if (w < 1.f) w = 0.f;
+        }
+        o[p] = w;
+    }
+}
+
 }  // namespace
 
 #define ST(s) reinterpret_cast<cudaStream_t>(s)
@@ -501,6 +555,16 @@ extern "C" int te_eraser_soft_scores(const float* word_scores, int batch, const 
         return TE_ERR_CUDA;
     }
     soft_kernel<<<batch, kThreads, 0, st>>>(word_scores, d_woff, d_soff, d_spans, d_tail, scores, flags);
+    TE_CUDA_CHECK_LAUNCH();
+    return TE_OK;
+}
+
+extern "C" int te_eraser_latex_weights(const float* maps, int batch, int seq, const int* lengths, int clamp, float* out,
+                                       void* stream) {
+    REQ(maps && lengths && out, "te_eraser_latex_weights: null argument");
+    REQ(batch > 0 && batch <= 65535 && seq > 0, "te_eraser_latex_weights: batch must lie in 1..65535 and seq be positive");
+    REQ(clamp == 0 || clamp == 1, "te_eraser_latex_weights: clamp must be 0 or 1");
+    latex_kernel<<<batch, kLatexThreads, 0, ST(stream)>>>(maps, seq, lengths, clamp, out);
     TE_CUDA_CHECK_LAUNCH();
     return TE_OK;
 }

@@ -41,6 +41,14 @@ With ``tokens_to_flip=True`` (CLI ``--tokens-to-flip``, with ``--faithfulness``)
 ``te_eraser_soft_scores`` call per batch scores the word scores, followed by a 0 per word past truncation, as
 ``metrics.py``'s soft predictions (``score_soft_tokens``: AUPRC, average precision, ROC AUC): ``soft_results.jsonl`` and
 ``soft_scores.json``.  Both are defined in DESIGN.md §1.
+
+With ``latex=True`` (CLI ``--latex``) each batch also draws the pipeline's LaTeX heat maps (``generate()``, ``:49-93,
+547-561``): one ``te_eraser_latex_weights`` launch turns the gold-class maps, and for the methods of ``LATEX_CF_METHODS``
+the maps of one more generator call for the class 1 - target, into ``generate()``'s colour weights, which join the batch's
+one device-to-host copy; ``latex_document`` writes the reference's bytes (``{j}_GT_{neg|pos}_{correct}.tex``,
+``{j}_CF.tex``).  ``--method ground_truth`` and ``--method generate_all`` write only the pipeline's other two figure
+files (``ground_truth_documents``, ``comparison_figures``); ``generate_all`` writes into ``{output_dir}/generate_all/``
+rather than the current directory.
 """
 import argparse
 import functools
@@ -75,6 +83,7 @@ METHOD_GENERATOR = {"transformer_attribution": ("ours", "generate_LRP"),
 FOLLOW_UP_FOLDER = {"attn_grad_rollout": "attn_grad_rollout"}
 FOLLOW_UP_GENERATOR = {"attn_grad_rollout": ("ours", "generate_attn_grad_rollout")}
 CHOICES = METHODS + tuple(FOLLOW_UP_GENERATOR)
+FIGURE_MODES = ("ground_truth", "generate_all")         # the pipeline's two figure-only modes (bert_pipeline.py:474-546)
 
 
 def topk_rationales(scores, ks=KS):
@@ -495,6 +504,169 @@ def soft_lines(annotations, docids, word_scores, n_words):
             for a, d, s, n in zip(annotations, docids, word_scores, n_words)]
 
 
+# ---- LaTeX heat maps: bert_pipeline.py's generate() and its ground_truth / generate_all modes -------------------------------
+# the methods whose counterfactual (index = 1 - target) map the pipeline also draws (:556-561), plus this port's
+# class-dependent attn_grad_rollout
+LATEX_CF_METHODS = ("transformer_attribution", "partial_lrp", "attn_gradcam", "lrp", "attn_grad_rollout")
+LATEX_ESCAPED = ("\\", "%", "&", "^", "#", "_", "{", "}")          # clean_word's characters, in its order
+_TCBSET = r"\tcbset{width=0.9\textwidth,boxrule=0pt,colback=red,arc=0pt,auto outer arc,left=0pt,right=0pt,boxsep=5pt}"
+_PARBOX = r"{\setlength{\fboxsep}{0pt}\colorbox{white!0}{\parbox{0.9\textwidth}{"
+_CJK_END = r"\end{CJK*}" + "\n" + r"\end{document}"
+LATEX_HEADER = "\n".join([r"\documentclass[varwidth=150mm]{standalone}", r"\special{papersize=210mm,297mm}",
+                          r"\usepackage{color}", r"\usepackage{tcolorbox}", r"\usepackage{CJK}", r"\usepackage{adjustbox}",
+                          _TCBSET, r"\begin{document}", r"\begin{CJK*}{UTF8}{gbsn}", _PARBOX]) + "\n"
+LATEX_FOOTER = "\n}}}\n" + _CJK_END
+
+
+def clean_word(word):
+    """One token as ``clean_word`` escapes it: a backslash before each of ``\\ % & ^ # _ { }``, in that order."""
+    for c in LATEX_ESCAPED:
+        word = word.replace(c, "\\" + c)
+    return word
+
+
+def latex_document(tokens, weights, color="red"):
+    """The text of the file ``generate(tokens, cam, ..., color)`` writes (``bert_pipeline.py:49-84``), from the tokens and
+    the colour weights (the host copy of ``ops.eraser_latex_weights``, one per token; extra weights are ignored).  Each
+    weight is printed as Python prints the float (``%s``); a token is stripped of ``$`` and escaped by ``clean_word``; a
+    token holding an escaped ``##`` joins the previous box with the ``\\#\\#`` removed, every other one follows a space."""
+    if len(weights) < len(tokens):
+        raise ValueError("latex_document: %d weights for %d tokens" % (len(weights), len(tokens)))
+    boxes = []
+    for t, w in zip(tokens, weights):
+        t = clean_word(t.replace("$", ""))
+        glued = "\\#\\#" in t
+        box = "\\colorbox{%s!%s}{\\strut %s}" % (color, float(w), t.replace("\\#\\#", "") if glued else t)
+        boxes.append(box if glued else " " + box)
+    return LATEX_HEADER + "".join(boxes) + LATEX_FOOTER
+
+
+def generate(text_list, attention_list, latex_file, color="red"):
+    """``generate()`` (``bert_pipeline.py:49-84``) with its signature: the weights of the first ``len(text_list)`` entries
+    of the CUDA tensor ``attention_list`` come from one ``te_eraser_latex_weights`` launch (no clamp: the pipeline
+    clamps before it calls), and ``latex_file`` receives ``latex_document``'s text."""
+    from . import ops
+    if not (torch.is_tensor(attention_list) and attention_list.is_cuda):
+        raise ValueError("generate: attention_list must be a CUDA tensor (the weights are computed on the GPU)")
+    n = len(text_list)
+    a = attention_list.reshape(1, -1).to(torch.float32).contiguous()
+    if not 1 <= n <= a.shape[1]:
+        raise ValueError("generate: %d tokens for %d attention values" % (n, a.shape[1]))
+    w = ops.eraser_latex_weights(a, [n], clamp=False)[0, :n].cpu().numpy()
+    with open(latex_file, "w", encoding="utf-8") as f:
+        f.write(latex_document(text_list, w.tolist(), color))
+
+
+def input_words(words, pieces):
+    """``get_input_words`` (``bert_pipeline.py:140-166``): the words that survive truncation, each as the characters of
+    the pieces it covers (``##`` stripped, ``[CLS]`` / ``[SEP]`` / ``[UNK]`` / ``[PAD]`` skipped), so a word cut by the
+    truncation keeps only its covered prefix.  Raises ``ValueError`` where the reference's alignment check fails."""
+    chars = "".join(p.replace("##", "") for p in pieces if p.replace("##", "") not in SPECIAL_PIECES)
+    out, start = [], 0
+    for w in words:
+        if start >= len(chars):
+            break
+        out.append(chars[start:start + len(w)])
+        start += len(w)
+    if out[:-1] != list(words[:len(out) - 1]):
+        raise ValueError("word pieces do not align with the document's words")
+    return out
+
+
+def _neg_pos(target):
+    return "neg" if target == 0 else "pos"
+
+
+def ground_truth_documents(annotations, documents, encodings):
+    """The ``ground_truth`` mode (``bert_pipeline.py:533-546``): {j: (``visual_results_{j}.tex``, text)} per annotation j
+    in dataset order.  The human rationale over ``input_words``: every evidence span of the annotation's first evidence
+    group marks its words, up to the first span that starts past the kept words; drawn in green (100 marked, 0 not; a
+    document marked everywhere or nowhere is a constant map, all 0)."""
+    out = {}
+    for j, ann in enumerate(annotations):
+        d = annotation_docid(ann)
+        words = input_words(documents[d].split(), encodings[d][1])
+        cam = [0] * len(words)
+        for ev in next(iter(ann.evidences)):
+            if ev.start_token >= len(cam):
+                break
+            for i in range(len(cam))[ev.start_token:ev.end_token]:
+                cam[i] = 1
+        weights = [0.0] * len(cam) if len(set(cam)) <= 1 else [100.0 * c for c in cam]
+        out[j] = ("visual_results_%d.tex" % j, latex_document(words, weights, color="green"))
+    return out
+
+
+# the eleven panels of the comparison page (bert_pipeline.py:476-497): (method folder, GT or CF), three per row
+FIGURE_PANELS = (("ground_truth", None), ("ours", "GT"), ("ours", "CF"), ("partial_lrp", "GT"), ("partial_lrp", "CF"),
+                 ("attn_gradcam", "GT"), ("attn_gradcam", "CF"), ("lrp", "GT"), ("lrp", "CF"), ("last_attn", "GT"),
+                 ("rollout", "GT"))
+
+
+def comparison_figure(j, target, correct, output_dir):
+    """The ``generate_all`` page of annotation j (``bert_pipeline.py:474-528``): (``{j}_{neg|pos}_{correct}.tex``, text),
+    a tabular of the eleven PDFs the other modes' files compile to under ``output_dir``."""
+    cls, ok = _neg_pos(target), int(correct)
+    paths = []
+    for folder, kind in FIGURE_PANELS:
+        name = ("visual_results_%d" % j if kind is None else "%d_GT_%s_%d" % (j, cls, ok) if kind == "GT"
+                else "%d_CF" % j)
+        paths.append(os.path.join(output_dir, "%s/%s.pdf" % (folder, name)))
+    pad = " " * 8
+    cells = [pad + r"\includegraphics[width=0.32\linewidth]{" + p + "}" for p in paths]
+    labels = ["(%s)" % chr(ord("a") + i) for i in range(len(paths))]
+    rows = []
+    for r in range(0, len(paths), 3):                       # the last row holds two panels and an empty third cell
+        row, lab = "&\n".join(cells[r:r + 3]), " & ".join(labels[r:r + 3])
+        if r + 3 > len(paths):
+            row, lab = row + "&", lab + "&"
+        rows.append(row + "\\\\\n" + pad + lab + "\\\\\n")
+    text = "\n".join([r"\documentclass[varwidth]{standalone}", r"\usepackage{color}", r"\usepackage{tcolorbox}",
+                      r"\usepackage{CJK}", _TCBSET, r"\begin{document}", r"\begin{CJK*}{UTF8}{gbsn}", _PARBOX,
+                      r"    \setlength{\tabcolsep}{2pt} % Default value: 6pt", r"    \begin{tabular}{ccc}", ""])
+    text += "".join(rows) + "    \\end{tabular}\n}}}\n" + _CJK_END + "\n)"
+    return "%d_%s_%d.tex" % (j, cls, ok), text
+
+
+def comparison_figures(annotations, evidence_classes, pred, output_dir):
+    """The ``generate_all`` mode: {j: (name, text)} per annotation j in dataset order; ``pred`` [annotations] holds the
+    predicted class indices (``predictions``), the correctness flag of each file name is pred == gold class."""
+    out = {}
+    for j, ann in enumerate(annotations):
+        t = evidence_classes[ann.classification]
+        out[j] = comparison_figure(j, t, int(pred[j]) == t, output_dir)
+    return out
+
+
+def predictions(model, annotations, encodings, batch_size=8, pad_id=0):
+    """The first-maximum argmax of the engine forward's logits for every annotation's document, in dataset order: one
+    forward per length-sorted padded batch, no attribution."""
+    eng = model.engine()
+    device = next(model.parameters()).device
+    docids = [annotation_docid(a) for a in annotations]
+    lens = np.array([len(encodings[d][0]) for d in docids], dtype=np.int64)
+    order = sorted(range(len(docids)), key=lambda i: -int(lens[i]))
+    pred = np.zeros(len(docids), dtype=np.int64)
+    for s0 in range(0, len(order), batch_size):
+        idx = order[s0:s0 + batch_size]
+        S = int(lens[idx[0]])
+        ids = torch.full((len(idx), S), pad_id, dtype=torch.long)
+        mask = torch.zeros((len(idx), S), dtype=torch.long)
+        for r, i in enumerate(idx):
+            ids[r, :lens[i]] = torch.as_tensor(encodings[docids[i]][0], dtype=torch.long)
+            mask[r, :lens[i]] = 1
+        pred[idx] = np.argmax(eng.forward(ids.to(device), mask.to(device)).cpu().numpy(), axis=1)
+    return pred
+
+
+def write_documents(docs, folder):
+    """Write {j: (name, text)} (``ground_truth_documents``, ``comparison_figures``) under ``folder``."""
+    os.makedirs(folder, exist_ok=True)
+    for name, text in docs.values():
+        with open(os.path.join(folder, name), "w", encoding="utf-8") as f:
+            f.write(text)
+
+
 def _sorted_chunks(eng, flat, lens, rows, cap, device):
     """The rows ``rows`` of flat [R, S] (host lengths ``lens[q]``), longest first, through the engine forward in padded
     chunks of at most ``cap`` rows (default: the engine's ``max_chunk`` at the chunk's length): yields (chunk, L, logits)."""
@@ -566,6 +738,17 @@ def _flip_search(eng, maps, ids, lens, ranges, woff, orders, pred0, n_words, fli
     return tokens, flipped, n_rows, real, padded
 
 
+LATEX_CF_GENERATORS = tuple({**METHOD_GENERATOR, **FOLLOW_UP_GENERATOR}[m][1] for m in LATEX_CF_METHODS)
+
+
+def latex_logits(eng, input_ids, attention_mask):
+    """A copy of the logits [B, C] of the engine's last forward when it ran on this whole batch (the generator's own
+    forward: no extra pass); otherwise (the generator chunked the batch) one forward of the batch."""
+    if tuple(eng.last) == tuple(input_ids.shape):
+        return eng.tensor("logits").to(torch.float32).clone()
+    return eng.forward(input_ids, attention_mask)
+
+
 def _generator_model(generator_method):
     f = generator_method
     while isinstance(f, functools.partial):
@@ -586,7 +769,7 @@ def _check_fraction(f, what):
 def eraser_eval(generator_method, documents, annotations, encodings, evidence_classes, batch_size=8, ks=KS,
                 iou_thresholds=(0.5,), pad_id=0, device=None, same_length=None, faithfulness=False,
                 aopc_thresholds=AOPC_THRESHOLDS, k_fraction=None, faith_chunk=None, soft_scores=False,
-                tokens_to_flip=False, flip_chunk=16):
+                tokens_to_flip=False, flip_chunk=16, latex=False):
     """The test loop of the pipeline (``bert_pipeline.py:456-582``) and ``metrics.py``'s hard scores on the engine.
 
     generator_method: a bound ``Generator`` method (``generate_LRP`` keeps its ``start_layer = 11``), called as
@@ -611,8 +794,24 @@ def eraser_eval(generator_method, documents, annotations, encodings, evidence_cl
     "scores"}; a NaN word score raises ``ValueError``.  With ``tokens_to_flip`` (needs ``faithfulness``) each batch's
     maps also drive the tokens-to-flip search (DESIGN.md §1) in rounds of ``flip_chunk`` selection sizes per document;
     "faithfulness" gains "tokens_to_flip" [docs], "flipped" [docs], "flip_scores" (``tokens_to_flip.json``),
-    "flip_rows", "flip_real_tokens" and "flip_padded_tokens", and its lines the ``tokens_to_flip`` field."""
+    "flip_rows", "flip_real_tokens" and "flip_padded_tokens", and its lines the ``tokens_to_flip`` field.
+
+    With ``latex`` (two classes only; the generator must be bound to a façade model) each batch also draws the
+    pipeline's LaTeX heat maps (``bert_pipeline.py:547-561``): the gold-class maps above and, for the generators of
+    ``LATEX_CF_METHODS`` (``generate_LRP``, ``generate_LRP_last_layer``, ``generate_attn_gradcam``, ``generate_full_lrp``,
+    ``generate_attn_grad_rollout``), one more call for the counterfactual class 1 - target go through one
+    ``te_eraser_latex_weights`` launch each, and the weights join the batch's one device-to-host copy with the logits of
+    the batch's engine forward (the correctness flag: first argmax == target).  A key "latex" holds {j: {"GT": (name,
+    text), "CF": (name, text)}} per annotation j in dataset order (``CF`` only for those methods); ``generate_LRP``'s
+    batches then hold one token length (its ``[CLS]`` entry, the row minimum, would see the padding)."""
     ks = tuple(int(k) for k in ks)
+    gen_name = getattr(getattr(generator_method, "func", generator_method), "__name__", "")
+    if latex:
+        if len(evidence_classes) != 2:
+            raise ValueError("latex needs exactly two classes: the counterfactual class is 1 - target")
+        latex_eng = _generator_model(generator_method).engine()
+        latex_cf = gen_name in LATEX_CF_GENERATORS
+        latex_docs = {}
     if tokens_to_flip and not faithfulness:
         raise ValueError("tokens_to_flip needs faithfulness (metrics.py reads it with the classification fields)")
     if tokens_to_flip and not 1 <= int(flip_chunk) <= _lib.ERASER_MAX_SELECTIONS:
@@ -633,8 +832,7 @@ def eraser_eval(generator_method, documents, annotations, encodings, evidence_cl
     order = np.full((n, kmax), -1, dtype=np.int64)
     counts = np.zeros((n, len(ks), ncol), dtype=np.int64)
     if same_length is None:
-        name = getattr(getattr(generator_method, "func", generator_method), "__name__", "")
-        same_length = name == "generate_attn_gradcam"
+        same_length = gen_name == "generate_attn_gradcam" or (latex and gen_name == "generate_LRP")
     ks_run = ks
     if faithfulness:
         fracs = [float(f) for f in aopc_thresholds]
@@ -698,6 +896,15 @@ def eraser_eval(generator_method, documents, annotations, encodings, evidence_cl
         maps = maps.reshape(len(idx), S).to(torch.float32).contiguous()
         res = ops.eraser_rationales(maps, wr, woff, sp, soff, ks_run, iou_thresholds)
         parts = [res["order"].reshape(len(idx), -1), res["counts"].reshape(len(idx), -1)]
+        if latex:
+            lens_b = [len(encodings[docids[i]][0]) for i in idx]
+            lat_logits = latex_logits(latex_eng, ids_d, mask_d)
+            lat_parts = [lat_logits.view(torch.int32), ops.eraser_latex_weights(maps, lens_b).view(torch.int32)]
+            if latex_cf:
+                cf = generator_method(input_ids=ids_d, attention_mask=mask_d,
+                                      index=torch.as_tensor([1 - targets[i] for i in idx], device=device))
+                lat_parts.append(ops.eraser_latex_weights(cf.reshape(len(idx), S).to(torch.float32).contiguous(),
+                                                          lens_b).view(torch.int32))
         if soft_scores:
             ssp, ssoff = [], [0]
             for i in idx:
@@ -717,7 +924,20 @@ def eraser_eval(generator_method, documents, annotations, encodings, evidence_cl
             parts.append(red["lengths"].reshape(B, -1).to(parts[0].dtype))
             if tokens_to_flip:                                      # te_logit_stats' pred: the first maximum
                 parts.append(ops.logit_stats(logits, torch.zeros(B, dtype=torch.int32, device=device))[0][:, None])
+        if latex:
+            lat0 = sum(p.shape[1] for p in parts)
+            parts += lat_parts
         host = torch.cat(parts, dim=1).cpu().numpy()
+        if latex:                                   # per row: [logits (nc) | gold-class weights (S) | counterfactual (S)]
+            nc = lat_logits.shape[1]
+            lat_host = np.ascontiguousarray(host[:, lat0:]).view(np.float32)
+            for r, i in enumerate(idx):
+                t, L, pieces, w = targets[i], lens_b[r], encodings[docids[i]][1], lat_host[r]
+                correct = int(np.argmax(w[:nc])) == t
+                doc = {"GT": ("%d_GT_%s_%d.tex" % (i, _neg_pos(t), correct), latex_document(pieces, w[nc:nc + L]))}
+                if latex_cf:
+                    doc["CF"] = ("%d_CF.tex" % i, latex_document(pieces, w[nc + S:nc + S + L]))
+                latex_docs[i] = doc
         kr = ks_run[-1]
         order[idx] = host[:, :kmax]
         counts[idx] = host[:, kr:kr + len(ks) * ncol].reshape(len(idx), len(ks), ncol)
@@ -772,6 +992,8 @@ def eraser_eval(generator_method, documents, annotations, encodings, evidence_cl
                 "tokens_to_flip": flip_tok, "flipped": flipped,
                 "flip_scores": flip_scores(annotations, docids, n_words, flip_tok, flipped), "flip_rows": flip_stats[0],
                 "flip_real_tokens": flip_stats[1], "flip_padded_tokens": flip_stats[2]})
+    if latex:
+        out["latex"] = {j: latex_docs[j] for j in range(n)}
     if soft_scores:
         out["soft"] = {"per_document": soft_doc, "single_class": single,
                        "lines": soft_lines(annotations, docids, soft_words, n_words),
@@ -804,6 +1026,8 @@ def write_results(results, folder):
             f.write("".join(line + "\n" for line in results["soft"]["lines"]))
         with open(os.path.join(folder, "soft_scores.json"), "w") as f:
             json.dump(results["soft"]["scores"], f, indent=4, sort_keys=True)
+    if "latex" in results:
+        write_documents({(j, k): v for j, doc in results["latex"].items() for k, v in doc.items()}, folder)
 
 
 # ---- command line ---------------------------------------------------------------------------------------------------------
@@ -813,7 +1037,9 @@ def build_parser():
     p.add_argument("--output_dir", dest="output_dir", required=True)
     p.add_argument("--model_params", dest="model_params", required=True,
                    help="the pipeline's JSON parameters (bert_vocab, bert_dir, max_length, evidence_classifier.classes)")
-    p.add_argument("--method", default="transformer_attribution", choices=CHOICES)
+    p.add_argument("--method", default="transformer_attribution", choices=CHOICES + FIGURE_MODES,
+                   help="an explanation method, or one of the pipeline's figure modes: ground_truth (the human "
+                        "rationales as LaTeX heat maps) and generate_all (the comparison page of every method's maps)")
     p.add_argument("--split", default="test")
     p.add_argument("--state-dict", dest="state_dict", default=None,
                    help="classifier weights (default: output_dir/classifier/classifier.pt, where the pipeline saves them)")
@@ -831,6 +1057,9 @@ def build_parser():
     p.add_argument("--tokens-to-flip", dest="tokens_to_flip", action="store_true",
                    help="also find each document's tokens to flip: the fewest best-ranked words whose removal changes "
                         "the prediction (needs --faithfulness)")
+    p.add_argument("--latex", action="store_true",
+                   help="also write the pipeline's LaTeX heat maps: {j}_GT_{neg|pos}_{correct}.tex for the gold class and, "
+                        "for %s, {j}_CF.tex for the other class (two classes only)" % ", ".join(LATEX_CF_METHODS))
     return p
 
 
@@ -849,6 +1078,8 @@ def parse_args(argv=None):
         p.error("--k-fraction must lie in (0, 1]")
     if args.tokens_to_flip and not args.faithfulness:
         p.error("--tokens-to-flip needs --faithfulness")
+    if args.method in FIGURE_MODES and (args.latex or args.faithfulness or args.soft_scores):
+        p.error("--method %s writes only its .tex files" % args.method)
     if args.state_dict is None:
         args.state_dict = os.path.join(args.output_dir, "classifier", "classifier.pt")
     return args
@@ -886,11 +1117,22 @@ def main(argv=None):
                                  params["max_length"])
     classes = params["evidence_classifier"]["classes"]
     evidence_classes = {c: i for i, c in enumerate(classes)}
+    if args.method == "ground_truth":
+        docs = ground_truth_documents(annotations, documents, encodings)
+        write_documents(docs, os.path.join(args.output_dir, "ground_truth"))
+        return docs
+    if args.method == "generate_all":                     # the classifier of transformer_attribution predicts (:467)
+        model = _generator_model(build_generator("transformer_attribution", params["bert_dir"], len(classes),
+                                                 args.state_dict))
+        pred = predictions(model, annotations, encodings, batch_size=args.batch_size)
+        docs = comparison_figures(annotations, evidence_classes, pred, args.output_dir)
+        write_documents(docs, os.path.join(args.output_dir, "generate_all"))
+        return docs
     gen = build_generator(args.method, params["bert_dir"], len(classes), args.state_dict)
     res = eraser_eval(gen, documents, annotations, encodings, evidence_classes, batch_size=args.batch_size,
                       iou_thresholds=args.iou_thresholds, faithfulness=args.faithfulness,
                       aopc_thresholds=args.aopc_thresholds, k_fraction=args.k_fraction, soft_scores=args.soft_scores,
-                      tokens_to_flip=args.tokens_to_flip)
+                      tokens_to_flip=args.tokens_to_flip, latex=args.latex)
     write_results(res, os.path.join(args.output_dir, {**METHOD_FOLDER, **FOLLOW_UP_FOLDER}[args.method]))
     for k in KS:
         print("top-%d token F1 %.4f (instance macro %.4f)" % (k, res["scores"][k]["token_prf"]["instance_micro"]["f1"],

@@ -749,6 +749,40 @@ def eraser_soft_scores(word_scores, word_offsets, spans, span_offsets, tail_coun
     return out
 
 
+@_on_device
+def eraser_latex_weights(maps, lengths, clamp=True, out=None):
+    """The colour weights ``bert_pipeline.py``'s ``generate()`` prints for each row b of maps [B, S] (padded rows, fp32
+    CUDA), over its first ``lengths[b]`` entries: optionally ``clamp(min=0)``, then 0 for a constant row, else
+    ``(100 * (a - min)) / (max - min)`` in fp32 with the reference's roundings, and values below 1 set to 0; NaN anywhere
+    in the row makes the row NaN; zeros past the length (see include/te_b200.h: te_eraser_latex_weights).  ``lengths``
+    [B] is a host sequence (1 <= L <= S) or an int32 CUDA tensor of checked lengths; ``out`` [B, S] fp32 may be given (a
+    view into a larger buffer, contiguous).  Returns ``out``."""
+    import numpy as np
+    _req(maps)
+    if maps.dim() != 2:
+        raise ValueError("eraser_latex_weights: maps [B, S] expected")
+    B, S = maps.shape
+    if torch.is_tensor(lengths) and lengths.is_cuda:
+        if lengths.dtype != torch.int32 or lengths.shape != (B,) or not lengths.is_contiguous() or \
+                lengths.device != maps.device:
+            raise ValueError("eraser_latex_weights: CUDA lengths must be int32 [B] contiguous on the maps' device")
+        lens = lengths
+    else:
+        host = _host_i32(lengths, "lengths", op="eraser_latex_weights")
+        if host.shape != (B,):
+            raise ValueError("eraser_latex_weights: lengths need B = %d entries" % B)
+        if B and (host.min() < 1 or host.max() > S):
+            raise ValueError("eraser_latex_weights: every length must lie in 1..S = %d" % S)
+        lens = torch.from_numpy(np.ascontiguousarray(host)).to(maps.device)
+    out = torch.empty_like(maps) if out is None else out
+    _req(out)
+    if out.shape != maps.shape or out.device != maps.device:
+        raise ValueError("eraser_latex_weights: out must be [B, S] on the maps' device")
+    check(_lib.load().te_eraser_latex_weights(ptr(maps), B, S, ptr(lens), int(bool(clamp)), ptr(out), _stream()),
+          "te_eraser_latex_weights")
+    return out
+
+
 # ---- input preparation (baselines/ViT/generate_visualizations.py: Resize((224, 224)) + ToTensor()) ---------------------------
 @_on_device
 def prepare_images(packed_u8, sizes, offsets, out_hw=(224, 224), mean=None, std=None):
