@@ -208,11 +208,14 @@ TE_API long long te_bert_derived_total(const te_bert_config* cfg);
 TE_API int te_bert_prepare_derived(const te_bert_config* cfg, const float* weights, float* derived, void* stream);
 TE_API long long te_bert_workspace_bytes(const te_bert_config* cfg, int batch, int seq);
 
-/* model(input_ids, attention_mask)[0]: ids / mask are int64 [batch, seq] (device); token_type_ids = 0,
- * position_ids = arange(seq) as in BERT.py:69-75; logits [batch, num_labels] (may be NULL). */
+/* model(input_ids, attention_mask, token_type_ids)[0]: ids / mask / token types are int64 [batch, seq] (device);
+ * token_type_ids may be NULL (every token in segment 0, as BERT.py:69-75 defaults it); position_ids = arange(seq).  An id
+ * outside [0, vocab_size) or a token type outside [0, type_vocab) never indexes its table: that token's embedding row is
+ * NaN, and with it the sample's logits.  logits [batch, num_labels] (may be NULL). */
 TE_API int te_bert_forward(const te_bert_config* cfg, const float* weights, const float* derived,
-                    const long long* input_ids, const long long* attention_mask, int batch, int seq, unsigned flags,
-                    float* logits, void* workspace, long long workspace_bytes, void* stream);
+                    const long long* input_ids, const long long* attention_mask, const long long* token_type_ids,
+                    int batch, int seq, unsigned flags, float* logits, void* workspace, long long workspace_bytes,
+                    void* stream);
 /* The rest of Generator.generate_LRP (ExplanationGenerator.py:33-59): arg-max (index[b] < 0), one-hot, class
  * gradient of every attention_probs, relprop (BertForSequenceClassification.relprop), relu(grad*cam) head mean,
  * +I, row-normalised rollout from start_layer, row 0 with element 0 replaced by the row minimum.
@@ -221,11 +224,12 @@ TE_API int te_bert_forward(const te_bert_config* cfg, const float* weights, cons
 TE_API int te_bert_attribute(const te_bert_config* cfg, const float* weights, const float* derived, int batch, int seq,
                              int* index, int start_layer, float alpha, unsigned flags, float* maps, void* workspace,
                              long long workspace_bytes, void* stream);
-/* te_bert_forward + te_bert_attribute (alpha = 1). */
+/* te_bert_forward + te_bert_attribute (alpha = 1).  te_bert_attribute starts from the saved activations and stops at the
+ * encoder input (BertModel.relprop, BERT.py:645-651), so it never reads the ids or the token types. */
 TE_API int te_bert_explain(const te_bert_config* cfg, const float* weights, const float* derived,
-                    const long long* input_ids, const long long* attention_mask, int batch, int seq, int* index,
-                    int start_layer, unsigned flags, float* maps, float* logits, void* workspace,
-                    long long workspace_bytes, void* stream);
+                    const long long* input_ids, const long long* attention_mask, const long long* token_type_ids,
+                    int batch, int seq, int* index, int start_layer, unsigned flags, float* maps, float* logits,
+                    void* workspace, long long workspace_bytes, void* stream);
 /* get_attn / get_attn_gradients / get_attn_cam of BertSelfAttention (BERT.py:281-297):
  * name in {"attn","attn_grad","attn_cam","hidden","logits","relevance_in"} and the scratch regions "tmp_d0".."tmp_d3",
  * "tmp_f0","tmp_f1", "tmp_3d0","tmp_3d1" as for te_vit_tensor.
@@ -519,6 +523,21 @@ TE_API int te_eraser_soft_scores(const float* word_scores, int batch, const int*
  * One launch (a block per row), no workspace. */
 TE_API int te_eraser_latex_weights(const float* maps, int batch, int seq, const int* lengths, int clamp, float* out,
                                    void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Word importance of the BERT notebook (BERT_explainability.ipynb: min-max normalised generate_LRP map, negated when the
+ * explained class is NEGATIVE)
+ * ---------------------------------------------------------------------------------------------- */
+/* Per row b of maps [batch, seq] (device, padded rows), over its first L = lengths[b] entries a (lengths: device int32,
+ * 1 <= L <= seq; the caller checks them, the kernel clips them to [0, seq]), with sign [batch] (device fp32, +1 or -1):
+ *   mn, mx = min(a), max(a), NaN if any entry is NaN (torch.min / max);
+ *   out[b, :L] = 0 when mx == mn, else ((a - mn) / (mx - mn)) * sign[b], each operation one IEEE fp32 rounding
+ *   (__fsub_rn, __fdiv_rn, __fmul_rn, no contraction), so a NaN row stays NaN;  out[b, L:seq] = 0.  maps[b, L:] is never
+ *   read.
+ * batch in 1..65535, seq >= 1, maps / lengths / sign / out non-NULL, else TE_ERR_ARG before anything is launched.
+ * One launch (a block per row), no workspace. */
+TE_API int te_token_importance(const float* maps, const int* lengths, const float* sign, int batch, int seq, float* out,
+                               void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Input preparation  (baselines/ViT/generate_visualizations.py:194-199: Resize((224, 224)) + ToTensor() on PIL images)

@@ -159,11 +159,14 @@ class BertForSequenceClassification(nn.Module):
 
     def forward(self, input_ids=None, attention_mask=None, token_type_ids=None, position_ids=None, head_mask=None,
                 inputs_embeds=None, labels=None, output_attentions=None, output_hidden_states=None, return_dict=None):
-        """``BertForSequenceClassification.forward`` (:23-81) with return_dict=False: returns ``(logits,)``."""
-        if token_type_ids is not None or position_ids is not None or head_mask is not None or inputs_embeds is not None:
-            raise NotImplementedError("only input_ids / attention_mask are used on the attribution path "
+        """``BertForSequenceClassification.forward`` (:23-81) with return_dict=False: returns ``(logits,)``.
+        ``token_type_ids`` (the segments of a sentence pair, what a tokenizer returns) enter the embeddings as in
+        ``BertEmbeddings.forward`` (``BERT.py:61-85``); None puts every token in segment 0, so ``model(**encoding)``
+        explains what the model was given."""
+        if position_ids is not None or head_mask is not None or inputs_embeds is not None:
+            raise NotImplementedError("position_ids, head_mask and inputs_embeds are not used on the attribution path "
                                       "(bert_pipeline.py:443,551)")
-        return (self.engine().forward(input_ids, attention_mask),)
+        return (self.engine().forward(input_ids, attention_mask, token_type_ids=token_type_ids),)
 
     def relprop(self, cam=None, **kwargs):
         """``relprop`` (:83-88): relevance at the encoder input [B,S,D]; leaves attn_cam / attn_gradients of every

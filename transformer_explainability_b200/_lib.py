@@ -81,9 +81,9 @@ PROTOTYPES = {
     "te_bert_derived_total": (c_ll, [_BCFG]),
     "te_bert_prepare_derived": (c_int, [_BCFG, _P, _P, _P]),
     "te_bert_workspace_bytes": (c_ll, [_BCFG, c_int, c_int]),
-    "te_bert_forward": (c_int, [_BCFG, _P, _P, _P, _P, c_int, c_int, c_uint, _P, _P, c_ll, _P]),
+    "te_bert_forward": (c_int, [_BCFG, _P, _P, _P, _P, _P, c_int, c_int, c_uint, _P, _P, c_ll, _P]),
     "te_bert_attribute": (c_int, [_BCFG, _P, _P, c_int, c_int, _P, c_int, c_float, c_uint, _P, _P, c_ll, _P]),
-    "te_bert_explain": (c_int, [_BCFG, _P, _P, _P, _P, c_int, c_int, _P, c_int, c_uint, _P, _P, _P, c_ll, _P]),
+    "te_bert_explain": (c_int, [_BCFG, _P, _P, _P, _P, _P, c_int, c_int, _P, c_int, c_uint, _P, _P, _P, c_ll, _P]),
     "te_bert_tensor": (c_int, [_BCFG, c_int, c_int, _P, c_char_p, c_int, ctypes.POINTER(_P), ctypes.POINTER(c_ll),
                                ctypes.POINTER(c_ll)]),
     "te_linear_relprop": (c_int, [_P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_float, c_uint, _P]),
@@ -127,6 +127,7 @@ PROTOTYPES = {
     "te_eraser_soft_workspace_bytes": (c_ll, [c_int, c_ll]),
     "te_eraser_soft_scores": (c_int, [_P, c_int, _P, _P, _P, _P, _P, _P, _P, c_ll, _P]),
     "te_eraser_latex_weights": (c_int, [_P, c_int, c_int, _P, c_int, _P, _P]),
+    "te_token_importance": (c_int, [_P, _P, _P, c_int, c_int, _P, _P]),
     "te_resize_coeffs": (c_int, [c_int, c_int, _P, _P]),
     "te_prepare_images_workspace_bytes": (c_ll, [c_int, c_int, c_int, c_int, c_int]),
     "te_prepare_images": (c_int, [_P, c_ll, c_int, _P, _P, c_int, c_int, _P, _P, _P, _P, _P, c_ll, _P]),

@@ -229,8 +229,9 @@ extern "C" int te_bert_prepare_derived(const te_bert_config* cfg, const float* w
 // forward  (BertForSequenceClassification.forward -> BertModel.forward)
 // =====================================================================================================
 extern "C" int te_bert_forward(const te_bert_config* cfg, const float* weights, const float* derived,
-                               const long long* input_ids, const long long* attention_mask, int batch, int seq,
-                               unsigned flags, float* logits, void* workspace, long long workspace_bytes, void* stream) {
+                               const long long* input_ids, const long long* attention_mask,
+                               const long long* token_type_ids, int batch, int seq, unsigned flags, float* logits,
+                               void* workspace, long long workspace_bytes, void* stream) {
     Dims d; Workspace ws;
     TE_TRY(check_ws(cfg, batch, seq, workspace, workspace_bytes, d, ws));
     if (!weights || !input_ids || !attention_mask) { te_set_last_error("te_bert_forward: null pointer"); return TE_ERR_ARG; }
@@ -249,7 +250,7 @@ extern "C" int te_bert_forward(const te_bert_config* cfg, const float* weights, 
     bind_weights(cfg, weights, w);
     const float scale = 1.0f / sqrtf((float)d.dh);
 
-    TE_TRY(te_launch_bert_embed(input_ids, w.word, w.pos, w.type, ws.tD[0], d.B, d.N, d.D, d.V, st));
+    TE_TRY(te_launch_bert_embed(input_ids, token_type_ids, w.word, w.pos, w.type, ws.tD[0], d.B, d.N, d.D, d.V, d.T, st));
     TE_TRY(layernorm(ws.tD[0], w.elnw, w.elnb, ws.layer[0].h, nullptr, nullptr));
     TE_TRY(te_launch_bert_mask(attention_mask, ws.maskadd, (long long)d.B * d.N, st));
 
@@ -424,11 +425,12 @@ extern "C" int te_bert_attribute(const te_bert_config* cfg, const float* weights
 }
 
 extern "C" int te_bert_explain(const te_bert_config* cfg, const float* weights, const float* derived,
-                               const long long* input_ids, const long long* attention_mask, int batch, int seq,
-                               int* index, int start_layer, unsigned flags, float* maps, float* logits, void* workspace,
-                               long long workspace_bytes, void* stream) {
-    TE_TRY(te_bert_forward(cfg, weights, derived, input_ids, attention_mask, batch, seq, flags, logits, workspace,
-                           workspace_bytes, stream));
+                               const long long* input_ids, const long long* attention_mask,
+                               const long long* token_type_ids, int batch, int seq, int* index, int start_layer,
+                               unsigned flags, float* maps, float* logits, void* workspace, long long workspace_bytes,
+                               void* stream) {
+    TE_TRY(te_bert_forward(cfg, weights, derived, input_ids, attention_mask, token_type_ids, batch, seq, flags, logits,
+                           workspace, workspace_bytes, stream));
     return te_bert_attribute(cfg, weights, derived, batch, seq, index, start_layer, 1.f, flags, maps, workspace, workspace_bytes,
                              stream);
 }

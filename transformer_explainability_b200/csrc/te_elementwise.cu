@@ -631,10 +631,12 @@ __global__ void average2_kernel(const float* __restrict__ a, const float* __rest
 // ------------------------------------------------------------------------------------------------
 // BERT extras: embeddings, additive mask, tanh, elementwise add, Add rule with a key-broadcast operand
 // ------------------------------------------------------------------------------------------------
-// (token_type + position) + word   (BertEmbeddings.forward, BERT.py:80-81; token_type_ids = 0, position_ids = arange)
-__global__ void bert_embed_kernel(const long long* __restrict__ ids, const float* __restrict__ word,
-                                  const float* __restrict__ pos, const float* __restrict__ type0,
-                                  float* __restrict__ out, int B, int S, int D, int vocab) {
+// (token_type + position) + word   (BertEmbeddings.forward, BERT.py:80-81; position_ids = arange).  tt == NULL: every
+// token is segment 0 (row 0 of the token-type table).
+__global__ void bert_embed_kernel(const long long* __restrict__ ids, const long long* __restrict__ tt,
+                                  const float* __restrict__ word, const float* __restrict__ pos,
+                                  const float* __restrict__ type, float* __restrict__ out, int B, int S, int D, int vocab,
+                                  int type_vocab) {
     const int d4 = D / 4;
     const long long total = (long long)B * S * d4;
     for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < total;
@@ -643,14 +645,16 @@ __global__ void bert_embed_kernel(const long long* __restrict__ ids, const float
         const long long rt = t / d4;
         const int s = (int)(rt % S);
         const long long id = ids[rt];
-        if (id < 0 || id >= vocab) {          // never index the table out of bounds: the row becomes NaN (loud, memory-safe)
+        const long long ty_id = tt ? tt[rt] : 0;
+        // never index a table out of bounds: the row becomes NaN (loud, memory-safe)
+        if (id < 0 || id >= vocab || ty_id < 0 || ty_id >= type_vocab) {
             const float qn = __int_as_float(0x7fc00000);
             *reinterpret_cast<float4*>(out + rt * D + q * 4) = make_float4(qn, qn, qn, qn);
             continue;
         }
         const float4 w = *reinterpret_cast<const float4*>(word + id * D + q * 4);
         const float4 p = *reinterpret_cast<const float4*>(pos + (long long)s * D + q * 4);
-        const float4 ty = *reinterpret_cast<const float4*>(type0 + q * 4);
+        const float4 ty = *reinterpret_cast<const float4*>(type + ty_id * D + q * 4);
         *reinterpret_cast<float4*>(out + rt * D + q * 4) =
             make_float4((ty.x + p.x) + w.x, (ty.y + p.y) + w.y, (ty.z + p.z) + w.z, (ty.w + p.w) + w.w);
     }
@@ -933,10 +937,11 @@ int te_launch_average2(const float* a, const float* b, float* out, long long n, 
     TE_CUDA_CHECK_LAUNCH();
     return TE_OK;
 }
-int te_launch_bert_embed(const long long* ids, const float* word, const float* pos, const float* type0, float* out,
-                         int B, int S, int D, int vocab, cudaStream_t st) {
+int te_launch_bert_embed(const long long* ids, const long long* token_type_ids, const float* word, const float* pos,
+                         const float* type, float* out, int B, int S, int D, int vocab, int type_vocab, cudaStream_t st) {
     TE_REQ(D % 4 == 0, "bert_embed: D % 4 != 0");
-    bert_embed_kernel<<<flat_grid((long long)B * S * (D / 4)), kThreads, 0, st>>>(ids, word, pos, type0, out, B, S, D, vocab);
+    bert_embed_kernel<<<flat_grid((long long)B * S * (D / 4)), kThreads, 0, st>>>(ids, token_type_ids, word, pos, type, out,
+                                                                                 B, S, D, vocab, type_vocab);
     TE_CUDA_CHECK_LAUNCH();
     return TE_OK;
 }

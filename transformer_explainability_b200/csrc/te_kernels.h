@@ -75,9 +75,10 @@ int te_launch_fill(float* p, float v, long long n, cudaStream_t st);
 // ---- BERT extras -------------------------------------------------------------------------------
 int te_launch_softmax_masked(float* s, long long rows, int N, int ld, const float* keymask, long long rows_per_batch,
                              cudaStream_t st);
-// ids outside [0, vocab) never index the table: their rows are written as NaN
-int te_launch_bert_embed(const long long* ids, const float* word, const float* pos, const float* type0, float* out,
-                         int B, int S, int D, int vocab, cudaStream_t st);
+// ids outside [0, vocab) and token types outside [0, type_vocab) never index a table: their rows are written as NaN.
+// token_type_ids == NULL: every token is segment 0.
+int te_launch_bert_embed(const long long* ids, const long long* token_type_ids, const float* word, const float* pos,
+                         const float* type, float* out, int B, int S, int D, int vocab, int type_vocab, cudaStream_t st);
 int te_launch_bert_mask(const long long* mask, float* out, long long n, cudaStream_t st);
 int te_launch_tanh(const float* x, float* y, long long n, cudaStream_t st);
 int te_launch_tanh_bwd(const float* dy, const float* y, float* dx, long long n, cudaStream_t st);

@@ -361,24 +361,38 @@ class BertEngine(_Engine):
     def max_chunk(self, seq, limit=None, reserve_bytes=4 << 30):
         return self._max_batch(limit, reserve_bytes, seq)
 
-    def _ids(self, input_ids, attention_mask):
+    def _ids(self, input_ids, attention_mask, token_type_ids=None):
         if not input_ids.is_cuda and input_ids.numel() and (int(input_ids.min()) < 0 or
                                                             int(input_ids.max()) >= self.cfg.vocab_size):
             raise ValueError("input_ids outside [0, vocab_size)")     # device-resident ids: the kernel writes NaN rows
         ids = input_ids.to(self.device, torch.int64).contiguous()
         if attention_mask is None:
             attention_mask = torch.ones_like(ids)
-        return ids, attention_mask.to(self.device, torch.int64).contiguous()
+        return ids, attention_mask.to(self.device, torch.int64).contiguous(), self._token_types(token_type_ids, ids.shape)
+
+    def _token_types(self, token_type_ids, shape):
+        """The segment of every token (BertEmbeddings' token_type_ids), int64 on the device; None: every token in segment 0
+        (the kernel reads no table row but row 0)."""
+        if token_type_ids is None:
+            return None
+        tt = torch.as_tensor(token_type_ids)
+        if tuple(tt.shape) != tuple(shape):
+            raise ValueError("token_type_ids must have the shape of input_ids %s, got %s" % (tuple(shape), tuple(tt.shape)))
+        if not tt.is_cuda and tt.numel() and (int(tt.min()) < 0 or int(tt.max()) >= self.cfg.type_vocab):
+            raise ValueError("token_type_ids outside [0, type_vocab_size)")   # device-resident: the kernel writes NaN rows
+        return tt.to(self.device, torch.int64).contiguous()
 
     @_on_engine_device
-    def forward(self, input_ids, attention_mask=None, flags=None):
-        ids, mask = self._ids(input_ids, attention_mask)
+    def forward(self, input_ids, attention_mask=None, flags=None, token_type_ids=None):
+        """``model(input_ids, attention_mask, token_type_ids)``: logits [B,C]; leaves the activations in the workspace.
+        token_type_ids: the segment of every token, the shape of input_ids; None puts every token in segment 0."""
+        ids, mask, tt = self._ids(input_ids, attention_mask, token_type_ids)
         b, s = ids.shape
         ws = self._workspace(b, s)
         fl = self.flags if flags is None else flags
         logits = torch.empty(b, self.cfg.num_labels, dtype=torch.float32, device=self.device)
         check(self.lib.te_bert_forward(ctypes.byref(self.cfg), ptr(self.weights), ptr(self._derived(fl)), ptr(ids),
-                                       ptr(mask), b, s, fl, ptr(logits), ptr(ws), ws.numel() * 4, self._stream()),
+                                       ptr(mask), ptr(tt), b, s, fl, ptr(logits), ptr(ws), ws.numel() * 4, self._stream()),
               "te_bert_forward")
         self.last = (b, s)
         return logits
@@ -401,8 +415,10 @@ class BertEngine(_Engine):
 
     @_on_engine_device
     def explain(self, input_ids, attention_mask=None, index=None, start_layer=11, flags=None, chunk=None,
-                return_logits=False):
-        ids, mask = self._ids(input_ids, attention_mask)
+                return_logits=False, token_type_ids=None):
+        """``Generator.generate_LRP`` of B independent sequences of one length: (maps [B,S], index [B] int32) and, with
+        ``return_logits``, the logits [B,C].  token_type_ids as for ``forward``."""
+        ids, mask, tt = self._ids(input_ids, attention_mask, token_type_ids)
         B, S = ids.shape
         chunk = min(B, chunk or self.max_chunk(S, limit=B))
         maps = torch.empty(B, S, dtype=torch.float32, device=self.device)
@@ -414,7 +430,8 @@ class BertEngine(_Engine):
             e = min(B, s0 + chunk)
             ws = self._workspace(e - s0, S)
             check(self.lib.te_bert_explain(ctypes.byref(self.cfg), ptr(self.weights), ptr(derived), ptr(ids[s0:e]),
-                                           ptr(mask[s0:e]), e - s0, S, ptr(idx_all[s0:e]), int(start_layer), fl,
+                                           ptr(mask[s0:e]), ptr(tt[s0:e]) if tt is not None else None, e - s0, S,
+                                           ptr(idx_all[s0:e]), int(start_layer), fl,
                                            ptr(maps[s0:e]), ptr(logits[s0:e]) if logits is not None else None, ptr(ws),
                                            ws.numel() * 4, self._stream()), "te_bert_explain")
             self.last = (e - s0, S)

@@ -783,6 +783,48 @@ def eraser_latex_weights(maps, lengths, clamp=True, out=None):
     return out
 
 
+@_on_device
+def token_importance(maps, lengths, sign, out=None):
+    """The word importance the BERT notebook shows for each row b of maps [B, S] (padded rows, fp32 CUDA), over its first
+    ``lengths[b]`` tokens: ``(a - min) / (max - min)`` times ``sign[b]`` (-1 where the explained class is NEGATIVE) in fp32
+    with one rounding per operation; 0 for a constant row, NaN anywhere in the row makes the row NaN, zeros past the length
+    (see include/te_b200.h: te_token_importance).  ``lengths`` [B] is a host sequence (1 <= L <= S) or an int32 CUDA
+    tensor of checked lengths; ``sign`` [B] a host sequence or an fp32 CUDA tensor; ``out`` [B, S] fp32 may be given (a
+    view into a larger buffer, contiguous).  Returns ``out``."""
+    import numpy as np
+    _req(maps)
+    if maps.dim() != 2:
+        raise ValueError("token_importance: maps [B, S] expected")
+    B, S = maps.shape
+    if torch.is_tensor(lengths) and lengths.is_cuda:
+        if lengths.dtype != torch.int32 or lengths.shape != (B,) or not lengths.is_contiguous() or \
+                lengths.device != maps.device:
+            raise ValueError("token_importance: CUDA lengths must be int32 [B] contiguous on the maps' device")
+        lens = lengths
+    else:
+        host = _host_i32(lengths, "lengths", op="token_importance")
+        if host.shape != (B,):
+            raise ValueError("token_importance: lengths need B = %d entries" % B)
+        if B and (host.min() < 1 or host.max() > S):
+            raise ValueError("token_importance: every length must lie in 1..S = %d" % S)
+        lens = torch.from_numpy(np.ascontiguousarray(host)).to(maps.device)
+    if torch.is_tensor(sign) and sign.is_cuda:
+        if sign.dtype != torch.float32 or sign.shape != (B,) or not sign.is_contiguous() or sign.device != maps.device:
+            raise ValueError("token_importance: a CUDA sign must be fp32 [B] contiguous on the maps' device")
+        sg = sign
+    else:
+        sg = torch.as_tensor(np.asarray(sign, dtype=np.float32).reshape(-1))
+        if sg.shape != (B,):
+            raise ValueError("token_importance: sign needs B = %d entries" % B)
+        sg = sg.to(maps.device)
+    out = torch.empty_like(maps) if out is None else out
+    _req(out)
+    if out.shape != maps.shape or out.device != maps.device:
+        raise ValueError("token_importance: out must be [B, S] on the maps' device")
+    check(_lib.load().te_token_importance(ptr(maps), ptr(lens), ptr(sg), B, S, ptr(out), _stream()), "te_token_importance")
+    return out
+
+
 # ---- input preparation (baselines/ViT/generate_visualizations.py: Resize((224, 224)) + ToTensor()) ---------------------------
 @_on_device
 def prepare_images(packed_u8, sizes, offsets, out_hw=(224, 224), mean=None, std=None):
