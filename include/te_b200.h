@@ -195,9 +195,28 @@ typedef struct te_bert_config {
     int intermediate;     /* 3072 */
     int num_labels;       /* 2 */
     float layer_norm_eps; /* 1e-12 */
+    int arch;             /* TE_BERT_ARCH_*: the model family; 0 = BERT */
+    int pad_token_id;     /* RoBERTa: the padding id its position ids count from (1); ignored by the other families */
 } te_bert_config;
 
-/* flat fp32 weight buffer keyed by the HF state_dict names (query|key|value of a layer are adjacent and are
+/* The encoder families te_bert_* run.  Every family is the same post-LN encoder layer (q/k/v, output dense, GELU MLP,
+ * two LayerNorms); only the embedding and the classifier head differ:
+ *   BERT        bert.*        position ids arange(seq); (type + position) + word; pooler.dense -> tanh -> classifier
+ *   RoBERTa     roberta.*     position ids pad + cumsum(ids != pad) for non-pad tokens, pad for pad tokens
+ *               (XLM-R too)   (create_position_ids_from_input_ids); (word + type) + position;
+ *                             classifier.dense -> tanh -> classifier.out_proj.  Needs 0 <= pad_token_id < vocab_size and
+ *                             seq + pad_token_id + 1 <= max_position (514 positions hold 512 tokens with pad 1).
+ *   DistilBERT  distilbert.*  position ids arange(seq); word + position, no token-type table (type_vocab must be 0, and a
+ *                             non-NULL token_type_ids is TE_ERR_ARG); pre_classifier -> ReLU -> classifier.
+ * BERT and RoBERTa need type_vocab > 0.  An invalid combination returns TE_ERR_ARG with a message.  The workspace size
+ * is the same function of (batch, seq, hidden, intermediate, layers, heads, num_labels) for every family, and
+ * te_bert_tensor("pooled") is the head activation's output (tanh or ReLU).  The relevance rules treat both activations
+ * as the identity, so relprop and rollout are the same for every family. */
+#define TE_BERT_ARCH_BERT 0
+#define TE_BERT_ARCH_ROBERTA 1
+#define TE_BERT_ARCH_DISTILBERT 2
+
+/* flat fp32 weight buffer keyed by the family's HF state_dict names (query|key|value of a layer are adjacent and are
  * used as one packed [3*hidden, hidden] weight); derived = tensor-core copies as for ViT. */
 TE_API int te_bert_num_weights(const te_bert_config* cfg);
 TE_API const char* te_bert_weight_name(const te_bert_config* cfg, int i);
@@ -209,9 +228,10 @@ TE_API int te_bert_prepare_derived(const te_bert_config* cfg, const float* weigh
 TE_API long long te_bert_workspace_bytes(const te_bert_config* cfg, int batch, int seq);
 
 /* model(input_ids, attention_mask, token_type_ids)[0]: ids / mask / token types are int64 [batch, seq] (device);
- * token_type_ids may be NULL (every token in segment 0, as BERT.py:69-75 defaults it); position_ids = arange(seq).  An id
- * outside [0, vocab_size) or a token type outside [0, type_vocab) never indexes its table: that token's embedding row is
- * NaN, and with it the sample's logits.  logits [batch, num_labels] (may be NULL). */
+ * token_type_ids may be NULL (every token in segment 0, as BERT.py:69-75 defaults it); position ids as the family
+ * computes them (above).  An id outside [0, vocab_size), a token type outside [0, type_vocab) or a position id outside
+ * [0, max_position) never indexes its table: that token's embedding row is NaN, and with it the sample's logits.
+ * logits [batch, num_labels] (may be NULL). */
 TE_API int te_bert_forward(const te_bert_config* cfg, const float* weights, const float* derived,
                     const long long* input_ids, const long long* attention_mask, const long long* token_type_ids,
                     int batch, int seq, unsigned flags, float* logits, void* workspace, long long workspace_bytes,

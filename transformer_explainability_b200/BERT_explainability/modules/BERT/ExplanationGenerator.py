@@ -4,7 +4,9 @@
 (``generate_LRP_last_layer``, ``generate_full_lrp``, ``generate_attn_last_layer``, ``generate_rollout``,
 ``generate_attn_gradcam``, reference ``:61-155``) are served from the same engine passes and the same kernels.
 Every generator accepts a batch of independent sequences of one length ([B,S] -> [B,S]); B = 1 is the reference call.
-Every generator also takes ``token_type_ids`` (the segments of sentence pairs, [B,S]); None puts every token in segment 0."""
+Every generator also takes ``token_type_ids`` (the segments of sentence pairs, [B,S]); None puts every token in segment 0.
+``model`` is any of the engine's encoder classifiers (BERT, RoBERTa / XLM-RoBERTa, DistilBERT): the generators read its
+layers through ``model.attention_views()``."""
 import torch
 
 from transformer_explainability_b200 import _lib, ops
@@ -31,7 +33,7 @@ class Generator:
 
     # ---- comparison generators (reference :61-155) ---------------------------------------------------------------
     def _last(self):
-        return self.model.bert.encoder.layer[-1].attention.self
+        return self.model.attention_views()[-1]
 
     def _forward(self, input_ids, attention_mask, token_type_ids):
         # without token types this stays the engine's two-argument call, which callers may wrap (e.g. to record shapes)
@@ -71,7 +73,7 @@ class Generator:
     def generate_rollout(self, input_ids, attention_mask, start_layer=0, index=None, token_type_ids=None):
         """``:115-127``: rollout of the head-averaged raw attention, row 0, [0] = 0."""
         self._forward(input_ids, attention_mask, token_type_ids)
-        mats = [ops.head_reduce(l.attention.self.get_attn(), mode="mean") for l in self.model.bert.encoder.layer]
+        mats = [ops.head_reduce(v.get_attn(), mode="mean") for v in self.model.attention_views()]
         rollout = compute_rollout_attention(mats, start_layer=start_layer)
         rollout[:, 0, 0] = 0
         return rollout[:, 0]

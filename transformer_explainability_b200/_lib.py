@@ -24,8 +24,12 @@ class TeBertConfig(ctypes.Structure):
     """``te_bert_config`` of include/te_b200.h."""
     _fields_ = [("vocab_size", c_int), ("max_position", c_int), ("type_vocab", c_int), ("hidden", c_int),
                 ("layers", c_int), ("heads", c_int), ("intermediate", c_int), ("num_labels", c_int),
-                ("layer_norm_eps", c_float)]
+                ("layer_norm_eps", c_float), ("arch", c_int), ("pad_token_id", c_int)]
 
+
+BERT_ARCH_BERT = 0              # TE_BERT_ARCH_BERT
+BERT_ARCH_ROBERTA = 1           # TE_BERT_ARCH_ROBERTA (also XLM-RoBERTa)
+BERT_ARCH_DISTILBERT = 2        # TE_BERT_ARCH_DISTILBERT
 
 FLAG_ZPLUS_TENSOR_CORES = 1
 FLAG_ROLLOUT_FUSED = 2

@@ -1,5 +1,9 @@
 // BERT (post-LN encoder + pooler + classifier) transformer-attribution engine.
 //
+// The same engine runs the RoBERTa / XLM-RoBERTa and DistilBERT sequence classifiers (te_bert_config.arch): their
+// encoder layer is this one, only the embedding (position ids, token-type table, order of the sum) and the head
+// (classifier.dense / out_proj, or pre_classifier -> ReLU -> classifier) differ, see include/te_b200.h.
+//
 // Reference wiring: BERT_explainability/modules/BERT/BERT.py (BertEmbeddings :61-85, BertSelfAttention :307-409,
 // BertSelfOutput :420-434, BertIntermediate :446-456, BertOutput :467-487, BertLayer :498-530, BertPooler :169-190,
 // BertModel.relprop :645-651), BertForSequenceClassification.py:23-88, ExplanationGenerator.py:7-59.
@@ -26,22 +30,43 @@ namespace {
 constexpr int kMaxDepth = 64;
 
 struct Dims {
-    int B, N, NP, D, H, dh, F, C, L, V, P, T;
+    int B, N, NP, D, H, dh, F, C, L, V, P, T, arch, pad;
     long long M;
     float eps;
 };
 
 static bool make_dims(const te_bert_config* c, int B, int S, Dims& d) {
     if (!c || c->layers <= 0 || c->layers > kMaxDepth || c->heads <= 0 || c->hidden % c->heads != 0 || c->hidden % 8 != 0 ||
-        c->intermediate % 4 != 0 || c->num_labels <= 0 || c->vocab_size <= 0 || c->max_position <= 0 ||
-        c->type_vocab <= 0) {
+        c->intermediate % 4 != 0 || c->num_labels <= 0 || c->vocab_size <= 0 || c->max_position <= 0) {
         te_set_last_error("te_bert: invalid config");
         return false;
     }
-    if (S <= 0 || S > c->max_position) { te_set_last_error("te_bert: sequence length out of range"); return false; }
+    if (c->arch != TE_BERT_ARCH_BERT && c->arch != TE_BERT_ARCH_ROBERTA && c->arch != TE_BERT_ARCH_DISTILBERT) {
+        te_set_last_error("te_bert: unknown arch (TE_BERT_ARCH_BERT, _ROBERTA or _DISTILBERT)");
+        return false;
+    }
+    if (c->arch == TE_BERT_ARCH_DISTILBERT ? c->type_vocab != 0 : c->type_vocab <= 0) {
+        te_set_last_error(c->arch == TE_BERT_ARCH_DISTILBERT ? "te_bert: DistilBERT has no token-type table (type_vocab must be 0)"
+                                                             : "te_bert: invalid config (type_vocab must be positive)");
+        return false;
+    }
+    if (c->arch == TE_BERT_ARCH_ROBERTA && (c->pad_token_id < 0 || c->pad_token_id >= c->vocab_size)) {
+        te_set_last_error("te_bert: RoBERTa pad_token_id outside [0, vocab_size)");
+        return false;
+    }
+    // RoBERTa positions run pad + 1 .. pad + S: the table needs S + pad + 1 rows
+    const long long max_seq = c->arch == TE_BERT_ARCH_ROBERTA ? (long long)c->max_position - c->pad_token_id - 1
+                                                              : c->max_position;
+    if (S <= 0 || S > max_seq) {
+        te_set_last_error(c->arch == TE_BERT_ARCH_ROBERTA
+                              ? "te_bert: sequence length out of range (RoBERTa: seq + pad_token_id + 1 <= max_position)"
+                              : "te_bert: sequence length out of range");
+        return false;
+    }
     d.B = B; d.N = S; d.NP = (S + 3) & ~3; d.D = c->hidden; d.H = c->heads; d.dh = c->hidden / c->heads;
     d.F = c->intermediate; d.C = c->num_labels; d.L = c->layers; d.V = c->vocab_size; d.P = c->max_position;
     d.T = c->type_vocab; d.M = (long long)B * S; d.eps = c->layer_norm_eps;
+    d.arch = c->arch; d.pad = c->pad_token_id;
     if (d.dh % 4 != 0) { te_set_last_error("te_bert: head_dim % 4 != 0"); return false; }
     return true;
 }
@@ -56,36 +81,50 @@ static WTable weight_table(const te_bert_config* c) {
         t.push_back({n, numel, off});
         off += pad ? ((numel + 31) & ~31LL) : numel;
     };
-    const std::string E = "bert.embeddings.";
+    // per family: the state_dict prefix, the layer's module names (in the order bind_weights reads them), the head
+    const bool distil = d.arch == TE_BERT_ARCH_DISTILBERT;
+    const std::string M = distil ? "distilbert." : d.arch == TE_BERT_ARCH_ROBERTA ? "roberta." : "bert.";
+    // q, k, v, attention output dense, its LayerNorm, intermediate dense, output dense, its LayerNorm
+    static const char* const kBertLayer[8] = {"attention.self.query", "attention.self.key", "attention.self.value",
+                                              "attention.output.dense", "attention.output.LayerNorm",
+                                              "intermediate.dense", "output.dense", "output.LayerNorm"};
+    static const char* const kDistilLayer[8] = {"attention.q_lin", "attention.k_lin", "attention.v_lin",
+                                                "attention.out_lin", "sa_layer_norm", "ffn.lin1", "ffn.lin2",
+                                                "output_layer_norm"};
+    const char* const* n = distil ? kDistilLayer : kBertLayer;
+    const std::string E = M + "embeddings.";
     add(E + "word_embeddings.weight", (long long)d.V * d.D);
     add(E + "position_embeddings.weight", (long long)d.P * d.D);
-    add(E + "token_type_embeddings.weight", (long long)d.T * d.D);
+    if (!distil) add(E + "token_type_embeddings.weight", (long long)d.T * d.D);
     add(E + "LayerNorm.weight", d.D);
     add(E + "LayerNorm.bias", d.D);
     for (int i = 0; i < d.L; ++i) {
-        const std::string L = "bert.encoder.layer." + std::to_string(i) + ".";
+        const std::string L = M + (distil ? "transformer.layer." : "encoder.layer.") + std::to_string(i) + ".";
         // query | key | value stored back to back (no padding): one packed [3D, D] weight, [3D] bias
-        add(L + "attention.self.query.weight", (long long)d.D * d.D, false);
-        add(L + "attention.self.key.weight", (long long)d.D * d.D, false);
-        add(L + "attention.self.value.weight", (long long)d.D * d.D, true);
-        add(L + "attention.self.query.bias", d.D, false);
-        add(L + "attention.self.key.bias", d.D, false);
-        add(L + "attention.self.value.bias", d.D, true);
-        add(L + "attention.output.dense.weight", (long long)d.D * d.D);
-        add(L + "attention.output.dense.bias", d.D);
-        add(L + "attention.output.LayerNorm.weight", d.D);
-        add(L + "attention.output.LayerNorm.bias", d.D);
-        add(L + "intermediate.dense.weight", (long long)d.F * d.D);
-        add(L + "intermediate.dense.bias", d.F);
-        add(L + "output.dense.weight", (long long)d.D * d.F);
-        add(L + "output.dense.bias", d.D);
-        add(L + "output.LayerNorm.weight", d.D);
-        add(L + "output.LayerNorm.bias", d.D);
+        add(L + n[0] + ".weight", (long long)d.D * d.D, false);
+        add(L + n[1] + ".weight", (long long)d.D * d.D, false);
+        add(L + n[2] + ".weight", (long long)d.D * d.D, true);
+        add(L + n[0] + ".bias", d.D, false);
+        add(L + n[1] + ".bias", d.D, false);
+        add(L + n[2] + ".bias", d.D, true);
+        add(L + n[3] + ".weight", (long long)d.D * d.D);
+        add(L + n[3] + ".bias", d.D);
+        add(L + n[4] + ".weight", d.D);
+        add(L + n[4] + ".bias", d.D);
+        add(L + n[5] + ".weight", (long long)d.F * d.D);
+        add(L + n[5] + ".bias", d.F);
+        add(L + n[6] + ".weight", (long long)d.D * d.F);
+        add(L + n[6] + ".bias", d.D);
+        add(L + n[7] + ".weight", d.D);
+        add(L + n[7] + ".bias", d.D);
     }
-    add("bert.pooler.dense.weight", (long long)d.D * d.D);
-    add("bert.pooler.dense.bias", d.D);
-    add("classifier.weight", (long long)d.C * d.D);
-    add("classifier.bias", d.C);
+    // head: dense [D, D] -> tanh / ReLU -> out [C, D]
+    const std::string hd = distil ? "pre_classifier." : d.arch == TE_BERT_ARCH_ROBERTA ? "classifier.dense." : "bert.pooler.dense.";
+    const std::string ho = d.arch == TE_BERT_ARCH_ROBERTA ? "classifier.out_proj." : "classifier.";
+    add(hd + "weight", (long long)d.D * d.D);
+    add(hd + "bias", d.D);
+    add(ho + "weight", (long long)d.C * d.D);
+    add(ho + "bias", d.C);
     t.push_back({"", 0, off});
     return t;
 }
@@ -102,7 +141,9 @@ static void bind_weights(const te_bert_config* c, const float* base, Weights& w)
     const WTable t = weight_table(c);
     size_t i = 0;
     auto next = [&]() { return base + t[i++].offset; };
-    w.word = next(); w.pos = next(); w.type = next(); w.elnw = next(); w.elnb = next();
+    w.word = next(); w.pos = next();
+    w.type = c->arch == TE_BERT_ARCH_DISTILBERT ? nullptr : next();
+    w.elnw = next(); w.elnb = next();
     for (int l = 0; l < c->layers; ++l) {
         LayerW& y = w.layer[l];
         y.qkvw = next(); next(); next();
@@ -235,6 +276,10 @@ extern "C" int te_bert_forward(const te_bert_config* cfg, const float* weights, 
     Dims d; Workspace ws;
     TE_TRY(check_ws(cfg, batch, seq, workspace, workspace_bytes, d, ws));
     if (!weights || !input_ids || !attention_mask) { te_set_last_error("te_bert_forward: null pointer"); return TE_ERR_ARG; }
+    if (token_type_ids && d.arch == TE_BERT_ARCH_DISTILBERT) {
+        te_set_last_error("te_bert_forward: DistilBERT takes no token_type_ids (it has no token-type table)");
+        return TE_ERR_ARG;
+    }
     Select sel;
     TE_TRY(decode_flags(sel, "te_bert_forward", flags, derived, 0, false));
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
@@ -250,7 +295,11 @@ extern "C" int te_bert_forward(const te_bert_config* cfg, const float* weights, 
     bind_weights(cfg, weights, w);
     const float scale = 1.0f / sqrtf((float)d.dh);
 
-    TE_TRY(te_launch_bert_embed(input_ids, token_type_ids, w.word, w.pos, w.type, ws.tD[0], d.B, d.N, d.D, d.V, d.T, st));
+    if (d.arch == TE_BERT_ARCH_BERT)
+        TE_TRY(te_launch_bert_embed(input_ids, token_type_ids, w.word, w.pos, w.type, ws.tD[0], d.B, d.N, d.D, d.V, d.T, st));
+    else      // RoBERTa: position ids counted from pad on the device; DistilBERT: arange, no token-type table
+        TE_TRY(te_launch_hf_embed(input_ids, token_type_ids, w.word, w.pos, w.type, ws.tD[0], d.B, d.N, d.D, d.V, d.P, d.T,
+                                  d.arch == TE_BERT_ARCH_ROBERTA ? d.pad : -1, st));
     TE_TRY(layernorm(ws.tD[0], w.elnw, w.elnb, ws.layer[0].h, nullptr, nullptr));
     TE_TRY(te_launch_bert_mask(attention_mask, ws.maskadd, (long long)d.B * d.N, st));
 
@@ -276,9 +325,10 @@ extern "C" int te_bert_forward(const te_bert_config* cfg, const float* weights, 
         TE_TRY(linear_fwd_tc(tw.w2, a.g, d.F, lw.w2, lw.b2, a.d2, a.s2, a.ao, d.M, d.F, d.D, TE_EPI_BIAS_ADD, st, &f16.fc2));
         TE_TRY(layernorm(a.s2, lw.ln2w, lw.ln2b, h_next, a.mean2, a.rstd2));
     }
-    // pooler (first token -> dense -> tanh), classifier
+    // pooler (first token -> dense -> tanh; DistilBERT's pre_classifier -> ReLU), classifier
     TE_TRY(linear_fwd(ws.h_last, d.N * d.D, w.poolw, w.poolb, ws.pd, nullptr, nullptr, d.B, d.D, d.D, TE_EPI_BIAS, st));
-    TE_TRY(te_launch_tanh(ws.pd, ws.pooled, (long long)d.B * d.D, st));
+    if (d.arch == TE_BERT_ARCH_DISTILBERT) TE_TRY(te_launch_relu(ws.pd, ws.pooled, (long long)d.B * d.D, st));
+    else TE_TRY(te_launch_tanh(ws.pd, ws.pooled, (long long)d.B * d.D, st));
     TE_TRY(linear_fwd(ws.pooled, d.D, w.clsw, w.clsb, ws.logits, nullptr, nullptr, d.B, d.D, d.C, TE_EPI_BIAS, st));
     if (logits && cudaMemcpyAsync(logits, ws.logits, sizeof(float) * d.B * d.C, cudaMemcpyDeviceToDevice, st) != cudaSuccess) {
         te_set_last_error("te_bert_forward: logits copy failed");
@@ -317,7 +367,10 @@ extern "C" int te_bert_attribute(const te_bert_config* cfg, const float* weights
     float* dxa = ws.tD[0]; float* dsx = ws.tD[1]; float* dctx = ws.tD[2]; float* dxn = ws.tD[3];
     float* dF = ws.tF[0]; float* dqkv = ws.t3D[0]; float* dS = ws.tA[0];
     TE_TRY(linear_bwd(ws.seed, w.clsw, ws.dpool, nullptr, d.B, d.D, d.C, TE_EPI_STORE, st));         // classifier
-    TE_TRY(te_launch_tanh_bwd(ws.dpool, ws.pooled, ws.dpd, (long long)d.B * d.D, st));               // pooler tanh
+    if (d.arch == TE_BERT_ARCH_DISTILBERT)
+        TE_TRY(te_launch_relu_bwd(ws.dpool, ws.pooled, ws.dpd, (long long)d.B * d.D, st));           // head ReLU
+    else
+        TE_TRY(te_launch_tanh_bwd(ws.dpool, ws.pooled, ws.dpd, (long long)d.B * d.D, st));           // pooler tanh
     TE_TRY(linear_bwd(ws.dpd, w.poolw, ws.dfirst, nullptr, d.B, d.D, d.D, TE_EPI_STORE, st));        // pooler dense
     TE_TRY(te_launch_fill(dxa, 0.f, MD, st));
     if (cudaMemcpy2DAsync(dxa, sizeof(float) * d.N * d.D, ws.dfirst, sizeof(float) * d.D, sizeof(float) * d.D, d.B,

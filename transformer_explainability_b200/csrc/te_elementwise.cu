@@ -659,6 +659,60 @@ __global__ void bert_embed_kernel(const long long* __restrict__ ids, const long 
             make_float4((ty.x + p.x) + w.x, (ty.y + p.y) + w.y, (ty.z + p.z) + w.z, (ty.w + p.w) + w.w);
     }
 }
+// RoBERTa / DistilBERT embeddings (transformers RobertaEmbeddings / distilbert Embeddings .forward).  Block (tile, b)
+// writes tokens [32 tile, 32 tile + 32) of row b.  pad >= 0 (RoBERTa, create_position_ids_from_input_ids): a token's
+// position is pad + (number of ids != pad up to and including it), or pad for a pad token; the count before the tile
+// is one block-wide count of the row's earlier ids, the count inside it one warp ballot.  pad < 0: position = token
+// index.  type != NULL: (word + type) + position (RoBERTa); type == NULL: word + position (DistilBERT).
+constexpr int kEmbedTile = 32;
+__global__ void __launch_bounds__(256) hf_embed_kernel(const long long* __restrict__ ids, const long long* __restrict__ tt,
+                                                       const float* __restrict__ word, const float* __restrict__ pos,
+                                                       const float* __restrict__ type, float* __restrict__ out, int S, int D,
+                                                       int vocab, int max_position, int type_vocab, int pad) {
+    __shared__ int spos[kEmbedTile];
+    const int b = blockIdx.y, s0 = blockIdx.x * kEmbedTile;
+    const long long* row = ids + (long long)b * S;
+    int before = 0;
+    if (pad >= 0)
+        for (int base = 0; base < s0; base += blockDim.x) {        // block-uniform trip count
+            const int s = base + (int)threadIdx.x;
+            before += __syncthreads_count(s < s0 && row[s] != pad);
+        }
+    if (threadIdx.x < kEmbedTile) {
+        const int lane = threadIdx.x, s = s0 + lane;
+        if (pad >= 0) {
+            const bool counted = s < S && row[s] != pad;
+            const unsigned upto = __ballot_sync(0xffffffffu, counted) & (0xffffffffu >> (31 - lane));
+            spos[lane] = counted ? pad + before + __popc(upto) : pad;
+        } else {
+            spos[lane] = s;
+        }
+    }
+    __syncthreads();
+    const int d4 = D / 4, n = min(kEmbedTile, S - s0);
+    for (int t = threadIdx.x; t < n * d4; t += blockDim.x) {
+        const int j = t / d4, q = t - j * d4;
+        const long long rt = (long long)b * S + s0 + j;
+        const long long id = ids[rt];
+        const long long ty_id = tt ? tt[rt] : 0;
+        const int p = spos[j];
+        float4* o = reinterpret_cast<float4*>(out + rt * D) + q;
+        // never index a table out of bounds: the row becomes NaN (loud, memory-safe)
+        if (id < 0 || id >= vocab || p < 0 || p >= max_position || (type && (ty_id < 0 || ty_id >= type_vocab))) {
+            const float qn = __int_as_float(0x7fc00000);
+            *o = make_float4(qn, qn, qn, qn);
+            continue;
+        }
+        const float4 w = reinterpret_cast<const float4*>(word + id * D)[q];
+        const float4 ps = reinterpret_cast<const float4*>(pos + (long long)p * D)[q];
+        if (type) {
+            const float4 ty = reinterpret_cast<const float4*>(type + ty_id * D)[q];
+            *o = make_float4((w.x + ty.x) + ps.x, (w.y + ty.y) + ps.y, (w.z + ty.z) + ps.z, (w.w + ty.w) + ps.w);
+        } else {
+            *o = make_float4(w.x + ps.x, w.y + ps.y, w.z + ps.z, w.w + ps.w);
+        }
+    }
+}
 // transformers 3.5.1 get_extended_attention_mask: (1 - mask) * -10000   (call site BERT.py:598)
 __global__ void bert_mask_kernel(const long long* __restrict__ mask, float* __restrict__ out, long long n) {
     for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < n; t += (long long)gridDim.x * blockDim.x)
@@ -672,6 +726,17 @@ __global__ void tanh_bwd_kernel(const float* __restrict__ dy, const float* __res
                                 long long n) {
     for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < n; t += (long long)gridDim.x * blockDim.x)
         dx[t] = dy[t] * (1.0f - y[t] * y[t]);
+}
+__global__ void relu_kernel(const float* __restrict__ x, float* __restrict__ y, long long n) {
+    for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < n; t += (long long)gridDim.x * blockDim.x) {
+        const float v = x[t];
+        y[t] = (v > 0.f || v != v) ? v : 0.f;             // torch.relu: NaN stays NaN
+    }
+}
+__global__ void relu_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ y, float* __restrict__ dx,
+                                long long n) {
+    for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < n; t += (long long)gridDim.x * blockDim.x)
+        dx[t] = y[t] > 0.f ? dy[t] : 0.f;
 }
 __global__ void add2_kernel(const float* a, const float* b, float* out, long long n4) {
     for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < n4;
@@ -945,6 +1010,16 @@ int te_launch_bert_embed(const long long* ids, const long long* token_type_ids, 
     TE_CUDA_CHECK_LAUNCH();
     return TE_OK;
 }
+int te_launch_hf_embed(const long long* ids, const long long* token_type_ids, const float* word, const float* pos,
+                       const float* type, float* out, int B, int S, int D, int vocab, int max_position, int type_vocab,
+                       int pad, cudaStream_t st) {
+    TE_REQ(D % 4 == 0, "hf_embed: D % 4 != 0");
+    TE_REQ(B >= 1 && B <= 65535 && S >= 1, "hf_embed: batch outside 1..65535 or empty sequence");
+    hf_embed_kernel<<<dim3((S + kEmbedTile - 1) / kEmbedTile, B), 256, 0, st>>>(ids, token_type_ids, word, pos, type, out, S,
+                                                                               D, vocab, max_position, type_vocab, pad);
+    TE_CUDA_CHECK_LAUNCH();
+    return TE_OK;
+}
 int te_launch_bert_mask(const long long* mask, float* out, long long n, cudaStream_t st) {
     bert_mask_kernel<<<flat_grid(n), kThreads, 0, st>>>(mask, out, n);
     TE_CUDA_CHECK_LAUNCH();
@@ -957,6 +1032,16 @@ int te_launch_tanh(const float* x, float* y, long long n, cudaStream_t st) {
 }
 int te_launch_tanh_bwd(const float* dy, const float* y, float* dx, long long n, cudaStream_t st) {
     tanh_bwd_kernel<<<flat_grid(n), kThreads, 0, st>>>(dy, y, dx, n);
+    TE_CUDA_CHECK_LAUNCH();
+    return TE_OK;
+}
+int te_launch_relu(const float* x, float* y, long long n, cudaStream_t st) {
+    relu_kernel<<<flat_grid(n), kThreads, 0, st>>>(x, y, n);
+    TE_CUDA_CHECK_LAUNCH();
+    return TE_OK;
+}
+int te_launch_relu_bwd(const float* dy, const float* y, float* dx, long long n, cudaStream_t st) {
+    relu_bwd_kernel<<<flat_grid(n), kThreads, 0, st>>>(dy, y, dx, n);
     TE_CUDA_CHECK_LAUNCH();
     return TE_OK;
 }

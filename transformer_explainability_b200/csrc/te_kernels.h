@@ -79,9 +79,18 @@ int te_launch_softmax_masked(float* s, long long rows, int N, int ld, const floa
 // token_type_ids == NULL: every token is segment 0.
 int te_launch_bert_embed(const long long* ids, const long long* token_type_ids, const float* word, const float* pos,
                          const float* type, float* out, int B, int S, int D, int vocab, int type_vocab, cudaStream_t st);
+// RoBERTa / DistilBERT embeddings, one launch.  pad >= 0: RoBERTa position ids (pad + running count of ids != pad for
+// non-pad tokens, pad for pad tokens) and (word + type) + position; pad < 0: arange and, with type == NULL (DistilBERT),
+// word + position.  token_type_ids == NULL: segment 0.  An id, token type or position outside its table gives a NaN row.
+int te_launch_hf_embed(const long long* ids, const long long* token_type_ids, const float* word, const float* pos,
+                       const float* type, float* out, int B, int S, int D, int vocab, int max_position, int type_vocab,
+                       int pad, cudaStream_t st);
 int te_launch_bert_mask(const long long* mask, float* out, long long n, cudaStream_t st);
 int te_launch_tanh(const float* x, float* y, long long n, cudaStream_t st);
 int te_launch_tanh_bwd(const float* dy, const float* y, float* dx, long long n, cudaStream_t st);
+// DistilBERT's head activation: y = relu(x) (NaN stays NaN, as torch.relu); dx = dy where y > 0, else 0
+int te_launch_relu(const float* x, float* y, long long n, cudaStream_t st);
+int te_launch_relu_bwd(const float* dy, const float* y, float* dx, long long n, cudaStream_t st);
 int te_launch_add2(const float* a, const float* b, float* out, long long n, cudaStream_t st);
 // Add.relprop for add([scores, key-broadcast mask]); only the scores' relevance is produced.
 // partial == NULL selects the layers_lrp variant: r1 = x1 * sd(r, x1 + mask), no ratio normalisation.

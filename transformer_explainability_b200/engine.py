@@ -337,10 +337,12 @@ class ViTEngine(_Engine):
 
 def bert_config(vocab_size=30522, max_position_embeddings=512, type_vocab_size=2, hidden_size=768,
                 num_hidden_layers=12, num_attention_heads=12, intermediate_size=3072, num_labels=2,
-                layer_norm_eps=1e-12):
+                layer_norm_eps=1e-12, arch=0, pad_token_id=0):
+    """``te_bert_config``.  arch: ``_lib.BERT_ARCH_BERT`` / ``_ROBERTA`` / ``_DISTILBERT`` (type_vocab_size 0);
+    pad_token_id: the id RoBERTa's position ids count from."""
     from ._lib import TeBertConfig
     return TeBertConfig(vocab_size, max_position_embeddings, type_vocab_size, hidden_size, num_hidden_layers,
-                        num_attention_heads, intermediate_size, num_labels, layer_norm_eps)
+                        num_attention_heads, intermediate_size, num_labels, layer_norm_eps, arch, pad_token_id)
 
 
 class BertEngine(_Engine):
@@ -375,6 +377,8 @@ class BertEngine(_Engine):
         (the kernel reads no table row but row 0)."""
         if token_type_ids is None:
             return None
+        if self.cfg.arch == _lib.BERT_ARCH_DISTILBERT:
+            raise ValueError("DistilBERT takes no token_type_ids: it has no token-type table")
         tt = torch.as_tensor(token_type_ids)
         if tuple(tt.shape) != tuple(shape):
             raise ValueError("token_type_ids must have the shape of input_ids %s, got %s" % (tuple(shape), tuple(tt.shape)))

@@ -7,8 +7,9 @@ pairs.
     python -m transformer_explainability_b200.text_visualization --model-dir mnli/ --text "A man plays." \\
         --text-pair "Somebody is playing." --output-dir out/
 
-``--model-dir`` is a local Hugging Face directory (``config.json``, ``vocab.txt``, ``model.safetensors`` or
-``pytorch_model.bin``), the layout ``from_pretrained`` leaves on disk; nothing is downloaded.  The notebook explains a
+``--model-dir`` is a local Hugging Face directory (``config.json``, the tokenizer's files, ``model.safetensors`` or
+``pytorch_model.bin``), the layout ``from_pretrained`` leaves on disk; nothing is downloaded.  ``config.json``'s
+``model_type`` picks the classifier: ``bert``, ``roberta``, ``xlm-roberta`` or ``distilbert`` (``MODEL_TYPES``).  The notebook explains a
 sentence with ``generate_LRP(start_layer=0)``, min-max normalises the map, negates it when the explained class is named
 ``NEGATIVE``, and shows captum's ``visualize_text`` table with the probability of the class.  Here, per batch of
 ``--batch-size`` sentences, tokenised as the notebook tokenises them (a pair with its ``token_type_ids``) and padded to the
@@ -86,18 +87,36 @@ def render_html(records):
 
 
 # ---- model and tokenizer -------------------------------------------------------------------------------------------------
+# config.json model_type -> (transformers config class, the engine's classifier: module, class)
+_M = "transformer_explainability_b200.BERT_explainability.modules.BERT."
+MODEL_TYPES = {
+    "bert": ("BertConfig", _M + "BertForSequenceClassification", "BertForSequenceClassification"),
+    "roberta": ("RobertaConfig", _M + "RobertaForSequenceClassification", "RobertaForSequenceClassification"),
+    "xlm-roberta": ("XLMRobertaConfig", _M + "RobertaForSequenceClassification", "XLMRobertaForSequenceClassification"),
+    "distilbert": ("DistilBertConfig", _M + "DistilBertForSequenceClassification",
+                   "DistilBertForSequenceClassification"),
+}
+
+
 def load_model(model_dir, device="cuda"):
-    """The engine's ``BertForSequenceClassification`` with the weights of a local Hugging Face directory."""
-    from transformers import BertConfig
-    from .BERT_explainability.modules.BERT.BertForSequenceClassification import BertForSequenceClassification
-    config = BertConfig.from_json_file(os.path.join(model_dir, "config.json"))
+    """The engine's classifier for ``config.json``'s ``model_type`` (``MODEL_TYPES``) with the weights of a local Hugging
+    Face directory."""
+    import importlib
+    import transformers
+    with open(os.path.join(model_dir, "config.json")) as f:
+        model_type = json.load(f).get("model_type", "bert")
+    if model_type not in MODEL_TYPES:
+        raise ValueError("%s: model_type %r is not supported; the supported types are %s"
+                         % (model_dir, model_type, ", ".join(sorted(MODEL_TYPES))))
+    config_cls, module, cls = MODEL_TYPES[model_type]
+    config = getattr(transformers, config_cls).from_json_file(os.path.join(model_dir, "config.json"))
     st = os.path.join(model_dir, "model.safetensors")
     if os.path.exists(st):
         from safetensors.torch import load_file
         sd = load_file(st)
     else:
         sd = torch.load(os.path.join(model_dir, "pytorch_model.bin"), map_location="cpu", weights_only=True)
-    model = BertForSequenceClassification(config)
+    model = getattr(importlib.import_module(module), cls)(config)
     res = model.load_state_dict(sd, strict=False)
     missing = [k for k in res.missing_keys if "position_ids" not in k]
     if missing:
@@ -139,8 +158,10 @@ def explain_batch(model, ids, tt, mask, names, class_index=None, start_layer=0, 
     dev = eng.device
     flags = eng.flags | (_lib.FLAG_ATTN_GRAD_ROLLOUT if method == "attn_grad_rollout" else 0)
     B, S = ids.shape
+    # segment ids reach the engine only for a model with a token-type table (DistilBERT has none)
+    tt_dev = tt.to(dev) if eng.cfg.type_vocab > 0 else None
     maps, idx, logits = eng.explain(ids.to(dev), mask.to(dev), index=class_index, start_layer=start_layer, flags=flags,
-                                    return_logits=True, token_type_ids=tt.to(dev))
+                                    return_logits=True, token_type_ids=tt_dev)
     C = logits.shape[1]
     lengths = mask.sum(dim=1).to(torch.int32)
     neg = torch.tensor([-1.0 if n == "NEGATIVE" else 1.0 for n in names], dtype=torch.float32, device=dev)
@@ -188,16 +209,18 @@ def run(model, tokenizer, texts, pairs=None, names=None, class_index=None, start
     for s in range(0, len(texts), batch_size):
         tx = texts[s:s + batch_size]
         px = pairs[s:s + batch_size] if pairs is not None else None
-        ids, tt, mask = tokenize(tokenizer, tx, px, model.config.max_position_embeddings)
+        ids, tt, mask = tokenize(tokenizer, tx, px, model.max_length())
         scores, probs, explained, predicted = explain_batch(model, ids, tt, mask, names, class_index, start_layer, method)
         records += records_for(tokenizer, tx, px, ids, tt, mask, scores, probs, explained, predicted, names)
     return records, write_outputs(records, output_dir)
 
 
 def build_parser():
-    p = argparse.ArgumentParser(description="The BERT notebook's word-importance view for sentences and sentence pairs")
+    p = argparse.ArgumentParser(description="The BERT notebook's word-importance view for sentences and sentence pairs, "
+                                            "for BERT, RoBERTa, XLM-RoBERTa and DistilBERT classifiers")
     p.add_argument("--model-dir", required=True,
-                   help="local Hugging Face directory: config.json, vocab.txt, model.safetensors or pytorch_model.bin")
+                   help="local Hugging Face directory: config.json (model_type %s), the tokenizer's files, "
+                        "model.safetensors or pytorch_model.bin" % " / ".join(MODEL_TYPES))
     p.add_argument("--text", action="append", required=True, help="a sentence (repeat for more)")
     p.add_argument("--text-pair", action="append", default=None,
                    help="the second sentence of the pair, one per --text (repeat in the same order)")
