@@ -57,12 +57,14 @@ import math
 import os
 import warnings
 from dataclasses import dataclass
+from types import SimpleNamespace
 from typing import FrozenSet, Optional, Tuple, Union
 
 import numpy as np
 import torch
 
-from . import _lib
+from . import _lib, ops
+from ._host import to_host
 
 KS = tuple(range(5, 85, 5))
 AOPC_THRESHOLDS = (0.01, 0.05, 0.1, 0.2, 0.5)              # metrics.py --aopc_thresholds
@@ -545,7 +547,6 @@ def generate(text_list, attention_list, latex_file, color="red"):
     """``generate()`` (``bert_pipeline.py:49-84``) with its signature: the weights of the first ``len(text_list)`` entries
     of the CUDA tensor ``attention_list`` come from one ``te_eraser_latex_weights`` launch (no clamp: the pipeline
     clamps before it calls), and ``latex_file`` receives ``latex_document``'s text."""
-    from . import ops
     if not (torch.is_tensor(attention_list) and attention_list.is_cuda):
         raise ValueError("generate: attention_list must be a CUDA tensor (the weights are computed on the GPU)")
     n = len(text_list)
@@ -638,24 +639,38 @@ def comparison_figures(annotations, evidence_classes, pred, output_dir):
     return out
 
 
+def _batch(idx, docids, encodings, pad_id, device, ranges=None, spans=None):
+    """The padded batch of the documents of annotations ``idx`` (length-sorted by the caller): ``ids`` / ``mask``
+    int64 [B, S] on ``device``, the token lengths ``lens``, and with ``ranges`` {docid: word ranges} and ``spans``
+    {(docid, docid): truth spans} the documents' word ranges and truth spans, flattened with their offsets
+    (``ranges[woff[b]:woff[b + 1]]``, ``spans[soff[b]:soff[b + 1]]``)."""
+    lens = [len(encodings[docids[i]][0]) for i in idx]
+    ids = torch.full((len(idx), max(lens)), pad_id, dtype=torch.long)
+    mask = torch.zeros((len(idx), max(lens)), dtype=torch.long)
+    wr, woff, sp, soff = [], [0], [], [0]
+    for r, i in enumerate(idx):
+        ids[r, :lens[r]] = torch.as_tensor(encodings[docids[i]][0], dtype=torch.long)
+        mask[r, :lens[r]] = 1
+        if ranges is not None:
+            wr.extend(ranges[docids[i]])
+            woff.append(len(wr))
+            sp.extend(spans.get((docids[i], docids[i]), []))
+            soff.append(len(sp))
+    return SimpleNamespace(idx=idx, docids=[docids[i] for i in idx], ids=ids.to(device), mask=mask.to(device), lens=lens,
+                           S=max(lens), ranges=wr, woff=woff, spans=sp, soff=soff)
+
+
 def predictions(model, annotations, encodings, batch_size=8, pad_id=0):
     """The first-maximum argmax of the engine forward's logits for every annotation's document, in dataset order: one
     forward per length-sorted padded batch, no attribution."""
     eng = model.engine()
     device = next(model.parameters()).device
     docids = [annotation_docid(a) for a in annotations]
-    lens = np.array([len(encodings[d][0]) for d in docids], dtype=np.int64)
-    order = sorted(range(len(docids)), key=lambda i: -int(lens[i]))
+    order = sorted(range(len(docids)), key=lambda i: -len(encodings[docids[i]][0]))
     pred = np.zeros(len(docids), dtype=np.int64)
     for s0 in range(0, len(order), batch_size):
-        idx = order[s0:s0 + batch_size]
-        S = int(lens[idx[0]])
-        ids = torch.full((len(idx), S), pad_id, dtype=torch.long)
-        mask = torch.zeros((len(idx), S), dtype=torch.long)
-        for r, i in enumerate(idx):
-            ids[r, :lens[i]] = torch.as_tensor(encodings[docids[i]][0], dtype=torch.long)
-            mask[r, :lens[i]] = 1
-        pred[idx] = np.argmax(eng.forward(ids.to(device), mask.to(device)).cpu().numpy(), axis=1)
+        b = _batch(order[s0:s0 + batch_size], docids, encodings, pad_id, device)
+        pred[b.idx] = np.argmax(to_host(eng.forward(b.ids, b.mask))[0], axis=1)
     return pred
 
 
@@ -689,7 +704,6 @@ def _flip_search(eng, maps, ids, lens, ranges, woff, orders, pred0, n_words, fli
     the full word order ``orders[b]``), in length-sorted chunks, and ``te_logit_stats`` gives their argmax; one copy of
     the round's predictions finds each document's first flip.  Returns (tokens [B], flipped [B], rows, real tokens,
     padded tokens)."""
-    from . import ops
     B, device = len(lens), maps.device
     W = np.diff(np.asarray(woff))
     comp_len = []                                                  # comp_len[b][k - 1]: the row length at selection k
@@ -716,19 +730,17 @@ def _flip_search(eng, maps, ids, lens, ranges, woff, orders, pred0, n_words, fli
                 rlen[rows[-1]] = comp_len[b][k - 1]
         red = ops.eraser_reduce_inputs(maps, ids, lens, ranges, woff, nsel)
         flat = red["ids"].reshape(B * J * 2, -1)
-        pred = torch.empty(len(rows), dtype=torch.int32, device=device)
-        slot, s = {}, 0
+        preds, order = [], []
         for chunk, L, logits in _sorted_chunks(eng, flat, rlen, rows, cap, device):
-            pred[s:s + len(chunk)] = ops.logit_stats(logits, torch.zeros(len(chunk), dtype=torch.int32, device=device))[0]
-            slot.update((q, s + i) for i, q in enumerate(chunk))
-            s += len(chunk)
+            preds.append(ops.logit_stats(logits, torch.zeros(len(chunk), dtype=torch.int32, device=device))[0])
+            order += chunk
             real += int(rlen[chunk].sum())
             padded += len(chunk) * L
         n_rows += len(rows)
-        ph = pred.cpu().numpy()
+        ph = dict(zip(order, np.concatenate(to_host(*preds))))           # row -> its prediction
         for b in live:
             ks = range(nxt[b], min(nxt[b] + J, W[b] + 1))
-            hit = next((k for j, k in enumerate(ks) if ph[slot[(b * J + j) * 2]] != pred0[b]), None)
+            hit = next((k for j, k in enumerate(ks) if ph[(b * J + j) * 2] != pred0[b]), None)
             if hit is not None:
                 tokens[b], flipped[b] = hit, True
             else:
@@ -766,6 +778,156 @@ def _check_fraction(f, what):
 
 
 # ---- the evaluation ---------------------------------------------------------------------------------------------------------
+# One unit per optional evaluation: the constructor sets it up and checks its arguments; per batch ``device(b, res)`` (b:
+# ``_batch`` with its gold-class maps and targets, res: ``eraser_rationales``' tensors) returns named tensors for the
+# batch's one ``to_host`` copy, and ``host(b, h)`` reads their host arrays; ``result()`` is its entry of the result.
+class _Latex:
+    """The pipeline's LaTeX heat maps: the weights of the gold-class maps and, for ``LATEX_CF_GENERATORS``, of one more
+    generator call for the class 1 - target, with the logits of the batch's engine forward."""
+    def __init__(self, generator_method, gen_name, encodings, evidence_classes):
+        if len(evidence_classes) != 2:
+            raise ValueError("latex needs exactly two classes: the counterfactual class is 1 - target")
+        self.eng = _generator_model(generator_method).engine()
+        self.generator_method, self.cf = generator_method, gen_name in LATEX_CF_GENERATORS
+        self.encodings, self.docs = encodings, {}
+
+    def device(self, b, res):
+        out = {"latex_logits": latex_logits(self.eng, b.ids, b.mask), "latex_gt": ops.eraser_latex_weights(b.maps, b.lens)}
+        if self.cf:
+            cf = self.generator_method(input_ids=b.ids, attention_mask=b.mask,
+                                       index=torch.as_tensor([1 - t for t in b.targets], device=b.ids.device))
+            out["latex_cf"] = ops.eraser_latex_weights(cf.reshape(len(b.idx), b.S).to(torch.float32).contiguous(), b.lens)
+        return out
+
+    def host(self, b, h):
+        for r, (i, d) in enumerate(zip(b.idx, b.docids)):
+            t, L, pieces = b.targets[r], b.lens[r], self.encodings[d][1]
+            correct = int(np.argmax(h["latex_logits"][r])) == t
+            doc = {"GT": ("%d_GT_%s_%d.tex" % (i, _neg_pos(t), correct), latex_document(pieces, h["latex_gt"][r, :L]))}
+            if self.cf:
+                doc["CF"] = ("%d_CF.tex" % i, latex_document(pieces, h["latex_cf"][r, :L]))
+            self.docs[i] = doc
+
+    def result(self):
+        return dict(sorted(self.docs.items()))
+
+
+class _Soft:
+    """``metrics.py``'s soft-token scores of the word scores (one ``te_eraser_soft_scores`` call per batch)."""
+    def __init__(self, truth, annotations, docids, ranges, n_words):
+        self.annotations, self.docids, self.n_words = annotations, docids, n_words
+        self.truths = [soft_truth(truth, a, d, len(ranges[d]), nw) for a, d, nw in zip(annotations, docids, n_words)]
+        self.per_doc, self.single = np.zeros((len(docids), 3), dtype=np.float64), np.zeros(len(docids), dtype=bool)
+        self.words = [None] * len(docids)
+
+    def device(self, b, res):
+        sp, soff = [], [0]
+        for i in b.idx:
+            sp.extend(self.truths[i][0])
+            soff.append(len(sp))
+        soft = ops.eraser_soft_scores(res["word_scores"], b.woff, sp, soff, [self.truths[i][1] for i in b.idx])
+        return {"soft_scores": soft["scores"], "soft_flags": soft["flags"], "word_scores": res["word_scores"]}
+
+    def host(self, b, h):
+        self.per_doc[b.idx] = h["soft_scores"]
+        self.single[b.idx] = h["soft_flags"][:, 0] != 0
+        bad = [d for d, nan in zip(b.docids, h["soft_flags"][:, 1]) if nan]
+        if bad:
+            raise ValueError("document %r has a NaN word score; metrics.py's soft-token scores (sklearn) reject NaN"
+                             % bad[0])
+        for r, i in enumerate(b.idx):
+            self.words[i] = h["word_scores"][b.woff[r]:b.woff[r + 1]]
+
+    def result(self):
+        return {"per_document": self.per_doc, "single_class": self.single,
+                "lines": soft_lines(self.annotations, self.docids, self.words, self.n_words),
+                "scores": soft_token_scores(self.per_doc, self.single)}
+
+
+class _Faithfulness:
+    """``metrics.py``'s faithfulness and, with ``tokens_to_flip``, the tokens-to-flip search.  The probabilities of the
+    reduced rows collect in one device buffer, which comes back at the end; ``kfull``: the largest k of the word orders."""
+    def __init__(self, generator_method, annotations, docids, ranges, truth, n_words, evidence_classes, aopc_thresholds,
+                 k_fraction, faith_chunk, tokens_to_flip, flip_chunk, kmax, device):
+        fracs = [float(f) for f in aopc_thresholds]
+        for f in fracs:
+            _check_fraction(f, "an AOPC threshold")
+        if not fracs:
+            raise ValueError("faithfulness needs at least one AOPC threshold")
+        if k_fraction is None:
+            k_fraction = human_fraction(annotations, docids, [len(ranges[d]) for d in docids], truth)
+        _check_fraction(float(k_fraction), "k_fraction")
+        self.fracs = [float(k_fraction)] + fracs
+        n, J = len(docids), len(self.fracs)
+        self.nsel = np.array([[select_count(f, len(ranges[d])) for f in self.fracs] for d in docids],
+                             dtype=np.int64).reshape(n, J)
+        self.eng = _generator_model(generator_method).engine()
+        self.names = [c for c, _ in sorted(evidence_classes.items(), key=lambda kv: kv[1])]
+        C = self.eng.cfg.num_labels
+        self.buf = torch.empty(n * 2 * J, C, dtype=torch.float32, device=device)
+        self.logits, self.probs = np.zeros((n, C), dtype=np.float32), np.zeros((n, C), dtype=np.float32)
+        self.red_slot, self.slot, self.real_tok, self.padded_tok = np.zeros((n, J, 2), dtype=np.int64), 0, 0, 0
+        self.selected = [None] * n
+        self.kfull = max(kmax, int(self.nsel[:, 0].max()) if n else 0)
+        self.flip = tokens_to_flip
+        if tokens_to_flip:                                          # the search needs every document's full order
+            if C < 2:
+                raise ValueError("tokens_to_flip needs at least two classes")
+            self.kfull = max([self.kfull] + [len(ranges[d]) for d in docids])
+            self.flip_tok, self.flipped, self.flip_stats = np.zeros(n, dtype=np.int64), np.zeros(n, dtype=bool), [0, 0, 0]
+        self.annotations, self.docids, self.n_words = annotations, docids, n_words
+        self.faith_chunk, self.flip_chunk = faith_chunk, int(flip_chunk)
+
+    def device(self, b, res):
+        logits = self.eng.forward(b.ids, b.mask)
+        out = {"logits": logits, "probs": ops.class_probs(logits)}
+        self.red = ops.eraser_reduce_inputs(b.maps, b.ids, b.lens, b.ranges, b.woff, self.nsel[b.idx])
+        out["red_lengths"] = self.red["lengths"]
+        if self.flip:                                               # te_logit_stats' pred: the first maximum
+            out["pred0"] = ops.logit_stats(logits, torch.zeros(len(b.idx), dtype=torch.int32, device=logits.device))[0]
+        return out
+
+    def host(self, b, h):
+        J = len(self.fracs)
+        self.logits[b.idx], self.probs[b.idx] = h["logits"], h["probs"]
+        for r, i in enumerate(b.idx):
+            self.selected[i] = h["order"][r, :self.nsel[i, 0]].tolist()
+        lens = h["red_lengths"].reshape(-1)                         # [B * J * 2], rows (document, selection, kind)
+        flat = self.red["ids"].reshape(len(lens), b.S)
+        for chunk, L, logits in _sorted_chunks(self.eng, flat, lens, range(len(lens)), self.faith_chunk, b.ids.device):
+            ops.class_probs(logits, out=self.buf[self.slot:self.slot + len(chunk)])
+            for q_i, q in enumerate(chunk):
+                r, rest = divmod(q, 2 * J)
+                self.red_slot[b.idx[r], rest // 2, rest % 2] = self.slot + q_i
+            self.slot += len(chunk)
+            self.real_tok += int(lens[chunk].sum())
+            self.padded_tok += len(chunk) * L
+        if self.flip:                                               # the batch's maps stay on the device until it ends
+            t, fl, *st = _flip_search(self.eng, b.maps, b.ids, b.lens, b.ranges, b.woff, h["order"], h["pred0"],
+                                      [self.n_words[i] for i in b.idx], self.flip_chunk, self.faith_chunk)
+            self.flip_tok[b.idx], self.flipped[b.idx] = t, fl
+            self.flip_stats = [a + c for a, c in zip(self.flip_stats, st)]
+
+    def result(self):
+        allp, = to_host(self.buf)
+        anns, docids, logits, probs = self.annotations, self.docids, self.logits, self.probs
+        pred = np.argmax(logits, axis=1)                                # the first maximum
+        comp, suff = allp[self.red_slot[:, :, 0]], allp[self.red_slot[:, :, 1]]
+        thr = self.fracs[1:]
+        out = {"fractions": self.fracs, "n_select": self.nsel, "pred": pred, "logits": logits, "probs": probs,
+               "comp": comp, "suff": suff,
+               "lines": faithfulness_lines(anns, docids, self.names, pred, probs, comp, suff, thr, self.selected,
+                                           self.flip_tok if self.flip else None),
+               "scores": classification_scores_from_probs(anns, self.names, pred, probs, comp, suff, thr, thr),
+               "real_tokens": self.real_tok, "padded_tokens": self.padded_tok}
+        if self.flip:
+            out.update({"tokens_to_flip": self.flip_tok, "flipped": self.flipped,
+                        "flip_scores": flip_scores(anns, docids, self.n_words, self.flip_tok, self.flipped),
+                        "flip_rows": self.flip_stats[0], "flip_real_tokens": self.flip_stats[1],
+                        "flip_padded_tokens": self.flip_stats[2]})
+        return out
+
+
 def eraser_eval(generator_method, documents, annotations, encodings, evidence_classes, batch_size=8, ks=KS,
                 iou_thresholds=(0.5,), pad_id=0, device=None, same_length=None, faithfulness=False,
                 aopc_thresholds=AOPC_THRESHOLDS, k_fraction=None, faith_chunk=None, soft_scores=False,
@@ -806,12 +968,7 @@ def eraser_eval(generator_method, documents, annotations, encodings, evidence_cl
     batches then hold one token length (its ``[CLS]`` entry, the row minimum, would see the padding)."""
     ks = tuple(int(k) for k in ks)
     gen_name = getattr(getattr(generator_method, "func", generator_method), "__name__", "")
-    if latex:
-        if len(evidence_classes) != 2:
-            raise ValueError("latex needs exactly two classes: the counterfactual class is 1 - target")
-        latex_eng = _generator_model(generator_method).engine()
-        latex_cf = gen_name in LATEX_CF_GENERATORS
-        latex_docs = {}
+    lat = _Latex(generator_method, gen_name, encodings, evidence_classes) if latex else None
     if tokens_to_flip and not faithfulness:
         raise ValueError("tokens_to_flip needs faithfulness (metrics.py reads it with the classification fields)")
     if tokens_to_flip and not 1 <= int(flip_chunk) <= _lib.ERASER_MAX_SELECTIONS:
@@ -827,48 +984,17 @@ def eraser_eval(generator_method, documents, annotations, encodings, evidence_cl
         owner = getattr(generator_method, "__self__", None)
         model = getattr(owner, "model", None)
         device = next(model.parameters()).device if model is not None else torch.device("cuda")
-    from . import ops
-    n, kmax, ncol = len(annotations), max(ks), 3 + len(iou_thresholds)
+    n, kmax = len(annotations), max(ks)
     order = np.full((n, kmax), -1, dtype=np.int64)
-    counts = np.zeros((n, len(ks), ncol), dtype=np.int64)
+    counts = np.zeros((n, len(ks), 3 + len(iou_thresholds)), dtype=np.int64)
     if same_length is None:
         same_length = gen_name == "generate_attn_gradcam" or (latex and gen_name == "generate_LRP")
-    ks_run = ks
-    if faithfulness:
-        fracs = [float(f) for f in aopc_thresholds]
-        for f in fracs:
-            _check_fraction(f, "an AOPC threshold")
-        if not fracs:
-            raise ValueError("faithfulness needs at least one AOPC threshold")
-        if k_fraction is None:
-            k_fraction = human_fraction(annotations, docids, [len(ranges[d]) for d in docids], truth)
-        _check_fraction(float(k_fraction), "k_fraction")
-        fracs = [float(k_fraction)] + fracs
-        J = len(fracs)
-        nsel = np.array([[select_count(f, len(ranges[d])) for f in fracs] for d in docids], dtype=np.int64).reshape(n, J)
-        eng = _generator_model(generator_method).engine()
-        names = [c for c, _ in sorted(evidence_classes.items(), key=lambda kv: kv[1])]
-        C = eng.cfg.num_labels
-        # device rows, in the order they are produced: [probs of the originals | of the reduced rows | original logits]
-        buf = torch.empty(n * (1 + 2 * J) + n, C, dtype=torch.float32, device=device)
-        orig_slot = np.zeros(n, dtype=np.int64)
-        red_slot = np.zeros((n, J, 2), dtype=np.int64)
-        n_orig, slot, real_tok, padded_tok = 0, n, 0, 0
-        selected = [None] * n
-        kfull = max(kmax, int(nsel[:, 0].max()) if n else 0)
-        if tokens_to_flip:                                          # the search needs every document's full order
-            if C < 2:
-                raise ValueError("tokens_to_flip needs at least two classes")
-            kfull = max([kfull] + [len(ranges[d]) for d in docids])
-            flip_tok = np.zeros(n, dtype=np.int64)
-            flipped = np.zeros(n, dtype=bool)
-            flip_stats = [0, 0, 0]
-        ks_run = ks + ((kfull,) if kfull > kmax else ())
-    if soft_scores:
-        soft_doc = np.zeros((n, 3), dtype=np.float64)
-        single = np.zeros(n, dtype=bool)
-        soft_words = [None] * n
-        soft_truths = [soft_truth(truth, a, d, len(ranges[d]), nw) for a, d, nw in zip(annotations, docids, n_words)]
+    faith = _Faithfulness(generator_method, annotations, docids, ranges, truth, n_words, evidence_classes,
+                          aopc_thresholds, k_fraction, faith_chunk, tokens_to_flip, flip_chunk, kmax,
+                          device) if faithfulness else None
+    soft = _Soft(truth, annotations, docids, ranges, n_words) if soft_scores else None
+    units = [u for u in (lat, soft, faith) if u is not None]            # the order of their device work
+    ks_run = ks + ((faith.kfull,) if faith is not None and faith.kfull > kmax else ())
     by_len = sorted(range(n), key=lambda i: len(encodings[docids[i]][0]))
     batches = []
     for i in by_len:
@@ -877,127 +1003,26 @@ def eraser_eval(generator_method, documents, annotations, encodings, evidence_cl
             batches.append([])
         batches[-1].append(i)
     for idx in batches:
-        S = max(len(encodings[docids[i]][0]) for i in idx)
-        ids = torch.full((len(idx), S), pad_id, dtype=torch.long)
-        mask = torch.zeros((len(idx), S), dtype=torch.long)
-        wr, woff, sp, soff = [], [0], [], [0]
-        for r, i in enumerate(idx):
-            d = docids[i]
-            e = encodings[d][0]
-            ids[r, :len(e)] = torch.as_tensor(e, dtype=torch.long)
-            mask[r, :len(e)] = 1
-            wr.extend(ranges[d])
-            woff.append(len(wr))
-            sp.extend(truth.spans_by_key.get((d, d), []))
-            soff.append(len(sp))
-        ids_d, mask_d = ids.to(device), mask.to(device)
-        maps = generator_method(input_ids=ids_d, attention_mask=mask_d,
-                                index=torch.as_tensor([targets[i] for i in idx], device=device))
-        maps = maps.reshape(len(idx), S).to(torch.float32).contiguous()
-        res = ops.eraser_rationales(maps, wr, woff, sp, soff, ks_run, iou_thresholds)
-        parts = [res["order"].reshape(len(idx), -1), res["counts"].reshape(len(idx), -1)]
-        if latex:
-            lens_b = [len(encodings[docids[i]][0]) for i in idx]
-            lat_logits = latex_logits(latex_eng, ids_d, mask_d)
-            lat_parts = [lat_logits.view(torch.int32), ops.eraser_latex_weights(maps, lens_b).view(torch.int32)]
-            if latex_cf:
-                cf = generator_method(input_ids=ids_d, attention_mask=mask_d,
-                                      index=torch.as_tensor([1 - targets[i] for i in idx], device=device))
-                lat_parts.append(ops.eraser_latex_weights(cf.reshape(len(idx), S).to(torch.float32).contiguous(),
-                                                          lens_b).view(torch.int32))
-        if soft_scores:
-            ssp, ssoff = [], [0]
-            for i in idx:
-                ssp.extend(soft_truths[i][0])
-                ssoff.append(len(ssp))
-            soft = ops.eraser_soft_scores(res["word_scores"], woff, ssp, ssoff, [soft_truths[i][1] for i in idx])
-            parts += [soft["scores"].view(torch.int32).reshape(len(idx), 6), soft["flags"]]
-        if faithfulness:
-            B, o = len(idx), n_orig
-            logits = eng.forward(ids_d, mask_d)
-            buf[n * (1 + 2 * J) + o:n * (1 + 2 * J) + o + B].copy_(logits)
-            ops.class_probs(logits, out=buf[o:o + B])
-            orig_slot[idx] = np.arange(o, o + B)
-            n_orig += B
-            tok_lens = [len(encodings[docids[i]][0]) for i in idx]
-            red = ops.eraser_reduce_inputs(maps, ids_d, tok_lens, wr, woff, nsel[idx])
-            parts.append(red["lengths"].reshape(B, -1).to(parts[0].dtype))
-            if tokens_to_flip:                                      # te_logit_stats' pred: the first maximum
-                parts.append(ops.logit_stats(logits, torch.zeros(B, dtype=torch.int32, device=device))[0][:, None])
-        if latex:
-            lat0 = sum(p.shape[1] for p in parts)
-            parts += lat_parts
-        host = torch.cat(parts, dim=1).cpu().numpy()
-        if latex:                                   # per row: [logits (nc) | gold-class weights (S) | counterfactual (S)]
-            nc = lat_logits.shape[1]
-            lat_host = np.ascontiguousarray(host[:, lat0:]).view(np.float32)
-            for r, i in enumerate(idx):
-                t, L, pieces, w = targets[i], lens_b[r], encodings[docids[i]][1], lat_host[r]
-                correct = int(np.argmax(w[:nc])) == t
-                doc = {"GT": ("%d_GT_%s_%d.tex" % (i, _neg_pos(t), correct), latex_document(pieces, w[nc:nc + L]))}
-                if latex_cf:
-                    doc["CF"] = ("%d_CF.tex" % i, latex_document(pieces, w[nc + S:nc + S + L]))
-                latex_docs[i] = doc
-        kr = ks_run[-1]
-        order[idx] = host[:, :kmax]
-        counts[idx] = host[:, kr:kr + len(ks) * ncol].reshape(len(idx), len(ks), ncol)
-        c0 = kr + len(ks_run) * ncol
-        if soft_scores:
-            soft_doc[idx] = np.ascontiguousarray(host[:, c0:c0 + 6]).view(np.float64)
-            single[idx] = host[:, c0 + 6] != 0
-            bad = [docids[i] for r, i in enumerate(idx) if host[r, c0 + 7]]
-            if bad:
-                raise ValueError("document %r has a NaN word score; metrics.py's soft-token scores (sklearn) reject NaN"
-                                 % bad[0])
-            ws_host = res["word_scores"].cpu().numpy()
-            for r, i in enumerate(idx):
-                soft_words[i] = ws_host[woff[r]:woff[r + 1]]
-            c0 += 8
-        if faithfulness:
-            for r, i in enumerate(idx):
-                selected[i] = host[r, :nsel[i, 0]].tolist()
-            lens = host[:, c0:c0 + 2 * J].reshape(-1)                    # [B * J * 2], rows (document, selection, kind)
-            flat = red["ids"].reshape(len(lens), S)
-            for chunk, L, logits_c in _sorted_chunks(eng, flat, lens, range(len(lens)), faith_chunk, device):
-                ops.class_probs(logits_c, out=buf[slot:slot + len(chunk)])
-                for q_i, q in enumerate(chunk):
-                    r, rest = divmod(q, 2 * J)
-                    red_slot[idx[r], rest // 2, rest % 2] = slot + q_i
-                slot += len(chunk)
-                real_tok += int(lens[chunk].sum())
-                padded_tok += len(chunk) * L
-            if tokens_to_flip:                                      # the batch's maps stay on the device until it ends
-                t, fl, *st = _flip_search(eng, maps, ids_d, tok_lens, wr, woff, host[:, :kr], host[:, c0 + 2 * J],
-                                          [n_words[i] for i in idx], int(flip_chunk), faith_chunk)
-                flip_tok[idx], flipped[idx] = t, fl
-                flip_stats = [a + b for a, b in zip(flip_stats, st)]
+        b = _batch(idx, docids, encodings, pad_id, device, ranges, truth.spans_by_key)
+        b.targets = [targets[i] for i in idx]
+        maps = generator_method(input_ids=b.ids, attention_mask=b.mask, index=torch.as_tensor(b.targets, device=device))
+        b.maps = maps.reshape(len(idx), b.S).to(torch.float32).contiguous()
+        res = ops.eraser_rationales(b.maps, b.ranges, b.woff, b.spans, b.soff, ks_run, iou_thresholds)
+        named = {"order": res["order"], "counts": res["counts"]}
+        for u in units:
+            named.update(u.device(b, res))
+        h = dict(zip(named, to_host(*named.values())))
+        order[idx] = h["order"][:, :kmax]
+        counts[idx] = h["counts"][:, :len(ks)]
+        for u in units:
+            u.host(b, h)
     lines = rationale_lines(docids, ks=ks, order=order)
     scores = {k: hard_scores(truth, docids, counts[:, i], order, iou_thresholds) for i, k in enumerate(ks)}
     out = {"docids": docids, "word_ranges": [ranges[d] for d in docids], "order": order, "counts": counts,
            "lines": lines, "scores": scores}
-    if faithfulness:
-        allp = buf.cpu().numpy()
-        logits = allp[n * (1 + 2 * J) + orig_slot]
-        pred = np.argmax(logits, axis=1)                                # the first maximum
-        probs, comp, suff = allp[orig_slot], allp[red_slot[:, :, 0]], allp[red_slot[:, :, 1]]
-        thr = fracs[1:]
-        out["faithfulness"] = {
-            "fractions": fracs, "n_select": nsel, "pred": pred, "logits": logits, "probs": probs, "comp": comp,
-            "suff": suff, "lines": faithfulness_lines(annotations, docids, names, pred, probs, comp, suff, thr, selected,
-                                                      flip_tok if tokens_to_flip else None),
-            "scores": classification_scores_from_probs(annotations, names, pred, probs, comp, suff, thr, thr),
-            "real_tokens": real_tok, "padded_tokens": padded_tok}
-        if tokens_to_flip:
-            out["faithfulness"].update({
-                "tokens_to_flip": flip_tok, "flipped": flipped,
-                "flip_scores": flip_scores(annotations, docids, n_words, flip_tok, flipped), "flip_rows": flip_stats[0],
-                "flip_real_tokens": flip_stats[1], "flip_padded_tokens": flip_stats[2]})
-    if latex:
-        out["latex"] = {j: latex_docs[j] for j in range(n)}
-    if soft_scores:
-        out["soft"] = {"per_document": soft_doc, "single_class": single,
-                       "lines": soft_lines(annotations, docids, soft_words, n_words),
-                       "scores": soft_token_scores(soft_doc, single)}
+    for key, u in (("faithfulness", faith), ("latex", lat), ("soft", soft)):
+        if u is not None:
+            out[key] = u.result()
     return out
 
 

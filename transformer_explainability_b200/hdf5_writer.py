@@ -303,9 +303,9 @@ def compute_saliency_and_save(loader, method_dir, method, lrp=None, baselines=No
     batch size 1)."""
     import torch
     from . import visualization
+    from ._host import to_host
     with ResultsWriter(method_dir, backend=backend) as out:
         for data, target in loader:
-            images = data.detach().cpu().numpy()
             x = normalize(data.to(device, torch.float32))
             index = target.to(device) if vis_class == "target" else None
             b = x.shape[0]
@@ -334,7 +334,7 @@ def compute_saliency_and_save(loader, method_dir, method, lrp=None, baselines=No
             else:
                 vis = visualization.relevance_to_heatmap(res.reshape(b, -1).float().contiguous()).reshape(
                     b, 1, data.shape[-2], data.shape[-1])
-            out.append(images, vis.detach().cpu().numpy(), target.detach().cpu().numpy())
+            out.append(*to_host(data, vis, target))
     return out.path
 
 

@@ -29,6 +29,7 @@ import numpy as np
 import torch
 
 from . import ops
+from ._host import to_host
 from .perturbation import str2bool
 
 METHODS = ("rollout", "transformer_attribution", "full_lrp", "lrp_last_layer", "attn_last_layer", "attn_gradcam")
@@ -158,7 +159,7 @@ def segmentation_eval(method, loader, lrp=None, orig_lrp=None, baselines=None, t
     mask as its batch), ``mean`` [N] fp32 (the threshold), ``degenerate`` [N] bool; the totals ``pixAcc, IoU, mIoU, mAP, mF1``; and,
     with ``pr_curve``, ``precision`` / ``recall`` over every pixel."""
     check_method(method)
-    rows, means, keys = [], [], []
+    rows, keys = [], []
     P = None
     for images, labels in loader:
         gen = {"new": baselines, "lrp": lrp, "orig": orig_lrp}[_MODEL[method]]
@@ -173,25 +174,21 @@ def segmentation_eval(method, loader, lrp=None, orig_lrp=None, baselines=None, t
             scale = H // grid
         P = H * H
         r = ops.seg_metrics(maps, labels.to(dev).reshape(B, -1), grid=grid, scale=scale, thr=thr, pr_keys=pr_curve)
-        packed = torch.cat([r["counts"], r["invalid"][:, None], r["degenerate"].to(torch.int64)[:, None],
-                            r["ap"].view(torch.int64)[:, None], r["mean"].view(torch.int32).to(torch.int64)[:, None],
-                            r["row_counts"].reshape(B, -1).to(torch.int64)], dim=1).cpu()
-        bad = int(packed[:, 4].sum())
+        *host, invalid = to_host(r["counts"], r["degenerate"], r["ap"], r["mean"], r["row_counts"], r["invalid"])
+        bad = int(invalid.sum())
         if bad:
             raise ValueError("segmentation labels must be 0 or 1: %d other values in this batch" % bad)
-        rows.append(packed)
+        rows.append(host)
         if pr_curve:
             keys.append(r["pr_keys"].reshape(-1))
-    packed = torch.cat(rows).numpy() if rows else np.zeros((0, 8), dtype=np.int64)
-    tp, fp, fn, tn = (packed[:, i] for i in range(4))
-    rc = packed[:, 8:].reshape(len(tp), -1, 3)
+    counts, degenerate, ap, mean, rc = (np.concatenate(c) for c in zip(*rows))
+    tp, fp, fn, tn = counts.T
     f1_den = 2 * rc[..., 0] + rc[..., 1] + rc[..., 2]
     with np.errstate(invalid="ignore", divide="ignore"):
         f1 = np.where(f1_den > 0, (2 * rc[..., 0]).astype(np.float64) / f1_den.astype(np.float64), 0.0)
     res = {"correct": tp + tn, "labeled": np.full(len(tp), P or 0, dtype=np.int64),
            "inter": np.stack([tn, tp], axis=1), "union": np.stack([tn + fp + fn, tp + fp + fn], axis=1),
-           "ap": packed[:, 6].copy().view(np.float64), "f1": f1,
-           "mean": packed[:, 7].astype(np.int32).view(np.float32), "degenerate": packed[:, 5] != 0}
+           "ap": ap, "f1": f1, "mean": mean, "degenerate": degenerate != 0}
     res.update(totals(res["correct"], res["labeled"], res["inter"], res["union"], res["ap"], res["f1"]))
     if pr_curve:
         if keys:

@@ -34,6 +34,7 @@ import os
 import numpy as np
 import torch
 
+from ._host import to_host
 from .visualization import METHODS, _check_method
 
 
@@ -157,24 +158,15 @@ def explain_batch(model, ids, tt, mask, names, class_index=None, start_layer=0, 
     eng = model.engine()
     dev = eng.device
     flags = eng.flags | (_lib.FLAG_ATTN_GRAD_ROLLOUT if method == "attn_grad_rollout" else 0)
-    B, S = ids.shape
     # segment ids reach the engine only for a model with a token-type table (DistilBERT has none)
     tt_dev = tt.to(dev) if eng.cfg.type_vocab > 0 else None
     maps, idx, logits = eng.explain(ids.to(dev), mask.to(dev), index=class_index, start_layer=start_layer, flags=flags,
                                     return_logits=True, token_type_ids=tt_dev)
-    C = logits.shape[1]
     lengths = mask.sum(dim=1).to(torch.int32)
     neg = torch.tensor([-1.0 if n == "NEGATIVE" else 1.0 for n in names], dtype=torch.float32, device=dev)
     sign = neg[idx.long()]
-    buf = torch.empty(B * S + B * C + B, dtype=torch.float32, device=dev)
-    ops.token_importance(maps, lengths.to(dev), sign, out=buf[:B * S].view(B, S))
-    ops.class_probs(logits, out=buf[B * S:B * S + B * C].view(B, C))
-    buf[B * S + B * C:].view(torch.int32).copy_(idx)
-    host = buf.cpu().numpy()
-    scores = host[:B * S].reshape(B, S)
-    probs = host[B * S:B * S + B * C].reshape(B, C)
-    explained = host[B * S + B * C:].view(np.int32).astype(np.int64)
-    return scores, probs, explained, probs.argmax(axis=1).astype(np.int64)
+    scores, probs, explained = to_host(ops.token_importance(maps, lengths.to(dev), sign), ops.class_probs(logits), idx)
+    return scores, probs, explained.astype(np.int64), probs.argmax(axis=1).astype(np.int64)
 
 
 def records_for(tokenizer, texts, pairs, ids, tt, mask, scores, probs, explained, predicted, names):

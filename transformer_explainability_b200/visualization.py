@@ -28,6 +28,8 @@ import time
 import numpy as np
 import torch
 
+from ._host import to_host
+
 MODELS = ("vit_base_patch16_224", "vit_large_patch16_224", "deit_base_patch16_224")
 MEAN = STD = (0.5, 0.5, 0.5)            # transforms.Normalize of the notebooks
 
@@ -208,17 +210,9 @@ def render_batch(model, packed, sizes, offsets, transform, class_indices=(), use
     for idx in cols:
         maps, _ = eng.attribute(index=idx.to(torch.int32), flags=flags)
         overlays.append(render_overlays(x, relevance_to_heatmap(maps), use_thresholding))
-    k = min(5, logits.shape[1])
-    top = logits.topk(k, dim=1)[1]
-    table = torch.stack([top.to(torch.float32), logits.gather(1, top), torch.softmax(logits, dim=1).gather(1, top)], 1)
-    img = torch.stack(overlays, 1)                                 # [B, K, 224, 224, 3]
-    flat = torch.cat([img.reshape(-1), table.reshape(-1).view(torch.uint8),
-                      torch.stack(cols, 1).to(torch.int64).reshape(-1).view(torch.uint8)]).cpu()
-    n_img, n_tab = img.numel(), table.numel() * 4
-    img_h = flat[:n_img].numpy().reshape(img.shape)
-    tab_h = flat[n_img:n_img + n_tab].numpy().view(np.float32).reshape(b, 3, k)
-    cls_h = flat[n_img + n_tab:].numpy().view(np.int64).reshape(b, len(cols))
-    return img_h, cls_h, tab_h[:, 0].astype(np.int64), tab_h[:, 1], tab_h[:, 2]
+    top = logits.topk(min(5, logits.shape[1]), dim=1)[1]
+    return to_host(torch.stack(overlays, 1), torch.stack(cols, 1), top, logits.gather(1, top),
+                   torch.softmax(logits, dim=1).gather(1, top))
 
 
 def run(model, paths, output_dir, class_indices=(), use_thresholding=False, transform="center-crop", batch_size=16,
