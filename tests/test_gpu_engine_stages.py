@@ -503,9 +503,7 @@ def bert_model():
 
 
 def bert_forward_checks(log, m, flags, T, ext):
-    p, dm, H = m["p64"], m["dm"], m["heads"]
-    fam = lin_family(flags)
-    D64 = lambda name, l=0: T[(name, l)].double()          # noqa: E731
+    p, dm = m["p64"], m["dm"]
     E = "bert.embeddings."
     ids = m["ids"].to(DEV)
     S = ids.shape[1]
@@ -513,6 +511,15 @@ def bert_forward_checks(log, m, flags, T, ext):
         p[E + "word_embeddings.weight"][ids]
     check_layernorm(log, "embeddings + ln", 0, emb, p[E + "LayerNorm.weight"], p[E + "LayerNorm.bias"], dm.eps,
                     T[("hidden", 0)])
+    bert_layer_checks(log, m, flags, T, ext)
+    bert_head_checks(log, m, T, torch.tanh)
+
+
+def bert_layer_checks(log, m, flags, T, ext):
+    """every encoder layer, each stage from the engine's own input to it"""
+    p, dm, H = m["p64"], m["dm"], m["heads"]
+    fam = lin_family(flags)
+    D64 = lambda name, l=0: T[(name, l)].double()          # noqa: E731
     for l in range(dm.depth):
         L = "bert.encoder.layer.%d." % l
         h_next = T[("hidden", l + 1)] if l + 1 < dm.depth else T[("h_last", 0)]
@@ -530,19 +537,26 @@ def bert_forward_checks(log, m, flags, T, ext):
                      T[("d2", l)], T[("s2", l)], D64("ao", l))
         check_layernorm(log, "ln2", l, D64("s2", l), p[L + "output.LayerNorm.weight"], p[L + "output.LayerNorm.bias"],
                         dm.eps, h_next, T[("mean2", l)], T[("rstd2", l)])
-    y, s = lin64(D64("h_last")[:, 0], p["bert.pooler.dense.weight"], p["bert.pooler.dense.bias"])
-    log.check("pooled", "-", elem(T[("pooled", 0)], torch.tanh(y), s + y.tanh().abs()), LIN_BOUND["simt"](dm.dim))
-    y, s = lin64(D64("pooled"), p["classifier.weight"], p["classifier.bias"])
+
+
+def bert_head_checks(log, m, T, act):
+    """pooled = act(dense(h_last[:, 0])) (BERT's pooler: tanh) and the logits; act is 1-Lipschitz, so the dense's scale
+    bounds it"""
+    p, dm = m["p64"], m["dm"]
+    y, s = lin64(T[("h_last", 0)].double()[:, 0], p["bert.pooler.dense.weight"], p["bert.pooler.dense.bias"])
+    log.check("pooled", "-", elem(T[("pooled", 0)], act(y), s + act(y).abs()), LIN_BOUND["simt"](dm.dim))
+    y, s = lin64(T[("pooled", 0)].double(), p["classifier.weight"], p["classifier.bias"])
     log.check("logits", "-", elem(T[("logits", 0)], y, s), LIN_BOUND["simt"](dm.dim))
 
 
-def bert_backward_checks(log, m, flags, T, G, seed, ext):
+def bert_backward_checks(log, m, flags, T, G, seed, ext, act=torch.tanh):
+    """b: the fp64 VJP from h_last through the head (act: its activation, BERT's pooler tanh)"""
     p, dm, H = m["p64"], m["dm"], m["heads"]
     bound = 2e-5 if fp32_backward(flags) else 3e-3
     rnd = tf32 if fp32_backward(flags) else bf16
     with torch.enable_grad():
         hl = T[("h_last", 0)].double().requires_grad_(True)
-        pooled = torch.tanh(F.linear(hl[:, 0], p["bert.pooler.dense.weight"], p["bert.pooler.dense.bias"]))
+        pooled = act(F.linear(hl[:, 0], p["bert.pooler.dense.weight"], p["bert.pooler.dense.bias"]))
         logits = F.linear(pooled, p["classifier.weight"], p["classifier.bias"])
         dx, = torch.autograd.grad((seed * logits).sum(), hl)
         for l in reversed(range(dm.depth)):

@@ -73,6 +73,64 @@ def test_roberta_position_ids():
     assert ohf.position_ids(ids, ohf.DISTILBERT, 0).tolist() == [list(range(6))] * 2
 
 
+# Sequence lengths around the engine's 32-token embedding tiles and its 256-token steps of the count of earlier tiles,
+# up to RoBERTa's 512.
+SEQ_LENGTHS = (31, 32, 33, 64, 65, 255, 256, 257, 300, 512)
+CLASS_TOKEN = 3                                      # not a pad id of any test (1, 0, 5)
+
+
+def position_patterns(S, pad, vocab=100, seed=0):
+    """One row per padding pattern of length S -> (ids [R, S], mask [R, S], names): no padding; right padding from
+    inside tile 0, from 32, 64 and 256 and from inside the last tile; left padding by 1, 31, 32, 40, 255, 256 and 257
+    pads; pad ids scattered among the real tokens with mask 1; the class token followed only by pads.  Patterns that
+    do not fit in S are left out.  Real tokens are drawn from [6, vocab), so none is a pad id of the tests."""
+    g = torch.Generator().manual_seed(seed * 1000 + S)
+    rows = []
+
+    def row(name, n_left=0, right=None):
+        ids = torch.randint(6, vocab, (S,), generator=g)
+        mask = torch.ones(S, dtype=torch.long)
+        ids[n_left] = CLASS_TOKEN
+        ids[:n_left], mask[:n_left] = pad, 0
+        if right is not None:
+            ids[right:], mask[right:] = pad, 0
+        rows.append((name, ids, mask))
+        return ids
+
+    row("full")
+    last = (S - 1) // 32 * 32
+    for r in sorted({5, 32, 64, 256, last + (S - last) // 2}):
+        if 0 < r < S:
+            row("right from %d" % r, right=r)
+    for n in (1, 31, 32, 40, 255, 256, 257):
+        if n < S:
+            row("left by %d" % n, n_left=n)
+    row("pad ids under mask 1")[2::7] = pad
+    row("class token, then pads", right=1)
+    return (torch.stack([r[1] for r in rows]), torch.stack([r[2] for r in rows]), [r[0] for r in rows])
+
+
+@pytest.mark.parametrize("pad", [1, 0, 5])
+@pytest.mark.parametrize("S", SEQ_LENGTHS)
+def test_position_ids_match_transformers(S, pad):
+    """The oracle's position ids are transformers' own, on every padding pattern, whatever the mask says."""
+    transformers = pytest.importorskip("transformers")
+    ids, mask, names = position_patterns(S, pad)
+    want = transformers.models.roberta.modeling_roberta.RobertaEmbeddings.create_position_ids_from_input_ids(ids, pad)
+    got = ohf.position_ids(ids, ohf.ROBERTA, pad)
+    bad = [names[r] for r in range(len(names)) if not torch.equal(got[r], want[r])]
+    assert not bad, bad
+    assert ohf.position_ids(ids, ohf.DISTILBERT, pad).tolist() == [list(range(S))] * len(names)
+    # the patterns hold what they are named for
+    assert bool((ids[mask == 0] == pad).all())
+    scattered = names.index("pad ids under mask 1")
+    assert bool((ids[scattered] == pad).any()) and bool((mask[scattered] == 1).all())
+    assert int(got.max()) == pad + S                                  # the full row reaches the last position
+    if S > 257:
+        left = names.index("left by 257")
+        assert got[left, :257].eq(pad).all() and got[left, 257:].tolist() == list(range(pad + 1, pad + S - 256))
+
+
 @pytest.mark.parametrize("name", FAMILIES)
 def test_oracle_maps_reproduce_fixture(golden, name):
     p, ids, mask, kw = _setup(name)
