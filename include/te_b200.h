@@ -84,6 +84,10 @@ extern "C" {
                                           * relprop-only precision flags (RULES_LRP*, ZPLUS_*, RELPROP_TF32) change nothing.
                                           * Combined with TE_FLAG_GRADIENTS_ONLY, _KEEP_ALL_CAMS or _RELPROP_TO_INPUT, or with
                                           * alpha != 1, te_*_attribute returns TE_ERR_ARG. */
+#define TE_FLAG_SIMILARITY_SEED 131072u  /* with TE_FLAG_ATTN_GRAD_ROLLOUT only (te_vit_attribute; otherwise TE_ERR_ARG): no arg-max
+                                          * and no one-hot; the class-gradient backward starts from the seed that
+                                          * te_vit_similarity_seed left in the workspace, and `index` is neither read nor
+                                          * written.  No LRP starts from a similarity gradient: the relprop needs a class. */
 
 TE_API const char* te_last_error(void);
 /* Process-wide tuning switches (not part of the reference surface).
@@ -112,9 +116,16 @@ typedef struct te_vit_config {
     int distilled;    /* 1: extra dist_token + head_dist, logits averaged (DeiT-distilled extension) */
     float eps_block;  /* 1e-6, ViT_LRP.py:184,187 */
     float eps_final;  /* 1e-5, ViT_LRP.py:266 */
+    /* CLIP-architecture image towers (timm pre_norm=True, Hugging Face CLIPVisionModel).  A zeroed tail is the model above. */
+    int pre_norm;     /* 1: a LayerNorm (norm_pre.weight / .bias, eps_block) over the assembled tokens before block 0 */
+    int act;          /* MLP activation: TE_VIT_ACT_GELU (erf) or TE_VIT_ACT_QUICK_GELU (x sigmoid(1.702 x)) */
 } te_vit_config;
+#define TE_VIT_ACT_GELU 0
+#define TE_VIT_ACT_QUICK_GELU 1
 
 /* Frozen weights live in ONE flat fp32 device buffer (also the unit of the NCCL broadcast).
+ * With pre_norm, norm_pre.weight and norm_pre.bias follow pos_embed.  patch_size need not be a multiple of 4 (14 for the
+ * /14 towers); method="full" needs in_chans * img_size^2 % 4 == 0.
  * Tensor i has the reference state_dict key te_vit_weight_name(i), te_vit_weight_numel(i) floats,
  * and starts at float offset te_vit_weight_offset(i) (every offset is a multiple of 32 floats). */
 TE_API int te_vit_num_weights(const te_vit_config* cfg);
@@ -153,10 +164,21 @@ TE_API int te_vit_attribute(const te_vit_config* cfg, const float* weights, cons
                             int start_layer, float alpha, unsigned flags, float* maps, void* workspace,
                             long long workspace_bytes, void* stream);
 
-/* te_vit_forward + te_vit_attribute (alpha = 1): one call per batch = LRP.generate_LRP for `batch` independent inputs. */
+/* te_vit_forward + te_vit_attribute (alpha = 1): one call per batch = LRP.generate_LRP for `batch` independent inputs.
+ * TE_FLAG_SIMILARITY_SEED returns TE_ERR_ARG (the seed is set between the forward and the attribute). */
 TE_API int te_vit_explain(const te_vit_config* cfg, const float* weights, const float* derived, const float* images,
                    int batch, int* index, int start_layer, unsigned flags, float* maps, float* logits, void* workspace,
                    long long workspace_bytes, void* stream);
+
+/* Image-text similarity of a CLIP image tower.  Precondition: te_vit_forward on this workspace, where the "logits" are the
+ * projected image embeddings x [batch, E] (E = num_classes; head.weight = the visual projection, head.bias zero).  text
+ * [batch, E] (device) is the text embedding paired with each image.  One launch writes
+ *   similarity[b] = logit_scale * cos(x_b, t_b)      (device, may be NULL)
+ * and into the workspace the seed d similarity / d x = logit_scale * (t^ - cos x^) / |x| that
+ * te_vit_attribute(flags | TE_FLAG_SIMILARITY_SEED | TE_FLAG_ATTN_GRAD_ROLLOUT) back-propagates.  A zero-norm x or t gives
+ * NaN.  Distilled models (two heads) return TE_ERR_ARG. */
+TE_API int te_vit_similarity_seed(const te_vit_config* cfg, int batch, const float* text, float logit_scale, float* similarity,
+                                  void* workspace, long long workspace_bytes, void* stream);
 
 /* Accessors into the workspace — get_attn / get_attn_gradients / get_attn_cam / get_v ...
  * (ViT_LRP.py:102-130).  name in {"attn","attn_grad","attn_cam","qkv","x_in","ctx","logits","rollout_mats"}, and the
@@ -362,7 +384,8 @@ TE_API int te_f16_block_split(const float* x, int rows, int cols, void* hi, void
  * ---------------------------------------------------------------------------------------------- */
 /* Linear GEMMs with their fused epilogues, through the engines' own kernel selection: forward y = x W^T, x [rows,in],
  * w [out,in]; backward dx = dy W, dy [rows,out].  epi: 0 STORE (y = x W^T), 1 BIAS (+ bias), 2 BIAS_GELU (y2 = erf-GELU(y)
- * as well), 3 BIAS_ADD (y2 = e0 + y as well); backward 0 STORE (dx = dy W), 4 GELU_BWD (dx = (dy W) * GELU'(e0)).  e0 / y2
+ * as well), 3 BIAS_ADD (y2 = e0 + y as well), 12 BIAS_QUICK_GELU (y2 = y sigmoid(1.702 y) as well); backward 0 STORE
+ * (dx = dy W), 4 GELU_BWD (dx = (dy W) * GELU'(e0)), 13 QUICK_GELU_BWD (dx = (dy W) * QuickGELU'(e0)).  e0 / y2
  * share the row stride of y (dx).  flags select the family: 0 fp32 SIMT; TE_FLAG_LINEAR_TENSOR_CORES 3xTF32;
  * + TE_FLAG_LINEAR_F16_SPLIT (forward) fp16 split; + TE_FLAG_BACKWARD_TF32 / TE_FLAG_BACKWARD_F16 (backward) single-pass
  * TF32 / fp16.  scratch (may be NULL for SIMT): 16*in*out floats for the derived weight copies; with the fp16 split
@@ -587,6 +610,19 @@ TE_API long long te_prepare_images_workspace_bytes(int batch, int max_in_h, int 
 TE_API int te_prepare_images(const unsigned char* packed, long long packed_bytes, int batch, const int* sizes,
                              const long long* offsets, int out_h, int out_w, const float* mean, const float* std,
                              float* out01, float* out_norm, void* workspace, long long workspace_bytes, void* stream);
+/* The same with Pillow's filter `resample`: TE_RESAMPLE_BILINEAR (the functions above) or TE_RESAMPLE_BICUBIC, Pillow's
+ * Image.BICUBIC (support 2, the cubic convolution kernel with a = -0.5, weights normalised and quantised exactly as for
+ * bilinear; the negative lobes take the 8-bit sums outside [0, 255], which the clip to uint8 handles): CLIP's preprocessing.
+ * ksize = 2 ceil(2 max(in / out, 1)) + 1 for bicubic.  Any other value returns TE_ERR_ARG. */
+#define TE_RESAMPLE_BILINEAR 2
+#define TE_RESAMPLE_BICUBIC 3
+TE_API int te_resample_coeffs(int in_size, int out_size, int resample, int* k, int* bounds);
+TE_API long long te_prepare_images_resample_workspace_bytes(int batch, int max_in_h, int max_in_w, int out_h, int out_w,
+                                                            int resample);
+TE_API int te_prepare_images_resample(const unsigned char* packed, long long packed_bytes, int batch, const int* sizes,
+                                      const long long* offsets, int out_h, int out_w, int resample, const float* mean,
+                                      const float* std, float* out01, float* out_norm, void* workspace,
+                                      long long workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }

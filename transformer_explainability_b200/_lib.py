@@ -17,7 +17,11 @@ class TeVitConfig(ctypes.Structure):
     """``te_vit_config`` of include/te_b200.h."""
     _fields_ = [("img_size", c_int), ("patch_size", c_int), ("in_chans", c_int), ("num_classes", c_int),
                 ("dim", c_int), ("depth", c_int), ("heads", c_int), ("mlp_dim", c_int), ("distilled", c_int),
-                ("eps_block", c_float), ("eps_final", c_float)]
+                ("eps_block", c_float), ("eps_final", c_float), ("pre_norm", c_int), ("act", c_int)]
+
+
+VIT_ACT_GELU = 0                # TE_VIT_ACT_GELU: erf GELU (timm ViT / DeiT)
+VIT_ACT_QUICK_GELU = 1          # TE_VIT_ACT_QUICK_GELU: x * sigmoid(1.702 x) (CLIP)
 
 
 class TeBertConfig(ctypes.Structure):
@@ -48,6 +52,7 @@ FLAG_ZPLUS_R_F16 = 8192
 FLAG_BACKWARD_F16 = 16384
 FLAG_RULES_LRP_TC = 32768       # with FLAG_RULES_LRP: its Linear rule on TF32 tensor cores (needs the derived weights too)
 FLAG_ATTN_GRAD_ROLLOUT = 65536  # attribute() explains with the LRP-free gradient-weighted attention rollout (ICCV 2021)
+FLAG_SIMILARITY_SEED = 131072   # with FLAG_ATTN_GRAD_ROLLOUT: start from te_vit_similarity_seed's seed, no arg-max / one-hot
 FLAG_TENSOR_CORES = FLAG_ZPLUS_TENSOR_CORES | FLAG_LINEAR_TENSOR_CORES      # the ones that need derived weights
 FLAG_ALL_FAST = FLAG_TENSOR_CORES | FLAG_ATTN_TENSOR_CORES | FLAG_ROLLOUT_FUSED
 # what bench.py runs by default: updated as faster selections pass the parity tests (tests/test_gpu_parity_full.py)
@@ -77,6 +82,7 @@ PROTOTYPES = {
                               ctypes.POINTER(c_ll)]),
     "te_set_option": (c_int, [c_char_p, c_int]),
     "te_vit_relprop_pixels": (c_int, [_CFG, _P, _P, c_int, c_uint, _P, _P, _P, c_ll, _P]),
+    "te_vit_similarity_seed": (c_int, [_CFG, c_int, _P, c_float, _P, _P, c_ll, _P]),
     "te_bert_num_weights": (c_int, [_BCFG]),
     "te_bert_weight_name": (c_char_p, [_BCFG, c_int]),
     "te_bert_weight_numel": (c_ll, [_BCFG, c_int]),
@@ -135,6 +141,9 @@ PROTOTYPES = {
     "te_resize_coeffs": (c_int, [c_int, c_int, _P, _P]),
     "te_prepare_images_workspace_bytes": (c_ll, [c_int, c_int, c_int, c_int, c_int]),
     "te_prepare_images": (c_int, [_P, c_ll, c_int, _P, _P, c_int, c_int, _P, _P, _P, _P, _P, c_ll, _P]),
+    "te_resample_coeffs": (c_int, [c_int, c_int, c_int, _P, _P]),
+    "te_prepare_images_resample_workspace_bytes": (c_ll, [c_int, c_int, c_int, c_int, c_int, c_int]),
+    "te_prepare_images_resample": (c_int, [_P, c_ll, c_int, _P, _P, c_int, c_int, c_int, _P, _P, _P, _P, _P, c_ll, _P]),
 }
 
 PERTURB_MAX_STEPS = 64          # TE_PERTURB_MAX_STEPS
@@ -146,6 +155,7 @@ ERASER_MAX_SELECTIONS = 64      # TE_ERASER_MAX_SELECTIONS
 ERASER_MAX_SEQ = 8192           # TE_ERASER_MAX_SEQ
 PREPARE_MAX_SIDE = 16384        # TE_PREPARE_MAX_SIDE
 PREPARE_MAX_OUT = 4096          # TE_PREPARE_MAX_OUT
+RESAMPLE = {"bilinear": 2, "bicubic": 3}   # TE_RESAMPLE_BILINEAR / TE_RESAMPLE_BICUBIC (Pillow's filter ids)
 
 _lib = None
 

@@ -102,7 +102,10 @@ class VisionTransformer(nn.Module):
 
     def __init__(self, img_size=224, patch_size=16, in_chans=3, num_classes=1000, embed_dim=768, depth=12,
                  num_heads=12, mlp_ratio=4., qkv_bias=False, mlp_head=False, drop_rate=0., attn_drop_rate=0.,
-                 distilled=False, norm_eps=None):
+                 distilled=False, norm_eps=None, pre_norm=False, act_layer="gelu"):
+        """pre_norm / act_layer: the CLIP-architecture image towers (timm ``pre_norm=True``): a LayerNorm ``norm_pre`` over
+        the assembled tokens before block 0 (the blocks' epsilon), and the MLP activation "gelu" (erf) or "quick_gelu"
+        (x * sigmoid(1.702 x)).  Both relevance rule libraries take LayerNorm and the activation as the identity."""
         super().__init__()
         if mlp_head:
             raise NotImplementedError("mlp_head=True is not used by any reference factory")
@@ -116,18 +119,22 @@ class VisionTransformer(nn.Module):
         self.cls_token = nn.Parameter(torch.zeros(1, 1, embed_dim))
         if distilled:
             self.dist_token = nn.Parameter(torch.zeros(1, 1, embed_dim))
+        if pre_norm:
+            self.norm_pre = nn.LayerNorm(embed_dim, eps=1e-6)
         self.blocks = nn.ModuleList([_Block(embed_dim, num_heads, mlp_ratio, qkv_bias) for _ in range(depth)])
         self.norm = nn.LayerNorm(embed_dim)
         if norm_eps is not None:               # ViT_new passes one norm_layer (one epsilon) to every LayerNorm
             self.norm.eps = norm_eps
             for blk in self.blocks:
                 blk.norm1.eps = blk.norm2.eps = norm_eps
+            if pre_norm:
+                self.norm_pre.eps = norm_eps
         self.head = nn.Linear(embed_dim, num_classes)
         if distilled:
             self.head_dist = nn.Linear(embed_dim, num_classes)
         self._link_views()
         self._cfg = vit_config(img_size, patch_size, in_chans, num_classes, embed_dim, depth, num_heads, mlp_ratio,
-                               distilled, self.blocks[0].norm1.eps, self.norm.eps)
+                               distilled, self.blocks[0].norm1.eps, self.norm.eps, pre_norm=pre_norm, act=act_layer)
         self._engine = None
         self._weights_version = None
         self.engine_flags = 0

@@ -51,8 +51,10 @@ extern "C" int te_linear_forward(const float* x, const float* w, const float* bi
                                  float* scratch, int rows, int in_features, int out_features, int epi, unsigned flags,
                                  void* stream) {
     REQ(x && w && y && rows > 0 && in_features > 0 && out_features > 0, "te_linear_forward: bad argument");
-    REQ(epi >= TE_EPI_STORE && epi <= TE_EPI_BIAS_ADD, "te_linear_forward: epilogue must be STORE, BIAS, BIAS_GELU or BIAS_ADD");
-    REQ(y2 || (epi != TE_EPI_BIAS_GELU && epi != TE_EPI_BIAS_ADD), "te_linear_forward: BIAS_GELU / BIAS_ADD need y2");
+    REQ((epi >= TE_EPI_STORE && epi <= TE_EPI_BIAS_ADD) || epi == TE_EPI_BIAS_QUICK_GELU,
+        "te_linear_forward: epilogue must be STORE, BIAS, BIAS_GELU, BIAS_ADD or BIAS_QUICK_GELU");
+    REQ(y2 || (epi != TE_EPI_BIAS_GELU && epi != TE_EPI_BIAS_ADD && epi != TE_EPI_BIAS_QUICK_GELU),
+        "te_linear_forward: BIAS_GELU / BIAS_ADD / BIAS_QUICK_GELU need y2");
     REQ(e0 || epi != TE_EPI_BIAS_ADD, "te_linear_forward: BIAS_ADD needs e0");
     REQ(!(flags & ~(TE_FLAG_LINEAR_TENSOR_CORES | TE_FLAG_LINEAR_F16_SPLIT)), "te_linear_forward: unknown family flags");
     const bool tc = (flags & TE_FLAG_LINEAR_TENSOR_CORES) != 0, f16 = (flags & TE_FLAG_LINEAR_F16_SPLIT) != 0;
@@ -76,8 +78,9 @@ extern "C" int te_linear_forward(const float* x, const float* w, const float* bi
 extern "C" int te_linear_backward(const float* dy, const float* w, const float* e0, float* dx, float* scratch, int rows,
                                   int in_features, int out_features, int epi, unsigned flags, void* stream) {
     REQ(dy && w && dx && rows > 0 && in_features > 0 && out_features > 0, "te_linear_backward: bad argument");
-    REQ(epi == TE_EPI_STORE || epi == TE_EPI_GELU_BWD, "te_linear_backward: epilogue must be STORE or GELU_BWD");
-    REQ(e0 || epi != TE_EPI_GELU_BWD, "te_linear_backward: GELU_BWD needs e0");
+    REQ(epi == TE_EPI_STORE || epi == TE_EPI_GELU_BWD || epi == TE_EPI_QUICK_GELU_BWD,
+        "te_linear_backward: epilogue must be STORE, GELU_BWD or QUICK_GELU_BWD");
+    REQ(e0 || (epi != TE_EPI_GELU_BWD && epi != TE_EPI_QUICK_GELU_BWD), "te_linear_backward: GELU_BWD / QUICK_GELU_BWD need e0");
     REQ(!(flags & ~(TE_FLAG_LINEAR_TENSOR_CORES | TE_FLAG_BACKWARD_TF32 | TE_FLAG_BACKWARD_F16)),
         "te_linear_backward: unknown family flags");
     const bool tc = (flags & TE_FLAG_LINEAR_TENSOR_CORES) != 0, f16 = (flags & TE_FLAG_BACKWARD_F16) != 0;

@@ -354,6 +354,7 @@ extern "C" int te_bert_attribute(const te_bert_config* cfg, const float* weights
     Select sel;
     TE_TRY(decode_flags(sel, "te_bert_attribute", flags, derived, start_layer, !grad_rollout, {ws.tF[1], ws.nF[1]},
                         {ws.t3D[1], d.M * 3LL * d.D}, d.M, std::max(3 * d.D, d.F)));
+    if (sel.seeded) { te_set_last_error("te_bert_attribute: TE_FLAG_SIMILARITY_SEED is a ViT (CLIP image tower) mode"); return TE_ERR_ARG; }
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     Weights w;
     bind_weights(cfg, weights, w);

@@ -58,6 +58,16 @@ __device__ __forceinline__ float te_gelu_grad(float x) {
     return cdf + x * pdf;
 }
 
+// QuickGELU of CLIP, q(x) = x sigma(1.702 x), and q'(x) = s (1 + 1.702 x (1 - s)) with s = sigma(1.702 x).  1 - s is taken as
+// sigma(-1.702 x), not by cancellation, so the x (1 - s) term keeps its relative precision in the tails.  An overflowing
+// exponential gives the limits (-0 and 0 for x -> -inf, x and 1 for x -> +inf).
+__device__ __forceinline__ float te_quick_gelu(float x) { return x / (1.0f + expf(-1.702f * x)); }
+__device__ __forceinline__ float te_quick_gelu_grad(float x) {
+    const float a = 1.702f * x;
+    const float s = 1.0f / (1.0f + expf(-a)), oms = 1.0f / (1.0f + expf(a));
+    return s * fmaf(a, oms, 1.0f);
+}
+
 // GELU'(x) = Phi(x) + x phi(x) for the single-pass (TF32-grade) backward epilogues: erf by Abramowitz-Stegun 7.1.26 (absolute
 // error 1.5e-7), one ex2.approx shared by erf's exp(-x^2/2) and the density — ~15 instructions against ~45 for erff + expf.
 __device__ __forceinline__ float te_gelu_grad_fast(float x) {

@@ -34,6 +34,49 @@ __global__ void im2col_kernel(const float* __restrict__ img, float* __restrict__
     }
 }
 
+// the same layout one float at a time, for patches that are not a multiple of 4 wide (14 for the /14 towers: a patch row
+// starts at no 16-byte boundary)
+__global__ void im2col_scalar_kernel(const float* __restrict__ img, float* __restrict__ patches, int B, int C, int H, int W,
+                                     int P) {
+    const int gw = W / P, gh = H / P;
+    const long long total = (long long)B * gh * gw * C * P * P;
+    for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < total;
+         t += (long long)gridDim.x * blockDim.x) {
+        long long r = t;
+        const int ix = (int)(r % P); r /= P;
+        const int iy = (int)(r % P); r /= P;
+        const int c = (int)(r % C); r /= C;
+        const int px = (int)(r % gw); r /= gw;
+        const int py = (int)(r % gh); r /= gh;
+        const int b = (int)r;
+        patches[t] = img[(((long long)b * C + c) * H + (py * P + iy)) * W + px * P + ix];
+    }
+}
+
+// CLIP's image-text similarity s = ls cos(x, t) of each sample and its gradient ls (t^ - cos x^) / |x| as the backward seed;
+// one block per sample
+__global__ void similarity_seed_kernel(const float* __restrict__ x, const float* __restrict__ t, float ls, float* __restrict__ sim,
+                                       float* __restrict__ seed, int E) {
+    const int b = blockIdx.x;
+    const float* xb = x + (long long)b * E;
+    const float* tb = t + (long long)b * E;
+    float xx = 0.f, tt = 0.f, xt = 0.f;
+    for (int i = threadIdx.x; i < E; i += blockDim.x) {
+        const float a = xb[i], c = tb[i];
+        xx = fmaf(a, a, xx); tt = fmaf(c, c, tt); xt = fmaf(a, c, xt);
+    }
+    __shared__ float red[3][kThreads / 32];
+    xx = te_warp_sum(xx); tt = te_warp_sum(tt); xt = te_warp_sum(xt);
+    if ((threadIdx.x & 31) == 0) { red[0][threadIdx.x >> 5] = xx; red[1][threadIdx.x >> 5] = tt; red[2][threadIdx.x >> 5] = xt; }
+    __syncthreads();
+    xx = tt = xt = 0.f;
+    for (int w = 0; w < kThreads / 32; ++w) { xx += red[0][w]; tt += red[1][w]; xt += red[2][w]; }
+    const float nx = sqrtf(xx), nt = sqrtf(tt), cosv = xt / (nx * nt);
+    if (threadIdx.x == 0 && sim) sim[b] = ls * cosv;
+    const float g = ls / nx;
+    for (int i = threadIdx.x; i < E; i += blockDim.x) seed[(long long)b * E + i] = g * (tb[i] / nt - cosv * (xb[i] / nx));
+}
+
 __global__ void assemble_tokens_kernel(const float* __restrict__ patch_out, const float* __restrict__ cls,
                                        const float* __restrict__ dist, const float* __restrict__ pos,
                                        float* __restrict__ x, int B, int N, int D, int n_prefix) {
@@ -822,9 +865,20 @@ inline int warp_rows_grid(long long rows) { return (int)((rows + (kThreads / 32)
 #define TE_REQ(c, msg) do { if (!(c)) { te_set_last_error(msg); return TE_ERR_ARG; } } while (0)
 
 int te_launch_im2col(const float* img, float* patches, int B, int C, int H, int W, int P, cudaStream_t st) {
-    TE_REQ(P % 4 == 0 && W % P == 0 && H % P == 0, "im2col: patch must divide the image and be a multiple of 4");
-    const long long total = (long long)B * (H / P) * (W / P) * C * P * (P / 4);
-    im2col_kernel<<<flat_grid(total), kThreads, 0, st>>>(img, patches, B, C, H, W, P);
+    TE_REQ(P > 0 && W % P == 0 && H % P == 0, "im2col: patch must divide the image");
+    if (P % 4 == 0 && W % 4 == 0) {
+        const long long total = (long long)B * (H / P) * (W / P) * C * P * (P / 4);
+        im2col_kernel<<<flat_grid(total), kThreads, 0, st>>>(img, patches, B, C, H, W, P);
+    } else {
+        im2col_scalar_kernel<<<flat_grid((long long)B * C * H * W), kThreads, 0, st>>>(img, patches, B, C, H, W, P);
+    }
+    TE_CUDA_CHECK_LAUNCH();
+    return TE_OK;
+}
+int te_launch_similarity_seed(const float* x, const float* t, float logit_scale, float* sim, float* seed, int B, int E,
+                              cudaStream_t st) {
+    TE_REQ(B > 0 && B <= 65535 && E > 0, "similarity_seed: bad shape");
+    similarity_seed_kernel<<<B, kThreads, 0, st>>>(x, t, logit_scale, sim, seed, E);
     TE_CUDA_CHECK_LAUNCH();
     return TE_OK;
 }

@@ -62,9 +62,10 @@ static inline int linear_fwd_tc(const float* dw, const float* x, int lda, const 
                                 float* y2, const float* e0, long long M, int in, int out, int epi, cudaStream_t st,
                                 const F16Split* fs = nullptr) {
     const bool f16 = dw && fs && fs->split;
-    if (f16 && epi != TE_EPI_GELU_BWD && te_tc_fwd16_supported(M, in, out, lda))
+    const bool act = epi == TE_EPI_BIAS_GELU || epi == TE_EPI_BIAS_QUICK_GELU;     // epilogues that may emit the split of y2
+    if (f16 && epi != TE_EPI_GELU_BWD && epi != TE_EPI_QUICK_GELU_BWD && te_tc_fwd16_supported(M, in, out, lda))
         return te_tc_linear_fwd16(fs->ready ? nullptr : x, lda, fs->split, fs->scale, dw, in, out, bias, y, y2, e0, M, epi, st,
-                                  epi == TE_EPI_BIAS_GELU ? fs->split_out : nullptr, epi == TE_EPI_BIAS_GELU ? fs->scale_out : nullptr);
+                                  act ? fs->split_out : nullptr, act ? fs->scale_out : nullptr);
     if (dw && te_tc_gemm3x_supported(M, in, out, lda))
         return te_tc_linear_fwd(x, lda, dw, in, out, bias, y, y2, e0, M, epi, st);      // epilogue ids coincide
     return linear_fwd(x, lda, w, bias, y, y2, e0, M, in, out, epi, st);
@@ -73,7 +74,8 @@ static inline int linear_fwd_tc(const float* dw, const float* x, int lda, const 
 // fs: hi-only split scratch of dy (M*out/2 floats + M*ceil(out/128)) -> single-pass fp16 kernel (TE_FLAG_BACKWARD_F16)
 static inline int linear_bwd_tc(const float* dw, const float* dy, const float* w, float* dx, const float* e0, long long M,
                                 int in, int out, int epi, cudaStream_t st, bool tf32 = false, const F16Split* fs = nullptr) {
-    const bool f16 = dw && fs && fs->split, single_epi = epi == TE_EPI_STORE || epi == TE_EPI_GELU_BWD;
+    const bool f16 = dw && fs && fs->split,
+               single_epi = epi == TE_EPI_STORE || epi == TE_EPI_GELU_BWD || epi == TE_EPI_QUICK_GELU_BWD;
     if (f16 && single_epi && te_tc_fwd16_supported(M, out, in, out))
         return te_tc_linear_bwd16(fs->ready ? nullptr : dy, out, fs->split, fs->scale, dw, in, out, dx, e0, M, epi, st);
     if (dw && tf32 && single_epi && te_tc_gemm3x_supported(M, out, in, out))
@@ -155,6 +157,7 @@ struct Select {
     bool lrp;             // rule library of modules/layers_lrp.py instead of layers_ours (TE_FLAG_RULES_LRP)
     ZplusVariant zv;      // bf16 / fp16 variants of the tensor-core z+ rule
     int low;              // lowest block the relprop must reach
+    bool seeded;          // the backward starts from the workspace's similarity seed (TE_FLAG_SIMILARITY_SEED)
 };
 // A workspace region an engine lends to a kernel while the region is idle, with the floats it holds.
 struct Lent { float* ptr; long long floats; };
@@ -172,6 +175,11 @@ static inline int decode_flags(Select& s, const char* fn, unsigned flags, const 
                                int widest_out = 0) {
     // the tensor-core flag of the Linear rule of the selected rule library: layers_ours (z+) or layers_lrp
     const bool lrp = (flags & TE_FLAG_RULES_LRP) != 0;
+    if ((flags & TE_FLAG_SIMILARITY_SEED) && !(flags & TE_FLAG_ATTN_GRAD_ROLLOUT)) {
+        te_set_last_error((std::string(fn) + ": TE_FLAG_SIMILARITY_SEED needs TE_FLAG_ATTN_GRAD_ROLLOUT (no LRP starts from a "
+                           "similarity gradient)").c_str());
+        return TE_ERR_ARG;
+    }
     const unsigned rule_tc = lrp ? (flags & TE_FLAG_RULES_LRP_TC) : (flags & TE_FLAG_ZPLUS_TENSOR_CORES);
     if (((flags & (TE_FLAG_LINEAR_TENSOR_CORES | (zplus ? TE_FLAG_ZPLUS_TENSOR_CORES : 0u))) || (zplus && rule_tc)) && !derived) {
         te_set_last_error((std::string(fn) + ": tensor-core flags need the derived weight buffer").c_str());
@@ -192,6 +200,7 @@ static inline int decode_flags(Select& s, const char* fn, unsigned flags, const 
     s.lrp = lrp;
     s.zv = te_zplus_from_flags(flags);
     s.low = (flags & (TE_FLAG_KEEP_ALL_CAMS | TE_FLAG_RELPROP_TO_INPUT)) ? 0 : start_layer;
+    s.seeded = (flags & TE_FLAG_SIMILARITY_SEED) != 0;
     return TE_OK;
 }
 

@@ -71,9 +71,10 @@ __device__ __forceinline__ void epilogue4(const TeGemm& p, float* __restrict__ C
     const int nv = min(4, p.N - col);
     float e[4] = {0.f, 0.f, 0.f, 0.f}, c[4] = {0.f, 0.f, 0.f, 0.f}, o[4], o2[4] = {0.f, 0.f, 0.f, 0.f};
     constexpr bool needE = (EPI == TE_EPI_BIAS_ADD || EPI == TE_EPI_GELU_BWD || EPI == TE_EPI_SD || EPI == TE_EPI_SD_SCALED ||
-                            EPI == TE_EPI_MUL || EPI == TE_EPI_MULPOS || EPI == TE_EPI_MULNEG_ACC || EPI == TE_EPI_MULPOS_ACC);
+                            EPI == TE_EPI_MUL || EPI == TE_EPI_MULPOS || EPI == TE_EPI_MULNEG_ACC || EPI == TE_EPI_MULPOS_ACC ||
+                            EPI == TE_EPI_QUICK_GELU_BWD);
     constexpr bool needC = (EPI == TE_EPI_MULNEG_ACC || EPI == TE_EPI_MULPOS_ACC || EPI == TE_EPI_ACCUM);
-    constexpr bool hasC2 = (EPI == TE_EPI_BIAS_GELU || EPI == TE_EPI_BIAS_ADD);
+    constexpr bool hasC2 = (EPI == TE_EPI_BIAS_GELU || EPI == TE_EPI_BIAS_ADD || EPI == TE_EPI_BIAS_QUICK_GELU);
     const long long co = (long long)row * p.ldc + col;
     if (needE) {
         const float* ep = E0 + (long long)row * p.lde0 + col;
@@ -94,13 +95,15 @@ __device__ __forceinline__ void epilogue4(const TeGemm& p, float* __restrict__ C
     for (int j = 0; j < 4; ++j) {
         const float a = acc[j];
         float bj = 0.f;
-        if (EPI == TE_EPI_BIAS || EPI == TE_EPI_BIAS_GELU || EPI == TE_EPI_BIAS_ADD)
+        if (EPI == TE_EPI_BIAS || EPI == TE_EPI_BIAS_GELU || EPI == TE_EPI_BIAS_ADD || EPI == TE_EPI_BIAS_QUICK_GELU)
             bj = (p.bias != nullptr && j < nv) ? __ldg(p.bias + col + j) : 0.f;
         if (EPI == TE_EPI_STORE) o[j] = p.alpha * a;
         else if (EPI == TE_EPI_BIAS) o[j] = a + bj;
         else if (EPI == TE_EPI_BIAS_GELU) { o[j] = a + bj; o2[j] = te_gelu(o[j]); }
         else if (EPI == TE_EPI_BIAS_ADD) { o[j] = a + bj; o2[j] = e[j] + o[j]; }
         else if (EPI == TE_EPI_GELU_BWD) o[j] = a * te_gelu_grad(e[j]);
+        else if (EPI == TE_EPI_BIAS_QUICK_GELU) { o[j] = a + bj; o2[j] = te_quick_gelu(o[j]); }
+        else if (EPI == TE_EPI_QUICK_GELU_BWD) o[j] = a * te_quick_gelu_grad(e[j]);
         else if (EPI == TE_EPI_SD) o[j] = te_sd(e[j], p.alpha * a);
         else if (EPI == TE_EPI_SD_SCALED) o[j] = p.scale * te_sd(e[j], p.alpha * a);
         else if (EPI == TE_EPI_MUL) o[j] = p.alpha * a * e[j];
@@ -271,6 +274,9 @@ int te_gemm_launch(TeGemm p, int alay, int blay, int xf, int epi, cudaStream_t s
     // backward
     TE_CASE(TE_L_K, TE_L_MN, TE_XF_NONE, TE_EPI_GELU_BWD)
     TE_CASE(TE_L_MN, TE_L_MN, TE_XF_NONE, TE_EPI_STORE)
+    // QuickGELU (CLIP) forward / backward epilogues: small tiles only, spill-free (the fp32 checker of the tensor-core families)
+    TE_CASE4(TE_L_K, TE_L_K, TE_XF_NONE, TE_EPI_BIAS_QUICK_GELU)
+    TE_CASE4(TE_L_K, TE_L_MN, TE_XF_NONE, TE_EPI_QUICK_GELU_BWD)
     // relprop
     TE_CASE(TE_L_K, TE_L_K, TE_XF_AB_POSNEG, TE_EPI_SD)
     TE_CASE(TE_L_K, TE_L_K, TE_XF_AB_POS, TE_EPI_SD)

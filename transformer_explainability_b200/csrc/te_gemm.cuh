@@ -34,7 +34,9 @@ enum {
     TE_EPI_MULNEG_ACC = 8, // C += min(E0,0) * acc
     TE_EPI_ACCUM = 9,      // C += alpha*acc
     TE_EPI_SD_SCALED = 10, // C = scale * safe_divide(E0, alpha*acc)
-    TE_EPI_MULPOS_ACC = 11 // C += max(E0,0) * acc
+    TE_EPI_MULPOS_ACC = 11, // C += max(E0,0) * acc
+    TE_EPI_BIAS_QUICK_GELU = 12,  // C = acc + bias[n] ; C2 = quick_gelu(C)   (CLIP's MLP activation)
+    TE_EPI_QUICK_GELU_BWD = 13    // C = acc * quick_gelu'(E0)
 };
 
 struct TeGemm {

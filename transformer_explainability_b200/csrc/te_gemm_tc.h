@@ -71,7 +71,8 @@ int te_tc_lrp_linear_relprop(const float* x, long long ldx, const float* derived
                              cudaStream_t st, float alpha = 1.f);
 
 // fp32-grade (3xTF32 split) Linear GEMMs; epilogues mirror the SIMT ones
-enum { TE_TC_EPI_STORE = 0, TE_TC_EPI_BIAS = 1, TE_TC_EPI_BIAS_GELU = 2, TE_TC_EPI_BIAS_ADD = 3, TE_TC_EPI_GELU_BWD = 4 };
+enum { TE_TC_EPI_STORE = 0, TE_TC_EPI_BIAS = 1, TE_TC_EPI_BIAS_GELU = 2, TE_TC_EPI_BIAS_ADD = 3, TE_TC_EPI_GELU_BWD = 4,
+       TE_TC_EPI_BIAS_QUICK_GELU = 12, TE_TC_EPI_QUICK_GELU_BWD = 13 };   // the ids of te_gemm.cuh
 bool te_tc_gemm3x_supported(long long rows, int K, int N, long long lda);
 int te_tc_linear_fwd(const float* x, long long ldx, const float* derived, int in_features, int out_features,
                      const float* bias, float* y, float* y2, const float* e0, long long rows, int epi, cudaStream_t st);
@@ -87,7 +88,8 @@ int te_tc_rowsplit_f16(const float* x, long long ldx, long long rows, int cols, 
 int te_tc_blocksplit_f16(const float* x, long long ldx, long long rows, int cols, float* split, float* scale_inv, cudaStream_t st,
                          bool hi_only = false);
 // x != NULL: split / scale are scratch filled by the pre-pass; x == NULL: they were filled by the producer of x
-// (te_launch_layernorm_split or the split_out / scale_out of the previous call, TE_TC_EPI_BIAS_GELU only: the split of y2)
+// (te_launch_layernorm_split or the split_out / scale_out of the previous call, TE_TC_EPI_BIAS_GELU / _BIAS_QUICK_GELU only:
+// the split of y2)
 int te_tc_linear_fwd16(const float* x, long long ldx, float* split, float* scale, const float* derived, int in_features,
                        int out_features, const float* bias, float* y, float* y2, const float* e0, long long rows, int epi,
                        cudaStream_t st, float* split_out = nullptr, float* scale_out = nullptr);

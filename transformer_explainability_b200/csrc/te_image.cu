@@ -1,7 +1,7 @@
 // Input preparation of the ViT evaluation commands (baselines/ViT/generate_visualizations.py:194-199: Resize((224, 224)) +
 // ToTensor() on PIL images): a ragged batch of decoded RGB uint8 images, packed HWC one after another in one device buffer,
-// resized with Pillow's 8-bit bilinear filter (ImagingResample, support 1, 22-bit fixed point, the intermediate image
-// rounded to uint8) and written as planar fp32 in [0, 1] and / or normalised.  The horizontal pass runs first, except for
+// resized with Pillow's 8-bit bilinear (support 1) or bicubic (support 2, a = -0.5) filter (ImagingResample, 22-bit fixed
+// point, the intermediate image rounded to uint8) and written as planar fp32 in [0, 1] and / or normalised.  The horizontal pass runs first, except for
 // an image taller than 100 times its width that shrinks vertically: Pillow 12's Image.resize runs that one as a vertical
 // resize followed by a horizontal one, and the order changes the rounding of the intermediate.
 //   * resize_first_kernel: grid (ceil(rows / kRows), batch), 256 threads, rows = the largest first-pass output height of the
@@ -119,11 +119,26 @@ __global__ void __launch_bounds__(kThreads) resize_second_kernel(const unsigned 
 
 long long up256(long long n) { return (n + 255) / 256 * 256; }
 
-// Pillow's ksize: 2 ceil(support) + 1 with support = max(in / out, 1) (bilinear support 1)
-int kernel_size(int in, int out) {
+// Pillow's filters (Resample.c): support and weight function.  Bilinear: the triangle, support 1; bicubic: the cubic
+// convolution kernel with a = -0.5, support 2 (its negative lobes make the 8-bit sums leave [0, 255]: clip8 clamps them)
+double filter_support(int resample) { return resample == TE_RESAMPLE_BICUBIC ? 2.0 : 1.0; }
+double filter_weight(int resample, double x) {
+    if (x < 0.0) x = -x;
+    if (resample == TE_RESAMPLE_BICUBIC) {
+        const double a = -0.5;
+        if (x < 1.0) return ((a + 2.0) * x - (a + 3.0)) * x * x + 1;
+        if (x < 2.0) return (((x - 5) * x + 8) * x - 4) * a;
+        return 0.0;
+    }
+    return x < 1.0 ? 1.0 - x : 0.0;
+}
+bool valid_filter(int resample) { return resample == TE_RESAMPLE_BILINEAR || resample == TE_RESAMPLE_BICUBIC; }
+
+// Pillow's ksize: 2 ceil(support) + 1 with support = the filter's support * max(in / out, 1)
+int kernel_size(int in, int out, int resample) {
     double fs = (double)in / out;
     if (fs < 1.0) fs = 1.0;
-    return (int)std::ceil(fs) * 2 + 1;
+    return (int)std::ceil(filter_support(resample) * fs) * 2 + 1;
 }
 
 // Pillow 12's Image.resize resizes an image taller than 100 times its width vertically first (two separate resizes)
@@ -136,8 +151,8 @@ long long mid_bound(int max_h, int max_w, int oh, int ow) {
 }
 
 // ints of one image's two tables
-long long table_ints(int h, int w, int oh, int ow) {
-    return (long long)ow * (kernel_size(w, ow) + 2) + (long long)oh * (kernel_size(h, oh) + 2);
+long long table_ints(int h, int w, int oh, int ow, int resample) {
+    return (long long)ow * (kernel_size(w, ow, resample) + 2) + (long long)oh * (kernel_size(h, oh, resample) + 2);
 }
 
 }  // namespace
@@ -145,16 +160,17 @@ long long table_ints(int h, int w, int oh, int ow) {
 #define ST(s) reinterpret_cast<cudaStream_t>(s)
 #define REQ(c, msg) do { if (!(c)) { te_set_last_error(msg); return TE_ERR_ARG; } } while (0)
 
-extern "C" int te_resize_coeffs(int in_size, int out_size, int* k, int* bounds) {
+extern "C" int te_resample_coeffs(int in_size, int out_size, int resample, int* k, int* bounds) {
     REQ(in_size >= 1 && in_size <= TE_PREPARE_MAX_SIDE, "te_resize_coeffs: input size outside 1..TE_PREPARE_MAX_SIDE");
     REQ(out_size >= 1 && out_size <= TE_PREPARE_MAX_OUT, "te_resize_coeffs: output size outside 1..TE_PREPARE_MAX_OUT");
-    const int ksize = kernel_size(in_size, out_size);
+    REQ(valid_filter(resample), "te_resample_coeffs: resample must be TE_RESAMPLE_BILINEAR or TE_RESAMPLE_BICUBIC");
+    const int ksize = kernel_size(in_size, out_size, resample);
     if (!k && !bounds) return ksize;
     REQ(k && bounds, "te_resize_coeffs: k and bounds must both be given or both be null");
-    // Pillow's precompute_coeffs (bilinear filter, box [0, in_size)), then normalize_coeffs_8bpc
+    // Pillow's precompute_coeffs (box [0, in_size)), then normalize_coeffs_8bpc
     const double scale = (double)in_size / out_size;
     const double filterscale = scale < 1.0 ? 1.0 : scale;
-    const double support = 1.0 * filterscale;
+    const double support = filter_support(resample) * filterscale;
     std::vector<double> w(ksize);
     for (int xx = 0; xx < out_size; ++xx) {
         const double center = (xx + 0.5) * scale;
@@ -166,9 +182,7 @@ extern "C" int te_resize_coeffs(int in_size, int out_size, int* k, int* bounds) 
         xmax -= xmin;
         double ww = 0.0;
         for (int x = 0; x < xmax; ++x) {
-            double t = (x + xmin - center + 0.5) * ss;
-            if (t < 0.0) t = -t;
-            w[x] = t < 1.0 ? 1.0 - t : 0.0;
+            w[x] = filter_weight(resample, (x + xmin - center + 0.5) * ss);
             ww += w[x];
         }
         int* kr = k + (long long)xx * ksize;
@@ -182,18 +196,29 @@ extern "C" int te_resize_coeffs(int in_size, int out_size, int* k, int* bounds) 
     }
     return ksize;
 }
-
-extern "C" long long te_prepare_images_workspace_bytes(int batch, int max_in_h, int max_in_w, int out_h, int out_w) {
-    if (batch <= 0 || batch > 65535 || max_in_h < 1 || max_in_h > TE_PREPARE_MAX_SIDE || max_in_w < 1 ||
-        max_in_w > TE_PREPARE_MAX_SIDE || out_h < 1 || out_h > TE_PREPARE_MAX_OUT || out_w < 1 || out_w > TE_PREPARE_MAX_OUT)
-        return TE_ERR_ARG;
-    return up256((long long)sizeof(ImageDesc) * batch) + up256(4LL * batch * table_ints(max_in_h, max_in_w, out_h, out_w)) +
-           up256(batch * mid_bound(max_in_h, max_in_w, out_h, out_w));
+extern "C" int te_resize_coeffs(int in_size, int out_size, int* k, int* bounds) {
+    return te_resample_coeffs(in_size, out_size, TE_RESAMPLE_BILINEAR, k, bounds);
 }
 
-extern "C" int te_prepare_images(const unsigned char* packed, long long packed_bytes, int batch, const int* sizes,
-                                 const long long* offsets, int out_h, int out_w, const float* mean, const float* std,
-                                 float* out01, float* out_norm, void* workspace, long long workspace_bytes, void* stream) {
+extern "C" long long te_prepare_images_resample_workspace_bytes(int batch, int max_in_h, int max_in_w, int out_h, int out_w,
+                                                                int resample) {
+    if (batch <= 0 || batch > 65535 || max_in_h < 1 || max_in_h > TE_PREPARE_MAX_SIDE || max_in_w < 1 ||
+        max_in_w > TE_PREPARE_MAX_SIDE || out_h < 1 || out_h > TE_PREPARE_MAX_OUT || out_w < 1 || out_w > TE_PREPARE_MAX_OUT ||
+        !valid_filter(resample))
+        return TE_ERR_ARG;
+    return up256((long long)sizeof(ImageDesc) * batch) +
+           up256(4LL * batch * table_ints(max_in_h, max_in_w, out_h, out_w, resample)) +
+           up256(batch * mid_bound(max_in_h, max_in_w, out_h, out_w));
+}
+extern "C" long long te_prepare_images_workspace_bytes(int batch, int max_in_h, int max_in_w, int out_h, int out_w) {
+    return te_prepare_images_resample_workspace_bytes(batch, max_in_h, max_in_w, out_h, out_w, TE_RESAMPLE_BILINEAR);
+}
+
+extern "C" int te_prepare_images_resample(const unsigned char* packed, long long packed_bytes, int batch, const int* sizes,
+                                          const long long* offsets, int out_h, int out_w, int resample, const float* mean,
+                                          const float* std, float* out01, float* out_norm, void* workspace,
+                                          long long workspace_bytes, void* stream) {
+    REQ(valid_filter(resample), "te_prepare_images: resample must be TE_RESAMPLE_BILINEAR or TE_RESAMPLE_BICUBIC");
     REQ(packed && sizes && offsets, "te_prepare_images: null argument");
     REQ(out01 || out_norm, "te_prepare_images: no output requested");
     REQ(batch > 0 && batch <= 65535, "te_prepare_images: batch must lie in 1..65535");
@@ -222,14 +247,14 @@ extern "C" int te_prepare_images(const unsigned char* packed, long long packed_b
         max_rows = rows > max_rows ? rows : max_rows;
     }
     REQ(workspace && (((uintptr_t)workspace) & 255u) == 0, "te_prepare_images: workspace null or not 256-byte aligned");
-    if (te_prepare_images_workspace_bytes(batch, max_h, max_w, out_h, out_w) > workspace_bytes) {
+    if (te_prepare_images_resample_workspace_bytes(batch, max_h, max_w, out_h, out_w, resample) > workspace_bytes) {
         te_set_last_error("te_prepare_images: workspace too small");
         return TE_ERR_WORKSPACE;
     }
     // host image: [descriptors | tables], copied as one block; the intermediate follows the table bound
     const long long desc_bytes = up256((long long)sizeof(ImageDesc) * batch);
     long long ints = 0;
-    for (int b = 0; b < batch; ++b) ints += table_ints(sizes[2 * b], sizes[2 * b + 1], out_h, out_w);
+    for (int b = 0; b < batch; ++b) ints += table_ints(sizes[2 * b], sizes[2 * b + 1], out_h, out_w, resample);
     std::vector<char> host(desc_bytes + 4 * ints);
     ImageDesc* desc = reinterpret_cast<ImageDesc*>(host.data());
     int* coef = reinterpret_cast<int*>(host.data() + desc_bytes);
@@ -243,10 +268,10 @@ extern "C" int te_prepare_images(const unsigned char* packed, long long packed_b
         d.w = w;
         d.vfirst = vertical_first(h, w, out_h);
         d.kx_off = toff;
-        d.kx = te_resize_coeffs(w, out_w, coef + toff, coef + toff + (long long)out_w * kernel_size(w, out_w));
+        d.kx = te_resample_coeffs(w, out_w, resample, coef + toff, coef + toff + (long long)out_w * kernel_size(w, out_w, resample));
         toff += (long long)out_w * (d.kx + 2);
         d.ky_off = toff;
-        d.ky = te_resize_coeffs(h, out_h, coef + toff, coef + toff + (long long)out_h * kernel_size(h, out_h));
+        d.ky = te_resample_coeffs(h, out_h, resample, coef + toff, coef + toff + (long long)out_h * kernel_size(h, out_h, resample));
         toff += (long long)out_h * (d.ky + 2);
         moff += d.vfirst ? 3LL * out_h * w : 3LL * h * out_w;
     }
@@ -254,7 +279,7 @@ extern "C" int te_prepare_images(const unsigned char* packed, long long packed_b
     const ImageDesc* d_desc = reinterpret_cast<const ImageDesc*>(p);
     const int* d_coef = reinterpret_cast<const int*>(p + desc_bytes);
     unsigned char* d_mid =
-        reinterpret_cast<unsigned char*>(p + desc_bytes + up256(4LL * batch * table_ints(max_h, max_w, out_h, out_w)));
+        reinterpret_cast<unsigned char*>(p + desc_bytes + up256(4LL * batch * table_ints(max_h, max_w, out_h, out_w, resample)));
     cudaStream_t st = ST(stream);
     if (cudaMemcpyAsync(p, host.data(), host.size(), cudaMemcpyHostToDevice, st) != cudaSuccess) {
         te_set_last_error("te_prepare_images: copy of the image descriptors failed");
@@ -267,4 +292,10 @@ extern "C" int te_prepare_images(const unsigned char* packed, long long packed_b
         d_mid, d_desc, d_coef, out_h, out_w, nrm, out01, out_norm);
     TE_CUDA_CHECK_LAUNCH();
     return TE_OK;
+}
+extern "C" int te_prepare_images(const unsigned char* packed, long long packed_bytes, int batch, const int* sizes,
+                                 const long long* offsets, int out_h, int out_w, const float* mean, const float* std,
+                                 float* out01, float* out_norm, void* workspace, long long workspace_bytes, void* stream) {
+    return te_prepare_images_resample(packed, packed_bytes, batch, sizes, offsets, out_h, out_w, TE_RESAMPLE_BILINEAR, mean, std,
+                                      out01, out_norm, workspace, workspace_bytes, stream);
 }

@@ -29,6 +29,9 @@ int te_launch_softmax_bwd(const float* p, const float* dp, float* ds, long long 
 int te_launch_argmax(const float* logits, int* index, int B, int C, int only_negative, cudaStream_t st);
 int te_launch_average2(const float* a, const float* b, float* out, long long n, cudaStream_t st);
 int te_launch_onehot(const int* index, float* seed, int B, int C, float value, cudaStream_t st);
+// sim[b] = ls cos(x_b, t_b) (sim may be NULL), seed[b] = ls (t^_b - cos x^_b) / |x_b|; x, t, seed [B, E]
+int te_launch_similarity_seed(const float* x, const float* t, float logit_scale, float* sim, float* seed, int B, int E,
+                              cudaStream_t st);
 // ---- LRP elementwise rules ---------------------------------------------------------------------
 int te_launch_sd(const float* a, const float* b, float* out, long long n, cudaStream_t st);
 int te_launch_clone_relprop(const float* x, const float* r1, const float* r2, const float* r3, float* out,

@@ -107,6 +107,35 @@ __global__ void zb_combine_kernel(const float* __restrict__ img, const float* __
     }
 }
 
+// the same one pixel at a time, for patches that are not a multiple of 4 wide (four adjacent pixels may span two patches)
+__global__ void zb_combine_scalar_kernel(const float* __restrict__ img, const float* __restrict__ t0, const float* __restrict__ t1,
+                                         const float* __restrict__ t2, const float* __restrict__ lo, const float* __restrict__ hi,
+                                         float* __restrict__ r_pixels, float* __restrict__ r_sum, int B, int C, int H, int W,
+                                         int P) {
+    const int gw = W / P, gh = H / P;
+    const long long total = (long long)B * H * W;
+    const long long K = (long long)C * P * P;
+    for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < total;
+         t += (long long)gridDim.x * blockDim.x) {
+        const int x = (int)(t % W);
+        const long long rt = t / W;
+        const int y = (int)(rt % H);
+        const int b = (int)(rt / H);
+        const int px = x / P, ix = x % P, py = y / P, iy = y % P;
+        const long long prow = ((long long)b * gh + py) * gw + px;
+        const float l = lo[b], h = hi[b];
+        float acc = 0.f;
+        for (int c = 0; c < C; ++c) {
+            const long long po = prow * K + ((long long)c * P + iy) * P + ix;
+            const long long io = (((long long)b * C + c) * H + y) * W + x;
+            const float o = (img[io] * t0[po] - l * t1[po]) - h * t2[po];
+            if (r_pixels) r_pixels[io] = o;
+            acc += o;
+        }
+        if (r_sum) r_sum[t] = acc;
+    }
+}
+
 inline int flat_grid(long long n) {
     long long g = (n + kThreads - 1) / kThreads;
     return (int)(g < 1 ? 1 : (g > 132LL * 16 ? 132LL * 16 : g));
@@ -121,8 +150,8 @@ long long te_patch_relprop_scratch_floats(int B, int C, int img, int P, int D) {
 
 int te_patch_relprop_run(const float* images, const float* weight, const float* r, long long r_sample_stride, int B,
                          int C, int img, int P, int D, float* scratch, float* r_pixels, float* r_sum, cudaStream_t st) {
-    TE_REQ(P % 4 == 0 && img % P == 0, "patch_relprop: patch must divide the image and be a multiple of 4");
-    TE_REQ(((long long)C * img * img) % 4 == 0, "patch_relprop: image size % 4 != 0");
+    TE_REQ(P > 0 && img % P == 0, "patch_relprop: patch must divide the image");
+    TE_REQ(((long long)C * img * img) % 4 == 0, "patch_relprop: in_chans * img_size^2 must be a multiple of 4");
     const long long np = (long long)(img / P) * (img / P), K = (long long)C * P * P, rows = (long long)B * np;
     auto al = [](long long n) { return (n + 63) & ~63LL; };
     float* patches = scratch;
@@ -152,8 +181,12 @@ int te_patch_relprop_run(const float* images, const float* weight, const float* 
         TE_TRY(te_gemm_launch(p, TE_L_K, TE_L_MN, which == 0 ? TE_XF_NONE : (which == 1 ? TE_XF_B_POS : TE_XF_B_NEG),
                               TE_EPI_STORE, st));
     }
-    zb_combine_kernel<<<flat_grid((long long)B * img * (img / 4)), kThreads, 0, st>>>(images, t0, t1, t2, lo, hi, r_pixels,
-                                                                                   r_sum, B, C, img, img, P);
+    if (P % 4 == 0)
+        zb_combine_kernel<<<flat_grid((long long)B * img * (img / 4)), kThreads, 0, st>>>(images, t0, t1, t2, lo, hi, r_pixels,
+                                                                                       r_sum, B, C, img, img, P);
+    else
+        zb_combine_scalar_kernel<<<flat_grid((long long)B * img * img), kThreads, 0, st>>>(images, t0, t1, t2, lo, hi, r_pixels,
+                                                                                        r_sum, B, C, img, img, P);
     TE_CUDA_CHECK_LAUNCH();
     return TE_OK;
 }

@@ -773,12 +773,17 @@ struct LinOut {
 template <int EPI, bool FAST_GRAD, class EF>
 __device__ __forceinline__ float2 lin_value(const LinOut& o, int col, float v0, float v1, EF e) {
     float2 b = make_float2(0.f, 0.f);
-    if ((EPI == TE_TC_EPI_BIAS || EPI == TE_TC_EPI_BIAS_GELU || EPI == TE_TC_EPI_BIAS_ADD) && o.bias)
+    if ((EPI == TE_TC_EPI_BIAS || EPI == TE_TC_EPI_BIAS_GELU || EPI == TE_TC_EPI_BIAS_ADD || EPI == TE_TC_EPI_BIAS_QUICK_GELU) &&
+        o.bias)
         b = *reinterpret_cast<const float2*>(o.bias + col);
     if (EPI == TE_TC_EPI_GELU_BWD) {
         const float2 ev = e();
         if (FAST_GRAD) return make_float2(v0 * te_gelu_grad_fast(ev.x), v1 * te_gelu_grad_fast(ev.y));
         return make_float2(v0 * te_gelu_grad(ev.x), v1 * te_gelu_grad(ev.y));
+    }
+    if (EPI == TE_TC_EPI_QUICK_GELU_BWD) {
+        const float2 ev = e();
+        return make_float2(v0 * te_quick_gelu_grad(ev.x), v1 * te_quick_gelu_grad(ev.y));
     }
     return make_float2(v0 + b.x, v1 + b.y);
 }
@@ -787,11 +792,13 @@ __device__ __forceinline__ void lin_store(const LinOut& o, int row, int col, flo
     *reinterpret_cast<float2*>(o.C + (long long)row * o.ldc + col) = y;
     float2 y2 = make_float2(0.f, 0.f);
     if (EPI == TE_TC_EPI_BIAS_GELU) y2 = make_float2(te_gelu(y.x), te_gelu(y.y));
+    if (EPI == TE_TC_EPI_BIAS_QUICK_GELU) y2 = make_float2(te_quick_gelu(y.x), te_quick_gelu(y.y));
     if (EPI == TE_TC_EPI_BIAS_ADD) {
         const float2 ev = e();
         y2 = make_float2(ev.x + y.x, ev.y + y.y);
     }
-    if (EPI == TE_TC_EPI_BIAS_GELU || EPI == TE_TC_EPI_BIAS_ADD) *reinterpret_cast<float2*>(o.C2 + (long long)row * o.ldc2 + col) = y2;
+    if (EPI == TE_TC_EPI_BIAS_GELU || EPI == TE_TC_EPI_BIAS_ADD || EPI == TE_TC_EPI_BIAS_QUICK_GELU)
+        *reinterpret_cast<float2*>(o.C2 + (long long)row * o.ldc2 + col) = y2;
 }
 
 // ---- Linear GEMMs: C = epi(A B^T), B = the weight copy [N, K] K-major --------------------------------------------------
@@ -829,7 +836,7 @@ struct LinProb : LinArgs {
     // E of GELU_BWD, staged by the producer on the TMA mainloop.  E of BIAS_ADD (the fp16-split forward, 64 KB stages) is
     // read from global memory before the first store: its 64 KB buffer would cost it one of three stages, and that form
     // runs faster with the stage.
-    static constexpr int EPI_MAPS = TMA && EPI == TE_TC_EPI_GELU_BWD ? 1 : 0;
+    static constexpr int EPI_MAPS = TMA && (EPI == TE_TC_EPI_GELU_BWD || EPI == TE_TC_EPI_QUICK_GELU_BWD) ? 1 : 0;
     __device__ int kblocks() const { return K / (F16 ? 64 : 32); }
     __device__ float chunk_scale(int row, int ch, int) const {
         if constexpr (F16) return row < o.M ? rs[(long long)row * rs_ld + ch] : 1.f;
@@ -1256,8 +1263,9 @@ unsigned stride_blocks(long long work, int per_block) {
     return (unsigned)(b < 1 ? 1 : b);
 }
 
-// The Linear GEMM of one operand form with the epilogue epi: the forward epilogues (STORE, BIAS, BIAS_GELU, BIAS_ADD) when
-// FWD, else the backward ones (STORE, GELU_BWD).  C [rows, N] = epi(A B^T); bias / e0 / y2 as in te_gemm_tc.h.
+// The Linear GEMM of one operand form with the epilogue epi: the forward epilogues (STORE, BIAS, BIAS_GELU, BIAS_ADD,
+// BIAS_QUICK_GELU) when FWD, else the backward ones (STORE, GELU_BWD, QUICK_GELU_BWD).  C [rows, N] = epi(A B^T); bias / e0 /
+// y2 as in te_gemm_tc.h.
 template <int EPI, int FORM>
 int lin_launch(const LinArgs& args, cudaStream_t st) {
     using P = LinProb<EPI, FORM>;
@@ -1278,6 +1286,8 @@ int linear(int K, const void* a, const void* a_lo, long long lda, const void* b,
         case TE_TC_EPI_BIAS_GELU: if constexpr (FWD) return lin_launch<TE_TC_EPI_BIAS_GELU, FORM>(g, st); break;
         case TE_TC_EPI_BIAS_ADD: if constexpr (FWD) return lin_launch<TE_TC_EPI_BIAS_ADD, FORM>(g, st); break;
         case TE_TC_EPI_GELU_BWD: if constexpr (!FWD) return lin_launch<TE_TC_EPI_GELU_BWD, FORM>(g, st); break;
+        case TE_TC_EPI_BIAS_QUICK_GELU: if constexpr (FWD) return lin_launch<TE_TC_EPI_BIAS_QUICK_GELU, FORM>(g, st); break;
+        case TE_TC_EPI_QUICK_GELU_BWD: if constexpr (!FWD) return lin_launch<TE_TC_EPI_QUICK_GELU_BWD, FORM>(g, st); break;
     }
     te_set_last_error((std::string(who) + ": unsupported epilogue").c_str());
     return TE_ERR_UNSUPPORTED;
@@ -1543,7 +1553,7 @@ int te_tc_linear_fwd16(const float* x, long long ldx, float* split, float* scale
                        int out_features, const float* bias, float* y, float* y2, const float* e0, long long rows, int epi,
                        cudaStream_t st, float* split_out, float* scale_out) {
     if (!a16(split) || !scale || !a16(derived) || !a16(y) || (y2 && !a16(y2)) || (e0 && !a16(e0)) || (bias && !a16(bias)) ||
-        (split_out && (!a16(split_out) || !scale_out || !y2 || epi != TE_TC_EPI_BIAS_GELU))) {
+        (split_out && (!a16(split_out) || !scale_out || !y2 || (epi != TE_TC_EPI_BIAS_GELU && epi != TE_TC_EPI_BIAS_QUICK_GELU)))) {
         te_set_last_error("te_tc_linear_fwd16: bad operands");
         return TE_ERR_ARG;
     }
@@ -1553,7 +1563,7 @@ int te_tc_linear_fwd16(const float* x, long long ldx, float* split, float* scale
     const TeDerived<const float> dv(derived, in_features, out_features);
     TE_TRY((linear<LIN_F16X3, true>(in_features, ah, al, in_features, dv.h_w, dv.l_w, scale, dv.s_w, rows, out_features, bias, e0,
                                     y, y2, epi, "te_tc_linear_fwd16", st)));
-    // the next Linear's A operand (BIAS_GELU only): the block-scaled split of y2 = gelu(y)
+    // the next Linear's A operand (BIAS_GELU / BIAS_QUICK_GELU only): the block-scaled split of y2 = gelu(y) / quick_gelu(y)
     if (split_out) return te_tc_blocksplit_f16(y2, out_features, rows, out_features, split_out, scale_out, st);
     return TE_OK;
 }

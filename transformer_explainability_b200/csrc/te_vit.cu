@@ -27,8 +27,12 @@ struct Dims {
 
 static bool make_dims(const te_vit_config* c, int B, Dims& d) {
     if (!c || c->depth <= 0 || c->depth > kMaxDepth || c->heads <= 0 || c->dim % c->heads != 0 || c->dim % 4 != 0 ||
-        c->mlp_dim % 4 != 0 || c->patch_size % 4 != 0 || c->img_size % c->patch_size != 0 || c->num_classes <= 0) {
+        c->mlp_dim % 4 != 0 || c->patch_size <= 0 || c->img_size % c->patch_size != 0 || c->num_classes <= 0) {
         te_set_last_error("te_vit: invalid config");
+        return false;
+    }
+    if ((c->pre_norm != 0 && c->pre_norm != 1) || (c->act != TE_VIT_ACT_GELU && c->act != TE_VIT_ACT_QUICK_GELU)) {
+        te_set_last_error("te_vit: pre_norm must be 0 or 1 and act TE_VIT_ACT_GELU or TE_VIT_ACT_QUICK_GELU");
         return false;
     }
     d.B = B; d.D = c->dim; d.H = c->heads; d.dh = c->dim / c->heads; d.F = c->mlp_dim; d.C = c->num_classes;
@@ -60,6 +64,10 @@ static WTable weight_table(const te_vit_config* c) {
     add("cls_token", d.D);
     if (c->distilled) add("dist_token", d.D);
     add("pos_embed", (long long)d.N * d.D);
+    if (c->pre_norm) {
+        add("norm_pre.weight", d.D);
+        add("norm_pre.bias", d.D);
+    }
     for (int i = 0; i < d.L; ++i) {
         const std::string p = "blocks." + std::to_string(i) + ".";
         add(p + "norm1.weight", d.D);
@@ -91,7 +99,7 @@ struct BlockW {
     const float *n1w, *n1b, *qkvw, *qkvb, *projw, *projb, *n2w, *n2b, *fc1w, *fc1b, *fc2w, *fc2b;
 };
 struct Weights {
-    const float *patchw, *patchb, *cls, *dist, *pos, *normw, *normb, *headw, *headb, *headdw, *headdb;
+    const float *patchw, *patchb, *cls, *dist, *pos, *prew, *preb, *normw, *normb, *headw, *headb, *headdw, *headdb;
     BlockW blk[kMaxDepth];
 };
 
@@ -102,6 +110,8 @@ static void bind_weights(const te_vit_config* c, const float* base, Weights& w) 
     w.patchw = next(); w.patchb = next(); w.cls = next();
     w.dist = c->distilled ? next() : nullptr;
     w.pos = next();
+    w.prew = c->pre_norm ? next() : nullptr;
+    w.preb = c->pre_norm ? next() : nullptr;
     for (int l = 0; l < c->depth; ++l) {
         BlockW& b = w.blk[l];
         b.n1w = next(); b.n1b = next(); b.qkvw = next(); b.qkvb = next(); b.projw = next(); b.projb = next();
@@ -239,7 +249,14 @@ extern "C" int te_vit_forward(const te_vit_config* cfg, const float* weights, co
     TE_TRY(te_launch_im2col(images, patches, d.B, d.Cin, d.img, d.img, d.P, st));
     TE_TRY(linear_fwd(patches, d.KP, w.patchw, w.patchb, patch_out, nullptr, nullptr, (long long)d.B * d.npatch, d.KP,
                       d.D, TE_EPI_BIAS, st));
-    TE_TRY(te_launch_assemble_tokens(patch_out, w.cls, w.dist, w.pos, ws.layer[0].x_in, d.B, d.N, d.D, d.prefix, st));
+    // pre-norm towers (CLIP ln_pre, timm norm_pre): the assembled tokens pass through a LayerNorm into block 0.  Its input lives
+    // in tD[2], idle until block 0's fc1 epilogue; nothing reads it later (the gradients stop at block start_layer's
+    // attention, and the relevance rules take the LayerNorm as the identity)
+    float* tokens = cfg->pre_norm ? ws.tD[2] : ws.layer[0].x_in;
+    TE_TRY(te_launch_assemble_tokens(patch_out, w.cls, w.dist, w.pos, tokens, d.B, d.N, d.D, d.prefix, st));
+    if (cfg->pre_norm)
+        TE_TRY(te_launch_layernorm(tokens, w.prew, w.preb, ws.layer[0].x_in, nullptr, nullptr, d.M, d.D, cfg->eps_block, st));
+    const int fc1_epi = cfg->act == TE_VIT_ACT_QUICK_GELU ? TE_EPI_BIAS_QUICK_GELU : TE_EPI_BIAS_GELU;
 
     for (int l = 0; l < d.L; ++l) {
         LayerAct& a = ws.layer[l];
@@ -258,8 +275,8 @@ extern "C" int te_vit_forward(const te_vit_config* cfg, const float* weights, co
         TE_TRY(te_util::linear_fwd_tc(lw.proj, a.ctx, d.D, bw.projw, bw.projb, a.attn_out, a.x_mid, a.x_in, d.M, d.D, d.D,
                                       TE_EPI_BIAS_ADD, st, &f16.proj));
         TE_TRY(layernorm(a.x_mid, bw.n2w, bw.n2b, a.xn2, a.mean2, a.rstd2));
-        TE_TRY(te_util::linear_fwd_tc(lw.fc1, a.xn2, d.D, bw.fc1w, bw.fc1b, a.h, a.g, nullptr, d.M, d.D, d.F,
-                                      TE_EPI_BIAS_GELU, st, &f16.fc1));
+        TE_TRY(te_util::linear_fwd_tc(lw.fc1, a.xn2, d.D, bw.fc1w, bw.fc1b, a.h, a.g, nullptr, d.M, d.D, d.F, fc1_epi, st,
+                                      &f16.fc1));
         TE_TRY(te_util::linear_fwd_tc(lw.fc2, a.g, d.F, bw.fc2w, bw.fc2b, a.mlp_out, x_next, a.x_mid, d.M, d.F, d.D,
                                       TE_EPI_BIAS_ADD, st, &f16.fc2));
     }
@@ -326,10 +343,13 @@ extern "C" int te_vit_attribute(const te_vit_config* cfg, const float* weights, 
     TE_TRY(te_util::decode_flags(sel, "te_vit_attribute", flags, derived, start_layer, !grad_rollout, {ws.tF[1], ws.nF[1]},
                                  {ws.t3D[1], M3D}, d.M, std::max(3 * d.D, d.F)));
 
-    // ---- class index and seeds  (ViT_explanation_generator.py:28-35) ---------------------------
-    TE_TRY(te_launch_argmax(ws.logits, index, d.B, d.C, /*only_negative=*/1, st));
-    const float seedv = cfg->distilled ? 0.5f : 1.0f;   // averaged heads: each gets half of the seed
-    TE_TRY(te_launch_onehot(index, ws.seed, d.B, d.C, seedv, st));
+    // ---- class index and seeds  (ViT_explanation_generator.py:28-35); TE_FLAG_SIMILARITY_SEED: te_vit_similarity_seed's ----
+    if (!sel.seeded) {
+        TE_TRY(te_launch_argmax(ws.logits, index, d.B, d.C, /*only_negative=*/1, st));
+        const float seedv = cfg->distilled ? 0.5f : 1.0f;   // averaged heads: each gets half of the seed
+        TE_TRY(te_launch_onehot(index, ws.seed, d.B, d.C, seedv, st));
+    }
+    const int fc2_bwd_epi = cfg->act == TE_VIT_ACT_QUICK_GELU ? TE_EPI_QUICK_GELU_BWD : TE_EPI_GELU_BWD;
 
     // ---- backward: d logit_c / d attn_l for every block  (what :145's hook captures) -------------
     float* dxa = ws.tD[0]; float* dxb = ws.tD[1]; float* dctx = ws.tD[2]; float* dxn = ws.tD[3];
@@ -351,7 +371,7 @@ extern "C" int te_vit_attribute(const te_vit_config* cfg, const float* weights, 
         const BlockW& bw = w.blk[l];
         const DerivedW lw = bind_derived(d, sel.lbase, l);
         // mlp branch
-        TE_TRY(te_util::linear_bwd_tc(lw.fc2, dxa, bw.fc2w, dF, a.h, d.M, d.F, d.D, TE_EPI_GELU_BWD, st, sel.btf, &sel.bfs));
+        TE_TRY(te_util::linear_bwd_tc(lw.fc2, dxa, bw.fc2w, dF, a.h, d.M, d.F, d.D, fc2_bwd_epi, st, sel.btf, &sel.bfs));
         TE_TRY(te_util::linear_bwd_tc(lw.fc1, dF, bw.fc1w, dxn, nullptr, d.M, d.D, d.F, TE_EPI_STORE, st, sel.btf, &sel.bfs));
         TE_TRY(te_launch_layernorm_bwd(dxn, a.x_mid, bw.n2w, a.mean2, a.rstd2, dxa, dxb, d.M, d.D, st));
         // attention branch
@@ -458,9 +478,27 @@ extern "C" int te_vit_relprop_pixels(const te_vit_config* cfg, const float* weig
                                 d.P, d.D, ws.pix, pixel_relevance, pixel_maps, st);
 }
 
+// ================================================================================================
+// CLIP image-text similarity and its gradient, the seed of te_vit_attribute(TE_FLAG_SIMILARITY_SEED)
+// ================================================================================================
+extern "C" int te_vit_similarity_seed(const te_vit_config* cfg, int batch, const float* text, float logit_scale, float* similarity,
+                                      void* workspace, long long workspace_bytes, void* stream) {
+    Dims d; Workspace ws;
+    TE_TRY(check_ws(cfg, batch, workspace, workspace_bytes, d, ws));
+    if (!text) { te_set_last_error("te_vit_similarity_seed: null pointer"); return TE_ERR_ARG; }
+    if (cfg->distilled) { te_set_last_error("te_vit_similarity_seed: a distilled model has two heads, not one embedding"); return TE_ERR_ARG; }
+    if (!isfinite(logit_scale)) { te_set_last_error("te_vit_similarity_seed: logit_scale must be finite"); return TE_ERR_ARG; }
+    return te_launch_similarity_seed(ws.logits, text, logit_scale, similarity, ws.seed, d.B, d.C,
+                                     reinterpret_cast<cudaStream_t>(stream));
+}
+
 extern "C" int te_vit_explain(const te_vit_config* cfg, const float* weights, const float* derived, const float* images,
                               int batch, int* index, int start_layer, unsigned flags, float* maps, float* logits,
                               void* workspace, long long workspace_bytes, void* stream) {
+    if (flags & TE_FLAG_SIMILARITY_SEED) {      // the forward here would leave no seed: te_vit_similarity_seed runs between
+        te_set_last_error("te_vit_explain: TE_FLAG_SIMILARITY_SEED needs te_vit_forward, te_vit_similarity_seed, te_vit_attribute");
+        return TE_ERR_ARG;
+    }
     TE_TRY(te_vit_forward(cfg, weights, derived, images, batch, flags, logits, workspace, workspace_bytes, stream));
     return te_vit_attribute(cfg, weights, derived, batch, index, start_layer, 1.f, flags, maps, workspace, workspace_bytes,
                             stream);

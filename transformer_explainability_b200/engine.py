@@ -46,10 +46,18 @@ def _on_engine_device(fn):
     return wrapped
 
 
+_VIT_ACTS = {"gelu": _lib.VIT_ACT_GELU, "quick_gelu": _lib.VIT_ACT_QUICK_GELU}
+
+
 def vit_config(img_size=224, patch_size=16, in_chans=3, num_classes=1000, embed_dim=768, depth=12, num_heads=12,
-               mlp_ratio=4., distilled=False, eps_block=1e-6, eps_final=1e-5):
+               mlp_ratio=4., distilled=False, eps_block=1e-6, eps_final=1e-5, pre_norm=False, act="gelu"):
+    """``te_vit_config``.  pre_norm: a LayerNorm (``norm_pre``, eps_block) over the assembled tokens before block 0, as CLIP's
+    ``ln_pre``; act: the MLP activation, "gelu" (erf) or "quick_gelu" (CLIP's x * sigmoid(1.702 x))."""
+    if act not in _VIT_ACTS:
+        raise ValueError("act must be one of %s, got %r" % (sorted(_VIT_ACTS), act))
     return TeVitConfig(img_size, patch_size, in_chans, num_classes, embed_dim, depth, num_heads,
-                       int(embed_dim * mlp_ratio), int(bool(distilled)), eps_block, eps_final)
+                       int(embed_dim * mlp_ratio), int(bool(distilled)), eps_block, eps_final, int(bool(pre_norm)),
+                       _VIT_ACTS[act])
 
 
 class _Engine:
@@ -175,13 +183,15 @@ class _Engine:
 class ViTEngine(_Engine):
     """Runs ``generate_LRP(method='transformer_attribution')`` for batches of independent inputs."""
     _prefix = "te_vit_"
-    _optional = ("qkv.bias",)       # qkv_bias=False models: zeros
+    # zeros when left out: qkv_bias=False models, and the bias-free patch embedding / projection head of CLIP image towers
+    _optional = ("qkv.bias", "patch_embed.proj.bias", "head.bias")
 
     def __init__(self, cfg, state_dict=None, device=None, flags=0):
         super().__init__(cfg, state_dict, device, flags)
         self.tokens = (cfg.img_size // cfg.patch_size) ** 2 + (2 if cfg.distilled else 1)
         self.prefix = 2 if cfg.distilled else 1
         self.last_batch = 0
+        self._seed_ready = False     # the workspace seed is the similarity gradient of the current forward's embeddings
 
     def workspace_bytes(self, batch):
         return self._workspace_bytes(batch)
@@ -206,6 +216,7 @@ class ViTEngine(_Engine):
                                       fl, ptr(logits), ptr(ws), ws.numel() * 4, self._stream()), "te_vit_forward")
         self.last_batch = b
         self._last_images = images
+        self._seed_ready = False
         return logits
 
     @_on_engine_device
@@ -229,13 +240,46 @@ class ViTEngine(_Engine):
         return out
 
     @_on_engine_device
-    def attribute(self, index=None, start_layer=0, flags=None, alpha=1.0):
+    def similarity(self, text_features, logit_scale):
+        """CLIP's ``logits_per_image`` of each image of the last ``forward`` with its own text embedding: the engine's "logits"
+        are then the projected image embeddings (num_classes = the embedding width).  text_features [B, E] (one row per
+        image; one row [E] is used for every image), logit_scale = exp(the model's logit_scale).  Returns the similarities
+        [B] and leaves their gradient in the workspace as the seed of ``attribute(similarity_seeded=True)``."""
+        b = self.last_batch
+        if b <= 0:
+            raise RuntimeError("similarity() needs a preceding forward()")
+        t = torch.as_tensor(text_features).to(self.device, torch.float32)
+        if t.dim() == 1:
+            t = t.unsqueeze(0)
+        if t.shape[-1] != self.cfg.num_classes or t.shape[0] not in (1, b):
+            raise ValueError("text_features must be [%d, %d] or [%d], got %s" % (b, self.cfg.num_classes, self.cfg.num_classes,
+                                                                               tuple(t.shape)))
+        t = t.expand(b, -1).contiguous()
+        ws = self._workspace(b)
+        sim = torch.empty(b, dtype=torch.float32, device=self.device)
+        check(self.lib.te_vit_similarity_seed(ctypes.byref(self.cfg), b, ptr(t), float(logit_scale), ptr(sim), ptr(ws),
+                                              ws.numel() * 4, self._stream()), "te_vit_similarity_seed")
+        self._seed_ready = True
+        return sim
+
+    @_on_engine_device
+    def attribute(self, index=None, start_layer=0, flags=None, alpha=1.0, similarity_seeded=False):
         """Backward + relprop + rollout on the activations of the last ``forward``.
         Returns (maps [B,N-prefix], index [B] int32).  alpha: ``model.relprop(..., alpha=alpha)``, the LRP-alpha-beta rule
-        (beta = alpha - 1) in every Linear.relprop; 1 is the z+ rule every generator uses."""
+        (beta = alpha - 1) in every Linear.relprop; 1 is the z+ rule every generator uses.
+        similarity_seeded: the gradient-weighted attention rollout (FLAG_ATTN_GRAD_ROLLOUT) of the image-text similarity
+        of the last ``similarity`` call (FLAG_SIMILARITY_SEED); index is not used and comes back as given (-1: none).  The
+        seed must belong to the current forward: a seeded call after another ``forward`` / ``explain`` or after a class
+        ``attribute`` (which overwrites the seed with a one-hot) without a new ``similarity`` raises RuntimeError."""
+        if similarity_seeded:
+            flags = (self.flags if flags is None else flags) | _lib.FLAG_SIMILARITY_SEED | _lib.FLAG_ATTN_GRAD_ROLLOUT
         b = self.last_batch
         if b <= 0:
             raise RuntimeError("attribute() needs a preceding forward()")
+        seeded = bool((self.flags if flags is None else flags) & _lib.FLAG_SIMILARITY_SEED)
+        if seeded and not self._seed_ready:
+            raise RuntimeError("a similarity-seeded attribute() needs similarity() after the last forward() and class "
+                               "attribute()")
         ws = self._workspace(b)
         idx = self._index_tensor(index, b)
         maps = torch.empty(b, self.tokens - self.prefix, dtype=torch.float32, device=self.device)
@@ -243,6 +287,7 @@ class ViTEngine(_Engine):
         check(self.lib.te_vit_attribute(ctypes.byref(self.cfg), ptr(self.weights), ptr(self._derived(fl)), b, ptr(idx),
                                         int(start_layer), float(alpha), fl, ptr(maps), ptr(ws), ws.numel() * 4, self._stream()),
               "te_vit_attribute")
+        self._seed_ready = seeded                # a class attribute() wrote its one-hot over the seed
         return maps, idx
 
     @_on_engine_device
@@ -265,6 +310,7 @@ class ViTEngine(_Engine):
                                           self._stream()), "te_vit_explain")
             self.last_batch = e - s
             self._last_images = images[s:e]
+            self._seed_ready = False
         if return_logits:
             return maps, idx_all, logits
         return maps, idx_all
@@ -326,6 +372,7 @@ class ViTEngine(_Engine):
         st["graph"].replay()
         self.last_batch = B
         self._last_images = st["images"]
+        self._seed_ready = False
         if return_logits:
             return st["maps"], st["idx"], st["logits"]
         return st["maps"], st["idx"]

@@ -84,7 +84,7 @@ LINEAR_FAMILIES = {
     "tf32": _lib.FLAG_LINEAR_TENSOR_CORES | _lib.FLAG_BACKWARD_TF32,                  # backward only
     "f16": _lib.FLAG_LINEAR_TENSOR_CORES | _lib.FLAG_BACKWARD_F16,                    # backward only
 }
-LINEAR_EPI = {"store": 0, "bias": 1, "bias_gelu": 2, "bias_add": 3, "gelu_bwd": 4}
+LINEAR_EPI = {"store": 0, "bias": 1, "bias_gelu": 2, "bias_add": 3, "gelu_bwd": 4, "bias_quick_gelu": 12, "quick_gelu_bwd": 13}
 ATTN_EPI = {"store": 0, "mul": 1, "sd": 2, "softmax": 3}
 # where the convenience functions fall back to when a family does not take the shape (every shape the fp16 kernels take,
 # 3xTF32 takes as well)
@@ -104,7 +104,7 @@ def _linear_forward(x, w, bias, e0, epi, family, fall_back):
     """x [rows,in] -> (y [rows,out], y2 or None), see linear_forward_epi."""
     rows, K, N = x.shape[0], x.shape[1], w.shape[0]
     y = torch.empty(rows, N, device=x.device, dtype=torch.float32)
-    y2 = torch.empty_like(y) if epi in ("bias_gelu", "bias_add") else None
+    y2 = torch.empty_like(y) if epi in ("bias_gelu", "bias_add", "bias_quick_gelu") else None
     scratch = _tc_scratch(w, x.device, split=(rows, K, False) if family == "f16_split" else None) if family != "simt" else None
     _linear_call(_lib.load().te_linear_forward, (ptr(x), ptr(w), ptr(bias), ptr(e0), ptr(y), ptr(y2), ptr(scratch), rows, K, N),
                  epi, family, fall_back)
@@ -179,7 +179,7 @@ def linear_backward_tf32(dy, w):
 @_on_device
 def linear_forward_epi(x, w, bias=None, e0=None, epi="bias", family="simt"):
     """y = x W^T (+ bias) with a fused epilogue on the kernel family named (LINEAR_FAMILIES) -> (y, y2); y2 is None unless
-    epi is "bias_gelu" (erf GELU of y) or "bias_add" (e0 + y)."""
+    epi is "bias_gelu" (erf GELU of y), "bias_quick_gelu" (CLIP's QuickGELU of y, y sigmoid(1.702 y)) or "bias_add" (e0 + y)."""
     _req(x, w, bias, e0)
     if x.dim() != 2 or w.dim() != 2 or w.shape[1] != x.shape[1] or (e0 is not None and e0.shape != (x.shape[0], w.shape[0])):
         raise ValueError("linear_forward_epi: x [rows,in], w [out,in], e0 [rows,out] expected")
@@ -188,7 +188,8 @@ def linear_forward_epi(x, w, bias=None, e0=None, epi="bias", family="simt"):
 
 @_on_device
 def linear_backward_epi(dy, w, e0=None, epi="store", family="simt"):
-    """dx = dy W, times GELU'(e0) with epi="gelu_bwd", on the kernel family named (LINEAR_FAMILIES)."""
+    """dx = dy W, times GELU'(e0) with epi="gelu_bwd" or QuickGELU'(e0) with epi="quick_gelu_bwd", on the kernel family
+    named (LINEAR_FAMILIES)."""
     _req(dy, w, e0)
     if dy.dim() != 2 or w.dim() != 2 or dy.shape[1] != w.shape[0] or (e0 is not None and e0.shape != (dy.shape[0], w.shape[1])):
         raise ValueError("linear_backward_epi: dy [rows,out], w [out,in], e0 [rows,in] expected")
@@ -827,10 +828,11 @@ def token_importance(maps, lengths, sign, out=None):
 
 # ---- input preparation (baselines/ViT/generate_visualizations.py: Resize((224, 224)) + ToTensor()) ---------------------------
 @_on_device
-def prepare_images(packed_u8, sizes, offsets, out_hw=(224, 224), mean=None, std=None):
+def prepare_images(packed_u8, sizes, offsets, out_hw=(224, 224), mean=None, std=None, resample="bilinear"):
     """A ragged batch of decoded RGB images, HWC uint8 each, packed into the 1-D uint8 CUDA tensor ``packed_u8`` at byte
     ``offsets[b]`` with ``sizes[b] = (h, w)`` (host sequences), resized to ``out_hw`` exactly as
-    ``PIL.Image.resize((w, h), BILINEAR)`` does (see include/te_b200.h: te_prepare_images).  Returns ``(out01, out_norm)``:
+    ``PIL.Image.resize((w, h), BILINEAR)`` does (see include/te_b200.h: te_prepare_images), or with ``resample="bicubic"``
+    as ``Image.resize((w, h), BICUBIC)`` does (CLIP's preprocessing).  Returns ``(out01, out_norm)``:
     fp32 CUDA [B, 3, h, w], out01 = ``ToTensor()`` of the resized image and out_norm = (out01 - mean) / std, None unless
     ``mean`` and ``std`` (three values each) are given."""
     import numpy as np
@@ -843,9 +845,12 @@ def prepare_images(packed_u8, sizes, offsets, out_hw=(224, 224), mean=None, std=
         raise ValueError("prepare_images: sizes [B, 2] and offsets [B] with B >= 1 expected")
     if (mean is None) != (std is None) or (mean is not None and (len(mean) != 3 or len(std) != 3)):
         raise ValueError("prepare_images: mean and std are given together, three values each")
+    if resample not in _lib.RESAMPLE:
+        raise ValueError("prepare_images: resample must be one of %s" % sorted(_lib.RESAMPLE))
+    filt = _lib.RESAMPLE[resample]
     oh, ow = (int(v) for v in out_hw)
     lib = _lib.load()
-    nbytes = check(lib.te_prepare_images_workspace_bytes(B, int(sz[:, 0].max()), int(sz[:, 1].max()), oh, ow),
+    nbytes = check(lib.te_prepare_images_resample_workspace_bytes(B, int(sz[:, 0].max()), int(sz[:, 1].max()), oh, ow, filt),
                    "te_prepare_images_workspace_bytes")
     dev = packed_u8.device
     ws = _workspace(nbytes, dev)
@@ -854,6 +859,6 @@ def prepare_images(packed_u8, sizes, offsets, out_hw=(224, 224), mean=None, std=
     mean_c = None if mean is None else (_lib.c_float * 3)(*[float(m) for m in mean])
     std_c = None if std is None else (_lib.c_float * 3)(*[float(s) for s in std])
     host = lambda a: a.ctypes.data_as(_lib.c_void_p)      # noqa: E731
-    check(lib.te_prepare_images(ptr(packed_u8), packed_u8.numel(), B, host(sz), host(off), oh, ow, mean_c, std_c, ptr(out01),
-                                ptr(out_norm), ptr(ws), ws.numel() * 4, _stream()), "te_prepare_images")
+    check(lib.te_prepare_images_resample(ptr(packed_u8), packed_u8.numel(), B, host(sz), host(off), oh, ow, filt, mean_c, std_c,
+                                         ptr(out01), ptr(out_norm), ptr(ws), ws.numel() * 4, _stream()), "te_prepare_images")
     return out01, out_norm
